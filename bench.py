@@ -6,7 +6,7 @@
 
 Workload (config.workload): CoTNet-50, 224x224, batch 256 per GPU, fwd + bwd + SGD-nesterov step, bf16 autocast
 over fp32 master weights, channels_last, synthetic ImageNet-shaped data -- BASELINE.json configs[1].
-A "step" is one pass of that over one synthetic batch.  The CoT layers (16 per step) run on the sm_100a kernels
+A "step" is one pass of that over one synthetic batch.  The CoT layers (16 per step) run on the sm_90a kernels
 of libcotb200.so through the reference's operator API; the rest of the backbone is stock PyTorch (north_star:
 "host code stays PyTorch").
 
@@ -17,6 +17,10 @@ One JSON line on stdout (rank 0):
   roofline       the dominant libcotb200 kernel of the step: algorithmic bytes / CUDA-event time vs measured HBM peak
   cpu_baseline   the oracle's CPU restatement of the reference model timed on this box's host cores (bounded sample)
   clocks         nvidia-smi SM clocks / throttle reasons sampled during the timed region
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step left its caller as DIR/<name>.npy (float32):
+the loss, and the fp32 master weights, momentum and EMA of the flat optimizer state (a fixed, seeded sample of
+DUMP_SAMPLE positions of each).  Inputs and initial weights are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -70,14 +74,16 @@ def parse():
     ap.add_argument("--no-cot-leg", action="store_true", help="skip the CoT-layers-only forward measurement")
     ap.add_argument("--exposed-comm", action="store_true", default=False,
                     help="N>1: also capture the step WITHOUT collectives and report the exposed communication time (a second graph "
-                         "capture next to the NCCL-carrying one; off by default: on the call-P box it invalidated its capture and the ranks "
-                         "then hung in the process-group teardown -- the N=1 vs N=2 step times give the same number: 38.36 vs 38.92 ms)")
+                         "capture next to the NCCL-carrying one; off by default: the second capture can invalidate the first, after "
+                         "which the ranks hang in the process-group teardown)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed step as DIR/<name>.npy")
     return ap.parse_args()
 
 
 # ----------------------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """Samples nvidia-smi during the timed region (B200_PROFILING.md 'clocks' line)."""
+    """Samples nvidia-smi during the timed region (the 'clocks' entry of the JSON line)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -135,18 +141,7 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(kernel):
-    """dram bytes per launch of `kernel` from the committed ncu summary (profiles/traffic.json), else None."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get(kernel)
-        except Exception:
-            return None
-    return None
+    return 3350.0, "fallback (H100 SXM data sheet)"
 
 
 # ----------------------------------------------------------------------------------------------- CPU baseline / reference arm
@@ -277,7 +272,7 @@ def peaks_all():
         d = json.load(open(p))
         return float(d["hbm_gbs"]), float(d["bf16_tflops"]), float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, 1590.0, 1400.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, 989.0, 989.0, "fallback (H100 SXM data sheet: dense BF16, HBM3)"
 
 
 def cot_forward_leg(model, x, steps):
@@ -324,6 +319,22 @@ def cot_forward_leg(model, x, steps):
     return per, e0.elapsed_time(e1) / steps
 
 
+DUMP_SAMPLE = 1 << 20
+
+
+def dump_outputs(d, arrays):
+    """Each tensor of `arrays` as d/<name>.npy in float32; tensors of more than DUMP_SAMPLE elements as the values at DUMP_SAMPLE
+    positions drawn by a fixed seed (the same positions for the same size), which keeps a dump under 64 MB."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            idx = torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(flat.numel()))
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(d, name + ".npy"), flat.float().cpu().numpy())
+
+
 def main_ours(a):
     from cotnet_b200 import _lib, roofline, trainer
     from cotnet_b200 import dist as cdist
@@ -339,9 +350,10 @@ def main_ours(a):
     dev = torch.device("cuda", local_rank)
     torch.cuda.set_device(dev)
     _lib.load()
-    torch.backends.cudnn.benchmark = True
-    if os.environ.get("COTB200_CUDNN_BENCH_LIMIT"):       # 0 = let cuDNN's autotuner try every algorithm (default: the first 10)
-        torch.backends.cudnn.benchmark_limit = int(os.environ["COTB200_CUDNN_BENCH_LIMIT"])
+    # the same arguments must compute the same step every run: cuDNN picks its algorithms by heuristics (autotuning by timing can
+    # pick a different algorithm, i.e. a different summation order, from run to run) and only deterministic ones
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True
     torch.manual_seed(1234 + rank)
 
     B, R = a.batch, a.res
@@ -378,10 +390,12 @@ def main_ours(a):
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for _ in range(a.steps):
-                model(x_res)
+                logits = model(x_res)
             e1.record()
             torch.cuda.synchronize()
         ms = cdist.max_over_ranks(e0.elapsed_time(e1), dev)
+        if a.dump_outputs and rank == 0:
+            dump_outputs(a.dump_outputs, {"logits": logits})
         graph_info = {"cuda_graph": False}
         launches, clk, e2e = 0, None, None
         model.train()
@@ -415,8 +429,16 @@ def main_ours(a):
         if rank == 0:
             clocks.start()
         l0 = _lib.launch_count()
-        ms = timed(lambda: ts.step(x_res, lab_res), a.steps)
+        last = {}
+
+        def timed_step():
+            last["loss"] = ts.step(x_res, lab_res)
+        ms = timed(timed_step, a.steps)
         launches = _lib.launch_count() - l0
+        if a.dump_outputs and rank == 0:
+            dump_outputs(a.dump_outputs, dict({"loss": last["loss"]},
+                                              **{n: getattr(ts, n) for n in ("P_big", "P_small", "M_big", "M_small", "E_big", "E_small")
+                                                 if getattr(ts, n, None) is not None}))
         if ts._graph is not None:      # replayed launches do not pass through the host-side counter: kernels captured x replays
             launches = graph_info.get("libcotb200_kernels_per_replay", 0) * a.steps
         clk = clocks.stop() if rank == 0 else None
@@ -454,7 +476,7 @@ def main_ours(a):
                 ours_ms = sum(v[1] for v in prof.values()) / 2
                 w_frac = sum(v[2] for v in cand.values()) / 1e9 / (sum(v[1] for v in cand.values()) / 1e3) / hbm
                 roof = {"bound": "hbm", "kernel": kname, "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": ach / hbm,
-                        "peak_source": src, "traffic": ncu_traffic(kname), "launches_per_step": cnt // 2,
+                        "peak_source": src, "launches_per_step": cnt // 2,
                         "avg_launch_us": 1e3 * tot_ms / cnt, "algorithmic_bytes_per_launch": tot_bytes / cnt,
                         "kernel_share_of_step": (tot_ms / 2) / (ms / a.steps),
                         "our_kernels_share_of_step": ours_ms / (ms / a.steps),
@@ -512,12 +534,12 @@ def main_ours(a):
                                    % (a.model, R, R, B, "[FORWARD ONLY diagnostic, eval mode]" if a.fwd_only else
                                       "fwd+bwd+SGD-nesterov(+EMA %s)" % ("off" if a.no_ema else "0.9999")),
                        "global_batch": B * world, "parallelism": "dp%d" % world,
-                       "l2": "per-step working set (activations, several GB) >> 126 MB L2; no explicit flush needed",
+                       "l2": "per-step working set (activations, several GB) >> 50 MB L2; no explicit flush needed",
                        "step": "cotnet_b200.trainer.TrainStep: weights %s, gradient bucket %s, %d comm chunk(s), overlap %s"
                                % (a.weights, str(ts.G_big.dtype), len(ts.plan["chunks"]), ts.overlap),
                        "cot_path": "libcotb200 (train_conv_backend=%s): LocalConv fwd/dX/dW, GroupNorm(9 taps) fwd/bwd, bn+SiLU+pool+"
                                    "radix-2 recombination fwd/bwd (also SplitAttnConv2d's tail), fused BatchNorm(+ReLU,+residual), NHWC pooling, "
-                                   "gradient fan-in; tcgen05: the block's 1x1 convolutions (embed.0 concat-free two-pair GEMM, embed.3, conv1x1) "
+                                   "gradient fan-in; wgmma: the block's 1x1 convolutions (embed.0 concat-free two-pair GEMM, embed.3, conv1x1) "
                                    "fwd + dgrad + wgrad with BatchNorm statistics in the epilogue, key_embed 3x3 grouped conv on the haloed-tile "
                                    "kernel (dim <= 128), the bottleneck's 1x1 convolutions of stages 1-2, the 7x7 stem as a 4-tap implicit GEMM "
                                    "(+ its weight gradient); gradient gather + SGD/EMA/bf16-copy kernel, uint8->bf16 NHWC normalise; cuDNN: "
@@ -530,8 +552,8 @@ def main_ours(a):
     if world > 1:
         # Every collective of this process is behind us (the timed region and the two profiled steps end with the gradient all-reduce;
         # the roofline legs of rank 0 launch no collective) and the JSON line is flushed.  Leave WITHOUT the process-group teardown and
-        # without the interpreter's exit handlers: with NCCL kernels living inside a CUDA graph (and after a failed optional capture, call
-        # P) the communicator teardown blocked both ranks for minutes.  torchrun sees exit code 0 from every rank.
+        # without the interpreter's exit handlers: with NCCL kernels living inside a CUDA graph (and after a failed optional capture)
+        # the communicator teardown can block both ranks for minutes.  torchrun sees exit code 0 from every rank.
         sys.stdout.flush()
         sys.stderr.flush()
         os._exit(0)

@@ -1,4 +1,4 @@
-"""cotnet_b200 -- B200-native (sm_100a) CoT-block hot path behind the reference's operator API.
+"""cotnet_b200 -- H100-native (sm_90a) CoT-block hot path behind the reference's operator API.
 
 Public surface mirrors JDAI-CV/CoTNet's ``cupy_layers`` / ``models.cotnet`` names for this path only
 (SURVEY.md section 8): LocalConvolution, aggregation_zeropad, aggregation_zeropad_mix, CotLayer, CoXtLayer, and the

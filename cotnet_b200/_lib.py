@@ -161,7 +161,7 @@ def launch_count() -> int:
 
 def require_cuda(t: torch.Tensor, what: str):
     if not t.is_cuda:
-        raise RuntimeError("cotb200 %s: tensor is on %s; the B200 kernels need CUDA tensors (no CPU fallback)" % (what, t.device))
+        raise RuntimeError("cotb200 %s: tensor is on %s; the H100 kernels need CUDA tensors (no CPU fallback)" % (what, t.device))
 
 
 def prof_enable(on: bool):

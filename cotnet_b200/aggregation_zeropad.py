@@ -5,7 +5,7 @@ Same names, signatures, shapes and error behaviour as the reference
     AggregationZeropad.apply(input, weight, kernel_size, stride, padding, dilation)   :112-186
     aggregation_zeropad(input, weight, kernel_size=3, stride=1, padding=0, dilation=1)  :188-197
     LocalConvolution(in_channels, out_channels, kernel_size, stride, padding, dilation, pad_mode)  :199-236
-but the kernels are the sm_100a ones in libcotb200.so reached through the C ABI (include/cotb200.h);
+but the kernels are the sm_90a ones in libcotb200.so reached through the C ABI (include/cotb200.h);
 dimensions are runtime arguments, so there is no per-shape NVRTC compile.
 
 Extensions over the reference (which is fp32/fp64 + NCHW-contiguous only, utils.py:8-12):

@@ -44,9 +44,8 @@ class Bottleneck(nn.Module):
 
     #: (opt-in, COTB200_FORK=1) training: hand the block output to the next block as TWO aliases (conv1 reads one, the shortcut the
     #: other) so that their gradients are summed inside bn3's backward kernels instead of by an autograd add (fused._two_grads).
-    #: MEASURED AND REJECTED as a default (one box, profiles/r02_bench_callO_*.json): CoTNet-50 38.59 ms with it, 37.97 without --
-    #: ATen's add runs at the HBM roof, while the extra read costs the BatchNorm backward kernels (0.6-0.75 of the roof) more than
-    #: the add saves (bn_bwd_sums 4.62 -> 5.18 ms, bn_bwd_apply 5.35 -> 6.14 ms).  Always False on the network's last block.
+    #: Off by default: ATen's add streams at the HBM roof, while the extra read costs the BatchNorm backward kernels, which run
+    #: below the roof, more than the add saves.  Always False on the network's last block.
     fork_output = os.environ.get("COTB200_FORK", "0") != "0"
 
     def forward(self, x):
@@ -121,9 +120,8 @@ class CoTResNet(nn.Module):
 
     def _stem_conv(self, x):
         """conv1 (models/resnet.py:552: 7x7/s2, 3 -> 64) with the input and the weight zero-padded to `stem_pad` channels:
-        identical arithmetic.  MEASURED AND REJECTED (tools/bench_stem.py, profiles/r01_notes.md): cuDNN's 3-channel kernels take
-        2.67 ms fwd+wgrad at bs256, the padded variants 2.87 ms (4 ch) / 3.44 ms (8 ch) -- the pad/cast traffic costs more
-        than the aligned kernels gain.  Kept behind COTB200_STEM_PAD (default 0 = off) for other cuDNN versions."""
+        identical arithmetic.  Off by default (COTB200_STEM_PAD = 0): the pad/cast traffic can cost more than the aligned cuDNN
+        kernels gain; tools/bench_stem.py compares the variants on the machine at hand."""
         C = x.shape[1]
         pad = self.stem_pad - C if (self.stem_pad and C < self.stem_pad and self.conv1.groups == 1) else 0
         if pad <= 0:
@@ -138,7 +136,7 @@ class CoTResNet(nn.Module):
     def forward_features(self, x):
         if fused.supported(x):
             if self.stem_pad == 0 and x.dtype == torch.bfloat16:
-                # conv1 + bn1 + ReLU: 7x7/s2 stem on the 4-tap tcgen05 implicit GEMM, BatchNorm statistics from its epilogue
+                # conv1 + bn1 + ReLU: 7x7/s2 stem on the 4-tap wgmma implicit GEMM, BatchNorm statistics from its epilogue
                 # (fused.stem_conv_bn falls back to cuDNN + the fused BatchNorm kernels for geometries it does not take)
                 x = fused.max_pool3x3s2(fused.stem_conv_bn(x, self.conv1, self.bn1, relu=True))
             else:

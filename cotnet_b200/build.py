@@ -1,10 +1,9 @@
-"""Build libcotb200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libcotb200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m cotnet_b200.build [--force] [--verbose]
 
 The shared library is the C-ABI boundary declared in include/cotb200.h; it links only the CUDA
-runtime (static) -- no torch, no cuBLAS/cuDNN.  The .so is git-ignored but travels to the GPU box
-with the gpurun snapshot.
+runtime (static) -- no torch, no cuBLAS/cuDNN.  The .so is a git-ignored build product.
 """
 import glob
 import os
@@ -42,7 +41,7 @@ def build(force=False, verbose=False):
     nvcc = _nvcc()
     if nvcc is None:
         if os.path.exists(OUT):
-            return OUT  # GPU box without a toolchain: use the prebuilt library from the snapshot
+            return OUT  # no toolchain: use the library built earlier
         raise RuntimeError("nvcc not found and no prebuilt libcotb200.so present")
     objs = []
     tmp = os.path.join(HERE, "build")
@@ -55,7 +54,7 @@ def build(force=False, verbose=False):
                 [os.path.getmtime(src)] + [os.path.getmtime(p) for p in glob.glob(os.path.join(CSRC, "*.cuh"))]
                 + [os.path.getmtime(os.path.join(os.path.dirname(HERE), "include", "cotb200.h"))]):
             continue
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
                "-Xcompiler", "-fPIC", "-c", src, "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
@@ -67,7 +66,7 @@ def build(force=False, verbose=False):
             print(out)
         if p.returncode != 0:
             raise RuntimeError("nvcc failed for %s:\n%s" % (src, out))
-    link = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "static", "-o", OUT] + objs
+    link = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-cudart", "static", "-o", OUT] + objs
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s" % r.stdout)

@@ -13,7 +13,7 @@ Forward maths is SURVEY.md Appendix A.  Differences from the reference's eager g
     descriptor is mean(y + k) and the output is a0*y + a1*k directly;
   * the memory format of the input is preserved (NCHW in -> NCHW-contiguous out as the reference's
     ``.contiguous()`` gives; channels_last in -> channels_last out, no transposes), and the LocalConv runs on
-    the B200 kernels (NHWC kernels for channels_last tensors).
+    the H100 kernels (NHWC kernels for channels_last tensors).
 """
 import os
 
@@ -111,10 +111,10 @@ class CotLayer(nn.Module):
         xk, xc, xv = fused.fan_out(x, 3)
         be = self.train_conv_backend
         if B * H * W < self.tc_min_pixels and be not in ("cudnn", "tc_e0"):
-            be = "tc_e0"           # small problems: only the concat-free embed.0 GEMM stays on tcgen05 (fixed per-launch costs dominate)
+            be = "tc_e0"           # small problems: only the concat-free embed.0 GEMM stays on wgmma (fixed per-launch costs dominate)
         if (be.endswith("+k") and self.dim <= self.tc_key_max_dim and fused.tc_supported(x, self.dim)
                 and self.key_embed[0].weight.dtype == x.dtype):
-            # key_embed on the haloed-tile tcgen05 convolution: forward with the BatchNorm statistics in the epilogue, data gradient by
+            # key_embed on the haloed-tile wgmma convolution: forward with the BatchNorm statistics in the epilogue, data gradient by
             # the same kernel (flipped / transposed weights); the grouped weight gradient stays on cuDNN
             ke = self.key_embed
             k = fused.TcConv3x3Fn.apply(xk, ke[0].weight, ke[1].weight, ke[1].bias, ke[1], ke[0].groups, True)
@@ -125,7 +125,7 @@ class CotLayer(nn.Module):
         kc, kt = fused.fan_out(k, 2)
         hybrid = (be in ("tc_e0", "tc_1x1", "tc_e0e3", "tc_all1x1") and fused.tc_supported(x, self.dim)
                   and k.dtype == x.dtype)
-        if hybrid:      # embed.0 as ONE tcgen05 GEMM over the operand pairs (x, W_x), (k, W_k): no concat, statistics in the epilogue
+        if hybrid:      # embed.0 as ONE wgmma GEMM over the operand pairs (x, W_x), (k, W_k): no concat, statistics in the epilogue
             em = self.embed
             e = fused.TcConv1x1Fn.apply(xc, kc, em[0].weight, None, em[1].weight, em[1].bias, em[1], True, None)
         else:
@@ -148,7 +148,7 @@ class CotLayer(nn.Module):
         u = fused.AggTapFn.apply(v.contiguous(memory_format=torch.channels_last), w, 1, gc)
         return fused.cot_tail(u, kt.contiguous(memory_format=torch.channels_last), self.bn, self.se)
 
-    # ---- inference path: every convolution of the block on the tcgen05 kernels, BatchNorms folded into epilogues ----
+    # ---- inference path: every convolution of the block on the wgmma kernels, BatchNorms folded into epilogues ----
     def _tc_eval_ok(self, x):
         return (not self.training and not torch.is_grad_enabled() and x.dtype == torch.bfloat16 and self.kernel_size == 3
                 and self.dim % 64 == 0 and tc.conv_tile(self.dim, 4) is not None and x.shape[3] <= 128)
@@ -199,7 +199,7 @@ class CotLayer(nn.Module):
 
     def _forward_tc_eval(self, x):
         """models/cotnet.py:79-104 in eval mode with NO cuDNN/cuBLAS call: 3x3 grouped key conv = implicit GEMM over TMA
-        pixel boxes, the three 1x1 convs = tcgen05 GEMMs on the NHWC pixel matrix (embed.0 consumes x and k as two
+        pixel boxes, the three 1x1 convs = wgmma GEMMs on the NHWC pixel matrix (embed.0 consumes x and k as two
         operand pairs, no concat), every BatchNorm / bias / ReLU is a GEMM epilogue."""
         B, C, H, W = x.shape
         p = self._tc_params(x.device)
@@ -209,8 +209,8 @@ class CotLayer(nn.Module):
         if self.eval_fused_agg and gc == 8 and H * W >= 32 and C <= 512 and p["ref"] is not None:
             # (opt-in, COTB200_EVAL_FUSED_AGG=1) logits in tap-major order + their per-sample column sums from ONE GEMM; GroupNorm
             # becomes a per-(sample, column) affine applied inside the LocalConv kernel, which also does bn + SiLU and the pooled
-            # descriptor.  Fewer launches and HBM passes, but measured SLOWER than the separate kernels (profiles/r02_ncu_targets_callI.md:
-            # the in-place weight-tile prologue makes the kernel shared-memory-latency bound, 349 us against 125 us at stage 1).
+            # descriptor.  Fewer launches and HBM passes, but the in-place weight-tile prologue makes the kernel
+            # shared-memory-latency bound, so it is not the default.
             l, cs, cq = tc.gemm_bf16_samplestats(e, p["we2p"], H * W, shift=p["be2p"])
             v = tc.gemm_bf16(x, p["wv"], scale=p["v_ss"][0], shift=p["v_ss"][1])
             out = fused.cot_eval_tail_fused(v.view(B, H, W, C).permute(0, 3, 1, 2), l, cs, cq, None, p["gnw_p"], p["gnb_p"],
@@ -219,7 +219,7 @@ class CotLayer(nn.Module):
                 return out
         if self.eval_samplestats and H * W >= 32:
             # (opt-in) GroupNorm statistics from the logits GEMM's own epilogue: saves the statistics pass over l, but the per-sample
-            # epilogue costs more than gn72_stats does (104 vs 40 + 40 us at stage 1, same profile)
+            # epilogue pays one global atomic per row group and column (and adds in a run-dependent order)
             l, cs, cq = tc.gemm_bf16_samplestats(e, p["we2"], H * W, shift=p["be2"])
             v = tc.gemm_bf16(x, p["wv"], scale=p["v_ss"][0], shift=p["v_ss"][1])
             J = l.shape[1]
@@ -233,7 +233,7 @@ class CotLayer(nn.Module):
         return fused.cot_tail(u, k, self.bn, self.se)
 
     def _forward_tc_train(self, x):
-        """Autograd-capable path with every convolution of the block on the tcgen05 kernels (forward + data gradients;
+        """Autograd-capable path with every convolution of the block on the wgmma kernels (forward + data gradients;
         BatchNorm batch statistics from the GEMM epilogues; no torch.cat, no separate statistics pass)."""
         B, C, H, W = x.shape
         ke, em, cv = self.key_embed, self.embed, self.conv1x1
@@ -248,27 +248,24 @@ class CotLayer(nn.Module):
 
     #: Training-mode convolution backend of the block (COTB200_TRAIN_CONV):
     #:   "cudnn"      cuDNN convolutions + the fused normalisation kernels
-    #:   "tc_e0"      embed.0 (the 2C -> C/2 conv on [x ; k]) as ONE concat-free two-operand-pair tcgen05 GEMM: forward with the
-    #:                BatchNorm statistics in the epilogue, data and weight gradients on the tcgen05 kernels
+    #:   "tc_e0"      embed.0 (the 2C -> C/2 conv on [x ; k]) as ONE concat-free two-operand-pair wgmma GEMM: forward with the
+    #:                BatchNorm statistics in the epilogue, data and weight gradients on the wgmma kernels
     #:   "tc_1x1" / "tc_e0e3" / "tc_all1x1"   + conv1x1 / + embed.3 / + both (all three 1x1 convolutions of the block; with
     #:                "tc_all1x1" the enclosing bottleneck's conv1 / conv3 / downsample of stages 1-2 as well, fused.conv1x1_bn)
-    #:   "...+k"      key_embed (grouped 3x3) on the haloed-tile tcgen05 convolution for dim <= tc_key_max_dim
-    #:   "tc"         the older all-tcgen05 autograd path (TcConv3x3Fn + TcConv1x1Fn for everything, per-tap conv at 7x7)
-    #: Inference (no_grad, eval) always takes the tcgen05 path when the shape allows.
-    #: Measured inside the whole CoTNet-50 bs256 training step (one CUDA graph, same box, profiles/r02_bench_cotnet50_callK_*.json):
-    #: tc_e0 39.23 ms, tc_e0+k 38.89, tc_all1x1 38.62, tc_all1x1+k 38.35  ->  "tc_all1x1+k" is the default (bf16 channels_last,
-    #: dim % 64 == 0; anything else uses cuDNN for that convolution).  Round 1 (before the warp-uniform MMA issue and the haloed
-    #: convolution): cudnn 42.80, tc_e0 41.29, tc 46.38 (profiles/r01_bench_conv_backends_run18.json).
+    #:   "...+k"      key_embed (grouped 3x3) on the haloed-tile wgmma convolution for dim <= tc_key_max_dim
+    #:   "tc"         the older all-wgmma autograd path (TcConv3x3Fn + TcConv1x1Fn for everything, per-tap conv at 7x7)
+    #: Inference (no_grad, eval) always takes the wgmma path when the shape allows.
+    #: "tc_all1x1+k" is the default (bf16 channels_last, dim % 64 == 0; anything else uses cuDNN for that convolution): it puts the
+    #: most of the step on this library.  tools/bench_conv.py and bench.py compare the backends (COTB200_TRAIN_CONV).
     train_conv_backend = os.environ.get("COTB200_TRAIN_CONV", "tc_all1x1+k")
-    #: "+k" suffix of the backend: key_embed on the haloed-tile tcgen05 convolution for dim <= this (stages 1-2: there it beats
-    #: cuDNN's grouped kernels 94 vs 159 us and 57 vs 74-82 us per call, profiles/r02_bench_halo_callJ.json; at 14x14 / 7x7 cuDNN wins)
+    #: "+k" suffix of the backend: key_embed on the haloed-tile wgmma convolution for dim <= this (stages 1-2;
+    #: at 14x14 / 7x7 cuDNN's grouped kernels are used)
     tc_key_max_dim = int(os.environ.get("COTB200_TC_KEY_MAX_DIM", "128"))
     #: pixels (B*H*W) below which the backend degrades to "tc_e0": on the 14x14 / 7x7 stages the fixed per-launch costs of the
-    #: all-tcgen05 path outweigh its byte savings (one box, profiles/r02_bench_callM_*.json: CoTNet-50 bs256 38.99 -> 38.90 ms,
-    #: SE-CoTNetD-101 bs128 43.58 -> 43.23, SE-CoTNetD-152 320^2 bs64 67.77 -> 67.48 with the threshold at 100 000)
+    #: all-wgmma path outweigh its byte savings
     tc_min_pixels = int(os.environ.get("COTB200_TC_MIN_PIXELS", "100000"))
     #: inference: GroupNorm-apply, LocalConv, bn + SiLU and the pooling in ONE kernel (cotb200_cot_agg_eval); default 0 = separate
-    #: kernels, which measure faster (11.65 -> 9.70 ms CoTNet-50 bs256 eval forward, profiles/r02_prof_cotnet50_eval_callI*.md)
+    #: kernels (the fused kernel is shared-memory-latency bound)
     eval_fused_agg = os.environ.get("COTB200_EVAL_FUSED_AGG", "0") != "0"
     #: inference: GroupNorm statistics from the logits GEMM epilogue (cotb200_gemm_bf16_samplestats) instead of gn9_stats
     eval_samplestats = os.environ.get("COTB200_EVAL_SAMPLESTATS", "0") != "0"
@@ -287,7 +284,7 @@ class CotLayer(nn.Module):
         # cast BEFORE the 6-D view: .to() on the 4-D tensor keeps channels_last, so the view below is the NHWC weight
         # layout the kernels take without a copy
         w = w.to(v.dtype).view(B, 1, C // 8, self.kernel_size * self.kernel_size, H, W)
-        y = self.local_conv(v, w)                                          # B200 LocalConv kernel
+        y = self.local_conv(v, w)                                          # H100 LocalConv kernel
         y = self.act(self.bn(y))
         return _keep_format(_radix2_tail(y, k, self.se), x)
 
@@ -328,9 +325,9 @@ class CoXtLayer(nn.Module):
     def _forward_fused(self, x):
         """channels_last fast path.  The grouped convolutions (groups 8 / 2 / 2 / 2, :113-133) run as DENSE convolutions with
         block-diagonal weights built from the grouped parameters (differentiable scatter, exact zeros elsewhere -- the same
-        arithmetic): cuDNN's grouped NHWC kernels for 12..96-channel groups spend most of their time in layout transforms
-        (profiles/r02_prof_cotnext50_*.md: 47 % of the step in tensorTransformGeneric), the extra dense FLOPs are free on an
-        HBM-bound block, and the dense form puts embed.0 on the concat-free two-pair tcgen05 GEMM like the CoT layer (the
+        arithmetic): cuDNN's grouped NHWC kernels for 12..96-channel groups spend much of their time in layout transforms
+        (tensorTransformGeneric in a torch.profiler trace), the extra dense FLOPs are free on an
+        HBM-bound block, and the dense form puts embed.0 on the concat-free two-pair wgmma GEMM like the CoT layer (the
         channel interleave of qk, :153-154, becomes a column permutation of the weight)."""
         B, C, H, W = x.shape
         cl = torch.channels_last
@@ -365,8 +362,8 @@ class CoXtLayer(nn.Module):
         u = fused.AggTapFn.apply(v.contiguous(memory_format=torch.channels_last), w, self.dw_group, gc)
         return fused.cot_tail(u, kt.contiguous(memory_format=torch.channels_last), self.bn, self.se)
 
-    #: CoXt: the dense block-diagonal form of its grouped 1x1 convolutions doubles their FLOPs; measured in the CoTNeXt-50 step
-    #: (profiles/r02_bench_cotnext50_callL*.json): tc_e0 61.20 ms, tc_all1x1 61.84 ms -> only embed.0 on the two-pair GEMM
+    #: CoXt: the dense block-diagonal form of its grouped 1x1 convolutions doubles their FLOPs, so only embed.0 (the concat-free
+    #: two-pair GEMM) runs on the wgmma kernels by default
     train_conv_backend = os.environ.get("COTB200_TRAIN_CONV_COXT", "tc_e0")
 
     def forward(self, x):

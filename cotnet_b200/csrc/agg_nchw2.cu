@@ -1,4 +1,4 @@
-// LocalConv 3x3 on NCHW tensors (the reference contract), second-generation kernels (sm_100a).
+// LocalConv 3x3 on NCHW tensors (the reference contract), second-generation kernels (sm_90a).
 //
 // Same arithmetic as agg_fwd_nchw_fast / agg_bwd_nchw_fast (agg_zeropad.cu) -- one thread owns the K*K weights of its
 // pixels in registers and loops over the C/wc channels sharing them -- but:
@@ -6,7 +6,7 @@
 //     the 3x3 neighbourhood of the group is 3 x (1 vector + 2 edge scalars) loads instead of 9 scalars per pixel;
 //   * one CTA row of the grid per (sample, weight-channel) plane: no 64-bit index decomposition per element;
 //   * interior fast path without any predication, edge path with zero fill;
-//   * bf16/fp16 use the mixed-precision FMA (fma.rn.f32.bf16 -> SASS FHFMA), no unpack instructions.
+//   * bf16/fp16 are widened to fp32 for the FMA (exact products, fp32 accumulation).
 // Requires W % PXV == 0 (56, 28 -> 4; 14 -> 2); other widths use the first-generation scalar kernels.
 #include <cstdlib>
 #include "common.cuh"
@@ -164,8 +164,7 @@ __device__ __forceinline__ void nchw2_bwd_body(const T* __restrict__ dp, const T
 }
 
 // 16-bit types: 2 CTAs per SM (the fused dX+dW variant otherwise takes 130 registers -> one 8-warp CTA per SM).  fp32 keeps
-// its 172 registers: capping it to 128 or splitting it into two launches measured SLOWER on the small planes this kernel
-// still serves (stage 3: 157 us uncapped vs 185-187 us; the large fp32 planes go through agg_nchw_tma.cu).
+// its 172 registers (capping it to 128 spills; the large fp32 planes go through agg_nchw_tma.cu).
 template <typename T, int PXV, bool DX, bool DW>
 __global__ void __launch_bounds__(256, (sizeof(T) == 2 ? 2 : 1))
 agg3_bwd_nchw2_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ w, T* __restrict__ dx,
@@ -224,8 +223,7 @@ int nchw2_bwd(int N, int C, int H, int W, int wc, long long dy_sn, const T* dy, 
     dim3 grid((H * (W / pxv) + 255) / 256, N * wc);
     const int rep = C / wc;
     COTB200_PROF_B(dx && dw ? "agg3_bwd_nchw2_dxdw" : (dx ? "agg3_bwd_nchw2_dx" : "agg3_bwd_nchw2_dw"), ((double)N * H * W) * ((dx && dw ? 3.0 : 2.0) * C + (dx && dw ? 18.0 : 9.0) * wc) * sizeof(T));
-    // COTB200_NCHW_SPLIT=1: fp32 dX and dW as two launches (measured: 488 vs 500 us at stage 1, 187 vs 157 us at stage 3 --
-    // not a win; kept as a switch).
+    // COTB200_NCHW_SPLIT=1: fp32 dX and dW as two launches (reads x and dy twice; kept as a switch).
     static int split_env = -1;
     if (split_env < 0) { const char* e = getenv("COTB200_NCHW_SPLIT"); split_env = (e && e[0] == '1') ? 1 : 0; }
     const bool split = split_env && sizeof(T) == 4 && dx && dw;

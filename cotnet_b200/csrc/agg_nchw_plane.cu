@@ -3,7 +3,7 @@
 //
 // The other NCHW kernels tile a plane over the grid; on a 14x14 plane that leaves 98 threads of a 256-thread CTA with 8-byte
 // accesses (the TMA ring cannot help: a 56-byte row is not a legal TMA stride) and the reference's own scalar kernel was faster
-// in backward (profiles/r02_bench_ref_kernels_callH.json: 183 vs 174 us at [256,256,14,14] fp32).  Here a CTA owns whole
+// in backward at [256,256,14,14] fp32.  Here a CTA owns whole
 // (sample, weight-channel) items -- the rep = C/wc channel planes that share one set of 9 weight planes:
 //   * all rep planes of x and/or dy are staged in shared memory as fp32 with a one-pixel ZERO halo (one load phase of
 //     independent coalesced loads, one barrier), so the tap loops have no boundary predicates at all;
@@ -115,8 +115,8 @@ template <typename T>
 int nchw_plane_launch(int mode, int N, int C, int H, int W, int wc, long long x_sn, long long y_sn, long long w_sn, const T* a, const T* b,
                       const T* w, T* o1, T* o2, cudaStream_t st, int* rc) {
   if constexpr (std::is_same<T, double>::value) { return 0; } else {
-    // COTB200_AGG_PLANE: 0 = off, 1 (default) = where it measured faster than the tiled kernels AND the reference's own kernels
-    // (backward on planes of >= 100 pixels: profiles/r02_bench_ref_kernels_callI.json), 2 = every small plane, forward included
+    // COTB200_AGG_PLANE: 0 = off, 1 (default) = backward on planes of >= 100 pixels, where it beats the tiled kernels and the
+    // reference's own kernels, 2 = every small plane, forward included
     static int level = -1;
     if (level < 0) { const char* e = getenv("COTB200_AGG_PLANE"); level = e ? atoi(e) : 1; }
     if (level <= 0) return 0;

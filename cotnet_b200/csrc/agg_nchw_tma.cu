@@ -1,7 +1,7 @@
-// LocalConv 3x3 on NCHW tensors (the reference contract, fp32 first): persistent CTAs fed by a TMA pipeline (sm_100a).
+// LocalConv 3x3 on NCHW tensors (the reference contract, fp32 first): persistent CTAs fed by a TMA pipeline (sm_90a).
 //
-// The register-resident NCHW kernels (agg_nchw2.cu) reach 0.34-0.43 of the HBM roof forward and about the speed of the
-// reference's own kernels backward (profiles/r01_bench_ref_kernels_run11.json): 80-170 registers, one or two 8-warp CTAs
+// The register-resident NCHW kernels (agg_nchw2.cu) stay well below the HBM roof forward and near the speed of the
+// reference's own kernels backward: 80-170 registers, one or two 8-warp CTAs
 // per SM, every warp waiting on global loads, and each halo row costs one vector + two scalar global loads.
 // Same cure as for the NHWC kernels (agg_tma.cu): one producer warp streams tiles into a shared-memory ring with
 // cp.async.bulk.tensor, the compute warps never touch global memory for their operands.

@@ -1,9 +1,8 @@
-// LocalConv 3x3 on NHWC tensors, second-generation kernels (sm_100a).
+// LocalConv 3x3 on NHWC tensors, second-generation kernels (sm_90a).
 //
-// First-generation kernels (agg_zeropad.cu) were instruction-issue bound: ncu showed ~640 issued instructions per
-// 8 outputs, 10% of them FMAs (profiles/r01_agg_v1_ncu.md).  These kernels remove that overhead:
-//   * bf16/fp16 operands feed the FMA directly through the sm_100 mixed-precision instruction
-//     `fma.rn.f32.{bf16,f16}` (SASS FHFMA): no unpack/convert instructions, fp32 accumulation;
+// First-generation kernels (agg_zeropad.cu) are instruction-issue bound: most issued instructions per output are address
+// arithmetic, not FMAs.  These kernels remove that overhead:
+//   * bf16/fp16 operands are widened to fp32 (exact) and accumulated with fp32 FMAs;
 //   * a 2-D grid gives every CTA one image row, so pixel coordinates need no runtime div/mod, and all tap offsets
 //     are 32-bit immediates added to one base pointer;
 //   * forward / dX: each thread produces PX=2 horizontally adjacent pixels of one 16-byte channel packet and

@@ -1,7 +1,7 @@
-// LocalConv 3x3 forward on NHWC tensors, third generation: persistent CTAs fed by a TMA pipeline (sm_100a).
+// LocalConv 3x3 forward on NHWC tensors, third generation: persistent CTAs fed by a TMA pipeline (sm_90a).
 //
-// ncu of the second generation (profiles/r01_agg_v2_ncu.md) shows the register-resident kernels are LATENCY bound:
-// 105 registers -> 2 CTAs/SM, 8 resident warps, every warp stalled on `long_scoreboard` (global loads), DRAM at 18 %.
+// The register-resident second-generation kernels are LATENCY bound: ~105 registers -> 2 CTAs/SM, 8 resident warps, every
+// warp stalled on global loads.
 // This kernel decouples the memory stream from the math:
 //   * warp 0 is a TMA producer: per tile it issues cp.async.bulk.tensor loads of the input band WITH its halo
 //     (4-D box {128 B of channels, W+2, TH+2, 1} fetched at (c0, -1, h0-1, n): out-of-bounds coordinates are
@@ -9,7 +9,7 @@
 //     shared-memory ring guarded by mbarriers (complete_tx);
 //   * the other warps consume: one thread per (pixel, 16-byte channel packet), operands read from shared memory
 //     with conflict-free 16-byte accesses (input rows are 128B-swizzled by TMA; the 8 lanes sharing a weight packet
-//     broadcast), bf16/fp16 through the mixed-precision FMA (FHFMA), result stored straight to global, coalesced;
+//     broadcast), bf16/fp16 widened into fp32 FMAs, result stored straight to global, coalesced;
 //   * CTAs are persistent (grid = resident CTAs), tiles = (sample, band of TH image rows) taken round-robin.
 // Weight layout: COTB200_NHWC_TAP (tap-major chunks of gc weight channels) -- the block-internal layout.
 #include <cuda.h>
@@ -341,7 +341,7 @@ agg3_eval_tma_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_cons
         last_n = n;
       }
       // k of this thread's pixels: issued now, consumed in the epilogue -- the global-load latency hides behind the TMA wait,
-      // the prologue and the tap loop (loading it at the point of use exposed ~1 us per item)
+      // the prologue and the tap loop (loading it at the point of use exposes its latency per item)
       const T* kt = kg + n * p.y_sn + (long long)h0 * p.W * p.y_sp;
       Pack<T, VEC> kpre[MAXI];
 #pragma unroll

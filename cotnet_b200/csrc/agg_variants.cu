@@ -1,4 +1,4 @@
-// The remaining LocalConv variants of the reference's cupy_layers package (SURVEY.md section 8f rank 4), sm_100a:
+// The remaining LocalConv variants of the reference's cupy_layers package (SURVEY.md section 8f rank 4), sm_90a:
 //
 //   aggregation_refpad            reflect padding          /root/reference/cupy_layers/aggregation_refpad.py:21-127
 //   aggregation_zeropad_dilate    per-weight-channel dilation, 3x3, stride 1   .../aggregation_zeropad_dilate.py:20-146

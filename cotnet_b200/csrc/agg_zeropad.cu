@@ -1,4 +1,4 @@
-// LocalConv ("aggregation_zeropad") kernels for sm_100a.
+// LocalConv ("aggregation_zeropad") kernels for sm_90a.
 //
 // Replaces the reference's NVRTC string kernels
 //   aggregation_zeropad_forward_kernel          /root/reference/cupy_layers/aggregation_zeropad.py:20-46

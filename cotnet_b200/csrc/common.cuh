@@ -1,4 +1,4 @@
-// Shared helpers for libcotb200 (sm_100a).  Host-side error plumbing + device-side element traits.
+// Shared helpers for libcotb200 (sm_90a).  Host-side error plumbing + device-side element traits.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -56,7 +56,7 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&s, cudaDevAttrMultiProcessorCount, dev);
-    if (s <= 0) s = 148;
+    if (s <= 0) s = 132;
   }
   return s;
 }
@@ -132,24 +132,101 @@ template <> __device__ __forceinline__ double to_acc<double>(double v) { return 
 template <> __device__ __forceinline__ float to_acc<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
 template <> __device__ __forceinline__ float to_acc<__half>(__half v) { return __half2float(v); }
 
-// d = a*b + c with 16-bit a, b consumed directly (sm_100 mixed-precision FMA, SASS FHFMA with .H0/.H1 operand selectors):
-// no unpack instructions in reductions over bf16/fp16 tensors.  Exact products, fp32 accumulation.
+// d = a*b + c with 16-bit a, b widened to fp32 and one fp32 FMA.  The product of two bf16 (or two fp16) values is exact in
+// fp32, so this is the single-rounding a*b + c.  (sm_90 has no mixed-precision fma.f32.bf16.)
 template <typename T> __device__ __forceinline__ float mfma(T a, T b, float c);
 template <> __device__ __forceinline__ float mfma<float>(float a, float b, float c) { return fmaf(a, b, c); }
 template <> __device__ __forceinline__ float mfma<__nv_bfloat16>(__nv_bfloat16 a, __nv_bfloat16 b, float c) {
-  float d;
-  asm("fma.rn.f32.bf16 %0, %1, %2, %3;" : "=f"(d) : "h"(__bfloat16_as_ushort(a)), "h"(__bfloat16_as_ushort(b)), "f"(c));
-  return d;
+  return fmaf(__bfloat162float(a), __bfloat162float(b), c);
 }
 template <> __device__ __forceinline__ float mfma<__half>(__half a, __half b, float c) {
-  float d;
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(d) : "h"(__half_as_ushort(a)), "h"(__half_as_ushort(b)), "f"(c));
-  return d;
+  return fmaf(__half2float(a), __half2float(b), c);
 }
 template <typename T> __device__ __forceinline__ T one_of();
 template <> __device__ __forceinline__ float one_of<float>() { return 1.f; }
 template <> __device__ __forceinline__ __nv_bfloat16 one_of<__nv_bfloat16>() { return __ushort_as_bfloat16((unsigned short)0x3F80); }
 template <> __device__ __forceinline__ __half one_of<__half>() { return __ushort_as_half((unsigned short)0x3C00); }
+
+// ---------------------------------------------------------------- deterministic cross-CTA sums
+// Floating-point atomics add the partial sums of the CTAs in the order the CTAs happen to finish, so such a sum changes from run
+// to run in its last bits, and a training run amplifies that into different weights.  Instead every CTA of a group stores its
+// partials to its own row of a scratch area and the LAST CTA of the group to arrive (ticket counters) adds the rows in row order.
+// The scratch of a launch is stream-ordered: DetScratch allocates it with cudaMallocAsync and zeroes its tickets with
+// cudaMemsetAsync on the launch's stream, and frees it with cudaFreeAsync on that stream after the launch (under graph capture
+// these become the graph's own allocation / memset / free nodes).  Launches on different streams never share scratch.
+struct DetArena { float* scr; unsigned* tick; };
+static constexpr int DET_TICKETS_PER_GROUP = 64;   // one reduction = 1 final ticket + up to 63 first-level tickets
+
+struct DetScratch {
+  DetArena a{nullptr, nullptr};
+  void* base = nullptr;
+  cudaStream_t st = nullptr;
+  // `floats` of scratch and `groups` independent reductions' tickets, on stream s
+  int alloc(size_t floats, int groups, cudaStream_t s) {
+    st = s;
+    const size_t tick_bytes = ((size_t)groups * DET_TICKETS_PER_GROUP * sizeof(unsigned) + 255) & ~(size_t)255;
+    cudaError_t e = cudaMallocAsync(&base, tick_bytes + floats * sizeof(float), st);
+    if (e == cudaSuccess && tick_bytes) e = cudaMemsetAsync(base, 0, tick_bytes, st);
+    if (e != cudaSuccess) { set_error("reduction scratch (%zu floats): %s", floats, cudaGetErrorString(e)); return (int)e; }
+    a.tick = (unsigned*)base;
+    a.scr = (float*)((char*)base + tick_bytes);
+    return 0;
+  }
+  ~DetScratch() { if (base) cudaFreeAsync(base, st); }
+};
+
+// Two levels keep the serial tail short: the rows are added in fixed blocks of `fan` rows by the last CTA of each block, the
+// block totals by the last block.  Everything about the order is a function of nslots only.
+__host__ __device__ __forceinline__ int det_fan(int nslots) {
+  const int f = (nslots + DET_TICKETS_PER_GROUP - 2) / (DET_TICKETS_PER_GROUP - 1);
+  return f < 16 ? 16 : f;
+}
+__host__ __device__ __forceinline__ int det_blocks(int nslots) { return (nslots + det_fan(nslots) - 1) / det_fan(nslots); }
+// floats of scratch one reduction of nslots rows of n values uses (its rows + the block totals)
+__host__ __device__ __forceinline__ size_t det_floats(int nslots, int n) { return (size_t)(nslots + det_blocks(nslots)) * n; }
+
+template <bool NAMED>
+__device__ __forceinline__ void det_bar(int nthr) {
+  if constexpr (NAMED) asm volatile("bar.sync 1, %0;" ::"r"(nthr) : "memory");
+  else __syncthreads();
+}
+
+// Adds rows [j0, j1) of scr (row pitch n) in row order, element k: four independent chains j = j0 + 4i + q added as ((0+1)+(2+3)).
+__device__ __forceinline__ float det_sum_rows(const float* scr, int n, int j0, int j1, int k) {
+  float t[4] = {0.f, 0.f, 0.f, 0.f};
+  int j = j0;
+  for (; j + 3 < j1; j += 4) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) t[q] += __ldcg(scr + (size_t)(j + q) * n + k);
+  }
+  for (int q = 0; j < j1; ++j, ++q) t[q] += __ldcg(scr + (size_t)j * n + k);
+  return (t[0] + t[1]) + (t[2] + t[3]);
+}
+
+// scr: the reduction's det_floats(nslots, n) area, rows [0, nslots) = one per CTA; ticket: its DET_TICKETS_PER_GROUP counters,
+// zeroed by DetScratch.  Every participating thread (tid < nthr; NAMED: barrier 1 instead of __syncthreads) calls this after
+// the CTA stored its own row `slot`.  add(k, total) runs in exactly one CTA with the run-to-run identical total of element k.
+template <bool NAMED = false, class F>
+__device__ __forceinline__ void det_finish(float* scr, int n, int slot, int nslots, unsigned* ticket, int tid, int nthr, F add) {
+  __shared__ unsigned s_det_last;
+  const int fan = det_fan(nslots), nblk = det_blocks(nslots), blk = slot / fan;
+  const int j0 = blk * fan, j1 = min(nslots, j0 + fan);
+  float* btot = scr + (size_t)nslots * n;
+  __threadfence();
+  det_bar<NAMED>(nthr);
+  if (tid == 0) s_det_last = atomicAdd(ticket + 1 + blk, 1u) == (unsigned)(j1 - j0 - 1) ? 1u : 0u;
+  det_bar<NAMED>(nthr);
+  if (!s_det_last) return;
+  __threadfence();
+  for (int k = tid; k < n; k += nthr) btot[(size_t)blk * n + k] = det_sum_rows(scr, n, j0, j1, k);
+  __threadfence();
+  det_bar<NAMED>(nthr);
+  if (tid == 0) s_det_last = atomicAdd(ticket, 1u) == (unsigned)(nblk - 1) ? 1u : 0u;
+  det_bar<NAMED>(nthr);
+  if (!s_det_last) return;
+  __threadfence();
+  for (int k = tid; k < n; k += nthr) add(k, det_sum_rows(btot, n, 0, nblk, k));
+}
 
 // dtype dispatch on the host
 #define COTB200_DISPATCH_DTYPE(dtype, ...)                                   \

@@ -1,4 +1,4 @@
-// GroupNorm over the 9 taps of each weight channel, second generation: "blocks of 72" staged by bulk async copies (sm_100a).
+// GroupNorm over the 9 taps of each weight channel, second generation: "blocks of 72" staged by bulk async copies (sm_90a).
 //
 // The logits l [B, HW, 9*wc] are in the reference channel order j = g*9 + t (models/cotnet.py:55-56), the normalised
 // weights ghat (and their gradient) in the tap-major order the LocalConv kernels read: chunk of 8 weight channels, position
@@ -7,13 +7,13 @@
 // 144-byte block, and the whole tensor is a flat array of such blocks.
 //
 // The first-generation kernels (norm_tail.cu) did that transpose with stride-9 scalar gathers from global memory:
-// 9 load instructions per 8 elements, 0.19-0.38 of the HBM roof (profiles/r01_bench_model_run11.json).  Here
+// 9 load instructions per 8 elements, far below the HBM roof.  Here
 //   * a CTA moves its tile (256 consecutive blocks, 36 KB) with ONE cp.async.bulk global->shared (mbarrier complete_tx)
 //     and writes its result with ONE cp.async.bulk shared->global: address generation leaves the SM's LSU entirely;
 //   * apply / bwd_apply: thread = one block, 9 conflict-free 16-byte shared loads, the transpose is register renaming
 //     (fully unrolled), per-(sample, column) coefficients come from a table in shared memory (broadcast reads);
 //   * stats: thread = one block, 8 group sums by warp shuffles;
-//   * bwd_sums: thread = one column, 16-bit shared loads, three mixed-precision FMAs per element (FHFMA on the bf16
+//   * bwd_sums: thread = one column, 16-bit shared loads, three fp32 FMAs per element (on the widened bf16
 //     operands: sum dg, sum dg*l, sum l), per-(sample, column) partials -> a tiny finish kernel derives s1, s2, dgamma,
 //     dbeta AND the bias gradient of the embed.3 convolution analytically (no extra pass over dl).
 // Algorithmic bytes: stats J, apply 2J, bwd_sums 2J, bwd_apply 3J (x px x s) -- unchanged; the point is reaching them.
@@ -26,6 +26,7 @@ struct GN72 {
   int B, HW, wc, nchunk, J;
   int bps;              // blocks of 72 per sample = HW * nchunk
   int tb;               // blocks per tile
+  DetArena det;         // scratch + tickets of the per-sample reductions over the CTAs of a sample
 };
 
 template <typename T> struct G7 {
@@ -56,7 +57,7 @@ __device__ __forceinline__ void g7_st_block(uint32_t sa, const T (&v)[72]) {
 // ------------------------------------------------------------------------------------------------ statistics
 // gsum[b,g] += sum_{t,px} (l + lbias) ; gsq likewise.   grid (X, B): CTA (x, b) walks the tiles x, x+X, .. of sample b with a
 // two-stage bulk-copy ring.  Thread = one block per tile; it keeps 72 per-COLUMN sums of the raw l and 8 per-group sums of
-// l^2, both by mixed-precision FMAs on the 16-bit operands (144 FHFMA + 9 LDS.128 per 144 bytes, no unpack, no per-element
+// l^2, both by fp32 FMAs on the widened 16-bit operands (9 LDS.128 per 144 bytes, no per-element
 // bias loads); the bias enters analytically at the end:  sum (l+b) = S_j + n*b_j,  sum (l+b)^2 = Q_g + 2*sum_t b_j*S_j + n*b_j^2.
 template <typename T>
 __global__ void __launch_bounds__(G7<T>::TB)
@@ -134,18 +135,22 @@ gn72_stats_kernel(const T* __restrict__ l, const float* __restrict__ lbias, floa
       q[i] += __shfl_xor_sync(0xffffffffu, q[i], off);
     }
   }
-  if ((tid & 31) < g.nchunk) {
+  // warps add their chunk totals in warp order (run-to-run identical sums), then the CTAs of the sample in CTA order
+  for (int w = 0; w < TB / 32; ++w) {
+    if (tid >> 5 == w && (tid & 31) < g.nchunk) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      atomicAdd(&s_acc[chunk * 8 + i], s[i]);
-      atomicAdd(&s_acc[g.wc + chunk * 8 + i], q[i]);
+      for (int i = 0; i < 8; ++i) {
+        s_acc[chunk * 8 + i] += s[i];
+        s_acc[g.wc + chunk * 8 + i] += q[i];
+      }
     }
+    __syncthreads();
   }
-  __syncthreads();
-  for (int gi = tid; gi < g.wc; gi += TB) {
-    atomicAdd(gsum + (long long)b * g.wc + gi, s_acc[gi]);
-    atomicAdd(gsq + (long long)b * g.wc + gi, s_acc[g.wc + gi]);
-  }
+  float* scr = g.det.scr + b * det_floats(gridDim.x, 2 * g.wc);
+  for (int i = tid; i < 2 * g.wc; i += TB) scr[(size_t)blockIdx.x * 2 * g.wc + i] = s_acc[i];
+  det_finish(scr, 2 * g.wc, blockIdx.x, gridDim.x, g.det.tick + b * DET_TICKETS_PER_GROUP, tid, TB, [&](int k, float t) {
+    if (k < g.wc) gsum[(long long)b * g.wc + k] += t; else gsq[(long long)b * g.wc + k - g.wc] += t;
+  });
 }
 
 // ------------------------------------------------------------------------------------------------ apply
@@ -206,7 +211,7 @@ __global__ void __launch_bounds__(G7_SUM_THREADS)
 gn72_bwd_sums_kernel(const T* __restrict__ dg, const T* __restrict__ l, float* __restrict__ P, GN72 g) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar;
-  __shared__ float s_p[3 * 576];
+  __shared__ float s_lane[3 * 576];                               // [3][RL][J] per-row-lane partials (J * RL <= 576)
   constexpr int TB = G7<T>::TB;
   const int tid = threadIdx.x, b = blockIdx.y;
   const int PR = TB / g.nchunk;                                   // pixels per tile
@@ -222,11 +227,11 @@ gn72_bwd_sums_kernel(const T* __restrict__ dg, const T* __restrict__ l, float* _
     bulk_load(smem_u32(s_dg), dg + goff, bytes, smem_u32(&bar));
     bulk_load(smem_u32(s_l), l + goff, bytes, smem_u32(&bar));
   }
-  for (int i = tid; i < 3 * g.J; i += G7_SUM_THREADS) s_p[i] = 0.f;
   __syncthreads();
   mbar_wait(smem_u32(&bar), 0);
   const int RL = G7_SUM_THREADS >= g.J ? G7_SUM_THREADS / g.J : 1;        // row lanes per column
-  for (int c = tid; c < g.J * RL; c += G7_SUM_THREADS) {
+  const int JR = g.J * RL;
+  for (int c = tid; c < JR; c += G7_SUM_THREADS) {
     const int j = c % g.J, rl = c / g.J;
     const int gi = j / 9, t = j - gi * 9;
     const int pos = (gi >> 3) * 72 + t * 8 + (gi & 7);
@@ -239,13 +244,21 @@ gn72_bwd_sums_kernel(const T* __restrict__ dg, const T* __restrict__ l, float* _
       a1 = mfma<T>(d, lv, a1);
       a2 = mfma<T>(lv, one, a2);
     }
-    atomicAdd(&s_p[j], a0);
-    atomicAdd(&s_p[g.J + j], a1);
-    atomicAdd(&s_p[2 * g.J + j], a2);
+    s_lane[c] = a0;
+    s_lane[JR + c] = a1;
+    s_lane[2 * JR + c] = a2;
   }
   __syncthreads();
+  // the CTA's row: row-lane partials added in lane order (run-to-run identical), then across the CTAs of the sample
   float* Pb = P + (long long)b * 3 * g.J;
-  for (int i = tid; i < 3 * g.J; i += G7_SUM_THREADS) atomicAdd(Pb + i, s_p[i]);
+  float* scr = g.det.scr + b * det_floats(gridDim.x, 3 * g.J);
+  for (int i = tid; i < 3 * g.J; i += G7_SUM_THREADS) {
+    const int pl = i / g.J, j = i - pl * g.J;
+    float v = 0.f;
+    for (int rl = 0; rl < RL; ++rl) v += s_lane[pl * JR + rl * g.J + j];
+    scr[(size_t)blockIdx.x * 3 * g.J + i] = v;
+  }
+  det_finish(scr, 3 * g.J, blockIdx.x, gridDim.x, g.det.tick + b * DET_TICKETS_PER_GROUP, tid, G7_SUM_THREADS, [&](int k, float t) { Pb[k] += t; });
 }
 
 // CTA = one group g, thread = sample b (strided): s1, s2 of (b, g) are written; the group's 9 columns of dgamma / dbeta /
@@ -399,7 +412,7 @@ static int g7_smem_attr(KFn fn, size_t smem) {
 template <typename T>
 int gn72_stats_launch(int B, int HW, int wc, const void* l, const float* lbias, float* gsum, float* gsq, cudaStream_t st) {
   constexpr int TB = G7<T>::TB;
-  const GN72 g = make_gn72(B, HW, wc, TB);
+  GN72 g = make_gn72(B, HW, wc, TB);
   const size_t smem = (size_t)2 * TB * 72 * sizeof(T);
   int rc = g7_smem_attr(gn72_stats_kernel<T>, smem);
   if (rc) return rc;
@@ -408,6 +421,9 @@ int gn72_stats_launch(int B, int HW, int wc, const void* l, const float* lbias, 
   int X = (4 * num_sms() + B - 1) / B;
   if (X > ntiles) X = ntiles;
   if (X < 1) X = 1;
+  DetScratch ds;
+  if ((rc = ds.alloc(B * det_floats(X, 2 * wc), B, st))) return rc;
+  g.det = ds.a;
   gn72_stats_kernel<T><<<dim3(X, B), TB, smem, st>>>((const T*)l, lbias, gsum, gsq, g);
   return check_launch("gn9_stats(gn72)");
 }
@@ -427,11 +443,14 @@ int gn72_apply_launch(int B, int HW, int wc, const void* l, const float* lbias, 
 template <typename T>
 int gn72_bwd_sums_launch(int B, int HW, int wc, const void* dg, const void* l, float* P, cudaStream_t st) {
   constexpr int TB = G7<T>::TB;
-  const GN72 g = make_gn72(B, HW, wc, TB);
+  GN72 g = make_gn72(B, HW, wc, TB);
   const size_t smem = (size_t)2 * TB * 72 * sizeof(T);
   int rc = g7_smem_attr(gn72_bwd_sums_kernel<T>, smem);
   if (rc) return rc;
   const int PR = TB / g.nchunk;
+  DetScratch ds;
+  if ((rc = ds.alloc(B * det_floats((HW + PR - 1) / PR, 3 * g.J), B, st))) return rc;
+  g.det = ds.a;
   gn72_bwd_sums_kernel<T><<<dim3((HW + PR - 1) / PR, B), G7_SUM_THREADS, smem, st>>>((const T*)dg, (const T*)l, P, g);
   return check_launch("gn9_bwd_sums(gn72)");
 }

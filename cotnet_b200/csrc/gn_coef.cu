@@ -1,4 +1,4 @@
-// GroupNorm(9 taps) statistics from per-sample COLUMN sums (sm_100a).
+// GroupNorm(9 taps) statistics from per-sample COLUMN sums (sm_90a).
 //
 // The logits GEMM (embed.3, models/cotnet.py:55) can emit, from its epilogue, the per-sample column sums of its raw
 // accumulator: csum[b, j] = sum_px acc[b, px, j], csq[b, j] = sum_px acc^2 (cotb200_gemm_bf16_samplestats).  GroupNorm's

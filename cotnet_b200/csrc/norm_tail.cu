@@ -1,4 +1,4 @@
-// Fused normalisation / split-attention kernels of the CoT block on NHWC tensors (sm_100a, HBM-bound).
+// Fused normalisation / split-attention kernels of the CoT block on NHWC tensors (sm_90a, HBM-bound).
 //
 // They replace long chains of eager element-wise / reduction launches of the reference block
 // (/root/reference/models/cotnet.py:89-104 and the GroupNorm at :56), each a full HBM round trip:
@@ -9,7 +9,7 @@
 //
 // One skeleton: a CTA owns (sample b, a chunk of rows); threads are (tx = 16-byte channel packet, ty = row lane), so a
 // warp always touches whole 128-byte lines; per-column partial sums live in registers, are reduced across ty through
-// shared memory and leave the CTA as ONE atomicAdd per column.
+// shared memory and leave the CTA through one deterministic reduction per column (det_cols).
 #include "common.cuh"
 
 namespace cotb200 {
@@ -23,6 +23,7 @@ struct RowsGeo {
   int ry;                // row lanes = NT_THREADS / cq_pad
   int cq_pad;            // power-of-two >= cq (thread x extent)
   int ld;                // row pitch in elements (== C unless the columns are processed in chunks)
+  DetArena det;          // scratch + tickets of the closing column reductions (det_cols)
 };
 
 // fast sigmoid: ex2 + approximate reciprocal (2 ulp) instead of an IEEE division (~10 instructions) per element
@@ -60,16 +61,18 @@ __device__ __forceinline__ void cta_col_reduce(float (&acc)[NS][VEC], float* sm,
   __syncthreads();
 }
 
-// dst[c] += src[c] for c < C: the CTA's column totals leave as 16-byte vector reductions (red.global.add.v4.f32: one L2 atomic
-// transaction per four columns) where the destination allows, scalar atomics otherwise.
-__device__ __forceinline__ void red_add_cols(float* __restrict__ dst, const float* __restrict__ src, int C) {
-  if ((C & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-    for (int c = threadIdx.x * 4; c < C; c += NT_THREADS * 4)
-      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + c), "f"(src[c]), "f"(src[c + 1]), "f"(src[c + 2]), "f"(src[c + 3]) : "memory");
-  } else {
-    for (int c = threadIdx.x; c < C; c += NT_THREADS) atomicAdd(dst + c, src[c]);
-  }
+// The CTA's n partial values val(k) leave through det_finish (common.cuh): one group over the whole grid, or (per_sample) one
+// group per sample b = blockIdx.y.  add(k, total) receives the run-to-run identical total of element k.
+template <class V, class F>
+__device__ __forceinline__ void det_cols(const RowsGeo& g, bool per_sample, int n, V val, F add) {
+  const int nslots = per_sample ? gridDim.x : gridDim.x * gridDim.y;
+  const int slot = per_sample ? blockIdx.x : blockIdx.y * gridDim.x + blockIdx.x;
+  float* scr = g.det.scr + (per_sample ? blockIdx.y * det_floats(nslots, n) : 0);
+  for (int k = threadIdx.x; k < n; k += NT_THREADS) scr[(size_t)slot * n + k] = val(k);
+  det_finish(scr, n, slot, nslots, g.det.tick + (per_sample ? blockIdx.y : 0) * DET_TICKETS_PER_GROUP, threadIdx.x, NT_THREADS, add);
 }
+// the first `ns` CTA total planes of cta_col_reduce (sm[(s * ry) * C + c], s < ns) as val(k), k = s * C + c
+#define NT_PLANES(sm, g) [&](int k) { const int s_ = k / (g).C; return (sm)[(s_ * (g).ry) * (g).C + (k - s_ * (g).C)]; }
 
 // ------------------------------------------------------------------------------------------------ column statistics
 // sum[c] += sum_rows x, sq[c] += sum_rows x^2       (BatchNorm batch statistics of u, models/cotnet.py:89)
@@ -93,8 +96,7 @@ col_stats_kernel(const T* __restrict__ x, float* __restrict__ sum, float* __rest
     }
   }
   cta_col_reduce<2, VEC>(acc, sm, g, tx, ty, active);
-  red_add_cols(sum, sm, g.C);
-  red_add_cols(sq, sm + g.ry * g.C, g.C);
+  det_cols(g, false, 2 * g.C, NT_PLANES(sm, g), [&](int k, float t) { if (k < g.C) sum[k] += t; else sq[k - g.C] += t; });
 }
 
 // ------------------------------------------------------------------------------------------------ tail forward
@@ -125,7 +127,7 @@ tail_pool_kernel(const T* __restrict__ u, const T* __restrict__ k, const float* 
     }
   }
   cta_col_reduce<1, VEC>(acc, sm, g, tx, ty, active);
-  red_add_cols(psum + (long long)b * g.C, sm, g.C);
+  det_cols(g, true, g.C, NT_PLANES(sm, g), [&](int k, float t) { psum[(long long)b * g.C + k] += t; });
 }
 
 // out = a0 * silu(u*scale+shift) + a1 * k        a: [B, C, 2] fp32          (models/cotnet.py:101-104)
@@ -190,10 +192,10 @@ tail_bwd_sums_kernel(const T* __restrict__ dout, const T* __restrict__ u, const 
     }
   }
   cta_col_reduce<2, VEC>(acc, sm, g, tx, ty, active);
-  for (int c = threadIdx.x; c < g.C; c += NT_THREADS) {
-    atomicAdd(S + ((long long)b * g.C + c) * 2, sm[c]);
-    atomicAdd(S + ((long long)b * g.C + c) * 2 + 1, sm[g.ry * g.C + c]);
-  }
+  det_cols(g, true, 2 * g.C, NT_PLANES(sm, g), [&](int k, float t) {
+    const int c = k < g.C ? k : k - g.C;
+    S[((long long)b * g.C + c) * 2 + (k < g.C ? 0 : 1)] += t;
+  });
 }
 
 // dz = (a0*dout + dpn) * silu'(z),  z = u*scale+shift  -- the gradient entering the BatchNorm.
@@ -234,8 +236,7 @@ tail_bwd_dz_sums_kernel(const T* __restrict__ dout, const T* __restrict__ u, con
     }
   }
   cta_col_reduce<2, VEC>(acc, sm, g, tx, ty, active);
-  red_add_cols(sum_dz, sm, g.C);
-  red_add_cols(sum_dzx, sm + g.ry * g.C, g.C);
+  det_cols(g, false, 2 * g.C, NT_PLANES(sm, g), [&](int k, float t) { if (k < g.C) sum_dz[k] += t; else sum_dzx[k - g.C] += t; });
 }
 
 // du = scale * (dz - c1 - xhat*c2)   [c1 = sum_dz/n, c2 = sum_dzx/n in training; 0 in eval]
@@ -374,8 +375,7 @@ bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T*
     }
   }
   cta_col_reduce<2, VEC>(acc, sm, g, tx, ty, active);
-  red_add_cols(sum_dz, sm, g.C);
-  red_add_cols(sum_dzx, sm + g.ry * g.C, g.C);
+  det_cols(g, false, 2 * g.C, NT_PLANES(sm, g), [&](int k, float t) { if (k < g.C) sum_dz[k] += t; else sum_dzx[k - g.C] += t; });
 }
 
 // dx = scale * (dz - c1 - xhat*c2)   (c1 = c2 = 0 in eval mode);   dres = dz when RES
@@ -487,12 +487,12 @@ gn_stats_kernel(const T* __restrict__ l, const float* __restrict__ lbias, float*
     }
   }
   cta_col_reduce<2, VEC>(acc, sm, g, tx, ty, active);
-  for (int gi = threadIdx.x; gi < wc; gi += NT_THREADS) {      // fold the 9 tap columns of each group
-    float s = 0.f, q = 0.f;
-    for (int t = 0; t < 9; ++t) { s += sm[gi * 9 + t]; q += sm[g.ry * g.C + gi * 9 + t]; }
-    atomicAdd(gsum + (long long)b * wc + gi, s);
-    atomicAdd(gsq + (long long)b * wc + gi, q);
-  }
+  det_cols(g, true, 2 * wc, [&](int k) {                        // fold the 9 tap columns of each group
+    const int pl = k < wc ? 0 : 1, gi = k - pl * wc;
+    float s = 0.f;
+    for (int t = 0; t < 9; ++t) s += sm[pl * g.ry * g.C + gi * 9 + t];
+    return s;
+  }, [&](int k, float t) { if (k < wc) gsum[(long long)b * wc + k] += t; else gsq[(long long)b * wc + k - wc] += t; });
 }
 
 // ghat[pos(j)] = (l[j] - mean[b,g]) * rstd[b,g] * gamma[j] + beta[j].  Thread = one OUTPUT packet (coalesced 16-byte
@@ -570,11 +570,7 @@ gn_bwd_sums_kernel(const T* __restrict__ dg, const T* __restrict__ l, const floa
   }
   cta_col_reduce<3, VEC>(acc, sm, g, tx, ty, active);
   float* Pb = P + (long long)b * 3 * g.C;
-  for (int j = threadIdx.x; j < g.C; j += NT_THREADS) {
-    atomicAdd(Pb + j, sm[j]);
-    atomicAdd(Pb + g.C + j, sm[g.ry * g.C + j]);
-    atomicAdd(Pb + 2 * g.C + j, sm[2 * g.ry * g.C + j]);
-  }
+  det_cols(g, true, 3 * g.C, NT_PLANES(sm, g), [&](int k, float t) { Pb[k] += t; });
 }
 
 // dl = rstd * ( dg*gamma - s1/n - lhat * s2/n ),  n = 9*HW
@@ -655,6 +651,16 @@ static int make_geo(RowsGeo& g, int B, int HW, int C, int vec, int nsums, size_t
   return 0;
 }
 
+// Stream-ordered scratch of the closing reduction of a reducing row kernel (det_cols) with geometry g and `nsums` planes of
+// g.C values: one group over the whole grid or one per sample, whichever the kernel uses.
+static int det_geo(DetScratch& ds, RowsGeo& g, int nsums, cudaStream_t st) {
+  const int gx = (g.HW + g.rows_per_cta - 1) / g.rows_per_cta, n = nsums * g.C;
+  const size_t per_sample = (size_t)g.B * det_floats(gx, n), whole = det_floats(gx * g.B, n);
+  const int rc = ds.alloc(per_sample > whole ? per_sample : whole, g.B, st);
+  g.det = ds.a;
+  return rc;
+}
+
 // Wide tensors (more than 256 packets per row, e.g. the 2048-channel bn3 of layer4 in fp32) are processed in equal
 // column chunks: returns the chunk width (a multiple of vec that divides C) or C itself.
 static int col_chunk(int C, int vec) {
@@ -714,6 +720,8 @@ extern "C" int cotb200_col_stats(int dtype, int B, int HW, int C, const void* x,
         RowsGeo g; size_t smem;
         int rc = make_geo(g, B, HW, cw, vec, 2, &smem);
         if (rc) return rc;
+        DetScratch ds;                                   // stream-ordered scratch of the closing reduction
+        if ((rc = det_geo(ds, g, 2, st))) return rc;
         g.ld = C;
         COTB200_PROF_B("col_stats", (double)B * HW * cw * sizeof(T));
         NT_DISPATCH_VEC(vec, { if ((rc = ensure_smem(col_stats_kernel<T, V>, smem))) return rc;
@@ -737,6 +745,8 @@ extern "C" int cotb200_tail_pool(int dtype, int B, int HW, int C, const void* u,
       RowsGeo g; size_t smem;
       int rc = make_geo(g, B, HW, C, vec, 1, &smem);
       if (rc) return rc;
+      DetScratch ds;                                   // stream-ordered scratch of the closing reduction
+      if ((rc = det_geo(ds, g, 1, st))) return rc;
       COTB200_PROF_B("tail_pool", (double)B * HW * C * 2 * sizeof(T));
       NT_DISPATCH_VEC(vec, { if ((rc = ensure_smem(tail_pool_kernel<T, V>, smem))) return rc;
                              tail_pool_kernel<T, V><<<NT_GRID, NT_THREADS, smem, st>>>((const T*)u, (const T*)k, scale, shift, psum, g); });
@@ -776,6 +786,8 @@ extern "C" int cotb200_tail_bwd_sums(int dtype, int B, int HW, int C, const void
       RowsGeo g; size_t smem;
       int rc = make_geo(g, B, HW, C, vec, 2, &smem);
       if (rc) return rc;
+      DetScratch ds;                                   // stream-ordered scratch of the closing reduction
+      if ((rc = det_geo(ds, g, 2, st))) return rc;
       COTB200_PROF_B("tail_bwd_sums", (double)B * HW * C * 3 * sizeof(T));
       NT_DISPATCH_VEC(vec, { if ((rc = ensure_smem(tail_bwd_sums_kernel<T, V>, smem))) return rc;
                              tail_bwd_sums_kernel<T, V><<<NT_GRID, NT_THREADS, smem, st>>>((const T*)dout, (const T*)u, (const T*)k, scale, shift, S, g); });
@@ -797,6 +809,8 @@ extern "C" int cotb200_tail_bwd_dz_sums(int dtype, int B, int HW, int C, const v
       RowsGeo g; size_t smem;
       int rc = make_geo(g, B, HW, C, vec, 2, &smem);
       if (rc) return rc;
+      DetScratch ds;                                   // stream-ordered scratch of the closing reduction
+      if ((rc = det_geo(ds, g, 2, st))) return rc;
       COTB200_PROF_B("tail_bwd_dz_sums", (double)B * HW * C * 2 * sizeof(T));
       NT_DISPATCH_VEC(vec, { if ((rc = ensure_smem(tail_bwd_dz_sums_kernel<T, V>, smem))) return rc;
                              tail_bwd_dz_sums_kernel<T, V><<<NT_GRID, NT_THREADS, smem, st>>>((const T*)dout, (const T*)u, scale, shift, mu, rstd, a, dpn, pscale, sum_dz, sum_dzx, g); });
@@ -843,6 +857,8 @@ extern "C" int cotb200_gn9_stats(int dtype, int B, int HW, int wc, int gc, const
       RowsGeo g; size_t smem;
       int rc = make_geo(g, B, HW, J, vec, 2, &smem);
       if (rc) return rc;
+      DetScratch ds;                                   // stream-ordered scratch of the closing reduction
+      if ((rc = det_geo(ds, g, 2, st))) return rc;
       NT_DISPATCH_VEC(vec, { if ((rc = ensure_smem(gn_stats_kernel<T, V>, smem))) return rc;
                              gn_stats_kernel<T, V><<<NT_GRID, NT_THREADS, smem, st>>>((const T*)l, lbias, gsum, gsq, g, wc); });
       return check_launch("gn9_stats");
@@ -894,6 +910,8 @@ extern "C" int cotb200_gn9_bwd_sums(int dtype, int B, int HW, int wc, int gc, co
           const int vec = pick_vec<T>(J, dg, l);
           RowsGeo g; size_t smem;
           if ((rc = make_geo(g, B, HW, J, vec, 3, &smem))) return rc;
+          DetScratch ds;                                   // stream-ordered scratch of the closing reduction
+          if ((rc = det_geo(ds, g, 3, st))) return rc;
           NT_DISPATCH_VEC(vec, { if ((rc = ensure_smem(gn_bwd_sums_kernel<T, V>, smem))) return rc;
                                  gn_bwd_sums_kernel<T, V><<<NT_GRID, NT_THREADS, smem, st>>>((const T*)dg, (const T*)l, lbias, mean, rstd, work, g, wc, gc); });
           if ((rc = check_launch("gn9_bwd_sums"))) return rc;
@@ -1009,6 +1027,8 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
         RowsGeo g; size_t smem;
         int rc = make_geo(g, B, HW, cw, vec, 2, &smem);
         if (rc) return rc;
+        DetScratch ds;                                   // stream-ordered scratch of the closing reduction
+        if ((rc = det_geo(ds, g, 2, st))) return rc;
         g.ld = C;
         const T* dp = (const T*)dy + c0; const T* xp = (const T*)x + c0; const T* yp = y ? (const T*)y + c0 : nullptr;
         const T* d2p = dy2 ? (const T*)dy2 + c0 : nullptr;

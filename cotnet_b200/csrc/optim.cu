@@ -1,4 +1,4 @@
-// Train-step plumbing of the data-parallel CoT path (SURVEY.md section 8f rank 3/4), sm_100a.
+// Train-step plumbing of the data-parallel CoT path (SURVEY.md section 8f rank 3/4), sm_90a.
 //
 // The reference's step (train.py:264-293) is, per parameter tensor: DDP bucket copy, optim.SGD(nesterov) update
 // (optim/optim_factory.py:54-56), ModelEmaV2 lerp over the whole state_dict (utils/model_ema.py:45-53), and -- under AMP --
@@ -14,7 +14,7 @@
 //   cotb200_multi_lerp     EMA of the buffers (BatchNorm running statistics, integer counters) by pointer table
 //   cotb200_u8_to_nhwc     uint8 NCHW batch -> (x - mean)/std in bf16/fp16/fp32 channels_last
 //
-// All HBM-bound streaming kernels: 16-byte accesses, grid = a few waves of 148 SMs, no atomics.
+// All HBM-bound streaming kernels: 16-byte accesses, grid = a few waves of 132 SMs, no atomics.
 #include "common.cuh"
 
 namespace cotb200 {
@@ -250,8 +250,8 @@ extern "C" int cotb200_u8_to_nhwc(int dtype, int N, int C, int H, int W, const v
 // (models/cotnet.py:69-77,92-101 with the BatchNorm of `se` folded: s1 = gamma * rstd, t1 = beta - mean * s1).
 // The eager form is ~10 launches of GEMV-sized ops per CoT layer.  Two tiny GEMMs [B, C] x [C, A] and [B, A] x [A, 2C]: the only
 // thing that matters is memory-level parallelism, so each is one launch of (16 samples x 32 outputs) tiles whose operands are
-// staged in shared memory with independent 16-byte loads (one latency round per 256-wide K chunk) -- the first version (one CTA
-// per 2 samples walking whole weight rows with dependent loads) took 63 us per layer at C = 512 (profiles/r02_prof_cotnet50_eval_callH.md).
+// staged in shared memory with independent 16-byte loads (one latency round per 256-wide K chunk) -- one CTA per 2 samples
+// walking whole weight rows with dependent loads is latency-bound.
 // fp32 throughout.
 namespace cotb200 {
 static constexpr int SE_TS = 16;     // samples per tile

@@ -1,9 +1,8 @@
-// 3x3 / stride 2 / pad 1 pooling on NHWC tensors (sm_100a).
+// 3x3 / stride 2 / pad 1 pooling on NHWC tensors (sm_90a).
 //
 // The CoT bottleneck down-samples with nn.AvgPool2d(3, 2, padding=1) in front of the CoT layer of every stride-2 block
-// (/root/reference/models/cotnet.py:199-202,237-238) and the trunk with nn.MaxPool2d(3, 2, 1)
-// (/root/reference/models/resnet.py:555).  ncu of the bs256 step showed ATen's channels_last pooling kernels at
-// 11.8 % of the step (avg_pool2d_backward: 1.1 ms per call for a 205 MB tensor -- ~0.3 TB/s); these are plain
+// (models/cotnet.py:199-202,237-238) and the trunk with nn.MaxPool2d(3, 2, 1) (models/resnet.py:555).  ATen's
+// channels_last pooling kernels run far below the HBM bandwidth (and its avg_pool2d backward is wrong in this torch build); these are plain
 // HBM-bound gathers: one thread per (output pixel, 16-byte channel packet), no atomics in backward (gather form).
 #include "common.cuh"
 

@@ -1,9 +1,9 @@
-// out = src0 + src1 (+ src2 + src3) over row-pitched [rows, C] views (sm_100a).
+// out = src0 + src1 (+ src2 + src3) over row-pitched [rows, C] views (sm_90a).
 //
 // Inside the CoT block x feeds three consumers (key_embed conv, the concat, conv1x1) and k two (the concat and the
-// radix-2 recombination): /root/reference/models/cotnet.py:80-84,97.  Autograd accumulates their gradients with a
+// radix-2 recombination): models/cotnet.py:80-84,97.  Autograd accumulates their gradients with a
 // chain of pairwise adds, and the concat's gradients are channel slices (pitch 2C) that ATen adds with its
-// non-vectorised strided kernel (ncu of the bs256 step: 89 launches, 58 us average).  This kernel does the whole
+// non-vectorised strided kernel (dozens of launches per step).  This kernel does the whole
 // accumulation in one pass of 16-byte packets: (n reads + 1 write) * C * rows * s bytes, HBM-bound.
 #include "common.cuh"
 

@@ -1,42 +1,44 @@
-// tcgen05 / TMEM / TMA GEMM family for the dense contractions of the CoT block (sm_100a only).
+// wgmma / TMA GEMM family for the dense contractions of the CoT block (sm_90a).
 //
 //   plain mode : D[M,N] = epi( A1[M,K1] * B1[N,K1]^T  (+ A2[M,K2] * B2[N,K2]^T) )
 //                1x1 convolutions on NHWC activations (rows = pixels).  The optional second operand pair is the
-//                concat-free form of  embed.0( cat[x, k] )  (/root/reference/models/cotnet.py:81,52).
+//                concat-free form of  embed.0( cat[x, k] )  (models/cotnet.py:81,52).
 //   conv mode  : 3x3 / pad 1 / stride 1 grouped convolution as an im2col-FREE implicit GEMM: for each tap the A
 //                tile is a 4-D TMA box {64 ch, W, hbox, bbox} of the NHWC input fetched at the tap's (dh,dw) offset;
 //                TMA's out-of-bounds zero fill IS the zero padding (key_embed.0, models/cotnet.py:44).
 //   stem mode  : 7x7 / stride 2 / pad 3 convolution of a 3-channel image (models/resnet.py:552) as a 4-tap implicit GEMM over
-//                the space-to-depth copy of the input made by stem_s2d_kernel (csrc/stem.cu): P[b, i, 2 + j, (di,dj,c)] =
+//                the space-to-depth copy of the input made by stem_s2d_kernel: P[b, i, 2 + j, (di,dj,c)] =
 //                x[b, 2i+di, 2j+dj, c], 16 channels per cell.  An output pixel's receptive field is 4 s2d rows x 4 cells x 16
 //                channels; one TMA box {64 elements, tile width, 1, 1} of a tensor map whose pixel stride (32 B) is SMALLER than
 //                its inner extent (128 B) fetches the overlapping 4-cell windows of a whole output row segment straight into the
 //                K-major A tile -- im2col done by the TMA address generator.
 //   epilogue   : per-column scale/shift (folded BatchNorm or bias), optional ReLU, bf16 store; optional per-column
-//                sum / sum-of-squares of the raw accumulator (training-mode BatchNorm statistics) reduced with a
-//                butterfly transpose-reduce in registers, one global atomic per column per CTA.
+//                sum / sum-of-squares of the stored bf16 values (training-mode BatchNorm statistics), summed
+//                per CTA in tile order and over the CTAs in CTA order (det_finish): identical from run to run.
 //
-// Structure (one CTA per 128-row x BN-col tile, 192 threads):
-//   warp 0  : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem stages, mbarrier complete_tx)
-//   warp 1  : TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128 x BN x 16, bf16 -> fp32 in TMEM)
-//   warps 2-5: epilogue (tcgen05.ld 32x32b, one TMEM lane quadrant per warp)
+// Structure (one CTA per 128-row x BN-col tile at a time, 288 threads):
+//   warps 0-7: two consumer warpgroups; warpgroup g issues the wgmma (m64n64k16, bf16 -> fp32 in registers) of rows
+//              64g .. 64g + 63 of the tile and runs the epilogue of those rows
+//   warp 8   : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem stages, mbarrier complete_tx)
 // All mbarrier waits are bounded (trap instead of hanging the GPU).
 #include <cuda.h>
 #include "common.cuh"
 #include "tma.cuh"
-#include "tc_umma.cuh"
+#include "tc_wgmma.cuh"
 
 namespace cotb200 {
 
-static constexpr int TC_BM = 128;      // UMMA M (cta_group::1)
+static constexpr int TC_BM = 128;      // rows of a tile: two warpgroups x 64
 static constexpr int TC_BK = 64;       // 64 bf16 = 128 B = one swizzle atom
 static constexpr int TC_STAGES = 6;
-static constexpr int TC_THREADS = 192;
+static constexpr int TC_THREADS = 288; // two consumer warpgroups + one producer warp
+static constexpr int TC_CONSUMERS = 256;
+static constexpr int TC_PRODUCER_WARP = 8;
 
 struct TcParams {
   int M, N;                 // valid rows (pixels) / output channels
   int rows_per_tile;        // D rows per CTA (128 plain; rows of the pixel box in conv mode)
-  int bn;                   // N tile (multiple of 16, <= 256)
+  int bn;                   // N tile (multiple of 64, <= 256)
   int mode;                 // 0 plain, 1 conv3x3, 2 stem (row-window conv)
   int kb1, kb2;             // plain: 64-wide k-blocks of operand pair 1 / 2
   int H, W, B, hbox, bbox;  // conv geometry
@@ -52,32 +54,37 @@ struct TcParams {
   float* col_sum;           // [N] or null
   float* col_sqsum;         // [N] or null
   int rows_per_sample;      // > 0: col_sum / col_sqsum are PER SAMPLE, [M / rows_per_sample, N] (GroupNorm statistics of the logits)
+  DetArena det;             // column statistics: per-CTA totals leave through det_finish (common.cuh)
 };
 
-// Butterfly transpose-reduce: each lane holds 32 column values of ITS row; afterwards lane j holds the sum over
-// the warp's 32 rows of column j.  31 shuffles instead of 32 x 5.
-__device__ __forceinline__ float warp_colsum32(float (&v)[32]) {
-  const unsigned lane = threadIdx.x & 31;
+// Writes one 64-column chunk of a warpgroup's accumulators (rows row0 .. row0 + 63 of the staging image) as bf16 after
+// scale / shift / ReLU into a 128B-swizzled [rows][128 B] slab.  sc / sh point at the chunk's 64 column constants.
+__device__ __forceinline__ void stage_chunk_bf16(const float (&acc)[32], uint32_t buf, int row0, const float* sc, const float* sh,
+                                                 int relu) {
+  const int lane = threadIdx.x & 31, wl = (threadIdx.x >> 5) & 3;
 #pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool upper = (lane & off) != 0;
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + wl * 16 + (lane >> 2) + 8 * h;
 #pragma unroll
-    for (int i = 0; i < off; ++i) {
-      const float send = upper ? v[i] : v[i + off];
-      const float keep = upper ? v[i + off] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+    for (int i = 0; i < 8; ++i) {
+      const int col = i * 8 + 2 * (lane & 3);
+      float lo = fmaf(acc[4 * i + 2 * h], sc[col], sh[col]);
+      float hi = fmaf(acc[4 * i + 2 * h + 1], sc[col + 1], sh[col + 1]);
+      if (relu) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
+      __nv_bfloat162 h2 = __floats2bfloat162_rn(lo, hi);
+      const uint32_t dst = buf + (uint32_t)(row * 128 + ((i ^ (row & 7)) << 4) + (lane & 3) * 4);
+      asm volatile("st.shared.u32 [%0], %1;" ::"r"(dst), "r"(*reinterpret_cast<uint32_t*>(&h2)) : "memory");
     }
   }
-  return v[0];
 }
 
+__device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
 // ---------------------------------------------------------------------------------------------- kernel
-// Persistent: every CTA loops over output tiles.  Three pipelines run concurrently --
-//   TMA producer  -> smem ring (full/empty mbarriers, continuous across tiles)
-//   MMA issuer    -> two TMEM accumulator buffers (tmem_full/tmem_empty mbarriers)
-//   epilogue warps drain buffer i while the MMAs of tile i+1 fill the other one.
-// (The first version launched one CTA per tile: ncu showed ~5 us of fixed per-CTA cost -- barrier init, TMEM alloc,
-//  a cold TMA round trip -- dominating tiles with 1-2 k-blocks; profiles/r01_tma_tc_ncu.md.)
+// Persistent: every CTA loops over output tiles.  The TMA producer runs ahead through a shared-memory ring (full/empty
+// mbarriers, continuous across tiles), so the operands of tile i+1 arrive while the consumer warpgroups run the epilogue of
+// tile i.  (One CTA per tile pays the fixed per-CTA cost -- barrier init, a cold TMA round trip -- on every tile, which
+// dominates tiles with 1-2 k-blocks.)
 __device__ __forceinline__ void tc_tile_origin(const TcParams& p, int tile_m, int& b0, int& h0, int& w0, long long& m0, int& rows_valid) {
   b0 = 0; h0 = 0; w0 = 0;
   if (p.mode == 0) {
@@ -102,7 +109,9 @@ __device__ __forceinline__ void tc_tile_origin(const TcParams& p, int tile_m, in
   }
 }
 
-__global__ void __launch_bounds__(TC_THREADS, 2)
+// MAXCH = most 64-column chunks of an N tile (accumulator registers per thread = 32 * MAXCH); MINB = CTAs per SM
+template <int MAXCH, int MINB>
+__global__ void __launch_bounds__(TC_THREADS, MINB)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapB1,
                const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapB2,
                const __grid_constant__ CUtensorMap mapD, const TcParams p) {
@@ -111,13 +120,13 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant_
   const int a_bytes = TC_BM * TC_BK * 2;             // 16 KB
   const int b_bytes = p.bn * TC_BK * 2;
   const int stage_bytes = a_bytes + ((b_bytes + 1023) & ~1023);
-  uint8_t* out_tile = smem + (size_t)p.stages * stage_bytes;      // [bn/64 slabs][128 rows][128 B], 128B-swizzled
-  __shared__ __align__(8) uint64_t s_full[TC_STAGES], s_empty[TC_STAGES], s_tfull[2], s_tempty[2];
-  __shared__ uint32_t s_tmem;
+  uint8_t* out_tile = smem + (size_t)p.stages * stage_bytes;      // two [128 rows][128 B] slabs, 128B-swizzled
+  __shared__ __align__(8) uint64_t s_full[TC_STAGES], s_empty[TC_STAGES];
   // per row-group partials of the tile's column statistics: [4][256] floats each, in DYNAMIC shared memory behind the two slab
   // buffers and only when statistics are requested (static tables would cost every launch its second resident CTA)
   float (*s_sum)[256] = reinterpret_cast<float (*)[256]>(out_tile + 2 * TC_BM * 128);
   float (*s_sq)[256] = s_sum + 4;
+  float* s_tot = &s_sq[4][0];                        // [2][N]: the CTA's column sums / sums of squares over all its tiles
   __shared__ __align__(16) float s_scale[256], s_shift[256];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -125,28 +134,19 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant_
   const int n_tiles = (p.N + p.bn - 1) / p.bn;
   const int total_tiles = p.m_tiles * n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA1) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB1) : "memory");
-    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(smem_u32(&s_tfull[a]), 1); mbar_init(smem_u32(&s_tempty[a]), 4); }
+    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), 2); }
     mbar_init_fence();
   }
-  uint32_t ncols = 32;
-  while ((int)ncols < 2 * p.bn) ncols <<= 1;           // two accumulator buffers
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (p.col_sum != nullptr && p.rows_per_sample == 0)
+  if (p.col_sum != nullptr && p.rows_per_sample == 0) {
     for (int i = threadIdx.x; i < 4 * 256; i += TC_THREADS) { (&s_sum[0][0])[i] = 0.f; (&s_sq[0][0])[i] = 0.f; }
-  tc_fence_before();
+    for (int i = threadIdx.x; i < 2 * p.N; i += TC_THREADS) s_tot[i] = 0.f;
+  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
-  if (warp == 0) {
+  if (warp == TC_PRODUCER_WARP) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int kbc = 0;                                      // k-block counter, continuous across tiles
@@ -184,213 +184,165 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp, warp-uniform; one elected lane issues) =====================
-    {
-      const uint32_t idesc = umma_idesc(p.bn);
-      int kbc = 0, ti = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ti) {
-        const int acc = ti & 1;
-        const uint32_t use = (uint32_t)(ti >> 1);
-        mbar_wait(smem_u32(&s_tempty[acc]), (use & 1) ^ 1);      // epilogue has drained this accumulator buffer
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * p.bn);
-        for (int kb = 0; kb < nkb; ++kb, ++kbc) {
-          const int s = kbc % p.stages;
-          const uint32_t ph = (kbc / p.stages) & 1;
-          mbar_wait(smem_u32(&s_full[s]), ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes), sb = sa + a_bytes;
-          const uint64_t da = umma_desc_sw128(sa), db = umma_desc_sw128(sb);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k) {
-              // advance 16 bf16 = 32 B inside the 128 B swizzle atom: start-address field += 2
-              umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-            }
-            umma_commit(smem_u32(&s_empty[s]));           // frees the smem stage when the MMAs above retire
-          }
-          __syncwarp();
-        }
-        if (elect_one()) umma_commit(smem_u32(&s_tfull[acc]));            // accumulator of this tile complete
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===================== epilogue (4 warps, TMEM lane quadrant = warp % 4) =====================
-    // TMEM -> registers -> (scale/shift/ReLU, bf16) -> 128B-swizzled smem SLAB of 64 columns -> one TMA store per slab.
-    // Two slab buffers alternate, so the store of slab i overlaps the conversion of slab i+1 and the staging area is 32 KB
-    // whatever the N tile (the first version staged the whole tile: 64 KB at N = 256 left room for two pipeline stages only and
-    // one CTA per SM -- profiles/r02_bench_conv_callC.json: 329 us for the stage-1 conv3 against cuDNN's 81).
-    // BatchNorm statistics are taken from the staged bf16 slab (what the normalisation will read back), one column pair per
-    // thread with the mixed-precision FMA -- the register butterfly of the first version cost 4 x 100 instructions per slab.
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
-    const int et = threadIdx.x - 64;                     // 0..127 among the epilogue threads
-    const bool stats = p.col_sum != nullptr;
-    const uint32_t out_base = smem_u32(out_tile);
-    const int nslab = (p.bn + 63) / 64;
-    int ti = 0, last_n0 = -1;
-    uint32_t slab_ctr = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++ti) {
-      const int tile_m = tile / n_tiles, n0 = (tile % n_tiles) * p.bn;
-      int b0, h0, w0, rows_valid; long long m0;
-      tc_tile_origin(p, tile_m, b0, h0, w0, m0, rows_valid);
-      const int acc = ti & 1;
-      const uint32_t use = (uint32_t)(ti >> 1);
-      const bool row_ok = r < rows_valid && (m0 + r) < p.M;
-      if (n0 != last_n0) {                               // per-column epilogue constants of this N tile -> smem
-        for (int j = et; j < p.bn; j += 128) {
-          const bool in = n0 + j < p.N;
-          s_scale[j] = (p.scale && in) ? __ldg(p.scale + n0 + j) : 1.f;
-          s_shift[j] = (p.shift && in) ? __ldg(p.shift + n0 + j) : 0.f;
-        }
-        last_n0 = n0;
-      }
-      mbar_wait(smem_u32(&s_tfull[acc]), use & 1);
-      __syncwarp();
-      tc_fence_after();
-      for (int sl = 0; sl < nslab; ++sl, ++slab_ctr) {
-        const uint32_t buf = out_base + (slab_ctr & 1u) * (uint32_t)(TC_BM * 128);
-        // the store that read this buffer two slabs ago must have finished READING it (at most the latest group may be pending)
-        if (et == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        // both 32-column halves of the slab are requested from TMEM before the single wait: one exposed TMEM round trip per slab
-        // instead of two (the epilogue is a latency chain: profiles/r02_ncu_targets_callI.md, wide-N tiles at 0.55-0.7 of the roof)
-        uint32_t rawA[32], rawB[32];
-        const bool hasB = (sl * 2 + 1) * 32 < p.bn;
-        tmem_ld32_issue(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * p.bn + sl * 64), rawA);
-        if (hasB) tmem_ld32_issue(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * p.bn + sl * 64 + 32), rawB);
-        tmem_ld_wait();
-#pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          if (cc == 1 && !hasB) break;
-          const int c = sl * 2 + cc;
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(cc == 0 ? rawA[j] : rawB[j]);
-#pragma unroll
-          for (int j8 = 0; j8 < 4; ++j8) {
-            const int col = c * 32 + j8 * 8;               // column inside the N tile
-            if (col < p.bn) {
-              const float4 sc0 = *reinterpret_cast<const float4*>(&s_scale[col]), sc1 = *reinterpret_cast<const float4*>(&s_scale[col + 4]);
-              const float4 sh0 = *reinterpret_cast<const float4*>(&s_shift[col]), sh1 = *reinterpret_cast<const float4*>(&s_shift[col + 4]);
-              const float scv[8] = {sc0.x, sc0.y, sc0.z, sc0.w, sc1.x, sc1.y, sc1.z, sc1.w};
-              const float shv[8] = {sh0.x, sh0.y, sh0.z, sh0.w, sh1.x, sh1.y, sh1.z, sh1.w};
-              uint32_t pk[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float lo = fmaf(v[j8 * 8 + 2 * e], scv[2 * e], shv[2 * e]);
-                float hi = fmaf(v[j8 * 8 + 2 * e + 1], scv[2 * e + 1], shv[2 * e + 1]);
-                if (p.relu) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
-                __nv_bfloat162 h2 = __floats2bfloat162_rn(lo, hi);
-                pk[e] = *reinterpret_cast<uint32_t*>(&h2);
-              }
-              const int chunk = cc * 4 + j8;               // 16-byte chunk inside the 128-byte slab row
-              const uint32_t dst = buf + (uint32_t)(r * 128 + ((chunk ^ (r & 7)) << 4));
-              asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]) : "memory");
-            }
-          }
-        }
-        if (sl == nslab - 1) {                             // accumulator buffer drained: hand it back to the MMA issuer
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&s_tempty[acc])) : "memory");
-        }
-        // make the generic-proxy smem writes visible to the async proxy, then one thread issues the bulk tensor store
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (et == 0) {
-          if (n0 + sl * 64 < p.N)
-            asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                         ::"l"(&mapD), "r"(buf), "r"(n0 + sl * 64), "r"((int)m0) : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-        if (stats && p.rows_per_sample > 0) {
-          // PER-SAMPLE column sums of the staged slab (GroupNorm over the 9 taps x H x W of one sample, models/cotnet.py:56): a row
-          // group of 32 rows touches at most two samples (rows_per_sample >= 32 is checked on the host); two partial sets per
-          // thread, straight to the [sample, column] tables
-          const int tp = et & 31, rg = et >> 5;
-          if (sl * 64 + 2 * tp < p.bn && n0 + sl * 64 + 2 * tp < p.N) {
-            const long long row0 = m0 + rg * 32;
-            const int s_lo = (int)(row0 / p.rows_per_sample);
-            const int rb = (int)min((long long)32, (long long)(s_lo + 1) * p.rows_per_sample - row0);   // rows [0, rb) belong to sample s_lo
-            const int nrow = min(32, min(rows_valid, (int)min((long long)TC_BM, p.M - m0)) - rg * 32);
-            const __nv_bfloat16 one = one_of<__nv_bfloat16>();
-            float sa[2] = {0.f, 0.f}, qa[2] = {0.f, 0.f}, sb[2] = {0.f, 0.f}, qb[2] = {0.f, 0.f};
-            uint32_t w2[32];
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-              const int row = rg * 32 + rr;
-              asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w2[rr]) : "r"(buf + (uint32_t)(row * 128 + (((tp >> 2) ^ (row & 7)) << 4) + (tp & 3) * 4)));
-            }
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-              if (rr < nrow) {
-                const __nv_bfloat16 lo = __ushort_as_bfloat16((unsigned short)(w2[rr] & 0xFFFFu)), hi = __ushort_as_bfloat16((unsigned short)(w2[rr] >> 16));
-                const int h = rr < rb ? 0 : 1;
-                if (h == 0) { sa[0] = mfma<__nv_bfloat16>(lo, one, sa[0]); qa[0] = mfma<__nv_bfloat16>(lo, lo, qa[0]);
-                              sb[0] = mfma<__nv_bfloat16>(hi, one, sb[0]); qb[0] = mfma<__nv_bfloat16>(hi, hi, qb[0]); }
-                else        { sa[1] = mfma<__nv_bfloat16>(lo, one, sa[1]); qa[1] = mfma<__nv_bfloat16>(lo, lo, qa[1]);
-                              sb[1] = mfma<__nv_bfloat16>(hi, one, sb[1]); qb[1] = mfma<__nv_bfloat16>(hi, hi, qb[1]); }
-              }
-            }
-            const int col = n0 + sl * 64 + 2 * tp;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              if ((h == 0 && nrow > 0) || (h == 1 && nrow > rb)) {
-                const long long srow = (long long)(s_lo + h) * p.N + col;
-                atomicAdd(p.col_sum + srow, sa[h]); atomicAdd(p.col_sqsum + srow, qa[h]);
-                if (col + 1 < p.N) { atomicAdd(p.col_sum + srow + 1, sb[h]); atomicAdd(p.col_sqsum + srow + 1, qb[h]); }
-              }
-            }
-          }
-        }
-        if (stats && p.rows_per_sample == 0) {
-          // column sums of the staged slab: thread = (column pair tp, row group rg of 32 rows); a warp reads one whole 128-byte
-          // row per step (conflict-free under the swizzle); bf16 operands go straight into the FMA
-          const int tp = et & 31, rg = et >> 5;
-          if (sl * 64 + 2 * tp < p.bn) {
-            float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-            const __nv_bfloat16 one = one_of<__nv_bfloat16>();
-            const int nrow = min(32, min(rows_valid, (int)min((long long)TC_BM, p.M - m0)) - rg * 32);      // valid rows of this row group
-            uint32_t w2[32];
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {               // all loads first (independent), then the arithmetic
-              const int row = rg * 32 + rr;
-              asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w2[rr]) : "r"(buf + (uint32_t)(row * 128 + (((tp >> 2) ^ (row & 7)) << 4) + (tp & 3) * 4)));
-            }
-#pragma unroll
-            for (int rr = 0; rr < 32; ++rr) {
-              if (rr < nrow) {
-                const __nv_bfloat16 lo = __ushort_as_bfloat16((unsigned short)(w2[rr] & 0xFFFFu)), hi = __ushort_as_bfloat16((unsigned short)(w2[rr] >> 16));
-                s0 = mfma<__nv_bfloat16>(lo, one, s0); q0 = mfma<__nv_bfloat16>(lo, lo, q0);
-                s1 = mfma<__nv_bfloat16>(hi, one, s1); q1 = mfma<__nv_bfloat16>(hi, hi, q1);
-              }
-            }
-            // one owner per (row group, column): plain stores, no atomics; every column of the tile is written once per tile
-            s_sum[rg][sl * 64 + 2 * tp] = s0; s_sq[rg][sl * 64 + 2 * tp] = q0;
-            s_sum[rg][sl * 64 + 2 * tp + 1] = s1; s_sq[rg][sl * 64 + 2 * tp + 1] = q1;
-          }
-        }
-      }
-      if (stats && p.rows_per_sample == 0) {
-        asm volatile("bar.sync 1, 128;" ::: "memory");      // every thread's shared-memory partials are in
-        for (int j = et; j < p.bn; j += 128) {
-          if (n0 + j < p.N) {
-            atomicAdd(p.col_sum + n0 + j, (s_sum[0][j] + s_sum[1][j]) + (s_sum[2][j] + s_sum[3][j]));
-            atomicAdd(p.col_sqsum + n0 + j, (s_sq[0][j] + s_sq[1][j]) + (s_sq[2][j] + s_sq[3][j]));
-          }
-        }
-      }
-    }
-    if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");     // all stores complete before the CTA exits
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
+
+  // ===================== consumers: wgmma main loop + epilogue (rows 64 wg .. 64 wg + 63 of each tile) =====================
+  // Epilogue: registers -> (scale/shift/ReLU, bf16) -> 128B-swizzled smem SLAB of 64 columns x 128 rows -> one TMA store per
+  // slab.  Two slab buffers alternate, so the store of slab i overlaps the conversion of slab i+1 and the staging area is 32 KB
+  // whatever the N tile.  BatchNorm statistics are taken from the staged bf16 slab (what the normalisation will read back), one
+  // column pair per thread of the first warpgroup.
+  const int wg = warp >> 2;
+  const int et = threadIdx.x;                          // 0..255 among the consumer threads
+  const bool stats = p.col_sum != nullptr;
+  const uint32_t out_base = smem_u32(out_tile);
+  const int nch = p.bn / 64;
+  int kbc = 0, last_n0 = -1;
+  uint32_t slab_ctr = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int tile_m = tile / n_tiles, n0 = (tile % n_tiles) * p.bn;
+    int b0, h0, w0, rows_valid; long long m0;
+    tc_tile_origin(p, tile_m, b0, h0, w0, m0, rows_valid);
+    if (n0 != last_n0) {                               // per-column epilogue constants of this N tile -> smem
+      for (int j = et; j < p.bn; j += TC_CONSUMERS) {
+        const bool in = n0 + j < p.N;
+        s_scale[j] = (p.scale && in) ? __ldg(p.scale + n0 + j) : 1.f;
+        s_shift[j] = (p.shift && in) ? __ldg(p.shift + n0 + j) : 0.f;
+      }
+      last_n0 = n0;
+    }
+    float acc[MAXCH][32];
+    int prev_s = 0;
+    for (int kb = 0; kb < nkb; ++kb, ++kbc) {
+      const int s = kbc % p.stages;
+      const uint32_t ph = (kbc / p.stages) & 1;
+      mbar_wait(smem_u32(&s_full[s]), ph);
+      const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes) + (uint32_t)wg * (64u * 128u), sb = smem_u32(smem + (size_t)s * stage_bytes) + a_bytes;
+      const uint64_t da = wgmma_desc_sw128(sa), db = wgmma_desc_sw128(sb);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k) {
+        // advance 16 bf16 = 32 B inside the 128 B swizzle atom: start-address field += 2; N chunks are 64 rows = 8 KB apart
+#pragma unroll
+        for (int c = 0; c < MAXCH; ++c)
+          if (c < nch) wgmma_m64n64k16<0, 0>(acc[c], da + 2 * k, db + (uint64_t)(c * 512) + 2 * k, (kb | k) != 0);
+      }
+      wgmma_commit();
+      if (kb > 0) {                                    // the MMAs of the previous stage have retired: hand it back to the producer
+        wgmma_wait<1>();
+        if ((et & 127) == 0) mbar_arrive(smem_u32(&s_empty[prev_s]));
+      }
+      prev_s = s;
+    }
+    wgmma_wait<0>();
+    if ((et & 127) == 0) mbar_arrive(smem_u32(&s_empty[prev_s]));
+#pragma unroll
+    for (int c = 0; c < MAXCH; ++c) if (c < nch) wgmma_fence_acc(acc[c]);
+
+#pragma unroll
+    for (int sl = 0; sl < MAXCH; ++sl) {
+      if (sl >= nch) break;
+      const uint32_t buf = out_base + (slab_ctr & 1u) * (uint32_t)(TC_BM * 128);
+      ++slab_ctr;
+      // the store that read this buffer two slabs ago must have finished READING it (at most the latest group may be pending)
+      if (et == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+      consumer_bar();
+      stage_chunk_bf16(acc[sl], buf, wg * 64, &s_scale[sl * 64], &s_shift[sl * 64], p.relu);
+      // make the generic-proxy smem writes visible to the async proxy, then one thread issues the bulk tensor store
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      consumer_bar();
+      if (et == 0) {
+        if (n0 + sl * 64 < p.N)
+          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                       ::"l"(&mapD), "r"(buf), "r"(n0 + sl * 64), "r"((int)m0) : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      }
+      if (stats && p.rows_per_sample > 0 && et < 128) {
+        // PER-SAMPLE column sums of the staged slab (GroupNorm over the 9 taps x H x W of one sample, models/cotnet.py:56): a row
+        // group of 32 rows touches at most two samples (rows_per_sample >= 32 is checked on the host); two partial sets per
+        // thread, straight to the [sample, column] tables
+        const int tp = et & 31, rg = et >> 5;
+        if (sl * 64 + 2 * tp < p.bn && n0 + sl * 64 + 2 * tp < p.N) {
+          const long long row0 = m0 + rg * 32;
+          const int s_lo = (int)(row0 / p.rows_per_sample);
+          const int rb = (int)min((long long)32, (long long)(s_lo + 1) * p.rows_per_sample - row0);   // rows [0, rb) belong to sample s_lo
+          const int nrow = min(32, min(rows_valid, (int)min((long long)TC_BM, p.M - m0)) - rg * 32);
+          const __nv_bfloat16 one = one_of<__nv_bfloat16>();
+          float sa[2] = {0.f, 0.f}, qa[2] = {0.f, 0.f}, sb[2] = {0.f, 0.f}, qb[2] = {0.f, 0.f};
+          uint32_t w2[32];
+#pragma unroll
+          for (int rr = 0; rr < 32; ++rr) {
+            const int row = rg * 32 + rr;
+            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w2[rr]) : "r"(buf + (uint32_t)(row * 128 + (((tp >> 2) ^ (row & 7)) << 4) + (tp & 3) * 4)));
+          }
+#pragma unroll
+          for (int rr = 0; rr < 32; ++rr) {
+            if (rr < nrow) {
+              const __nv_bfloat16 lo = __ushort_as_bfloat16((unsigned short)(w2[rr] & 0xFFFFu)), hi = __ushort_as_bfloat16((unsigned short)(w2[rr] >> 16));
+              const int h = rr < rb ? 0 : 1;
+              if (h == 0) { sa[0] = mfma<__nv_bfloat16>(lo, one, sa[0]); qa[0] = mfma<__nv_bfloat16>(lo, lo, qa[0]);
+                            sb[0] = mfma<__nv_bfloat16>(hi, one, sb[0]); qb[0] = mfma<__nv_bfloat16>(hi, hi, qb[0]); }
+              else        { sa[1] = mfma<__nv_bfloat16>(lo, one, sa[1]); qa[1] = mfma<__nv_bfloat16>(lo, lo, qa[1]);
+                            sb[1] = mfma<__nv_bfloat16>(hi, one, sb[1]); qb[1] = mfma<__nv_bfloat16>(hi, hi, qb[1]); }
+            }
+          }
+          const int col = n0 + sl * 64 + 2 * tp;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if ((h == 0 && nrow > 0) || (h == 1 && nrow > rb)) {
+              const long long srow = (long long)(s_lo + h) * p.N + col;
+              atomicAdd(p.col_sum + srow, sa[h]); atomicAdd(p.col_sqsum + srow, qa[h]);
+              if (col + 1 < p.N) { atomicAdd(p.col_sum + srow + 1, sb[h]); atomicAdd(p.col_sqsum + srow + 1, qb[h]); }
+            }
+          }
+        }
+      }
+      if (stats && p.rows_per_sample == 0 && et < 128) {
+        // column sums of the staged slab: thread = (column pair tp, row group rg of 32 rows); a warp reads one whole 128-byte
+        // row per step (conflict-free under the swizzle)
+        const int tp = et & 31, rg = et >> 5;
+        if (sl * 64 + 2 * tp < p.bn) {
+          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+          const __nv_bfloat16 one = one_of<__nv_bfloat16>();
+          const int nrow = min(32, min(rows_valid, (int)min((long long)TC_BM, p.M - m0)) - rg * 32);      // valid rows of this row group
+          uint32_t w2[32];
+#pragma unroll
+          for (int rr = 0; rr < 32; ++rr) {               // all loads first (independent), then the arithmetic
+            const int row = rg * 32 + rr;
+            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w2[rr]) : "r"(buf + (uint32_t)(row * 128 + (((tp >> 2) ^ (row & 7)) << 4) + (tp & 3) * 4)));
+          }
+#pragma unroll
+          for (int rr = 0; rr < 32; ++rr) {
+            if (rr < nrow) {
+              const __nv_bfloat16 lo = __ushort_as_bfloat16((unsigned short)(w2[rr] & 0xFFFFu)), hi = __ushort_as_bfloat16((unsigned short)(w2[rr] >> 16));
+              s0 = mfma<__nv_bfloat16>(lo, one, s0); q0 = mfma<__nv_bfloat16>(lo, lo, q0);
+              s1 = mfma<__nv_bfloat16>(hi, one, s1); q1 = mfma<__nv_bfloat16>(hi, hi, q1);
+            }
+          }
+          // one owner per (row group, column): plain stores, no atomics; every column of the tile is written once per tile
+          s_sum[rg][sl * 64 + 2 * tp] = s0; s_sq[rg][sl * 64 + 2 * tp] = q0;
+          s_sum[rg][sl * 64 + 2 * tp + 1] = s1; s_sq[rg][sl * 64 + 2 * tp + 1] = q1;
+        }
+      }
+    }
+    if (stats && p.rows_per_sample == 0) {
+      consumer_bar();                                  // every thread's shared-memory partials are in
+      for (int j = et; j < p.bn; j += TC_CONSUMERS) {  // one owner per column: the CTA's totals add up in tile order
+        if (n0 + j < p.N) {
+          s_tot[n0 + j] += (s_sum[0][j] + s_sum[1][j]) + (s_sum[2][j] + s_sum[3][j]);
+          s_tot[p.N + n0 + j] += (s_sq[0][j] + s_sq[1][j]) + (s_sq[2][j] + s_sq[3][j]);
+        }
+      }
+    }
+  }
+  if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");     // all stores complete before the CTA exits
+  if (stats && p.rows_per_sample == 0) {
+    consumer_bar();
+    const int n = 2 * p.N;
+    for (int i = et; i < n; i += TC_CONSUMERS) p.det.scr[(size_t)blockIdx.x * n + i] = s_tot[i];
+    det_finish<true>(p.det.scr, n, blockIdx.x, gridDim.x, p.det.tick, et, TC_CONSUMERS, [&](int k, float t) {
+      if (k < p.N) p.col_sum[k] += t; else p.col_sqsum[k - p.N] += t;
+    });
   }
 }
 
@@ -449,15 +401,16 @@ static int tc_launch(const CUtensorMap& a1, const CUtensorMap& b1, const CUtenso
   CUtensorMap dmap;
   int rcd = make_map_2d(&dmap, p.D, p.M, p.N, p.ldd, p.rows_per_tile);
   if (rcd) return rcd;
-  const int out_bytes = 2 * TC_BM * 128 + ((p.col_sum && p.rows_per_sample == 0) ? 2 * 4 * 256 * 4 : 0);   // two slab buffers (+ statistics partials)
+  // two slab buffers (+ statistics partials of a tile and the CTA's column totals)
+  const int out_bytes = 2 * TC_BM * 128 + ((p.col_sum && p.rows_per_sample == 0) ? 2 * 4 * 256 * 4 + 2 * p.N * 4 : 0);
   const int a_bytes = TC_BM * TC_BK * 2, b_bytes = p.bn * TC_BK * 2;
   const int stage_bytes = a_bytes + ((b_bytes + 1023) & ~1023);
   p.m_tiles = m_tiles;
-  // two CTAs per SM (two epilogue teams, two MMA issuers) when at least 3 stages fit next to each other and the two pairs of
-  // accumulator buffers fit the 512 TMEM columns; else one CTA with as many stages as the ring supports
+  // two CTAs per SM (two epilogue teams, two producers) when N tiles of <= 128 columns keep the accumulators of a consumer thread
+  // at <= 64 registers and at least 2 stages fit next to each other; else one CTA with as many stages as the ring supports
   int per_sm = 2;
   p.stages = (104 * 1024 - out_bytes) / stage_bytes;
-  if (p.stages < 2 || 2 * p.bn > 256) {
+  if (p.stages < 2 || p.bn > 128) {
     per_sm = 1;
     p.stages = (200 * 1024 - out_bytes) / stage_bytes;
   }
@@ -466,23 +419,32 @@ static int tc_launch(const CUtensorMap& a1, const CUtensorMap& b1, const CUtenso
   const int smem = p.stages * stage_bytes + out_bytes + 1024;
   static PerDevFlag configured_d;
   if (bool& configured = configured_d.get(); !configured) {
-    cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<4, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024);
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
     configured = true;
   }
   const int total = m_tiles * ((p.N + p.bn - 1) / p.bn);
   int grid = per_sm * num_sms();                          // resident CTAs only: a second wave would start from a cold pipeline
   if (grid > total) grid = total;
+  DetScratch ds;
+  if (p.col_sum && p.rows_per_sample == 0) {
+    if (p.N > 4096) { set_error("%s: N=%d too wide for the statistics epilogue", what, p.N); return COTB200_EUNSUPPORTED; }
+    int rcs = ds.alloc(det_floats(grid, 2 * p.N), 1, st);
+    if (rcs) return rcs;
+    p.det = ds.a;
+  }
   COTB200_PROF_B(what, alg_bytes);
-  tc_gemm_kernel<<<grid, TC_THREADS, smem, st>>>(a1, b1, a2, b2, dmap, p);
+  if (per_sm == 2) tc_gemm_kernel<2, 2><<<grid, TC_THREADS, smem, st>>>(a1, b1, a2, b2, dmap, p);
+  else tc_gemm_kernel<4, 1><<<grid, TC_THREADS, smem, st>>>(a1, b1, a2, b2, dmap, p);
   return check_launch(what);
 }
 
 static int pick_bn_wide(int N);
 static int pick_bn(int N, int K = 1 << 30) {
-  // short contractions (K <= 128) with a wide output are epilogue-bound: TMEM drains at 64 B/clk per SM, so a 256-column tile
-  // needs > 1 us just to leave TMEM while its operands arrived in a fraction of that.  Two CTAs per SM with 128-column tiles
-  // run two epilogues side by side (the re-read A tile is small and comes from L2).
+  // short contractions (K <= 128) with a wide output are epilogue-bound: the operands of a 256-column tile arrive in a fraction
+  // of the time its epilogue takes.  Two CTAs per SM with 128-column tiles run two epilogues side by side (the re-read A tile is
+  // small and comes from L2).
   if (K <= 128 && N > 128) {
     const int parts = (N + 127) / 128;
     const int bn = (((N + parts - 1) / parts) + 63) & ~63;
@@ -491,9 +453,8 @@ static int pick_bn(int N, int K = 1 << 30) {
   return pick_bn_wide(N);
 }
 static int pick_bn_wide(int N) {
-  // One N tile when N fits a single UMMA (<= 256): bn = N rounded up to 16, columns beyond N are clipped by the TMA store.
-  // Several N tiles: bn must be a multiple of 64 so that every 64-column store slab lies inside its own tile.
-  if (N <= 256) return (N + 15) & ~15;
+  // bn is a multiple of 64 (whole n64 wgmma chunks; every 64-column store slab lies inside its own tile), <= 256: rows of B
+  // beyond N are zero-filled by the TMA and columns of D beyond N are clipped by the TMA store.
   const int parts = (N + 255) / 256;
   const int bn = (((N + parts - 1) / parts) + 63) & ~63;
   return bn > 256 ? 256 : bn;
@@ -501,32 +462,27 @@ static int pick_bn_wide(int N) {
 
 // ---------------------------------------------------------------------------------------------- 3x3 conv, haloed-tile kernel
 // conv mode of tc_gemm_kernel fetches one pixel box PER TAP: every input pixel travels L2 -> shared memory nine times and the
-// kernel is L2-bound (120 us at [256,64,56,56] against a 32 us HBM roof, profiles/r01_tc_ncu_v3.md).  Here a CTA loads ONE haloed
-// tile {64 ch, W+2, R+2} of the NHWC input per work item (TMA out-of-bounds fill = zero padding on all four sides) and the nine
-// taps are nine UMMA A-descriptors INTO THAT TILE: with the output pixels enumerated in padded coordinates q = r*(W+2) + c, the A
-// rows of tap (dh, dw) are the smem rows q + (dh+1)*(W+2) + (dw+1) -- a contiguous row range, i.e. the same K-major SW128
-// descriptor with a start address moved by a whole number of 128-byte rows (the 128B swizzle is a function of the absolute shared
-// memory address, which is how TMA wrote the tile).  Outputs with c >= W are garbage columns that are never stored.
+// kernel is L2-bound.  Here a CTA loads ONE haloed tile {64 ch, W+2, R+2} of the NHWC input per work item (TMA out-of-bounds
+// fill = zero padding on all four sides) and the nine taps are nine wgmma A-descriptors INTO THAT TILE: with the output pixels
+// enumerated in padded coordinates q = r*(W+2) + c, the A rows of tap (dh, dw) are the smem rows q + (dh+1)*(W+2) + (dw+1) -- a
+// contiguous row range, i.e. the same K-major SW128 descriptor with a start address moved by a whole number of 128-byte rows (the
+// 128B swizzle is a function of the absolute shared memory address, which is how TMA wrote the tile).  Outputs with c >= W are
+// garbage columns that are never stored.
 //   * weights of the CTA's 64 output channels (9 taps x 64 x 64, 72 KB) stay resident in shared memory: CTAs are bound to one
 //     N tile, work items of that N tile are strided over the CTAs bound to it;
-//   * accumulators: MB <= 2 M-blocks of 128 padded pixels x 64 columns, double-buffered in TMEM across work items;
-//   * epilogue: TMEM -> scale/shift/ReLU -> bf16 -> compacted (garbage columns dropped) 128B-swizzled image of the R x W output
-//     pixels -> ONE TMA store; BatchNorm column statistics from the staged image, accumulated in registers over ALL work items of
-//     the CTA (its N tile never changes) and flushed with one atomic per column per CTA.
+//   * accumulators: MB <= 2 M-blocks of 128 padded pixels x 64 columns; warpgroup g owns rows 64g .. 64g + 63 of each M-block;
+//   * epilogue: registers -> scale/shift/ReLU -> bf16 -> compacted (garbage columns dropped) 128B-swizzled image of the R x W
+//     output pixels -> ONE TMA store; BatchNorm column statistics from the staged image, accumulated in registers over ALL work
+//     items of the CTA (its N tile never changes) and leaving through one deterministic reduction (det_finish).
 // Geometry: bn = 64 (kc = 1), R | H, R*(W+2) <= 256.  Everything else stays on conv mode of tc_gemm_kernel.
 struct HcParams {
   int B, H, W, C, R, MB, Wp, n_tiles, bands, items;   // items = B * bands work items per N tile
-  int a_stage_bytes, stages, box_bytes, relu, base_off;
+  int a_stage_bytes, stages, box_bytes, relu;
   const float* scale; const float* shift; float* col_sum; float* col_sqsum;
+  DetArena det;
 };
 
 static constexpr int HC_WBYTES = 9 * 64 * 128;          // resident weights of one N tile
-
-__device__ __forceinline__ uint64_t umma_desc_sw128_rows(uint32_t saddr, int base_off) {
-  uint64_t d = umma_desc_sw128(saddr);
-  if (base_off) d |= (uint64_t)((saddr >> 7) & 7u) << 49;
-  return d;
-}
 
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapW,
@@ -536,37 +492,27 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_co
   uint8_t* w_s = smem;                                               // [9][64 rows][128 B] SW128
   uint8_t* a_s = smem + HC_WBYTES;                                    // stages x haloed tile
   uint8_t* o_s = a_s + (size_t)p.stages * p.a_stage_bytes;           // [R*W rows][128 B] SW128 compacted output image
-  __shared__ __align__(8) uint64_t s_full[4], s_empty[4], s_wfull, s_tfull[2], s_tempty[2];
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t s_full[4], s_empty[4], s_wfull;
   __shared__ __align__(16) float s_scale[64], s_shift[64];
   __shared__ float s_part[2][4][64];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nt = blockIdx.x % p.n_tiles, n0 = nt * 64;
   const int first = blockIdx.x / p.n_tiles, step = gridDim.x / p.n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapX) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
-    for (int s = 0; s < 4; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), 1); }
+    for (int s = 0; s < 4; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), 2); }
     mbar_init(smem_u32(&s_wfull), 1);
-    for (int a = 0; a < 2; ++a) { mbar_init(smem_u32(&s_tfull[a]), 1); mbar_init(smem_u32(&s_tempty[a]), 4); }
     mbar_init_fence();
-  }
-  const uint32_t ncols = p.MB == 1 ? 128u : 256u;                     // two buffers x MB x 64 columns
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   if (threadIdx.x < 64) {
     s_scale[threadIdx.x] = p.scale ? __ldg(p.scale + n0 + threadIdx.x) : 1.f;
     s_shift[threadIdx.x] = p.shift ? __ldg(p.shift + n0 + threadIdx.x) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
-  if (warp == 0) {
+  if (warp == TC_PRODUCER_WARP) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       const uint32_t wf = smem_u32(&s_wfull);
@@ -583,153 +529,124 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_co
         tma_load_4d(smem_u32(a_s + (size_t)s * p.a_stage_bytes), &mapX, full, n0, -1, h0 - 1, b);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp, warp-uniform; one elected lane issues) =====================
-    {
-      const uint32_t idesc = umma_idesc(64);
-      mbar_wait(smem_u32(&s_wfull), 0);
-      tc_fence_after();
-      const uint32_t wb = smem_u32(w_s);
-      int it = 0;
-      for (int m = first; m < p.items; m += step, ++it) {
-        const int s = it % p.stages;
-        const uint32_t ph = (it / p.stages) & 1;
-        const int acc = it & 1;
-        const uint32_t use = (uint32_t)(it >> 1);
-        mbar_wait(smem_u32(&s_tempty[acc]), (use & 1) ^ 1);
-        tc_fence_after();
-        mbar_wait(smem_u32(&s_full[s]), ph);
-        tc_fence_after();
-        const uint32_t ab = smem_u32(a_s + (size_t)s * p.a_stage_bytes);
-        if (elect_one()) {
-          for (int mb = 0; mb < p.MB; ++mb) {
-            const uint32_t tmem_d = tmem_base + (uint32_t)((acc * p.MB + mb) * 64);
+    return;
+  }
+
+  // ===================== consumers: nine-tap wgmma + epilogue =====================
+  const int wg = warp >> 2, wl = warp & 3;
+  const int et = threadIdx.x;
+  const bool stats = p.col_sum != nullptr;
+  const uint32_t ob = smem_u32(o_s);
+  const uint32_t wb = smem_u32(w_s);
+  const int RW = p.R * p.W;
+  const int tp = et & 31, rg = (et >> 5) & 3;
+  float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;                     // statistics of columns 2tp, 2tp+1 over rows rg, rg+4, ... (et < 128)
+  mbar_wait(smem_u32(&s_wfull), 0);
+  int it = 0;
+  for (int m = first; m < p.items; m += step, ++it) {
+    const int s = it % p.stages;
+    const uint32_t ph = (it / p.stages) & 1;
+    const int b = m / p.bands, h0 = (m - b * p.bands) * p.R;
+    mbar_wait(smem_u32(&s_full[s]), ph);
+    const uint32_t ab = smem_u32(a_s + (size_t)s * p.a_stage_bytes);
+    float acc[2][32];
+    wgmma_fence();
 #pragma unroll
-            for (int t = 0; t < 9; ++t) {
-              const int row = mb * 128 + (t / 3) * p.Wp + (t % 3);          // first smem row of this tap's A operand
-              const uint64_t da = umma_desc_sw128_rows(ab + (uint32_t)row * 128u, p.base_off);
-              const uint64_t db = umma_desc_sw128(wb + (uint32_t)t * 8192u);
+    for (int mb = 0; mb < 2; ++mb) {
+      if (mb < p.MB) {
 #pragma unroll
-              for (int k = 0; k < 4; ++k) umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (t | k) != 0);
-            }
-          }
-          umma_commit(smem_u32(&s_empty[s]));
-          umma_commit(smem_u32(&s_tfull[acc]));
+        for (int t = 0; t < 9; ++t) {
+          const int row = mb * 128 + wg * 64 + (t / 3) * p.Wp + (t % 3);  // first smem row of this tap's A operand
+          const uint64_t da = wgmma_desc_sw128(ab + (uint32_t)row * 128u);
+          const uint64_t db = wgmma_desc_sw128(wb + (uint32_t)t * 8192u);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_m64n64k16<0, 0>(acc[mb], da + 2 * k, db + 2 * k, (t | k) != 0);
         }
-        __syncwarp();
       }
     }
-  } else {
-    // ===================== epilogue =====================
-    const int quad = warp & 3;
-    const int et = threadIdx.x - 64;
-    const bool stats = p.col_sum != nullptr;
-    const uint32_t ob = smem_u32(o_s);
-    const int RW = p.R * p.W;
-    const int tp = et & 31, rg = et >> 5;
-    float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;                     // statistics of columns 2tp, 2tp+1 over rows rg, rg+4, ...
-    int it = 0;
-    for (int m = first; m < p.items; m += step, ++it) {
-      const int acc = it & 1;
-      const uint32_t use = (uint32_t)(it >> 1);
-      const int b = m / p.bands, h0 = (m - b * p.bands) * p.R;
-      mbar_wait(smem_u32(&s_tfull[acc]), use & 1);
-      __syncwarp();
-      tc_fence_after();
-      // the previous item's store must have finished READING the staging image
-      if (et == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      for (int mb = 0; mb < p.MB; ++mb) {
-        const int q = mb * 128 + quad * 32 + lane;                   // padded output pixel
-        const int ro = q / p.Wp, co = q - ro * p.Wp;
-        const bool ok = ro < p.R && co < p.W;
-        const int prow = ro * p.W + co;                              // row of the compacted image
-        uint32_t rawA[32], rawB[32];                                   // both halves of the 64 columns in flight, one wait
-        tmem_ld32_issue(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((acc * p.MB + mb) * 64), rawA);
-        tmem_ld32_issue(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((acc * p.MB + mb) * 64 + 32), rawB);
-        tmem_ld_wait();
-        if (ok) {
+    wgmma_commit();
+    wgmma_wait<0>();
+    if ((et & 127) == 0) mbar_arrive(smem_u32(&s_empty[s]));      // haloed tile consumed
 #pragma unroll
-          for (int c = 0; c < 2; ++c) {
+    for (int mb = 0; mb < 2; ++mb) if (mb < p.MB) wgmma_fence_acc(acc[mb]);
+    // the previous item's store must have finished READING the staging image
+    if (et == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    consumer_bar();
 #pragma unroll
-            for (int j8 = 0; j8 < 4; ++j8) {
-              const int col = c * 32 + j8 * 8;
-              const float4 sc0 = *reinterpret_cast<const float4*>(&s_scale[col]), sc1 = *reinterpret_cast<const float4*>(&s_scale[col + 4]);
-              const float4 sh0 = *reinterpret_cast<const float4*>(&s_shift[col]), sh1 = *reinterpret_cast<const float4*>(&s_shift[col + 4]);
-              const float scv[8] = {sc0.x, sc0.y, sc0.z, sc0.w, sc1.x, sc1.y, sc1.z, sc1.w};
-              const float shv[8] = {sh0.x, sh0.y, sh0.z, sh0.w, sh1.x, sh1.y, sh1.z, sh1.w};
-              uint32_t pk[4];
+    for (int mb = 0; mb < 2; ++mb) {
+      if (mb < p.MB) {
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const uint32_t r0 = c == 0 ? rawA[j8 * 8 + 2 * e] : rawB[j8 * 8 + 2 * e];
-                const uint32_t r1 = c == 0 ? rawA[j8 * 8 + 2 * e + 1] : rawB[j8 * 8 + 2 * e + 1];
-                float lo = fmaf(__uint_as_float(r0), scv[2 * e], shv[2 * e]);
-                float hi = fmaf(__uint_as_float(r1), scv[2 * e + 1], shv[2 * e + 1]);
-                if (p.relu) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
-                __nv_bfloat162 h2 = __floats2bfloat162_rn(lo, hi);
-                pk[e] = *reinterpret_cast<uint32_t*>(&h2);
-              }
-              const int chunk = c * 4 + j8;
-              const uint32_t dst = ob + (uint32_t)(prow * 128 + ((chunk ^ (prow & 7)) << 4));
-              asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]) : "memory");
+        for (int h = 0; h < 2; ++h) {
+          const int q = mb * 128 + wg * 64 + wl * 16 + (lane >> 2) + 8 * h;   // padded output pixel
+          const int ro = q / p.Wp, co = q - ro * p.Wp;
+          if (ro < p.R && co < p.W) {
+            const int prow = ro * p.W + co;                            // row of the compacted image
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int col = i * 8 + 2 * (lane & 3);
+              float lo = fmaf(acc[mb][4 * i + 2 * h], s_scale[col], s_shift[col]);
+              float hi = fmaf(acc[mb][4 * i + 2 * h + 1], s_scale[col + 1], s_shift[col + 1]);
+              if (p.relu) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
+              __nv_bfloat162 h2 = __floats2bfloat162_rn(lo, hi);
+              const uint32_t dst = ob + (uint32_t)(prow * 128 + ((i ^ (prow & 7)) << 4) + (lane & 3) * 4);
+              asm volatile("st.shared.u32 [%0], %1;" ::"r"(dst), "r"(*reinterpret_cast<uint32_t*>(&h2)) : "memory");
             }
           }
         }
       }
-      // accumulator buffer drained
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&s_tempty[acc]));
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (et == 0) {
-        const int m0 = (b * p.H + h0) * p.W;
-        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                     ::"l"(&mapD), "r"(ob), "r"(n0), "r"(m0) : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
-      if (stats) {
-        const __nv_bfloat16 one = one_of<__nv_bfloat16>();
-        for (int r0 = rg; r0 < RW; r0 += 32) {                       // 8 rows per batch: loads first, then the arithmetic
-          uint32_t w2[8];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const int row = r0 + 4 * u;
-            w2[u] = 0u;
-            if (row < RW) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w2[u]) : "r"(ob + (uint32_t)(row * 128 + (((tp >> 2) ^ (row & 7)) << 4) + (tp & 3) * 4)));
-          }
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const __nv_bfloat16 lo = __ushort_as_bfloat16((unsigned short)(w2[u] & 0xFFFFu)), hi = __ushort_as_bfloat16((unsigned short)(w2[u] >> 16));
-            s0 = mfma<__nv_bfloat16>(lo, one, s0); q0 = mfma<__nv_bfloat16>(lo, lo, q0);
-            s1 = mfma<__nv_bfloat16>(hi, one, s1); q1 = mfma<__nv_bfloat16>(hi, hi, q1);
-          }
-        }
-      }
     }
-    if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    if (stats) {
-      s_part[0][rg][2 * tp] = s0; s_part[0][rg][2 * tp + 1] = s1;
-      s_part[1][rg][2 * tp] = q0; s_part[1][rg][2 * tp + 1] = q1;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (et < 64) {
-        atomicAdd(p.col_sum + n0 + et, (s_part[0][0][et] + s_part[0][1][et]) + (s_part[0][2][et] + s_part[0][3][et]));
-        atomicAdd(p.col_sqsum + n0 + et, (s_part[1][0][et] + s_part[1][1][et]) + (s_part[1][2][et] + s_part[1][3][et]));
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    consumer_bar();
+    if (et == 0) {
+      const int m0 = (b * p.H + h0) * p.W;
+      asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                   ::"l"(&mapD), "r"(ob), "r"(n0), "r"(m0) : "memory");
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+    if (stats && et < 128) {
+      const __nv_bfloat16 one = one_of<__nv_bfloat16>();
+      for (int r0 = rg; r0 < RW; r0 += 32) {                       // 8 rows per batch: loads first, then the arithmetic
+        uint32_t w2[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          const int row = r0 + 4 * u;
+          w2[u] = 0u;
+          if (row < RW) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w2[u]) : "r"(ob + (uint32_t)(row * 128 + (((tp >> 2) ^ (row & 7)) << 4) + (tp & 3) * 4)));
+        }
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          const __nv_bfloat16 lo = __ushort_as_bfloat16((unsigned short)(w2[u] & 0xFFFFu)), hi = __ushort_as_bfloat16((unsigned short)(w2[u] >> 16));
+          s0 = mfma<__nv_bfloat16>(lo, one, s0); q0 = mfma<__nv_bfloat16>(lo, lo, q0);
+          s1 = mfma<__nv_bfloat16>(hi, one, s1); q1 = mfma<__nv_bfloat16>(hi, hi, q1);
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
+  if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  if (stats) {
+    if (et < 128) {
+      s_part[0][rg][2 * tp] = s0; s_part[0][rg][2 * tp + 1] = s1;
+      s_part[1][rg][2 * tp] = q0; s_part[1][rg][2 * tp + 1] = q1;
+    }
+    consumer_bar();
+    // the CTA's row of the deterministic reduction: its 64 columns' totals, zeros for the other N tiles
+    const int n = 2 * p.C;
+    for (int i = et; i < n; i += TC_CONSUMERS) {
+      const int pl = i < p.C ? 0 : 1, c = i - pl * p.C;
+      float v = 0.f;
+      if (c >= n0 && c < n0 + 64) v = (s_part[pl][0][c - n0] + s_part[pl][1][c - n0]) + (s_part[pl][2][c - n0] + s_part[pl][3][c - n0]);
+      p.det.scr[(size_t)blockIdx.x * n + i] = v;
+    }
+    det_finish<true>(p.det.scr, n, blockIdx.x, gridDim.x, p.det.tick, et, TC_CONSUMERS, [&](int k, float t) {
+      if (k < p.C) p.col_sum[k] += t; else p.col_sqsum[k - p.C] += t;
+    });
   }
 }
 
 // returns 1 when the haloed-tile kernel took the convolution (*rc = status), 0 when conv mode of tc_gemm_kernel should run
 static int conv3x3_halo_launch(int B, int H, int W, int C, const void* X, long long ldx, const void* Wp, int bn, void* D, long long ldd,
                                const float* scale, const float* shift, int relu, float* col_sum, float* col_sqsum, cudaStream_t st, int* rc) {
-  static int mode = -2;                       // COTB200_CONV_HALO: 0 = off, 1 (default) = on, 2 = on with descriptor base offsets
+  static int mode = -2;                       // COTB200_CONV_HALO: 0 = off, 1 (default) = on
   if (mode == -2) { const char* e = getenv("COTB200_CONV_HALO"); mode = e ? atoi(e) : 1; }
   if (mode <= 0 || bn != 64 || C % 64 || W + 2 > 256 || ldx != C || ldd != C) return 0;
   const int Wpad = W + 2;
@@ -749,7 +666,7 @@ static int conv3x3_halo_launch(int B, int H, int W, int C, const void* X, long l
   p.stages = (220 * 1024 - HC_WBYTES - out_bytes) / p.a_stage_bytes;
   if (p.stages > 4) p.stages = 4;
   if (p.stages < 2) return 0;
-  p.relu = relu; p.base_off = mode == 2 ? 1 : 0;
+  p.relu = relu;
   p.scale = scale; p.shift = shift; p.col_sum = col_sum; p.col_sqsum = col_sqsum;
   CUtensorMap mx, mw, md;
   EncodeTiledFn enc = encode_fn();
@@ -774,6 +691,11 @@ static int conv3x3_halo_launch(int B, int H, int W, int C, const void* X, long l
   }
   int grid = (num_sms() / p.n_tiles) * p.n_tiles;
   if (grid > p.items * p.n_tiles) grid = p.items * p.n_tiles;
+  DetScratch ds;
+  if (col_sum) {
+    if ((*rc = ds.alloc(det_floats(grid, 2 * C), 1, st))) return 1;
+    p.det = ds.a;
+  }
   COTB200_PROF_B("tc_conv3x3_halo", 2.0 * (2.0 * (double)B * H * W * C + 9.0 * (double)C * 64));
   tc_conv3x3_halo_kernel<<<grid, TC_THREADS, smem, st>>>(mx, mw, md, p);
   *rc = check_launch("tc_conv3x3_halo");

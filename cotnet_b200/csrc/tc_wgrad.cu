@@ -1,32 +1,32 @@
-// Weight gradient of the 1x1 convolutions on the 5th-gen tensor cores (sm_100a):
+// Weight gradient of the 1x1 convolutions on the Hopper tensor cores (wgmma, sm_90a):
 //
 //     OUT[R, Cc] += A[M, R]^T * [B1 | B2][M, Cc]            (contraction over the M pixels)
 //
 // A = dY (gradient of the convolution output, NHWC rows = pixels), B = the convolution input(s); OUT = dW in fp32.
 // Replaces cuDNN's wgrad / the cuBLAS `dY^T X` of the autograd functions for  embed.0 / embed.3 / conv1x1.0 of the CoT layer
-// (/root/reference/models/cotnet.py:52,55,60) and conv1 / conv3 / downsample of the enclosing bottleneck (:228-264).
+// (models/cotnet.py:52,55,60) and conv1 / conv3 / downsample of the enclosing bottleneck (:228-264).
 //
 // Both operands are "MN-major" for the MMA (the contraction index -- pixels -- is the SLOW index of the row-major pixel
 // matrices), so the TMA tiles are used exactly as they land: a box {64 channels, 64 pixels} with the 128-byte swizzle IS
-// the canonical MN-major SWIZZLE_128B UMMA layout (64 MN elements contiguous, 8 K rows per 1024-byte atom).  No transpose
-// anywhere: tcgen05.mma with a_major = b_major = MN (instruction-descriptor bits 15/16).
+// the canonical MN-major SWIZZLE_128B wgmma layout (64 MN elements contiguous, 8 K rows per 1024-byte atom).  No transpose
+// anywhere: wgmma with both transpose flags set (tc_wgmma.cuh).
 //
-// Split-K over pixels: CTA (tile_r, tile_c, split) accumulates a [128 x BC] fp32 tile of dW in TMEM over its pixel range
-// (4-stage TMA ring, single-thread MMA issue), then adds it to OUT with vectorised global reductions.  Algorithmic bytes:
-// (R + Cc) * M * 2 (each operand read once) + the dW tile traffic; HBM-bound for every layer of the network.
-//   warp 0: TMA producer   warp 1: TMEM alloc + MMA issuer   warps 2-5: epilogue (TMEM lane quadrant = warp % 4)
+// Split-K over pixels: CTA (tile_r, tile_c, split) accumulates a [128 x BC] fp32 tile of dW in registers over its pixel range
+// (4-stage TMA ring) and stores it as that split's partial; wgrad_reduce_kernel adds the partials to OUT in split order.  Algorithmic bytes: (R + Cc) * M * 2 (each operand
+// read once) + the dW tile traffic; HBM-bound for every layer of the network.
+//   warps 0-7: two consumer warpgroups (warpgroup g: rows 64g .. 64g + 63 of the tile = A box g)   warp 8: TMA producer
 #include <cuda.h>
 #include <cstdlib>
 #include "common.cuh"
 #include "tma.cuh"
-#include "tc_umma.cuh"
+#include "tc_wgmma.cuh"
 
 namespace cotb200 {
 
-static constexpr int WG_BR = 128;          // rows of OUT per CTA (UMMA M)
+static constexpr int WG_BR = 128;          // rows of OUT per CTA (two warpgroups x 64)
 static constexpr int WG_PX = 64;           // pixels per pipeline stage (4 MMAs of K = 16)
 static constexpr int WG_STAGES = 4;
-static constexpr int WG_THREADS = 192;
+static constexpr int WG_THREADS = 288;     // two consumer warpgroups + one producer warp
 static constexpr int WG_BOX_BYTES = 64 * WG_PX * 2;    // one {64 ch, 64 px} bf16 box = 8 KB
 
 struct WgParams {
@@ -35,13 +35,14 @@ struct WgParams {
   int tiles_r, tiles_c, splits;
   int kb_total;              // ceil(M / 64)
   int transpose;             // 0: OUT[r * ldo + c]   1: OUT[c * ldo + r]
-  int lbo, sbo;              // UMMA descriptor offsets (bytes) -- see wg_desc_offsets()
+  int lbo, sbo;              // wgmma descriptor offsets (bytes) -- see wgmma_desc_mn_sw128()
   int px;                    // pixels per pipeline stage (multiple of 16): 64, or one output row of the stem convolution
   int stages;                // ring depth (<= WG_STAGES)
   int stem_ho;               // > 0: B = the stem's window matrices (4-D map, csrc/tc_gemm.cu stem mode); pixel block kb = (sample kb / stem_ho,
                              //      output row kb % stem_ho), column block j = s2d row tap a
   long long ldo;
   float* out;
+  float* part;               // [splits][R][Cc] fp32 partial tiles of the split-K reduction (wgrad_reduce_kernel adds them in split order)
 };
 
 __global__ void __launch_bounds__(WG_THREADS, 1)
@@ -49,8 +50,7 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 const __grid_constant__ CUtensorMap mapB2, const WgParams p) {
   extern __shared__ __align__(1024) uint8_t wg_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wg_smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ __align__(8) uint64_t s_full[WG_STAGES], s_empty[WG_STAGES], s_tfull;
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t s_full[WG_STAGES], s_empty[WG_STAGES];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nbb = p.bc / 64;                                   // B boxes per stage
   const int box_bytes = 128 * p.px;                            // one {64 ch, px pixels} bf16 box
@@ -65,110 +65,134 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
   const int kb_lo = split * per, kb_hi = min(p.kb_total, kb_lo + per);
   const int nkb = kb_hi - kb_lo;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB1) : "memory");
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), 1); }
-    mbar_init(smem_u32(&s_tfull), 1);
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), 2); }
     mbar_init_fence();
   }
-  uint32_t ncols = 32;
-  while ((int)ncols < p.bc) ncols <<= 1;
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
-  if (nkb > 0) {
-    if (warp == 0) {
-      if (lane == 0) {
-        for (int i = 0; i < nkb; ++i) {
-          const int s = i % p.stages;
-          const uint32_t ph = (i / p.stages) & 1;
-          mbar_wait(smem_u32(&s_empty[s]), ph ^ 1);
-          const uint32_t full = smem_u32(&s_full[s]);
-          const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes), sb = sa + a_bytes;
-          const int px = (kb_lo + i) * p.px;
-          mbar_expect_tx(full, (uint32_t)stage_bytes);            // TMA counts whole boxes (zero-filled parts included)
-          tma_load_2d(sa, &mapA, full, r0, px);                    // out-of-range channels / pixels are zero-filled: they add 0
-          tma_load_2d(sa + box_bytes, &mapA, full, r0 + 64, px);
-          if (p.stem_ho > 0) {
-            const int b = (kb_lo + i) / p.stem_ho, oh = (kb_lo + i) - b * p.stem_ho;
-            for (int j = 0; j < nbb; ++j)                          // tap a = c0 / 64 + j: the windows of s2d row oh - 2 + a
-              tma_load_4d(sb + j * box_bytes, &mapB1, full, 0, 0, oh - 2 + c0 / 64 + j, b);
-          } else {
-            for (int j = 0; j < nbb; ++j) {
-              const int c = c0 + j * 64;
-              if (c < p.C1) tma_load_2d(sb + j * box_bytes, &mapB1, full, c, px);
-              else tma_load_2d(sb + j * box_bytes, &mapB2, full, c - p.C1, px);
-            }
-          }
-        }
-      }
-    } else if (warp == 1) {
-      {                                                          // whole warp, warp-uniform; one elected lane issues (tc_umma.cuh)
-        const uint32_t idesc = umma_idesc_mn(WG_BR, p.bc);
-        for (int i = 0; i < nkb; ++i) {
-          const int s = i % p.stages;
-          const uint32_t ph = (i / p.stages) & 1;
-          mbar_wait(smem_u32(&s_full[s]), ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes), sb = sa + a_bytes;
-          // MN blocks of 64 channels are WG_BOX_BYTES apart (LBO); 8-pixel K groups are 1024 B apart (SBO)
-          const uint64_t da = umma_desc_mn_sw128(sa, p.lbo, p.sbo), db = umma_desc_mn_sw128(sb, p.lbo, p.sbo);
-          if (elect_one()) {
-            for (int k = 0; k < p.px / 16; ++k)                      // 16 pixels = two 1024-byte atoms: start address += 2048 B
-              umma_f16(tmem_base, da + (uint64_t)(k * (2048 >> 4)), db + (uint64_t)(k * (2048 >> 4)), idesc, (i | k) != 0);
-            umma_commit(smem_u32(&s_empty[s]));
-          }
-          __syncwarp();
-        }
-        if (elect_one()) umma_commit(smem_u32(&s_tfull));
-        __syncwarp();
-      }
-    } else {
-      // ===================== epilogue: TMEM -> registers -> global reductions =====================
-      const int quad = warp & 3;
-      const int r = r0 + quad * 32 + lane;
-      mbar_wait(smem_u32(&s_tfull), 0);
-      __syncwarp();
-      tc_fence_after();
-      for (int c = 0; c * 32 < p.bc; ++c) {
-        uint32_t raw[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(c * 32), raw);
-        if (r < p.R) {
-          const int cb = c0 + c * 32;
-          if (!p.transpose) {
-            float* o = p.out + (long long)r * p.ldo + cb;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              if (cb + j + 3 < p.Cc) {
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o + j), "f"(__uint_as_float(raw[j])),
-                             "f"(__uint_as_float(raw[j + 1])), "f"(__uint_as_float(raw[j + 2])), "f"(__uint_as_float(raw[j + 3])) : "memory");
-              } else {
-#pragma unroll
-                for (int e = 0; e < 4; ++e) if (cb + j + e < p.Cc) atomicAdd(o + j + e, __uint_as_float(raw[j + e]));
-              }
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)                           // lanes = consecutive r: coalesced scalar reductions
-              if (cb + j < p.Cc) atomicAdd(p.out + (long long)(cb + j) * p.ldo + r, __uint_as_float(raw[j]));
+  if (warp == 8) {
+    if (lane == 0) {
+      for (int i = 0; i < nkb; ++i) {
+        const int s = i % p.stages;
+        const uint32_t ph = (i / p.stages) & 1;
+        mbar_wait(smem_u32(&s_empty[s]), ph ^ 1);
+        const uint32_t full = smem_u32(&s_full[s]);
+        const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes), sb = sa + a_bytes;
+        const int px = (kb_lo + i) * p.px;
+        mbar_expect_tx(full, (uint32_t)stage_bytes);            // TMA counts whole boxes (zero-filled parts included)
+        tma_load_2d(sa, &mapA, full, r0, px);                    // out-of-range channels / pixels are zero-filled: they add 0
+        tma_load_2d(sa + box_bytes, &mapA, full, r0 + 64, px);
+        if (p.stem_ho > 0) {
+          const int b = (kb_lo + i) / p.stem_ho, oh = (kb_lo + i) - b * p.stem_ho;
+          for (int j = 0; j < nbb; ++j)                          // tap a = c0 / 64 + j: the windows of s2d row oh - 2 + a
+            tma_load_4d(sb + j * box_bytes, &mapB1, full, 0, 0, oh - 2 + c0 / 64 + j, b);
+        } else {
+          for (int j = 0; j < nbb; ++j) {
+            const int c = c0 + j * 64;
+            if (c < p.C1) tma_load_2d(sb + j * box_bytes, &mapB1, full, c, px);
+            else tma_load_2d(sb + j * box_bytes, &mapB2, full, c - p.C1, px);
           }
         }
       }
     }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
+
+  // ===================== consumers: wgmma over the pixel range, then registers -> global reductions =====================
+  const int wg = warp >> 2, wl = warp & 3;
+  float acc[4][32];
+  if (nkb <= 0) {                                              // an empty split still stores its (zero) partial
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
   }
+  int prev_s = 0;
+  for (int i = 0; i < nkb; ++i) {
+    const int s = i % p.stages;
+    const uint32_t ph = (i / p.stages) & 1;
+    mbar_wait(smem_u32(&s_full[s]), ph);
+    const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes), sb = sa + a_bytes;
+    // A: this warpgroup's 64 rows are box wg; B: 64-column chunk c is box c.  8-pixel K groups are 1024 B apart (SBO),
+    // 16 pixels = two 1024-byte atoms: start address += 2048 B per K step
+    const uint64_t da = wgmma_desc_mn_sw128(sa + (uint32_t)(wg * box_bytes), p.lbo, p.sbo);
+    const uint64_t db = wgmma_desc_mn_sw128(sb, p.lbo, p.sbo);
+    wgmma_fence();
+    for (int k = 0; k < p.px / 16; ++k) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (c < nbb)
+          wgmma_m64n64k16<1, 1>(acc[c], da + (uint64_t)(k * (2048 >> 4)), db + (uint64_t)((c * box_bytes) >> 4) + (uint64_t)(k * (2048 >> 4)),
+                                (i | k) != 0);
+    }
+    wgmma_commit();
+    if (i > 0) {                                                 // the previous stage's MMAs have retired: hand it back
+      wgmma_wait<1>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(smem_u32(&s_empty[prev_s]));
+    }
+    prev_s = s;
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int c = 0; c < 4; ++c) if (c < nbb) wgmma_fence_acc(acc[c]);
+  float* part = p.part + (size_t)split * p.R * p.Cc;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    if (c >= nbb) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + wg * 64 + wl * 16 + (lane >> 2) + 8 * h;
+      if (r >= p.R) continue;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int cb = c0 + c * 64 + j * 8 + 2 * (lane & 3);
+        float* o = part + (size_t)r * p.Cc + cb;
+        if (cb + 1 < p.Cc) *reinterpret_cast<float2*>(o) = make_float2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]);
+        else if (cb < p.Cc) *o = acc[c][4 * j + 2 * h];
+      }
+    }
+  }
+}
+
+// OUT += the sum of the split-K partial tiles, added in split order (run-to-run identical; float atomics would add them in the
+// order the CTAs finish)
+__global__ void __launch_bounds__(256)
+wgrad_reduce_kernel(const float* __restrict__ part, int splits, int R, int Cc, float* __restrict__ out, long long ldo, int transpose) {
+  const long long n = (long long)R * Cc;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float t = 0.f;
+    for (int s = 0; s < splits; ++s) t += __ldg(part + (size_t)s * n + i);
+    const int r = (int)(i / Cc), c = (int)(i - (long long)r * Cc);
+    float* o = transpose ? out + (long long)c * ldo + r : out + (long long)r * ldo + c;
+    *o += t;
+  }
+}
+
+static int wgrad_launch(const CUtensorMap& ma, const CUtensorMap& mb1, const CUtensorMap& mb2, WgParams p, int grid, int smem,
+                        cudaStream_t st, const char* what, double alg_bytes) {
+  DetScratch ds;                                               // the partials, stream-ordered (common.cuh)
+  int rc = ds.alloc((size_t)p.splits * p.R * p.Cc, 0, st);
+  if (rc) return rc;
+  p.part = ds.a.scr;
+  static PerDevFlag configured_d;
+  if (bool& configured = configured_d.get(); !configured) {
+    cudaError_t e = cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
+    configured = true;
+  }
+  {
+    COTB200_PROF_B(what, alg_bytes);
+    tc_wgrad_kernel<<<grid, WG_THREADS, smem, st>>>(ma, mb1, mb2, p);
+    if ((rc = check_launch(what))) return rc;
+  }
+  const long long n = (long long)p.R * p.Cc;
+  const int rgrid = (int)((n + 255) / 256 < 4LL * num_sms() ? (n + 255) / 256 : 4LL * num_sms());
+  COTB200_PROF_B("wgrad_reduce", 4.0 * (double)n * (p.splits + 2));
+  wgrad_reduce_kernel<<<rgrid, 256, 0, st>>>(p.part, p.splits, p.R, p.Cc, p.out, p.ldo, p.transpose);
+  return check_launch("wgrad_reduce");
 }
 
 // bf16 pixel matrix [rows = pixels, cols = channels] with pitch ld: box {64 channels, 64 pixels}, 128B swizzle, zero OOB fill
@@ -216,8 +240,7 @@ extern "C" int cotb200_wgrad_bf16(int M, int R, const void* A, long long lda, in
   const int per = (p.kb_total + splits - 1) / splits;
   splits = (p.kb_total + per - 1) / per;                       // no empty splits
   p.splits = splits;
-  // MN blocks of 64 channels are one box (8 KB) apart = LBO; 8-pixel K groups are 1024 B apart = SBO (validated on the B200
-  // against fp32 matmul; the swapped convention reads past the operand tiles).
+  // MN blocks of 64 channels are one box (8 KB) apart = LBO; 8-pixel K groups are 1024 B apart = SBO.
   p.lbo = WG_BOX_BYTES; p.sbo = 1024;
   p.px = WG_PX; p.stages = WG_STAGES; p.stem_ho = 0;
   CUtensorMap ma, mb1, mb2;
@@ -226,15 +249,7 @@ extern "C" int cotb200_wgrad_bf16(int M, int R, const void* A, long long lda, in
   if ((rc = wg_make_map(&mb1, B1, M, C1, ldb1))) return rc;
   if (C2 > 0) { if ((rc = wg_make_map(&mb2, B2, M, C2, ldb2))) return rc; } else mb2 = mb1;
   const int smem = WG_STAGES * (2 * WG_BOX_BYTES + (p.bc / 64) * WG_BOX_BYTES) + 1024;
-  static PerDevFlag configured_d;
-  if (bool& configured = configured_d.get(); !configured) {
-    cudaError_t e = cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
-    configured = true;
-  }
-  COTB200_PROF_B("tc_wgrad", 2.0 * (double)M * (R + Cc) + 4.0 * (double)R * Cc);
-  tc_wgrad_kernel<<<tiles * splits, WG_THREADS, smem, st>>>(ma, mb1, mb2, p);
-  return check_launch("tc_wgrad");
+  return wgrad_launch(ma, mb1, mb2, p, tiles * splits, smem, st, "tc_wgrad", 2.0 * (double)M * (R + Cc) + 4.0 * (double)R * Cc);
 }
 
 
@@ -293,13 +308,6 @@ extern "C" int cotb200_stem7x7s2_wgrad_bf16(int B, int H, int W, const void* dY,
     }
   }
   const int smem = p.stages * stage_bytes + 1024;
-  static PerDevFlag configured_d;
-  if (bool& configured = configured_d.get(); !configured) {
-    cudaError_t e = cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
-    configured = true;
-  }
-  COTB200_PROF_B("tc_stem_wgrad", 2.0 * (double)p.M * N + (double)B * Hh * (Wh + 4) * 32 + 4.0 * N * 256);
-  tc_wgrad_kernel<<<p.splits, WG_THREADS, smem, st>>>(ma, mb, mb, p);
-  return check_launch("tc_stem_wgrad");
+  return wgrad_launch(ma, mb, mb, p, p.splits, smem, st, "tc_stem_wgrad",
+                      2.0 * (double)p.M * N + (double)B * Hh * (Wh + 4) * 32 + 4.0 * N * 256);
 }

@@ -1,4 +1,4 @@
-// PTX wrappers shared by the TMA / mbarrier pipelines (agg_tma.cu, agg_nchw_tma.cu, gn72.cu, tc_gemm.cu), sm_100a.
+// PTX wrappers shared by the TMA / mbarrier pipelines (agg_tma.cu, agg_nchw_tma.cu, gn72.cu, tc_gemm.cu), sm_90a.
 // Every wait is a BOUNDED try_wait spin that __trap()s: a broken pipeline aborts the launch instead of hanging the GPU.
 #pragma once
 #include <cuda.h>

@@ -92,7 +92,7 @@ def broadcast_module_(module, src=0):
 class FlatGrads:
     """All gradients of a replica in ONE flat buffer: every `p.grad` is a view (same strides as `p`) into `flat`, so
     backward accumulates straight into the bucket, `zero_()` is one memset and the data-parallel reduction is ONE
-    all-reduce(mean) per step -- the gradients of CoTNet-50 are 89 MB, ~0.25 ms on NVLink 5, so there is nothing to
+    all-reduce(mean) per step -- the gradients of CoTNet-50 are 89 MB, a fraction of a millisecond on NVLink, so there is nothing to
     gain from DDP's bucketed overlap, and without DDP's autograd hooks the whole fwd+bwd replays from a CUDA graph
     (the collective is issued eagerly between the fwd+bwd graph and the optimizer graph)."""
 

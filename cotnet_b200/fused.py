@@ -78,7 +78,7 @@ def _zeros_esc(shape, device):
     """Zeros that ESCAPE the autograd function as gradients (BatchNorm d-gamma / d-beta sums).  Plain torch.zeros in general -- a
     gradient must survive until its owner reads it -- but a trainer that gathers every gradient inside the step (TrainStep: one gather
     launch into the flat bucket before the next step_begin()) may take them from the pre-zeroed arena too: ~140 fill launches per
-    CoTNet-50 step less (profiles/r02_launches_cotnet50_callN.md)."""
+    CoTNet-50 step less."""
     return _zeros(shape, device) if _ARENA.escape_ok else torch.zeros(*shape, dtype=torch.float32, device=device)
 
 
@@ -176,7 +176,7 @@ def _bn_batch_stats(x, bn, weight, bias, lib, st, dt):
 
 
 def _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt):
-    """Training-mode BatchNorm tail shared by BNActFn and the tcgen05 functions: ONE kernel finalises the batch statistics
+    """Training-mode BatchNorm tail shared by BNActFn and the wgmma functions: ONE kernel finalises the batch statistics
     (sums = [2, C] column sums over the B*H*W rows of x), updates the running buffers and applies scale/shift(+res)(+ReLU).
     Returns ss = [4, C] (scale, shift, mean, rstd) for the backward."""
     B, C, H, W = x.shape
@@ -254,7 +254,7 @@ class BNActFn(Function):
 def _two_grads(grads):
     """Incoming gradients of a (possibly forked) output: (dy, dy2) as channels_last tensors, dy2 None when there is one gradient.
     A forked BatchNorm output feeds two consumers -- the next bottleneck's conv1 and its shortcut (models/cotnet.py:228-262) -- and
-    autograd would add their gradients with a separate kernel (read 2 + write 1 of the block-sized tensor, 1.2 ms per CoTNet-50 step);
+    autograd would add their gradients with a separate kernel (read 2 + write 1 of the block-sized tensor);
     handing both to the BatchNorm backward kernels, which sum them in fp32 while they stream dy anyway, costs one extra read each."""
     g = [t.contiguous(memory_format=torch.channels_last) for t in grads if t is not None]
     if not g:
@@ -688,10 +688,10 @@ def split_attn_tail(u, bn0: torch.nn.BatchNorm2d, fc1, bn1, fc2):
 
 
 # ====================================================================================================================
-# Dense parts of the block on the tcgen05 kernels, with autograd.
+# Dense parts of the block on the wgmma kernels, with autograd.
 #   forward      : tc GEMM / implicit-GEMM conv; training-mode BatchNorm statistics come out of the GEMM epilogue
 #   data gradient: the same tc kernels (transposed weights; the 3x3 conv with flipped taps)
-#   weight grad  : 1x1: the MN-major tcgen05 kernel (tc_wgrad.cu); the grouped 3x3 still goes through cuDNN
+#   weight grad  : 1x1: the MN-major wgmma kernel (tc_wgrad.cu); the grouped 3x3 still goes through cuDNN
 # ====================================================================================================================
 from . import tc as _tc  # noqa: E402
 import os as _os  # noqa: E402
@@ -817,11 +817,11 @@ class TcConv1x1Fn(Function):
             _tc.gemm_bf16(dpre, wt[K1:], out=_rows2d(da2))
         dw = None
         if ctx.needs_input_grad[2]:
-            # weight gradient dW = dpre^T [a1 | a2] on the MN-major tcgen05 kernel (csrc/tc_wgrad.cu): the NHWC tiles are
+            # weight gradient dW = dpre^T [a1 | a2] on the MN-major wgmma kernel (csrc/tc_wgrad.cu): the NHWC tiles are
             # consumed as they land, fp32 accumulation, one launch for both operand pairs
             if N * (K1 + K2) >= 1024 * 1024 or (N * (K1 + K2) >= 256 * 1024 and M >= 40000):
                 # large, compute-shaped weight gradients (bottleneck convolutions of stages 3-4): the library kernel is faster
-                # (profiles/r02_bench_conv_*.json); everything byte-heavy stays on the MN-major tcgen05 kernel
+                # ; everything byte-heavy stays on the MN-major wgmma kernel
                 parts = [torch.mm(d2.t(), _rows2d(a1))]
                 if a2 is not None:
                     parts.append(torch.mm(d2.t(), _rows2d(a2)))
@@ -905,7 +905,7 @@ class TcConv3x3Fn(Function):
 
 class StemConvBNFn(Function):
     """act1(bn1(conv1(x))) of the trunk (models/resnet.py:552-554,601-603): 7x7 / stride 2 / pad 3, 3 -> N channels, on the 4-tap
-    tcgen05 implicit GEMM (cotb200_stem7x7s2_bf16) with the BatchNorm statistics in its epilogue.  x: channels_last bf16.
+    wgmma implicit GEMM (cotb200_stem7x7s2_bf16) with the BatchNorm statistics in its epilogue.  x: channels_last bf16.
     Backward: fused BatchNorm backward kernels; the weight gradient of the 3-channel convolution stays on cuDNN (the image
     needs no gradient)."""
 
@@ -960,7 +960,7 @@ class StemConvBNFn(Function):
         if ctx.needs_input_grad[0]:
             dx = torch.nn.grad.conv2d_input(x.shape, wq, dpre, stride=2, padding=3)
         if ctx.needs_input_grad[1]:
-            # weight gradient on the MN-major tcgen05 wgrad kernel over the space-to-depth image of the forward (one stage = one
+            # weight gradient on the MN-major wgmma wgrad kernel over the space-to-depth image of the forward (one stage = one
             # output row, the four row taps as four B boxes); geometries it does not take: cuDNN
             if scratch is not None and stem_wgrad_tc:
                 dw = _tc.stem7x7s2_wgrad(dpre, scratch, x.shape, N)
@@ -970,13 +970,13 @@ class StemConvBNFn(Function):
         return dx, dw, sums[1].to(bndt), sums[0].to(bndt), None, None
 
 
-#: the trunk's 7x7 stem convolution on the tcgen05 implicit GEMM (0 = cuDNN, the round-1 path)
+#: the trunk's 7x7 stem convolution on the wgmma implicit GEMM (0 = cuDNN, the round-1 path)
 stem_tc = _os.environ.get("COTB200_STEM_TC", "1") != "0"
 stem_wgrad_tc = _os.environ.get("COTB200_STEM_WGRAD_TC", "1") != "0"
 
 
 def stem_conv_bn(x, conv, bn, relu=True):
-    """act(bn(conv(x))) for the 7x7/s2 stem.  tcgen05 path for channels_last bf16 3-channel images of even size (and an image
+    """act(bn(conv(x))) for the 7x7/s2 stem.  wgmma path for channels_last bf16 3-channel images of even size (and an image
     row of at most 256 output pixels per tile segment); anything else: cuDNN + the fused BatchNorm kernels."""
     w = conv.weight
     if (stem_tc and x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.shape[1] == 3 and tuple(w.shape[1:]) == (3, 7, 7)
@@ -987,14 +987,14 @@ def stem_conv_bn(x, conv, bn, relu=True):
     return bn_act(conv(x).contiguous(memory_format=torch.channels_last), bn, relu=relu)
 
 
-#: which 1x1 convolutions of the ENCLOSING bottleneck (conv1 / conv3 / stride-1 downsample) run on the tcgen05 kernels in
+#: which 1x1 convolutions of the ENCLOSING bottleneck (conv1 / conv3 / stride-1 downsample) run on the wgmma kernels in
 #: training: "tc_all1x1" = all of them (forward with the BatchNorm statistics in the epilogue, data and weight gradients),
 #: anything else = cuDNN + the fused BatchNorm kernels.  Same environment variable as CotLayer.train_conv_backend.
 trunk_conv_backend = _os.environ.get("COTB200_TRAIN_CONV", "tc_all1x1+k").replace("+k", "")
 
 
-#: the bottleneck convolutions of stages 3-4 (weights of 256K .. 1M elements, 12.5K-50K pixels) are compute-shaped; measured per
-#: shape (profiles/r02_bench_conv_*.json) cuDNN's 2-CTA kernels win there, the tcgen05 path wins on the byte-heavy stages 1-2
+#: the bottleneck convolutions of stages 3-4 (weights of 256K .. 1M elements, 12.5K-50K pixels) are compute-shaped
+#: (K = 1024 / 2048) and stay on cuDNN; the wgmma path takes the byte-heavy stages 1-2
 TC_TRUNK_MAX_WEIGHT = int(_os.environ.get("COTB200_TC_TRUNK_MAX_WEIGHT", str(128 * 1024)))
 
 
@@ -1002,7 +1002,7 @@ TC_MIN_PIXELS = int(_os.environ.get("COTB200_TC_MIN_PIXELS", "100000"))
 
 
 def conv1x1_bn(x, conv, bn, relu, res=None, fork=False):
-    """act(BN(conv1x1(x)) (+ res)) for the bottleneck's 1x1 convolutions (models/cotnet.py:229-235,249-262): on the tcgen05
+    """act(BN(conv1x1(x)) (+ res)) for the bottleneck's 1x1 convolutions (models/cotnet.py:229-235,249-262): on the wgmma
     GEMMs when the backend says so and the geometry allows (bf16 channels_last, stride 1, dense, no bias), else cuDNN + the
     fused BatchNorm kernels."""
     w = conv.weight

@@ -1,4 +1,4 @@
-"""Thin torch-side wrappers of the tcgen05 GEMM / implicit-GEMM conv entry points (include/cotb200.h).
+"""Thin torch-side wrappers of the wgmma GEMM / implicit-GEMM conv entry points (include/cotb200.h).
 
 These are plumbing for the fused CoT block and for the unit tests: they allocate outputs with torch, pass raw
 pointers + the current stream to the C ABI, and never fall back to cuBLAS/cuDNN."""
@@ -107,7 +107,7 @@ def prepare_conv3x3_weight(weight, groups, transpose_for_dgrad=False):
     transpose_for_dgrad: build the weight of the data-gradient convolution (taps flipped, in/out swapped per group)."""
     C, cg = weight.shape[0], weight.shape[1]
     bn = conv_tile(C, groups)
-    assert bn is not None, "unsupported grouped-conv geometry for the tcgen05 path"
+    assert bn is not None, "unsupported grouped-conv geometry for the wgmma path"
     w = weight.detach().float().view(groups, cg, cg, 3, 3)            # [g, out, in, kh, kw]
     if transpose_for_dgrad:
         w = w.permute(0, 2, 1, 3, 4).flip(3, 4)                       # dX = conv(dY, W^T flipped)

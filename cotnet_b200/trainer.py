@@ -1,4 +1,4 @@
-"""One data-parallel training step of a CoT network, B200-native (SURVEY.md section 8e + 8f rank 3).
+"""One data-parallel training step of a CoT network, H100-native (SURVEY.md section 8e + 8f rank 3).
 
 Mirrors the body of the reference's training loop -- forward under autocast, loss, backward, ``optimizer.step()``,
 ``model_ema.update(model)`` (/root/reference/train.py:255-277) -- and what DistributedDataParallel does around it
@@ -31,8 +31,8 @@ from . import _lib, fused
 
 #: COTB200_BOOKKEEPING=0: one `num_batches_tracked += 1` kernel per BatchNorm instead of one multi-tensor add per step.
 #: COTB200_ARENA_ESCAPE=1 (opt-in): BatchNorm / GroupNorm gradient sums from the pre-zeroed step arena instead of torch.zeros (~140 fill
-#: launches per step less; 37.89 vs 37.98 ms on one box, profiles/r02_bench_callQ_*.json).  Off by default: it is worth < 0.1 ms and the
-#: gradients of 1-D parameters would then alias memory that the next step_begin() recycles.
+#: launches per step less).  Off by default: the gradients of 1-D parameters would then alias memory that the next step_begin()
+#: recycles.
 import os as _os
 _BOOKKEEPING = _os.environ.get("COTB200_BOOKKEEPING", "1") != "0"
 _ARENA_ESCAPE = _os.environ.get("COTB200_ARENA_ESCAPE", "0") != "0"

@@ -1,15 +1,21 @@
 /*
- * cotb200.h -- C ABI of libcotb200.so: the B200-native (sm_100a) kernels of the CoT-block hot path.
+ * cotb200.h -- C ABI of libcotb200.so: the H100-native (sm_90a) kernels of the CoT-block hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  The reference has no C ABI: its "FFI" is CuPy --
  *   load_kernel(name, code, **literals) -> cupy.cuda.compile_with_cache(code).get_function(name)
- *                                                       (/root/reference/cupy_layers/utils.py:14-18)
+ *                                                       (cupy_layers/utils.py:14-18)
  *   f(block=(1024,1,1), grid=(GET_BLOCKS(n),1,1), args=[ptr,...], stream=Stream(ptr=current_stream))
- *                                                       (/root/reference/cupy_layers/aggregation_zeropad.py:130-143)
+ *                                                       (cupy_layers/aggregation_zeropad.py:130-143)
  * with every dimension baked into the NVRTC source.  Each entry point below names the reference launch it
  * replaces; dimensions are runtime arguments (no per-shape JIT), pointers are raw device pointers, the
- * stream is a cudaStream_t passed as void*.  No torch types, no allocation, no hidden synchronisation:
- * every call is asynchronous on the given stream and safe under CUDA-graph capture.
+ * stream is a cudaStream_t passed as void*.  No torch types, no hidden synchronisation: every call is asynchronous on
+ * the given stream and safe under CUDA-graph capture.
+ *
+ * Reductions over many CTAs (the statistics and backward sums below, the GEMM / convolution statistics epilogues, the split
+ * weight gradients) are deterministic: partial sums are added in a fixed order, so the same inputs give bit-identical results
+ * from run to run.  Those calls take their scratch stream-ordered: cudaMallocAsync + cudaMemsetAsync before the launch and
+ * cudaFreeAsync after it, all on the given stream (from the device's default memory pool; inside a graph capture they become
+ * the graph's own allocation, memset and free nodes).  Calls on different streams therefore never share scratch.
  *
  * Return value: 0 on success; >0 = cudaError_t from the launch; <0 = COTB200_E* argument error.
  * cotb200_last_error() returns a thread-local, human-readable description of the last failure.
@@ -139,8 +145,8 @@ int cotb200_agg_zeropad_mix_merge_bwd(const cotb200_agg_desc* d, int k2h, int k2
 
 /* ---- fused normalisation / split-attention kernels on NHWC tensors [B, HW, C] (channel contiguous), fp32 math ----
  * They replace chains of eager launches of the reference block (models/cotnet.py:56 and :89-104).
- * dtype: COTB200_F32 / BF16 / F16.  All float* arguments are fp32 device arrays; sums are ACCUMULATED (+=) with
- * atomics, so the caller zeroes them. */
+ * dtype: COTB200_F32 / BF16 / F16.  All float* arguments are fp32 device arrays; sums are ACCUMULATED (+=), in a fixed
+ * order (see the top of this file), so the caller zeroes them. */
 
 /* sum[c] += sum_rows x, sq[c] += sum_rows x^2 : BatchNorm batch statistics (nn.BatchNorm2d training mode, :65,:89) */
 int cotb200_col_stats(int dtype, int B, int HW, int C, const void* x, float* sum, float* sq, void* stream);
@@ -251,7 +257,7 @@ int cotb200_pool3s2_fwd(int dtype, int mode, int N, int H, int W, int C, const v
 int cotb200_pool3s2_bwd(int dtype, int mode, int N, int H, int W, int C, const void* dy, const void* idx, void* dx,
                         void* stream);
 
-/* ---- dense contractions of the block on the 5th-gen tensor cores (tcgen05.mma, TMEM accumulators, TMA operands) ----
+/* ---- dense contractions of the block on the Hopper tensor cores (wgmma, register accumulators, TMA operands) ----
  * bf16 operands, fp32 accumulation, bf16 output.  Row-major everywhere; "ld*" are row pitches in elements.
  *
  * cotb200_gemm_bf16:  D[M,N] = epi( A1[M,K1] B1[N,K1]^T + A2[M,K2] B2[N,K2]^T )      (K2 == 0: single product)
@@ -297,7 +303,7 @@ int cotb200_conv3x3_bf16(int B, int H, int W, int C, const void* X, long long ld
 
 /* cotb200_stem7x7s2_bf16: the stem convolution conv1 = nn.Conv2d(3, N, 7, stride=2, padding=3, bias=False)
  *   (models/resnet.py:552, called at :601; cuDNN in the reference) on an NHWC bf16 image X[B,H,W,3] (dense, H and W even) as a
- *   4-tap implicit tcgen05 GEMM: a space-to-depth copy of the image (scratch, cotb200_stem7x7s2_scratch_bytes bytes, 16-byte
+ *   4-tap implicit wgmma GEMM: a space-to-depth copy of the image (scratch, cotb200_stem7x7s2_scratch_bytes bytes, 16-byte
  *   aligned) turns the 7x7/s2 window into 4 rows x 4 cells x 16 channels, and one TMA box per row fetches the overlapping
  *   windows of a whole output-row segment as the K-major A tile (K = 4 x 64).  D[B*(H/2)*(W/2), N] bf16 (row pitch ldd).
  *   Wm [N, 256] bf16: Wm[n, a*64 + a2*16 + (di*2+dj)*3 + c] = weight[n, c, 2a+di-1, 2a2+dj-1] (0 where an index is -1 and
@@ -311,15 +317,15 @@ int cotb200_stem7x7s2_bf16(int B, int H, int W, const void* X, const void* Wm, i
 /* cotb200_stem7x7s2_wgrad_bf16: weight gradient of that convolution in the packed layout of Wm (cuDNN wgrad in the reference's
  *   autograd graph):  dWm[n, a*64 + j] += sum_px dY[px, n] * window_a(px)[j], fp32 [N, 256], ZEROED by the caller.  dY [B*(H/2)*(W/2), N]
  *   bf16 (row pitch ldy); scratch = the space-to-depth image cotb200_stem7x7s2_bf16 filled for the same X.  One pipeline stage of
- *   the MN-major tcgen05 wgrad kernel = one output row (W/2 pixels, a multiple of 16, <= 128).  COTB200_EUNSUPPORTED otherwise. */
+ *   the MN-major wgmma wgrad kernel = one output row (W/2 pixels, a multiple of 16, <= 128).  COTB200_EUNSUPPORTED otherwise. */
 int cotb200_stem7x7s2_wgrad_bf16(int B, int H, int W, const void* dY, long long ldy, int N, const void* scratch, float* dWm,
                                  void* stream);
 
 /* cotb200_wgrad_bf16: weight gradient of a 1x1 convolution,  OUT += A[M,R]^T [B1[M,C1] | B2[M,C2]]  (contraction over the M
- *   pixels; A = dY, B = the convolution input(s); bf16 operands, fp32 accumulation in TMEM, fp32 OUT).  Replaces cuDNN's wgrad
+ *   pixels; A = dY, B = the convolution input(s); bf16 operands, fp32 accumulation, fp32 OUT).  Replaces cuDNN's wgrad
  *   for embed.0 / embed.3 / conv1x1.0 (models/cotnet.py:52,55,60) and the bottleneck's 1x1 convolutions (:228-264).
  *   Both operands are consumed MN-major straight from their NHWC tiles (no transposes).  Split over pixel ranges across the
- *   SMs; partial tiles are added to OUT with global reductions, so the caller ZEROES OUT first.
+ *   SMs; the partial tiles are added to OUT in split order by a second kernel, so the caller ZEROES OUT first.
  *   transpose = 0: OUT[r*ldo + c] (r < R, c < C1+C2); transpose = 1: OUT[c*ldo + r].
  *   Requirements: R, C1, C2 multiples of 8 (C1 a multiple of 64 when C2 > 0); operands 16-byte aligned. */
 int cotb200_wgrad_bf16(int M, int R, const void* A, long long lda, int C1, const void* B1, long long ldb1,

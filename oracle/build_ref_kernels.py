@@ -1,4 +1,4 @@
-"""Compile the REFERENCE's own LocalConv CUDA kernels to sm_100 cubins under oracle/_ref/.  TEST INFRASTRUCTURE ONLY.
+"""Compile the REFERENCE's own LocalConv CUDA kernels to sm_90a cubins under oracle/_ref/.  TEST INFRASTRUCTURE ONLY.
 
     python -m oracle.build_ref_kernels            # needs /root/reference (build container); writes oracle/_ref/
 
@@ -8,7 +8,7 @@ aggregation_zeropad_mix.py:20-207), substitutes every dimension as a literal (cu
 /root/reference does not exist on the GPU box, so this recipe performs exactly that build step ahead of time:
 
   * the reference module is imported unmodified (oracle/ref_import.py shims `cupy`);
-  * `cupy.cuda.compile_with_cache` is pointed at nvcc (`-cubin -arch=sm_100a`), and the reference's OWN
+  * `cupy.cuda.compile_with_cache` is pointed at nvcc (`-cubin -arch=sm_90a`), and the reference's OWN
     `load_kernel(name, code, **literals)` is called with the literals its forward/backward pass for a shape
     (aggregation_zeropad.py:130-139,155-163,170,179; mix :230-241,257-269,274,284);
   * only BINARY outputs land in oracle/_ref/ (one cubin per kernel x shape x dtype + manifest.json with the launch
@@ -64,7 +64,7 @@ def _compile_with_cache(code):
     with tempfile.TemporaryDirectory() as td:            # the source text never touches the repository
         src, dst = os.path.join(td, "k.cu"), os.path.join(td, "k.cubin")
         open(src, "w").write(code)
-        subprocess.run(["nvcc", "-cubin", "-arch=sm_100a", "-O3", "-o", dst, src], check=True, capture_output=True)
+        subprocess.run(["nvcc", "-cubin", "-arch=sm_90a", "-O3", "-o", dst, src], check=True, capture_output=True)
         return _NvccModule(open(dst, "rb").read())
 
 

@@ -5,7 +5,7 @@ The reference touches exactly two CuPy entry points (cupy_layers/utils.py:14-18)
     @cupy.memoize(for_each_device=True)           -> a per-(device, arguments) memo decorator
     cupy.cuda.compile_with_cache(code)            -> NVRTC compile of the substituted kernel source; .get_function(name)
 and launches the returned function as  f(block=(..), grid=(..), args=[ptr, ...], stream=Stream(ptr=...))
-(cupy_layers/aggregation_zeropad.py:140-143).  Here the compile step is `nvcc -cubin -arch=sm_100a` (NVRTC and nvcc share
+(cupy_layers/aggregation_zeropad.py:140-143).  Here the compile step is `nvcc -cubin -arch=sm_90a` (NVRTC and nvcc share
 the front end; the image has no CuPy) and the launch goes through the CUDA driver API with ctypes.  The kernel SOURCE is
 the reference's string, untouched; it lives only in a temporary directory.
 """
@@ -61,7 +61,7 @@ def compile_with_cache(code):
     with tempfile.TemporaryDirectory() as td:
         src, dst = os.path.join(td, "k.cu"), os.path.join(td, "k.cubin")
         open(src, "w").write(code)
-        subprocess.run(["nvcc", "-cubin", "-arch=sm_100a", "-O3", "-o", dst, src], check=True, capture_output=True)
+        subprocess.run(["nvcc", "-cubin", "-arch=sm_90a", "-O3", "-o", dst, src], check=True, capture_output=True)
         return _Module(open(dst, "rb").read())
 
 

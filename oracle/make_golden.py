@@ -204,6 +204,56 @@ TRAIN_FIXTURES = [("cotnet50_train_bf16w.npz", "cotnet50", 3001, 224, 16, True),
                   ("se_cotnetd152_train_320.npz", "se_cotnetd_152", 3004, 320, 4, False)]
 
 
+def _live_layer_fixture(fname):
+    """CotLayer(64) eval output at 7x7 from the reference's module code (tests/test_oracle.py checks the restatement against it)."""
+    ref = ref_import.load()
+    gen = torch.Generator().manual_seed(77)
+    sd = cot_ref.init_state_dict("cot", 64, gen)
+    x = torch.relu(torch.randn(2, 64, 7, 7, generator=gen, dtype=torch.float64))
+    m = ref.CotLayer(64, 3).double()
+    m.load_state_dict(sd, strict=True)
+    m.eval()
+    with torch.no_grad():
+        y = m(x)
+    np.savez_compressed(os.path.join(OUT, fname), y=y.numpy())
+
+
+HYBRID_TRAIN_SEED = 31
+
+
+def hybrid_train_inputs():
+    return (torch.randn(2, 3, 64, 64, dtype=torch.float64, generator=torch.Generator().manual_seed(5)),
+            torch.randn(2, 1000, dtype=torch.float64, generator=torch.Generator().manual_seed(6)))
+
+
+def hybrid_train_record(m, seed=HYBRID_TRAIN_SEED):
+    """One fp64 training step of SE-CoTNetD-50 (seeded state, hybrid_train_inputs): output, every parameter gradient pinned as
+    (sum, <grad, proj_vector>, ||grad||^2), and the sums of the running statistics after the step."""
+    x, cot = hybrid_train_inputs()
+    m.train()
+    y = m(x)
+    names = [n for n, _ in m.named_parameters()]
+    grads = torch.autograd.grad((y * cot).sum(), [p for _, p in m.named_parameters()])
+    g = np.array([[t.sum().item(), (t * proj_vector(n, t.shape, seed)).sum().item(), (t * t).sum().item()]
+                  for n, t in zip(names, grads)])
+    run = np.array([v.sum().item() for k, v in m.state_dict().items() if k.endswith("running_mean") or k.endswith("running_var")])
+    return y.detach().numpy(), g, run
+
+
+def _hybrid_live_fixture(fname, seed=HYBRID_TRAIN_SEED):
+    """State-dict layout of SE-CoTNetD-50/101/152 and one training step of SE-CoTNetD-50 from the reference's model code
+    (tests/test_hybrid_cpu.py)."""
+    import json
+    ref = ref_import.load()
+    rec = {}
+    for name in ("se_cotnetd_50", "se_cotnetd_101", "se_cotnetd_152"):
+        sd = getattr(ref.hybrid, name)().state_dict()
+        rec["layout/" + name] = np.frombuffer(json.dumps([[k, list(v.shape)] for k, v in sd.items()]).encode(), dtype=np.uint8)
+    m = hybrid_seeded_state(ref.hybrid.se_cotnetd_50(zero_init_last_bn=False), seed).double()
+    rec["y"], rec["grads"], rec["running"] = hybrid_train_record(m, seed)
+    np.savez_compressed(os.path.join(OUT, fname), **rec)
+
+
 def main():
     if len(sys.argv) > 1 and sys.argv[1] == "train":
         os.makedirs(OUT, exist_ok=True)
@@ -225,6 +275,8 @@ def main():
     _agg_fixture("agg_cot_k3.npz", 3, 1, 2, 16, 2, 7, 6, 13)
     _mix_fixture("agg_mix_selftest.npz", 14)
     _hybrid_fixture("se_cotnetd50_eval_logits.npz", 2024)
+    _live_layer_fixture("cot_layer_live_7x7.npz")
+    _hybrid_live_fixture("se_cotnetd50_train_fp64.npz")
     _trunk_fixture("cotnet50_eval_logits.npz", "cotnet50", 2025)
     _trunk_fixture("cotnext50_eval_logits.npz", "cotnext50_2x48d", 2026)
 

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 box with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -23,7 +23,7 @@ def pytest_collection_modifyitems(config, items):
         has_cuda = False
     if has_cuda:
         return
-    skip = pytest.mark.skip(reason="no CUDA device (GPU tests run on the B200 box: pytest -m gpu)")
+    skip = pytest.mark.skip(reason="no CUDA device (GPU tests run on the H100 box: pytest -m gpu)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

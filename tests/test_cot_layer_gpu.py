@@ -202,7 +202,7 @@ def test_backbone_training_step_matches_oracle_fp32():
 @pytest.mark.parametrize("backend", ["tc", "tc_e0", "tc_1x1", "tc_e0e3", "tc_all1x1", "tc_all1x1+k"])
 @pytest.mark.parametrize("dim,H", [(64, 28), (128, 14), (256, 14), (512, 7)])
 def test_tc_training_backend_vs_oracle(dim, H, backend):
-    """train_conv_backend='tc': every convolution of the block on the tcgen05 kernels, forward + backward, vs the oracle."""
+    """train_conv_backend='tc': every convolution of the block on the wgmma kernels, forward + backward, vs the oracle."""
     gen = torch.Generator().manual_seed(dim)
     sd64 = cot_ref.init_state_dict("cot", dim, gen, dtype=torch.float64, perturb=True)
     dtype = torch.bfloat16
@@ -229,7 +229,7 @@ def test_tc_training_backend_vs_oracle(dim, H, backend):
         rel["tc" if be != "cudnn" else "cudnn"] = (((out.double().cpu() - want.detach()).norm() / want.detach().norm()).item(),
                         ((x.grad.double().cpu() - xr.grad).norm() / xr.grad.norm()).item())
     # bf16 activations between the stages: ReLU masks come from rounded pre-activations and four batch-statistics
-    # BatchNorms amplify that -- the Frobenius error of ANY bf16 pipeline sits at the percent level here.  The tcgen05
+    # BatchNorms amplify that -- the Frobenius error of ANY bf16 pipeline sits at the percent level here.  The wgmma
     # backend must be as close to the fp64 oracle as the cuDNN backend is.
     assert rel["tc"][0] <= 3e-2, "forward relative L2 %.3e" % rel["tc"][0]
     assert rel["tc"][1] <= max(8e-2, 2.0 * rel["cudnn"][1] + 2e-2), "dX relative L2 tc %.3e vs cudnn %.3e" % (rel["tc"][1], rel["cudnn"][1])

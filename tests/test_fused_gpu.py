@@ -224,7 +224,7 @@ def test_pool3x3s2(dtype, C, H, W, mode):
     ref_mod = nn.AvgPool2d(3, 2, padding=1) if mode == 0 else nn.MaxPool2d(3, 2, 1)
     # NCHW-contiguous reference on purpose: ATen's channels_last avg_pool2d BACKWARD kernel of this torch build
     # (avg_pool2d_backward_out_cuda_frame_nhwc) disagrees with its own NCHW and CPU implementations by O(1)
-    # (tools/debug_pool.py, profiles/r01_notes.md); the NCHW path is the semantic definition.
+    # (tools/debug_pool.py); the NCHW path is the semantic definition.
     xr = x.detach().float().contiguous().requires_grad_(True)
     yr = ref_mod(xr)
     cot = _cl(torch.randn(yr.shape, generator=g, device="cuda").to(dtype))
@@ -275,7 +275,7 @@ def test_forked_output_sums_the_two_gradients_in_the_bn_backward(dtype, tol, pat
     import copy
     from cotnet_b200 import fused
     if path == "tc_conv1x1" and dtype != torch.bfloat16:
-        pytest.skip("the tcgen05 path is bf16 only")
+        pytest.skip("the wgmma path is bf16 only")
     g = torch.Generator(device="cuda").manual_seed(17)
     B, K, N, H = 6, 64, 128, 14
     x = torch.randn(B, K if path == "tc_conv1x1" else N, H, H, generator=g, device="cuda").to(dtype).contiguous(memory_format=torch.channels_last)

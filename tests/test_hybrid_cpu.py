@@ -56,6 +56,24 @@ def test_golden_logits_se_cotnetd_50(cpu_op):
     assert err <= 1e-5, err
 
 
+def test_stored_reference_state_dict_and_train_step(cpu_op):
+    """The state-dict layout of SE-CoTNetD-50/101/152 and one fp64 training step of SE-CoTNetD-50 (output, every parameter
+    gradient, running statistics) against the reference's model code, as stored in tests/golden/se_cotnetd50_train_fp64.npz
+    (oracle/make_golden.py); test_live_reference_state_dict_and_forward checks the same live where a reference checkout exists."""
+    import json
+    from cotnet_b200 import backbone_hybrid as bh
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "se_cotnetd50_train_fp64.npz"))
+    for name in ("se_cotnetd_50", "se_cotnetd_101", "se_cotnetd_152"):
+        want = json.loads(bytes(g["layout/" + name]).decode())
+        assert [[k, list(v.shape)] for k, v in bh.MODELS[name]().state_dict().items()] == want, name
+    m = make_golden.hybrid_seeded_state(bh.se_cotnetd_50(zero_init_last_bn=False), make_golden.HYBRID_TRAIN_SEED).double()
+    y, grads, run = make_golden.hybrid_train_record(m)
+    assert np.abs(y - g["y"]).max() <= 1e-10 * max(1.0, np.abs(g["y"]).max())
+    scale = np.abs(g["grads"]).max(axis=0)
+    assert (np.abs(grads - g["grads"]) <= 1e-9 * scale + 1e-300).all()
+    assert np.allclose(run, g["running"], rtol=1e-12, atol=1e-12)
+
+
 @pytest.mark.skipif(not ref_import.available(), reason="reference tree not present")
 def test_live_reference_state_dict_and_forward(cpu_op):
     from cotnet_b200 import backbone_hybrid as bh

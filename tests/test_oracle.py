@@ -85,20 +85,22 @@ def test_block_restatement_matches_reference_golden(golden_dir, name, fn):
             assert (got.double() - ref.double()).abs().max() < 1e-12, k
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not present (GPU box)")
-def test_restatement_vs_live_reference_module():
-    """Same check against the live reference module (build container only) at another size."""
-    ref = ref_import.load()
+def test_restatement_vs_live_reference_module(golden_dir):
+    """Same check against the reference module at another size: its output is stored in tests/golden/cot_layer_live_7x7.npz
+    (oracle/make_golden.py) and, where a reference checkout exists, recomputed live as well."""
     gen = torch.Generator().manual_seed(77)
     sd = cot_ref.init_state_dict("cot", 64, gen)
     x = torch.relu(torch.randn(2, 64, 7, 7, generator=gen, dtype=torch.float64))
-    m = ref.CotLayer(64, 3).double()
-    m.load_state_dict(sd, strict=True)
-    m.eval()
-    with torch.no_grad():
-        want = m(x)
     got = cot_ref.cot_layer(x, {k: v.clone() for k, v in sd.items()}, training=False)
-    assert (got - want).abs().max() < 1e-11
+    wants = [torch.from_numpy(np.load(os.path.join(golden_dir, "cot_layer_live_7x7.npz"))["y"])]
+    if ref_import.available():
+        m = ref_import.load().CotLayer(64, 3).double()
+        m.load_state_dict(sd, strict=True)
+        m.eval()
+        with torch.no_grad():
+            wants.append(m(x))
+    for want in wants:
+        assert (got - want).abs().max() < 1e-11
 
 
 def test_reference_kernel_cubins_are_consistent():

@@ -1,18 +1,19 @@
 """Parity of libcotb200 against the REFERENCE'S OWN GPU kernels on identical inputs.
 
-oracle/_ref/*.cubin are the reference's kernel sources (cupy_layers/aggregation_zeropad.py:20-110,
-aggregation_zeropad_mix.py:20-207) compiled ahead of time by oracle/build_ref_kernels.py exactly as its
-`load_kernel` would at first use; oracle/ref_kernels.py launches them like :140-143.  This is the bar BASELINE.json
+The reference's kernel sources (cupy_layers/aggregation_zeropad.py:20-110, aggregation_zeropad_mix.py:20-207), compiled by
+oracle/build_ref_kernels.py exactly as its `load_kernel` would at first use and launched like :140-143, were run on these
+seeded inputs by oracle/ref_golden.py; tests/golden/ref_kernels.npz holds their outputs at 1024 seeded positions per array,
+and the tests compare ours at the same positions.  This is the bar BASELINE.json
 states: "outputs must match the reference CuPy aggregation_zeropad path on identical inputs within 1e-3 (fp32) /
 1e-2 (bf16)"; fp64 keeps the reference self-test gate 1e-9.  Also cross-checks the CPU oracle against the same kernels.
 """
 import pytest
 import torch
 
-from oracle import agg_ref, ref_kernels
+from oracle import agg_ref, ref_golden
+from oracle.ref_golden import sampled
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not ref_kernels.available(), reason="oracle/_ref not built (needs /root/reference at build time)")]
+pytestmark = pytest.mark.gpu
 
 TOL = {"double": 1e-9, "float": 1e-3}
 _RK = {}
@@ -20,12 +21,14 @@ _RK = {}
 
 def rk():
     if "k" not in _RK:
-        _RK["k"] = ref_kernels.RefKernels()
+        _RK["k"] = ref_golden.GoldenRef()
     return _RK["k"]
 
 
 def _close(a, b, tol, what):
-    err = (a.double() - b.double()).abs()
+    """a: our full output; b: the reference's values at the stored positions"""
+    a = sampled(a)
+    err = (a - b.double()).abs()
     assert bool((err <= tol + tol * b.double().abs()).all()), "%s: max err %.3e" % (what, err.max().item())
 
 
@@ -38,8 +41,8 @@ AGG_CASES = [("cfg1", "float"), ("cfg1", "double"), ("selftest_k5", "double"), (
 def test_agg_matches_reference_kernels(tag, dtype):
     import cotnet_b200
     e, x, w, dy = rk().make_inputs(tag, dtype)
-    y_ref = rk().agg_forward(tag, x, w)
-    dx_ref, dw_ref = rk().agg_backward(tag, dy, x, w)
+    y_ref, dx_ref, dw_ref = [rk().ref("agg", tag, dtype, 0, n) for n in ("y", "dx", "dw")]
+    _close(x, rk().ref("agg", tag, dtype, 0, "x"), 0, "inputs")
     xo, wo = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
     y = cotnet_b200.aggregation_zeropad(xo, wo, e["k"], 1, e["pad"], 1)
     dx, dw = torch.autograd.grad(y, (xo, wo), dy)
@@ -47,7 +50,7 @@ def test_agg_matches_reference_kernels(tag, dtype):
     _close(y, y_ref, tol, "forward")
     _close(dx, dx_ref, tol, "dX")
     _close(dw, dw_ref, tol, "dW")
-    assert y.shape == y_ref.shape and y.dtype == y_ref.dtype and y.is_contiguous()
+    assert y.shape == (e["N"], e["heads"] * e["C"], e["Ho"], e["Wo"]) and y.dtype == x.dtype and y.is_contiguous()
 
 
 @pytest.mark.parametrize("tag", ["s1_b8", "s2_b256", "s4_b256", "cfg1"])
@@ -57,8 +60,8 @@ def test_agg_bf16_channels_last_vs_reference_kernels(tag):
     import cotnet_b200
     e, x, w, dy = rk().make_inputs(tag, "float", seed=3)
     x, w, dy = [t.to(torch.bfloat16).float() for t in (x, w, dy)]
-    y_ref = rk().agg_forward(tag, x, w)
-    dx_ref, dw_ref = rk().agg_backward(tag, dy, x, w)
+    _close(x, rk().ref("agg_bf16", tag, "float", 3, "x"), 0, "inputs")
+    y_ref, dx_ref, dw_ref = [rk().ref("agg_bf16", tag, "float", 3, n) for n in ("y", "dx", "dw")]
     xo = x.to(torch.bfloat16).contiguous(memory_format=torch.channels_last).requires_grad_(True)
     wo = w.to(torch.bfloat16).permute(0, 4, 5, 1, 2, 3).contiguous().permute(0, 3, 4, 5, 1, 2).requires_grad_(True)
     y = cotnet_b200.aggregation_zeropad(xo, wo, 3, 1, 1, 1)
@@ -66,7 +69,7 @@ def test_agg_bf16_channels_last_vs_reference_kernels(tag):
     _close(y, y_ref, 1e-2, "forward")
     _close(dx, dx_ref, 1e-2, "dX")
     # dW sums 8 products of O(1) values: judge relative to the typical magnitude like the other bf16 tests
-    err = (dw.double() - dw_ref.double()).abs()
+    err = (sampled(dw) - dw_ref).abs()
     assert bool((err <= 2e-2 + 1e-2 * dw_ref.double().abs()).all()), "dW: max err %.3e" % err.max().item()
 
 
@@ -74,8 +77,8 @@ def test_agg_bf16_channels_last_vs_reference_kernels(tag):
 def test_mix_matches_reference_kernels(tag, dtype):
     import cotnet_b200
     e, x, w1, w2, dy = rk().make_inputs(tag, dtype, op="mix")
-    y_ref = rk().mix_forward(tag, x, w1, w2)
-    dx_ref, dw1_ref, dw2_ref = rk().mix_backward(tag, dy, x, w1, w2)
+    _close(x, rk().ref("mix", tag, dtype, 0, "x"), 0, "inputs")
+    y_ref, dx_ref, dw1_ref, dw2_ref = [rk().ref("mix", tag, dtype, 0, n) for n in ("y", "dx", "dw1", "dw2")]
     xo, w1o, w2o = [t.clone().requires_grad_(True) for t in (x, w1, w2)]
     y = cotnet_b200.aggregation_zeropad_mix(xo, w1o, w2o, 3, 5, 1, 1, 2, 1)
     dx, dw1, dw2 = torch.autograd.grad(y, (xo, w1o, w2o), dy)
@@ -92,10 +95,10 @@ def test_mix_matches_reference_kernels(tag, dtype):
 def test_cpu_oracle_matches_reference_kernels(tag, dtype):
     """Pins oracle/agg_ref.py (the CPU restatement every other parity test trusts) to the reference's real kernels."""
     e, x, w, dy = rk().make_inputs(tag, dtype, seed=5)
-    y_ref = rk().agg_forward(tag, x, w)
-    dx_ref, dw_ref = rk().agg_backward(tag, dy, x, w)
+    _close(x, rk().ref("agg", tag, dtype, 5, "x"), 0, "inputs")
+    y_ref, dx_ref, dw_ref = [rk().ref("agg", tag, dtype, 5, n) for n in ("y", "dx", "dw")]
     xc, wc = x.cpu().requires_grad_(True), w.cpu().requires_grad_(True)
     yo = agg_ref.agg_zeropad_unfold(xc, wc, e["k"], 1, e["pad"], 1)
     dxo, dwo = torch.autograd.grad(yo, (xc, wc), dy.cpu())
     for a, b, n in ((yo, y_ref, "forward"), (dxo, dx_ref, "dX"), (dwo, dw_ref, "dW")):
-        _close(a, b.cpu(), 1e-9, "oracle " + n)
+        _close(a, b, 1e-9, "oracle " + n)

@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05/TMA GEMM and implicit-GEMM 3x3 conv against fp32 torch math on the same
+"""GPU tests of the wgmma/TMA GEMM and implicit-GEMM 3x3 conv against fp32 torch math on the same
 bf16-representable operands (tolerance: bf16 output rounding, atol=rtol=1e-2)."""
 import pytest
 import torch
@@ -88,7 +88,7 @@ def test_conv3x3(C, groups, H, B):
 @pytest.mark.parametrize("M,N,K1,K2", [(3136, 64, 256, 0), (3136, 256, 64, 0), (1000, 32, 64, 64), (12544, 72, 32, 0), (200, 128, 128, 0),
                                        (6272, 512, 2048, 0), (6272, 2048, 512, 0), (4096, 64, 64, 64), (70, 16, 24, 0), (3136, 48, 96, 96)])
 def test_wgrad(M, N, K1, K2):
-    """dW = dY^T [A1 | A2] on the MN-major tcgen05 kernel (TMA tiles consumed as they land) vs fp32 matmul."""
+    """dW = dY^T [A1 | A2] on the MN-major wgmma kernel (TMA tiles consumed as they land) vs fp32 matmul."""
     tc = _tc()
     g = torch.Generator(device="cuda").manual_seed(M + N)
     dy = torch.randn(M, N, generator=g, device="cuda").bfloat16()
@@ -159,7 +159,7 @@ def _rel_l2(a, b, tol=3e-2):
 @pytest.mark.parametrize("training", [False, True])
 @pytest.mark.parametrize("two", [False, True])
 def test_tc_conv1x1_fn_autograd(training, two):
-    """TcConv1x1Fn (tcgen05 forward + data gradient, BN statistics from the epilogue) vs eager conv+BN+ReLU in fp32."""
+    """TcConv1x1Fn (wgmma forward + data gradient, BN statistics from the epilogue) vs eager conv+BN+ReLU in fp32."""
     import copy
     import torch.nn as nn
     from cotnet_b200 import fused
@@ -250,7 +250,7 @@ def test_tc_conv3x3_fn_autograd(training):
 
 @pytest.mark.parametrize("B,H,W,N", [(2, 224, 224, 64), (3, 64, 96, 64), (1, 32, 480, 32)])
 def test_stem7x7s2_vs_conv2d(B, H, W, N):
-    """conv1 of the trunk (models/resnet.py:552) on the 4-tap tcgen05 implicit GEMM against fp32 torch math on the same bf16 operands;
+    """conv1 of the trunk (models/resnet.py:552) on the 4-tap wgmma implicit GEMM against fp32 torch math on the same bf16 operands;
     raw output + BatchNorm column statistics, and the eval epilogue (folded scale / shift + ReLU)."""
     g = torch.Generator(device="cuda").manual_seed(B + H + W)
     x = torch.randn(B, 3, H, W, generator=g, device="cuda").bfloat16().contiguous(memory_format=torch.channels_last)
@@ -272,7 +272,7 @@ def test_stem7x7s2_vs_conv2d(B, H, W, N):
 
 
 def test_stem_conv_bn_autograd_vs_cudnn_path():
-    """fused.stem_conv_bn (tcgen05 stem + statistics epilogue + fused BatchNorm) against the cuDNN convolution + the same fused
+    """fused.stem_conv_bn (wgmma stem + statistics epilogue + fused BatchNorm) against the cuDNN convolution + the same fused
     BatchNorm kernels: outputs, BatchNorm buffers and parameter gradients."""
     import copy
     from cotnet_b200 import fused
@@ -301,7 +301,7 @@ def test_stem_conv_bn_autograd_vs_cudnn_path():
 
 @pytest.mark.parametrize("B,H,W,N", [(2, 224, 224, 64), (3, 64, 96, 64), (5, 32, 160, 32)])
 def test_stem7x7s2_wgrad_vs_conv2d_weight(B, H, W, N):
-    """Weight gradient of the stem convolution on the MN-major tcgen05 kernel (one stage = one output row over the space-to-depth
+    """Weight gradient of the stem convolution on the MN-major wgmma kernel (one stage = one output row over the space-to-depth
     image) against fp32 torch math on the same bf16 operands."""
     g = torch.Generator(device="cuda").manual_seed(B + H)
     x = torch.randn(B, 3, H, W, generator=g, device="cuda").bfloat16().contiguous(memory_format=torch.channels_last)

@@ -1,15 +1,15 @@
 """The remaining cupy_layers variants (SURVEY.md section 8f rank 4) -- aggregation_refpad, aggregation_zeropad_dilate,
-aggregation_zeropad_mix_merge -- against (a) the REFERENCE'S OWN kernels compiled to cubins (oracle/_ref, incl. the
-reference's host-side border fold for the refpad input gradient) and (b) the CPU oracle's Unfold identities, which are the
+aggregation_zeropad_mix_merge -- against (a) the REFERENCE'S OWN kernels (incl. the reference's host-side border fold for the
+refpad input gradient), as their outputs stored at seeded positions in tests/golden/ref_kernels.npz (oracle/ref_golden.py), and (b) the CPU oracle's Unfold identities, which are the
 right-hand sides of the reference's self-tests (aggregation_refpad.py:223-251, aggregation_zeropad_dilate.py:258-306,
 aggregation_zeropad_mix_merge.py:332-366).  Gates: fp64 1e-9 (the reference's own), fp32 1e-3, bf16 1e-2."""
 import pytest
 import torch
 
-from oracle import agg_ref, ref_kernels
+from oracle import agg_ref, ref_golden
+from oracle.ref_golden import sampled
 
 pytestmark = pytest.mark.gpu
-needs_ref = pytest.mark.skipif(not ref_kernels.available(), reason="oracle/_ref not built")
 
 TOL = {"double": 1e-9, "float": 1e-3}
 _RK = {}
@@ -17,7 +17,7 @@ _RK = {}
 
 def rk():
     if "k" not in _RK:
-        _RK["k"] = ref_kernels.RefKernels()
+        _RK["k"] = ref_golden.GoldenRef()
     return _RK["k"]
 
 
@@ -26,53 +26,50 @@ def _close(a, b, tol, what):
     assert bool((err <= tol + tol * b.double().abs()).all()), "%s: max err %.3e" % (what, err.max().item())
 
 
-@needs_ref
 @pytest.mark.parametrize("tag,dtype", [("refpad_selftest", "double"), ("refpad_selftest", "float"), ("refpad_k3", "double"),
                                        ("refpad_k3", "float"), ("refpad_s2_b8", "float")])
 def test_refpad_matches_reference_kernels(tag, dtype):
     import cotnet_b200
     e, x, w, dy = rk().make_variant_inputs(tag, dtype, "refpad")
-    y_ref = rk().refpad_forward(tag, x, w)
-    dx_ref, dw_ref = rk().refpad_backward(tag, dy, x, w)
+    _close(sampled(x), rk().ref("refpad", tag, dtype, 0, "x"), 0, "inputs")
+    y_ref, dx_ref, dw_ref = [rk().ref("refpad", tag, dtype, 0, n) for n in ("y", "dx", "dw")]
     xo, wo = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
     y = cotnet_b200.aggregation_refpad(xo, wo, e["k"], 1, e["pad"], 1)
     dx, dw = torch.autograd.grad(y, (xo, wo), dy)
     tol = TOL[dtype]
-    _close(y, y_ref, tol, "forward")
-    _close(dx, dx_ref, tol, "dX")
-    _close(dw, dw_ref, tol, "dW")
+    _close(sampled(y), y_ref, tol, "forward")
+    _close(sampled(dx), dx_ref, tol, "dX")
+    _close(sampled(dw), dw_ref, tol, "dW")
 
 
-@needs_ref
 @pytest.mark.parametrize("tag,dtype", [("dilate_selftest", "double"), ("dilate_selftest", "float"), ("dilate_s2_b8", "float")])
 def test_dilate_matches_reference_kernels(tag, dtype):
     import cotnet_b200
     e, x, w, dil, dy = rk().make_variant_inputs(tag, dtype, "dilate")
-    y_ref = rk().dilate_forward(tag, x, w, dil)
-    dx_ref, dw_ref = rk().dilate_backward(tag, dy, x, w, dil)
+    _close(sampled(x), rk().ref("dilate", tag, dtype, 0, "x"), 0, "inputs")
+    y_ref, dx_ref, dw_ref = [rk().ref("dilate", tag, dtype, 0, n) for n in ("y", "dx", "dw")]
     xo, wo = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
     y = cotnet_b200.aggregation_zeropad_dilate(xo, wo, dil, 3, 1)
     dx, dw = torch.autograd.grad(y, (xo, wo), dy)
     tol = TOL[dtype]
-    _close(y, y_ref, tol, "forward")
-    _close(dx, dx_ref, tol, "dX")
-    _close(dw, dw_ref, tol, "dW")
+    _close(sampled(y), y_ref, tol, "forward")
+    _close(sampled(dx), dx_ref, tol, "dX")
+    _close(sampled(dw), dw_ref, tol, "dW")
 
 
-@needs_ref
 @pytest.mark.parametrize("tag,dtype", [("merge_selftest", "double"), ("merge_selftest", "float"), ("merge_s1_b8", "float")])
 def test_mix_merge_matches_reference_kernels(tag, dtype):
     import cotnet_b200
     e, x, w, dy = rk().make_variant_inputs(tag, dtype, "merge")
-    y_ref = rk().merge_forward(tag, x, w)
-    dx_ref, dw_ref = rk().merge_backward(tag, dy, x, w)
+    _close(sampled(x), rk().ref("merge", tag, dtype, 0, "x"), 0, "inputs")
+    y_ref, dx_ref, dw_ref = [rk().ref("merge", tag, dtype, 0, n) for n in ("y", "dx", "dw")]
     xo, wo = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
     y = cotnet_b200.aggregation_zeropad_mix_merge(xo, wo, e["heads"], e["wc"], 3, 5, 1, 1, 2, 1)
     dx, dw = torch.autograd.grad(y, (xo, wo), dy)
     tol = TOL[dtype]
-    _close(y, y_ref, tol, "forward")
-    _close(dx, dx_ref, tol, "dX")
-    _close(dw, dw_ref, tol, "dW")
+    _close(sampled(y), y_ref, tol, "forward")
+    _close(sampled(dx), dx_ref, tol, "dX")
+    _close(sampled(dw), dw_ref, tol, "dW")
 
 
 # ---------------------------------------------------------------- vs the CPU oracle (runs also where oracle/_ref is absent)

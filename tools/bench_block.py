@@ -8,7 +8,7 @@ Arms (same module weights, same inputs, CUDA-event timing, >= 3 warm-ups, inputs
              with only the LocalConv op on our kernel -- what "drop in the op only" gives; stands in for the GPU
              reference block (the CuPy op itself cannot run here: SURVEY.md D5)
   fused      this repo, cuDNN convolutions + fused BatchNorm / GroupNorm / tail kernels (training-capable path)
-  tc         this repo, eval mode: every convolution on the tcgen05 kernels, BatchNorms folded (no cuDNN/cuBLAS)
+  tc         this repo, eval mode: every convolution on the wgmma kernels, BatchNorms folded (no cuDNN/cuBLAS)
 Roofline (SURVEY 8d): max(FLOPs / bf16 peak, 2*C*px*2 bytes / HBM peak) for the fully fused block."""
 import argparse
 import json

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """conv1x1 -> BatchNorm(batch stats) -> ReLU, forward + backward, at every 1x1-conv shape of the CoTNet-50 bs256 step:
-cuDNN conv + fused BN kernels (the default training backend) against the tcgen05 GEMM with the statistics epilogue
+cuDNN conv + fused BN kernels (the default training backend) against the wgmma GEMM with the statistics epilogue
 (TcConv1x1Fn).  Decides which convolutions the 'tc' training backend should take."""
 import argparse
 import json

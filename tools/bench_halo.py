@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """3x3 grouped key convolution (key_embed.0, models/cotnet.py:44) per CoTNet-50 stage shape, bs256, bf16 NHWC: the haloed-tile
-tcgen05 kernel (variants through COTB200_CONV_HALO / COTB200_HALO_MAXPX, one subprocess each) against the per-tap conv mode and
+wgmma kernel (variants through COTB200_CONV_HALO / COTB200_HALO_MAXPX, one subprocess each) against the per-tap conv mode and
 cuDNN's grouped convolution.  CUDA events, inputs rotated through > 126 MB."""
 import json
 import os

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """GPU REFERENCE ARM: the UNMODIFIED reference model (its eager module graph, its own NVRTC-style kernels for the LocalConv
-op) timed on the same box as bench.py -- BASELINE.md section 4 rows 2-3, the honest "x over the reference on a B200".
+op) timed on the same box as bench.py -- BASELINE.md section 4 rows 2-3, the honest "x over the reference on a H100".
 
     python tools/make_ref_snapshot.py                      # in the build container: baseline/_ref/ (git-ignored) <- reference packages
     python tools/bench_reference_gpu.py --model cotnet50 --batch 256 --amp bf16 [--steps 10] [--json out.json]

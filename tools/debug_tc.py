@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Debug helper: per-gradient errors of the tcgen05-backed autograd functions vs eager fp32."""
+"""Debug helper: per-gradient errors of the wgmma-backed autograd functions vs eager fp32."""
 import copy
 import os
 import sys

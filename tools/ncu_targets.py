@@ -4,7 +4,7 @@
     ncu --set full --clock-control none --import-source on --profile-from-start off -o gpurun_out/targets \
         python tools/ncu_targets.py [--what eval,gemm,train]
 
-  eval  : one eval-mode CotLayer forward (tcgen05 path, 8 launches) at the stage-1 and stage-3 shapes of CoTNet-50 bs256
+  eval  : one eval-mode CotLayer forward (wgmma path, 8 launches) at the stage-1 and stage-3 shapes of CoTNet-50 bs256
   gemm  : the 1x1-convolution GEMMs of the training step with the BatchNorm-statistics epilogue, and their data-gradient GEMMs
   train : one training-mode CotLayer forward + backward at the stage-1 shape (LocalConv dX / dW, GroupNorm, tail kernels)
 """

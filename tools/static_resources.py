@@ -22,10 +22,10 @@ def main():
     out = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "profiles", "r01_static_resources.md")
     rows = []
     for src in sorted(glob.glob(os.path.join(CSRC, "*.cu"))):
-        p = subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-I" + os.path.join(ROOT, "include"),
+        p = subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-I" + os.path.join(ROOT, "include"),
                             "-Xptxas", "-v", "-c", "-o", "/dev/null", src], capture_output=True, text=True)
         text = p.stderr
-        for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_100a'\n[^\n]*\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, "
+        for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_90a'\n[^\n]*\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, "
                              r"(\d+) bytes spill loads\n[^\n]*Used (\d+) registers(?:, used (\d+) barriers)?(?:, (\d+) bytes smem)?", text):
             rows.append((os.path.basename(src), m.group(1), int(m.group(5)), int(m.group(3)) + int(m.group(4)), int(m.group(7) or 0)))
     names = demangle([r[1] for r in rows])
@@ -43,7 +43,7 @@ def main():
                 continue
         keep.append((src, short.replace("(int)", "").replace("(bool)", ""), regs, spill, smem))
     with open(out, "w") as f:
-        f.write("# static resources of the libcotb200 kernels (`ptxas -v`, sm_100a; bf16 / fp32 instantiations)\n\n")
+        f.write("# static resources of the libcotb200 kernels (`ptxas -v`, sm_90a; bf16 / fp32 instantiations)\n\n")
         f.write("65 536 registers and 227 KB of shared memory per SM: `regs x threads` bounds the resident CTAs of the register-heavy\n"
                 "kernels (LocalConv gen 2, fused NCHW backward), dynamic shared memory those of the TMA / bulk-copy pipelines.\n\n")
         f.write("| source | kernel | registers | spill bytes | static smem |\n|---|---|---|---|---|\n")
