@@ -27,6 +27,12 @@ class AggDesc(ctypes.Structure):
             "x_sn", "x_sp", "w_sn", "w_sp", "y_sn", "y_sp")]
 
 
+class Mix(ctypes.Structure):
+    """struct cotb200_mix (include/cotb200.h): one step's batch Mixup / CutMix parameters."""
+    _fields_ = [("mode", ctypes.c_int), ("lam", ctypes.c_float), ("one_minus_lam", ctypes.c_float), ("target_lam", ctypes.c_float),
+                ("y0", ctypes.c_int), ("y1", ctypes.c_int), ("x0", ctypes.c_int), ("x1", ctypes.c_int)]
+
+
 _lock = threading.Lock()
 _lib = None
 
@@ -62,6 +68,10 @@ SYMBOLS = {
     "cotb200_bn_bwd_apply": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 9 + [ctypes.c_float, ctypes.c_int, _VP, _VP, _VP]),
     "cotb200_bn_bwd_sums2": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_int, _VP, _VP, _VP]),
     "cotb200_bn_bwd_apply2": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 10 + [ctypes.c_float, ctypes.c_int, _VP, _VP, _VP]),
+    "cotb200_bn_apply_ds": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 4 + [ctypes.c_int, _VP, _VP, _VP]),
+    "cotb200_bn_apply_batch_ds": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_float] * 3 + [ctypes.c_int] * 2 + [_VP] * 7),
+    "cotb200_bn_bwd_sums_ds": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_int, _VP, _VP, _VP, _VP]),
+    "cotb200_bn_bwd_apply_ds": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 10 + [ctypes.c_float, ctypes.c_int, _VP, _VP, _VP, _VP]),
     "cotb200_bn_finalize": (ctypes.c_int, [ctypes.c_int] + [_VP] * 6 + [ctypes.c_float] * 3 + [ctypes.c_int] * 2 + [_VP] * 5),
     "cotb200_gn9_stats": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP] * 5),
     "cotb200_gn9_apply": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP] * 8),
@@ -96,6 +106,11 @@ SYMBOLS = {
     "cotb200_multi_lerp": (ctypes.c_int, [_VP, ctypes.c_int, _VP, _VP]),
     "cotb200_u8_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
                                           _VP, _VP, _VP]),
+    "cotb200_u8_mix_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
+                                              _VP, _VP, _VP, _VP]),
+    "cotb200_soft_ce": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP, _VP]),
+    "cotb200_soft_ce_bwd": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP, _VP,
+                                                                 ctypes.c_longlong, _VP]),
 }
 
 

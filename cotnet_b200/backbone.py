@@ -48,10 +48,12 @@ class Bottleneck(nn.Module):
     #: below the roof, more than the add saves.  Always False on the network's last block.
     fork_output = os.environ.get("COTB200_FORK", "0") != "0"
 
-    def forward(self, x):
+    def forward(self, x, drop_scale=None):
+        """drop_scale: None or [B] per-sample stochastic-depth scales applied to bn3's output before the residual add
+        (models/cotnet.py:256-257); the trunk draws them (StochasticDepth)."""
         xs = x if isinstance(x, tuple) else (x, x)
         if fused.supported(xs[0]):
-            return self._forward_fused(xs)
+            return self._forward_fused(xs, drop_scale)
         x = xs[0]
         residual = x
         x = self.act1(self.bn1(self.conv1(x)))
@@ -59,12 +61,14 @@ class Bottleneck(nn.Module):
             x = self.avd(x)
         x = self.conv2(x)
         x = self.bn3(self.conv3(x))
+        if drop_scale is not None:
+            x = x * drop_scale.to(x.dtype).view(-1, 1, 1, 1)
         if self.downsample is not None:
             residual = self.downsample(residual)
         x += residual
         return self.act3(x)
 
-    def _forward_fused(self, xs):
+    def _forward_fused(self, xs, drop_scale=None):
         """channels_last path: bn1+ReLU and bn3+residual+ReLU (SURVEY section 8f rank 1) run on the fused BatchNorm
         kernels (2 passes each way) instead of ATen's channels_last batch-norm kernels."""
         cl = torch.channels_last
@@ -77,11 +81,72 @@ class Bottleneck(nn.Module):
             residual = fused.conv1x1_bn(residual, self.downsample[0], self.downsample[1], relu=False)
         fork = self.fork_output and torch.is_grad_enabled() and self.training
         return fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=True,
-                                res=residual.contiguous(memory_format=cl), fork=fork)
+                                res=residual.contiguous(memory_format=cl), fork=fork, drop_scale=drop_scale)
 
 
-class CoTResNet(nn.Module):
-    def __init__(self, layers, num_classes=1000, in_chans=3, cardinality=1, base_width=64, zero_init_last_bn=True):
+class StochasticDepth:
+    """Stochastic depth and classifier dropout of the reference trunks (``drop_path_rate`` / ``drop_rate`` of create_model;
+    models/resnet.py:409-440,608-609, models/cotnet_hybrid.py:275,442-443), shared by CoTResNet and CoTHybridNet.
+
+    Block i of the n bottlenecks drops its residual branch with probability ``drop_path_rate * i / (n - 1)``.  In training the
+    trunk draws every block's per-sample scales with ONE ``torch.rand(n, B)`` (fp32) per forward, s = floor(keep + u) / keep,
+    so a captured CUDA graph draws new masks at every replay (torch's Philox offsets); the scales reach the fused BatchNorm
+    kernels of bn3 (``fused.conv1x1_bn(drop_scale=)``).  No parameter or buffer is added: state dicts do not change.
+
+    While stochastic depth is active (training mode, drop_path_rate > 0) the trunk calls the bottlenecks one by one to hand each
+    its scales, so the ``layer1`` .. ``layer4`` Sequential containers are not called: hooks registered on those four modules do
+    not fire then (hooks on the blocks and everything inside them do).  In eval mode, or with drop_path_rate 0, the stages run
+    as before."""
+
+    #: test hook: a [n_blocks, B] tensor of per-sample scales used instead of the random draw (training mode only)
+    fixed_drop_path_scales = None
+
+    def _init_regularisers(self, drop_rate, drop_path_rate):
+        self.drop_rate = float(drop_rate)
+        self.drop_path_rate = float(drop_path_rate)
+        blocks = self.blocks()
+        n = len(blocks)
+        for i, blk in enumerate(blocks):
+            blk.drop_path_rate = self.drop_path_rate * i / (n - 1)
+        self._dp_keep = {}
+
+    def blocks(self):
+        return [b for name in ("layer1", "layer2", "layer3", "layer4") for b in getattr(self, name)]
+
+    def drop_path_rates(self):
+        return [b.drop_path_rate for b in self.blocks()]
+
+    def _drop_path_scales(self, x):
+        if not (self.training and self.drop_path_rate > 0.):
+            return None
+        B = x.shape[0]
+        if self.fixed_drop_path_scales is not None:
+            s = self.fixed_drop_path_scales.to(device=x.device, dtype=torch.float32)
+            assert s.shape == (len(self.blocks()), B), "fixed_drop_path_scales must be [n_blocks, B]"
+            return s.contiguous()
+        keep = self._dp_keep.get(x.device)
+        if keep is None:
+            keep = torch.tensor([1. - r for r in self.drop_path_rates()], dtype=torch.float32, device=x.device).view(-1, 1)
+            self._dp_keep[x.device] = keep
+        return torch.floor(keep + torch.rand(keep.shape[0], B, dtype=torch.float32, device=x.device)) / keep
+
+    def _run_blocks(self, x):
+        s = self._drop_path_scales(x)
+        if s is None:
+            return self.layer4(self.layer3(self.layer2(self.layer1(x))))
+        for i, blk in enumerate(self.blocks()):
+            x = blk(x, drop_scale=s[i] if blk.drop_path_rate > 0. else None)
+        return x
+
+    def _classifier(self, x):
+        if self.drop_rate:
+            x = F.dropout(x, p=self.drop_rate, training=self.training)
+        return self.fc(x)
+
+
+class CoTResNet(StochasticDepth, nn.Module):
+    def __init__(self, layers, num_classes=1000, in_chans=3, cardinality=1, base_width=64, zero_init_last_bn=True,
+                 drop_rate=0., drop_path_rate=0.):
         super().__init__()
         self.num_classes = num_classes
         inplanes = 64
@@ -106,6 +171,7 @@ class CoTResNet(nn.Module):
         self.num_features = inplanes
         self.global_pool = nn.AdaptiveAvgPool2d(1)
         self.fc = nn.Linear(self.num_features, num_classes)
+        self._init_regularisers(drop_rate, drop_path_rate)
         # models/resnet.py:575-584
         for m in self.modules():
             if isinstance(m, nn.Conv2d):
@@ -143,11 +209,11 @@ class CoTResNet(nn.Module):
                 x = fused.max_pool3x3s2(fused.bn_act(self._stem_conv(x).contiguous(memory_format=torch.channels_last), self.bn1, relu=True))
         else:
             x = self.maxpool(self.act1(self.bn1(self.conv1(x))))
-        return self.layer4(self.layer3(self.layer2(self.layer1(x))))
+        return self._run_blocks(x)
 
     def forward(self, x):
         x = self.global_pool(self.forward_features(x)).flatten(1)
-        return self.fc(x)
+        return self._classifier(x)
 
     def cot_layers(self):
         return [m for m in self.modules() if isinstance(m, (CotLayer, CoXtLayer))]

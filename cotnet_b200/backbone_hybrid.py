@@ -23,6 +23,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import fused
+from .backbone import StochasticDepth
 from .cot_layer import CoTLayer
 
 
@@ -82,7 +83,7 @@ class SplitAttnConv2d(nn.Module):
 
 
 class CoTBottleneck(nn.Module):
-    """models/cotnet_hybrid.py:118-204 (cardinality 1, base_width 64, no drop block / drop path)."""
+    """models/cotnet_hybrid.py:118-204 (cardinality 1, base_width 64, no drop block; drop path through forward's drop_scale)."""
     expansion = 4
 
     def __init__(self, block_idx, inplanes, planes, stride=1, downsample=None, aa_layer=None, radix=1, avd=False,
@@ -125,7 +126,7 @@ class CoTBottleneck(nn.Module):
 
     fork_output = os.environ.get("COTB200_FORK", "0") != "0"             # see backbone.Bottleneck.fork_output
 
-    def forward(self, x):
+    def forward(self, x, drop_scale=None):
         cl = torch.channels_last
         xs = x if isinstance(x, tuple) else (x, x)
         x, xres = xs
@@ -142,7 +143,7 @@ class CoTBottleneck(nn.Module):
                 residual = fused.conv1x1_bn(d[0](xres).contiguous(memory_format=cl), d[1], d[2], relu=False)
             fork = self.fork_output and torch.is_grad_enabled() and self.training
             return fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=True,
-                                    res=residual.contiguous(memory_format=cl), fork=fork)
+                                    res=residual.contiguous(memory_format=cl), fork=fork, drop_scale=drop_scale)
         residual = x
         y = self.act1(self.bn1(self.conv1(x)))
         if self.avd is not None and self.avd_first:
@@ -151,6 +152,8 @@ class CoTBottleneck(nn.Module):
         if self.avd is not None and not self.avd_first:
             y = self.avd(y)
         y = self.bn3(self.conv3(y))
+        if drop_scale is not None:                                                   # :194-195
+            y = y * drop_scale.to(y.dtype).view(-1, 1, 1, 1)
         if self.downsample is not None:
             residual = self.downsample(residual)
         y = y + residual
@@ -163,11 +166,11 @@ def _downsample_avg(in_channels, out_channels, stride):
     return nn.Sequential(pool, nn.Conv2d(in_channels, out_channels, 1, stride=1, padding=0, bias=False), nn.BatchNorm2d(out_channels))
 
 
-class CoTHybridNet(nn.Module):
+class CoTHybridNet(StochasticDepth, nn.Module):
     """models/cotnet_hybrid.py:338-452 for stem_type='deep', avg_down=True, output_stride=32."""
 
     def __init__(self, layers, num_classes=1000, in_chans=3, stem_width=64, aa_layer=None, zero_init_last_bn=True,
-                 block_args=None):
+                 block_args=None, drop_rate=0., drop_path_rate=0.):
         super().__init__()
         block_args = dict(block_args or {})
         inplanes = stem_width * 2
@@ -189,6 +192,7 @@ class CoTHybridNet(nn.Module):
         self.num_features = 2048
         self.global_pool = nn.AdaptiveAvgPool2d(1)
         self.fc = nn.Linear(self.num_features, num_classes)
+        self._init_regularisers(drop_rate, drop_path_rate)
         for m in self.modules():                                                     # :415-424
             if isinstance(m, nn.Conv2d):
                 nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
@@ -209,10 +213,10 @@ class CoTHybridNet(nn.Module):
             x = fused.bn_act(c[6](x).contiguous(memory_format=cl), self.bn1, relu=True)
         else:
             x = self.act1(self.bn1(self.conv1(x)))
-        return self.layer4(self.layer3(self.layer2(self.layer1(x))))
+        return self._run_blocks(x)
 
     def forward(self, x):
-        return self.fc(self.global_pool(self.forward_features(x)).flatten(1))
+        return self._classifier(self.global_pool(self.forward_features(x)).flatten(1))
 
     def cot_layers(self):
         return [m for m in self.modules() if isinstance(m, CoTLayer)]

@@ -292,10 +292,12 @@ struct BnFin {
   float* scale; float* shift; float* mean; float* rstd;
 };
 
-template <typename T, int VEC, int ACT, bool RES, bool FIN>
+// DS (stochastic depth, models/cotnet.py:256-257): y = act(ds[b]*(x*scale + shift) (+ res)), ds [B] per-sample scales in
+// {0, 1/keep}; the kernels see the flattened rows, so the sample of row r is r / ds_hw.  DS == false compiles to the plain form.
+template <typename T, int VEC, int ACT, bool RES, bool FIN, bool DS = false>
 __global__ void __launch_bounds__(NT_THREADS)
 bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float* __restrict__ scale,
-                const float* __restrict__ shift, T* __restrict__ y, RowsGeo g, BnFin f) {
+                const float* __restrict__ shift, T* __restrict__ y, RowsGeo g, BnFin f, const float* __restrict__ ds, int ds_hw) {
   const int tx = threadIdx.x % g.cq_pad, ty = threadIdx.x / g.cq_pad;
   if (!(tx < g.cq && ty < g.ry)) return;
   const int b = blockIdx.y, r0 = blockIdx.x * g.rows_per_cta, r1 = min(g.HW, r0 + g.rows_per_cta);
@@ -326,9 +328,12 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
     Pack<T, VEC> rv;
     if (RES) rv = ld_pack<T, VEC>(res + base + (long long)r * g.ld);
     Pack<T, VEC> o;
+    float s = 1.f;
+    if (DS) s = __ldg(ds + r / ds_hw);
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
       float z = fmaf(to_acc(xv.v[i]), sc[i], sh[i]);
+      if (DS) z *= s;
       if (RES) z += to_acc(rv.v[i]);
       if (ACT == 1) z = fmaxf(z, 0.f);
       o.v[i] = Elem<T>::from(z);
@@ -338,12 +343,12 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
 }
 
 // dz = dy * [y > 0] (ACT==1: mask read from y ; ACT==2: mask recomputed as x*scale+shift > 0, one HBM pass less) ;
-// sum_dz[c] += dz ; sum_dzx[c] += dz * xhat
-template <typename T, int VEC, int ACT>
+// sum_dz[c] += dz ; sum_dzx[c] += dz * xhat.   DS: the BatchNorm output was scaled by ds[b], so its gradient is ds[b]*dz.
+template <typename T, int VEC, int ACT, bool DS = false>
 __global__ void __launch_bounds__(NT_THREADS)
 bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T* __restrict__ x, const T* __restrict__ y, const float* __restrict__ scale,
                    const float* __restrict__ shift, const float* __restrict__ mu, const float* __restrict__ rstd,
-                   float* __restrict__ sum_dz, float* __restrict__ sum_dzx, RowsGeo g) {
+                   float* __restrict__ sum_dz, float* __restrict__ sum_dzx, RowsGeo g, const float* __restrict__ ds, int ds_hw) {
   extern __shared__ float sm[];
   const int tx = threadIdx.x % g.cq_pad, ty = threadIdx.x / g.cq_pad;
   const bool active = tx < g.cq && ty < g.ry;
@@ -362,13 +367,16 @@ bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T*
       Pack<T, VEC> yv, d2;
       if (ACT == 1) yv = ld_pack<T, VEC>(y + base + (long long)r * g.ld);
       if (dy2) d2 = ld_pack<T, VEC>(dy2 + base + (long long)r * g.ld);    // two-consumer output: dy = dy + dy2, summed here in fp32
+      float s = 1.f;
+      if (DS) s = __ldg(ds + r / ds_hw);
 #pragma unroll
       for (int i = 0; i < VEC; ++i) {
         float dz = to_acc(dv.v[i]);
         if (dy2) dz += to_acc(d2.v[i]);
         const float xf = to_acc(xv.v[i]);
         if (ACT == 1 && !(to_acc(yv.v[i]) > 0.f)) dz = 0.f;
-        if (ACT == 2 && !(fmaf(xf, sc[i], sh[i]) > 0.f)) dz = 0.f;       // the forward's own fp32 z: identical mask, y not read
+        if (ACT == 2 && !((DS ? fmaf(xf, sc[i], sh[i]) * s : fmaf(xf, sc[i], sh[i])) > 0.f)) dz = 0.f;   // the forward's own fp32 z: identical mask, y not read
+        if (DS) dz *= s;
         acc[0][i] += dz;
         acc[1][i] = fmaf(dz, (xf - m[i]) * rs[i], acc[1][i]);
       }
@@ -379,12 +387,13 @@ bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T*
 }
 
 // dx = scale * (dz - c1 - xhat*c2)   (c1 = c2 = 0 in eval mode);   dres = dz when RES
-template <typename T, int VEC, int ACT, bool RES>
+// DS: dx = scale * (ds[b]*dz - c1 - xhat*c2), dres = dz
+template <typename T, int VEC, int ACT, bool RES, bool DS = false>
 __global__ void __launch_bounds__(NT_THREADS)
 bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T* __restrict__ x, const T* __restrict__ y, const float* __restrict__ scale,
                     const float* __restrict__ shift, const float* __restrict__ mu, const float* __restrict__ rstd,
                     const float* __restrict__ c1, const float* __restrict__ c2, float inv_n, T* __restrict__ dx,
-                    T* __restrict__ dres, RowsGeo g) {
+                    T* __restrict__ dres, RowsGeo g, const float* __restrict__ ds, int ds_hw) {
   const int tx = threadIdx.x % g.cq_pad, ty = threadIdx.x / g.cq_pad;
   if (!(tx < g.cq && ty < g.ry)) return;
   const int b = blockIdx.y, r0 = blockIdx.x * g.rows_per_cta, r1 = min(g.HW, r0 + g.rows_per_cta);
@@ -403,14 +412,16 @@ bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T
     if (ACT == 1) yv = ld_pack<T, VEC>(y + base + (long long)r * g.ld);
     if (dy2) d2 = ld_pack<T, VEC>(dy2 + base + (long long)r * g.ld);
     Pack<T, VEC> o, o2;
+    float s = 1.f;
+    if (DS) s = __ldg(ds + r / ds_hw);
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
       float dz = to_acc(dv.v[i]);
       if (dy2) dz += to_acc(d2.v[i]);
       const float xf = to_acc(xv.v[i]);
       if (ACT == 1 && !(to_acc(yv.v[i]) > 0.f)) dz = 0.f;
-      if (ACT == 2 && !(fmaf(xf, sc[i], sh[i]) > 0.f)) dz = 0.f;
-      o.v[i] = Elem<T>::from(sc[i] * (dz - k1[i] - (xf - m[i]) * rs[i] * k2[i]));
+      if (ACT == 2 && !((DS ? fmaf(xf, sc[i], sh[i]) * s : fmaf(xf, sc[i], sh[i])) > 0.f)) dz = 0.f;
+      o.v[i] = Elem<T>::from(sc[i] * ((DS ? dz * s : dz) - k1[i] - (xf - m[i]) * rs[i] * k2[i]));
       if (RES) o2.v[i] = Elem<T>::from(dz);
     }
     st_pack<T, VEC>(dx + base + (long long)r * g.ld, o);
@@ -948,10 +959,13 @@ extern "C" int cotb200_gn9_bwd_apply(int dtype, int B, int HW, int wc, int gc, c
   return 0;
 }
 
-#define BN_APPLY_LAUNCH(ACT, RES, FIN) bn_apply_kernel<T, V, ACT, RES, FIN><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f)
+#define BN_APPLY_LAUNCH(ACT, RES, FIN)                                                                                   \
+  do { if (sscale) bn_apply_kernel<T, V, ACT, RES, FIN, true><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f, sscale, ds_hw); \
+       else bn_apply_kernel<T, V, ACT, RES, FIN><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f, nullptr, 1); } while (0)
 static int bn_apply_impl(const char* what, int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
-                         const float* shift, int relu, void* y, const BnFin* fin, void* stream) {
+                         const float* shift, int relu, void* y, const BnFin* fin, const float* sscale, void* stream) {
   if (dtype == COTB200_F64) { set_error("%s: fp64 not supported", what); return COTB200_EDTYPE; }
+  const int ds_hw = HW;           // rows per sample: the sample of flattened row r is r / ds_hw
   { const long long rows = (long long)B * HW; if (rows > 2147483647LL) { set_error("%s: too many rows", what); return COTB200_ETOOBIG; }
     HW = (int)rows; B = 1; }      // per-channel affine: flatten [B, HW] -> rows
   cudaStream_t st = (cudaStream_t)stream;
@@ -995,7 +1009,13 @@ static int bn_apply_impl(const char* what, int dtype, int B, int HW, int C, cons
 extern "C" int cotb200_bn_apply(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
                                 const float* shift, int relu, void* y, void* stream) {
   if (!x || !scale || !shift || !y) { set_error("bn_apply: NULL pointer"); return COTB200_ENULL; }
-  return bn_apply_impl("bn_apply", dtype, B, HW, C, x, res, scale, shift, relu, y, nullptr, stream);
+  return bn_apply_impl("bn_apply", dtype, B, HW, C, x, res, scale, shift, relu, y, nullptr, nullptr, stream);
+}
+
+extern "C" int cotb200_bn_apply_ds(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
+                                   const float* shift, int relu, void* y, const float* sample_scale, void* stream) {
+  if (!x || !scale || !shift || !y) { set_error("bn_apply_ds: NULL pointer"); return COTB200_ENULL; }
+  return bn_apply_impl("bn_apply_ds", dtype, B, HW, C, x, res, scale, shift, relu, y, nullptr, sample_scale, stream);
 }
 
 extern "C" int cotb200_bn_apply_batch(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum,
@@ -1005,16 +1025,32 @@ extern "C" int cotb200_bn_apply_batch(int dtype, int B, int HW, int C, const voi
   if (!x || !y || !sum || !sq || !scale || !shift || !mean || !rstd) { set_error("bn_apply_batch: NULL pointer"); return COTB200_ENULL; }
   if (update_running && (!running_mean || !running_var)) { set_error("bn_apply_batch: running buffers missing"); return COTB200_ENULL; }
   BnFin f{sum, sq, weight, bias, running_mean, running_var, n, eps, momentum, update_running, scale, shift, mean, rstd};
-  return bn_apply_impl("bn_apply_batch", dtype, B, HW, C, x, res, nullptr, nullptr, relu, y, &f, stream);
+  return bn_apply_impl("bn_apply_batch", dtype, B, HW, C, x, res, nullptr, nullptr, relu, y, &f, nullptr, stream);
 }
 
+extern "C" int cotb200_bn_apply_batch_ds(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum,
+                                         const float* sq, const float* weight, const float* bias, float* running_mean,
+                                         float* running_var, float n, float eps, float momentum, int update_running, int relu,
+                                         void* y, float* scale, float* shift, float* mean, float* rstd, const float* sample_scale,
+                                         void* stream) {
+  if (!x || !y || !sum || !sq || !scale || !shift || !mean || !rstd) { set_error("bn_apply_batch_ds: NULL pointer"); return COTB200_ENULL; }
+  if (update_running && (!running_mean || !running_var)) { set_error("bn_apply_batch_ds: running buffers missing"); return COTB200_ENULL; }
+  BnFin f{sum, sq, weight, bias, running_mean, running_var, n, eps, momentum, update_running, scale, shift, mean, rstd};
+  return bn_apply_impl("bn_apply_batch_ds", dtype, B, HW, C, x, res, nullptr, nullptr, relu, y, &f, sample_scale, stream);
+}
+
+#define BN_BWD_SUMS_LAUNCH(ACT, DS, YP)                                                                               \
+  do { if ((rc = ensure_smem(bn_bwd_sums_kernel<T, V, ACT, DS>, smem))) return rc;                                    \
+       bn_bwd_sums_kernel<T, V, ACT, DS><<<NT_GRID, NT_THREADS, smem, st>>>(dp, d2p, xp, YP, scp, shp, mu + c0, rstd + c0,  \
+                                                                             sum_dz + c0, sum_dzx + c0, g, sscale, ds_hw); } while (0)
 static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
                             const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
-                            float* sum_dz, float* sum_dzx, void* stream) {
+                            float* sum_dz, float* sum_dzx, const float* sscale, void* stream) {
   if (!dy || !x || !mu || !rstd || !sum_dz || !sum_dzx || (relu == 1 && !y) || (relu == 2 && (!scale || !shift))) {
     set_error("bn_bwd_sums: NULL pointer"); return COTB200_ENULL; }
   if (relu < 0 || relu > 2) { set_error("bn_bwd_sums: relu must be 0, 1 or 2"); return COTB200_EINVAL; }
   if (dtype == COTB200_F64) { set_error("bn_bwd_sums: fp64 not supported"); return COTB200_EDTYPE; }
+  const int ds_hw = HW;           // rows per sample (drop-path scales)
   { const long long rows = (long long)B * HW; if (rows > 2147483647LL) { set_error("cotb200_bn_bwd_sums: too many rows"); return COTB200_ETOOBIG; }
     HW = (int)rows; B = 1; }      // per-channel statistics: flatten [B, HW] -> rows
   cudaStream_t st = (cudaStream_t)stream;
@@ -1035,12 +1071,11 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
         COTB200_PROF_B("bn_bwd_sums", (double)B * HW * cw * (2 + (relu == 1 ? 1 : 0) + (dy2 ? 1 : 0)) * sizeof(T));
         const float* scp = scale ? scale + c0 : nullptr; const float* shp = shift ? shift + c0 : nullptr;
         NT_DISPATCH_VEC(vec, {
-          if (relu == 1) { if ((rc = ensure_smem(bn_bwd_sums_kernel<T, V, 1>, smem))) return rc;
-                           bn_bwd_sums_kernel<T, V, 1><<<NT_GRID, NT_THREADS, smem, st>>>(dp, d2p, xp, yp, scp, shp, mu + c0, rstd + c0, sum_dz + c0, sum_dzx + c0, g); }
-          else if (relu == 2) { if ((rc = ensure_smem(bn_bwd_sums_kernel<T, V, 2>, smem))) return rc;
-                                bn_bwd_sums_kernel<T, V, 2><<<NT_GRID, NT_THREADS, smem, st>>>(dp, d2p, xp, nullptr, scp, shp, mu + c0, rstd + c0, sum_dz + c0, sum_dzx + c0, g); }
-          else { if ((rc = ensure_smem(bn_bwd_sums_kernel<T, V, 0>, smem))) return rc;
-                 bn_bwd_sums_kernel<T, V, 0><<<NT_GRID, NT_THREADS, smem, st>>>(dp, d2p, xp, nullptr, scp, shp, mu + c0, rstd + c0, sum_dz + c0, sum_dzx + c0, g); }
+          if (sscale) {
+            if (relu == 1) BN_BWD_SUMS_LAUNCH(1, true, yp); else if (relu == 2) BN_BWD_SUMS_LAUNCH(2, true, nullptr); else BN_BWD_SUMS_LAUNCH(0, true, nullptr);
+          } else {
+            if (relu == 1) BN_BWD_SUMS_LAUNCH(1, false, yp); else if (relu == 2) BN_BWD_SUMS_LAUNCH(2, false, nullptr); else BN_BWD_SUMS_LAUNCH(0, false, nullptr);
+          }
         });
         if ((rc = check_launch("bn_bwd_sums"))) return rc;
       }
@@ -1050,14 +1085,20 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
   return 0;
 }
 
-#define BN_BWD_APPLY_LAUNCH(ACT, RES, YP, DRP) bn_bwd_apply_kernel<T, V, ACT, RES><<<NT_GRID, NT_THREADS, 0, st>>>(dp, d2p, xp, YP, scale + c0, shp, mu + c0, rstd + c0, k1, k2, inv_n, dxp, DRP, g)
+#define BN_BWD_APPLY_LAUNCH(ACT, RES, YP, DRP)                                                                         \
+  do { if (sscale) bn_bwd_apply_kernel<T, V, ACT, RES, true><<<NT_GRID, NT_THREADS, 0, st>>>(dp, d2p, xp, YP, scale + c0, shp, mu + c0, \
+                                                               rstd + c0, k1, k2, inv_n, dxp, DRP, g, sscale, ds_hw);      \
+       else bn_bwd_apply_kernel<T, V, ACT, RES><<<NT_GRID, NT_THREADS, 0, st>>>(dp, d2p, xp, YP, scale + c0, shp, mu + c0,  \
+                                                               rstd + c0, k1, k2, inv_n, dxp, DRP, g, nullptr, 1); } while (0)
 static int bn_bwd_apply_impl(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
                              const float* scale, const float* shift, const float* mu, const float* rstd,
-                             const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres, void* stream) {
+                             const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres, const float* sscale,
+                             void* stream) {
   if (!dy || !x || !scale || !mu || !rstd || !dx || (relu == 1 && !y) || (relu == 2 && !shift)) {
     set_error("bn_bwd_apply: NULL pointer"); return COTB200_ENULL; }
   if (relu < 0 || relu > 2) { set_error("bn_bwd_apply: relu must be 0, 1 or 2"); return COTB200_EINVAL; }
   if (dtype == COTB200_F64) { set_error("bn_bwd_apply: fp64 not supported"); return COTB200_EDTYPE; }
+  const int ds_hw = HW;           // rows per sample (drop-path scales)
   { const long long rows = (long long)B * HW; if (rows > 2147483647LL) { set_error("cotb200_bn_bwd_apply: too many rows"); return COTB200_ETOOBIG; }
     HW = (int)rows; B = 1; }      // per-channel statistics: flatten [B, HW] -> rows
   cudaStream_t st = (cudaStream_t)stream;
@@ -1111,20 +1152,31 @@ extern "C" int cotb200_bn_finalize(int C, const float* sum, const float* sq, con
 extern "C" int cotb200_bn_bwd_sums(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y,
                                    const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
                                    float* sum_dz, float* sum_dzx, void* stream) {
-  return bn_bwd_sums_impl(dtype, B, HW, C, dy, nullptr, x, y, scale, shift, mu, rstd, relu, sum_dz, sum_dzx, stream);
+  return bn_bwd_sums_impl(dtype, B, HW, C, dy, nullptr, x, y, scale, shift, mu, rstd, relu, sum_dz, sum_dzx, nullptr, stream);
 }
 extern "C" int cotb200_bn_bwd_sums2(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
                                     const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
                                     float* sum_dz, float* sum_dzx, void* stream) {
-  return bn_bwd_sums_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, relu, sum_dz, sum_dzx, stream);
+  return bn_bwd_sums_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, relu, sum_dz, sum_dzx, nullptr, stream);
+}
+extern "C" int cotb200_bn_bwd_sums_ds(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
+                                      const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
+                                      float* sum_dz, float* sum_dzx, const float* sample_scale, void* stream) {
+  return bn_bwd_sums_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, relu, sum_dz, sum_dzx, sample_scale, stream);
 }
 extern "C" int cotb200_bn_bwd_apply(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y,
                                     const float* scale, const float* shift, const float* mu, const float* rstd,
                                     const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres, void* stream) {
-  return bn_bwd_apply_impl(dtype, B, HW, C, dy, nullptr, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, stream);
+  return bn_bwd_apply_impl(dtype, B, HW, C, dy, nullptr, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, nullptr, stream);
 }
 extern "C" int cotb200_bn_bwd_apply2(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
                                      const float* scale, const float* shift, const float* mu, const float* rstd,
                                      const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres, void* stream) {
-  return bn_bwd_apply_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, stream);
+  return bn_bwd_apply_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, nullptr, stream);
+}
+extern "C" int cotb200_bn_bwd_apply_ds(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
+                                       const float* scale, const float* shift, const float* mu, const float* rstd,
+                                       const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres,
+                                       const float* sample_scale, void* stream) {
+  return bn_bwd_apply_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, sample_scale, stream);
 }

@@ -175,50 +175,85 @@ def _bn_batch_stats(x, bn, weight, bias, lib, st, dt):
     return _bn_prepare(bn, weight, bias, C, float(B * H * W), None, x.device, st), False
 
 
-def _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt):
+def _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds=None):
     """Training-mode BatchNorm tail shared by BNActFn and the wgmma functions: ONE kernel finalises the batch statistics
     (sums = [2, C] column sums over the B*H*W rows of x), updates the running buffers and applies scale/shift(+res)(+ReLU).
+    ds: None or the [B] fp32 per-sample drop-path scales applied to the BatchNorm output before the residual add.
     Returns ss = [4, C] (scale, shift, mean, rstd) for the backward."""
     B, C, H, W = x.shape
     ss = torch.empty(4, C, dtype=torch.float32, device=x.device)
     update, mom, rm, rv = _bn_running(bn, True)
     w32 = None if weight is None else weight.detach().float().contiguous()
     b32 = None if bias is None else bias.detach().float().contiguous()
-    _lib.check(lib.cotb200_bn_apply_batch(dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), sums[0].data_ptr(), sums[1].data_ptr(),
-                                          _lib.ptr(w32), _lib.ptr(b32), _lib.ptr(rm), _lib.ptr(rv), float(B * H * W),
-                                          float(bn.eps), float(mom), 1 if update else 0, 1 if relu else 0, y.data_ptr(),
-                                          ss[0].data_ptr(), ss[1].data_ptr(), ss[2].data_ptr(), ss[3].data_ptr(), st),
-               "bn_apply_batch")
+    args = (dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), sums[0].data_ptr(), sums[1].data_ptr(), _lib.ptr(w32), _lib.ptr(b32),
+            _lib.ptr(rm), _lib.ptr(rv), float(B * H * W), float(bn.eps), float(mom), 1 if update else 0, 1 if relu else 0,
+            y.data_ptr(), ss[0].data_ptr(), ss[1].data_ptr(), ss[2].data_ptr(), ss[3].data_ptr())
+    if ds is None:
+        _lib.check(lib.cotb200_bn_apply_batch(*args, st), "bn_apply_batch")
+    else:
+        _lib.check(lib.cotb200_bn_apply_batch_ds(*args, ds.data_ptr(), st), "bn_apply_batch_ds")
     _bn_running_writeback(bn, update, rm, rv)
     return ss
+
+
+def _drop_scale(ds, x):
+    """The per-sample drop-path scales as the kernels take them: fp32 [B], contiguous, on x's device (None stays None)."""
+    if ds is None:
+        return None
+    ds = ds.detach()
+    assert ds.dim() == 1 and ds.shape[0] == x.shape[0] and ds.device == x.device, "drop_scale must be [B] on the input's device"
+    return ds.float().contiguous()
+
+
+def _bn_bwd(lib, dt, B, HW, C, dy, dy2, x, y, scale, shift, mean, rstd, rcode, sums, batch, inv_n, dx, dres, ds, st):
+    """BatchNorm backward (sums + apply) of the plain / two-gradient form, or of the drop-path form when ds is given."""
+    if sums is not None:
+        args = (dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), _lib.ptr(y), _lib.ptr(scale), _lib.ptr(shift),
+                mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(), sums[1].data_ptr())
+        if ds is None:
+            _lib.check(lib.cotb200_bn_bwd_sums2(*args, st), "bn_bwd_sums")
+        else:
+            _lib.check(lib.cotb200_bn_bwd_sums_ds(*args, ds.data_ptr(), st), "bn_bwd_sums_ds")
+    args = (dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), _lib.ptr(y), scale.data_ptr(), _lib.ptr(shift),
+            mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None, _lib.ptr(sums[1]) if batch else None,
+            inv_n, rcode, dx.data_ptr(), _lib.ptr(dres))
+    if ds is None:
+        _lib.check(lib.cotb200_bn_bwd_apply2(*args, st), "bn_bwd_apply")
+    else:
+        _lib.check(lib.cotb200_bn_bwd_apply_ds(*args, ds.data_ptr(), st), "bn_bwd_apply_ds")
 
 
 class BNActFn(Function):
     """y = act(BatchNorm2d(x) (+ res)) on channels_last tensors: col_stats + bn_finalize + bn_apply forward,
     bn_bwd_sums + bn_bwd_apply backward.  Replaces the nn.BatchNorm2d / nn.ReLU (/ residual add) modules of
     models/cotnet.py:45-46,53-54,61-62 and :231-235,:249-262 -- ATen's channels_last batch-norm kernels are the largest
-    single cost of the eager step."""
+    single cost of the eager step.  drop_scale: None or [B] per-sample stochastic-depth scales (models/cotnet.py:256-257),
+    y = act(drop_scale[b]*BatchNorm2d(x) (+ res)) in the same kernels."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, res, bn, relu, fork=False):
+    def forward(ctx, x, weight, bias, res, bn, relu, fork=False, drop_scale=None):
         assert _is_cl(x) and (res is None or (_is_cl(res) and res.dtype == x.dtype and res.shape == x.shape))
         ctx.set_materialize_grads(False)
         B, C, H, W = x.shape
         lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.dtype_code(x)
         x = x.detach()
+        ds = _drop_scale(drop_scale, x)
         y = torch.empty_like(x, memory_format=torch.channels_last)
         batch = bool(bn.training or bn.running_mean is None)
         if batch:       # training: column sums, then ONE kernel that finalises the statistics in its prologue and applies them
             sums = _zeros((2, C,), x.device)
             _lib.check(lib.cotb200_col_stats(dt, B, H * W, C, x.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(), st), "col_stats")
-            ss = _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt)   # [4,C]: scale, shift, mean, rstd
+            ss = _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds)   # [4,C]: scale, shift, mean, rstd
         else:
             ss = _bn_prepare(bn, weight, bias, C, float(B * H * W), None, x.device, st)
-            _lib.check(lib.cotb200_bn_apply(dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), ss[0].data_ptr(), ss[1].data_ptr(),
-                                            1 if relu else 0, y.data_ptr(), st), "bn_apply")
+            args = (dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), ss[0].data_ptr(), ss[1].data_ptr(), 1 if relu else 0, y.data_ptr())
+            if ds is None:
+                _lib.check(lib.cotb200_bn_apply(*args, st), "bn_apply")
+            else:
+                _lib.check(lib.cotb200_bn_apply_ds(*args, ds.data_ptr(), st), "bn_apply_ds")
         # ReLU mask in the backward: with a residual it must come from y; without one it is recomputed from x and the
         # forward's own scale/shift (relu code 2) and y is neither saved nor read
-        ctx.save_for_backward(x, y if (relu and res is not None) else None, ss)
+        ctx.save_for_backward(x, y if (relu and res is not None) else None, ss, ds)
         ctx.cfg = (relu, batch, res is not None, weight.dtype, bias.dtype)
         if fork:            # two aliases of ONE tensor: each consumer's gradient reaches backward() separately (see _two_grads)
             return y, y.detach()
@@ -226,29 +261,24 @@ class BNActFn(Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        x, y, ss = ctx.saved_tensors
+        x, y, ss, ds = ctx.saved_tensors
         relu, batch, has_res, wdt, bdt = ctx.cfg
         B, C, H, W = x.shape
         lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.dtype_code(x)
         dy, dy2 = _two_grads(grads)
         if dy is None:
-            return (None,) * 7
+            return (None,) * 8
         rcode = 0 if not relu else (1 if y is not None else 2)
         sums = None
         if batch or ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
             sums = _zeros_esc((2, C,), x.device)       # escapes as dgamma/dbeta
-            _lib.check(lib.cotb200_bn_bwd_sums2(dt, B, H * W, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), _lib.ptr(y), ss[0].data_ptr(),
-                                                ss[1].data_ptr(), ss[2].data_ptr(), ss[3].data_ptr(), rcode,
-                                                sums[0].data_ptr(), sums[1].data_ptr(), st), "bn_bwd_sums")
         dx = torch.empty_like(x, memory_format=torch.channels_last)
         dres = torch.empty_like(x, memory_format=torch.channels_last) if (has_res and ctx.needs_input_grad[3]) else None
-        _lib.check(lib.cotb200_bn_bwd_apply2(dt, B, H * W, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), _lib.ptr(y), ss[0].data_ptr(),
-                                             ss[1].data_ptr(), ss[2].data_ptr(), ss[3].data_ptr(),
-                                             _lib.ptr(sums[0]) if batch else None, _lib.ptr(sums[1]) if batch else None,
-                                             1.0 / float(B * H * W), rcode, dx.data_ptr(), _lib.ptr(dres), st), "bn_bwd_apply")
+        _bn_bwd(lib, dt, B, H * W, C, dy, dy2, x, y, ss[0], ss[1], ss[2], ss[3], rcode, sums, batch, 1.0 / float(B * H * W), dx, dres,
+                ds, st)
         dgamma = sums[1].to(wdt) if ctx.needs_input_grad[1] else None
         dbeta = sums[0].to(bdt) if ctx.needs_input_grad[2] else None
-        return dx, dgamma, dbeta, dres, None, None, None
+        return dx, dgamma, dbeta, dres, None, None, None, None
 
 
 def _two_grads(grads):
@@ -264,10 +294,10 @@ def _two_grads(grads):
     return g[0], g[1]
 
 
-def bn_act(x, bn: torch.nn.BatchNorm2d, relu=False, res=None, fork=False):
+def bn_act(x, bn: torch.nn.BatchNorm2d, relu=False, res=None, fork=False, drop_scale=None):
     """Fused BatchNorm2d (+ residual add) (+ ReLU) with the module's parameters / buffers / train-eval semantics.
-    fork=True returns two aliases of the output (see _two_grads)."""
-    return BNActFn.apply(x, bn.weight, bn.bias, res, bn, relu, fork)
+    fork=True returns two aliases of the output (see _two_grads); drop_scale: per-sample stochastic-depth scales [B] or None."""
+    return BNActFn.apply(x, bn.weight, bn.bias, res, bn, relu, fork, drop_scale)
 
 
 class GroupNorm9Fn(Function):
@@ -722,25 +752,27 @@ class TcConv1x1Fn(Function):
     bn = nn.BatchNorm2d or None (then `cbias` is the conv bias or None)."""
 
     @staticmethod
-    def forward(ctx, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res=None):
-        return TcConv1x1Fn._fwd(ctx, False, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res)
+    def forward(ctx, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res=None, drop_scale=None):
+        return TcConv1x1Fn._fwd(ctx, False, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res, drop_scale)
 
     @staticmethod
     def backward(ctx, *grads):
         return TcConv1x1Fn._bwd(ctx, grads)
 
     @staticmethod
-    def _fwd(ctx, fork, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res):
+    def _fwd(ctx, fork, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res, drop_scale=None):
         assert _is_cl(a1) and a1.dtype == torch.bfloat16 and (a2 is None or (_is_cl(a2) and a2.dtype == a1.dtype))
         if fork:
             ctx.set_materialize_grads(False)
         assert res is None or (bn is not None and _is_cl(res) and res.dtype == a1.dtype)
+        assert drop_scale is None or bn is not None
         B, K1, H, W = a1.shape
         K2 = 0 if a2 is None else a2.shape[1]
         N = weight.shape[0]
         M = B * H * W
         lib, st, dt = _lib.load(), _lib.stream_ptr(a1), _lib.dtype_code(a1)
         a1, a2 = a1.detach(), (None if a2 is None else a2.detach())
+        ds = _drop_scale(drop_scale, a1)
         wb = weight.detach().reshape(N, K1 + K2).to(torch.bfloat16).contiguous()
         b1, b2 = wb[:, :K1], (wb[:, K1:] if K2 else None)
         out = torch.empty((B, N, H, W), dtype=torch.bfloat16, device=a1.device, memory_format=torch.channels_last)
@@ -754,22 +786,26 @@ class TcConv1x1Fn(Function):
             sums = _zeros((2, N,), a1.device)
             pre = torch.empty_like(out, memory_format=torch.channels_last)
             _tc.gemm_bf16(a1, b1, a2, b2, stats=(sums[0], sums[1]), out=_rows2d(pre))
-            ss = _bn_apply_batch(pre, None if res is None else res.detach(), sums, bn, bn_w, bn_b, relu, out, lib, st, dt)
+            ss = _bn_apply_batch(pre, None if res is None else res.detach(), sums, bn, bn_w, bn_b, relu, out, lib, st, dt, ds)
             scale, shift, mean, rstd = ss[0], ss[1], ss[2], ss[3]
         else:
             scale, shift, mean, rstd = _bn_eval_fold(bn, bn_w, bn_b)
-            if res is None:
+            if res is None and ds is None:
                 _tc.gemm_bf16(a1, b1, a2, b2, scale=scale, shift=shift, relu=relu, out=out2d)
             else:       # eval mode with a residual: raw GEMM, then the fused scale/shift + residual + ReLU kernel
                 pre = torch.empty_like(out, memory_format=torch.channels_last)
                 _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(pre))
-                _lib.check(lib.cotb200_bn_apply(dt, B, H * W, N, pre.data_ptr(), res.data_ptr(), scale.data_ptr(), shift.data_ptr(),
-                                                1 if relu else 0, out.data_ptr(), st), "bn_apply")
+                args = (dt, B, H * W, N, pre.data_ptr(), _lib.ptr(res), scale.data_ptr(), shift.data_ptr(), 1 if relu else 0,
+                        out.data_ptr())
+                if ds is None:
+                    _lib.check(lib.cotb200_bn_apply(*args, st), "bn_apply")
+                else:
+                    _lib.check(lib.cotb200_bn_apply_ds(*args, ds.data_ptr(), st), "bn_apply_ds")
         need_bwd = any(ctx.needs_input_grad)
         if need_bwd and bn is not None and pre is None:      # eval-mode module under grad: BN backward needs the raw conv output
             pre = torch.empty_like(out, memory_format=torch.channels_last)
             _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(pre))
-        ctx.save_for_backward(a1, a2, wb, pre, out if relu else None, scale, mean, rstd)
+        ctx.save_for_backward(a1, a2, wb, pre, out if relu else None, scale, mean, rstd, ds)
         ctx.cfg = (relu, batch, bn is not None, cbias is not None, weight.dtype, weight.shape,
                    None if bn_w is None else bn_w.dtype, None if cbias is None else cbias.dtype, K1, K2, res is not None)
         if fork:
@@ -779,11 +815,11 @@ class TcConv1x1Fn(Function):
 
     @staticmethod
     def _bwd(ctx, grads):
-        a1, a2, wb, pre, y, scale, mean, rstd = ctx.saved_tensors
+        a1, a2, wb, pre, y, scale, mean, rstd, ds = ctx.saved_tensors
         relu, batch, has_bn, has_bias, wdt, wshape, bndt, cbdt, K1, K2, has_res = ctx.cfg
         dy, dy2 = _two_grads(grads)
         if dy is None:
-            return (None,) * 9
+            return (None,) * 10
         B, N, H, W = dy.shape
         M = B * H * W
         lib, st, dt = _lib.load(), _lib.stream_ptr(dy), _lib.BF16
@@ -792,15 +828,9 @@ class TcConv1x1Fn(Function):
             sums = _zeros_esc((2, N,), dy.device)      # escapes as dgamma/dbeta
             if has_res and ctx.needs_input_grad[8]:
                 dres = torch.empty_like(dy, memory_format=torch.channels_last)
-            _lib.check(lib.cotb200_bn_bwd_sums2(dt, B, H * W, N, dy.data_ptr(), _lib.ptr(dy2), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                                None, mean.data_ptr(), rstd.data_ptr(), 1 if relu else 0, sums[0].data_ptr(),
-                                                sums[1].data_ptr(), st),
-                       "bn_bwd_sums")
             dpre = torch.empty_like(dy, memory_format=torch.channels_last)
-            _lib.check(lib.cotb200_bn_bwd_apply2(dt, B, H * W, N, dy.data_ptr(), _lib.ptr(dy2), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                                 None, mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
-                                                 _lib.ptr(sums[1]) if batch else None, 1.0 / M, 1 if relu else 0,
-                                                 dpre.data_ptr(), _lib.ptr(dres), st), "bn_bwd_apply")
+            _bn_bwd(lib, dt, B, H * W, N, dy, dy2, pre, y, scale, None, mean, rstd, 1 if relu else 0, sums, batch, 1.0 / M, dpre, dres,
+                    ds, st)
             dgamma, dbeta = sums[1].to(bndt), sums[0].to(bndt)
         else:
             dpre = dy if not relu else dy * (y > 0)
@@ -830,7 +860,7 @@ class TcConv1x1Fn(Function):
                 acc = _zeros((N, K1 + K2,), dy.device)
                 _tc.wgrad_bf16(dpre, a1, a2, out=acc)
                 dw = acc.reshape(wshape).to(wdt)
-        return da1, da2, dw, dcb, dgamma, dbeta, None, None, dres
+        return da1, da2, dw, dcb, dgamma, dbeta, None, None, dres, None
 
 
 class TcConv1x1ForkFn(Function):
@@ -838,8 +868,8 @@ class TcConv1x1ForkFn(Function):
     kernels (_two_grads) instead of by an autograd add kernel."""
 
     @staticmethod
-    def forward(ctx, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res=None):
-        return TcConv1x1Fn._fwd(ctx, True, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res)
+    def forward(ctx, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res=None, drop_scale=None):
+        return TcConv1x1Fn._fwd(ctx, True, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res, drop_scale)
 
     @staticmethod
     def backward(ctx, *grads):
@@ -1001,17 +1031,20 @@ TC_TRUNK_MAX_WEIGHT = int(_os.environ.get("COTB200_TC_TRUNK_MAX_WEIGHT", str(128
 TC_MIN_PIXELS = int(_os.environ.get("COTB200_TC_MIN_PIXELS", "100000"))
 
 
-def conv1x1_bn(x, conv, bn, relu, res=None, fork=False):
+def conv1x1_bn(x, conv, bn, relu, res=None, fork=False, drop_scale=None):
     """act(BN(conv1x1(x)) (+ res)) for the bottleneck's 1x1 convolutions (models/cotnet.py:229-235,249-262): on the wgmma
     GEMMs when the backend says so and the geometry allows (bf16 channels_last, stride 1, dense, no bias), else cuDNN + the
-    fused BatchNorm kernels."""
+    fused BatchNorm kernels.  drop_scale: None or [B] stochastic-depth scales, act(drop_scale[b]*BN(conv1x1(x)) + res)
+    (models/cotnet.py:256-262)."""
     w = conv.weight
     if (trunk_conv_backend == "tc_all1x1" and x.dtype == torch.bfloat16 and supported(x) and conv.kernel_size == (1, 1)
             and conv.stride == (1, 1) and conv.groups == 1 and conv.bias is None and w.shape[0] % 8 == 0 and w.shape[1] % 8 == 0
             and w.shape[0] * w.shape[1] <= TC_TRUNK_MAX_WEIGHT and x.shape[0] * x.shape[2] * x.shape[3] >= TC_MIN_PIXELS
             and (torch.is_grad_enabled() or not bn.training)):
-        return (TcConv1x1ForkFn if fork else TcConv1x1Fn).apply(x, None, w, None, bn.weight, bn.bias, bn, relu, res)
-    return bn_act(conv(x).contiguous(memory_format=torch.channels_last), bn, relu=relu, res=res, fork=fork)
+        if drop_scale is None:
+            return (TcConv1x1ForkFn if fork else TcConv1x1Fn).apply(x, None, w, None, bn.weight, bn.bias, bn, relu, res)
+        return (TcConv1x1ForkFn if fork else TcConv1x1Fn).apply(x, None, w, None, bn.weight, bn.bias, bn, relu, res, drop_scale)
+    return bn_act(conv(x).contiguous(memory_format=torch.channels_last), bn, relu=relu, res=res, fork=fork, drop_scale=drop_scale)
 
 
 def tc_supported(x, dim):

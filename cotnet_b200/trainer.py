@@ -132,9 +132,13 @@ class TrainStep:
 
     def __init__(self, model, lr=0.05, momentum=0.9, weight_decay=1e-4, nesterov=True, ema_decay=None,
                  loss_fn=None, amp_dtype=torch.bfloat16, weights="bf16", bucket_dtype=None, comm_chunks=3, overlap=True,
-                 process_group=None):
+                 process_group=None, label_smoothing=0.):
+        """label_smoothing > 0, or a `mix` given to the step, selects the soft-target loss (soft_target_cross_entropy) that the
+        reference recipe trains with (train.py:198-209); otherwise the loss is `loss_fn` (default F.cross_entropy)."""
         self.model = model
         self.loss_fn = loss_fn or (lambda out, lab: F.cross_entropy(out.float(), lab))
+        self.label_smoothing = float(label_smoothing)
+        self._gmix = None
         self.amp_dtype = amp_dtype
         self.nesterov = bool(nesterov)
         self.pg = process_group
@@ -301,7 +305,14 @@ class TrainStep:
             torch.cuda.current_stream(self.dev).wait_stream(self.comm_stream)
 
     # ------------------------------------------------------------------ the step
-    def forward_backward(self, x, lab):
+    def _loss(self, out, lab, mix_dev):
+        if mix_dev is None and self.label_smoothing == 0.:
+            return self.loss_fn(out, lab)
+        return SoftTargetCrossEntropyFn.apply(out, lab, mix_dev, self.label_smoothing)
+
+    def forward_backward(self, x, lab, mix=None):
+        """mix: None, a MixParams (MixupCutmix.draw) or its 32-byte device struct -- the loss reads the mixed targets' lam from it."""
+        mix_dev = mix.on_stream(self.dev) if isinstance(mix, MixParams) else mix
         if self._cuda:
             fused.step_begin(self.dev)
             # every gradient of this step is gathered into the flat bucket before the next step_begin(): the BatchNorm gradient sums
@@ -319,7 +330,7 @@ class TrainStep:
             self._flushed[c] = False
         with torch.autocast(self.dev.type, dtype=self.amp_dtype, enabled=self.amp_dtype is not None):
             out = self.model(x)
-            loss = self.loss_fn(out, lab)
+            loss = self._loss(out, lab, mix_dev)
         if self._cuda:
             fused.flush_bn_counters()
             fused.defer_bn_counters(False)
@@ -344,24 +355,26 @@ class TrainStep:
         if self.ema and self._lerp_n:
             _lib.check(lib.cotb200_multi_lerp(self._lerp_tab.data_ptr(), self._lerp_n, self.hyper.data_ptr(), st), "multi_lerp")
 
-    def step_eager(self, x, lab):
-        loss = self.forward_backward(x, lab)
+    def step_eager(self, x, lab, mix=None):
+        loss = self.forward_backward(x, lab, mix)
         self.optimizer_step()
         return loss
 
     # ------------------------------------------------------------------ CUDA graph
-    def capture(self, x, lab, warmup=3, capture_nccl=True):
-        """Warm up (cuDNN autotune, allocator) and capture the whole step.  Returns a dict describing the launch mode."""
+    def capture(self, x, lab, warmup=3, capture_nccl=True, mix=None):
+        """Warm up (cuDNN autotune, allocator) and capture the whole step.  Returns a dict describing the launch mode.
+        With `mix` (a MixParams) the graph's loss reads a static copy of the mixing parameters that step(mix=) refreshes."""
         side = torch.cuda.Stream(device=self.dev)
         side.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(side):
             for _ in range(warmup):
-                self.step_eager(x, lab)
+                self.step_eager(x, lab, mix)
         torch.cuda.current_stream(self.dev).wait_stream(side)
         torch.cuda.synchronize(self.dev)
         for t in self._tabs + [self._tab_small]:
             t.done = None
         self._gx, self._glab = x.clone(), lab.clone()
+        self._gmix = None if mix is None else mix.dev.clone()
         info = {"cuda_graph": True}
         lc0 = _lib.launch_count()
         try:
@@ -370,7 +383,7 @@ class TrainStep:
             g = torch.cuda.CUDAGraph()
             self._capturing = True
             with torch.cuda.graph(g):
-                self._gloss = self.step_eager(self._gx, self._glab)
+                self._gloss = self.step_eager(self._gx, self._glab, self._gmix)
             self._capturing = False
             self._graph = ("one", g)
             info["graphs"] = "fwd+bwd+gather%s+optimizer in ONE graph" % ("+NCCL (side-stream branches)" if self.world > 1 else "")
@@ -386,7 +399,7 @@ class TrainStep:
             g1, g2 = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
             self._capturing = True
             with torch.cuda.graph(g1):
-                self._gloss = self.forward_backward(self._gx, self._glab)
+                self._gloss = self.forward_backward(self._gx, self._glab, self._gmix)
             with torch.cuda.graph(g2):
                 self.optimizer_step()
             self._capturing = False
@@ -396,13 +409,20 @@ class TrainStep:
         info["libcotb200_kernels_per_replay"] = _lib.launch_count() - lc0
         return info
 
-    def step(self, x=None, lab=None):
-        """One step; (x, lab) are copied into the graph's static inputs when a graph is active and they are given."""
+    def step(self, x=None, lab=None, mix=None):
+        """One step; (x, lab) and the mixing parameters `mix` (MixupCutmix.draw) are copied into the graph's static inputs
+        when a graph is active and they are given.  A graph captured with `mix` needs one at every step (it would otherwise replay
+        the previous step's lam and box), and a graph captured without it refuses one."""
         if self._graph is None:
-            return self.step_eager(x, lab)
+            return self.step_eager(x, lab, mix)
         if x is not None and x is not self._gx:
             self._gx.copy_(x, non_blocking=True)
             self._glab.copy_(lab, non_blocking=True)
+        if (mix is None) != (self._gmix is None):
+            raise ValueError("TrainStep.step: this graph was captured %s mixing parameters; pass mix= %s"
+                             % (("without", "to capture() first") if mix is not None else ("with", "(MixupCutmix.draw) at every step")))
+        if mix is not None:
+            self._gmix.copy_(mix.on_stream(self.dev), non_blocking=True)
         if self._graph[0] == "one":
             self._graph[1].replay()
         else:
@@ -420,7 +440,7 @@ class TrainStep:
         world, self.world = self.world, 1
         try:
             if self._graph is None:
-                return timed(lambda: self.step_eager(self._gx, self._glab), steps)
+                return timed(lambda: self.step_eager(self._gx, self._glab, self._gmix), steps)
             if self._graph[0] == "two":
                 def run():
                     self._graph[1].replay()
@@ -430,7 +450,7 @@ class TrainStep:
             g = torch.cuda.CUDAGraph()
             self._capturing = True
             with torch.cuda.graph(g):
-                self.step_eager(self._gx, self._glab)
+                self.step_eager(self._gx, self._glab, self._gmix)
             self._capturing = False
             for _ in range(2):
                 g.replay()
@@ -476,9 +496,11 @@ class TrainStep:
         return out
 
 
-def normalize_u8(x_u8, mean, std, dtype=torch.bfloat16):
+def normalize_u8(x_u8, mean, std, dtype=torch.bfloat16, mix=None):
     """uint8 NCHW batch [N,C,H,W] (CUDA) -> (x - mean)/std as a channels_last tensor of `dtype`: the PrefetchLoader's
-    normalisation (datasets/loader.py:86-90) + the layout / precision the AMP forward wants, in ONE kernel."""
+    normalisation (datasets/loader.py:86-90) + the layout / precision the AMP forward wants, in ONE kernel.
+    mix: a MixParams of MixupCutmix.draw -- the batch is Mixup / CutMix-ed first, on the uint8 values, exactly like
+    FastCollateMixup (datasets/mixup.py:282-299), in the same kernel."""
     assert x_u8.is_cuda and x_u8.dtype == torch.uint8 and x_u8.dim() == 4 and x_u8.is_contiguous()
     N, C, H, W = x_u8.shape
     y = torch.empty((N, C, H, W), dtype=dtype, device=x_u8.device, memory_format=torch.channels_last)
@@ -490,7 +512,146 @@ def normalize_u8(x_u8, mean, std, dtype=torch.bfloat16):
     if not (C == 3 and (H * W) % 4 == 0):
         md = torch.tensor(mean, dtype=torch.float32, device=x_u8.device)
         sd = torch.tensor(std, dtype=torch.float32, device=x_u8.device)
-    rc = _lib.load().cotb200_u8_to_nhwc(_lib.dtype_code(y), N, C, H, W, x_u8.data_ptr(), y.data_ptr(), mh, sh, _lib.ptr(md), _lib.ptr(sd),
-                                        _lib.stream_ptr(x_u8))
-    _lib.check(rc, "u8_to_nhwc")
+    if mix is None:
+        rc = _lib.load().cotb200_u8_to_nhwc(_lib.dtype_code(y), N, C, H, W, x_u8.data_ptr(), y.data_ptr(), mh, sh, _lib.ptr(md),
+                                            _lib.ptr(sd), _lib.stream_ptr(x_u8))
+        _lib.check(rc, "u8_to_nhwc")
+        return y
+    mix.check(N, H, W)
+    rc = _lib.load().cotb200_u8_mix_to_nhwc(_lib.dtype_code(y), N, C, H, W, x_u8.data_ptr(), y.data_ptr(), mh, sh, _lib.ptr(md),
+                                            _lib.ptr(sd), mix.on_stream(x_u8.device).data_ptr(), _lib.stream_ptr(x_u8))
+    _lib.check(rc, "u8_mix_to_nhwc")
     return y
+
+
+# ---------------------------------------------------------------------------------------------------- the training recipe
+class MixParams:
+    """One step's batch Mixup / CutMix parameters (struct cotb200_mix): `host` holds the values (a ctypes _lib.Mix), `dev` a
+    device copy that the kernels read, `target_lam` the float64 lam of the draw (the struct holds it rounded to fp32).
+    The device copy is made from a freshly pinned buffer of torch's caching host allocator, which does not hand that buffer out
+    again before the copy has finished: the next draw() never races it.  The copy is issued on the stream current at draw();
+    every consumer takes the struct through on_stream(), which orders its own current stream after that copy (an event wait)
+    and tells the allocator that stream uses the memory, so drawing and consuming on different streams is safe."""
+    MODES = (0, 1, 2)
+
+    def __init__(self, host, device=None, target_lam=None):
+        self.host = host
+        self.target_lam = float(host.target_lam if target_lam is None else target_lam)
+        self.dev = self._copied = None
+        if device is not None:
+            self.dev = torch.frombuffer(bytearray(bytes(host)), dtype=torch.uint8).pin_memory().to(device, non_blocking=True)
+            self._copied = torch.cuda.Event()
+            self._copied.record(torch.cuda.current_stream(self.dev.device))
+
+    mode = property(lambda self: self.host.mode)
+    box = property(lambda self: (self.host.y0, self.host.y1, self.host.x0, self.host.x1))
+
+    def check(self, N, H, W):
+        h = self.host
+        if h.mode not in self.MODES:
+            raise ValueError("mix: unknown mode %d (0 none, 1 mixup, 2 cutmix)" % h.mode)
+        if N % 2:
+            raise ValueError("mix: batch size %d must be even (the partner of sample n is N-1-n)" % N)
+        if h.mode == 2 and not (0 <= h.y0 <= h.y1 <= H and 0 <= h.x0 <= h.x1 <= W):
+            raise ValueError("mix: CutMix box %s outside the %dx%d image" % (self.box, H, W))
+
+    def on_stream(self, device):
+        """The device struct, ready for use on `device`'s current stream."""
+        if self.dev is None or self.dev.device != torch.device(device):
+            raise ValueError("mix: no device copy on %s (MixupCutmix(device=...))" % device)
+        st = torch.cuda.current_stream(self.dev.device)
+        st.wait_event(self._copied)
+        self.dev.record_stream(st)
+        return self.dev
+
+
+class MixupCutmix:
+    """Batch-mode Mixup / CutMix of the reference configs (FastCollateMixup, datasets/mixup.py; mode 'batch', correct_lam,
+    no cutmix_minmax), drawing its parameters from its own np.random.RandomState(seed) in the reference's call order:
+    rand < prob, rand < switch_prob, beta, randint (box centre row), randint (box centre column).
+    `enabled = False` turns mixing off (mixup_off_epoch); draws then give lam = 1 without consuming random numbers."""
+
+    def __init__(self, mixup_alpha=0.8, cutmix_alpha=1.0, prob=1.0, switch_prob=0.5, label_smoothing=0.1, num_classes=1000,
+                 seed=0, correct_lam=True, device="cuda"):
+        if not (mixup_alpha > 0. or cutmix_alpha > 0.):
+            raise ValueError("MixupCutmix: mixup_alpha or cutmix_alpha must be > 0")
+        self.mixup_alpha, self.cutmix_alpha = float(mixup_alpha), float(cutmix_alpha)
+        self.prob, self.switch_prob = float(prob), float(switch_prob)
+        self.label_smoothing, self.num_classes = float(label_smoothing), int(num_classes)
+        self.correct_lam = bool(correct_lam)
+        self.rng = np.random.RandomState(seed)
+        self.enabled = True
+        self.device = None if device is None else torch.device(device)
+
+    def _params_per_batch(self):                                    # datasets/mixup.py:143-159
+        lam, use_cutmix = 1., False
+        if self.enabled and self.rng.rand() < self.prob:
+            if self.mixup_alpha > 0. and self.cutmix_alpha > 0.:
+                use_cutmix = self.rng.rand() < self.switch_prob
+                lam_mix = (self.rng.beta(self.cutmix_alpha, self.cutmix_alpha) if use_cutmix
+                           else self.rng.beta(self.mixup_alpha, self.mixup_alpha))
+            elif self.mixup_alpha > 0.:
+                lam_mix = self.rng.beta(self.mixup_alpha, self.mixup_alpha)
+            else:
+                use_cutmix = True
+                lam_mix = self.rng.beta(self.cutmix_alpha, self.cutmix_alpha)
+            lam = float(lam_mix)
+        return lam, bool(use_cutmix)
+
+    def draw(self, B, H, W):
+        """Parameters of the next batch of B images of H x W as a MixParams (host struct + device copy)."""
+        if B % 2:
+            raise ValueError("MixupCutmix: batch size %d must be even" % B)
+        lam, use_cutmix = self._params_per_batch()
+        m = _lib.Mix()
+        if use_cutmix:                                              # rand_bbox + cutmix_bbox_and_lam (:30-87), margin 0
+            ratio = np.sqrt(1 - lam)
+            cut_h, cut_w = int(H * ratio), int(W * ratio)
+            cy, cx = self.rng.randint(0, H), self.rng.randint(0, W)
+            m.y0, m.y1 = int(np.clip(cy - cut_h // 2, 0, H)), int(np.clip(cy + cut_h // 2, 0, H))
+            m.x0, m.x1 = int(np.clip(cx - cut_w // 2, 0, W)), int(np.clip(cx + cut_w // 2, 0, W))
+            if self.correct_lam:
+                lam = 1. - (m.y1 - m.y0) * (m.x1 - m.x0) / float(H * W)
+        m.mode = 0 if lam == 1. else (2 if use_cutmix else 1)
+        # numpy 2 weak scalars: float32 pixels * python float multiplies by the float rounded to fp32 (:296)
+        m.lam, m.one_minus_lam = float(np.float32(lam)), float(np.float32(1 - lam))
+        m.target_lam = lam
+        return MixParams(m, self.device, lam)
+
+
+class SoftTargetCrossEntropyFn(torch.autograd.Function):
+    """SoftTargetCrossEntropy()(logits, mixup_target(labels, K, lam, smoothing)) (loss/cross_entropy.py:29-36,
+    datasets/mixup.py:17-27) on cotb200_soft_ce / cotb200_soft_ce_bwd; lam is read on the device from `mix_dev` (the struct of
+    a MixParams; None = no mixing, i.e. LabelSmoothingCrossEntropy, and plain cross entropy with smoothing 0).  logits
+    [B, K] fp32 / bf16 / fp16 with unit column stride; labels int64 [B].  Returns the fp32 batch mean."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, mix_dev, smoothing):
+        assert logits.is_cuda and logits.dim() == 2 and logits.stride(1) == 1 and labels.dtype == torch.int64
+        B, K = logits.shape
+        logits, labels = logits.detach(), labels.contiguous()
+        rows = torch.empty(2, B, dtype=torch.float32, device=logits.device)
+        loss = torch.empty((), dtype=torch.float32, device=logits.device)
+        lib, st, dt = _lib.load(), _lib.stream_ptr(logits), _lib.dtype_code(logits)
+        _lib.check(lib.cotb200_soft_ce(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), _lib.ptr(mix_dev),
+                                       float(smoothing), rows.data_ptr(), loss.data_ptr(), st), "soft_ce")
+        ctx.save_for_backward(logits, labels, mix_dev, rows)
+        ctx.smoothing = float(smoothing)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        logits, labels, mix_dev, rows = ctx.saved_tensors
+        B, K = logits.shape
+        dloss = dloss.float().contiguous()
+        dz = torch.empty(B, K, dtype=torch.float32, device=logits.device)
+        lib, st, dt = _lib.load(), _lib.stream_ptr(logits), _lib.dtype_code(logits)
+        _lib.check(lib.cotb200_soft_ce_bwd(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), _lib.ptr(mix_dev),
+                                           ctx.smoothing, rows.data_ptr(), dloss.data_ptr(), dz.data_ptr(), K, st), "soft_ce_bwd")
+        return dz.to(logits.dtype), None, None, None
+
+
+def soft_target_cross_entropy(logits, labels, mix=None, smoothing=0.):
+    """The recipe's loss: mean over the batch of -sum_c t_c log softmax(logits)_c with t = mixup_target(labels, K, mix.target_lam,
+    smoothing).  mix: None or a MixParams (MixupCutmix.draw)."""
+    return SoftTargetCrossEntropyFn.apply(logits, labels, None if mix is None else mix.on_stream(logits.device), smoothing)

@@ -212,6 +212,25 @@ int cotb200_bn_bwd_apply2(int dtype, int B, int HW, int C, const void* dy, const
 int cotb200_bn_bwd_apply(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y, const float* scale,
                          const float* shift, const float* mu, const float* rstd, const float* c1, const float* c2,
                          float inv_n, int relu, void* dx, void* dres, void* stream);
+/* Stochastic depth (DropPath after bn3, models/cotnet.py:256-257) inside the same kernels.  sample_scale: device fp32 [B] = s_b,
+ * 0 for a dropped sample and 1/keep for a kept one (NULL = all 1: then each call is its plain form above, bit for bit).
+ *   forward:  y = act(s_b*(x*scale + shift) (+ res))
+ *   backward: g = dy*mask (dy := dy + dy2 when dy2 != NULL); dres = g; the BatchNorm output gradient is s_b*g, so
+ *             sum_dz += sum s_b*g, sum_dzx += sum s_b*g*xhat and dx = scale*(s_b*g - c1*inv_n - xhat*c2*inv_n).
+ * The batch statistics (cotb200_col_stats, the GEMM epilogue) still cover every sample, dropped or not. */
+int cotb200_bn_apply_ds(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
+                        const float* shift, int relu, void* y, const float* sample_scale, void* stream);
+int cotb200_bn_apply_batch_ds(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum, const float* sq,
+                              const float* weight, const float* bias, float* running_mean, float* running_var, float n,
+                              float eps, float momentum, int update_running, int relu, void* y, float* scale, float* shift,
+                              float* mean, float* rstd, const float* sample_scale, void* stream);
+int cotb200_bn_bwd_sums_ds(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
+                           const float* scale, const float* shift, const float* mu, const float* rstd, int relu, float* sum_dz,
+                           float* sum_dzx, const float* sample_scale, void* stream);
+int cotb200_bn_bwd_apply_ds(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
+                            const float* scale, const float* shift, const float* mu, const float* rstd, const float* c1,
+                            const float* c2, float inv_n, int relu, void* dx, void* dres, const float* sample_scale,
+                            void* stream);
 /* One launch for the BatchNorm bookkeeping: from the column sums of cotb200_col_stats (or a GEMM epilogue) compute
  * scale = gamma*rstd, shift = beta - mean*scale, mean, rstd, and update running_mean / running_var like nn.BatchNorm2d
  * (momentum, unbiased variance).  use_batch = 0: eval mode, statistics read from the running buffers. */
@@ -370,6 +389,37 @@ int cotb200_multi_lerp(const cotb200_seg2* segs_dev, int n_segs, const float* hy
  * pass.  C == 3 with H*W % 4 == 0 takes mean_host/std_host (host arrays of 3); anything else needs the device arrays. */
 int cotb200_u8_to_nhwc(int dtype, int N, int C, int H, int W, const void* x_u8, void* y, const float* mean_host,
                        const float* std_host, const float* mean_dev, const float* std_dev, void* stream);
+
+/* ---- the training recipe of the reference configs: batch Mixup / CutMix and the soft-target loss ----
+ * Per-step parameters of FastCollateMixup in batch mode (datasets/mixup.py:143-159,282-299, correct_lam).  The struct lives
+ * in DEVICE memory and is read by the kernels, never passed by value, so a captured CUDA graph follows every step's draw.
+ *   mode 0: no mixing (lam = 1); 1: mixup; 2: CutMix with the box rows [y0, y1) x columns [x0, x1).
+ *   lam, one_minus_lam: the blend weights, each rounded to fp32 from the float64 draw (numpy's weak-scalar rule).
+ *   target_lam: the weight of the sample's own label in the soft target (the box-corrected lam for CutMix). */
+typedef struct cotb200_mix {
+  int mode;
+  float lam, one_minus_lam, target_lam;
+  int y0, y1, x0, x1;
+} cotb200_mix;
+/* cotb200_u8_to_nhwc of the mixed batch: sample n is mixed with its partner N-1-n before the normalisation.  mode 1:
+ * rint(x_n*lam + x_p*(1-lam)) in fp32 without FMA contraction (ties to even, np.rint); mode 2: x_p's pixels inside the box;
+ * mode 0: bit-equal to cotb200_u8_to_nhwc.  N must be even when mix != NULL; mix == NULL means mode 0. */
+int cotb200_u8_mix_to_nhwc(int dtype, int N, int C, int H, int W, const void* x_u8, void* y, const float* mean_host,
+                           const float* std_host, const float* mean_dev, const float* std_dev, const cotb200_mix* mix,
+                           void* stream);
+/* Soft-target cross entropy of SoftTargetCrossEntropy(mixup_target(labels, K, lam, smoothing)) (loss/cross_entropy.py:29-36,
+ * datasets/mixup.py:17-27) without materialising the target: per row b, with off = smoothing/K, on = 1 - smoothing + off,
+ *   loss_b = lse(z_b) - off*sum_c z_bc - (on - off)*(lam*z_b[y_b] + (1-lam)*z_b[y_{B-1-b}]),  lam = mix->target_lam.
+ * mix == NULL: lam = 1 (LabelSmoothingCrossEntropy; with smoothing 0 plain cross entropy).  logits: fp32 / bf16 / fp16
+ * [B, K] with row pitch ld; labels int64 [B].  rows: fp32 [2, B] written: rows[b] = lse(z_b) (the backward reads it),
+ * rows[B + b] = loss_b.  loss: fp32 [1] written with the batch mean, the rows added in a fixed order.  A label outside
+ * [0, K) makes its row (and the mean) NaN; it is never read out of bounds.  An odd B with mix != NULL is rejected. */
+int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, const cotb200_mix* mix,
+                    float smoothing, float* rows, float* loss, void* stream);
+/* dz[b, c] = dloss[0]/B * (softmax(z_b)_c - t_bc), fp32 [B, K] with row pitch ldz; dloss is read from device memory. */
+int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
+                        const cotb200_mix* mix, float smoothing, const float* rows, const float* dloss, float* dz,
+                        long long ldz, void* stream);
 
 #ifdef __cplusplus
 }
