@@ -292,12 +292,39 @@ struct BnFin {
   float* scale; float* shift; float* mean; float* rstd;
 };
 
+// 1-bit ReLU masks (relu code 3): bit c%8 of byte c/8 of row r is [y > 0] of the STORED output, so the backward reads 1/8 byte per
+// element instead of y.  Row pitch mld = C/8 bytes (C % 8 == 0).  A thread owns VEC channels, i.e. VEC bits of one byte; the
+// MASK_LANES = 8/VEC threads of a byte are adjacent lanes of one row (cq_pad is a power of two >= MASK_LANES), OR-ed by shuffles.
+template <int VEC> struct MaskLanes { static constexpr int G = 8 / VEC; };
+template <int VEC>
+__device__ __forceinline__ void store_mask_bits(unsigned char* __restrict__ mask, long long row_off, int tx, unsigned bits) {
+  constexpr int G = MaskLanes<VEC>::G;
+  if constexpr (G > 1) {
+    const unsigned lane = threadIdx.x & 31u, gm = ((1u << G) - 1u) << (lane & ~(unsigned)(G - 1));
+    bits <<= (tx % G) * VEC;
+#pragma unroll
+    for (int o = 1; o < G; o <<= 1) bits |= __shfl_xor_sync(gm, bits, o);
+    if (tx % G == 0) mask[row_off + tx / G] = (unsigned char)bits;
+  } else {
+    mask[row_off + tx] = (unsigned char)bits;
+  }
+}
+// the VEC bits of this thread's channels, bit i = channel tx*VEC + i
+template <int VEC>
+__device__ __forceinline__ unsigned load_mask_bits(const unsigned char* __restrict__ mask, long long row_off, int tx) {
+  constexpr int G = MaskLanes<VEC>::G;
+  return (unsigned)__ldg(mask + row_off + tx / G) >> ((tx % G) * VEC);
+}
+
 // DS (stochastic depth, models/cotnet.py:256-257): y = act(ds[b]*(x*scale + shift) (+ res)), ds [B] per-sample scales in
 // {0, 1/keep}; the kernels see the flattened rows, so the sample of row r is r / ds_hw.  DS == false compiles to the plain form.
-template <typename T, int VEC, int ACT, bool RES, bool FIN, bool DS = false>
+// MSK: also write the 1-bit ReLU mask of y (ACT == 1).
+template <typename T, int VEC, int ACT, bool RES, bool FIN, bool DS = false, bool MSK = false>
 __global__ void __launch_bounds__(NT_THREADS)
 bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float* __restrict__ scale,
-                const float* __restrict__ shift, T* __restrict__ y, RowsGeo g, BnFin f, const float* __restrict__ ds, int ds_hw) {
+                const float* __restrict__ shift, T* __restrict__ y, RowsGeo g, BnFin f, const float* __restrict__ ds, int ds_hw,
+                unsigned char* __restrict__ mask, int mld) {
+  static_assert(!MSK || ACT == 1, "the mask is the ReLU's");
   const int tx = threadIdx.x % g.cq_pad, ty = threadIdx.x / g.cq_pad;
   if (!(tx < g.cq && ty < g.ry)) return;
   const int b = blockIdx.y, r0 = blockIdx.x * g.rows_per_cta, r1 = min(g.HW, r0 + g.rows_per_cta);
@@ -339,16 +366,24 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
       o.v[i] = Elem<T>::from(z);
     }
     st_pack<T, VEC>(y + base + (long long)r * g.ld, o);
+    if constexpr (MSK) {
+      unsigned bits = 0;
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) bits |= (to_acc(o.v[i]) > 0.f ? 1u : 0u) << i;
+      store_mask_bits<VEC>(mask, (long long)r * mld, tx, bits);
+    }
   }
 }
 
-// dz = dy * [y > 0] (ACT==1: mask read from y ; ACT==2: mask recomputed as x*scale+shift > 0, one HBM pass less) ;
+// dz = dy * [y > 0] (ACT==1: mask read from y ; ACT==2: mask recomputed as x*scale+shift > 0, one HBM pass less ;
+// ACT==3: mask read from the 1-bit mask the forward wrote) ;
 // sum_dz[c] += dz ; sum_dzx[c] += dz * xhat.   DS: the BatchNorm output was scaled by ds[b], so its gradient is ds[b]*dz.
 template <typename T, int VEC, int ACT, bool DS = false>
 __global__ void __launch_bounds__(NT_THREADS)
 bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T* __restrict__ x, const T* __restrict__ y, const float* __restrict__ scale,
                    const float* __restrict__ shift, const float* __restrict__ mu, const float* __restrict__ rstd,
-                   float* __restrict__ sum_dz, float* __restrict__ sum_dzx, RowsGeo g, const float* __restrict__ ds, int ds_hw) {
+                   float* __restrict__ sum_dz, float* __restrict__ sum_dzx, RowsGeo g, const float* __restrict__ ds, int ds_hw,
+                   const unsigned char* __restrict__ mask, int mld) {
   extern __shared__ float sm[];
   const int tx = threadIdx.x % g.cq_pad, ty = threadIdx.x / g.cq_pad;
   const bool active = tx < g.cq && ty < g.ry;
@@ -365,7 +400,9 @@ bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T*
       const Pack<T, VEC> dv = ld_pack<T, VEC>(dy + base + (long long)r * g.ld);
       const Pack<T, VEC> xv = ld_pack<T, VEC>(x + base + (long long)r * g.ld);
       Pack<T, VEC> yv, d2;
+      unsigned mb = 0;
       if (ACT == 1) yv = ld_pack<T, VEC>(y + base + (long long)r * g.ld);
+      if (ACT == 3) mb = load_mask_bits<VEC>(mask, (long long)r * mld, tx);
       if (dy2) d2 = ld_pack<T, VEC>(dy2 + base + (long long)r * g.ld);    // two-consumer output: dy = dy + dy2, summed here in fp32
       float s = 1.f;
       if (DS) s = __ldg(ds + r / ds_hw);
@@ -375,6 +412,7 @@ bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T*
         if (dy2) dz += to_acc(d2.v[i]);
         const float xf = to_acc(xv.v[i]);
         if (ACT == 1 && !(to_acc(yv.v[i]) > 0.f)) dz = 0.f;
+        if (ACT == 3 && !((mb >> i) & 1u)) dz = 0.f;
         if (ACT == 2 && !((DS ? fmaf(xf, sc[i], sh[i]) * s : fmaf(xf, sc[i], sh[i])) > 0.f)) dz = 0.f;   // the forward's own fp32 z: identical mask, y not read
         if (DS) dz *= s;
         acc[0][i] += dz;
@@ -393,7 +431,8 @@ __global__ void __launch_bounds__(NT_THREADS)
 bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T* __restrict__ x, const T* __restrict__ y, const float* __restrict__ scale,
                     const float* __restrict__ shift, const float* __restrict__ mu, const float* __restrict__ rstd,
                     const float* __restrict__ c1, const float* __restrict__ c2, float inv_n, T* __restrict__ dx,
-                    T* __restrict__ dres, RowsGeo g, const float* __restrict__ ds, int ds_hw) {
+                    T* __restrict__ dres, RowsGeo g, const float* __restrict__ ds, int ds_hw,
+                    const unsigned char* __restrict__ mask, int mld) {
   const int tx = threadIdx.x % g.cq_pad, ty = threadIdx.x / g.cq_pad;
   if (!(tx < g.cq && ty < g.ry)) return;
   const int b = blockIdx.y, r0 = blockIdx.x * g.rows_per_cta, r1 = min(g.HW, r0 + g.rows_per_cta);
@@ -409,7 +448,9 @@ bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T
     const Pack<T, VEC> dv = ld_pack<T, VEC>(dy + base + (long long)r * g.ld);
     const Pack<T, VEC> xv = ld_pack<T, VEC>(x + base + (long long)r * g.ld);
     Pack<T, VEC> yv, d2;
+    unsigned mb = 0;
     if (ACT == 1) yv = ld_pack<T, VEC>(y + base + (long long)r * g.ld);
+    if (ACT == 3) mb = load_mask_bits<VEC>(mask, (long long)r * mld, tx);
     if (dy2) d2 = ld_pack<T, VEC>(dy2 + base + (long long)r * g.ld);
     Pack<T, VEC> o, o2;
     float s = 1.f;
@@ -420,6 +461,7 @@ bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T
       if (dy2) dz += to_acc(d2.v[i]);
       const float xf = to_acc(xv.v[i]);
       if (ACT == 1 && !(to_acc(yv.v[i]) > 0.f)) dz = 0.f;
+      if (ACT == 3 && !((mb >> i) & 1u)) dz = 0.f;
       if (ACT == 2 && !((DS ? fmaf(xf, sc[i], sh[i]) * s : fmaf(xf, sc[i], sh[i])) > 0.f)) dz = 0.f;
       o.v[i] = Elem<T>::from(sc[i] * ((DS ? dz * s : dz) - k1[i] - (xf - m[i]) * rs[i] * k2[i]));
       if (RES) o2.v[i] = Elem<T>::from(dz);
@@ -960,12 +1002,25 @@ extern "C" int cotb200_gn9_bwd_apply(int dtype, int B, int HW, int wc, int gc, c
 }
 
 #define BN_APPLY_LAUNCH(ACT, RES, FIN)                                                                                   \
-  do { if (sscale) bn_apply_kernel<T, V, ACT, RES, FIN, true><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f, sscale, ds_hw); \
-       else bn_apply_kernel<T, V, ACT, RES, FIN><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f, nullptr, 1); } while (0)
+  do { if (sscale) bn_apply_kernel<T, V, ACT, RES, FIN, true><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f, sscale, ds_hw, \
+                                                                                               nullptr, 0); \
+       else bn_apply_kernel<T, V, ACT, RES, FIN><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f, nullptr, 1, nullptr, 0); } while (0)
+#define BN_APPLY_MASK_LAUNCH()                                                                                           \
+  do { if (sscale) bn_apply_kernel<T, V, 1, true, true, true, true><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f, sscale, \
+                                                                                                     ds_hw, mp, mld); \
+       else bn_apply_kernel<T, V, 1, true, true, false, true><<<NT_GRID, NT_THREADS, 0, st>>>(xp, rp, scp, shp, yp, g, f, nullptr, 1, \
+                                                                                               mp, mld); } while (0)
+// C % 8 == 0 and every column chunk starts on a mask byte: the geometry the 1-bit mask kernels need
+static bool mask_geo_ok(int C, int vec) {
+  const int cw = col_chunk(C, vec);
+  return C % 8 == 0 && cw && cw % 8 == 0;
+}
 static int bn_apply_impl(const char* what, int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
-                         const float* shift, int relu, void* y, const BnFin* fin, const float* sscale, void* stream) {
+                         const float* shift, int relu, void* y, const BnFin* fin, const float* sscale, void* stream,
+                         unsigned char* mask = nullptr) {
   if (dtype == COTB200_F64) { set_error("%s: fp64 not supported", what); return COTB200_EDTYPE; }
   const int ds_hw = HW;           // rows per sample: the sample of flattened row r is r / ds_hw
+  const int mld = C / 8;          // mask row pitch (bytes)
   { const long long rows = (long long)B * HW; if (rows > 2147483647LL) { set_error("%s: too many rows", what); return COTB200_ETOOBIG; }
     HW = (int)rows; B = 1; }      // per-channel affine: flatten [B, HW] -> rows
   cudaStream_t st = (cudaStream_t)stream;
@@ -974,12 +1029,14 @@ static int bn_apply_impl(const char* what, int dtype, int B, int HW, int C, cons
       const int vec = pick_vec<T>(C, x, res, y);
       const int cw = col_chunk(C, vec);
       if (!cw) { set_error("%s: cannot tile %d channels", what, C); return COTB200_EINVAL; }
+      if (mask && !mask_geo_ok(C, vec)) { set_error("%s: the 1-bit mask needs C %% 8 == 0 (C = %d)", what, C); return COTB200_EINVAL; }
       for (int c0 = 0; c0 < C; c0 += cw) {
         RowsGeo g; size_t smem;
         int rc = make_geo(g, B, HW, cw, vec, 1, &smem);
         if (rc) return rc;
         g.ld = C;
         const T* xp = (const T*)x + c0; const T* rp = res ? (const T*)res + c0 : nullptr; T* yp = (T*)y + c0;
+        unsigned char* mp = mask ? mask + c0 / 8 : nullptr;
         BnFin f{};
         if (fin) {
           f = *fin;
@@ -988,9 +1045,11 @@ static int bn_apply_impl(const char* what, int dtype, int B, int HW, int C, cons
           f.scale += c0; f.shift += c0; f.mean += c0; f.rstd += c0;
         }
         const float* scp = scale ? scale + c0 : nullptr; const float* shp = shift ? shift + c0 : nullptr;
-        COTB200_PROF_B(fin ? "bn_apply_batch" : "bn_apply", (double)B * HW * cw * (2 + (res ? 1 : 0)) * sizeof(T));
+        COTB200_PROF_B(fin ? "bn_apply_batch" : "bn_apply", (double)B * HW * (cw * (2 + (res ? 1 : 0)) * sizeof(T) + (mask ? cw / 8 : 0)));
         NT_DISPATCH_VEC(vec, {
-          if (fin) {
+          if (mask) {
+            BN_APPLY_MASK_LAUNCH();
+          } else if (fin) {
             if (relu) { if (res) BN_APPLY_LAUNCH(1, true, true); else BN_APPLY_LAUNCH(1, false, true); }
             else { if (res) BN_APPLY_LAUNCH(0, true, true); else BN_APPLY_LAUNCH(0, false, true); }
           } else {
@@ -1039,16 +1098,30 @@ extern "C" int cotb200_bn_apply_batch_ds(int dtype, int B, int HW, int C, const 
   return bn_apply_impl("bn_apply_batch_ds", dtype, B, HW, C, x, res, nullptr, nullptr, relu, y, &f, sample_scale, stream);
 }
 
+extern "C" int cotb200_bn_apply_batch_mask(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum,
+                                           const float* sq, const float* weight, const float* bias, float* running_mean,
+                                           float* running_var, float n, float eps, float momentum, int update_running, void* y,
+                                           float* scale, float* shift, float* mean, float* rstd, const float* sample_scale,
+                                           unsigned char* mask, void* stream) {
+  if (!x || !res || !y || !mask || !sum || !sq || !scale || !shift || !mean || !rstd) {
+    set_error("bn_apply_batch_mask: NULL pointer"); return COTB200_ENULL; }
+  if (update_running && (!running_mean || !running_var)) { set_error("bn_apply_batch_mask: running buffers missing"); return COTB200_ENULL; }
+  BnFin f{sum, sq, weight, bias, running_mean, running_var, n, eps, momentum, update_running, scale, shift, mean, rstd};
+  return bn_apply_impl("bn_apply_batch_mask", dtype, B, HW, C, x, res, nullptr, nullptr, 1, y, &f, sample_scale, stream, mask);
+}
+
 #define BN_BWD_SUMS_LAUNCH(ACT, DS, YP)                                                                               \
   do { if ((rc = ensure_smem(bn_bwd_sums_kernel<T, V, ACT, DS>, smem))) return rc;                                    \
        bn_bwd_sums_kernel<T, V, ACT, DS><<<NT_GRID, NT_THREADS, smem, st>>>(dp, d2p, xp, YP, scp, shp, mu + c0, rstd + c0,  \
-                                                                             sum_dz + c0, sum_dzx + c0, g, sscale, ds_hw); } while (0)
+                                                                             sum_dz + c0, sum_dzx + c0, g, sscale, ds_hw, mp, mld); } while (0)
+// relu code 3 (the 1-bit mask of cotb200_bn_apply_batch_mask) is reached through the _mask entry points only
 static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
                             const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
-                            float* sum_dz, float* sum_dzx, const float* sscale, void* stream) {
-  if (!dy || !x || !mu || !rstd || !sum_dz || !sum_dzx || (relu == 1 && !y) || (relu == 2 && (!scale || !shift))) {
+                            float* sum_dz, float* sum_dzx, const float* sscale, void* stream, const unsigned char* mask = nullptr) {
+  if (relu < 0 || relu > (mask ? 3 : 2)) { set_error("bn_bwd_sums: relu must be 0, 1 or 2"); return COTB200_EINVAL; }
+  if (!dy || !x || !mu || !rstd || !sum_dz || !sum_dzx || (relu == 1 && !y) || (relu == 2 && (!scale || !shift)) || (relu == 3 && !mask)) {
     set_error("bn_bwd_sums: NULL pointer"); return COTB200_ENULL; }
-  if (relu < 0 || relu > 2) { set_error("bn_bwd_sums: relu must be 0, 1 or 2"); return COTB200_EINVAL; }
+  const int mld = C / 8;          // mask row pitch (bytes)
   if (dtype == COTB200_F64) { set_error("bn_bwd_sums: fp64 not supported"); return COTB200_EDTYPE; }
   const int ds_hw = HW;           // rows per sample (drop-path scales)
   { const long long rows = (long long)B * HW; if (rows > 2147483647LL) { set_error("cotb200_bn_bwd_sums: too many rows"); return COTB200_ETOOBIG; }
@@ -1059,6 +1132,7 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
       const int vec = pick_vec<T>(C, dy, x, relu == 1 ? y : nullptr, dy2);
       const int cw = col_chunk(C, vec);
       if (!cw) { set_error("bn_bwd_sums: cannot tile %d channels", C); return COTB200_EINVAL; }
+      if (relu == 3 && !mask_geo_ok(C, vec)) { set_error("bn_bwd_sums: the 1-bit mask needs C %% 8 == 0 (C = %d)", C); return COTB200_EINVAL; }
       for (int c0 = 0; c0 < C; c0 += cw) {
         RowsGeo g; size_t smem;
         int rc = make_geo(g, B, HW, cw, vec, 2, &smem);
@@ -1068,13 +1142,16 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
         g.ld = C;
         const T* dp = (const T*)dy + c0; const T* xp = (const T*)x + c0; const T* yp = y ? (const T*)y + c0 : nullptr;
         const T* d2p = dy2 ? (const T*)dy2 + c0 : nullptr;
-        COTB200_PROF_B("bn_bwd_sums", (double)B * HW * cw * (2 + (relu == 1 ? 1 : 0) + (dy2 ? 1 : 0)) * sizeof(T));
+        const unsigned char* mp = relu == 3 ? mask + c0 / 8 : nullptr;
+        COTB200_PROF_B("bn_bwd_sums", (double)B * HW * (cw * (2 + (relu == 1 ? 1 : 0) + (dy2 ? 1 : 0)) * sizeof(T) + (relu == 3 ? cw / 8 : 0)));
         const float* scp = scale ? scale + c0 : nullptr; const float* shp = shift ? shift + c0 : nullptr;
         NT_DISPATCH_VEC(vec, {
           if (sscale) {
-            if (relu == 1) BN_BWD_SUMS_LAUNCH(1, true, yp); else if (relu == 2) BN_BWD_SUMS_LAUNCH(2, true, nullptr); else BN_BWD_SUMS_LAUNCH(0, true, nullptr);
+            if (relu == 1) BN_BWD_SUMS_LAUNCH(1, true, yp); else if (relu == 2) BN_BWD_SUMS_LAUNCH(2, true, nullptr);
+            else if (relu == 3) BN_BWD_SUMS_LAUNCH(3, true, nullptr); else BN_BWD_SUMS_LAUNCH(0, true, nullptr);
           } else {
-            if (relu == 1) BN_BWD_SUMS_LAUNCH(1, false, yp); else if (relu == 2) BN_BWD_SUMS_LAUNCH(2, false, nullptr); else BN_BWD_SUMS_LAUNCH(0, false, nullptr);
+            if (relu == 1) BN_BWD_SUMS_LAUNCH(1, false, yp); else if (relu == 2) BN_BWD_SUMS_LAUNCH(2, false, nullptr);
+            else if (relu == 3) BN_BWD_SUMS_LAUNCH(3, false, nullptr); else BN_BWD_SUMS_LAUNCH(0, false, nullptr);
           }
         });
         if ((rc = check_launch("bn_bwd_sums"))) return rc;
@@ -1087,16 +1164,17 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
 
 #define BN_BWD_APPLY_LAUNCH(ACT, RES, YP, DRP)                                                                         \
   do { if (sscale) bn_bwd_apply_kernel<T, V, ACT, RES, true><<<NT_GRID, NT_THREADS, 0, st>>>(dp, d2p, xp, YP, scale + c0, shp, mu + c0, \
-                                                               rstd + c0, k1, k2, inv_n, dxp, DRP, g, sscale, ds_hw);      \
+                                                               rstd + c0, k1, k2, inv_n, dxp, DRP, g, sscale, ds_hw, mp, mld); \
        else bn_bwd_apply_kernel<T, V, ACT, RES><<<NT_GRID, NT_THREADS, 0, st>>>(dp, d2p, xp, YP, scale + c0, shp, mu + c0,  \
-                                                               rstd + c0, k1, k2, inv_n, dxp, DRP, g, nullptr, 1); } while (0)
+                                                               rstd + c0, k1, k2, inv_n, dxp, DRP, g, nullptr, 1, mp, mld); } while (0)
 static int bn_bwd_apply_impl(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
                              const float* scale, const float* shift, const float* mu, const float* rstd,
                              const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres, const float* sscale,
-                             void* stream) {
-  if (!dy || !x || !scale || !mu || !rstd || !dx || (relu == 1 && !y) || (relu == 2 && !shift)) {
+                             void* stream, const unsigned char* mask = nullptr) {
+  if (relu < 0 || relu > (mask ? 3 : 2)) { set_error("bn_bwd_apply: relu must be 0, 1 or 2"); return COTB200_EINVAL; }
+  if (!dy || !x || !scale || !mu || !rstd || !dx || (relu == 1 && !y) || (relu == 2 && !shift) || (relu == 3 && !mask)) {
     set_error("bn_bwd_apply: NULL pointer"); return COTB200_ENULL; }
-  if (relu < 0 || relu > 2) { set_error("bn_bwd_apply: relu must be 0, 1 or 2"); return COTB200_EINVAL; }
+  const int mld = C / 8;          // mask row pitch (bytes)
   if (dtype == COTB200_F64) { set_error("bn_bwd_apply: fp64 not supported"); return COTB200_EDTYPE; }
   const int ds_hw = HW;           // rows per sample (drop-path scales)
   { const long long rows = (long long)B * HW; if (rows > 2147483647LL) { set_error("cotb200_bn_bwd_apply: too many rows"); return COTB200_ETOOBIG; }
@@ -1109,6 +1187,7 @@ static int bn_bwd_apply_impl(int dtype, int B, int HW, int C, const void* dy, co
       if (dy2 && ((uintptr_t)dy2 & (vec * sizeof(T) - 1))) vec = 1;
       const int cw = col_chunk(C, vec);
       if (!cw) { set_error("bn_bwd_apply: cannot tile %d channels", C); return COTB200_EINVAL; }
+      if (relu == 3 && !mask_geo_ok(C, vec)) { set_error("bn_bwd_apply: the 1-bit mask needs C %% 8 == 0 (C = %d)", C); return COTB200_EINVAL; }
       for (int c0 = 0; c0 < C; c0 += cw) {
         RowsGeo g; size_t smem;
         int rc = make_geo(g, B, HW, cw, vec, 1, &smem);
@@ -1118,11 +1197,14 @@ static int bn_bwd_apply_impl(int dtype, int B, int HW, int C, const void* dy, co
         T* dxp = (T*)dx + c0; T* drp = dres ? (T*)dres + c0 : nullptr;
         const T* d2p = dy2 ? (const T*)dy2 + c0 : nullptr;
         const float* k1 = c1 ? c1 + c0 : nullptr; const float* k2 = c2 ? c2 + c0 : nullptr;
-        COTB200_PROF_B("bn_bwd_apply", (double)B * HW * cw * (3 + (relu == 1 ? 1 : 0) + (dres ? 1 : 0) + (dy2 ? 1 : 0)) * sizeof(T));
+        const unsigned char* mp = relu == 3 ? mask + c0 / 8 : nullptr;
+        COTB200_PROF_B("bn_bwd_apply", (double)B * HW * (cw * (3 + (relu == 1 ? 1 : 0) + (dres ? 1 : 0) + (dy2 ? 1 : 0)) * sizeof(T)
+                                                         + (relu == 3 ? cw / 8 : 0)));
         const float* shp = shift ? shift + c0 : nullptr;
         NT_DISPATCH_VEC(vec, {
           if (relu == 1) { if (dres) BN_BWD_APPLY_LAUNCH(1, true, yp, drp); else BN_BWD_APPLY_LAUNCH(1, false, yp, nullptr); }
           else if (relu == 2) { if (dres) BN_BWD_APPLY_LAUNCH(2, true, nullptr, drp); else BN_BWD_APPLY_LAUNCH(2, false, nullptr, nullptr); }
+          else if (relu == 3) { if (dres) BN_BWD_APPLY_LAUNCH(3, true, nullptr, drp); else BN_BWD_APPLY_LAUNCH(3, false, nullptr, nullptr); }
           else { if (dres) BN_BWD_APPLY_LAUNCH(0, true, nullptr, drp); else BN_BWD_APPLY_LAUNCH(0, false, nullptr, nullptr); }
         });
         if ((rc = check_launch("bn_bwd_apply"))) return rc;
@@ -1179,4 +1261,20 @@ extern "C" int cotb200_bn_bwd_apply_ds(int dtype, int B, int HW, int C, const vo
                                        const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres,
                                        const float* sample_scale, void* stream) {
   return bn_bwd_apply_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, sample_scale, stream);
+}
+// ---- 1-bit ReLU mask (relu code 3): the mask cotb200_bn_apply_batch_mask wrote replaces y
+extern "C" int cotb200_bn_bwd_sums_mask(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x,
+                                        const unsigned char* mask, const float* mu, const float* rstd, float* sum_dz, float* sum_dzx,
+                                        const float* sample_scale, void* stream) {
+  if (!mask) { set_error("bn_bwd_sums_mask: NULL pointer"); return COTB200_ENULL; }
+  return bn_bwd_sums_impl(dtype, B, HW, C, dy, dy2, x, nullptr, nullptr, nullptr, mu, rstd, 3, sum_dz, sum_dzx, sample_scale, stream,
+                          mask);
+}
+extern "C" int cotb200_bn_bwd_apply_mask(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x,
+                                         const unsigned char* mask, const float* scale, const float* mu, const float* rstd,
+                                         const float* c1, const float* c2, float inv_n, void* dx, void* dres, const float* sample_scale,
+                                         void* stream) {
+  if (!mask) { set_error("bn_bwd_apply_mask: NULL pointer"); return COTB200_ENULL; }
+  return bn_bwd_apply_impl(dtype, B, HW, C, dy, dy2, x, nullptr, scale, nullptr, mu, rstd, c1, c2, inv_n, 3, dx, dres, sample_scale,
+                           stream, mask);
 }

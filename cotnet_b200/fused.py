@@ -10,10 +10,25 @@ They turn the reference block's long eager chains into a few HBM passes while ke
 
 All tensors are channels_last (NHWC memory); math is fp32; outputs keep the input dtype.
 """
+import os as _os
+
 import torch
 from torch.autograd import Function
 
 from . import _lib
+
+#: ReLU mask of the BatchNorm backward without reading y back (on by default; COTB200_BN_MASK=0 restores the y-reading path):
+#: with a residual the forward also writes a 1-bit mask (relu code 3), without one the wgmma functions recompute it from their
+#: own pre-activation and scale/shift (relu code 2).  Bit-identical either way; read at call time so tests can flip it.
+BN_MASK = _os.environ.get("COTB200_BN_MASK", "1") != "0"
+
+
+def _relu_mask_buf(x):
+    """[B*H*W, C/8] uint8 for the 1-bit ReLU mask of x's BatchNorm output, or None when the mask path does not apply."""
+    B, C, H, W = x.shape
+    if not BN_MASK or C % 8:
+        return None
+    return torch.empty(B * H * W, C // 8, dtype=torch.uint8, device=x.device)
 
 
 class _ZeroArena:
@@ -175,10 +190,11 @@ def _bn_batch_stats(x, bn, weight, bias, lib, st, dt):
     return _bn_prepare(bn, weight, bias, C, float(B * H * W), None, x.device, st), False
 
 
-def _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds=None):
+def _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds=None, mask=None):
     """Training-mode BatchNorm tail shared by BNActFn and the wgmma functions: ONE kernel finalises the batch statistics
     (sums = [2, C] column sums over the B*H*W rows of x), updates the running buffers and applies scale/shift(+res)(+ReLU).
     ds: None or the [B] fp32 per-sample drop-path scales applied to the BatchNorm output before the residual add.
+    mask: None or the uint8 buffer of _relu_mask_buf (relu and res required) that receives the 1-bit ReLU mask of y.
     Returns ss = [4, C] (scale, shift, mean, rstd) for the backward."""
     B, C, H, W = x.shape
     ss = torch.empty(4, C, dtype=torch.float32, device=x.device)
@@ -188,7 +204,11 @@ def _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds=Non
     args = (dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), sums[0].data_ptr(), sums[1].data_ptr(), _lib.ptr(w32), _lib.ptr(b32),
             _lib.ptr(rm), _lib.ptr(rv), float(B * H * W), float(bn.eps), float(mom), 1 if update else 0, 1 if relu else 0,
             y.data_ptr(), ss[0].data_ptr(), ss[1].data_ptr(), ss[2].data_ptr(), ss[3].data_ptr())
-    if ds is None:
+    if mask is not None:
+        assert relu and res is not None
+        margs = args[:16] + args[17:]          # the mask form has no relu argument: it is always ReLU
+        _lib.check(lib.cotb200_bn_apply_batch_mask(*margs, _lib.ptr(ds), mask.data_ptr(), st), "bn_apply_batch_mask")
+    elif ds is None:
         _lib.check(lib.cotb200_bn_apply_batch(*args, st), "bn_apply_batch")
     else:
         _lib.check(lib.cotb200_bn_apply_batch_ds(*args, ds.data_ptr(), st), "bn_apply_batch_ds")
@@ -206,7 +226,18 @@ def _drop_scale(ds, x):
 
 
 def _bn_bwd(lib, dt, B, HW, C, dy, dy2, x, y, scale, shift, mean, rstd, rcode, sums, batch, inv_n, dx, dres, ds, st):
-    """BatchNorm backward (sums + apply) of the plain / two-gradient form, or of the drop-path form when ds is given."""
+    """BatchNorm backward (sums + apply) of the plain / two-gradient form, or of the drop-path form when ds is given.
+    rcode 3: `y` is the 1-bit ReLU mask of _bn_apply_batch(mask=...)."""
+    if rcode == 3:
+        if sums is not None:
+            _lib.check(lib.cotb200_bn_bwd_sums_mask(dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), y.data_ptr(),
+                                                    mean.data_ptr(), rstd.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(),
+                                                    _lib.ptr(ds), st), "bn_bwd_sums_mask")
+        _lib.check(lib.cotb200_bn_bwd_apply_mask(dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), y.data_ptr(), scale.data_ptr(),
+                                                 mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
+                                                 _lib.ptr(sums[1]) if batch else None, inv_n, dx.data_ptr(), _lib.ptr(dres), _lib.ptr(ds),
+                                                 st), "bn_bwd_apply_mask")
+        return
     if sums is not None:
         args = (dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), _lib.ptr(y), _lib.ptr(scale), _lib.ptr(shift),
                 mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(), sums[1].data_ptr())
@@ -240,10 +271,12 @@ class BNActFn(Function):
         ds = _drop_scale(drop_scale, x)
         y = torch.empty_like(x, memory_format=torch.channels_last)
         batch = bool(bn.training or bn.running_mean is None)
+        mask = None
         if batch:       # training: column sums, then ONE kernel that finalises the statistics in its prologue and applies them
             sums = _zeros((2, C,), x.device)
             _lib.check(lib.cotb200_col_stats(dt, B, H * W, C, x.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(), st), "col_stats")
-            ss = _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds)   # [4,C]: scale, shift, mean, rstd
+            mask = _relu_mask_buf(x) if (relu and res is not None) else None
+            ss = _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds, mask)   # [4,C]: scale, shift, mean, rstd
         else:
             ss = _bn_prepare(bn, weight, bias, C, float(B * H * W), None, x.device, st)
             args = (dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), ss[0].data_ptr(), ss[1].data_ptr(), 1 if relu else 0, y.data_ptr())
@@ -251,24 +284,24 @@ class BNActFn(Function):
                 _lib.check(lib.cotb200_bn_apply(*args, st), "bn_apply")
             else:
                 _lib.check(lib.cotb200_bn_apply_ds(*args, ds.data_ptr(), st), "bn_apply_ds")
-        # ReLU mask in the backward: with a residual it must come from y; without one it is recomputed from x and the
-        # forward's own scale/shift (relu code 2) and y is neither saved nor read
-        ctx.save_for_backward(x, y if (relu and res is not None) else None, ss, ds)
-        ctx.cfg = (relu, batch, res is not None, weight.dtype, bias.dtype)
+        # ReLU mask in the backward: with a residual it comes from the 1-bit mask the forward wrote (relu code 3) or from y;
+        # without one it is recomputed from x and the forward's own scale/shift (relu code 2) and y is neither saved nor read
+        rcode = 0 if not relu else (2 if res is None else (3 if mask is not None else 1))
+        ctx.save_for_backward(x, mask if rcode == 3 else (y if rcode == 1 else None), ss, ds)
+        ctx.cfg = (rcode, batch, res is not None, weight.dtype, bias.dtype)
         if fork:            # two aliases of ONE tensor: each consumer's gradient reaches backward() separately (see _two_grads)
             return y, y.detach()
         return y
 
     @staticmethod
     def backward(ctx, *grads):
-        x, y, ss, ds = ctx.saved_tensors
-        relu, batch, has_res, wdt, bdt = ctx.cfg
+        x, y, ss, ds = ctx.saved_tensors          # y: the forward output (rcode 1), its 1-bit ReLU mask (rcode 3) or None
+        rcode, batch, has_res, wdt, bdt = ctx.cfg
         B, C, H, W = x.shape
         lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.dtype_code(x)
         dy, dy2 = _two_grads(grads)
         if dy is None:
             return (None,) * 8
-        rcode = 0 if not relu else (1 if y is not None else 2)
         sums = None
         if batch or ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
             sums = _zeros_esc((2, C,), x.device)       # escapes as dgamma/dbeta
@@ -724,7 +757,6 @@ def split_attn_tail(u, bn0: torch.nn.BatchNorm2d, fc1, bn1, fc2):
 #   weight grad  : 1x1: the MN-major wgmma kernel (tc_wgrad.cu); the grouped 3x3 still goes through cuDNN
 # ====================================================================================================================
 from . import tc as _tc  # noqa: E402
-import os as _os  # noqa: E402
 
 
 def _rows2d(t):
@@ -777,8 +809,9 @@ class TcConv1x1Fn(Function):
         b1, b2 = wb[:, :K1], (wb[:, K1:] if K2 else None)
         out = torch.empty((B, N, H, W), dtype=torch.bfloat16, device=a1.device, memory_format=torch.channels_last)
         out2d = _rows2d(out)
-        pre = scale = mean = rstd = None
+        pre = scale = shift = mean = rstd = mask = None
         batch = False
+        rcode = 1 if relu else 0                 # ReLU mask of the backward: read from `out` unless the batch path below avoids it
         if bn is None:
             _tc.gemm_bf16(a1, b1, a2, b2, shift=None if cbias is None else cbias.detach().float().contiguous(), relu=relu, out=out2d)
         elif bn.training or bn.running_mean is None:
@@ -786,7 +819,10 @@ class TcConv1x1Fn(Function):
             sums = _zeros((2, N,), a1.device)
             pre = torch.empty_like(out, memory_format=torch.channels_last)
             _tc.gemm_bf16(a1, b1, a2, b2, stats=(sums[0], sums[1]), out=_rows2d(pre))
-            ss = _bn_apply_batch(pre, None if res is None else res.detach(), sums, bn, bn_w, bn_b, relu, out, lib, st, dt, ds)
+            if relu and BN_MASK:                 # 1-bit mask with a residual, recomputed from pre (code 2) without one
+                mask = _relu_mask_buf(pre) if res is not None else None
+                rcode = 3 if mask is not None else (2 if res is None else 1)
+            ss = _bn_apply_batch(pre, None if res is None else res.detach(), sums, bn, bn_w, bn_b, relu, out, lib, st, dt, ds, mask)
             scale, shift, mean, rstd = ss[0], ss[1], ss[2], ss[3]
         else:
             scale, shift, mean, rstd = _bn_eval_fold(bn, bn_w, bn_b)
@@ -805,8 +841,9 @@ class TcConv1x1Fn(Function):
         if need_bwd and bn is not None and pre is None:      # eval-mode module under grad: BN backward needs the raw conv output
             pre = torch.empty_like(out, memory_format=torch.channels_last)
             _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(pre))
-        ctx.save_for_backward(a1, a2, wb, pre, out if relu else None, scale, mean, rstd, ds)
-        ctx.cfg = (relu, batch, bn is not None, cbias is not None, weight.dtype, weight.shape,
+        ctx.save_for_backward(a1, a2, wb, pre, mask if rcode == 3 else (out if rcode == 1 else None), scale,
+                              shift if rcode == 2 else None, mean, rstd, ds)
+        ctx.cfg = (relu, rcode, batch, bn is not None, cbias is not None, weight.dtype, weight.shape,
                    None if bn_w is None else bn_w.dtype, None if cbias is None else cbias.dtype, K1, K2, res is not None)
         if fork:
             assert bn is not None, "fork needs the BatchNorm form (the sum of the two gradients happens in its backward kernels)"
@@ -815,8 +852,8 @@ class TcConv1x1Fn(Function):
 
     @staticmethod
     def _bwd(ctx, grads):
-        a1, a2, wb, pre, y, scale, mean, rstd, ds = ctx.saved_tensors
-        relu, batch, has_bn, has_bias, wdt, wshape, bndt, cbdt, K1, K2, has_res = ctx.cfg
+        a1, a2, wb, pre, y, scale, shift, mean, rstd, ds = ctx.saved_tensors     # y: output (rcode 1), 1-bit mask (rcode 3) or None
+        relu, rcode, batch, has_bn, has_bias, wdt, wshape, bndt, cbdt, K1, K2, has_res = ctx.cfg
         dy, dy2 = _two_grads(grads)
         if dy is None:
             return (None,) * 10
@@ -829,8 +866,7 @@ class TcConv1x1Fn(Function):
             if has_res and ctx.needs_input_grad[8]:
                 dres = torch.empty_like(dy, memory_format=torch.channels_last)
             dpre = torch.empty_like(dy, memory_format=torch.channels_last)
-            _bn_bwd(lib, dt, B, H * W, N, dy, dy2, pre, y, scale, None, mean, rstd, 1 if relu else 0, sums, batch, 1.0 / M, dpre, dres,
-                    ds, st)
+            _bn_bwd(lib, dt, B, H * W, N, dy, dy2, pre, y, scale, shift, mean, rstd, rcode, sums, batch, 1.0 / M, dpre, dres, ds, st)
             dgamma, dbeta = sums[1].to(bndt), sums[0].to(bndt)
         else:
             dpre = dy if not relu else dy * (y > 0)
@@ -901,27 +937,30 @@ class TcConv3x3Fn(Function):
             _tc.conv3x3_bf16(x, wp, bnt, scale=scale, shift=shift, relu=relu, out=out)
             if any(ctx.needs_input_grad):
                 pre = _tc.conv3x3_bf16(x, wp, bnt)
-        ctx.save_for_backward(x, weight.detach(), pre, out if relu else None, scale, mean, rstd)
-        ctx.cfg = (relu, batch, groups, bn_w.dtype)
+        # ReLU mask of the backward: recomputed from pre and the apply kernel's own scale/shift (code 2) in training; the eval
+        # output comes out of the convolution's epilogue (fp32 accumulator, not the stored pre), so there it is read from `out`
+        rcode = 0 if not relu else (2 if (batch and BN_MASK) else 1)
+        ctx.save_for_backward(x, weight.detach(), pre, out if rcode == 1 else None, scale, shift if rcode == 2 else None, mean, rstd)
+        ctx.cfg = (rcode, batch, groups, bn_w.dtype)
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, pre, y, scale, mean, rstd = ctx.saved_tensors
-        relu, batch, groups, bndt = ctx.cfg
+        x, weight, pre, y, scale, shift, mean, rstd = ctx.saved_tensors
+        rcode, batch, groups, bndt = ctx.cfg
         B, C, H, W = x.shape
         M = B * H * W
         lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.BF16
         dy = dy.contiguous(memory_format=torch.channels_last)
         sums = _zeros_esc((2, C,), x.device)          # escapes as dgamma/dbeta
         _lib.check(lib.cotb200_bn_bwd_sums(dt, B, H * W, C, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                           None, mean.data_ptr(), rstd.data_ptr(), 1 if relu else 0, sums[0].data_ptr(),
+                                           _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(),
                                            sums[1].data_ptr(), st),
                    "bn_bwd_sums")
         dpre = torch.empty_like(dy, memory_format=torch.channels_last)
         _lib.check(lib.cotb200_bn_bwd_apply(dt, B, H * W, C, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                            None, mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
-                                            _lib.ptr(sums[1]) if batch else None, 1.0 / M, 1 if relu else 0,
+                                            _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
+                                            _lib.ptr(sums[1]) if batch else None, 1.0 / M, rcode,
                                             dpre.data_ptr(), None, st), "bn_bwd_apply")
         dx = dw = None
         if ctx.needs_input_grad[0]:
@@ -964,26 +1003,28 @@ class StemConvBNFn(Function):
                 raise RuntimeError("cotb200 stem7x7s2: geometry not supported")
             if any(ctx.needs_input_grad):
                 pre = _tc.stem7x7s2_bf16(xd, wm)
-        ctx.save_for_backward(xd, weight.detach(), pre, out if relu else None, scale, mean, rstd, scratch)
-        ctx.cfg = (relu, batch, bn_w.dtype)
+        rcode = 0 if not relu else (2 if (batch and BN_MASK) else 1)    # as in TcConv3x3Fn
+        ctx.save_for_backward(xd, weight.detach(), pre, out if rcode == 1 else None, scale, shift if rcode == 2 else None, mean, rstd,
+                              scratch)
+        ctx.cfg = (rcode, batch, bn_w.dtype)
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, pre, y, scale, mean, rstd, scratch = ctx.saved_tensors
-        relu, batch, bndt = ctx.cfg
+        x, weight, pre, y, scale, shift, mean, rstd, scratch = ctx.saved_tensors
+        rcode, batch, bndt = ctx.cfg
         B, N, Ho, Wo = dy.shape
         M = B * Ho * Wo
         lib, st, dt = _lib.load(), _lib.stream_ptr(dy), _lib.BF16
         dy = dy.contiguous(memory_format=torch.channels_last)
         sums = _zeros_esc((2, N,), dy.device)          # escapes as dgamma/dbeta
         _lib.check(lib.cotb200_bn_bwd_sums(dt, B, Ho * Wo, N, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                           None, mean.data_ptr(), rstd.data_ptr(), 1 if relu else 0, sums[0].data_ptr(),
+                                           _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(),
                                            sums[1].data_ptr(), st), "bn_bwd_sums")
         dpre = torch.empty_like(dy, memory_format=torch.channels_last)
         _lib.check(lib.cotb200_bn_bwd_apply(dt, B, Ho * Wo, N, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                            None, mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
-                                            _lib.ptr(sums[1]) if batch else None, 1.0 / M, 1 if relu else 0,
+                                            _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
+                                            _lib.ptr(sums[1]) if batch else None, 1.0 / M, rcode,
                                             dpre.data_ptr(), None, st), "bn_bwd_apply")
         dx = dw = None
         wq = weight.to(dpre.dtype)

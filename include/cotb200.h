@@ -231,6 +231,22 @@ int cotb200_bn_bwd_apply_ds(int dtype, int B, int HW, int C, const void* dy, con
                             const float* scale, const float* shift, const float* mu, const float* rstd, const float* c1,
                             const float* c2, float inv_n, int relu, void* dx, void* dres, const float* sample_scale,
                             void* stream);
+/* 1-bit ReLU mask for BatchNorms with a residual input (relu code 3).  With a residual the mask cannot be recomputed from x
+ * (code 2), and reading y back costs two full passes of the widest tensors of the bottleneck.  The training-mode apply writes,
+ * next to y, mask [B*HW, C/8] bytes: bit c%8 of byte c/8 of a row = [y > 0] of the STORED y (so the mask equals relu code 1's
+ * bit for bit); the backward kernels read the mask instead of y (C/8 bytes per row instead of C elements).  Needs C % 8 == 0.
+ * Otherwise these are cotb200_bn_apply_batch_ds (relu = 1, res required), cotb200_bn_bwd_sums_ds and cotb200_bn_bwd_apply_ds:
+ * dy2 and sample_scale may be NULL. */
+int cotb200_bn_apply_batch_mask(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum, const float* sq,
+                                const float* weight, const float* bias, float* running_mean, float* running_var, float n,
+                                float eps, float momentum, int update_running, void* y, float* scale, float* shift,
+                                float* mean, float* rstd, const float* sample_scale, unsigned char* mask, void* stream);
+int cotb200_bn_bwd_sums_mask(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x,
+                             const unsigned char* mask, const float* mu, const float* rstd, float* sum_dz, float* sum_dzx,
+                             const float* sample_scale, void* stream);
+int cotb200_bn_bwd_apply_mask(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x,
+                              const unsigned char* mask, const float* scale, const float* mu, const float* rstd, const float* c1,
+                              const float* c2, float inv_n, void* dx, void* dres, const float* sample_scale, void* stream);
 /* One launch for the BatchNorm bookkeeping: from the column sums of cotb200_col_stats (or a GEMM epilogue) compute
  * scale = gamma*rstd, shift = beta - mean*scale, mean, rstd, and update running_mean / running_var like nn.BatchNorm2d
  * (momentum, unbiased variance).  use_batch = 0: eval mode, statistics read from the running buffers. */
