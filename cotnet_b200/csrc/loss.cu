@@ -6,6 +6,9 @@
 // with off = smoothing/K, on = 1 - smoothing + off.  One CTA per row (two passes over the row, the second from L1/L2), then one
 // CTA adds the B row losses in a fixed order: the loss is bit-identical from run to run.  lam = mix->target_lam is read from
 // device memory so that a captured graph follows every step's Mixup / CutMix draw.
+//
+// Also the validation metric: top-k hit counts (utils/meters.py:12-19 accuracy(), evaler/evaler.py:37-57) accumulated as int64
+// on the device, one warp per row, so that a captured eval graph needs no host synchronisation per batch.
 #include "common.cuh"
 
 namespace cotb200 {
@@ -95,6 +98,64 @@ static int soft_ce_check(const char* what, int dtype, int B, int K, const void* 
   return 0;
 }
 
+// ---------------------------------------------------------------- top-k hits
+static constexpr int TK_THREADS = 256;               // 8 warps = 8 rows per CTA
+static constexpr int TK_MAX_K = 4;
+
+struct TopkKs { int k[TK_MAX_K]; };
+
+// rank(b) = #{c : z_c > z_y} + #{c < y : z_c == z_y}; row b is a hit at k iff rank < k.  Without ties this is the position of
+// the label in a descending sort, i.e. what output.topk(k) + eq counts; ties go to the lower class index.  A NaN label logit is
+// a miss (no comparison with it holds, so it is tested explicitly); NaN competitors never outrank.  The row's warp streams its K
+// logits once; per CTA the counters are added in shared memory, then one integer atomic per counter: exact in any order.
+template <typename T>
+__global__ void __launch_bounds__(TK_THREADS)
+topk_hits_kernel(const T* __restrict__ z, long long ld, const long long* __restrict__ labels, const int* __restrict__ valid_dev,
+                 int B, int K, int nk, TopkKs ks, unsigned long long* __restrict__ counts) {
+  __shared__ unsigned sm[TK_THREADS / 32][TK_MAX_K + 2];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int b = blockIdx.x * (TK_THREADS / 32) + warp;
+  const int nvalid = valid_dev ? min(max(__ldg(valid_dev), 0), B) : B;
+  unsigned hit[TK_MAX_K] = {}, counted = 0, bad = 0;
+  if (b < nvalid) {
+    counted = 1;
+    const long long y = __ldg(labels + b);
+    if (y < 0 || y >= K) {
+      bad = 1;
+    } else {
+      const T* zr = z + (long long)b * ld;
+      const int yi = (int)y;
+      const float zy = to_acc(zr[yi]);
+      if (zy == zy) {
+        int r = 0;
+#pragma unroll 4
+        for (int c = lane; c < K; c += 32) {
+          const float x = to_acc(zr[c]);
+          r += (x > zy) | ((x == zy) & (c < yi));
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
+#pragma unroll
+        for (int i = 0; i < TK_MAX_K; ++i) hit[i] = (i < nk && r < ks.k[i]) ? 1u : 0u;
+      }
+    }
+  }
+  if (lane == 0) {                                   // sm row: hits@k for the nk values of k, rows counted, bad labels
+#pragma unroll
+    for (int i = 0; i < TK_MAX_K; ++i) sm[warp][i] = hit[i];
+    sm[warp][TK_MAX_K] = counted;
+    sm[warp][TK_MAX_K + 1] = bad;
+  }
+  __syncthreads();
+  if (threadIdx.x < nk + 2) {                        // counts[j] for j < nk from slot j, counts[nk], counts[nk + 1] from the last two
+    const int j = threadIdx.x, slot = j < nk ? j : TK_MAX_K + (j - nk);
+    unsigned s = 0;
+#pragma unroll
+    for (int w = 0; w < TK_THREADS / 32; ++w) s += sm[w][slot];
+    if (s) atomicAdd(counts + j, (unsigned long long)s);
+  }
+}
+
 }  // namespace cotb200
 
 using namespace cotb200;
@@ -132,6 +193,30 @@ extern "C" int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, 
       COTB200_PROF_B("soft_ce_bwd", (double)B * K * (sizeof(T) + 4));
       soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, mix, B, K, off, onoff, rows, dloss, dz, ldz);
       return check_launch("soft_ce_bwd");
+    }
+  });
+  return 0;
+}
+
+extern "C" int cotb200_topk_hits(int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
+                                 const int* valid_dev, int nk, const int* ks, long long* counts_dev, void* stream) {
+  if (!logits || !labels || !ks || !counts_dev) { set_error("topk_hits: NULL pointer"); return COTB200_ENULL; }
+  if (B <= 0 || K <= 0 || ld < K) { set_error("topk_hits: bad dims B=%d K=%d ld=%lld", B, K, ld); return COTB200_EINVAL; }
+  if (nk < 1 || nk > TK_MAX_K) { set_error("topk_hits: %d values of k (1..%d supported)", nk, TK_MAX_K); return COTB200_EINVAL; }
+  TopkKs kk = {};
+  for (int i = 0; i < nk; ++i) {
+    if (ks[i] < 1 || ks[i] > K) { set_error("topk_hits: k=%d outside 1..K=%d", ks[i], K); return COTB200_EINVAL; }
+    kk.k[i] = ks[i];
+  }
+  if (dtype == COTB200_F64) { set_error("topk_hits: fp64 not supported"); return COTB200_EDTYPE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = (B + TK_THREADS / 32 - 1) / (TK_THREADS / 32);
+  COTB200_DISPATCH_DTYPE(dtype, {
+    if constexpr (!std::is_same<T, double>::value) {
+      COTB200_PROF_B("topk_hits", (double)B * K * sizeof(T));
+      topk_hits_kernel<T><<<grid, TK_THREADS, 0, st>>>((const T*)logits, ld, labels, valid_dev, B, K, nk, kk,
+                                                       reinterpret_cast<unsigned long long*>(counts_dev));
+      return check_launch("topk_hits");
     }
   });
   return 0;

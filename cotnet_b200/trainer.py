@@ -486,6 +486,38 @@ class TrainStep:
             out[n] = e
         return out
 
+    def distribute_bn(self, reduce=True, ema=True):
+        """The reference's end-of-epoch distribute_bn (utils/distributed.py:57-67; train.py:346-352), for the model and, with
+        `ema`, again for the EMA copies of its buffers: every buffer whose name contains running_mean / running_var is averaged
+        over the ranks (`reduce`: SUM, then / float(world), the reference's arithmetic) or broadcast from rank 0.  All of them
+        travel in ONE flat fp32 collective and are copied back into the original tensors, whose storage does not move (the EMA
+        lerp table and captured graphs hold their pointers).  num_batches_tracked is untouched.  Nothing happens at world 1."""
+        if self.world <= 1:
+            return
+        names = [n for n, _ in self.model.named_buffers()]
+        pick = [i for i, n in enumerate(names) if "running_mean" in n or "running_var" in n]
+        bufs = list(self.model.buffers())
+        sel = [bufs[i] for i in pick]
+        if ema and self.ema:
+            sel += [self.ema_buffers[i] for i in pick]
+        if not sel:
+            return
+        bad = [names[i] for i in pick if bufs[i].dtype != torch.float32]
+        if bad:
+            raise TypeError("distribute_bn: running statistics must be fp32 (%s)" % ", ".join(bad[:3]))
+        with torch.no_grad():
+            flat = torch.cat([b.reshape(-1) for b in sel])
+            if reduce:
+                dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=self.pg)
+                flat /= float(self.world)
+            else:
+                dist.broadcast(flat, src=0 if self.pg is None else dist.get_global_rank(self.pg, 0), group=self.pg)
+            off = 0
+            for b in sel:
+                n = b.numel()
+                b.copy_(flat[off:off + n].view_as(b))
+                off += n
+
     def grads(self):
         """name -> gradient view into the flat buckets (after forward_backward / a step)."""
         out = {}

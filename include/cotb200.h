@@ -437,6 +437,18 @@ int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long l
                         const cotb200_mix* mix, float smoothing, const float* rows, const float* dloss, float* dz,
                         long long ldz, void* stream);
 
+/* ---- validation metric ----
+ * Top-k hit counts of utils/meters.py:12-19 (accuracy(): output.topk(maxk) then eq), accumulated on the device so that a
+ * captured eval graph needs no host synchronisation per batch.  logits: fp32 / bf16 / fp16 [B, K] with row pitch ld; labels
+ * int64 [B].  Rank rule: rank(b) = #{c : z_c > z_y} + #{c < y : z_c == z_y}; row b is a hit at k iff rank(b) < k.  On rows
+ * without ties this equals accuracy(); on tied rows the lower class index wins (torch's topk order there is unspecified).  A
+ * NaN label logit is a miss; NaN competitors never outrank.  Only rows b < *valid_dev count (valid_dev: device int, clamped to
+ * [0, B]; NULL = all B rows), so a captured graph takes a short last batch.  ks: HOST array of nk (1..4) values, each in 1..K.
+ * counts_dev: int64 [nk + 2], ACCUMULATED (+=): hits at each k, rows counted, rows whose label is outside [0, K) (a miss).
+ * Integer sums: exact and independent of order. */
+int cotb200_topk_hits(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, const int* valid_dev,
+                      int nk, const int* ks, long long* counts_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
