@@ -116,6 +116,8 @@ SYMBOLS = {
                                                                  ctypes.c_longlong, _VP]),
     "cotb200_topk_hits": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int),
                                                                _VP, _VP]),
+    "cotb200_aug_resize_crop": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP, ctypes.c_longlong, _VP, _VP, _VP, ctypes.c_longlong, _VP, _VP]),
+    "cotb200_aug_randaug": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP] * 4),
 }
 
 

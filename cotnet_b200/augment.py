@@ -1,0 +1,303 @@
+"""The reference's image augmentation on the GPU, byte-equal to its PIL pipeline given the same random draws.
+
+DataLoader workers still decode (JPEG -> RGB uint8 HWC, the reference dataset's ``.convert('RGB')``).  From there:
+
+* ``TrainAugment``: RandomResizedCrop(scale, ratio, interpolation) + RandomHorizontalFlip(0.5) + RandAugment
+  (``rand-m15-mstd0.5-n2`` and its hyper-parameters, datasets/transforms_factory.py:44-129).  ``draw`` consumes a
+  ``random.Random``, an ``np.random.RandomState`` and a torch CPU ``Generator`` in the reference's call order, so a seeded draw
+  equals what the reference's transforms draw from the global generators; ``collate`` does that inside DataLoader workers
+  and packs the batch into one ragged buffer; ``__call__`` runs the kernels (cotb200_aug_resize_crop, cotb200_aug_randaug)
+  and returns the uint8 NCHW batch that fast_collate builds, ready for ``normalize_u8(mix=MixupCutmix.draw(...))``.
+* ``EvalTransform``: Resize(floor(size / crop_pct)) + CenterCrop(size) (:132-166) on the same resize kernel.
+
+oracle/aug_ref.py restates every step in numpy; tests/golden/augment.npz holds the reference's own outputs.
+"""
+import ctypes
+import math
+import re
+from collections import namedtuple
+
+import numpy as np
+import torch
+
+from . import _lib
+
+BILINEAR, BICUBIC = 0, 1
+#: op ids: the positions in the reference's _RAND_TRANSFORMS (the `op` of struct cotb200_aug_op)
+OPS = ("AutoContrast", "Equalize", "Invert", "Rotate", "Posterize", "Solarize", "SolarizeAdd", "Color", "Contrast",
+       "Brightness", "Sharpness", "ShearX", "ShearY", "TranslateX", "TranslateY", "Cutout")
+AFFINE_OPS = (3, 11, 12, 13, 14)
+MAX_LEVEL = 10.          # rand_augment.py _MAX_LEVEL (level -> argument scale)
+MAG_CLIP = 15            # AugmentOp.MAX_LEVEL (magnitude clip)
+
+_OP_DTYPE = np.dtype([("op", "<i4"), ("filter", "<i4"), ("v", "<i4", (4,)), ("factor", "<f4"), ("pad_", "<i4"),
+                      ("m", "<f8", (6,))], align=True)
+#: struct cotb200_aug_sample (include/cotb200.h)
+SAMPLE_DTYPE = np.dtype([("offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("ci", "<i4"), ("cj", "<i4"), ("ch", "<i4"),
+                         ("cw", "<i4"), ("rh", "<i4"), ("rw", "<i4"), ("oi", "<i4"), ("oj", "<i4"), ("filter", "<i4"),
+                         ("flip", "<i4"), ("tmp_offset", "<i8"), ("ops", _OP_DTYPE, (2,))], align=True)
+assert _OP_DTYPE.itemsize == 80 and SAMPLE_DTYPE.itemsize == 224
+
+_INTERP = {"bilinear": BILINEAR, "bicubic": BICUBIC}
+
+#: what a worker's collate hands to the main process: concatenated HWC images, the drawn parameter structs, the labels
+AugBatch = namedtuple("AugBatch", "data params labels")
+
+
+def _parse_rand(config_str):
+    """rand_augment_transform's config string -> (magnitude, num_layers, magnitude_std)."""
+    parts = config_str.split("-")
+    if parts[0] != "rand":
+        raise ValueError("only RandAugment ('rand-...') is supported, got %r" % config_str)
+    mag, n, mstd = 10, 2, 0.
+    for c in parts[1:]:
+        cs = re.split(r"(\d.*)", c)
+        if len(cs) < 2:
+            continue
+        key, val = cs[:2]
+        if key == "mstd":
+            mstd = float(val)
+        elif key == "m":
+            mag = int(val)
+        elif key == "n":
+            n = int(val)
+        elif key == "inc":
+            pass
+        else:
+            raise ValueError("RandAugment section %r is not supported" % c)
+    if n > 2:
+        raise ValueError("at most 2 RandAugment layers are supported, got %d" % n)
+    return mag, n, mstd
+
+
+def rotate_matrix(degrees, w, h):
+    """The inverse affine matrix Image.rotate(degrees) builds for a w x h image (centre (w/2, h/2), no translation)."""
+    cx, cy = w / 2, h / 2
+    angle = -math.radians(degrees % 360.0)
+    m = [round(math.cos(angle), 15), round(math.sin(angle), 15), 0.0,
+         round(-math.sin(angle), 15), round(math.cos(angle), 15), 0.0]
+    a, b, c, d, e, f = m
+    m[2], m[5] = a * -cx + b * -cy + c, d * -cx + e * -cy + f
+    m[2] += cx
+    m[5] += cy
+    return m
+
+
+def eval_geometry(H, W, size=224, crop_pct=0.875):
+    """torchvision Resize(floor(size / crop_pct)) + CenterCrop(size) of an H x W image: (resized h, resized w, top, left)."""
+    short = int(math.floor(size / crop_pct))
+    if W <= H:
+        rw, rh = short, int(short * H / W)
+    else:
+        rh, rw = short, int(short * W / H)
+    return rh, rw, int(round((rh - size) / 2.0)), int(round((rw - size) / 2.0))
+
+
+def rrc_params(H, W, scale, ratio, rnd):
+    """RandomResizedCropAndInterpolation.get_params (datasets/transforms.py:89-130) -> (i, j, h, w)."""
+    area = W * H
+    for _ in range(10):
+        target_area = rnd.uniform(*scale) * area
+        log_ratio = (math.log(ratio[0]), math.log(ratio[1]))
+        aspect_ratio = math.exp(rnd.uniform(*log_ratio))
+        w = int(round(math.sqrt(target_area * aspect_ratio)))
+        h = int(round(math.sqrt(target_area / aspect_ratio)))
+        if w <= W and h <= H:
+            i = rnd.randint(0, H - h)
+            j = rnd.randint(0, W - w)
+            return i, j, h, w
+    in_ratio = W / H
+    if in_ratio < min(ratio):
+        w = W
+        h = int(round(w / min(ratio)))
+    elif in_ratio > max(ratio):
+        h = H
+        w = int(round(h * max(ratio)))
+    else:
+        w = W
+        h = H
+    return (H - h) // 2, (W - w) // 2, h, w
+
+
+class TrainAugment:
+    """The reference's training transform (transforms_imagenet_train with use_prefetcher=True) on the GPU."""
+
+    def __init__(self, size=224, scale=(0.08, 1.0), ratio=(3. / 4., 4. / 3.), interpolation="bicubic", hflip=0.5,
+                 auto_augment="rand-m15-mstd0.5-n2", translate_const=100, cutout_const=40):
+        if interpolation != "random" and interpolation not in _INTERP:
+            raise ValueError("interpolation must be 'bilinear', 'bicubic' or 'random', got %r" % (interpolation,))
+        self.size = int(size)
+        self.scale, self.ratio = tuple(scale), tuple(ratio)
+        self.interpolation = interpolation
+        self.hflip = hflip
+        self.magnitude, self.num_layers, self.mstd = _parse_rand(auto_augment) if auto_augment else (0, 0, 0.)
+        self.translate_const, self.cutout_const = translate_const, cutout_const
+
+    def _filter(self, rnd):
+        if self.interpolation == "random":
+            return rnd.choice((BILINEAR, BICUBIC))
+        return _INTERP[self.interpolation]
+
+    def _op(self, i, rnd, nrnd):
+        """AugmentOp.__call__ of op i (rand_augment.py:287-296): the draws and the resolved argument, or None (not applied)."""
+        if rnd.random() > rnd.uniform(0.2, 0.8):
+            return None
+        mag = self.magnitude
+        if self.mstd > 0:
+            mag = rnd.gauss(mag, self.mstd)
+        mag = min(MAG_CLIP, max(0, mag))
+        name, S = OPS[i], self.size
+        op = {"id": i, "arg": 0.0}
+
+        def negate(v):
+            return -v if rnd.random() > 0.5 else v
+
+        if name == "Rotate":
+            deg = negate((mag / MAX_LEVEL) * 30.)
+            op.update(arg=deg, matrix=rotate_matrix(deg, S, S), filter=self._filter(rnd))
+        elif name in ("ShearX", "ShearY"):
+            f = negate((mag / MAX_LEVEL) * 0.3)
+            op.update(arg=f, matrix=(1, f, 0, 0, 1, 0) if name == "ShearX" else (1, 0, 0, f, 1, 0), filter=self._filter(rnd))
+        elif name in ("TranslateX", "TranslateY"):
+            t = negate((mag / MAX_LEVEL) * float(self.translate_const))
+            op.update(arg=t, matrix=(1, 0, t, 0, 1, 0) if name == "TranslateX" else (1, 0, 0, 0, 1, t), filter=self._filter(rnd))
+        elif name == "Posterize":
+            op["arg"] = op["iarg"] = int((mag / MAX_LEVEL) * 4)
+        elif name == "Solarize":
+            op["arg"] = op["iarg"] = int((mag / MAX_LEVEL) * 256)
+        elif name == "SolarizeAdd":
+            op["arg"] = op["iarg"] = int((mag / MAX_LEVEL) * 110)
+        elif name in ("Color", "Contrast", "Brightness", "Sharpness"):
+            op["arg"] = op["factor"] = (mag / MAX_LEVEL) * 1.8 + 0.1
+        elif name == "Cutout":
+            op["arg"] = px = int((mag / MAX_LEVEL) * self.cutout_const)
+            x0 = nrnd.uniform(S)            # numpy reads uniform(w) as low = w, high = 1.0; kept as the reference does
+            y0 = nrnd.uniform(S)
+            x0 = int(max(0, x0 - px))
+            y0 = int(max(0, y0 - px))
+            op["box"] = (x0, y0, min(S, x0 + 2 * px), min(S, y0 + 2 * px))
+        return op
+
+    def draw_one(self, H, W, rnd, nrnd, tgen):
+        """The draws of one H x W image as a dict (the form oracle/aug_ref.train_sample takes)."""
+        i, j, h, w = rrc_params(H, W, self.scale, self.ratio, rnd)
+        p = dict(i=i, j=j, h=h, w=w, filter=self._filter(rnd), flip=False, ops=[])
+        if self.hflip > 0:
+            p["flip"] = bool(torch.rand(1, generator=tgen) < self.hflip)
+        if self.num_layers:
+            for k in nrnd.choice(len(OPS), self.num_layers, replace=True):
+                p["ops"].append(self._op(int(k), rnd, nrnd))
+        return p
+
+    def draw(self, sizes, py_random, np_random, torch_gen):
+        """Per-sample parameters of images of `sizes` [(H, W), ...], drawn image by image in the reference's order:
+        crop, filter (interpolation 'random' only), flip, the op choice, then per op apply / magnitude / sign (/ filter) and
+        Cutout's two positions.  Returns the list of dicts; ``pack`` turns it into the device structs."""
+        return [self.draw_one(int(H), int(W), py_random, np_random, torch_gen) for H, W in sizes]
+
+    def pack(self, sizes, draws):
+        """numpy SAMPLE_DTYPE [N] of the draws (offsets of consecutive images of `sizes` in one buffer, scratch offsets)."""
+        S = self.size
+        rec = np.zeros(len(draws), SAMPLE_DTYPE)
+        off = tmp = 0
+        for n, ((H, W), p) in enumerate(zip(sizes, draws)):
+            r = rec[n]
+            r["offset"], r["h"], r["w"] = off, H, W
+            r["ci"], r["cj"], r["ch"], r["cw"] = p["i"], p["j"], p["h"], p["w"]
+            r["rh"] = r["rw"] = S
+            r["filter"], r["flip"], r["tmp_offset"] = p["filter"], int(p["flip"]), tmp
+            off += 3 * H * W
+            tmp += 3 * S * p["h"]
+            for s in range(2):
+                pack_op(r["ops"][s], p["ops"][s] if s < len(p["ops"]) else None)
+        return rec
+
+    def collate(self, batch):
+        """DataLoader collate_fn (runs in the workers): [(HWC uint8 array, label), ...] -> AugBatch of CPU tensors, drawing
+        from the worker's global `random`, `np.random` and torch generators as the reference's transforms do.  With the
+        DataLoader's pin_memory=True the main process receives it pinned."""
+        import random
+        imgs = [np.ascontiguousarray(b[0], dtype=np.uint8) for b in batch]
+        for a in imgs:
+            if a.ndim != 3 or a.shape[2] != 3:
+                raise ValueError("expected HWC RGB uint8 images, got shape %s" % (a.shape,))
+        sizes = [a.shape[:2] for a in imgs]
+        rec = self.pack(sizes, self.draw(sizes, random, np.random, torch.default_generator))
+        data = torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs]))
+        return AugBatch(data, torch.from_numpy(rec.view(np.uint8).copy()),
+                        torch.tensor([int(b[1]) for b in batch], dtype=torch.int64))
+
+    def __call__(self, batch, device=None):
+        """AugBatch -> (uint8 [N, 3, S, S] on `device`, labels on `device`), on the current stream."""
+        out = run(batch, self.size, device, randaug=self.num_layers > 0)
+        return out, batch.labels.to(out.device, non_blocking=True)
+
+
+def pack_op(dst, op):
+    dst["op"] = -1
+    if op is None:
+        return
+    i = op["id"]
+    dst["op"] = i
+    if i in AFFINE_OPS:
+        dst["m"] = op["matrix"]
+        dst["filter"] = op["filter"]
+    elif "iarg" in op:
+        dst["v"][0] = op["iarg"]
+    elif "factor" in op:
+        dst["factor"] = op["factor"]
+    elif "box" in op:
+        dst["v"] = op["box"]
+
+
+class EvalTransform:
+    """transforms_imagenet_eval (use_prefetcher=True): Resize(floor(size / crop_pct), interpolation) + CenterCrop(size)."""
+
+    def __init__(self, size=224, crop_pct=0.875, interpolation="bicubic"):
+        self.size, self.crop_pct, self.filter = int(size), crop_pct, _INTERP[interpolation]
+
+    def pack(self, sizes):
+        S = self.size
+        rec = np.zeros(len(sizes), SAMPLE_DTYPE)
+        off = tmp = 0
+        for n, (H, W) in enumerate(sizes):
+            rh, rw, top, left = eval_geometry(H, W, S, self.crop_pct)
+            r = rec[n]
+            r["offset"], r["h"], r["w"], r["ch"], r["cw"] = off, H, W, H, W
+            r["rh"], r["rw"], r["oi"], r["oj"], r["filter"], r["tmp_offset"] = rh, rw, top, left, self.filter, tmp
+            r["ops"]["op"] = -1
+            off += 3 * H * W
+            tmp += 3 * S * H
+        return rec
+
+    def collate(self, batch):
+        imgs = [np.ascontiguousarray(b[0], dtype=np.uint8) for b in batch]
+        rec = self.pack([a.shape[:2] for a in imgs])
+        data = torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs]))
+        return AugBatch(data, torch.from_numpy(rec.view(np.uint8).copy()),
+                        torch.tensor([int(b[1]) for b in batch], dtype=torch.int64))
+
+    def __call__(self, batch, device=None):
+        out = run(batch, self.size, device, randaug=False)
+        return out, batch.labels.to(out.device, non_blocking=True)
+
+
+def run(batch, S, device=None, randaug=True):
+    """The kernels on an AugBatch: H2D copies of the ragged buffer and the structs, resize-crop (+ flip), then RandAugment
+    in place.  Returns uint8 [N, 3, S, S] on `device` (default: the current CUDA device)."""
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    rec = batch.params.numpy().view(SAMPLE_DTYPE)
+    N = len(rec)
+    data = batch.data.to(device, non_blocking=True)
+    params = batch.params.to(device, non_blocking=True)
+    tmp_bytes = int((3 * S * rec["ch"].astype(np.int64)).sum())
+    tmp = torch.empty(max(tmp_bytes, 1), dtype=torch.uint8, device=device)
+    out = torch.empty(N, 3, S, S, dtype=torch.uint8, device=device)
+    lib = _lib.load()
+    st = _lib.stream_ptr(out)
+    host = rec.ctypes.data_as(ctypes.c_void_p)
+    _lib.check(lib.cotb200_aug_resize_crop(N, S, data.data_ptr(), data.numel(), host, params.data_ptr(), tmp.data_ptr(),
+                                           tmp.numel(), out.data_ptr(), st), "aug_resize_crop")
+    if randaug and (rec["ops"]["op"] >= 0).any():
+        _lib.check(lib.cotb200_aug_randaug(N, S, host, params.data_ptr(), out.data_ptr(), st), "aug_randaug")
+    return out

@@ -449,6 +449,49 @@ int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long l
 int cotb200_topk_hits(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, const int* valid_dev,
                       int nk, const int* ks, long long* counts_dev, void* stream);
 
+/* ---- image augmentation of the reference's input pipeline, byte-equal to its PIL transforms ----
+ * RandomResizedCrop + horizontal flip + RandAugment (datasets/transforms_factory.py:44-129, datasets/rand_augment.py) and the
+ * eval Resize + CenterCrop (:132-166) on a ragged batch of decoded HWC uint8 RGB images.  Every value the host draws lives in
+ * DEVICE memory (an array of cotb200_aug_sample); the host copy of the same array is only validated, so that nothing is
+ * ever read out of bounds.  Output: uint8 NCHW [N, 3, S, S], the batch fast_collate builds.
+ * One RandAugment op.  op: -1 none, else the index in the reference's _RAND_TRANSFORMS: 0 AutoContrast, 1 Equalize, 2 Invert,
+ * 3 Rotate, 4 Posterize, 5 Solarize, 6 SolarizeAdd, 7 Color, 8 Contrast, 9 Brightness, 10 Sharpness, 11 ShearX, 12 ShearY,
+ * 13 TranslateX, 14 TranslateY, 15 Cutout. */
+#define COTB200_AUG_MAX_OPS 2
+typedef struct cotb200_aug_op {
+  int op;
+  int filter;          /* affine ops (3, 11..14): 0 bilinear, 1 bicubic */
+  int v[4];            /* Posterize bits, Solarize threshold, SolarizeAdd addend in v[0]; Cutout box x0, y0, x1, y1 (ends inclusive) */
+  float factor;        /* enhance ops (7..10): the Image.blend factor, rounded to fp32 as Pillow does */
+  int pad_;
+  double m[6];         /* affine ops: Image.transform's inverse matrix (x_in = m0 x + m1 y + m2, y_in = m3 x + m4 y + m5) */
+} cotb200_aug_op;
+/* One image: the crop (ci, cj, ch, cw) of the h x w source at byte `offset` is resized to rh x rw with `filter` (0 bilinear,
+ * 1 bicubic; Pillow's two-pass resample, horizontal first, 22-bit fixed-point weights); the output is the window rows
+ * [oi, oi + S) x columns [oj, oj + S) of that, mirrored left-right when flip.  tmp_offset: this image's 3*S*ch bytes of the
+ * scratch buffer (horizontal-pass rows).  Then ops[0], ops[1] in order. */
+typedef struct cotb200_aug_sample {
+  long long offset;
+  int h, w;
+  int ci, cj, ch, cw;
+  int rh, rw;
+  int oi, oj;
+  int filter, flip;
+  long long tmp_offset;
+  cotb200_aug_op ops[COTB200_AUG_MAX_OPS];
+} cotb200_aug_sample;
+/* Resize-crop (+ flip) of N images into out [N, 3, S, S].  src: src_bytes of concatenated HWC images; tmp: tmp_bytes of scratch.
+ * params_host / params_dev: the same N samples on the host (validated) and on the device (read by the kernels).  Rejected with
+ * COTB200_EINVAL: an image smaller than 1 x 1, an offset or scratch range past its buffer, a crop or window outside its image, a
+ * bad filter; COTB200_EUNSUPPORTED: a downscale whose filter taps exceed the kernel's shared memory. */
+int cotb200_aug_resize_crop(int N, int S, const unsigned char* src, long long src_bytes, const cotb200_aug_sample* params_host,
+                            const cotb200_aug_sample* params_dev, unsigned char* tmp, long long tmp_bytes, unsigned char* out,
+                            void* stream);
+/* RandAugment ops of each sample applied in place to out [N, 3, S, S] (one CTA per image, the image held in shared memory).
+ * An unknown op id or a bad argument is rejected with COTB200_EINVAL; S above 256 with COTB200_EUNSUPPORTED. */
+int cotb200_aug_randaug(int N, int S, const cotb200_aug_sample* params_host, const cotb200_aug_sample* params_dev,
+                        unsigned char* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
