@@ -904,7 +904,7 @@ extern "C" int cotb200_gn9_stats(int dtype, int B, int HW, int wc, int gc, const
   const bool fast = gn72_ok(dtype, wc, gc, false, l, nullptr, nullptr);
   COTB200_DISPATCH_DTYPE(dtype, {
     if constexpr (!std::is_same<T, double>::value) {
-      COTB200_PROF_B("gn9_stats", (double)B * HW * J * sizeof(T));
+      COTB200_PROF_B(fast ? "gn72_stats" : "gn9_stats", (double)B * HW * J * sizeof(T));
       if (fast) return gn72_stats_launch<T>(B, HW, wc, l, lbias, gsum, gsq, st);
       const int vec = pick_vec<T>(J, l);
       RowsGeo g; size_t smem;
@@ -930,7 +930,7 @@ extern "C" int cotb200_gn9_apply(int dtype, int B, int HW, int wc, int gc, const
   const bool fast = gn72_ok(dtype, wc, gc, true, l, out, nullptr);
   COTB200_DISPATCH_DTYPE(dtype, {
     if constexpr (!std::is_same<T, double>::value) {
-      COTB200_PROF_B("gn9_apply", (double)B * HW * J * 2 * sizeof(T));
+      COTB200_PROF_B(fast ? "gn72_apply" : "gn9_apply", (double)B * HW * J * 2 * sizeof(T));
       if (fast) return gn72_apply_launch<T>(B, HW, wc, l, lbias, mean, rstd, gamma, beta, out, st);
       const int vec = pick_vec<T>(J, l, out);
       RowsGeo g; size_t smem;
@@ -956,7 +956,7 @@ extern "C" int cotb200_gn9_bwd_sums(int dtype, int B, int HW, int wc, int gc, co
     if constexpr (!std::is_same<T, double>::value) {
       int rc;
       {
-        COTB200_PROF_B("gn9_bwd_sums", (double)B * HW * J * 2 * sizeof(T));
+        COTB200_PROF_B(fast ? "gn72_bwd_sums" : "gn9_bwd_sums", (double)B * HW * J * 2 * sizeof(T));
         if (fast) {
           if ((rc = gn72_bwd_sums_launch<T>(B, HW, wc, dg, l, work, st))) return rc;
         } else {
@@ -988,7 +988,7 @@ extern "C" int cotb200_gn9_bwd_apply(int dtype, int B, int HW, int wc, int gc, c
   const bool fast = gn72_ok(dtype, wc, gc, true, dg, l, dl);
   COTB200_DISPATCH_DTYPE(dtype, {
     if constexpr (!std::is_same<T, double>::value) {
-      COTB200_PROF_B("gn9_bwd_apply", (double)B * HW * J * 3 * sizeof(T));
+      COTB200_PROF_B(fast ? "gn72_bwd_apply" : "gn9_bwd_apply", (double)B * HW * J * 3 * sizeof(T));
       if (fast) return gn72_bwd_apply_launch<T>(B, HW, wc, dg, l, lbias, mean, rstd, gamma, s1, s2, dl, st);
       const int vec = pick_vec<T>(J, dg, l, dl);
       RowsGeo g; size_t smem;
