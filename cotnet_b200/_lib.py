@@ -33,6 +33,25 @@ class Mix(ctypes.Structure):
                 ("y0", ctypes.c_int), ("y1", ctypes.c_int), ("x0", ctypes.c_int), ("x1", ctypes.c_int)]
 
 
+CLIP_NORM, CLIP_VALUE, CLIP_AGC = 1, 2, 3
+
+
+class ClipUnit(ctypes.Structure):
+    """struct cotb200_clip_unit (include/cotb200.h): one AGC unit of a flat range."""
+    _fields_ = [("offset", ctypes.c_longlong), ("numel", ctypes.c_int), ("range", ctypes.c_int)]
+
+
+class ClipSeg(ctypes.Structure):
+    """struct cotb200_clip_seg (include/cotb200.h): one warp's piece of the optimizer's flat range, with its AGC unit (-1: none)."""
+    _fields_ = [("offset", ctypes.c_longlong), ("numel", ctypes.c_int), ("unit", ctypes.c_int)]
+
+
+class Clip(ctypes.Structure):
+    """struct cotb200_clip (include/cotb200.h): the clip of one cotb200_sgd_ema_step_clip call."""
+    _fields_ = [("mode", ctypes.c_int), ("value", ctypes.c_float), ("factor", ctypes.c_void_p), ("segs", ctypes.c_void_p),
+                ("n_segs", ctypes.c_int), ("pad_", ctypes.c_int)]
+
+
 _lock = threading.Lock()
 _lib = None
 
@@ -107,6 +126,12 @@ SYMBOLS = {
     "cotb200_multi_gather": (ctypes.c_int, [_VP, _VP, ctypes.c_int, ctypes.c_int, _VP, ctypes.c_float, _VP]),
     "cotb200_sgd_ema_step": (ctypes.c_int, [ctypes.c_longlong, _VP, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP]),
     "cotb200_multi_lerp": (ctypes.c_int, [_VP, ctypes.c_int, _VP, _VP]),
+    "cotb200_clip_seg_max": (ctypes.c_int, []),
+    "cotb200_grad_norm": (ctypes.c_int, [ctypes.c_longlong, ctypes.c_int, _VP, _VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP]),
+    "cotb200_unit_norms": (ctypes.c_int, [ctypes.c_int, _VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, ctypes.c_float,
+                                          _VP, _VP, _VP]),
+    "cotb200_sgd_ema_step_clip": (ctypes.c_int, [ctypes.c_longlong, _VP, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int,
+                                                 ctypes.POINTER(Clip), _VP]),
     "cotb200_u8_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
                                           _VP, _VP, _VP]),
     "cotb200_u8_mix_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),

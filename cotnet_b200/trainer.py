@@ -75,6 +75,65 @@ def plan_flat(named_params, comm_chunks=3):
     return {"big": big, "small": small, "n_big": ob, "n_small": os_, "chunks": chunks}
 
 
+#: solver.clip_mode of the reference (utils/clip_grad.py:dispatch_clip_grad) -> the library's clip mode
+CLIP_MODES = {"norm": _lib.CLIP_NORM, "value": _lib.CLIP_VALUE, "agc": _lib.CLIP_AGC}
+
+
+def plan_clip_units(model, plan):
+    """The units of adaptive_clip_grad (utils/clip_grad.py:12-24) in the flat buckets of `plan` (plan_flat).  Like train.py:271
+    (model_parameters(model, exclude_head=True), models/helpers.py:270-273) the last two of model.parameters() -- the classifier
+    head -- are left out.  A parameter of >= 2 dims has one unit per index of dim 0 (unitwise_norm over dims 1..), anything else
+    is one unit.  Returns (units, head): units = [(bucket, offset, numel)] in bucket order (0 = big, 1 = small) and offset order;
+    head = names of the parameters left out.  The rows of a >= 2-D parameter must be contiguous in its slot (dim 0 its outermost
+    dense dimension; channels_last convolution weights are); anything else raises ValueError."""
+    params = list(model.parameters())
+    left_out = {id(p) for p in params[-2:]}
+    head = [n for n, p in model.named_parameters() if id(p) in left_out]
+    units = []
+    for bucket, key in ((0, "big"), (1, "small")):
+        for name, p, off in plan[key]:
+            if id(p) in left_out or p.numel() == 0:
+                continue
+            if p.dim() > 1 and p.shape[0] > 1:
+                rows = p.shape[0]
+                row = p.numel() // rows
+                inner = sum(s * (k - 1) for s, k in zip(p.stride()[1:], p.shape[1:]))
+                if p.stride(0) != row or inner >= row:
+                    raise ValueError("clip_mode='agc': the rows along dim 0 of %s (shape %s, strides %s) are not contiguous in its "
+                                     "flat slot, so its units cannot be clipped in place" % (name, tuple(p.shape), p.stride()))
+                units.extend((bucket, off + r * row, row) for r in range(rows))
+            else:
+                units.append((bucket, off, p.numel()))
+    return units, head
+
+
+def _clip_segments(units, n, seg_max):
+    """cotb200_clip_seg table of one flat range [0, n): units = [(unit index, offset, numel)] in offset order; the gaps (slot padding,
+    parameters left out) get unit -1; every piece holds at most seg_max elements."""
+    segs = []
+
+    def add(off, ln, u):
+        for a in range(off, off + ln, seg_max):
+            segs.append((a, min(seg_max, off + ln - a), u))
+    pos = 0
+    for u, off, ln in units:
+        if off > pos:
+            add(pos, off - pos, -1)
+        add(off, ln, u)
+        pos = off + ln
+    if pos < n:
+        add(pos, n - pos, -1)
+    return segs
+
+
+def _table(struct, rows, dev):
+    arr = (struct * max(1, len(rows)))()
+    for i, r in enumerate(rows):
+        arr[i].offset, arr[i].numel = r[0], r[1]
+        setattr(arr[i], struct._fields_[2][0], r[2])
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
+
+
 class _Seg(ctypes.Structure):
     _fields_ = [("ptr", ctypes.c_void_p), ("offset", ctypes.c_longlong), ("numel", ctypes.c_longlong),
                 ("dtype", ctypes.c_int), ("pad_", ctypes.c_int)]
@@ -132,9 +191,17 @@ class TrainStep:
 
     def __init__(self, model, lr=0.05, momentum=0.9, weight_decay=1e-4, nesterov=True, ema_decay=None,
                  loss_fn=None, amp_dtype=torch.bfloat16, weights="bf16", bucket_dtype=None, comm_chunks=3, overlap=True,
-                 process_group=None, label_smoothing=0.):
+                 process_group=None, label_smoothing=0., clip_grad=None, clip_mode="norm"):
         """label_smoothing > 0, or a `mix` given to the step, selects the soft-target loss (soft_target_cross_entropy) that the
-        reference recipe trains with (train.py:198-209); otherwise the loss is `loss_fn` (default F.cross_entropy)."""
+        reference recipe trains with (train.py:198-209); otherwise the loss is `loss_fn` (default F.cross_entropy).
+        clip_grad > 0 clips the averaged gradients before the update like the reference's solver.clip_grad / solver.clip_mode
+        (train.py:270-273): 'norm' (clip_grad_norm_, norm 2; the norm is left in `grad_norm`, an fp32 device scalar), 'value'
+        (clip_grad_value_) or 'agc' (adaptive_clip_grad without the classifier head).  None or <= 0: no clipping."""
+        if clip_mode not in CLIP_MODES:
+            raise ValueError("TrainStep: unknown clip_mode %r (one of %s)" % (clip_mode, ", ".join(CLIP_MODES)))
+        self.clip_grad = float(clip_grad) if clip_grad is not None and clip_grad > 0 else None
+        self.clip_mode = clip_mode
+        self.grad_norm = None
         self.model = model
         self.loss_fn = loss_fn or (lambda out, lab: F.cross_entropy(out.float(), lab))
         self.label_smoothing = float(label_smoothing)
@@ -226,6 +293,49 @@ class TrainStep:
         if self.overlap:
             for _, p, _ in plan["big"]:
                 p.register_post_accumulate_grad_hook(self._on_grad)
+        self._clips = None
+        if self.clip_grad is not None and self._cuda:
+            self._init_clip()
+
+    # ------------------------------------------------------------------ gradient clipping
+    def _init_clip(self):
+        """Device tables and descriptors of the clip: one cotb200_clip per bucket, launched from optimizer_step()."""
+        mode, c, dev = CLIP_MODES[self.clip_mode], self.clip_grad, self.dev
+        n = (self.plan["n_big"], self.plan["n_small"])
+        descs = [_lib.Clip(mode=mode, value=c), _lib.Clip(mode=mode, value=c)]
+        if self.clip_mode == "norm":
+            self._clip_out = torch.zeros(2, dtype=torch.float32, device=dev)      # N, f
+            self.grad_norm = self._clip_out[0]
+            for d in descs:
+                d.factor = self._clip_out.data_ptr() + 4
+        elif self.clip_mode == "agc":
+            units, self.clip_head = plan_clip_units(self.model, self.plan)
+            self._agc_units = _table(_lib.ClipUnit, [(off, ln, b) for b, off, ln in units], dev)
+            self._agc_n, self._agc_elems = len(units), sum(ln for _, _, ln in units)
+            self._agc_factor = torch.ones(max(1, len(units)), dtype=torch.float32, device=dev)
+            seg_max = int(self.lib.cotb200_clip_seg_max())
+            self._agc_segs = []
+            for b in (0, 1):
+                segs = _clip_segments([(i, off, ln) for i, (bb, off, ln) in enumerate(units) if bb == b], n[b], seg_max)
+                self._agc_segs.append(_table(_lib.ClipSeg, segs, dev))
+                descs[b].factor, descs[b].segs, descs[b].n_segs = self._agc_factor.data_ptr(), self._agc_segs[b].data_ptr(), len(segs)
+        self._clips = descs
+
+    def _launch_clip_factors(self, st):
+        """The kernels that produce the clip factors from this step's gradients (and, for agc, the weights before the update)."""
+        lib, c = self.lib, self.clip_grad
+        gs_big, gs_small = self.hyper.data_ptr() + 16, self.hyper_small.data_ptr() + 16        # hyper[4] = grad_scale
+        ranges = [(n, G, gs) for n, G, gs in ((self.plan["n_big"], self.G_big, gs_big), (self.plan["n_small"], self.G_small, gs_small)) if n]
+        if self.clip_mode == "norm":
+            (n0, G0, g0), (n1, G1, g1) = ranges[0], (ranges[1] if len(ranges) > 1 else (0, None, None))
+            _lib.check(lib.cotb200_grad_norm(n0, _lib.dtype_code(G0), G0.data_ptr(), g0, n1, _lib.ptr(G1), g1, c,
+                                             self._clip_out.data_ptr(), st), "grad_norm")
+        elif self.clip_mode == "agc" and self._agc_n:
+            small = bool(self.plan["n_small"])
+            _lib.check(lib.cotb200_unit_norms(self._agc_n, self._agc_units.data_ptr(), self._agc_elems, self.P_big.data_ptr(),
+                                              _lib.dtype_code(self.G_big), self.G_big.data_ptr(), gs_big,
+                                              self.P_small.data_ptr() if small else None, self.G_small.data_ptr() if small else None,
+                                              gs_small if small else None, c, self._agc_factor.data_ptr(), None, st), "unit_norms")
 
     # ------------------------------------------------------------------ hyper-parameters
     def set_lr(self, lr):
@@ -343,15 +453,20 @@ class TrainStep:
     def optimizer_step(self):
         st = torch.cuda.current_stream(self.dev).cuda_stream
         lib = self.lib
+        if self._clips is not None:
+            self._launch_clip_factors(st)
+            sgd = lambda *a, clip: lib.cotb200_sgd_ema_step_clip(*a, ctypes.byref(clip), st)   # noqa: E731
+        else:
+            sgd = lambda *a, clip: lib.cotb200_sgd_ema_step(*a, st)                            # noqa: E731
+        clips = self._clips or (None, None)
         if self.plan["n_big"]:
-            _lib.check(lib.cotb200_sgd_ema_step(self.plan["n_big"], self.P_big.data_ptr(), self.M_big.data_ptr(),
-                                                _lib.dtype_code(self.G_big), self.G_big.data_ptr(), _lib.ptr(self.E_big),
-                                                _lib.ptr(self.Pb), self.hyper.data_ptr(), 1 if self.nesterov else 0, st),
-                       "sgd_ema_step")
+            _lib.check(sgd(self.plan["n_big"], self.P_big.data_ptr(), self.M_big.data_ptr(), _lib.dtype_code(self.G_big),
+                           self.G_big.data_ptr(), _lib.ptr(self.E_big), _lib.ptr(self.Pb), self.hyper.data_ptr(),
+                           1 if self.nesterov else 0, clip=clips[0]), "sgd_ema_step")
         if self.plan["n_small"]:
-            _lib.check(lib.cotb200_sgd_ema_step(self.plan["n_small"], self.P_small.data_ptr(), self.M_small.data_ptr(), _lib.F32,
-                                                self.G_small.data_ptr(), _lib.ptr(self.E_small), None,
-                                                self.hyper_small.data_ptr(), 1 if self.nesterov else 0, st), "sgd_ema_step")
+            _lib.check(sgd(self.plan["n_small"], self.P_small.data_ptr(), self.M_small.data_ptr(), _lib.F32,
+                           self.G_small.data_ptr(), _lib.ptr(self.E_small), None, self.hyper_small.data_ptr(),
+                           1 if self.nesterov else 0, clip=clips[1]), "sgd_ema_step")
         if self.ema and self._lerp_n:
             _lib.check(lib.cotb200_multi_lerp(self._lerp_tab.data_ptr(), self._lerp_n, self.hyper.data_ptr(), st), "multi_lerp")
 

@@ -400,6 +400,52 @@ int cotb200_sgd_ema_step(long long n, float* P, float* M, int g_dtype, const voi
 /* dst = decay*dst + (1-decay)*src per segment (fp32; int64 with the reference's float round trip): ModelEmaV2 over the
  * BUFFERS of the state_dict (BatchNorm running statistics / counters), one launch. decay = hyper_dev[3]. */
 int cotb200_multi_lerp(const cotb200_seg2* segs_dev, int n_segs, const float* hyper_dev, void* stream);
+
+/* ---- gradient clipping on the flat buckets (train.py:270-273 -> utils/clip_grad.py:dispatch_clip_grad) ----
+ * g' = G[i] * grad_scale is the averaged gradient the optimizer reads; the clip acts on g' in fp32 inside the optimizer pass
+ * and never writes the bucket.  Modes (torch semantics, NaN propagated as torch.clamp does):
+ *   NORM  (clip_grad_norm_, norm 2):  g' * f,  f = min(1, c / (N + 1e-6)),  N = ||g'|| over every element of both buckets
+ *   VALUE (clip_grad_value_):          clamp(g', -c, c)
+ *   AGC   (adaptive_clip_grad):        per unit u (a row along dim 0 of a >=2-D parameter, or a whole 1-D parameter):
+ *                                      m = max(||P_u||, 1e-3) * c,  n = ||g'_u||;  g'_u unchanged if n < m, else
+ *                                      g'_u * (m / max(n, 1e-6)).  P_u: the fp32 master weights before the update. */
+enum { COTB200_CLIP_NORM = 1, COTB200_CLIP_VALUE = 2, COTB200_CLIP_AGC = 3 };
+typedef struct cotb200_clip_unit {    /* AGC: one unit, `numel` consecutive elements of flat range `range` (0 or 1) */
+  long long offset;
+  int numel;
+  int range;
+} cotb200_clip_unit;
+typedef struct cotb200_clip_seg {     /* AGC: one piece of the optimizer's flat range, handled by one warp */
+  long long offset;
+  int numel;                          /* 1 .. cotb200_clip_seg_max() */
+  int unit;                           /* index into the factors; -1: factor 1 (slot padding, parameters left out) */
+} cotb200_clip_seg;
+typedef struct cotb200_clip {         /* the clip of one cotb200_sgd_ema_step_clip call */
+  int mode;                           /* COTB200_CLIP_* */
+  float value;                        /* VALUE: c (> 0) */
+  const float* factor;                /* NORM: device pointer to f (out[1] of cotb200_grad_norm); AGC: device per-unit factors */
+  const cotb200_clip_seg* segs;       /* AGC: device table of segments tiling [0, n) in order */
+  int n_segs;
+  int pad_;
+} cotb200_clip;
+/* Largest cotb200_clip_seg.numel: the caller cuts longer pieces. */
+int cotb200_clip_seg_max(void);
+/* out[0] = N = sqrt(sum over both ranges of (G*gs)^2), out[1] = f = min(1, max_norm / (N + 1e-6)) (fp32, device).  Range 0:
+ * n0 elements of fp32 or bf16 (g0_dtype), range 1: n1 fp32 elements (n1 = 0: none); each scaled by its device scalar gs0 / gs1.
+ * n0, n1 multiples of 4.  Deterministic: the partial sums are added in a fixed order. */
+int cotb200_grad_norm(long long n0, int g0_dtype, const void* G0, const float* gs0, long long n1, const float* G1, const float* gs1,
+                      float max_norm, float* out, void* stream);
+/* AGC factors: factor[u] = 1 when ||g'_u|| < m_u, else m_u / max(||g'_u||, 1e-6), for every unit of the device table (one warp
+ * per unit, a fixed summation order).  Range 0 = (P0, G0 of g0_dtype, gs0), range 1 = (P1, G1 fp32, gs1; all NULL if no unit
+ * lies there).  norms: NULL, or device fp32 [n_units][2] receiving (||P_u||, ||g'_u||).  unit_elems = the sum of the units'
+ * numel (the launch's algorithmic bytes). */
+int cotb200_unit_norms(int n_units, const cotb200_clip_unit* units_dev, long long unit_elems, const float* P0, int g0_dtype,
+                       const void* G0, const float* gs0, const float* P1, const float* G1, const float* gs1, float clip_factor,
+                       float* factor, float* norms, void* stream);
+/* cotb200_sgd_ema_step with the clip applied to g' = G*grad_scale on the way in: the update reads the clipped g' in place of
+ * G*grad_scale.  A factor of 1 or a clamp that does not bind gives bit-for-bit the result of cotb200_sgd_ema_step. */
+int cotb200_sgd_ema_step_clip(long long n, float* P, float* M, int g_dtype, const void* G, float* E, void* Pb,
+                              const float* hyper_dev, int nesterov, const cotb200_clip* clip, void* stream);
 /* y[n,h,w,c] = (x_u8[n,c,h,w] - mean[c]) / std[c]: uint8 NCHW batch -> normalised channels_last tensor of `dtype`
  * (PrefetchLoader, datasets/loader.py:66-67,86-90, + the channels_last / bf16 conversion of the AMP forward) in one
  * pass.  C == 3 with H*W % 4 == 0 takes mean_host/std_host (host arrays of 3); anything else needs the device arrays. */
