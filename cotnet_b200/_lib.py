@@ -52,6 +52,21 @@ class Clip(ctypes.Structure):
                 ("n_segs", ctypes.c_int), ("pad_", ctypes.c_int)]
 
 
+OPT_SGD, OPT_MOMENTUM, OPT_ADAM, OPT_ADAMW, OPT_NADAM, OPT_RADAM, OPT_ADADELTA, OPT_RMSPROP, OPT_RMSPROPTF = range(1, 10)
+
+
+class OptState(ctypes.Structure):
+    """struct cotb200_opt_state (include/cotb200.h): the device scalars of one optimizer."""
+    _fields_ = [("t", ctypes.c_double), ("m_schedule", ctypes.c_double), ("c", ctypes.c_float * 4), ("sync", ctypes.c_int),
+                ("slow_init", ctypes.c_int)]
+
+
+class Opt(ctypes.Structure):
+    """struct cotb200_opt (include/cotb200.h): the optimizer of one cotb200_opt_step call."""
+    _fields_ = [("rule", ctypes.c_int), ("eps", ctypes.c_float), ("lookahead_k", ctypes.c_int), ("lookahead_alpha", ctypes.c_float),
+                ("M", ctypes.c_void_p), ("V", ctypes.c_void_p), ("S", ctypes.c_void_p), ("state", ctypes.c_void_p)]
+
+
 _lock = threading.Lock()
 _lib = None
 
@@ -132,6 +147,10 @@ SYMBOLS = {
                                           _VP, _VP, _VP]),
     "cotb200_sgd_ema_step_clip": (ctypes.c_int, [ctypes.c_longlong, _VP, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int,
                                                  ctypes.POINTER(Clip), _VP]),
+    "cotb200_opt_prepare": (ctypes.c_int, [ctypes.POINTER(Opt), _VP, ctypes.c_int, _VP]),
+    "cotb200_opt_step": (ctypes.c_int, [ctypes.c_longlong, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.POINTER(Opt), ctypes.POINTER(Clip),
+                                        _VP]),
+    "cotb200_lookahead_sync": (ctypes.c_int, [ctypes.c_longlong, _VP, _VP, ctypes.POINTER(Opt), _VP]),
     "cotb200_u8_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
                                           _VP, _VP, _VP]),
     "cotb200_u8_mix_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),

@@ -6,26 +6,14 @@
 //
 //   cotb200_grad_norm          NORM: N = ||g'|| over both buckets, one launch, deterministic (det_finish); f = min(1, c/(N+1e-6))
 //   cotb200_unit_norms         AGC: ||P_u||, ||g'_u|| and the factor of every unit, one warp per unit
-//   cotb200_sgd_ema_step_clip  the update of cotb200_sgd_ema_step with the clip of any mode
 //
-// With a factor of 1 or a clamp that does not bind, g' goes into the update unchanged: the same arithmetic, bit for bit, as
-// cotb200_sgd_ema_step.
+// The update passes that apply the factors -- cotb200_sgd_ema_step_clip and cotb200_opt_step -- are in opt.cu.  With a factor of 1
+// or a clamp that does not bind, g' goes into the update unchanged: the same arithmetic, bit for bit, as cotb200_sgd_ema_step.
 #include "common.cuh"
 
 namespace cotb200 {
 
 static constexpr int CLIP_SEG_MAX = 4096;        // elements per AGC segment (one warp): 32 float4 per lane at most
-
-// torch.clamp semantics: a NaN operand stays NaN (fminf / fmaxf would return the bound)
-__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return x < lo ? lo : (x > hi ? hi : x); }
-
-template <bool NESTEROV>
-__device__ __forceinline__ void sgd_elem(float& p, float& m, float gc, float lr, float mu, float wd) {
-  const float g = fmaf(wd, p, gc);                // gc replaces grad*gscale of sgd_ema_kernel (optim.cu)
-  m = fmaf(mu, m, g);
-  const float st = NESTEROV ? fmaf(mu, m, g) : m;
-  p = fmaf(-lr, st, p);
-}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -117,100 +105,6 @@ unit_norms_kernel(const cotb200_clip_unit* __restrict__ units, int n_units, cons
   if (norms) { norms[2 * u] = pn; norms[2 * u + 1] = gn; }
 }
 
-// ------------------------------------------------------------------------------------------------ sgd_ema_step_clip
-// NORM / VALUE: one factor or bound for the whole range -- the grid-stride float4 loop of sgd_ema_kernel (optim.cu).
-template <int MODE>
-__device__ __forceinline__ float clip_uniform(float g, float f, float c) {
-  if constexpr (MODE == COTB200_CLIP_NORM) return g * f;
-  else return clamp_nan(g, -c, c);
-}
-
-template <typename TG, bool NESTEROV, int MODE>
-__global__ void __launch_bounds__(256)
-sgd_ema_clip_kernel(float* __restrict__ P, float* __restrict__ M, const TG* __restrict__ G, float* __restrict__ E,
-                    __nv_bfloat16* __restrict__ Pb, const float* __restrict__ hyper, long long n4, const float* __restrict__ fdev, float c) {
-  const float lr = __ldg(hyper), mu = __ldg(hyper + 1), wd = __ldg(hyper + 2), dec = __ldg(hyper + 3), gs = __ldg(hyper + 4);
-  const float f = MODE == COTB200_CLIP_NORM ? __ldg(fdev) : 1.f;
-  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
-    float4 p = reinterpret_cast<float4*>(P)[i];
-    float4 m = reinterpret_cast<float4*>(M)[i];
-    const Pack<TG, 4> gp = ld_pack<TG, 4>(G + i * 4);
-    float pv[4] = {p.x, p.y, p.z, p.w}, mv[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) sgd_elem<NESTEROV>(pv[k], mv[k], clip_uniform<MODE>((float)to_acc(gp.v[k]) * gs, f, c), lr, mu, wd);
-    reinterpret_cast<float4*>(P)[i] = make_float4(pv[0], pv[1], pv[2], pv[3]);
-    reinterpret_cast<float4*>(M)[i] = make_float4(mv[0], mv[1], mv[2], mv[3]);
-    if (E) {
-      float4 e = reinterpret_cast<float4*>(E)[i];
-      e.x = fmaf(dec, e.x, (1.f - dec) * pv[0]); e.y = fmaf(dec, e.y, (1.f - dec) * pv[1]);
-      e.z = fmaf(dec, e.z, (1.f - dec) * pv[2]); e.w = fmaf(dec, e.w, (1.f - dec) * pv[3]);
-      reinterpret_cast<float4*>(E)[i] = e;
-    }
-    if (Pb) {
-      Pack<__nv_bfloat16, 4> o;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) o.v[k] = __float2bfloat16_rn(pv[k]);
-      st_pack<__nv_bfloat16, 4>(Pb + i * 4, o);
-    }
-  }
-}
-
-// AGC: one warp per segment of the host's table, so the factor is uniform inside a warp.  Segments start and end anywhere (the
-// stem's 147-element rows put unit boundaries inside a float4): the elements before the first and after the last 16-byte
-// boundary of the segment are updated one by one, the rest as float4.  Two warps may write different elements of one float4;
-// no byte is written twice.
-template <typename TG, bool NESTEROV>
-__device__ __forceinline__ void agc_scalar(float* P, float* M, const TG* G, float* E, __nv_bfloat16* Pb, long long j, float f,
-                                           float lr, float mu, float wd, float dec, float gs) {
-  float p = P[j], m = M[j];
-  sgd_elem<NESTEROV>(p, m, ((float)to_acc(G[j]) * gs) * f, lr, mu, wd);
-  P[j] = p; M[j] = m;
-  if (E) E[j] = fmaf(dec, E[j], (1.f - dec) * p);
-  if (Pb) Pb[j] = __float2bfloat16_rn(p);
-}
-
-template <typename TG, bool NESTEROV>
-__global__ void __launch_bounds__(256)
-sgd_ema_agc_kernel(float* __restrict__ P, float* __restrict__ M, const TG* __restrict__ G, float* __restrict__ E,
-                   __nv_bfloat16* __restrict__ Pb, const float* __restrict__ hyper, const cotb200_clip_seg* __restrict__ segs, int n_segs,
-                   const float* __restrict__ factor) {
-  const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (w >= n_segs) return;
-  const float lr = __ldg(hyper), mu = __ldg(hyper + 1), wd = __ldg(hyper + 2), dec = __ldg(hyper + 3), gs = __ldg(hyper + 4);
-  const cotb200_clip_seg s = segs[w];
-  const float f = s.unit >= 0 ? __ldg(factor + s.unit) : 1.f;
-  const long long a = s.offset, b = s.offset + s.numel;
-  const long long a4 = (a + 3) >> 2, b4 = b >> 2;                     // float4 indices [a4, b4) lie inside [a, b)
-  if (a4 >= b4) {                                                      // no whole float4 inside
-    for (long long j = a + lane; j < b; j += 32) agc_scalar<TG, NESTEROV>(P, M, G, E, Pb, j, f, lr, mu, wd, dec, gs);
-    return;
-  }
-  if (a + lane < a4 * 4) agc_scalar<TG, NESTEROV>(P, M, G, E, Pb, a + lane, f, lr, mu, wd, dec, gs);
-  if (b4 * 4 + lane < b) agc_scalar<TG, NESTEROV>(P, M, G, E, Pb, b4 * 4 + lane, f, lr, mu, wd, dec, gs);
-  for (long long i = a4 + lane; i < b4; i += 32) {
-    float4 p = reinterpret_cast<float4*>(P)[i];
-    float4 m = reinterpret_cast<float4*>(M)[i];
-    const Pack<TG, 4> gp = ld_pack<TG, 4>(G + i * 4);
-    float pv[4] = {p.x, p.y, p.z, p.w}, mv[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) sgd_elem<NESTEROV>(pv[k], mv[k], ((float)to_acc(gp.v[k]) * gs) * f, lr, mu, wd);
-    reinterpret_cast<float4*>(P)[i] = make_float4(pv[0], pv[1], pv[2], pv[3]);
-    reinterpret_cast<float4*>(M)[i] = make_float4(mv[0], mv[1], mv[2], mv[3]);
-    if (E) {
-      float4 e = reinterpret_cast<float4*>(E)[i];
-      e.x = fmaf(dec, e.x, (1.f - dec) * pv[0]); e.y = fmaf(dec, e.y, (1.f - dec) * pv[1]);
-      e.z = fmaf(dec, e.z, (1.f - dec) * pv[2]); e.w = fmaf(dec, e.w, (1.f - dec) * pv[3]);
-      reinterpret_cast<float4*>(E)[i] = e;
-    }
-    if (Pb) {
-      Pack<__nv_bfloat16, 4> o;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) o.v[k] = __float2bfloat16_rn(pv[k]);
-      st_pack<__nv_bfloat16, 4>(Pb + i * 4, o);
-    }
-  }
-}
-
 static unsigned clip_stream_grid(long long items, int per_sm) {
   long long blocks = (items + 255) / 256;
   const long long cap = (long long)num_sms() * per_sm;
@@ -266,46 +160,4 @@ extern "C" int cotb200_unit_norms(int n_units, const cotb200_clip_unit* units_de
     unit_norms_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(units_dev, n_units, P0, (const __nv_bfloat16*)G0, gs0, P1, G1, gs1, clip_factor,
                                                            factor, norms);
   return check_launch("unit_norms");
-}
-
-extern "C" int cotb200_sgd_ema_step_clip(long long n, float* P, float* M, int g_dtype, const void* G, float* E, void* Pb,
-                                         const float* hyper_dev, int nesterov, const cotb200_clip* clip, void* stream) {
-  if (!P || !M || !G || !hyper_dev || !clip) { set_error("sgd_ema_step_clip: NULL pointer"); return COTB200_ENULL; }
-  if (n <= 0 || (n & 3)) { set_error("sgd_ema_step_clip: n=%lld must be a positive multiple of 4 (pad the flat range)", n); return COTB200_EINVAL; }
-  const int mode = clip->mode;
-  if (mode != COTB200_CLIP_NORM && mode != COTB200_CLIP_VALUE && mode != COTB200_CLIP_AGC) {
-    set_error("sgd_ema_step_clip: unknown clip mode %d", mode); return COTB200_EINVAL;
-  }
-  if (mode != COTB200_CLIP_VALUE && !clip->factor) { set_error("sgd_ema_step_clip: the clip has no factor pointer"); return COTB200_ENULL; }
-  if (mode == COTB200_CLIP_AGC && !clip->segs) { set_error("sgd_ema_step_clip: agc needs the segment table"); return COTB200_ENULL; }
-  if (mode == COTB200_CLIP_AGC && clip->n_segs <= 0) { set_error("sgd_ema_step_clip: agc needs segments"); return COTB200_EINVAL; }
-  if (mode == COTB200_CLIP_VALUE && !(clip->value > 0.f)) { set_error("sgd_ema_step_clip: clip value must be > 0"); return COTB200_EINVAL; }
-  if (!aligned16(P) || !aligned16(M) || (E && !aligned16(E)) || (reinterpret_cast<uintptr_t>(G) & (g_dtype == COTB200_F32 ? 15 : 7)) || (Pb && (reinterpret_cast<uintptr_t>(Pb) & 7))) {
-    set_error("sgd_ema_step_clip: flat buffers must be 16-byte aligned"); return COTB200_EALIGN;
-  }
-  if (g_dtype != COTB200_F32 && g_dtype != COTB200_BF16) { set_error("sgd_ema_step_clip: gradient dtype must be fp32 or bf16"); return COTB200_EDTYPE; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long n4 = n / 4;
-  double bytes = (double)n * (8.0 + 8.0 + (g_dtype == COTB200_F32 ? 4.0 : 2.0) + (E ? 8.0 : 0.0) + (Pb ? 2.0 : 0.0));
-  if (mode == COTB200_CLIP_AGC) {
-    bytes += (double)clip->n_segs * (16.0 + 4.0);
-    COTB200_PROF_B("sgd_ema_step_clip", bytes);
-    const unsigned grid = (unsigned)((clip->n_segs + 7) / 8);
-#define GO(TG, NES) sgd_ema_agc_kernel<TG, NES><<<grid, 256, 0, st>>>(P, M, (const TG*)G, E, (__nv_bfloat16*)Pb, hyper_dev, clip->segs, \
-                                                                      clip->n_segs, clip->factor)
-    if (g_dtype == COTB200_F32) { if (nesterov) GO(float, true); else GO(float, false); }
-    else { if (nesterov) GO(__nv_bfloat16, true); else GO(__nv_bfloat16, false); }
-#undef GO
-    return check_launch("sgd_ema_step_clip");
-  }
-  COTB200_PROF_B("sgd_ema_step_clip", bytes + (mode == COTB200_CLIP_NORM ? 4.0 : 0.0));
-  const unsigned grid = clip_stream_grid(n4, 16);
-#define GO(TG, NES, MODE) sgd_ema_clip_kernel<TG, NES, MODE><<<grid, 256, 0, st>>>(P, M, (const TG*)G, E, (__nv_bfloat16*)Pb, hyper_dev, n4, \
-                                                                                   clip->factor, clip->value)
-#define GO2(TG, MODE) { if (nesterov) GO(TG, true, MODE); else GO(TG, false, MODE); }
-  if (mode == COTB200_CLIP_NORM) { if (g_dtype == COTB200_F32) GO2(float, COTB200_CLIP_NORM) else GO2(__nv_bfloat16, COTB200_CLIP_NORM) }
-  else { if (g_dtype == COTB200_F32) GO2(float, COTB200_CLIP_VALUE) else GO2(__nv_bfloat16, COTB200_CLIP_VALUE) }
-#undef GO2
-#undef GO
-  return check_launch("sgd_ema_step_clip");
 }

@@ -16,7 +16,9 @@ Mirrors the body of the reference's training loop -- forward under autocast, los
   captured in ONE CUDA graph (fork/join through events); if NCCL cannot be captured the collectives run eagerly between
   a fwd+bwd graph and an optimizer graph.
 * **One optimizer pass.**  ``cotb200_sgd_ema_step``: SGD-nesterov + weight decay + EMA + bf16 copy, hyper-parameters read
-  from device memory (LR schedules work under graph replay); ``cotb200_multi_lerp`` for the EMA of the buffers.
+  from device memory (LR schedules work under graph replay); ``cotb200_multi_lerp`` for the EMA of the buffers.  The other
+  update rules of the reference's create_optimizer (``opt=``) are ``cotb200_opt_prepare`` (the per-step scalars, on the device)
+  and one ``cotb200_opt_step`` pass per bucket.
 
 There is no CPU fallback of the kernels; the planning logic (``plan_flat``) is pure Python and unit-tested on CPU.
 """
@@ -107,6 +109,38 @@ def plan_clip_units(model, plan):
     return units, head
 
 
+#: solver.opt names of create_optimizer (optim/optim_factory.py:34-120) that TrainStep runs -> the library's update rule.
+#: 'sgd' follows TrainStep's `nesterov` argument (True by default, the factory's SGD).
+OPT_RULES = {"sgd": _lib.OPT_SGD, "nesterov": _lib.OPT_SGD, "momentum": _lib.OPT_MOMENTUM, "adam": _lib.OPT_ADAM,
+             "adamw": _lib.OPT_ADAMW, "nadam": _lib.OPT_NADAM, "radam": _lib.OPT_RADAM, "adadelta": _lib.OPT_ADADELTA,
+             "rmsprop": _lib.OPT_RMSPROP, "rmsproptf": _lib.OPT_RMSPROPTF}
+#: names create_optimizer also accepts, and why their update is not a per-element pass over the flat buckets
+OPT_UNSUPPORTED = {"adamp": "a per-tensor projection", "sgdp": "a per-tensor projection", "novograd": "per-tensor gradient norms",
+                   "nvnovograd": "per-tensor gradient norms", "adafactor": "factored second moments",
+                   "adahessian": "Hessian-vector products"}
+LOOKAHEAD_ALPHA, LOOKAHEAD_K = 0.5, 6           # Lookahead(optimizer) as create_optimizer builds it (optim/lookahead.py)
+
+
+def parse_opt(name, nesterov=True):
+    """solver.opt as create_optimizer reads it (lower case; the part after the last '_' names the rule, a first part 'lookahead'
+    wraps it in Lookahead) -> (rule name, library rule code, lookahead).  Unsupported names raise ValueError."""
+    low = str(name).lower()
+    parts = low.split("_")
+    base, lookahead = parts[-1], len(parts) > 1 and parts[0] == "lookahead"
+    supported = ", ".join(sorted(OPT_RULES)) + " and lookahead_<any of these>"
+    if "fused" in low:
+        raise ValueError("opt=%r: the fused optimizers need apex with amp; TrainStep supports %s" % (name, supported))
+    if base in OPT_UNSUPPORTED:
+        raise ValueError("opt=%r: %s needs %s, not a per-element update; TrainStep supports %s"
+                         % (name, base, OPT_UNSUPPORTED[base], supported))
+    if base not in OPT_RULES:
+        raise ValueError("opt=%r: unknown optimizer; TrainStep supports %s" % (name, supported))
+    rule = OPT_RULES[base]
+    if base == "sgd" and not nesterov:
+        rule = _lib.OPT_MOMENTUM
+    return base, rule, lookahead
+
+
 def _clip_segments(units, n, seg_max):
     """cotb200_clip_seg table of one flat range [0, n): units = [(unit index, offset, numel)] in offset order; the gaps (slot padding,
     parameters left out) get unit -1; every piece holds at most seg_max elements."""
@@ -191,14 +225,20 @@ class TrainStep:
 
     def __init__(self, model, lr=0.05, momentum=0.9, weight_decay=1e-4, nesterov=True, ema_decay=None,
                  loss_fn=None, amp_dtype=torch.bfloat16, weights="bf16", bucket_dtype=None, comm_chunks=3, overlap=True,
-                 process_group=None, label_smoothing=0., clip_grad=None, clip_mode="norm"):
+                 process_group=None, label_smoothing=0., clip_grad=None, clip_mode="norm", opt="sgd", opt_eps=1e-8):
         """label_smoothing > 0, or a `mix` given to the step, selects the soft-target loss (soft_target_cross_entropy) that the
         reference recipe trains with (train.py:198-209); otherwise the loss is `loss_fn` (default F.cross_entropy).
         clip_grad > 0 clips the averaged gradients before the update like the reference's solver.clip_grad / solver.clip_mode
         (train.py:270-273): 'norm' (clip_grad_norm_, norm 2; the norm is left in `grad_norm`, an fp32 device scalar), 'value'
-        (clip_grad_value_) or 'agc' (adaptive_clip_grad without the classifier head).  None or <= 0: no clipping."""
+        (clip_grad_value_) or 'agc' (adaptive_clip_grad without the classifier head).  None or <= 0: no clipping.
+        opt / opt_eps are solver.opt / solver.opt_eps of create_optimizer (parse_opt): sgd (nesterov per `nesterov`), nesterov,
+        momentum, adam, adamw, nadam, radam, adadelta, rmsprop, rmsproptf, each optionally as lookahead_<name>; lr, momentum and
+        weight_decay are the factory's, everything else its defaults."""
         if clip_mode not in CLIP_MODES:
             raise ValueError("TrainStep: unknown clip_mode %r (one of %s)" % (clip_mode, ", ".join(CLIP_MODES)))
+        self.opt_name, rule, self.lookahead = parse_opt(opt, nesterov)
+        if rule in (_lib.OPT_SGD, _lib.OPT_MOMENTUM):
+            nesterov = rule == _lib.OPT_SGD
         self.clip_grad = float(clip_grad) if clip_grad is not None and clip_grad > 0 else None
         self.clip_mode = clip_mode
         self.grad_norm = None
@@ -296,6 +336,30 @@ class TrainStep:
         self._clips = None
         if self.clip_grad is not None and self._cuda:
             self._init_clip()
+        self._opts = None                           # plain SGD without Lookahead: cotb200_sgd_ema_step(_clip), no step counter
+        self.V_big = self.V_small = self.S_big = self.S_small = self.opt_state = None
+        if (rule not in (_lib.OPT_SGD, _lib.OPT_MOMENTUM) or self.lookahead) and self._cuda:
+            self._init_opt(rule, float(opt_eps), momentum)
+
+    # ------------------------------------------------------------------ update rules
+    def _init_opt(self, rule, eps, momentum):
+        """State buffers and the two cotb200_opt descriptors (big, small) of a rule other than plain SGD."""
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        nb, ns = self.plan["n_big"], self.plan["n_small"]
+        self.rule = rule
+        if rule not in (_lib.OPT_SGD, _lib.OPT_MOMENTUM):
+            fill = 1.0 if rule == _lib.OPT_RMSPROPTF else 0.0       # rmsprop_tf.py:94: square_avg starts at 1
+            self.V_big, self.V_small = torch.full((nb,), fill, **f32), torch.full((ns,), fill, **f32)
+        if self.lookahead:
+            self.S_big, self.S_small = torch.zeros(nb, **f32), torch.zeros(ns, **f32)
+        st = _lib.OptState(m_schedule=1.0)
+        self.opt_state = torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(self.dev)
+        self._opt_uses_m = not (rule in (_lib.OPT_RMSPROP, _lib.OPT_RMSPROPTF) and not momentum > 0)
+        self._opts = []
+        for M, V, S in ((self.M_big, self.V_big, self.S_big), (self.M_small, self.V_small, self.S_small)):
+            self._opts.append(_lib.Opt(rule=rule, eps=eps, lookahead_k=LOOKAHEAD_K if self.lookahead else 0,
+                                       lookahead_alpha=LOOKAHEAD_ALPHA, M=M.data_ptr() if self._opt_uses_m else None,
+                                       V=_lib.ptr(V), S=_lib.ptr(S), state=self.opt_state.data_ptr()))
 
     # ------------------------------------------------------------------ gradient clipping
     def _init_clip(self):
@@ -453,6 +517,9 @@ class TrainStep:
     def optimizer_step(self):
         st = torch.cuda.current_stream(self.dev).cuda_stream
         lib = self.lib
+        if self._opts is not None:
+            self._rule_step(st)
+            return
         if self._clips is not None:
             self._launch_clip_factors(st)
             sgd = lambda *a, clip: lib.cotb200_sgd_ema_step_clip(*a, ctypes.byref(clip), st)   # noqa: E731
@@ -469,6 +536,38 @@ class TrainStep:
                            1 if self.nesterov else 0, clip=clips[1]), "sgd_ema_step")
         if self.ema and self._lerp_n:
             _lib.check(lib.cotb200_multi_lerp(self._lerp_tab.data_ptr(), self._lerp_n, self.hyper.data_ptr(), st), "multi_lerp")
+
+    def _rule_step(self, st):
+        """optimizer.step() of a rule other than plain SGD: the per-step scalars, one cotb200_opt_step per bucket, the EMA of the
+        buffers."""
+        lib = self.lib
+        _lib.check(lib.cotb200_opt_prepare(ctypes.byref(self._opts[0]), self.hyper.data_ptr(), 1, st), "opt_prepare")
+        if self._clips is not None:
+            self._launch_clip_factors(st)
+        clips = [ctypes.byref(c) for c in self._clips] if self._clips is not None else [None, None]
+        for n, P, G, E, Pb, hyper, opt, clip in (
+                (self.plan["n_big"], self.P_big, self.G_big, self.E_big, self.Pb, self.hyper, self._opts[0], clips[0]),
+                (self.plan["n_small"], self.P_small, self.G_small, self.E_small, None, self.hyper_small, self._opts[1], clips[1])):
+            if n:
+                _lib.check(lib.cotb200_opt_step(n, P.data_ptr(), _lib.dtype_code(G), G.data_ptr(), _lib.ptr(E), _lib.ptr(Pb),
+                                                hyper.data_ptr(), ctypes.byref(opt), clip, st), "opt_step")
+        if self.ema and self._lerp_n:
+            _lib.check(lib.cotb200_multi_lerp(self._lerp_tab.data_ptr(), self._lerp_n, self.hyper.data_ptr(), st), "multi_lerp")
+
+    def sync_lookahead(self):
+        """Lookahead.sync_lookahead, the reference's end-of-epoch call (train.py:295-296): slow += alpha (fast - slow); fast = slow
+        for every parameter (the first synchronisation only creates the slow weights), and the bf16 copy of the weights.  Runs
+        eagerly on the current stream; the step counter and the EMA do not move.  Nothing happens without Lookahead, as the
+        reference only calls it on a Lookahead optimizer."""
+        if not self.lookahead or self._opts is None:
+            return
+        st = torch.cuda.current_stream(self.dev).cuda_stream
+        lib = self.lib
+        _lib.check(lib.cotb200_opt_prepare(ctypes.byref(self._opts[0]), self.hyper.data_ptr(), 0, st), "opt_prepare")
+        for n, P, Pb, opt in ((self.plan["n_big"], self.P_big, self.Pb, self._opts[0]),
+                              (self.plan["n_small"], self.P_small, None, self._opts[1])):
+            if n:
+                _lib.check(lib.cotb200_lookahead_sync(n, P.data_ptr(), _lib.ptr(Pb), ctypes.byref(opt), st), "lookahead_sync")
 
     def step_eager(self, x, lab, mix=None):
         loss = self.forward_backward(x, lab, mix)
@@ -586,6 +685,34 @@ class TrainStep:
             out[n] = _strided_view(self.P_big, p, off)
         for n, p, off in self.plan["small"]:
             out[n] = _strided_view(self.P_small, p, off)
+        return out
+
+    def optimizer_state(self):
+        """name -> {state key of the reference's optimizer: view}: fp32 views into the flat state buffers (exp_avg, exp_avg_sq,
+        square_avg, acc_delta, momentum_buffer, slow_buffer) and 0-dim fp64 views of the device scalars `step` (updates done)
+        and, for nadam, `m_schedule`.  slow_buffer holds the slow weights once the first Lookahead synchronisation has run."""
+        rule = self.rule if self._opts is not None else (_lib.OPT_SGD if self.nesterov else _lib.OPT_MOMENTUM)
+        uses_m = self._opt_uses_m if self._opts is not None else True
+        keys = {_lib.OPT_ADADELTA: ("acc_delta", "square_avg"), _lib.OPT_RMSPROP: ("momentum_buffer", "square_avg"),
+                _lib.OPT_RMSPROPTF: ("momentum_buffer", "square_avg"), _lib.OPT_SGD: ("momentum_buffer", None),
+                _lib.OPT_MOMENTUM: ("momentum_buffer", None)}.get(rule, ("exp_avg", "exp_avg_sq"))
+        scal = {}
+        if self.opt_state is not None and rule not in (_lib.OPT_SGD, _lib.OPT_MOMENTUM):
+            d = self.opt_state[:16].view(torch.float64)
+            scal["step"] = d[0]
+            if rule == _lib.OPT_NADAM:
+                scal["m_schedule"] = d[1]
+        out = {}
+        for key, M, V, S in (("big", self.M_big, self.V_big, self.S_big), ("small", self.M_small, self.V_small, self.S_small)):
+            for n, p, off in self.plan[key]:
+                d = dict(scal)
+                if uses_m:
+                    d[keys[0]] = _strided_view(M, p, off)
+                if V is not None:
+                    d[keys[1]] = _strided_view(V, p, off)
+                if S is not None:
+                    d["slow_buffer"] = _strided_view(S, p, off)
+                out[n] = d
         return out
 
     def ema_state(self):

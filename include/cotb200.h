@@ -446,6 +446,51 @@ int cotb200_unit_norms(int n_units, const cotb200_clip_unit* units_dev, long lon
  * G*grad_scale.  A factor of 1 or a clamp that does not bind gives bit-for-bit the result of cotb200_sgd_ema_step. */
 int cotb200_sgd_ema_step_clip(long long n, float* P, float* M, int g_dtype, const void* G, float* E, void* Pb,
                               const float* hyper_dev, int nesterov, const cotb200_clip* clip, void* stream);
+
+/* ---- the update rules of create_optimizer (optim/optim_factory.py) on the flat buckets ----
+ * One pass per flat range: g' = G*grad_scale, the clip (cotb200_clip, NULL: none), the rule, the Lookahead synchronisation when
+ * this step has one, E = decay*E + (1-decay)*P of the final weights, and the bf16 copy Pb.  hyper_dev is the fp32[5] of
+ * cotb200_sgd_ema_step ({lr, momentum, weight_decay, ema_decay, grad_scale}); betas, rho and alpha are the factory's defaults:
+ *   SGD / MOMENTUM  torch.optim.SGD, nesterov / not                     M = momentum_buffer
+ *   ADAM            torch.optim.Adam (L2 decay), betas (0.9, 0.999)     M = exp_avg, V = exp_avg_sq
+ *   ADAMW           optim/adamw.py: P *= 1 - lr*wd, then Adam           M, V as ADAM
+ *   NADAM           optim/nadam.py (L2 decay, schedule_decay 4e-3)      M, V as ADAM; m_schedule in the state (fp64)
+ *   RADAM           optim/radam.py RAdam: P += -wd*lr*P; rectified update once N_sma >= 5, else P -= step_size*M
+ *   ADADELTA        torch.optim.Adadelta, rho 0.9                       M = acc_delta, V = square_avg
+ *   RMSPROP         torch.optim.RMSprop, alpha 0.9                      V = square_avg (from 0), M = momentum_buffer or NULL
+ *   RMSPROPTF       optim/rmsprop_tf.py, alpha 0.9, lr in momentum      V = square_avg (the caller fills it with 1), M or NULL
+ * Lookahead (optim/lookahead.py) wraps any of them: every lookahead_k-th update, S += alpha (P - S); P = S, where the first
+ * synchronisation creates S from P (P unchanged). */
+enum {
+  COTB200_OPT_SGD = 1, COTB200_OPT_MOMENTUM = 2, COTB200_OPT_ADAM = 3, COTB200_OPT_ADAMW = 4, COTB200_OPT_NADAM = 5,
+  COTB200_OPT_RADAM = 6, COTB200_OPT_ADADELTA = 7, COTB200_OPT_RMSPROP = 8, COTB200_OPT_RMSPROPTF = 9
+};
+typedef struct cotb200_opt_state {    /* device; the caller initialises t = 0, m_schedule = 1, the rest 0 */
+  double t;                           /* updates done (every cotb200_opt_prepare with advance) */
+  double m_schedule;                  /* NADAM: the product of the momentum caches */
+  float c[4];                         /* this step's coefficients of the rule (cotb200_opt_prepare) */
+  int sync;                           /* this step's Lookahead action: 0 none, 1 create S = P, 2 S += alpha (P - S); P = S */
+  int slow_init;                      /* S holds the slow weights */
+} cotb200_opt_state;
+typedef struct cotb200_opt {          /* the optimizer of one flat range */
+  int rule;                           /* COTB200_OPT_* */
+  float eps;                          /* solver.opt_eps */
+  int lookahead_k;                    /* 0: no Lookahead */
+  float lookahead_alpha;
+  float* M;                           /* fp32 state buffers of the range, 16-byte aligned (see the table above) */
+  float* V;
+  float* S;                           /* Lookahead's slow weights */
+  cotb200_opt_state* state;           /* device, shared by the ranges of one optimizer */
+} cotb200_opt;
+/* Once per step before the passes: t += 1 (advance != 0) and everything that depends only on t and lr = hyper_dev[0], in fp64
+ * (bias corrections, Nadam's momentum caches and m_schedule, RAdam's N_sma and step size, the Lookahead flag).  advance = 0:
+ * only the flag, set to synchronise now (TrainStep.sync_lookahead).  One thread. */
+int cotb200_opt_prepare(const cotb200_opt* opt, const float* hyper_dev, int advance, void* stream);
+/* The pass over a flat range of n (multiple of 4) elements.  G fp32 or bf16 (g_dtype); E, Pb NULL: none; clip NULL: none. */
+int cotb200_opt_step(long long n, float* P, int g_dtype, const void* G, float* E, void* Pb, const float* hyper_dev,
+                     const cotb200_opt* opt, const cotb200_clip* clip, void* stream);
+/* The Lookahead synchronisation prepared by cotb200_opt_prepare(advance = 0), and the bf16 copy Pb (NULL: none). */
+int cotb200_lookahead_sync(long long n, float* P, void* Pb, const cotb200_opt* opt, void* stream);
 /* y[n,h,w,c] = (x_u8[n,c,h,w] - mean[c]) / std[c]: uint8 NCHW batch -> normalised channels_last tensor of `dtype`
  * (PrefetchLoader, datasets/loader.py:66-67,86-90, + the channels_last / bf16 conversion of the AMP forward) in one
  * pass.  C == 3 with H*W % 4 == 0 takes mean_host/std_host (host arrays of 3); anything else needs the device arrays. */
