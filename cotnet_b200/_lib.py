@@ -121,12 +121,6 @@ SYMBOLS = {
     "cotb200_gemm_bf16": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, ctypes.c_longlong]
                           + [ctypes.c_int, _VP, ctypes.c_longlong, _VP, ctypes.c_longlong]
                           + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_int, _VP, _VP, _VP]),
-    "cotb200_gemm_bf16_samplestats": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, ctypes.c_longlong, _VP, ctypes.c_longlong,
-                                                     _VP, _VP, ctypes.c_int, ctypes.c_int, _VP, _VP, _VP]),
-    "cotb200_gn9_from_colsums": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP, _VP, _VP, ctypes.c_float, _VP, _VP, _VP]),
-    "cotb200_gn9_coef_from_colsums": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 5 + [ctypes.c_float, _VP, _VP]),
-    "cotb200_mix2": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 5),
-    "cotb200_cot_agg_eval": (ctypes.c_int, [_DP] + [_VP] * 9),
     "cotb200_conv3x3_bf16": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP,
                                                                  ctypes.c_longlong, _VP, _VP, ctypes.c_int, _VP, _VP, _VP]),
     "cotb200_stem7x7s2_scratch_bytes": (ctypes.c_longlong, [ctypes.c_int] * 3),

@@ -184,29 +184,14 @@ class CoTResNet(StochasticDepth, nn.Module):
                 if hasattr(m, "zero_init_last_bn"):
                     m.zero_init_last_bn()
 
-    def _stem_conv(self, x):
-        """conv1 (models/resnet.py:552: 7x7/s2, 3 -> 64) with the input and the weight zero-padded to `stem_pad` channels:
-        identical arithmetic.  Off by default (COTB200_STEM_PAD = 0): the pad/cast traffic can cost more than the aligned cuDNN
-        kernels gain; tools/bench_stem.py compares the variants on the machine at hand."""
-        C = x.shape[1]
-        pad = self.stem_pad - C if (self.stem_pad and C < self.stem_pad and self.conv1.groups == 1) else 0
-        if pad <= 0:
-            return self.conv1(x)
-        c1 = self.conv1
-        xp = F.pad(x, (0, 0, 0, 0, 0, pad)).contiguous(memory_format=torch.channels_last)
-        wp = F.pad(c1.weight, (0, 0, 0, 0, 0, pad)).contiguous(memory_format=torch.channels_last)
-        return F.conv2d(xp, wp, c1.bias, c1.stride, c1.padding, c1.dilation, 1)
-
-    stem_pad = int(os.environ.get("COTB200_STEM_PAD", "0"))
-
     def forward_features(self, x):
         if fused.supported(x):
-            if self.stem_pad == 0 and x.dtype == torch.bfloat16:
+            if x.dtype == torch.bfloat16:
                 # conv1 + bn1 + ReLU: 7x7/s2 stem on the 4-tap wgmma implicit GEMM, BatchNorm statistics from its epilogue
                 # (fused.stem_conv_bn falls back to cuDNN + the fused BatchNorm kernels for geometries it does not take)
                 x = fused.max_pool3x3s2(fused.stem_conv_bn(x, self.conv1, self.bn1, relu=True))
             else:
-                x = fused.max_pool3x3s2(fused.bn_act(self._stem_conv(x).contiguous(memory_format=torch.channels_last), self.bn1, relu=True))
+                x = fused.max_pool3x3s2(fused.bn_act(self.conv1(x).contiguous(memory_format=torch.channels_last), self.bn1, relu=True))
         else:
             x = self.maxpool(self.act1(self.bn1(self.conv1(x))))
         return self._run_blocks(x)

@@ -169,24 +169,8 @@ class CotLayer(nn.Module):
         with torch.no_grad():
             wk, bnk = tc.prepare_conv3x3_weight(self.key_embed[0].weight, 4)
             we1 = self.embed[0].weight.detach().view(C // 2, 2 * C).to(torch.bfloat16)
-            # tap-major column order of the logits (COTB200_NHWC_TAP, chunks of 8 weight channels): position j' holds reference
-            # column ref[j'] = g*9 + t -- permuting embed.3's rows makes the GEMM emit that order for free
-            wc, gcw = C // 8, fused.tap_chunk(C // 8)
-            ref = None
-            if gcw:
-                jp = torch.arange(9 * wc, device=device)
-                g_ = (jp // (9 * gcw)) * gcw + jp % gcw
-                t_ = (jp // gcw) % 9
-                ref = g_ * 9 + t_
-            gn = self.embed[4]
-            w3 = self.embed[3].weight.detach().view(-1, C // 2)
             cache = {
                 "key": key, "wk": wk, "bnk": bnk, "k_ss": fold(self.key_embed[1]),
-                "ref": ref,
-                "we2p": None if ref is None else w3[ref].to(torch.bfloat16).contiguous(),
-                "be2p": None if ref is None else self.embed[3].bias.detach().float()[ref].contiguous(),
-                "gnw_p": None if ref is None else gn.weight.detach().float()[ref].contiguous(),
-                "gnb_p": None if ref is None else gn.bias.detach().float()[ref].contiguous(),
                 "bn_ss": fold(self.bn),
                 "we1x": we1[:, :C].contiguous(), "we1k": we1[:, C:].contiguous(), "e_ss": fold(self.embed[1]),
                 "we2": self.embed[3].weight.detach().view(-1, C // 2).to(torch.bfloat16).contiguous(),
@@ -206,29 +190,10 @@ class CotLayer(nn.Module):
         k = tc.conv3x3_bf16(x, p["wk"], p["bnk"], scale=p["k_ss"][0], shift=p["k_ss"][1], relu=True)
         e = tc.gemm_bf16(x, p["we1x"], k, p["we1k"], scale=p["e_ss"][0], shift=p["e_ss"][1], relu=True)
         gc = fused.tap_chunk(C // 8)
-        if self.eval_fused_agg and gc == 8 and H * W >= 32 and C <= 512 and p["ref"] is not None:
-            # (opt-in, COTB200_EVAL_FUSED_AGG=1) logits in tap-major order + their per-sample column sums from ONE GEMM; GroupNorm
-            # becomes a per-(sample, column) affine applied inside the LocalConv kernel, which also does bn + SiLU and the pooled
-            # descriptor.  Fewer launches and HBM passes, but the in-place weight-tile prologue makes the kernel
-            # shared-memory-latency bound, so it is not the default.
-            l, cs, cq = tc.gemm_bf16_samplestats(e, p["we2p"], H * W, shift=p["be2p"])
-            v = tc.gemm_bf16(x, p["wv"], scale=p["v_ss"][0], shift=p["v_ss"][1])
-            out = fused.cot_eval_tail_fused(v.view(B, H, W, C).permute(0, 3, 1, 2), l, cs, cq, None, p["gnw_p"], p["gnb_p"],
-                                            float(self.embed[4].eps), gc, p["bn_ss"], k, self.se)
-            if out is not None:
-                return out
-        if self.eval_samplestats and H * W >= 32:
-            # (opt-in) GroupNorm statistics from the logits GEMM's own epilogue: saves the statistics pass over l, but the per-sample
-            # epilogue pays one global atomic per row group and column (and adds in a run-dependent order)
-            l, cs, cq = tc.gemm_bf16_samplestats(e, p["we2"], H * W, shift=p["be2"])
-            v = tc.gemm_bf16(x, p["wv"], scale=p["v_ss"][0], shift=p["v_ss"][1])
-            J = l.shape[1]
-            w = fused.group_norm9_from_colsums(l.view(B, H, W, J).permute(0, 3, 1, 2), self.embed[4], gc, cs, cq, None)
-        else:
-            l = tc.gemm_bf16(e, p["we2"], shift=p["be2"])
-            v = tc.gemm_bf16(x, p["wv"], scale=p["v_ss"][0], shift=p["v_ss"][1])
-            J = l.shape[1]
-            w = fused.group_norm9(l.view(B, H, W, J).permute(0, 3, 1, 2), self.embed[4], gc)
+        l = tc.gemm_bf16(e, p["we2"], shift=p["be2"])
+        v = tc.gemm_bf16(x, p["wv"], scale=p["v_ss"][0], shift=p["v_ss"][1])
+        J = l.shape[1]
+        w = fused.group_norm9(l.view(B, H, W, J).permute(0, 3, 1, 2), self.embed[4], gc)
         u = fused.AggTapFn.apply(v.view(B, H, W, C).permute(0, 3, 1, 2), w, 1, gc)
         return fused.cot_tail(u, k, self.bn, self.se)
 
@@ -264,11 +229,6 @@ class CotLayer(nn.Module):
     #: pixels (B*H*W) below which the backend degrades to "tc_e0": on the 14x14 / 7x7 stages the fixed per-launch costs of the
     #: all-wgmma path outweigh its byte savings
     tc_min_pixels = int(os.environ.get("COTB200_TC_MIN_PIXELS", "100000"))
-    #: inference: GroupNorm-apply, LocalConv, bn + SiLU and the pooling in ONE kernel (cotb200_cot_agg_eval); default 0 = separate
-    #: kernels (the fused kernel is shared-memory-latency bound)
-    eval_fused_agg = os.environ.get("COTB200_EVAL_FUSED_AGG", "0") != "0"
-    #: inference: GroupNorm statistics from the logits GEMM epilogue (cotb200_gemm_bf16_samplestats) instead of gn9_stats
-    eval_samplestats = os.environ.get("COTB200_EVAL_SAMPLESTATS", "0") != "0"
 
     def forward(self, x):
         B, C, H, W = x.shape

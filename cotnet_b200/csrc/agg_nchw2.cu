@@ -8,7 +8,6 @@
 //   * interior fast path without any predication, edge path with zero fill;
 //   * bf16/fp16 are widened to fp32 for the FMA (exact products, fp32 accumulation).
 // Requires W % PXV == 0 (56, 28 -> 4; 14 -> 2); other widths use the first-generation scalar kernels.
-#include <cstdlib>
 #include "common.cuh"
 
 namespace cotb200 {
@@ -223,14 +222,8 @@ int nchw2_bwd(int N, int C, int H, int W, int wc, long long dy_sn, const T* dy, 
     dim3 grid((H * (W / pxv) + 255) / 256, N * wc);
     const int rep = C / wc;
     COTB200_PROF_B(dx && dw ? "agg3_bwd_nchw2_dxdw" : (dx ? "agg3_bwd_nchw2_dx" : "agg3_bwd_nchw2_dw"), ((double)N * H * W) * ((dx && dw ? 3.0 : 2.0) * C + (dx && dw ? 18.0 : 9.0) * wc) * sizeof(T));
-    // COTB200_NCHW_SPLIT=1: fp32 dX and dW as two launches (reads x and dy twice; kept as a switch).
-    static int split_env = -1;
-    if (split_env < 0) { const char* e = getenv("COTB200_NCHW_SPLIT"); split_env = (e && e[0] == '1') ? 1 : 0; }
-    const bool split = split_env && sizeof(T) == 4 && dx && dw;
 #define NCHW2_LAUNCH(P)                                                                                              \
-  if (split) { agg3_bwd_nchw2_kernel<T, P, true, false><<<grid, 256, 0, st>>>(dy, x, w, dx, nullptr, C, H, W, wc, rep, dy_sn); \
-               agg3_bwd_nchw2_kernel<T, P, false, true><<<grid, 256, 0, st>>>(dy, x, w, nullptr, dw, C, H, W, wc, rep, dy_sn); } \
-  else if (dx && dw) agg3_bwd_nchw2_kernel<T, P, true, true><<<grid, 256, 0, st>>>(dy, x, w, dx, dw, C, H, W, wc, rep, dy_sn); \
+  if (dx && dw) agg3_bwd_nchw2_kernel<T, P, true, true><<<grid, 256, 0, st>>>(dy, x, w, dx, dw, C, H, W, wc, rep, dy_sn); \
   else if (dx) agg3_bwd_nchw2_kernel<T, P, true, false><<<grid, 256, 0, st>>>(dy, x, w, dx, dw, C, H, W, wc, rep, dy_sn); \
   else agg3_bwd_nchw2_kernel<T, P, false, true><<<grid, 256, 0, st>>>(dy, x, w, dx, dw, C, H, W, wc, rep, dy_sn);
     if (pxv == 4) { NCHW2_LAUNCH(4) } else { NCHW2_LAUNCH(2) }

@@ -18,7 +18,6 @@
 // Requirements: K=3, stride 1, pad 1, heads 1, dense NCHW, W % PXV == 0, W*sizeof(T) % 16 == 0 (TMA global strides):
 // fp32 W in {56, 28, ..}, 16-bit W = 56; everything else stays on agg_nchw2.cu / the generic kernels.
 #include <cuda.h>
-#include <cstdlib>
 #include "common.cuh"
 #include "tma.cuh"
 
@@ -230,12 +229,6 @@ static bool nt_make_map(CUtensorMap* m, const void* base, const long long (&d)[5
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static bool nchw_tma_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("COTB200_AGG_NCHW_TMA"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
-
 static inline int nt_round_up(int a, int b) { return (a + b - 1) / b * b; }
 
 // mode 0: A = x, B = w, out = y ; mode 1: A = dy, B = w, out = dx ; mode 2: A = x, B = dy, out = dw.
@@ -245,7 +238,7 @@ template <typename T>
 int nchw_tma_launch(int mode, int N, int C, int H, int W, int wc, long long a_sn, long long b_sn, long long out_sn, const T* A,
                     const T* Bp, T* out, cudaStream_t st, int* rc) {
   if constexpr (std::is_same<T, double>::value) { return 0; } else {
-    if (!nchw_tma_enabled() || C % wc) return 0;
+    if (C % wc) return 0;
     const int rep = C / wc, es = (int)sizeof(T), al = 16 / es;
     int pxv = 0;
     if (W % 4 == 0) pxv = 4; else if (W % 2 == 0 && es == 4) pxv = 2;

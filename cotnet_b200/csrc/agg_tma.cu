@@ -13,7 +13,6 @@
 //   * CTAs are persistent (grid = resident CTAs), tiles = (sample, band of TH image rows) taken round-robin.
 // Weight layout: COTB200_NHWC_TAP (tap-major chunks of gc weight channels) -- the block-internal layout.
 #include <cuda.h>
-#include <cstdlib>
 #include "common.cuh"
 #include "tma.cuh"
 
@@ -251,180 +250,6 @@ agg3_dw_tma_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_consta
 }
 
 
-// ------------------------------------------------------------------------------------------------ fused inference kernel
-// out = SiLU(bn(LocalConv(v, GroupNorm(l))))  and  psum[n, c] += sum_px (out + k)     (models/cotnet.py:85-98, eval mode)
-//   * prologue: the weight tile arrives as the RAW logits l (tap-major); the consumer warps turn it into the normalised
-//     weights in place, w = l * a[n, j] + c[n, j] (a, c per sample and logit column: GroupNorm statistics + affine, from
-//     cotb200_gn9_from_colsums) -- once per weight element instead of once per use (8 channels share a weight), and the
-//     normalised weights never exist in HBM;
-//   * main loop: as agg3_fwd_tma_kernel;
-//   * epilogue: eval-mode BatchNorm (scale/shift) + SiLU on the accumulators, the result is stored, and (out + k) is pooled per
-//     channel: registers -> warp shuffle over the lanes that own the same channel packet -> shared memory -> one global atomic
-//     per (tile, channel).  The separate GroupNorm-apply and pooling passes of the block disappear.
-struct AggEvalP {
-  const float2* coef;        // [N, J] (a, c)
-  const float* scale;        // [C] eval BatchNorm folded
-  const float* shift;
-  const void* k;             // [N, H, W, C] like the output
-  float* psum;               // [N, C]
-};
-
-template <typename T>
-__global__ void __launch_bounds__(1024, 1)
-agg3_eval_tma_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapW, T* __restrict__ y,
-                     const AggTmaP p, const AggEvalP q) {
-  constexpr int VEC = 16 / (int)sizeof(T);
-  extern __shared__ __align__(1024) uint8_t at_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ __align__(8) uint64_t s_full[AT_MAX_STAGES], s_empty[AT_MAX_STAGES];
-  __shared__ __align__(16) float2 s_coef[576];
-  __shared__ __align__(16) float s_ss[2][512];
-  __shared__ float s_pool[2][512];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ncw = (blockDim.x >> 5) - 1;
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapX) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
-    for (int s = 0; s < p.stages; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), ncw); }
-    mbar_init_fence();
-  }
-  for (int i = threadIdx.x; i < p.C; i += blockDim.x) {
-    s_ss[0][i] = q.scale[i]; s_ss[1][i] = q.shift[i];
-    s_pool[0][i] = 0.f; s_pool[1][i] = 0.f;
-  }
-  __syncthreads();
-  if (warp == 0) {
-    at_producer<T>(mapX, mapW, p, smem, s_full, s_empty, lane);
-  } else {
-    const int ct = threadIdx.x - 32, nct = ncw * 32;
-    const int CQ = p.C / VEC;
-    const int items = p.TH * p.W * CQ;
-    const int Wp = p.W + 2;
-    constexpr int MAXI = 2;
-    int i_hl[MAXI], i_rc[MAXI], i_xb[MAXI], i_ch[MAXI], i_wb[MAXI], i_ob[MAXI], i_c0[MAXI];
-#pragma unroll
-    for (int kk = 0; kk < MAXI; ++kk) {
-      const int item = ct + kk * nct;
-      i_hl[kk] = -1; i_c0[kk] = 0;
-      if (item < items) {
-        const int qq = item % CQ, px = item / CQ;
-        const int hl = px / p.W, wl = px - hl * p.W;
-        const int c0 = qq * VEC;
-        const int g0 = (c0 / p.Cf) * p.wcf + (c0 % p.Cf) % p.wcf;
-        const int cb = c0 * (int)sizeof(T);
-        const int e0 = (g0 / p.gc) * 9 * p.gc + g0 % p.gc;
-        i_hl[kk] = hl;
-        i_rc[kk] = (hl + 1) * Wp + wl + 1;
-        i_xb[kk] = (cb >> 7) * p.slab_bytes;
-        i_ch[kk] = (cb >> 4) & 7;
-        i_wb[kk] = (px * p.J + e0) * (int)sizeof(T);
-        i_ob[kk] = (hl * p.W + wl) * p.y_sp + c0;
-        i_c0[kk] = c0;
-      }
-    }
-    // all items of a thread share the channel packet when the consumer count is a multiple of CQ (host guarantees it)
-    const uint32_t smem_base = smem_u32(smem);
-    const int wtap = p.gc * (int)sizeof(T);
-    const int JP = p.J / VEC;                                  // 16-byte packets per weight row
-    const int npk = p.TH * p.W * JP;
-    const T* kg = reinterpret_cast<const T*>(q.k);
-    int it = 0, last_n = -1;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      const int s = it % p.stages;
-      const uint32_t ph = (it / p.stages) & 1;
-      const int n = tile / p.bands, h0 = (tile - n * p.bands) * p.TH;
-      const int par = it & 1;
-      if (n != last_n) {                                        // (a, c) of this sample -> shared memory
-        asm volatile("bar.sync 2, %0;" ::"r"(nct) : "memory");  // nobody still reads the previous sample's table
-        // stored element-major, [VEC][JP]: the prologue's lanes walk jp, so lane-consecutive float2 reads are conflict-free
-        for (int j = ct; j < p.J; j += nct) s_coef[(j % VEC) * JP + j / VEC] = __ldg(q.coef + (long long)n * p.J + j);
-        last_n = n;
-      }
-      // k of this thread's pixels: issued now, consumed in the epilogue -- the global-load latency hides behind the TMA wait,
-      // the prologue and the tap loop (loading it at the point of use exposes its latency per item)
-      const T* kt = kg + n * p.y_sn + (long long)h0 * p.W * p.y_sp;
-      Pack<T, VEC> kpre[MAXI];
-#pragma unroll
-      for (int kk = 0; kk < MAXI; ++kk)
-        if (i_hl[kk] >= 0 && h0 + i_hl[kk] < p.H) kpre[kk] = ld_pack<T, VEC>(kt + i_ob[kk]);
-      mbar_wait(smem_u32(&s_full[s]), ph);
-      const uint32_t xs = smem_base + (uint32_t)(s * p.stage_bytes);
-      const uint32_t ws = xs + (uint32_t)(p.slabs * p.slab_bytes);
-      asm volatile("bar.sync 2, %0;" ::"r"(nct) : "memory");    // table visible; every warp has seen the stage arrive
-      // ---- prologue: GroupNorm affine on the weight tile, in place
-      for (int pk = ct; pk < npk; pk += nct) {
-        const int row = pk / JP, jp = pk - row * JP;
-        const uint32_t addr = ws + (uint32_t)((row * p.J + jp * VEC) * (int)sizeof(T));
-        Pack<T, VEC> lv = lds_pack<T, VEC>(addr);
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) {
-          const float2 ac = s_coef[i * JP + jp];
-          lv.v[i] = Elem<T>::from(fmaf(to_acc(lv.v[i]), ac.x, ac.y));
-        }
-        const uint4 u = *reinterpret_cast<const uint4*>(&lv);
-        asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(u.x), "r"(u.y), "r"(u.z), "r"(u.w) : "memory");
-      }
-      asm volatile("bar.sync 2, %0;" ::"r"(nct) : "memory");
-      T* yt = y + n * p.y_sn + (long long)h0 * p.W * p.y_sp;
-      float pacc[VEC];
-#pragma unroll
-      for (int i = 0; i < VEC; ++i) pacc[i] = 0.f;
-#pragma unroll
-      for (int kk = 0; kk < MAXI; ++kk) {
-        if (i_hl[kk] < 0 || h0 + i_hl[kk] >= p.H) continue;
-        const uint32_t xb = xs + (uint32_t)i_xb[kk];
-        const uint32_t wb = ws + (uint32_t)i_wb[kk];
-        float acc[VEC];
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
-#pragma unroll
-        for (int t = 0; t < 9; ++t) {
-          const int r = i_rc[kk] + (t / 3 - 1) * Wp + (t % 3 - 1);
-          const Pack<T, VEC> wv = lds_pack<T, VEC>(wb + t * wtap);
-          const Pack<T, VEC> xv = lds_pack<T, VEC>(xb + r * 128 + ((i_ch[kk] ^ (r & 7)) << 4));
-#pragma unroll
-          for (int i = 0; i < VEC; ++i) acc[i] = mfma<T>(wv.v[i], xv.v[i], acc[i]);
-        }
-        const Pack<T, VEC> kv = kpre[kk];
-        Pack<T, VEC> o;
-        float bsc[VEC], bsh[VEC];                               // folded BatchNorm of the channel packet: 128-bit shared loads
-#pragma unroll
-        for (int i = 0; i < VEC; i += 4) {
-          *reinterpret_cast<float4*>(&bsc[i]) = *reinterpret_cast<const float4*>(&s_ss[0][i_c0[kk] + i]);
-          *reinterpret_cast<float4*>(&bsh[i]) = *reinterpret_cast<const float4*>(&s_ss[1][i_c0[kk] + i]);
-        }
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) {
-          const float z = fmaf(acc[i], bsc[i], bsh[i]);
-          float sg;
-          if constexpr (sizeof(T) == 2) { float th; asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(0.5f * z)); sg = fmaf(0.5f, th, 0.5f); }
-          else sg = __fdividef(1.f, 1.f + __expf(-z));
-          o.v[i] = Elem<T>::from(z * sg);
-          pacc[i] += to_acc(o.v[i]) + to_acc(kv.v[i]);          // pool what is stored (bf16-rounded), like a separate pass would
-        }
-        st_pack<T, VEC>(yt + i_ob[kk], o);
-      }
-      // the tile was WRITTEN by the generic proxy (prologue); order those writes before the TMA refill of the stage
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&s_empty[s]));        // this warp is done with the stage
-      // ---- pooled (out + k): lanes owning the same channel packet are CQ apart
-      for (int off = CQ; off < 32; off <<= 1)
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) pacc[i] += __shfl_xor_sync(0xffffffffu, pacc[i], off);
-      if (lane < CQ || CQ >= 32) {
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) atomicAdd(&s_pool[par][i_c0[0] + i], pacc[i]);
-      }
-      asm volatile("bar.sync 2, %0;" ::"r"(nct) : "memory");
-      for (int c = ct; c < p.C; c += nct) {
-        atomicAdd(q.psum + (long long)n * p.C + c, s_pool[par][c]);
-        s_pool[par][c] = 0.f;
-      }
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------ host
 typedef CUresult (*AtEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -484,15 +309,12 @@ struct Nhwc2Args {
 // returns 1 if handled (rc in *rc), 0 if the caller should use the register-resident kernels
 struct AtLaunch { AggTmaP p; CUtensorMap ma, mb; int threads, smem, grid; };
 
-// geometry, tensor maps and launch shape shared by the forward / dX / dW kernels and the fused inference kernel;
+// geometry, tensor maps and launch shape of the forward / dX / dW kernels;
 // returns false when the TMA path cannot take the call
 template <typename T>
 static bool at_setup(int mode, const Nhwc2Args& a, const T* A, const T* Bp, const T* out, AtLaunch& L) {
   if constexpr (std::is_same<T, double>::value) { return false; } else {
     constexpr int VEC = 16 / (int)sizeof(T);
-    static int disabled = -1;
-    if (disabled < 0) { const char* e = getenv("COTB200_AGG_TMA"); disabled = (e && e[0] == '0') ? 1 : 0; }
-    if (disabled) return false;
     if (a.layout != COTB200_NHWC_TAP) return false;
     const int Cf = a.C / a.fold, wcf = a.wc / a.fold;
     if ((a.C * (int)sizeof(T)) % 128 || wcf % VEC || a.gc < VEC || a.gc % VEC || a.wc % a.gc) return false;
@@ -600,36 +422,6 @@ static int agg_tma_launch(int mode, const Nhwc2Args& a, const T* A, const T* Bp,
   }
 }
 
-// fused inference forward; returns 1 if handled
-template <typename T>
-int agg_tma_eval(const Nhwc2Args& a, const T* v, const T* l, T* y, const float* coef, const float* scale, const float* shift, const T* k,
-                 float* psum, cudaStream_t st, int* rc) {
-  if constexpr (std::is_same<T, double>::value) { return 0; } else {
-    constexpr int VEC = 16 / (int)sizeof(T);
-    AtLaunch L;
-    if (!at_setup<T>(0, a, v, l, y, L)) return 0;
-    const int CQ = a.C / VEC;
-    if (a.C > 512 || L.p.J > 576 || (CQ & (CQ - 1))) return 0;          // static tables; power-of-two packet count for the shuffles
-    // every item of a thread must own the same channel packet: (consumer threads) % CQ == 0
-    int cw = L.threads / 32 - 1;
-    while (cw > 0 && (cw * 32) % CQ) --cw;
-    if (cw <= 0 || (long long)L.p.TH * a.W * CQ > 2LL * cw * 32) return 0;
-    const int threads = (cw + 1) * 32;
-    static PerDevFlag cfgd;
-    if (bool& cfgf = cfgd.get(); !cfgf) {
-      cudaError_t e = cudaFuncSetAttribute(agg3_eval_tma_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024);
-      if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(agg eval): %s", cudaGetErrorString(e)); *rc = (int)e; return 1; }
-      cfgf = true;
-    }
-    if (L.smem > 204 * 1024) return 0;
-    AggEvalP q{reinterpret_cast<const float2*>(coef), scale, shift, k, psum};
-    COTB200_PROF_B("agg3_eval_tma", ((double)a.N * a.H * a.W) * (3.0 * a.C + 9.0 * a.wc) * sizeof(T));
-    agg3_eval_tma_kernel<T><<<L.grid, threads, L.smem, st>>>(L.ma, L.mb, y, L.p, q);
-    *rc = check_launch("agg3_eval_tma");
-    return 1;
-  }
-}
-
 template <typename T> int agg_tma_fwd(const Nhwc2Args& a, const T* x, const T* w, T* y, cudaStream_t st, int* rc) {
   return agg_tma_launch<T>(0, a, x, w, y, st, rc);
 }
@@ -641,7 +433,6 @@ template <typename T> int agg_tma_dw(const Nhwc2Args& a, const T* dy, const T* x
 }
 
 #define COTB200_INST3(T)                                                                              \
-  template int agg_tma_eval<T>(const Nhwc2Args&, const T*, const T*, T*, const float*, const float*, const float*, const T*, float*, cudaStream_t, int*); \
   template int agg_tma_fwd<T>(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);          \
   template int agg_tma_dx<T>(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);           \
   template int agg_tma_dw<T>(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);

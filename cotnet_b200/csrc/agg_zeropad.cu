@@ -481,14 +481,12 @@ template <typename T> int nhwc2_fwd(const Nhwc2Args&, const T*, const T*, T*, cu
 template <typename T> int agg_tma_fwd(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);   // agg_tma.cu
 template <typename T> int agg_tma_dx(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
 template <typename T> int agg_tma_dw(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
-template <typename T> int agg_tma_eval(const Nhwc2Args&, const T*, const T*, T*, const float*, const float*, const float*, const T*, float*,
-                                       cudaStream_t, int*);
 template <typename T> int nhwc2_dx(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
 template <typename T> int nhwc2_dw(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
 // TMA-pipelined NCHW kernels (agg_nchw_tma.cu): mode 0 fwd / 1 dX / 2 dW
 template <typename T> int nchw_tma_launch(int, int, int, int, int, int, long long, long long, long long, const T*, const T*, T*,
                                           cudaStream_t, int*);
-// small-plane NCHW kernels (agg_nchw_plane.cu): mode 0 fwd / 1 dX / 2 dW / 3 dX + dW
+// small-plane NCHW backward kernels (agg_nchw_plane.cu): mode 1 dX / 2 dW / 3 dX + dW
 template <typename T> int nchw_plane_launch(int, int, int, int, int, int, long long, long long, long long, const T*, const T*, const T*, T*, T*,
                                             cudaStream_t, int*);
 // second-generation NCHW kernels (agg_nchw2.cu)
@@ -586,7 +584,6 @@ static int fwd_impl(const Geo& g, const T* x, const T* w, T* y, cudaStream_t st)
   }
   if (g.layout == COTB200_NCHW && nofold(g) && fits32(g) && is_same3(g, 3) && g.w_sn == (long long)g.wc * 9 * g.H * g.W) {
     int rc2 = 0;
-    if (g.H * g.W <= 256 && nchw_plane_launch<T>(0, g.N, g.C, g.H, g.W, g.wc, g.x_sn, g.y_sn, g.w_sn, x, (const T*)nullptr, w, y, (T*)nullptr, st, &rc2)) return rc2;
     if (g.x_sn == (long long)g.C * g.H * g.W &&
         nchw_tma_launch<T>(0, g.N, g.C, g.H, g.W, g.wc, g.x_sn, 0, g.y_sn, x, w, y, st, &rc2)) return rc2;
     if (nchw2_fwd<T>(g.N, g.C, g.H, g.W, g.wc, g.y_sn, x, w, y, st, &rc2)) return rc2;
@@ -897,27 +894,6 @@ extern "C" int cotb200_agg_zeropad_mix_merge_bwd(const cotb200_agg_desc* d, int 
       rc = check_launch("agg_mix_merge_dw");
     }
     return rc;
-  });
-  return 0;
-}
-
-
-// ---- fused inference step of the CoT block: GroupNorm affine on the logits + LocalConv + eval BatchNorm + SiLU + pooled (y + k)
-// (models/cotnet.py:85-98); TAP layout, 3x3 / stride 1 / pad 1 only.  Returns COTB200_EUNSUPPORTED when the TMA kernel cannot take
-// the geometry (the caller then runs the separate kernels).
-extern "C" int cotb200_cot_agg_eval(const cotb200_agg_desc* d, const void* v, const void* l, const float* coef, const float* bn_scale,
-                                    const float* bn_shift, const void* k, void* y, float* psum, void* stream) {
-  Geo g;
-  int rc = resolve(d, g);
-  if (rc) return rc;
-  if (!v || !l || !coef || !bn_scale || !bn_shift || !k || !y || !psum) { set_error("cot_agg_eval: NULL pointer"); return COTB200_ENULL; }
-  if (g.layout != COTB200_NHWC_TAP || !is_same3(g, 3) || !nofold(g)) { set_error("cot_agg_eval: needs the NHWC_TAP layout, 3x3/s1/p1, no fold"); return COTB200_EUNSUPPORTED; }
-  cudaStream_t st = (cudaStream_t)stream;
-  COTB200_DISPATCH_DTYPE(d->dtype, {
-    int rc2 = 0;
-    if (agg_tma_eval<T>(nhwc2_args(g), (const T*)v, (const T*)l, (T*)y, coef, bn_scale, bn_shift, (const T*)k, psum, st, &rc2)) return rc2;
-    set_error("cot_agg_eval: geometry not supported by the TMA kernel");
-    return COTB200_EUNSUPPORTED;
   });
   return 0;
 }

@@ -380,16 +380,10 @@ gn72_bwd_apply_kernel(const T* __restrict__ dg, const T* __restrict__ l, const f
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static bool gn72_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("COTB200_GN72"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
-
 // usable when the tensor is a flat array of 72-element blocks: wc in {8,16,32,64} = every CoTNet stage (gc == 8 for the
 // permuting kernels), 16-byte aligned pointers, 16-bit or fp32 elements.
 bool gn72_ok(int dtype, int wc, int gc, bool permuting, const void* p0, const void* p1, const void* p2) {
-  if (!gn72_enabled() || dtype == COTB200_F64) return false;
+  if (dtype == COTB200_F64) return false;
   if (wc != 8 && wc != 16 && wc != 32 && wc != 64) return false;      // chunk count must divide the warp (shuffles) and the tile
   if (permuting && gc != 8) return false;
   return aligned16(p0) && (!p1 || aligned16(p1)) && (!p2 || aligned16(p2));

@@ -437,43 +437,3 @@ extern "C" int cotb200_se_eval(int B, int C, int A, const float* psum, float inv
   se_fc_kernel<1><<<g2, 256, smem, st>>>(z_scratch, 1.f, W3, b3, nullptr, nullptr, a, B, A, 2 * C);
   return check_launch("se_eval fc2");
 }
-
-// ------------------------------------------------------------------------------------------------ radix-2 recombination of stored y
-// out[b, px, c] = a[b, c, 0] * y + a[b, c, 1] * k      (models/cotnet.py:101-104 when y = SiLU(bn(.)) is already materialised by the
-// fused inference kernel): 3 C-passes, 16-byte packets, NHWC rows.
-namespace cotb200 {
-template <typename T, int VEC>
-__global__ void __launch_bounds__(256)
-mix2_kernel(const T* __restrict__ y, const T* __restrict__ k, const float* __restrict__ a, T* __restrict__ out, long long total, int CQ,
-            long long HWCQ) {
-  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
-    const long long b = i / HWCQ;
-    const int q = (int)(i % CQ);
-    const Pack<T, VEC> yv = ld_pack<T, VEC>(y + i * VEC), kv = ld_pack<T, VEC>(k + i * VEC);
-    const float* ab = a + ((long long)b * CQ + q) * VEC * 2;
-    Pack<T, VEC> o;
-#pragma unroll
-    for (int e = 0; e < VEC; ++e) o.v[e] = Elem<T>::from(fmaf(__ldg(ab + 2 * e), to_acc(yv.v[e]), __ldg(ab + 2 * e + 1) * to_acc(kv.v[e])));
-    st_pack<T, VEC>(out + i * VEC, o);
-  }
-}
-}  // namespace cotb200
-
-extern "C" int cotb200_mix2(int dtype, int B, int HW, int C, const void* y, const void* k, const float* a, void* out, void* stream) {
-  if (!y || !k || !a || !out) { set_error("mix2: NULL pointer"); return COTB200_ENULL; }
-  if (B <= 0 || HW <= 0 || C <= 0) { set_error("mix2: non-positive dims"); return COTB200_EINVAL; }
-  if (dtype == COTB200_F64) { set_error("mix2: fp64 not supported"); return COTB200_EDTYPE; }
-  cudaStream_t st = (cudaStream_t)stream;
-  COTB200_DISPATCH_DTYPE(dtype, {
-    if constexpr (!std::is_same<T, double>::value) {
-      constexpr int VEC = 16 / (int)sizeof(T);
-      if (C % VEC || !aligned16(y) || !aligned16(k) || !aligned16(out)) { set_error("mix2: C %% %d != 0 or unaligned tensors", VEC); return COTB200_EALIGN; }
-      const int CQ = C / VEC;
-      const long long total = (long long)B * HW * CQ;
-      COTB200_PROF_B("mix2", (double)B * HW * C * 3 * sizeof(T));
-      mix2_kernel<T, VEC><<<stream_grid(total), 256, 0, st>>>((const T*)y, (const T*)k, a, (T*)out, total, CQ, (long long)HW * CQ);
-      return check_launch("mix2");
-    }
-  });
-  return 0;
-}

@@ -53,7 +53,6 @@ struct TcParams {
   const float* shift;       // [N] or null (=0)
   float* col_sum;           // [N] or null
   float* col_sqsum;         // [N] or null
-  int rows_per_sample;      // > 0: col_sum / col_sqsum are PER SAMPLE, [M / rows_per_sample, N] (GroupNorm statistics of the logits)
   DetArena det;             // column statistics: per-CTA totals leave through det_finish (common.cuh)
 };
 
@@ -140,7 +139,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant_
     for (int s = 0; s < TC_STAGES; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), 2); }
     mbar_init_fence();
   }
-  if (p.col_sum != nullptr && p.rows_per_sample == 0) {
+  if (p.col_sum != nullptr) {
     for (int i = threadIdx.x; i < 4 * 256; i += TC_THREADS) { (&s_sum[0][0])[i] = 0.f; (&s_sq[0][0])[i] = 0.f; }
     for (int i = threadIdx.x; i < 2 * p.N; i += TC_THREADS) s_tot[i] = 0.f;
   }
@@ -257,47 +256,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant_
                        ::"l"(&mapD), "r"(buf), "r"(n0 + sl * 64), "r"((int)m0) : "memory");
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       }
-      if (stats && p.rows_per_sample > 0 && et < 128) {
-        // PER-SAMPLE column sums of the staged slab (GroupNorm over the 9 taps x H x W of one sample, models/cotnet.py:56): a row
-        // group of 32 rows touches at most two samples (rows_per_sample >= 32 is checked on the host); two partial sets per
-        // thread, straight to the [sample, column] tables
-        const int tp = et & 31, rg = et >> 5;
-        if (sl * 64 + 2 * tp < p.bn && n0 + sl * 64 + 2 * tp < p.N) {
-          const long long row0 = m0 + rg * 32;
-          const int s_lo = (int)(row0 / p.rows_per_sample);
-          const int rb = (int)min((long long)32, (long long)(s_lo + 1) * p.rows_per_sample - row0);   // rows [0, rb) belong to sample s_lo
-          const int nrow = min(32, min(rows_valid, (int)min((long long)TC_BM, p.M - m0)) - rg * 32);
-          const __nv_bfloat16 one = one_of<__nv_bfloat16>();
-          float sa[2] = {0.f, 0.f}, qa[2] = {0.f, 0.f}, sb[2] = {0.f, 0.f}, qb[2] = {0.f, 0.f};
-          uint32_t w2[32];
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr) {
-            const int row = rg * 32 + rr;
-            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w2[rr]) : "r"(buf + (uint32_t)(row * 128 + (((tp >> 2) ^ (row & 7)) << 4) + (tp & 3) * 4)));
-          }
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr) {
-            if (rr < nrow) {
-              const __nv_bfloat16 lo = __ushort_as_bfloat16((unsigned short)(w2[rr] & 0xFFFFu)), hi = __ushort_as_bfloat16((unsigned short)(w2[rr] >> 16));
-              const int h = rr < rb ? 0 : 1;
-              if (h == 0) { sa[0] = mfma<__nv_bfloat16>(lo, one, sa[0]); qa[0] = mfma<__nv_bfloat16>(lo, lo, qa[0]);
-                            sb[0] = mfma<__nv_bfloat16>(hi, one, sb[0]); qb[0] = mfma<__nv_bfloat16>(hi, hi, qb[0]); }
-              else        { sa[1] = mfma<__nv_bfloat16>(lo, one, sa[1]); qa[1] = mfma<__nv_bfloat16>(lo, lo, qa[1]);
-                            sb[1] = mfma<__nv_bfloat16>(hi, one, sb[1]); qb[1] = mfma<__nv_bfloat16>(hi, hi, qb[1]); }
-            }
-          }
-          const int col = n0 + sl * 64 + 2 * tp;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if ((h == 0 && nrow > 0) || (h == 1 && nrow > rb)) {
-              const long long srow = (long long)(s_lo + h) * p.N + col;
-              atomicAdd(p.col_sum + srow, sa[h]); atomicAdd(p.col_sqsum + srow, qa[h]);
-              if (col + 1 < p.N) { atomicAdd(p.col_sum + srow + 1, sb[h]); atomicAdd(p.col_sqsum + srow + 1, qb[h]); }
-            }
-          }
-        }
-      }
-      if (stats && p.rows_per_sample == 0 && et < 128) {
+      if (stats && et < 128) {
         // column sums of the staged slab: thread = (column pair tp, row group rg of 32 rows); a warp reads one whole 128-byte
         // row per step (conflict-free under the swizzle)
         const int tp = et & 31, rg = et >> 5;
@@ -325,7 +284,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant_
         }
       }
     }
-    if (stats && p.rows_per_sample == 0) {
+    if (stats) {
       consumer_bar();                                  // every thread's shared-memory partials are in
       for (int j = et; j < p.bn; j += TC_CONSUMERS) {  // one owner per column: the CTA's totals add up in tile order
         if (n0 + j < p.N) {
@@ -336,7 +295,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant_
     }
   }
   if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");     // all stores complete before the CTA exits
-  if (stats && p.rows_per_sample == 0) {
+  if (stats) {
     consumer_bar();
     const int n = 2 * p.N;
     for (int i = et; i < n; i += TC_CONSUMERS) p.det.scr[(size_t)blockIdx.x * n + i] = s_tot[i];
@@ -402,7 +361,7 @@ static int tc_launch(const CUtensorMap& a1, const CUtensorMap& b1, const CUtenso
   int rcd = make_map_2d(&dmap, p.D, p.M, p.N, p.ldd, p.rows_per_tile);
   if (rcd) return rcd;
   // two slab buffers (+ statistics partials of a tile and the CTA's column totals)
-  const int out_bytes = 2 * TC_BM * 128 + ((p.col_sum && p.rows_per_sample == 0) ? 2 * 4 * 256 * 4 + 2 * p.N * 4 : 0);
+  const int out_bytes = 2 * TC_BM * 128 + (p.col_sum ? 2 * 4 * 256 * 4 + 2 * p.N * 4 : 0);
   const int a_bytes = TC_BM * TC_BK * 2, b_bytes = p.bn * TC_BK * 2;
   const int stage_bytes = a_bytes + ((b_bytes + 1023) & ~1023);
   p.m_tiles = m_tiles;
@@ -428,7 +387,7 @@ static int tc_launch(const CUtensorMap& a1, const CUtensorMap& b1, const CUtenso
   int grid = per_sm * num_sms();                          // resident CTAs only: a second wave would start from a cold pipeline
   if (grid > total) grid = total;
   DetScratch ds;
-  if (p.col_sum && p.rows_per_sample == 0) {
+  if (p.col_sum) {
     if (p.N > 4096) { set_error("%s: N=%d too wide for the statistics epilogue", what, p.N); return COTB200_EUNSUPPORTED; }
     int rcs = ds.alloc(det_floats(grid, 2 * p.N), 1, st);
     if (rcs) return rcs;
@@ -441,7 +400,7 @@ static int tc_launch(const CUtensorMap& a1, const CUtensorMap& b1, const CUtenso
 }
 
 static int pick_bn_wide(int N);
-static int pick_bn(int N, int K = 1 << 30) {
+static int pick_bn(int N, int K) {
   // short contractions (K <= 128) with a wide output are epilogue-bound: the operands of a 256-column tile arrive in a fraction
   // of the time its epilogue takes.  Two CTAs per SM with 128-column tiles run two epilogues side by side (the re-read A tile is
   // small and comes from L2).
@@ -646,12 +605,9 @@ tc_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_co
 // returns 1 when the haloed-tile kernel took the convolution (*rc = status), 0 when conv mode of tc_gemm_kernel should run
 static int conv3x3_halo_launch(int B, int H, int W, int C, const void* X, long long ldx, const void* Wp, int bn, void* D, long long ldd,
                                const float* scale, const float* shift, int relu, float* col_sum, float* col_sqsum, cudaStream_t st, int* rc) {
-  static int mode = -2;                       // COTB200_CONV_HALO: 0 = off, 1 (default) = on
-  if (mode == -2) { const char* e = getenv("COTB200_CONV_HALO"); mode = e ? atoi(e) : 1; }
-  if (mode <= 0 || bn != 64 || C % 64 || W + 2 > 256 || ldx != C || ldd != C) return 0;
+  if (bn != 64 || C % 64 || W + 2 > 256 || ldx != C || ldd != C) return 0;
   const int Wpad = W + 2;
-  static int maxpx = -1;                      // COTB200_HALO_MAXPX: padded output pixels per work item (128 -> one M block, more ring stages)
-  if (maxpx < 0) { const char* e = getenv("COTB200_HALO_MAXPX"); maxpx = e ? atoi(e) : 256; if (maxpx < 128) maxpx = 128; if (maxpx > 256) maxpx = 256; }
+  const int maxpx = 256;                      // padded output pixels per work item: at most two 128-row M blocks
   int R = 0;
   for (int r = 1; r <= H; ++r) if (H % r == 0 && r * Wpad <= maxpx && r * W <= 256) R = r;
   if (R == 0) return 0;
@@ -730,27 +686,6 @@ extern "C" int cotb200_gemm_bf16(int M, int N, int K1, const void* A1, long long
   } else { a2 = a1; b2 = b1; }
   return tc_launch(a1, b1, a2, b2, p, (M + TC_BM - 1) / TC_BM, st, "tc_gemm_1x1",
                    2.0 * ((double)M * (K1 + K2 + N) + (double)N * (K1 + K2)));
-}
-
-// Same GEMM; col_sum / col_sqsum are accumulated PER SAMPLE of rows_per_sample consecutive rows: [M / rows_per_sample, N].
-extern "C" int cotb200_gemm_bf16_samplestats(int M, int N, int K1, const void* A1, long long lda1, const void* B1, long long ldb1, void* D,
-                                             long long ldd, const float* scale, const float* shift, int relu, int rows_per_sample,
-                                             float* samp_sum, float* samp_sqsum, void* stream) {
-  if (M <= 0 || N <= 0 || K1 <= 0) { set_error("gemm_bf16_samplestats: bad dims"); return COTB200_EINVAL; }
-  if (!A1 || !B1 || !D || !samp_sum || !samp_sqsum) { set_error("gemm_bf16_samplestats: NULL operand"); return COTB200_ENULL; }
-  if ((N & 7) || (K1 & 7) || (ldd & 7)) { set_error("gemm_bf16_samplestats: N, K, ldd must be multiples of 8"); return COTB200_EALIGN; }
-  if (rows_per_sample < 32 || M % rows_per_sample) { set_error("gemm_bf16_samplestats: rows_per_sample=%d must be >= 32 and divide M=%d", rows_per_sample, M); return COTB200_EINVAL; }
-  cudaStream_t st = (cudaStream_t)stream;
-  TcParams p{};
-  p.M = M; p.N = N; p.rows_per_tile = TC_BM; p.bn = pick_bn(N); p.mode = 0;
-  p.kb1 = (K1 + TC_BK - 1) / TC_BK; p.kb2 = 0;
-  p.relu = relu; p.ldd = ldd; p.D = (__nv_bfloat16*)D; p.scale = scale; p.shift = shift; p.col_sum = samp_sum; p.col_sqsum = samp_sqsum;
-  p.rows_per_sample = rows_per_sample;
-  CUtensorMap a1, b1;
-  int rc;
-  if ((rc = make_map_2d(&a1, A1, M, K1, lda1, TC_BM))) return rc;
-  if ((rc = make_map_2d(&b1, B1, N, K1, ldb1, p.bn))) return rc;
-  return tc_launch(a1, b1, a1, b1, p, (M + TC_BM - 1) / TC_BM, st, "tc_gemm_1x1", 2.0 * ((double)M * (K1 + N) + (double)N * K1));
 }
 
 // 3x3 / pad 1 / stride 1 convolution, NHWC bf16, with dense-per-N-tile prepared weights

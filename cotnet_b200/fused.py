@@ -41,7 +41,6 @@ class _ZeroArena:
     def __init__(self):
         self.buf = {}                  # device -> [buffer, used]
         self.active = False
-        self.escape_ok = False         # a trainer that consumes every gradient before the next step_begin() may set this (see _zeros_esc)
 
     def begin(self, device):
         ent = self.buf.get(device)
@@ -87,18 +86,6 @@ def _zeros(shape, device):
     if t is None:
         return torch.zeros(*shape, dtype=torch.float32, device=device)
     return t.view(*shape)
-
-
-def _zeros_esc(shape, device):
-    """Zeros that ESCAPE the autograd function as gradients (BatchNorm d-gamma / d-beta sums).  Plain torch.zeros in general -- a
-    gradient must survive until its owner reads it -- but a trainer that gathers every gradient inside the step (TrainStep: one gather
-    launch into the flat bucket before the next step_begin()) may take them from the pre-zeroed arena too: ~140 fill launches per
-    CoTNet-50 step less."""
-    return _zeros(shape, device) if _ARENA.escape_ok else torch.zeros(*shape, dtype=torch.float32, device=device)
-
-
-def arena_escape_ok(on=True):
-    _ARENA.escape_ok = bool(on)
 
 
 #: BatchNorm `num_batches_tracked += 1` bookkeeping: one tiny kernel per BatchNorm per step (~106 in CoTNet-50).  A trainer may defer
@@ -304,7 +291,7 @@ class BNActFn(Function):
             return (None,) * 8
         sums = None
         if batch or ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            sums = _zeros_esc((2, C,), x.device)       # escapes as dgamma/dbeta
+            sums = torch.zeros(2, C, dtype=torch.float32, device=x.device)  # escapes as dgamma/dbeta
         dx = torch.empty_like(x, memory_format=torch.channels_last)
         dres = torch.empty_like(x, memory_format=torch.channels_last) if (has_res and ctx.needs_input_grad[3]) else None
         _bn_bwd(lib, dt, B, H * W, C, dy, dy2, x, y, ss[0], ss[1], ss[2], ss[3], rcode, sums, batch, 1.0 / float(B * H * W), dx, dres,
@@ -371,7 +358,7 @@ class GroupNorm9Fn(Function):
         dg = dg.contiguous(memory_format=torch.channels_last)
         lib, st, dt = _lib.load(), _lib.stream_ptr(l), _lib.dtype_code(l)
         sums = torch.empty(2, B, wc, dtype=torch.float32, device=l.device)      # s1, s2 (written)
-        dgb = _zeros_esc((3, J,), l.device)            # dgamma, dbeta, dlbias (escape)
+        dgb = torch.zeros(3, J, dtype=torch.float32, device=l.device)  # dgamma, dbeta, dlbias (escape)
         work = _zeros((3 * B * J,), l.device)                                     # per-sample column partials
         want_db = lb32 is not None and ctx.needs_input_grad[5]
         _lib.check(lib.cotb200_gn9_bwd_sums(dt, B, HW, wc, ctx.gc, dg.data_ptr(), l.data_ptr(), _lib.ptr(lb32), mean.data_ptr(),
@@ -495,7 +482,7 @@ class CotTailFn(Function):
         grads = torch.autograd.grad(a, [p_leaf] + mlp_params, grad_outputs=S, allow_unused=True)
         dpn = grads[0].contiguous()                      # d/d(pooled mean); the kernels apply the 1/HW (pscale)
         mlp_grads = [None if g is None else g for g in grads[1:]]
-        sums = _zeros_esc((2, C,), u.device)          # escapes as dgamma/dbeta
+        sums = torch.zeros(2, C, dtype=torch.float32, device=u.device)  # escapes as dgamma/dbeta
         need_param = ctx.needs_input_grad[2] or ctx.needs_input_grad[3]
         if ctx.training or need_param:
             _lib.check(lib.cotb200_tail_bwd_dz_sums(dt, B, HW, C, dout.data_ptr(), u.data_ptr(), scale.data_ptr(), shift.data_ptr(),
@@ -674,60 +661,6 @@ def _cot_tail_eval(u, k, bn, se):
     return out
 
 
-def group_norm9_from_colsums(l, gn: torch.nn.GroupNorm, gc, csum, csq, lbias_in_stats):
-    """Inference GroupNorm(9 taps) whose statistics come from the logits GEMM's epilogue (per-sample column sums of the raw
-    accumulator, cotb200_gemm_bf16_samplestats): one tiny kernel turns them into mean / rstd, then the apply kernel.  `l` already
-    contains the embed.3 bias and so do the sums (they are taken from the stored logits): `lbias_in_stats` is None unless the
-    sums come from somewhere that has not seen the bias."""
-    B, J, H, W = l.shape
-    wc = J // 9
-    lib, st, dt = _lib.load(), _lib.stream_ptr(l), _lib.dtype_code(l)
-    mr = torch.empty(2, B * wc, dtype=torch.float32, device=l.device)
-    _lib.check(lib.cotb200_gn9_from_colsums(B, H * W, wc, 0, csum.data_ptr(), csq.data_ptr(), _lib.ptr(lbias_in_stats), float(gn.eps),
-                                            mr[0].data_ptr(), mr[1].data_ptr(), st), "gn9_from_colsums")
-    g32, b32 = _f32(gn.weight), _f32(gn.bias)
-    out = torch.empty_like(l, memory_format=torch.channels_last)
-    _lib.check(lib.cotb200_gn9_apply(dt, B, H * W, wc, gc, l.data_ptr(), None, mr[0].data_ptr(), mr[1].data_ptr(), g32.data_ptr(),
-                                     b32.data_ptr(), out.data_ptr(), st), "gn9_apply")
-    return out
-
-
-def cot_eval_tail_fused(v, l2d, csum, csq, lbias_p, gamma_p, beta_p, eps, gc, bn_ss, k, se):
-    """Inference tail of the CoT block from the logits GEMM on: coefficient kernel (GroupNorm statistics -> per-(sample, column)
-    affine), the fused LocalConv kernel (GroupNorm affine + aggregation + bn + SiLU + pooled (y + k)), the SE kernel, and the
-    recombination -- 4 launches for models/cotnet.py:85-104.  v, k: channels_last [B,C,H,W]; l2d: [B*H*W, 9C/8] tap-major logits
-    (bias included) with per-sample column sums csum / csq of the pre-bias accumulator.  Returns None when the fused kernel cannot
-    take the geometry (the caller then uses the separate kernels)."""
-    B, C, H, W = v.shape
-    wc = C // 8
-    lib, st, dt = _lib.load(), _lib.stream_ptr(v), _lib.dtype_code(v)
-    coef = torch.empty(B, 9 * wc, 2, dtype=torch.float32, device=v.device)
-    _lib.check(lib.cotb200_gn9_coef_from_colsums(B, H * W, wc, gc, csum.data_ptr(), csq.data_ptr(), _lib.ptr(lbias_p), gamma_p.data_ptr(),
-                                                 beta_p.data_ptr(), float(eps), coef.data_ptr(), st), "gn9_coef_from_colsums")
-    d = _lib.AggDesc()
-    d.n, d.c, d.h, d.w = B, C, H, W
-    d.heads, d.wc = 1, wc
-    d.kh = d.kw = 3
-    d.sh = d.sw = d.ph = d.pw = d.dh = d.dw = 1
-    d.ho, d.wo = H, W
-    d.dtype, d.layout, d.gc, d.fold = dt, _lib.NHWC_TAP, gc, 1
-    y = torch.empty_like(v, memory_format=torch.channels_last)
-    psum = torch.zeros(B, C, dtype=torch.float32, device=v.device)
-    rc = lib.cotb200_cot_agg_eval(d, v.data_ptr(), l2d.data_ptr(), coef.data_ptr(), bn_ss[0].data_ptr(), bn_ss[1].data_ptr(), k.data_ptr(),
-                                  y.data_ptr(), psum.data_ptr(), st)
-    if rc == -7:                                   # COTB200_EUNSUPPORTED
-        return None
-    _lib.check(rc, "cot_agg_eval")
-    w0, b0, s1, t1, w3, b3 = _se_eval_params(se)
-    a = torch.empty(B, C, 2, dtype=torch.float32, device=v.device)
-    zs = torch.empty(B, w0.shape[0], dtype=torch.float32, device=v.device)
-    _lib.check(lib.cotb200_se_eval(B, C, w0.shape[0], psum.data_ptr(), 1.0 / (H * W), w0.data_ptr(), _lib.ptr(b0), s1.data_ptr(),
-                                   t1.data_ptr(), w3.data_ptr(), _lib.ptr(b3), a.data_ptr(), zs.data_ptr(), st), "se_eval")
-    out = torch.empty_like(v, memory_format=torch.channels_last)
-    _lib.check(lib.cotb200_mix2(dt, B, H * W, C, y.data_ptr(), k.data_ptr(), a.data_ptr(), out.data_ptr(), st), "mix2")
-    return out
-
-
 def cot_tail(u, k, bn: torch.nn.BatchNorm2d, se: torch.nn.Module):
     if (not torch.is_grad_enabled() and not bn.training and not se[1].training and k is not None and se[1].running_mean is not None
             and bn.running_mean is not None and isinstance(se[2], torch.nn.ReLU)):
@@ -862,7 +795,7 @@ class TcConv1x1Fn(Function):
         lib, st, dt = _lib.load(), _lib.stream_ptr(dy), _lib.BF16
         dgamma = dbeta = dcb = dres = None
         if has_bn:
-            sums = _zeros_esc((2, N,), dy.device)      # escapes as dgamma/dbeta
+            sums = torch.zeros(2, N, dtype=torch.float32, device=dy.device)  # escapes as dgamma/dbeta
             if has_res and ctx.needs_input_grad[8]:
                 dres = torch.empty_like(dy, memory_format=torch.channels_last)
             dpre = torch.empty_like(dy, memory_format=torch.channels_last)
@@ -952,7 +885,7 @@ class TcConv3x3Fn(Function):
         M = B * H * W
         lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.BF16
         dy = dy.contiguous(memory_format=torch.channels_last)
-        sums = _zeros_esc((2, C,), x.device)          # escapes as dgamma/dbeta
+        sums = torch.zeros(2, C, dtype=torch.float32, device=x.device)  # escapes as dgamma/dbeta
         _lib.check(lib.cotb200_bn_bwd_sums(dt, B, H * W, C, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
                                            _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(),
                                            sums[1].data_ptr(), st),
@@ -1017,7 +950,7 @@ class StemConvBNFn(Function):
         M = B * Ho * Wo
         lib, st, dt = _lib.load(), _lib.stream_ptr(dy), _lib.BF16
         dy = dy.contiguous(memory_format=torch.channels_last)
-        sums = _zeros_esc((2, N,), dy.device)          # escapes as dgamma/dbeta
+        sums = torch.zeros(2, N, dtype=torch.float32, device=dy.device)  # escapes as dgamma/dbeta
         _lib.check(lib.cotb200_bn_bwd_sums(dt, B, Ho * Wo, N, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
                                            _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(),
                                            sums[1].data_ptr(), st), "bn_bwd_sums")
@@ -1033,7 +966,7 @@ class StemConvBNFn(Function):
         if ctx.needs_input_grad[1]:
             # weight gradient on the MN-major wgmma wgrad kernel over the space-to-depth image of the forward (one stage = one
             # output row, the four row taps as four B boxes); geometries it does not take: cuDNN
-            if scratch is not None and stem_wgrad_tc:
+            if scratch is not None:
                 dw = _tc.stem7x7s2_wgrad(dpre, scratch, x.shape, N)
             if dw is None:
                 dw = torch.nn.grad.conv2d_weight(x, weight.shape, dpre, stride=2, padding=3)
@@ -1041,16 +974,11 @@ class StemConvBNFn(Function):
         return dx, dw, sums[1].to(bndt), sums[0].to(bndt), None, None
 
 
-#: the trunk's 7x7 stem convolution on the wgmma implicit GEMM (0 = cuDNN, the round-1 path)
-stem_tc = _os.environ.get("COTB200_STEM_TC", "1") != "0"
-stem_wgrad_tc = _os.environ.get("COTB200_STEM_WGRAD_TC", "1") != "0"
-
-
 def stem_conv_bn(x, conv, bn, relu=True):
     """act(bn(conv(x))) for the 7x7/s2 stem.  wgmma path for channels_last bf16 3-channel images of even size (and an image
     row of at most 256 output pixels per tile segment); anything else: cuDNN + the fused BatchNorm kernels."""
     w = conv.weight
-    if (stem_tc and x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.shape[1] == 3 and tuple(w.shape[1:]) == (3, 7, 7)
+    if (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.shape[1] == 3 and tuple(w.shape[1:]) == (3, 7, 7)
             and conv.stride == (2, 2) and conv.padding == (3, 3) and conv.dilation == (1, 1) and conv.bias is None
             and x.shape[2] % 2 == 0 and x.shape[3] % 2 == 0 and w.shape[0] % 8 == 0 and w.shape[0] <= 256
             and x.is_contiguous(memory_format=torch.channels_last)):

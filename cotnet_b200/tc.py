@@ -39,22 +39,6 @@ def gemm_bf16(a1, b1, a2=None, b2=None, scale=None, shift=None, relu=False, stat
     return out
 
 
-def gemm_bf16_samplestats(a1, b1, rows_per_sample, shift=None, out=None):
-    """D = a1 @ b1.T (+ shift), plus PER-SAMPLE column sums / sums of squares of the raw accumulator: returns (D, csum, csq) with
-    csum, csq fp32 [M / rows_per_sample, N] -- the GroupNorm statistics of the logits from the GEMM epilogue."""
-    M, K1, lda1 = _rows(a1)
-    N = b1.shape[0]
-    assert b1.shape[1] == K1 and a1.dtype == torch.bfloat16 and b1.dtype == torch.bfloat16 and M % rows_per_sample == 0
-    if out is None:
-        out = torch.empty((M, N), dtype=torch.bfloat16, device=a1.device)
-    st = torch.zeros((2, M // rows_per_sample, N), dtype=torch.float32, device=a1.device)
-    rc = _lib.load().cotb200_gemm_bf16_samplestats(M, N, K1, a1.data_ptr(), lda1, b1.data_ptr(), b1.stride(0), out.data_ptr(), out.stride(0),
-                                                   None, _lib.ptr(shift), 0, rows_per_sample, st[0].data_ptr(), st[1].data_ptr(),
-                                                   _lib.stream_ptr(a1))
-    _lib.check(rc, "gemm_bf16_samplestats")
-    return out, st[0], st[1]
-
-
 def wgrad_bf16(dy, a1, a2=None, out=None):
     """dW [N, K1 (+K2)] fp32 = dy[M, N]^T @ [a1 | a2][M, K]: the weight gradient of a 1x1 convolution with output gradient dy and
     input(s) a1 (, a2).  Operands: 2-D row-major or channels_last activations (rows = pixels), bf16.  `out` (fp32, zeroed) may be

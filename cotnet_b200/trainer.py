@@ -31,14 +31,6 @@ import torch.nn.functional as F
 
 from . import _lib, fused
 
-#: COTB200_BOOKKEEPING=0: one `num_batches_tracked += 1` kernel per BatchNorm instead of one multi-tensor add per step.
-#: COTB200_ARENA_ESCAPE=1 (opt-in): BatchNorm / GroupNorm gradient sums from the pre-zeroed step arena instead of torch.zeros (~140 fill
-#: launches per step less).  Off by default: the gradients of 1-D parameters would then alias memory that the next step_begin()
-#: recycles.
-import os as _os
-_BOOKKEEPING = _os.environ.get("COTB200_BOOKKEEPING", "1") != "0"
-_ARENA_ESCAPE = _os.environ.get("COTB200_ARENA_ESCAPE", "0") != "0"
-
 ALIGN = 8          # elements: every parameter slot starts 16-byte aligned in the bf16 bucket (32 B in fp32)
 
 
@@ -489,12 +481,8 @@ class TrainStep:
         mix_dev = mix.on_stream(self.dev) if isinstance(mix, MixParams) else mix
         if self._cuda:
             fused.step_begin(self.dev)
-            # every gradient of this step is gathered into the flat bucket before the next step_begin(): the BatchNorm gradient sums
-            # may live in the step arena, and the ~100 `num_batches_tracked += 1` kernels become one multi-tensor add after the forward
-            if _ARENA_ESCAPE:
-                fused.arena_escape_ok(True)
-            if _BOOKKEEPING:
-                fused.defer_bn_counters(True)
+            # the ~100 `num_batches_tracked += 1` kernels become one multi-tensor add after the forward
+            fused.defer_bn_counters(True)
         for _, p, _ in self.plan["big"]:
             p.grad = None
         for _, p, _ in self.plan["small"]:
@@ -510,8 +498,6 @@ class TrainStep:
             fused.defer_bn_counters(False)
         loss.backward()
         self._finish_grads()
-        if self._cuda:
-            fused.arena_escape_ok(False)
         return loss
 
     def optimizer_step(self):

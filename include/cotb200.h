@@ -106,21 +106,6 @@ int cotb200_agg_zeropad_mix_bwd(const cotb200_agg_desc* d, int k2h, int k2w, int
                                 const void* dy, const void* x, const void* w1, const void* w2,
                                 void* dx, void* dw1, void* dw2, void* stream);
 
-/* Fused inference step of the CoT block (models/cotnet.py:85-98 in eval mode), one kernel on the TMA ring:
- *   w = l * a[n,j] + c[n,j]          GroupNorm of the logits as a per-(sample, column) affine (coef = [N, 9*wc, 2] fp32, tap-major
- *                                    column order, from cotb200_gn9_from_colsums) applied to the weight tile in shared memory
- *   u = LocalConv(v, w)              3x3 / stride 1 / zero pad 1
- *   y = SiLU(u * bn_scale + bn_shift)      eval-mode BatchNorm folded, y stored
- *   psum[n, c] += sum_px (y + k)     the pooled descriptor of the split attention (caller zeroes psum)
- * d: NHWC_TAP layout, l in tap-major column order with chunk width d->gc.  Returns COTB200_EUNSUPPORTED when the geometry does
- * not fit the kernel. */
-int cotb200_cot_agg_eval(const cotb200_agg_desc* d, const void* v, const void* l, const float* coef, const float* bn_scale,
-                         const float* bn_shift, const void* k, void* y, float* psum, void* stream);
-
-/* out = a[b,c,0]*y + a[b,c,1]*k on NHWC tensors [B, HW, C]: the radix-2 recombination (models/cotnet.py:101-104) when
- * y = SiLU(bn(.)) was already stored by cotb200_cot_agg_eval.  a [B,C,2] fp32. */
-int cotb200_mix2(int dtype, int B, int HW, int C, const void* y, const void* k, const float* a, void* out, void* stream);
-
 /* ---- the remaining LocalConv variants of cupy_layers (SURVEY.md section 8f rank 4); NCHW (reference contract), any dtype ----
  * Reflect padding instead of zero padding (cupy_layers/aggregation_refpad.py:21-127; launches :153-160,:183-207).
  * Padding must be smaller than the input (one reflection), like nn.ReflectionPad2d.  dX is gathered directly on the
@@ -307,24 +292,6 @@ int cotb200_gemm_bf16(int M, int N, int K1, const void* A1, long long lda1, cons
                       int K2, const void* A2, long long lda2, const void* B2, long long ldb2,
                       void* D, long long ldd, const float* scale, const float* shift, int relu,
                       float* col_sum, float* col_sqsum, void* stream);
-
-/* cotb200_gemm_bf16_samplestats: the single-product GEMM above whose statistics epilogue accumulates PER SAMPLE:
- *   samp_sum / samp_sqsum [M / rows_per_sample, N] += column sums / sums of squares of the STORED output (scale / shift
- *   applied, bf16-rounded) over the rows_per_sample consecutive rows (= H*W pixels) of each sample.  With
- *   cotb200_gn9_from_colsums (bias = NULL: it is already in the stored logits) this gives the GroupNorm statistics of the
- *   attention logits (models/cotnet.py:55-56) without a pass over them.  rows_per_sample >= 32, M % it == 0. */
-int cotb200_gemm_bf16_samplestats(int M, int N, int K1, const void* A1, long long lda1, const void* B1, long long ldb1,
-                                  void* D, long long ldd, const float* scale, const float* shift, int relu,
-                                  int rows_per_sample, float* samp_sum, float* samp_sqsum, void* stream);
-/* mean[b,g], rstd[b,g] of GroupNorm(wc groups of 9 taps) from per-sample column sums csum / csq [B, 9*wc] of the logits.
- * bias [9*wc]: a bias that is NOT yet contained in the summed values is accounted for analytically (NULL when the sums were
- * taken over the final logits); column order given by gc like cotb200_gn9_apply. */
-int cotb200_gn9_from_colsums(int B, int HW, int wc, int gc, const float* csum, const float* csq, const float* bias,
-                             float eps, float* mean, float* rstd, void* stream);
-/* Same statistics, returned as the per-(sample, column) affine of the normalisation: coef[b, j] = (rstd*gamma_j,
- * beta_j - mean*rstd*gamma_j) with gamma / beta [9*wc] in the SAME column order as csum (what cotb200_cot_agg_eval takes). */
-int cotb200_gn9_coef_from_colsums(int B, int HW, int wc, int gc, const float* csum, const float* csq, const float* bias,
-                                  const float* gamma, const float* beta, float eps, float* coef, void* stream);
 
 /* cotb200_conv3x3_bf16: 3x3 / stride 1 / zero-pad 1 grouped convolution on an NHWC bf16 tensor X[B,H,W,C] (pixel pitch
  *   ldx) as an im2col-free implicit GEMM; replaces key_embed.0 = nn.Conv2d(dim, dim, 3, padding=1, groups=4)

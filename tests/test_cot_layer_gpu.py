@@ -233,24 +233,3 @@ def test_tc_training_backend_vs_oracle(dim, H, backend):
     # backend must be as close to the fp64 oracle as the cuDNN backend is.
     assert rel["tc"][0] <= 3e-2, "forward relative L2 %.3e" % rel["tc"][0]
     assert rel["tc"][1] <= max(8e-2, 2.0 * rel["cudnn"][1] + 2e-2), "dX relative L2 tc %.3e vs cudnn %.3e" % (rel["tc"][1], rel["cudnn"][1])
-
-
-
-@pytest.mark.parametrize("dim,H", [(64, 56), (256, 14)])
-@pytest.mark.parametrize("variant", ["fused_agg", "samplestats"])
-def test_eval_optin_variants_match_default(dim, H, variant):
-    """The opt-in inference variants (COTB200_EVAL_FUSED_AGG / COTB200_EVAL_SAMPLESTATS: GroupNorm statistics from the logits GEMM
-    epilogue, GroupNorm-apply + LocalConv + bn + SiLU + pool in one kernel) against the default inference path (separate kernels) on the
-    same module: same arithmetic up to bf16 rounding of the intermediates."""
-    gen = torch.Generator().manual_seed(dim)
-    sd64 = cot_ref.init_state_dict("cot", dim, gen, dtype=torch.float64, perturb=True)
-    m = _mods().CotLayer(dim, 3)
-    m.load_state_dict(sd64, strict=True)
-    m = m.to(torch.bfloat16).cuda().to(memory_format=torch.channels_last).eval()
-    x = torch.relu(torch.randn(4, dim, H, H, generator=gen)).to(torch.bfloat16).cuda().contiguous(memory_format=torch.channels_last)
-    with torch.no_grad():
-        base = m(x).float()
-        setattr(m, "eval_" + variant, True)          # instance attribute shadows the class default
-        got = m(x).float()
-    rel = ((got - base).norm() / base.norm()).item()
-    assert rel <= 1e-2, rel

@@ -851,48 +851,6 @@ def test_graph_with_forked_reductions():
         assert _equal(og, eager), "forked graph replay %d differs bitwise from eager" % r
 
 
-# ================================================================================================ positive control (reported only)
-def test_atomic_samplestats_positive_control():
-    """cotb200_gemm_bf16_samplestats still adds its per-sample statistics with float atomics (an opt-in inference path).  The same
-    repeat harness is run on it to show whether repeats can expose a reordering at all; the outcome is printed, not asserted."""
-    lib = _lib.load()
-    g = _gen(17)
-    B, HW, K, N = 8, 3136, 64, 144
-    M = B * HW
-    mag = 10.0 ** (torch.rand(M, 1, generator=g, device="cuda") * 6 - 3)      # rows over six decades: reordering shows in the sums
-    a = (torch.randn(M, K, generator=g, device="cuda") * mag).bfloat16()
-    w = (torch.randn(N, K, generator=g, device="cuda") / 8).bfloat16()
-
-    def call(o, st):
-        _lib.check(lib.cotb200_gemm_bf16_samplestats(M, N, K, a.data_ptr(), K, w.data_ptr(), K, o[0].data_ptr(), N, None, None, 0, HW,
-                                                     o[1].data_ptr(), o[2].data_ptr(), st), "gemm_bf16_samplestats")
-
-    def run(o, st=None):
-        o[1].zero_()
-        o[2].zero_()
-        call(o, torch.cuda.current_stream().cuda_stream if st is None else st)
-
-    def new():
-        return [torch.empty(M, N, dtype=torch.bfloat16, device="cuda"), torch.empty(B, N, device="cuda"), torch.empty(B, N, device="cuda")]
-
-    first = new()
-    run(first)
-    differ = 0
-    for _ in range(4):
-        o = new()
-        run(o)
-        differ += not _equal(o[1:], first[1:])
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    o = new()
-    _load_on(side)
-    run(o)
-    torch.cuda.current_stream().wait_stream(side)
-    differ += not _equal(o[1:], first[1:])
-    torch.cuda.synchronize()
-    print("positive control (atomic per-sample statistics): %d of 5 repeats differ bitwise from the first run" % differ)
-
-
 # ================================================================================================ model level
 @pytest.fixture
 def deterministic_cudnn():

@@ -28,12 +28,11 @@ def test_tc_gemm_constants():
     # tc_launch: two CTAs per SM under 104 KB, else one under 200 KB; the statistics smem; the grid of resident CTAs
     for snippet in ("p.stages = (104 * 1024 - out_bytes) / stage_bytes;", "if (p.stages < 2 || p.bn > 128) {",
                     "p.stages = (200 * 1024 - out_bytes) / stage_bytes;", "2 * 4 * 256 * 4 + 2 * p.N * 4",
-                    "int grid = per_sm * num_sms();", "p.bn = pick_bn(N, K1 + K2);", "p.bn = pick_bn(N); p.mode = 0;",
-                    "p.bn = pick_bn_wide(N); p.mode = 2;"):
+                    "int grid = per_sm * num_sms();", "p.bn = pick_bn(N, K1 + K2);", "p.bn = pick_bn_wide(N); p.mode = 2;"):
         assert snippet in s, snippet
     # conv3x3_halo_launch: the 256-pixel cap, its 4 stages, the 220 KB budget, the grid bound to whole N-tile sets
     assert "static constexpr int HC_WBYTES = 9 * 64 * 128;" in s
-    for snippet in ("r * Wpad <= maxpx && r * W <= 256", "maxpx = e ? atoi(e) : 256;", "if (p.stages > 4) p.stages = 4;",
+    for snippet in ("r * Wpad <= maxpx && r * W <= 256", "const int maxpx = 256;", "if (p.stages > 4) p.stages = 4;",
                     "p.stages = (220 * 1024 - HC_WBYTES - out_bytes) / p.a_stage_bytes;",
                     "int grid = (num_sms() / p.n_tiles) * p.n_tiles;", "while (H % hb) --hb;"):
         assert snippet in s, snippet

@@ -190,13 +190,13 @@ def at_setup(mode, es, N, C, H, W, wc):
     return TH, bands, stages
 
 
-def at_plan(mode, es, N, C, H, W, wc, sms, name=None):
+def at_plan(mode, es, N, C, H, W, wc, sms):
     """the plan of the TMA kernel, or None when at_setup declines the geometry"""
     if at_setup(mode, es, N, C, H, W, wc) is None:
         return None
     TH, bands, stages = at_setup(mode, es, N, C, H, W, wc)
     total = N * bands
-    return Plan(name or AT_NAMES[mode], min(sms, total), total, stages, TH=TH, bands=bands)
+    return Plan(AT_NAMES[mode], min(sms, total), total, stages, TH=TH, bands=bands)
 
 
 # cotnet_b200/csrc/agg_nchw_tma.cu: nchw_tma_launch (tile = (sample, weight channel, band))
@@ -291,25 +291,6 @@ def gemm_sizes(case, sms):
     return _search(make)
 
 
-# per-sample statistics: rows_per_sample = H*W with sample boundaries inside row tiles; values |D| <= K = 64, so every per-sample
-# sum (<= 784 * 64) and sum of squares (<= 784 * 4096) is an integer below 2^24: exact in any order
-SAMPLESTATS_CASES = [(784, 144, 64), (196, 288, 64)]      # (rows_per_sample, N = 9 * wc, K)
-
-
-def samplestats_sizes(case, sms):
-    rps, N, K = case
-    bn = pick_bn(N)
-
-    def make(B):
-        M = B * rps
-        mt = _cdiv(M, TC_BM)
-        p = tc_launch("tc_gemm_1x1", N, bn, mt, _cdiv(K, TC_BK), False, sms)
-        ok = rps % TC_BM != 0 and M % TC_BM != 0 and p.max_tiles * TC_BM >= 2 * rps
-        return [p], ok, dict(B=B, M=M, mem=M * (K + N) * 2 + 4 * M * N * 8)
-
-    return _search(make)
-
-
 # 3x3 convolutions: (C, groups, bn, H, W, transposed weight (data gradient), statistics, operands).  cg = C / groups = 16 with
 # {-1, 0, 1} operands: |D| <= 9 * 16 = 144.  bn = 64 is the haloed-tile kernel, bn in {128, 192, 256} conv mode of the GEMM kernel
 # (the weight is packed for that N tile: zero outside each output channel's group).
@@ -385,20 +366,6 @@ def agg_sizes(case, sms):
     return _search(make)
 
 
-# fused inference kernel: bf16, C = 64, wc = 8 (float operands: GroupNorm affine, SiLU)
-EVAL_CASES = [("bf16", 64, 8, 56, 56, 8), ("bf16", 128, 16, 28, 28, 8)]
-
-
-def eval_sizes(case, sms):
-    dt, C, wc, H, W, _ = case
-    es = DTYPES[dt][1]
-
-    def make(N):
-        return [at_plan(0, es, N, C, H, W, wc, sms, name="agg3_eval_tma")], True, dict(N=N, mem=N * H * W * (3 * C + 9 * wc) * (es + 8 * 3))
-
-    return _search(make)
-
-
 # NCHW TMA LocalConv: (dtype size, C, wc, H, W); {-2..2} operands, 8 sharers per weight channel: exact
 NCHW_CASES = [("fp32", 64, 8, 56, 56), ("bf16", 64, 8, 56, 56)]
 
@@ -427,9 +394,8 @@ def gn_sizes(case, sms):
     return _search(make)
 
 
-ALL_CASES = ([(gemm_sizes, c) for c in GEMM_CASES] + [(samplestats_sizes, c) for c in SAMPLESTATS_CASES]
-             + [(conv_sizes, c) for c in CONV_CASES] + [(stem_sizes, c) for c in STEM_CASES] + [(agg_sizes, c) for c in AGG_CASES]
-             + [(eval_sizes, c) for c in EVAL_CASES] + [(nchw_sizes, c) for c in NCHW_CASES] + [(gn_sizes, c) for c in GN_CASES])
+ALL_CASES = ([(gemm_sizes, c) for c in GEMM_CASES] + [(conv_sizes, c) for c in CONV_CASES] + [(stem_sizes, c) for c in STEM_CASES]
+             + [(agg_sizes, c) for c in AGG_CASES] + [(nchw_sizes, c) for c in NCHW_CASES] + [(gn_sizes, c) for c in GN_CASES])
 
 
 # ================================================================================================ helpers
@@ -548,43 +514,6 @@ def test_gemm_bf16(case):
             d_abs += D[i0:i1].double().abs().sum(0)
         _sums_close(cs, s_ref, d_abs, what + " col_sum")
         _sums_close(cq, q_ref, q_ref, what + " col_sqsum")
-
-
-@pytest.mark.parametrize("case", SAMPLESTATS_CASES, ids=lambda c: "rps%d-N%d-K%d" % c)
-def test_gemm_samplestats_and_gn9_from_colsums(case):
-    rps, N, K = case
-    (plan,), sz = samplestats_sizes(case, _sms())
-    B, M = sz["B"], sz["M"]
-    _assert_regime([plan], samples_inside_tiles=rps % TC_BM != 0)
-    print("samplestats %s B=%d: %s" % (case, B, plan))
-    g = _gen(rps + N + K)
-    a, w = _ints((M, K), -1, 1, g, torch.bfloat16), _ints((N, K), -1, 1, g, torch.bfloat16)
-    D = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device="cuda")
-    cs, cq = torch.zeros(B, N, device="cuda"), torch.zeros(B, N, device="cuda")
-    lib = _lib.load()
-    with kernels_ran("tc_gemm_1x1"):
-        _lib.check(lib.cotb200_gemm_bf16_samplestats(M, N, K, a.data_ptr(), K, w.data_ptr(), K, D.data_ptr(), N, None, None, 0, rps,
-                                                     cs.data_ptr(), cq.data_ptr(), _st()), "gemm_bf16_samplestats")
-    torch.cuda.synchronize()
-    what = "samplestats %s (%s)" % (case, plan)
-    s_ref = torch.empty(B, N, dtype=torch.float64, device="cuda")
-    q_ref = torch.empty_like(s_ref)
-    step = max(1, (1 << 16) // rps)
-    for b0, b1 in _chunks(B, step):
-        ref = a[b0 * rps:b1 * rps].double() @ w.double().t()
-        _equal_exact(D[b0 * rps:b1 * rps], ref, what + " samples %d.." % b0)
-        r = ref.view(b1 - b0, rps, N)
-        s_ref[b0:b1], q_ref[b0:b1] = r.sum(1), (r * r).sum(1)
-    _equal_exact(cs, s_ref, what + " per-sample sums")
-    _equal_exact(cq, q_ref, what + " per-sample sums of squares")
-    wc = N // 9
-    mr = torch.empty(2, B * wc, device="cuda")
-    _lib.check(lib.cotb200_gn9_from_colsums(B, rps, wc, 0, cs.data_ptr(), cq.data_ptr(), None, 1e-5, mr[0].data_ptr(), mr[1].data_ptr(),
-                                            _st()), "gn9_from_colsums")
-    mean = s_ref.view(B, wc, 9).sum(-1) / (9 * rps)
-    var = q_ref.view(B, wc, 9).sum(-1) / (9 * rps) - mean * mean
-    assert torch.allclose(mr[0].view(B, wc).double(), mean, atol=3e-3, rtol=3e-3), what + " GroupNorm mean"
-    assert torch.allclose(mr[1].view(B, wc).double(), torch.rsqrt(var + 1e-5), atol=3e-3, rtol=5e-3), what + " GroupNorm rstd"
 
 
 # ================================================================================================ 3x3 convolutions
@@ -818,59 +747,6 @@ def test_agg_tma_fwd_dx_dw(case):
         else:
             for name, got, ref in refs:
                 _equal_exact(got[n0:n1], ref, "%s %s samples %d.." % (what, name, n0))
-
-
-# ================================================================================================ fused inference kernel
-@pytest.mark.parametrize("case", EVAL_CASES, ids=lambda c: "%s-C%d-wc%d-%dx%d-gc%d" % c)
-def test_cot_agg_eval(case):
-    """GroupNorm affine of the logits -> LocalConv -> eval BatchNorm -> SiLU, and psum = pooled (y + k), against torch"""
-    dt, C, wc, H, W, gc = case
-    (plan,), sz = eval_sizes(case, _sms())
-    N = sz["N"]
-    _assert_regime([plan], samples_per_cta=plan.max_tiles >= 2)
-    print("cot_agg_eval %s N=%d: %s" % (case, N, plan))
-    dtype = DTYPES[dt][0]
-    J = 9 * wc
-    g = _gen(C + wc + H)
-    v = torch.randn(N, H, W, C, generator=g, device="cuda").to(dtype)
-    l = (0.5 + torch.randn(N, H, W, J, generator=g, device="cuda")).to(dtype)             # tap-major storage order
-    k = torch.randn(N, H, W, C, generator=g, device="cuda").to(dtype)
-    gamma = 0.5 + torch.rand(J, generator=g, device="cuda")                                 # reference column order g*9 + t
-    beta = 0.3 * torch.randn(J, generator=g, device="cuda")
-    bn_scale = 0.5 + torch.rand(C, generator=g, device="cuda")
-    bn_shift = 0.2 * torch.randn(C, generator=g, device="cuda")
-    # GroupNorm(wc groups of 9 taps) of l as the per-(sample, storage column) affine a * l + c
-    e = torch.arange(J, device="cuda")
-    grp = (e // (9 * gc)) * gc + e % gc                                                      # storage column -> group, tap
-    tap = (e % (9 * gc)) // gc
-    lg = l.double().view(N, H * W, J)
-    mean = torch.zeros(N, wc, dtype=torch.float64, device="cuda").index_add_(1, grp, lg.sum(1)) / (9 * H * W)
-    msq = torch.zeros(N, wc, dtype=torch.float64, device="cuda").index_add_(1, grp, (lg * lg).sum(1)) / (9 * H * W)
-    rstd = torch.rsqrt(msq - mean * mean + 1e-5)
-    a = rstd[:, grp] * gamma.double()[grp * 9 + tap]
-    c = beta.double()[grp * 9 + tap] - mean[:, grp] * a
-    coef = torch.stack([a, c], -1).float().contiguous()                                      # [N, J, 2]
-    y = torch.full((N, H, W, C), float("nan"), dtype=dtype, device="cuda")
-    psum = torch.zeros(N, C, device="cuda")
-    d = _desc(N, C, H, W, wc, dtype, _lib.NHWC_TAP, gc)
-    lib = _lib.load()
-    with kernels_ran("agg3_eval_tma"):
-        _lib.check(lib.cotb200_cot_agg_eval(d, v.data_ptr(), l.data_ptr(), coef.data_ptr(), bn_scale.data_ptr(), bn_shift.data_ptr(),
-                                            k.data_ptr(), y.data_ptr(), psum.data_ptr(), _st()), "cot_agg_eval")
-    torch.cuda.synchronize()
-    what = "cot_agg_eval %s (%s)" % (case, plan)
-    pos = _tap_pos(C, wc, 1, gc)
-    cf = coef.double()
-    for n0, n1 in _chunks(N, 8):
-        # the kernel stores the normalised weight tile in the storage type before the convolution
-        wn = (l[n0:n1].double() * cf[n0:n1, None, None, :, 0] + cf[n0:n1, None, None, :, 1]).to(dtype).double()
-        z = agg_fwd_ref(v[n0:n1].double(), wn, pos) * bn_scale.double() + bn_shift.double()
-        ref = z * torch.sigmoid(z)
-        err = (y[n0:n1].double() - ref).abs()
-        assert bool((err <= 2e-2 + 2e-2 * ref.abs()).all()), "%s y samples %d..: max err %.3e" % (what, n0, float(err.max()))
-    # the pool sums what was stored: (y + k) over the pixels of each sample
-    t = (y.double() + k.double()).view(N, H * W, C)
-    _sums_close(psum, t.sum(1), (y.double().abs() + k.double().abs()).view(N, H * W, C).sum(1), what + " psum")
 
 
 # ================================================================================================ NCHW TMA LocalConv

@@ -111,38 +111,6 @@ def test_wgrad_channels_last_views_and_accumulate():
     assert ((out - 1.0 - want).norm() / want.norm()).item() <= 2e-3
 
 
-@pytest.mark.parametrize("B,HW,K,wc", [(5, 49, 256, 64), (3, 196, 128, 32), (2, 3136, 32, 8), (7, 64, 64, 16)])
-def test_gemm_samplestats_and_gn_from_colsums(B, HW, K, wc):
-    """Per-sample column statistics from the GEMM epilogue -> GroupNorm(9 taps) mean / rstd, vs torch on the fp32 product."""
-    from cotnet_b200 import _lib
-    tc = _tc()
-    g = torch.Generator(device="cuda").manual_seed(B * HW)
-    J = 9 * wc
-    a = torch.randn(B * HW, K, generator=g, device="cuda").bfloat16()
-    w = (torch.randn(J, K, generator=g, device="cuda") / K ** 0.5).bfloat16()
-    bias = torch.randn(J, generator=g, device="cuda")
-    d, cs, cq = tc.gemm_bf16_samplestats(a, w, HW, shift=bias)
-    acc = a.float() @ w.float().t()
-    _close(d, acc + bias)
-    df = d.float()                                   # the sums are those of the STORED logits (bias included, bf16-rounded)
-    assert torch.allclose(cs, df.view(B, HW, J).sum(1), atol=1e-2, rtol=1e-4)
-    assert torch.allclose(cq, (df * df).view(B, HW, J).sum(1), atol=1e-2, rtol=1e-4)
-    mr = torch.empty(2, B * wc, device="cuda")
-    lib = _lib.load()
-    _lib.check(lib.cotb200_gn9_from_colsums(B, HW, wc, 0, cs.data_ptr(), cq.data_ptr(), None, 1e-5, mr[0].data_ptr(),
-                                            mr[1].data_ptr(), torch.cuda.current_stream().cuda_stream), "gn9_from_colsums")
-    l = (acc + bias).view(B, HW, wc, 9).permute(0, 2, 1, 3).reshape(B, wc, HW * 9)
-    assert torch.allclose(mr[0].view(B, wc), l.mean(-1), atol=3e-3, rtol=3e-3)
-    assert torch.allclose(mr[1].view(B, wc), torch.rsqrt(l.var(-1, unbiased=False) + 1e-5), atol=3e-3, rtol=5e-3)
-    # analytic bias path of the finalize kernel: sums of (values - bias) + bias == the same statistics
-    cs2 = cs - HW * bias
-    cq2 = cq - 2 * bias * cs + HW * bias * bias
-    mr2 = torch.empty(2, B * wc, device="cuda")
-    _lib.check(lib.cotb200_gn9_from_colsums(B, HW, wc, 0, cs2.data_ptr(), cq2.data_ptr(), bias.data_ptr(), 1e-5, mr2[0].data_ptr(),
-                                            mr2[1].data_ptr(), torch.cuda.current_stream().cuda_stream), "gn9_from_colsums")
-    assert torch.allclose(mr2, mr, atol=1e-3, rtol=1e-3)
-
-
 def _cl(t):
     return t.contiguous(memory_format=torch.channels_last)
 

@@ -1,10 +1,11 @@
 #!/usr/bin/env python
 """3x3 grouped key convolution (key_embed.0, models/cotnet.py:44) per CoTNet-50 stage shape, bs256, bf16 NHWC: the haloed-tile
-wgmma kernel (variants through COTB200_CONV_HALO / COTB200_HALO_MAXPX, one subprocess each) against the per-tap conv mode and
-cuDNN's grouped convolution.  CUDA events, inputs rotated through > 126 MB."""
+wgmma kernel (geometries it rejects run on the per-tap conv mode) against cuDNN's grouped convolution.  CUDA events, inputs
+rotated through > 126 MB.
+
+    python tools/bench_halo.py [out.json]"""
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -12,7 +13,7 @@ sys.path.insert(0, ROOT)
 STAGES = [(64, 56), (128, 28), (256, 14), (512, 7)]
 
 
-def child():
+def main():
     import torch
     import torch.nn.functional as F
     from cotnet_b200 import tc
@@ -44,23 +45,9 @@ def child():
                           "tc_stats_us": t(lambda x: tc.conv3x3_bf16(x, wp, bn, stats=(cs, cq), out=o)),
                           "cudnn_us": t(lambda x: F.conv2d(x, wcl, None, 1, 1, 1, 4)),
                           "roof_us": round(2 * B * H * H * C * 2 / 6485.2e3, 1)}
-    print("RESULT " + json.dumps(out), flush=True)
-
-
-def main():
-    if os.environ.get("BENCH_HALO_CHILD"):
-        return child()
-    res = {}
-    for name, env in (("halo_256", {"COTB200_CONV_HALO": "1", "COTB200_HALO_MAXPX": "256"}),
-                      ("halo_128", {"COTB200_CONV_HALO": "1", "COTB200_HALO_MAXPX": "128"}),
-                      ("per_tap", {"COTB200_CONV_HALO": "0"})):
-        e = dict(os.environ, BENCH_HALO_CHILD="1", **env)
-        r = subprocess.run([sys.executable, os.path.abspath(__file__)], env=e, capture_output=True, text=True, timeout=600)
-        line = [l for l in r.stdout.splitlines() if l.startswith("RESULT ")]
-        res[name] = json.loads(line[-1][7:]) if line else {"error": (r.stderr or r.stdout)[-400:]}
-        print(name, json.dumps(res[name]), flush=True)
+    print(json.dumps(out), flush=True)
     if len(sys.argv) > 1:
-        json.dump(res, open(sys.argv[1], "w"), indent=1)
+        json.dump(out, open(sys.argv[1], "w"), indent=1)
 
 
 if __name__ == "__main__":
