@@ -156,6 +156,8 @@ SYMBOLS = {
                                                                _VP, _VP]),
     "cotb200_aug_resize_crop": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP, ctypes.c_longlong, _VP, _VP, _VP, ctypes.c_longlong, _VP, _VP]),
     "cotb200_aug_randaug": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP] * 4),
+    "cotb200_aug_color_jitter": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP] * 4),
+    "cotb200_aug_erase": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP] * 4),
 }
 
 

@@ -13,6 +13,9 @@
 // RandAugment runs one CTA per image with the S x S x 3 image in shared memory (150,528 B at S = 224): histograms, the L mean
 // and the LUTs are built there and the image is written to HBM once.  Ops that read neighbours (Sharpness, the affine ops)
 // read the previous state from the output buffer in global memory and write shared memory.
+//
+// ColorJitter (+ RandomVerticalFlip), the reference's colour transform when RandAugment is off, runs the same way: one CTA per
+// image in shared memory, between resize-crop and RandAugment, sharing RandAugment's enhance blends.
 #include "common.cuh"
 
 namespace cotb200 {
@@ -244,6 +247,33 @@ __device__ __forceinline__ int smooth_px(const unsigned char* pl, int S, int x, 
   return ss <= 0.f ? 0 : ss >= 255.f ? 255 : (int)__fadd_rn(ss, 0.5f);
 }
 
+// ImageEnhance.Color / Contrast / Brightness (op OP_COLOR, OP_CONTRAST, OP_BRIGHTNESS) of the planar image img [3][n_pix] in
+// shared memory, in place: Image.blend(degenerate, img, factor) with the degenerate L (Color), int(mean(L) + 0.5) (Contrast) or
+// 0 (Brightness).  Every thread of the CTA calls it; lsum is a shared scratch word.  Ends with the CTA synchronised.
+__device__ void enhance_blend(unsigned char* img, int n_pix, int op, float factor, unsigned long long* lsum) {
+  int mean = 0;
+  if (op == OP_CONTRAST) {                            // int(mean(L) + 0.5), ImageEnhance.Contrast
+    if (threadIdx.x == 0) *lsum = 0;
+    __syncthreads();
+    unsigned long long part = 0;
+    for (int i = threadIdx.x; i < n_pix; i += blockDim.x) part += l_of(img[i], img[n_pix + i], img[2 * n_pix + i]);
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(lsum, part);
+    __syncthreads();
+    mean = (int)__dadd_rn(__ddiv_rn((double)*lsum, (double)n_pix), 0.5);
+  } else {
+    __syncthreads();
+  }
+  for (int i = threadIdx.x; i < n_pix; i += blockDim.x) {
+    const int r = img[i], gg = img[n_pix + i], b = img[2 * n_pix + i];
+    const int d = op == OP_COLOR ? l_of(r, gg, b) : op == OP_CONTRAST ? mean : 0;
+    img[i] = blend_px(d, r, factor);
+    img[n_pix + i] = blend_px(d, gg, factor);
+    img[2 * n_pix + i] = blend_px(d, b, factor);
+  }
+  __syncthreads();
+}
+
 __global__ void __launch_bounds__(RA_THREADS)
 aug_randaug_kernel(const cotb200_aug_sample* __restrict__ params, int S, unsigned char* out) {
   extern __shared__ unsigned char sm_img[];          // [3][S][S]
@@ -297,27 +327,7 @@ aug_randaug_kernel(const cotb200_aug_sample* __restrict__ params, int S, unsigne
       continue;
     }
     if (op.op >= OP_COLOR && op.op <= OP_BRIGHTNESS) {
-      int mean = 0;
-      if (op.op == OP_CONTRAST) {                     // int(mean(L) + 0.5), ImageEnhance.Contrast
-        if (threadIdx.x == 0) lsum = 0;
-        __syncthreads();
-        unsigned long long part = 0;
-        for (int i = threadIdx.x; i < n_pix; i += blockDim.x) part += l_of(sm_img[i], sm_img[n_pix + i], sm_img[2 * n_pix + i]);
-        for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-        if ((threadIdx.x & 31) == 0) atomicAdd(&lsum, part);
-        __syncthreads();
-        mean = (int)__dadd_rn(__ddiv_rn((double)lsum, (double)n_pix), 0.5);
-      } else {
-        __syncthreads();
-      }
-      for (int i = threadIdx.x; i < n_pix; i += blockDim.x) {
-        const int r = sm_img[i], gg = sm_img[n_pix + i], b = sm_img[2 * n_pix + i];
-        const int d = op.op == OP_COLOR ? l_of(r, gg, b) : op.op == OP_CONTRAST ? mean : 0;
-        sm_img[i] = blend_px(d, r, op.factor);
-        sm_img[n_pix + i] = blend_px(d, gg, op.factor);
-        sm_img[2 * n_pix + i] = blend_px(d, b, op.factor);
-      }
-      __syncthreads();
+      enhance_blend(sm_img, n_pix, op.op, op.factor, &lsum);
       g_current = false;
       continue;
     }
@@ -379,6 +389,87 @@ aug_randaug_kernel(const cotb200_aug_sample* __restrict__ params, int S, unsigne
   }
   if (!g_current)
     for (int i = threadIdx.x; i < n_all; i += blockDim.x) g[i] = sm_img[i];
+}
+
+// ---------------------------------------------------------------- ColorJitter + vertical flip
+// torchvision ColorJitter on PIL images: brightness / contrast / saturation are ImageEnhance.Brightness / Contrast / Color
+// (enhance_blend), hue is adjust_hue: Pillow's RGB -> HSV, h += uint8(int32(hue_factor * 255)) (mod 256), Pillow's HSV -> RGB.
+// The two conversions follow Pillow's C arithmetic: float where it declares float, double where its expressions promote, C
+// round() (half away from zero) and truncating casts; every operation is an explicit _rn intrinsic so that nothing contracts.
+enum { JIT_BRIGHTNESS = 0, JIT_CONTRAST, JIT_SATURATION, JIT_HUE, JIT_COUNT };
+
+__device__ __forceinline__ int clip255(int v) { return v < 0 ? 0 : v > 255 ? 255 : v; }
+
+__device__ __forceinline__ void rgb_to_hsv_px(int r, int g, int b, int& h, int& s, int& v) {
+  const int maxc = max(r, max(g, b)), minc = min(r, min(g, b));
+  v = maxc;
+  if (maxc == minc) { h = 0; s = 0; return; }
+  const float cr = (float)(maxc - minc);
+  const float sf = __fdiv_rn(cr, (float)maxc);
+  const float rc = __fdiv_rn((float)(maxc - r), cr), gc = __fdiv_rn((float)(maxc - g), cr), bc = __fdiv_rn((float)(maxc - b), cr);
+  float hf;
+  if (r == maxc) hf = __fsub_rn(bc, gc);
+  else if (g == maxc) hf = (float)__dsub_rn(__dadd_rn(2.0, (double)rc), (double)bc);
+  else hf = (float)__dsub_rn(__dadd_rn(4.0, (double)gc), (double)rc);
+  hf = (float)fmod(__dadd_rn(__ddiv_rn((double)hf, 6.0), 1.0), 1.0);
+  h = clip255((int)__dmul_rn((double)hf, 255.0));
+  s = clip255((int)__dmul_rn((double)sf, 255.0));
+}
+
+__device__ __forceinline__ void hsv_to_rgb_px(int h, int s, int v, int& r, int& g, int& b) {
+  if (s == 0) { r = g = b = v; return; }
+  const double hh = __ddiv_rn(__dmul_rn((double)h, 6.0), 255.0);
+  const int i = (int)floor(hh);
+  const float f = (float)__dsub_rn(hh, (double)(float)i);
+  const float fs = (float)__ddiv_rn((double)s, 255.0);
+  const double vf = (double)v;
+  const int p = clip255((int)round(__dmul_rn(vf, __dsub_rn(1.0, (double)fs))));
+  const int q = clip255((int)round(__dmul_rn(vf, __dsub_rn(1.0, (double)__fmul_rn(fs, f)))));
+  const int t = clip255((int)round(__dmul_rn(vf, __dsub_rn(1.0, __dmul_rn((double)fs, __dsub_rn(1.0, (double)f))))));
+  switch (i % 6) {
+    case 0: r = v; g = t; b = p; break;
+    case 1: r = q; g = v; b = p; break;
+    case 2: r = p; g = v; b = t; break;
+    case 3: r = p; g = q; b = v; break;
+    case 4: r = t; g = p; b = v; break;
+    default: r = v; g = p; b = q; break;
+  }
+}
+
+__global__ void __launch_bounds__(RA_THREADS)
+aug_jitter_kernel(const cotb200_aug_jitter* __restrict__ params, int S, unsigned char* out) {
+  extern __shared__ unsigned char sm_img[];          // [3][S][S]
+  __shared__ unsigned long long lsum;
+  const cotb200_aug_jitter p = params[blockIdx.x];
+  bool any = p.vflip != 0;
+  for (int k = 0; k < JIT_COUNT; ++k) any = any || p.order[k] >= 0;
+  if (!any) return;                                  // the image stays as resize-crop wrote it
+  const int n_pix = S * S, n_all = 3 * n_pix;
+  unsigned char* g = out + (long long)blockIdx.x * n_all;
+  for (int i = threadIdx.x; i < n_all; i += blockDim.x) {
+    const int c = i / n_pix, y = (i % n_pix) / S, x = i % S;
+    sm_img[i] = g[p.vflip ? c * n_pix + (S - 1 - y) * S + x : i];   // RandomVerticalFlip: a row mirror of the S x S image
+  }
+  __syncthreads();
+  for (int k = 0; k < JIT_COUNT; ++k) {
+    const int op = p.order[k];
+    if (op < 0) continue;
+    if (op == JIT_HUE) {
+      const int shift = (int)(unsigned char)(int)__dmul_rn(p.hue, 255.0);   // np.int32(hue_factor * 255).astype(np.uint8)
+      for (int i = threadIdx.x; i < n_pix; i += blockDim.x) {
+        int h, s, v, r, gg, b;
+        rgb_to_hsv_px(sm_img[i], sm_img[n_pix + i], sm_img[2 * n_pix + i], h, s, v);
+        hsv_to_rgb_px((h + shift) & 255, s, v, r, gg, b);
+        sm_img[i] = (unsigned char)r;
+        sm_img[n_pix + i] = (unsigned char)gg;
+        sm_img[2 * n_pix + i] = (unsigned char)b;
+      }
+      __syncthreads();
+    } else {
+      enhance_blend(sm_img, n_pix, op == JIT_BRIGHTNESS ? OP_BRIGHTNESS : op == JIT_CONTRAST ? OP_CONTRAST : OP_COLOR, p.factor[op], &lsum);
+    }
+  }
+  for (int i = threadIdx.x; i < n_all; i += blockDim.x) g[i] = sm_img[i];
 }
 
 static int check_samples(const char* what, int N, int S, const cotb200_aug_sample* h) {
@@ -466,4 +557,34 @@ extern "C" int cotb200_aug_randaug(int N, int S, const cotb200_aug_sample* param
   COTB200_PROF_B("aug_randaug", 6.0 * N * S * S);
   aug_randaug_kernel<<<N, RA_THREADS, smem, st>>>(params_dev, S, out);
   return check_launch("aug_randaug");
+}
+
+extern "C" int cotb200_aug_color_jitter(int N, int S, const cotb200_aug_jitter* params_host, const cotb200_aug_jitter* params_dev,
+                                  unsigned char* out, void* stream) {
+  if (!params_host) { set_error("aug_color_jitter: params_host is NULL"); return COTB200_ENULL; }
+  if (N <= 0 || S <= 0) { set_error("aug_color_jitter: bad dims N=%d S=%d", N, S); return COTB200_EINVAL; }
+  if (!params_dev || !out) { set_error("aug_color_jitter: NULL pointer"); return COTB200_ENULL; }
+  if (S > RA_MAX_S) { set_error("aug_color_jitter: S=%d above %d (the image is held in shared memory)", S, RA_MAX_S); return COTB200_EUNSUPPORTED; }
+  for (int n = 0; n < N; ++n) {
+    const cotb200_aug_jitter& p = params_host[n];
+    if (p.vflip != 0 && p.vflip != 1) { set_error("aug_color_jitter: sample %d: vflip %d not 0 or 1", n, p.vflip); return COTB200_EINVAL; }
+    bool seen[JIT_COUNT] = {};
+    for (int k = 0; k < JIT_COUNT; ++k) {
+      const int op = p.order[k];
+      if (op == -1) continue;
+      if (op < -1 || op >= JIT_COUNT || seen[op]) {
+        set_error("aug_color_jitter: sample %d: order[%d] = %d is unknown or repeated", n, k, op); return COTB200_EINVAL;
+      }
+      seen[op] = true;
+      if (op == JIT_HUE ? !(p.hue >= -0.5 && p.hue <= 0.5) : !(isfinite(p.factor[op]) && p.factor[op] >= 0.f)) {
+        set_error("aug_color_jitter: sample %d: factor of op %d out of range", n, op); return COTB200_EINVAL;
+      }
+    }
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaFuncSetAttribute(aug_jitter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * RA_MAX_S * RA_MAX_S);
+  if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
+  COTB200_PROF_B("aug_jitter", 6.0 * N * S * S);
+  aug_jitter_kernel<<<N, RA_THREADS, 3 * S * S, st>>>(params_dev, S, out);
+  return check_launch("aug_jitter");
 }

@@ -549,6 +549,49 @@ int cotb200_aug_resize_crop(int N, int S, const unsigned char* src, long long sr
  * An unknown op id or a bad argument is rejected with COTB200_EINVAL; S above 256 with COTB200_EUNSUPPORTED. */
 int cotb200_aug_randaug(int N, int S, const cotb200_aug_sample* params_host, const cotb200_aug_sample* params_dev,
                         unsigned char* out, void* stream);
+/* ColorJitter + RandomVerticalFlip of one image (transforms_factory.py:75-76,100-109, torchvision ColorJitter on PIL images).
+ * vflip: 0/1, a row mirror of the S x S output, applied first.  order: the ops in application order (torchvision's randperm),
+ * -1 entries skipped, each op at most once: 0 brightness (ImageEnhance.Brightness), 1 contrast (ImageEnhance.Contrast),
+ * 2 saturation (ImageEnhance.Color), 3 hue (adjust_hue).  factor[op]: the Image.blend factor of ops 0..2 (>= 0, rounded to
+ * fp32 as Pillow does); hue: adjust_hue's hue_factor in [-0.5, 0.5], shifting H by uint8(int32(hue * 255)) mod 256 between
+ * Pillow's RGB -> HSV and HSV -> RGB conversions. */
+typedef struct cotb200_aug_jitter {
+  int vflip;
+  int order[4];
+  float factor[3];
+  double hue;
+} cotb200_aug_jitter;
+/* ColorJitter (+ vflip) of each sample applied in place to out [N, 3, S, S], after cotb200_aug_resize_crop and before
+ * cotb200_aug_randaug (one CTA per image, the image held in shared memory; a sample with nothing to do is not touched).
+ * params_host / params_dev: the same N structs on the host (validated) and on the device (read by the kernel).  Rejected with
+ * COTB200_EINVAL: a vflip other than 0/1, an unknown or repeated op, a factor below 0 or not finite, a hue outside
+ * [-0.5, 0.5]; S above 256 with COTB200_EUNSUPPORTED. */
+int cotb200_aug_color_jitter(int N, int S, const cotb200_aug_jitter* params_host, const cotb200_aug_jitter* params_dev,
+                       unsigned char* out, void* stream);
+/* Random erasing of the normalised batch (datasets/random_erasing.py, applied by PrefetchLoader after the normalisation,
+ * datasets/loader.py:90-91).  The host draws the boxes; one buffer holds a cotb200_erase header followed directly by its n_boxes
+ * cotb200_erase_box entries, grouped by sample n in increasing order, each sample's boxes in draw order with k = 0, 1, ...
+ * (k < COTB200_ERASE_MAX_COUNT).  A box covers rows [top, top + h) x columns [left, left + w) of sample n; where boxes of a
+ * sample overlap, the later one wins.  mode 0 ('const'): 0; 1 ('rand'): one N(0,1) value per (sample, box, channel); 2
+ * ('pixel'): one N(0,1) value per element.  The values come from Philox4x32-10 with key = seed and counter = (y * W + x, or
+ * 0xffffffff in mode 1, n, k, c / 4), Box-Muller-transformed, so they depend on the draw and the seed alone. */
+#define COTB200_ERASE_MAX_COUNT 32
+typedef struct cotb200_erase {
+  int mode;
+  int n_boxes;
+  unsigned long long seed;
+} cotb200_erase;
+typedef struct cotb200_erase_box {
+  int n, k;
+  int top, left, h, w;
+} cotb200_erase_box;
+/* Erases the boxes in place in y, a channels_last [N, C, H, W] tensor of dtype fp32 / bf16 / fp16 (the output of
+ * cotb200_u8_to_nhwc / cotb200_u8_mix_to_nhwc); written values are rounded to the dtype (round to nearest even).  erase_host /
+ * erase_dev: the same buffer on the host (validated) and on the device (read by the kernel).  Only the erased pixels are
+ * touched; n_boxes = 0 launches nothing.  Rejected with COTB200_EINVAL: a bad mode, a box outside its image or the batch, boxes
+ * out of order, a sample with more than COTB200_ERASE_MAX_COUNT boxes; COTB200_EDTYPE: another dtype. */
+int cotb200_aug_erase(int dtype, int N, int C, int H, int W, void* y, const cotb200_erase* erase_host,
+                      const cotb200_erase* erase_dev, void* stream);
 
 #ifdef __cplusplus
 }
