@@ -152,6 +152,9 @@ SYMBOLS = {
     "cotb200_soft_ce": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP, _VP]),
     "cotb200_soft_ce_bwd": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP, _VP,
                                                                  ctypes.c_longlong, _VP]),
+    "cotb200_jsd_ce": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP, ctypes.c_longlong, _VP, ctypes.c_float, ctypes.c_float, _VP, _VP, _VP]),
+    "cotb200_jsd_ce_bwd": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP, ctypes.c_longlong, _VP, ctypes.c_float, ctypes.c_float, _VP, _VP,
+                                                                _VP, ctypes.c_longlong, _VP]),
     "cotb200_topk_hits": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int),
                                                                _VP, _VP]),
     "cotb200_aug_resize_crop": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP, ctypes.c_longlong, _VP, _VP, _VP, ctypes.c_longlong, _VP, _VP]),

@@ -10,6 +10,9 @@ DataLoader workers still decode (JPEG -> RGB uint8 HWC, the reference dataset's 
   and returns the uint8 NCHW batch that fast_collate builds, ready for ``normalize_u8(mix=MixupCutmix.draw(...))``.
   With ``vflip`` a RandomVerticalFlip follows the horizontal one; without ``auto_augment``, ``color_jitter`` gives torchvision's
   ColorJitter (:100-109), both in one more kernel (cotb200_aug_color_jitter) between resize-crop and RandAugment.
+  With ``num_splits`` S >= 2 it is the reference's AugMixDataset over the separated transform (datasets/dataset.py:181-215,
+  transforms_factory.py:44-129): a clean view (crop, flips) and S - 1 views that each add their own RandAugment or ColorJitter
+  draw to the same crop, in fast_collate's split-major order, for the JSD loss (trainer.jsd_cross_entropy).
 * ``EvalTransform``: Resize(floor(size / crop_pct)) + CenterCrop(size) (:132-166) on the same resize kernel.
 * ``RandomErasing``: the reference's random erasing of the normalised batch (datasets/random_erasing.py, applied by
   PrefetchLoader, datasets/loader.py:72-91), boxes drawn on the host in its order and erased by one kernel (cotb200_aug_erase).
@@ -171,7 +174,12 @@ class TrainAugment:
     """The reference's training transform (transforms_imagenet_train with use_prefetcher=True) on the GPU."""
 
     def __init__(self, size=224, scale=(0.08, 1.0), ratio=(3. / 4., 4. / 3.), interpolation="bicubic", hflip=0.5,
-                 auto_augment="rand-m15-mstd0.5-n2", translate_const=100, cutout_const=40, vflip=0., color_jitter=None):
+                 auto_augment="rand-m15-mstd0.5-n2", translate_const=100, cutout_const=40, vflip=0., color_jitter=None,
+                 num_splits=0):
+        """num_splits: augmentation.aug_splits of the reference (0 and 1: one view per image)."""
+        if int(num_splits) != num_splits or num_splits < 0:
+            raise ValueError("num_splits must be 0 or a positive integer, got %r" % (num_splits,))
+        self.num_splits = int(num_splits) if num_splits >= 2 else 0
         if interpolation != "random" and interpolation not in _INTERP:
             raise ValueError("interpolation must be 'bilinear', 'bicubic' or 'random', got %r" % (interpolation,))
         self.size = int(size)
@@ -229,14 +237,9 @@ class TrainAugment:
             op["box"] = (x0, y0, min(S, x0 + 2 * px), min(S, y0 + 2 * px))
         return op
 
-    def draw_one(self, H, W, rnd, nrnd, tgen):
-        """The draws of one H x W image as a dict (the form oracle/aug_ref.train_sample takes)."""
-        i, j, h, w = rrc_params(H, W, self.scale, self.ratio, rnd)
-        p = dict(i=i, j=j, h=h, w=w, filter=self._filter(rnd), flip=False, ops=[])
-        if self.hflip > 0:
-            p["flip"] = bool(torch.rand(1, generator=tgen) < self.hflip)
-        if self.vflip > 0:
-            p["vflip"] = bool(torch.rand(1, generator=tgen) < self.vflip)
+    def _secondary(self, rnd, nrnd, tgen):
+        """The colour part's draws: RandAugment's ops, or ColorJitter's."""
+        p = dict(ops=[])
         if self.num_layers:
             for k in nrnd.choice(len(OPS), self.num_layers, replace=True):
                 p["ops"].append(self._op(int(k), rnd, nrnd))
@@ -246,12 +249,29 @@ class TrainAugment:
             p["jitter"] = dict(order=[k for k in perm if f[k] is not None], factors=f)
         return p
 
+    def draw_one(self, H, W, rnd, nrnd, tgen):
+        """The draws of one H x W image as a dict (the form oracle/aug_ref.train_sample takes).  With num_splits S >= 2 the dict
+        holds the clean view's draws (no ops) and, under "views", the S - 1 augmented views' colour draws, drawn after the
+        clean view's as AugMixDataset.__getitem__ runs them."""
+        i, j, h, w = rrc_params(H, W, self.scale, self.ratio, rnd)
+        p = dict(i=i, j=j, h=h, w=w, filter=self._filter(rnd), flip=False)
+        if self.hflip > 0:
+            p["flip"] = bool(torch.rand(1, generator=tgen) < self.hflip)
+        if self.vflip > 0:
+            p["vflip"] = bool(torch.rand(1, generator=tgen) < self.vflip)
+        if self.num_splits:
+            p["ops"] = []
+            p["views"] = [self._secondary(rnd, nrnd, tgen) for _ in range(self.num_splits - 1)]
+        else:
+            p.update(self._secondary(rnd, nrnd, tgen))
+        return p
+
     def draw(self, sizes, py_random, np_random, torch_gen):
         """Per-sample parameters of images of `sizes` [(H, W), ...], drawn image by image in the reference's order:
         crop, filter (interpolation 'random' only), flip, vertical flip (vflip > 0 only), the op choice, then per op apply /
         magnitude / sign (/ filter) and Cutout's two positions; or, with ColorJitter, randperm(4) and one uniform per enabled
         factor in brightness, contrast, saturation, hue order.  Returns the list of dicts; ``pack`` and ``pack_jitter`` turn it
-        into the device structs."""
+        into the device structs; ``pack_views`` the augmented views' ones when num_splits >= 2."""
         return [self.draw_one(int(H), int(W), py_random, np_random, torch_gen) for H, W in sizes]
 
     def pack(self, sizes, draws):
@@ -267,6 +287,16 @@ class TrainAugment:
             r["filter"], r["flip"], r["tmp_offset"] = p["filter"], int(p["flip"]), tmp
             off += 3 * H * W
             tmp += 3 * S * p["h"]
+            for s in range(2):
+                pack_op(r["ops"][s], p["ops"][s] if s < len(p["ops"]) else None)
+        return rec
+
+    def pack_views(self, draws):
+        """numpy SAMPLE_DTYPE [(S-1) * N] of the augmented views' RandAugment ops, split-major (view v of sample n at
+        v * N + n); the other fields stay 0, as cotb200_aug_randaug reads only the ops."""
+        views = [p["views"][v] for v in range(self.num_splits - 1) for p in draws]
+        rec = np.zeros(len(views), SAMPLE_DTYPE)
+        for r, p in zip(rec, views):
             for s in range(2):
                 pack_op(r["ops"][s], p["ops"][s] if s < len(p["ops"]) else None)
         return rec
@@ -305,15 +335,28 @@ class TrainAugment:
                 raise ValueError("expected HWC RGB uint8 images, got shape %s" % (a.shape,))
         sizes = [a.shape[:2] for a in imgs]
         draws = self.draw(sizes, random, np.random, torch.default_generator)
+        return self.collate_draws(imgs, [int(b[1]) for b in batch], draws)
+
+    def collate_draws(self, imgs, labels, draws):
+        """AugBatch of HWC uint8 `imgs` with their labels and draws.  With num_splits S >= 2 each image is shipped once; the
+        structs are the B clean samples then the (S-1) * B views (pack_views), the jitter structs and the labels cover all S * B
+        rows in fast_collate's order (labels repeated per split)."""
+        sizes = [a.shape[:2] for a in imgs]
         rec = self.pack(sizes, draws)
+        jit = [draws]
+        if self.num_splits:
+            rec = np.concatenate([rec, self.pack_views(draws)])
+            jit += [[p["views"][k] for p in draws] for k in range(self.num_splits - 1)]
         data = torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs]))
-        jitter = torch.from_numpy(self.pack_jitter(draws).view(np.uint8).copy()) if self.has_jitter_kernel else None
-        return AugBatch(data, torch.from_numpy(rec.view(np.uint8).copy()),
-                        torch.tensor([int(b[1]) for b in batch], dtype=torch.int64), jitter)
+        jitter = None
+        if self.has_jitter_kernel:
+            jitter = torch.from_numpy(np.concatenate([self.pack_jitter(d) for d in jit]).view(np.uint8).copy())
+        lab = torch.tensor(labels, dtype=torch.int64)
+        return AugBatch(data, torch.from_numpy(rec.view(np.uint8).copy()), lab.repeat(max(1, self.num_splits)), jitter)
 
     def __call__(self, batch, device=None):
         """AugBatch -> (uint8 [N, 3, S, S] on `device`, labels on `device`), on the current stream."""
-        out = run(batch, self.size, device, randaug=self.num_layers > 0)
+        out = run(batch, self.size, device, randaug=self.num_layers > 0, num_splits=self.num_splits)
         return out, batch.labels.to(out.device, non_blocking=True)
 
 
@@ -366,33 +409,54 @@ class EvalTransform:
         return out, batch.labels.to(out.device, non_blocking=True)
 
 
-def run(batch, S, device=None, randaug=True):
+def run(batch, S, device=None, randaug=True, num_splits=0):
     """The kernels on an AugBatch: H2D copies of the ragged buffer and the structs, resize-crop (+ flip), vertical flip and
     ColorJitter when the batch carries them, then RandAugment in place.  Returns uint8 [N, 3, S, S] on `device` (default: the
-    current CUDA device)."""
+    current CUDA device).  With num_splits >= 2 (TrainAugment(num_splits=...)'s batch of B images) the clean views are
+    resized, cropped and flipped into out[:B] and copied into each of the num_splits - 1 blocks after it, where the views'
+    ColorJitter or RandAugment run in place: N = num_splits * B."""
     device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     rec = batch.params.numpy().view(SAMPLE_DTYPE)
     N = len(rec)
+    splits = num_splits if num_splits >= 2 else 1
+    if N % splits:
+        raise ValueError("AugBatch: %d sample structs are not %d splits" % (N, splits))
+    B = N // splits
     data = batch.data.to(device, non_blocking=True)
     params = batch.params.to(device, non_blocking=True)
-    tmp_bytes = int((3 * S * rec["ch"].astype(np.int64)).sum())
+    tmp_bytes = int((3 * S * rec["ch"][:B].astype(np.int64)).sum())
     tmp = torch.empty(max(tmp_bytes, 1), dtype=torch.uint8, device=device)
     out = torch.empty(N, 3, S, S, dtype=torch.uint8, device=device)
     lib = _lib.load()
     st = _lib.stream_ptr(out)
     host = rec.ctypes.data_as(ctypes.c_void_p)
-    _lib.check(lib.cotb200_aug_resize_crop(N, S, data.data_ptr(), data.numel(), host, params.data_ptr(), tmp.data_ptr(),
+    _lib.check(lib.cotb200_aug_resize_crop(B, S, data.data_ptr(), data.numel(), host, params.data_ptr(), tmp.data_ptr(),
                                            tmp.numel(), out.data_ptr(), st), "aug_resize_crop")
+    jrec = jdev = None
     if batch.jitter is not None:
         jrec = batch.jitter.numpy().view(JITTER_DTYPE)
         if len(jrec) != N:
             raise ValueError("AugBatch: %d jitter structs for %d samples" % (len(jrec), N))
         if jrec["vflip"].any() or (jrec["order"] >= 0).any():
             jdev = batch.jitter.to(device, non_blocking=True)
-            _lib.check(lib.cotb200_aug_color_jitter(N, S, jrec.ctypes.data_as(ctypes.c_void_p), jdev.data_ptr(), out.data_ptr(),
-                                                    st), "aug_color_jitter")
-    if randaug and (rec["ops"]["op"] >= 0).any():
-        _lib.check(lib.cotb200_aug_randaug(N, S, host, params.data_ptr(), out.data_ptr(), st), "aug_randaug")
+
+    def jitter(lo, hi):
+        if jdev is not None and (jrec["vflip"][lo:hi].any() or (jrec["order"][lo:hi] >= 0).any()):
+            _lib.check(lib.cotb200_aug_color_jitter(hi - lo, S, jrec[lo:].ctypes.data_as(ctypes.c_void_p),
+                                                    jdev.data_ptr() + lo * JITTER_DTYPE.itemsize, out[lo].data_ptr(), st),
+                       "aug_color_jitter")
+
+    def randaug_(lo, hi):
+        if randaug and (rec["ops"]["op"][lo:hi] >= 0).any():
+            _lib.check(lib.cotb200_aug_randaug(hi - lo, S, rec[lo:].ctypes.data_as(ctypes.c_void_p),
+                                               params.data_ptr() + lo * SAMPLE_DTYPE.itemsize, out[lo].data_ptr(), st),
+                       "aug_randaug")
+    jitter(0, B)
+    if splits > 1:                                  # the augmented views start from the clean view, vertical flip included
+        for k in range(1, splits):
+            out[k * B:(k + 1) * B].copy_(out[:B])
+        jitter(B, N)
+    randaug_(B if splits > 1 else 0, N)
     return out
 
 

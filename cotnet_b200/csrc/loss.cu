@@ -7,8 +7,14 @@
 // CTA adds the B row losses in a fixed order: the loss is bit-identical from run to run.  lam = mix->target_lam is read from
 // device memory so that a captured graph follows every step's Mixup / CutMix draw.
 //
+// JsdCrossEntropy (loss/jsd.py) of the augmentation splits: label-smoothed cross entropy on the clean split plus alpha/S times
+// the KL divergence of every split's softmax from their clamped mixture.  One CTA per clean row handles its S rows; the row losses
+// are added by the same fixed-order launch as the soft-target loss.
+//
 // Also the validation metric: top-k hit counts (utils/meters.py:12-19 accuracy(), evaler/evaler.py:37-57) accumulated as int64
 // on the device, one warp per row, so that a captured eval graph needs no host synchronisation per batch.
+#include <climits>
+
 #include "common.cuh"
 
 namespace cotb200 {
@@ -31,6 +37,20 @@ __device__ __forceinline__ float ce_block_reduce(float v, float* sm, Op op) {
 
 __device__ __forceinline__ float ce_lam(const cotb200_mix* mix) { return mix ? mix->target_lam : 1.f; }
 
+// log-sum-exp and sum of one row, every thread of the CTA gets both
+template <typename T>
+__device__ __forceinline__ float ce_row_lse(const T* __restrict__ zr, int K, float* sm, float& sz) {
+  float mx = -INFINITY;
+  sz = 0.f;
+  for (int c = threadIdx.x; c < K; c += CE_THREADS) { const float v = to_acc(zr[c]); mx = fmaxf(mx, v); sz += v; }
+  mx = ce_block_reduce(mx, sm, [](float a, float b_) { return fmaxf(a, b_); });
+  sz = ce_block_reduce(sz, sm, [](float a, float b_) { return a + b_; });
+  float se = 0.f;
+  for (int c = threadIdx.x; c < K; c += CE_THREADS) se += expf(to_acc(zr[c]) - mx);
+  se = ce_block_reduce(se, sm, [](float a, float b_) { return a + b_; });
+  return mx + logf(se);
+}
+
 template <typename T>
 __global__ void __launch_bounds__(CE_THREADS)
 soft_ce_rows_kernel(const T* __restrict__ z, long long ld, const long long* __restrict__ labels, const cotb200_mix* __restrict__ mix,
@@ -38,15 +58,9 @@ soft_ce_rows_kernel(const T* __restrict__ z, long long ld, const long long* __re
   __shared__ float sm[CE_THREADS / 32];
   const int b = blockIdx.x;
   const T* zr = z + (long long)b * ld;
-  float mx = -INFINITY, sz = 0.f;
-  for (int c = threadIdx.x; c < K; c += CE_THREADS) { const float v = to_acc(zr[c]); mx = fmaxf(mx, v); sz += v; }
-  mx = ce_block_reduce(mx, sm, [](float a, float b_) { return fmaxf(a, b_); });
-  sz = ce_block_reduce(sz, sm, [](float a, float b_) { return a + b_; });
-  float se = 0.f;
-  for (int c = threadIdx.x; c < K; c += CE_THREADS) se += expf(to_acc(zr[c]) - mx);
-  se = ce_block_reduce(se, sm, [](float a, float b_) { return a + b_; });
+  float sz;
+  const float lse = ce_row_lse(zr, K, sm, sz);
   if (threadIdx.x == 0) {
-    const float lse = mx + logf(se);
     const float lam = ce_lam(mix);
     const long long y = labels[b];
     float own = __int_as_float(0x7fffffff), other = 0.f;
@@ -86,6 +100,121 @@ soft_ce_bwd_kernel(const T* __restrict__ z, long long ld, const long long* __res
     const float t = off + (c == y ? w_own : 0.f) + (c == yp ? w_other : 0.f);
     dr[c] = ok ? g * (expf(to_acc(zr[c]) - lse) - t) : __int_as_float(0x7fffffff);
   }
+}
+
+// ---------------------------------------------------------------- JSD + cross entropy of the augmentation splits
+static constexpr int JSD_MAX_S = 8;
+
+// class c of clean row b: p[s] = softmax(z_{b+sB})_c, lp[s] = its log (0 where p underflows to 0: the xlogy limit), the log of the
+// clamped mixture, and whether the clamp passes (torch's clamp mask is inclusive)
+template <typename T>
+__device__ __forceinline__ float jsd_class(const T* __restrict__ z, long long ld, int b, int B, int S, int c, const float* lse,
+                                           float* p, float* lp, bool& pass) {
+  float msum = 0.f;
+#pragma unroll
+  for (int s = 0; s < JSD_MAX_S; ++s) {
+    if (s < S) {
+      const float d = to_acc(z[(long long)(b + s * B) * ld + c]) - lse[s];
+      p[s] = expf(d);
+      lp[s] = p[s] > 0.f ? d : 0.f;
+      msum += p[s];
+    }
+  }
+  const float m = msum / (float)S;
+  pass = m >= 1e-7f && m <= 1.f;
+  return logf(fminf(fmaxf(m, 1e-7f), 1.f));
+}
+
+template <typename T>
+__global__ void __launch_bounds__(CE_THREADS)
+jsd_ce_rows_kernel(const T* __restrict__ z, long long ld, const long long* __restrict__ labels, int S, int B, int K, float off,
+                   float onoff, float alpha_s, float* __restrict__ rows) {
+  __shared__ float sm[CE_THREADS / 32];
+  const int b = blockIdx.x;
+  float lse[JSD_MAX_S], sz0 = 0.f;
+#pragma unroll
+  for (int s = 0; s < JSD_MAX_S; ++s) {
+    lse[s] = 0.f;
+    if (s < S) {
+      float sz;
+      lse[s] = ce_row_lse(z + (long long)(b + s * B) * ld, K, sm, sz);
+      if (s == 0) sz0 = sz;
+      if (threadIdx.x == 0) rows[b + s * B] = lse[s];
+    }
+  }
+  float kl = 0.f;
+  for (int c = threadIdx.x; c < K; c += CE_THREADS) {
+    float p[JSD_MAX_S], lp[JSD_MAX_S];
+    bool pass;
+    const float lm = jsd_class(z, ld, b, B, S, c, lse, p, lp, pass);
+#pragma unroll
+    for (int s = 0; s < JSD_MAX_S; ++s)
+      if (s < S) kl += p[s] * lp[s] - p[s] * lm;
+  }
+  kl = ce_block_reduce(kl, sm, [](float a, float b_) { return a + b_; });
+  if (threadIdx.x == 0) {
+    const long long y = labels[b];
+    const float own = (y >= 0 && y < K) ? to_acc(z[(long long)b * ld + y]) : __int_as_float(0x7fffffff);
+    rows[(long long)S * B + b] = (lse[0] - (off * sz0 + onoff * own)) + alpha_s * kl;
+  }
+}
+
+// dL/dp_sc = a (lp_sc - log m_c + [clamp binds]),  a = dloss * alpha / (S B); dz_sc = p_sc (dL/dp_sc - sum_c' p_sc' dL/dp_sc'),
+// plus dloss / B (p_0c - t_c) on the clean split
+template <typename T>
+__global__ void __launch_bounds__(CE_THREADS)
+jsd_ce_bwd_kernel(const T* __restrict__ z, long long ld, const long long* __restrict__ labels, int S, int B, int K, float off,
+                  float onoff, float alpha_sb, const float* __restrict__ rows, const float* __restrict__ dloss,
+                  float* __restrict__ dz, long long ldz) {
+  __shared__ float sm[CE_THREADS / 32];
+  const int b = blockIdx.x;
+  const float dl = __ldg(dloss), g = dl / (float)B, a = dl * alpha_sb;
+  const long long y = labels[b];
+  const bool ok = y >= 0 && y < K;
+  float lse[JSD_MAX_S], dot[JSD_MAX_S];
+#pragma unroll
+  for (int s = 0; s < JSD_MAX_S; ++s) {
+    lse[s] = s < S ? rows[b + s * B] : 0.f;
+    dot[s] = 0.f;
+  }
+  for (int c = threadIdx.x; c < K; c += CE_THREADS) {
+    float p[JSD_MAX_S], lp[JSD_MAX_S];
+    bool pass;
+    const float lm = jsd_class(z, ld, b, B, S, c, lse, p, lp, pass);
+#pragma unroll
+    for (int s = 0; s < JSD_MAX_S; ++s)
+      if (s < S) dot[s] += p[s] * (lp[s] - lm + (pass ? 0.f : 1.f));
+  }
+#pragma unroll
+  for (int s = 0; s < JSD_MAX_S; ++s)
+    if (s < S) dot[s] = ce_block_reduce(dot[s], sm, [](float u, float v) { return u + v; });
+  for (int c = threadIdx.x; c < K; c += CE_THREADS) {
+    float p[JSD_MAX_S], lp[JSD_MAX_S];
+    bool pass;
+    const float lm = jsd_class(z, ld, b, B, S, c, lse, p, lp, pass);
+    const float t = off + (c == y ? onoff : 0.f);
+#pragma unroll
+    for (int s = 0; s < JSD_MAX_S; ++s) {
+      if (s < S) {
+        float d = a * p[s] * ((lp[s] - lm + (pass ? 0.f : 1.f)) - dot[s]);
+        if (s == 0) d += g * (p[0] - t);
+        dz[(long long)(b + s * B) * ldz + c] = ok ? d : __int_as_float(0x7fffffff);
+      }
+    }
+  }
+}
+
+static int jsd_check(const char* what, int dtype, int S, int B, int K, const void* logits, long long ld, const long long* labels,
+                     float smoothing, float alpha) {
+  if (!logits || !labels) { set_error("%s: NULL pointer", what); return COTB200_ENULL; }
+  if (S < 2 || S > JSD_MAX_S) { set_error("%s: %d splits (2..%d supported)", what, S, JSD_MAX_S); return COTB200_EINVAL; }
+  if (B <= 0 || K <= 0 || ld < K || (long long)S * B > INT_MAX) {
+    set_error("%s: bad dims S=%d B=%d K=%d ld=%lld", what, S, B, K, ld); return COTB200_EINVAL;
+  }
+  if (!(smoothing >= 0.f && smoothing < 1.f)) { set_error("%s: smoothing %g outside [0, 1)", what, (double)smoothing); return COTB200_EINVAL; }
+  if (!(alpha >= 0.f && alpha < INFINITY)) { set_error("%s: alpha %g not finite and >= 0", what, (double)alpha); return COTB200_EINVAL; }
+  if (dtype == COTB200_F64) { set_error("%s: fp64 not supported", what); return COTB200_EDTYPE; }
+  return 0;
 }
 
 static int soft_ce_check(const char* what, int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
@@ -193,6 +322,45 @@ extern "C" int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, 
       COTB200_PROF_B("soft_ce_bwd", (double)B * K * (sizeof(T) + 4));
       soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, mix, B, K, off, onoff, rows, dloss, dz, ldz);
       return check_launch("soft_ce_bwd");
+    }
+  });
+  return 0;
+}
+
+extern "C" int cotb200_jsd_ce(int dtype, int S, int B, int K, const void* logits, long long ld, const long long* labels,
+                              float smoothing, float alpha, float* rows, float* loss, void* stream) {
+  int rc = jsd_check("jsd_ce", dtype, S, B, K, logits, ld, labels, smoothing, alpha);
+  if (rc) return rc;
+  if (!rows || !loss) { set_error("jsd_ce: NULL pointer"); return COTB200_ENULL; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const float off = smoothing / (float)K, onoff = 1.f - smoothing;
+  COTB200_DISPATCH_DTYPE(dtype, {
+    if constexpr (!std::is_same<T, double>::value) {
+      COTB200_PROF_B("jsd_ce", 2.0 * S * B * K * sizeof(T));
+      jsd_ce_rows_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, S, B, K, off, onoff, alpha / (float)S, rows);
+      if ((rc = check_launch("jsd_ce"))) return rc;
+      soft_ce_mean_kernel<<<1, CE_THREADS, 0, st>>>(rows + (long long)S * B, B, loss);
+      return check_launch("jsd_ce_mean");
+    }
+  });
+  return 0;
+}
+
+extern "C" int cotb200_jsd_ce_bwd(int dtype, int S, int B, int K, const void* logits, long long ld, const long long* labels,
+                                  float smoothing, float alpha, const float* rows, const float* dloss, float* dz, long long ldz,
+                                  void* stream) {
+  int rc = jsd_check("jsd_ce_bwd", dtype, S, B, K, logits, ld, labels, smoothing, alpha);
+  if (rc) return rc;
+  if (!rows || !dloss || !dz) { set_error("jsd_ce_bwd: NULL pointer"); return COTB200_ENULL; }
+  if (ldz < K) { set_error("jsd_ce_bwd: ldz %lld < K %d", ldz, K); return COTB200_EINVAL; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const float off = smoothing / (float)K, onoff = 1.f - smoothing;
+  COTB200_DISPATCH_DTYPE(dtype, {
+    if constexpr (!std::is_same<T, double>::value) {
+      COTB200_PROF_B("jsd_ce_bwd", (double)S * B * K * (2 * sizeof(T) + 4));
+      jsd_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, S, B, K, off, onoff, alpha / (float)(S * B), rows,
+                                                     dloss, dz, ldz);
+      return check_launch("jsd_ce_bwd");
     }
   });
   return 0;

@@ -217,9 +217,12 @@ class TrainStep:
 
     def __init__(self, model, lr=0.05, momentum=0.9, weight_decay=1e-4, nesterov=True, ema_decay=None,
                  loss_fn=None, amp_dtype=torch.bfloat16, weights="bf16", bucket_dtype=None, comm_chunks=3, overlap=True,
-                 process_group=None, label_smoothing=0., clip_grad=None, clip_mode="norm", opt="sgd", opt_eps=1e-8):
+                 process_group=None, label_smoothing=0., clip_grad=None, clip_mode="norm", opt="sgd", opt_eps=1e-8, jsd_splits=0):
         """label_smoothing > 0, or a `mix` given to the step, selects the soft-target loss (soft_target_cross_entropy) that the
         reference recipe trains with (train.py:198-209); otherwise the loss is `loss_fn` (default F.cross_entropy).
+        jsd_splits = S >= 2 selects JsdCrossEntropy(num_splits=S, alpha=12, smoothing=label_smoothing) (jsd_cross_entropy), the
+        reference's loss.jsd with augmentation.aug_splits = S (train.py:199-201): the batch is S splits of the same images in
+        TrainAugment(num_splits=S)'s order, so its size must be a multiple of S, and it cannot be mixed (train.py:157).
         clip_grad > 0 clips the averaged gradients before the update like the reference's solver.clip_grad / solver.clip_mode
         (train.py:270-273): 'norm' (clip_grad_norm_, norm 2; the norm is left in `grad_norm`, an fp32 device scalar), 'value'
         (clip_grad_value_) or 'agc' (adaptive_clip_grad without the classifier head).  None or <= 0: no clipping.
@@ -237,6 +240,9 @@ class TrainStep:
         self.model = model
         self.loss_fn = loss_fn or (lambda out, lab: F.cross_entropy(out.float(), lab))
         self.label_smoothing = float(label_smoothing)
+        if int(jsd_splits) != jsd_splits or jsd_splits < 0 or jsd_splits == 1:
+            raise ValueError("TrainStep: jsd_splits must be 0 (off) or >= 2, got %r" % (jsd_splits,))
+        self.jsd_splits = int(jsd_splits)
         self._gmix = None
         self.amp_dtype = amp_dtype
         self.nesterov = bool(nesterov)
@@ -472,12 +478,19 @@ class TrainStep:
 
     # ------------------------------------------------------------------ the step
     def _loss(self, out, lab, mix_dev):
+        if self.jsd_splits:
+            return JsdCrossEntropyFn.apply(out, lab, self.jsd_splits, self.label_smoothing, JSD_ALPHA)
         if mix_dev is None and self.label_smoothing == 0.:
             return self.loss_fn(out, lab)
         return SoftTargetCrossEntropyFn.apply(out, lab, mix_dev, self.label_smoothing)
 
     def forward_backward(self, x, lab, mix=None):
         """mix: None, a MixParams (MixupCutmix.draw) or its 32-byte device struct -- the loss reads the mixed targets' lam from it."""
+        if self.jsd_splits:
+            if mix is not None:
+                raise ValueError("TrainStep: the JSD loss takes augmentation splits, which the reference does not mix (train.py:157)")
+            if x.shape[0] % self.jsd_splits:
+                raise ValueError("TrainStep: batch of %d is not %d augmentation splits" % (x.shape[0], self.jsd_splits))
         mix_dev = mix.on_stream(self.dev) if isinstance(mix, MixParams) else mix
         if self._cuda:
             fused.step_begin(self.dev)
@@ -915,3 +928,56 @@ def soft_target_cross_entropy(logits, labels, mix=None, smoothing=0.):
     """The recipe's loss: mean over the batch of -sum_c t_c log softmax(logits)_c with t = mixup_target(labels, K, mix.target_lam,
     smoothing).  mix: None or a MixParams (MixupCutmix.draw)."""
     return SoftTargetCrossEntropyFn.apply(logits, labels, None if mix is None else mix.on_stream(logits.device), smoothing)
+
+
+#: JsdCrossEntropy's alpha as train.py:199-201 builds it (the module's default)
+JSD_ALPHA = 12.
+
+
+class JsdCrossEntropyFn(torch.autograd.Function):
+    """JsdCrossEntropy(num_splits, alpha, smoothing)(logits, labels) (loss/jsd.py) on cotb200_jsd_ce / cotb200_jsd_ce_bwd: the
+    label-smoothed cross entropy of the clean split plus alpha/S times the KL divergence of every split's softmax from their
+    clamped mixture.  logits [S*B, K] fp32 / bf16 / fp16 with unit column stride, split-major (fast_collate's order); labels int64
+    [>= B], only the first B read.  Returns the fp32 loss.  Where a probability underflows to 0 the gradient takes the xlogy limit
+    (0) instead of the reference's NaN."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, num_splits, smoothing, alpha):
+        assert logits.is_cuda and logits.dim() == 2 and logits.stride(1) == 1 and labels.dtype == torch.int64
+        N, K = logits.shape
+        S = int(num_splits)
+        B = N // S
+        logits, labels = logits.detach(), labels.contiguous()
+        rows = torch.empty(N + B, dtype=torch.float32, device=logits.device)
+        loss = torch.empty((), dtype=torch.float32, device=logits.device)
+        lib, st, dt = _lib.load(), _lib.stream_ptr(logits), _lib.dtype_code(logits)
+        _lib.check(lib.cotb200_jsd_ce(dt, S, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), float(smoothing),
+                                      float(alpha), rows.data_ptr(), loss.data_ptr(), st), "jsd_ce")
+        ctx.save_for_backward(logits, labels, rows)
+        ctx.args = (S, B, float(smoothing), float(alpha))
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        logits, labels, rows = ctx.saved_tensors
+        S, B, smoothing, alpha = ctx.args
+        K = logits.shape[1]
+        dloss = dloss.float().contiguous()
+        dz = torch.empty(S * B, K, dtype=torch.float32, device=logits.device)
+        lib, st, dt = _lib.load(), _lib.stream_ptr(logits), _lib.dtype_code(logits)
+        _lib.check(lib.cotb200_jsd_ce_bwd(dt, S, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), smoothing, alpha,
+                                          rows.data_ptr(), dloss.data_ptr(), dz.data_ptr(), K, st), "jsd_ce_bwd")
+        return dz.to(logits.dtype), None, None, None, None
+
+
+def jsd_cross_entropy(logits, labels, num_splits, smoothing=0., alpha=JSD_ALPHA):
+    """The reference's JsdCrossEntropy(num_splits, alpha, smoothing)(logits, labels) for a batch of `num_splits` augmentation
+    splits (TrainAugment(num_splits=...)'s order): see JsdCrossEntropyFn."""
+    S = int(num_splits)
+    if S != num_splits or S < 2:
+        raise ValueError("jsd_cross_entropy: num_splits must be an integer >= 2, got %r" % (num_splits,))
+    if logits.dim() != 2 or logits.shape[0] % S:
+        raise ValueError("jsd_cross_entropy: %s logits are not %d splits of [B, K]" % (tuple(logits.shape), S))
+    if labels.shape[0] < logits.shape[0] // S:
+        raise ValueError("jsd_cross_entropy: %d labels for %d clean rows" % (labels.shape[0], logits.shape[0] // S))
+    return JsdCrossEntropyFn.apply(logits, labels, S, smoothing, alpha)

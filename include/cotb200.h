@@ -494,6 +494,24 @@ int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long long ld, c
 int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
                         const cotb200_mix* mix, float smoothing, const float* rows, const float* dloss, float* dz,
                         long long ldz, void* stream);
+/* JsdCrossEntropy(num_splits=S, alpha, smoothing) (loss/jsd.py) of the augmentation splits.  logits: fp32 / bf16 / fp16
+ * [S*B, K] with row pitch ld, split-major (row b + s*B is view s of sample b, view 0 the clean one); labels int64, only the
+ * first B read.  Per clean row b, with p_sc = softmax(z_{b+sB})_c and m_c = clamp((sum_{s=0..S-1} p_sc) / S, 1e-7, 1):
+ *   loss_b = ce_b + alpha/S * sum_s sum_c (xlogy(p_sc, p_sc) - p_sc log m_c),
+ * ce_b the cotb200_soft_ce row of z_b without mixing (LabelSmoothingCrossEntropy; plain cross entropy at smoothing 0).  rows:
+ * fp32 [S*B + B] written: rows[b + s*B] = lse(z_{b+sB}) (the backward reads them), rows[S*B + b] = loss_b.  loss: fp32 [1],
+ * the mean of the B row losses added in a fixed order.  2 <= S <= 8, 0 <= smoothing < 1, alpha finite and >= 0.  A label
+ * outside [0, K) makes its row (and the mean) NaN; it is never read out of bounds.
+ * Where p_sc underflows to exactly 0 the term is taken at its xlogy limit, 0 in the loss and in the gradient; the reference's
+ * autograd returns NaN there (0 * log 0 in the derivative of xlogy). */
+int cotb200_jsd_ce(int dtype, int S, int B, int K, const void* logits, long long ld, const long long* labels,
+                   float smoothing, float alpha, float* rows, float* loss, void* stream);
+/* dz = dloss[0] * d(mean_b loss_b)/dz, fp32 [S*B, K] with row pitch ldz: per split the softmax Jacobian applied to
+ * alpha/(S*B) * (log p_sc - log m_c + [the clamp binds at c]) (torch's clamp passes the gradient on the closed interval
+ * [1e-7, 1]), plus the cross-entropy gradient on split 0.  dloss is read from device memory; an invalid label makes all S rows
+ * of its sample NaN. */
+int cotb200_jsd_ce_bwd(int dtype, int S, int B, int K, const void* logits, long long ld, const long long* labels,
+                       float smoothing, float alpha, const float* rows, const float* dloss, float* dz, long long ldz, void* stream);
 
 /* ---- validation metric ----
  * Top-k hit counts of utils/meters.py:12-19 (accuracy(): output.topk(maxk) then eq), accumulated on the device so that a
