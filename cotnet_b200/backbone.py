@@ -11,7 +11,6 @@ max-pool, [3,4,6,3]/[3,4,23,3] stages, 1x1 conv down-sample, 3x3/2 avg-pool in f
 of stride-2 blocks (``avd``, :199-202,:237-238), global average pool + fc.
 """
 import math
-import os
 
 import torch
 import torch.nn as nn
@@ -42,19 +41,11 @@ class Bottleneck(nn.Module):
     def zero_init_last_bn(self):
         nn.init.zeros_(self.bn3.weight)
 
-    #: (opt-in, COTB200_FORK=1) training: hand the block output to the next block as TWO aliases (conv1 reads one, the shortcut the
-    #: other) so that their gradients are summed inside bn3's backward kernels instead of by an autograd add (fused._two_grads).
-    #: Off by default: ATen's add streams at the HBM roof, while the extra read costs the BatchNorm backward kernels, which run
-    #: below the roof, more than the add saves.  Always False on the network's last block.
-    fork_output = os.environ.get("COTB200_FORK", "0") != "0"
-
     def forward(self, x, drop_scale=None):
         """drop_scale: None or [B] per-sample stochastic-depth scales applied to bn3's output before the residual add
         (models/cotnet.py:256-257); the trunk draws them (StochasticDepth)."""
-        xs = x if isinstance(x, tuple) else (x, x)
-        if fused.supported(xs[0]):
-            return self._forward_fused(xs, drop_scale)
-        x = xs[0]
+        if fused.supported(x):
+            return self._forward_fused(x, drop_scale)
         residual = x
         x = self.act1(self.bn1(self.conv1(x)))
         if self.avd is not None:
@@ -68,20 +59,19 @@ class Bottleneck(nn.Module):
         x += residual
         return self.act3(x)
 
-    def _forward_fused(self, xs, drop_scale=None):
+    def _forward_fused(self, x, drop_scale=None):
         """channels_last path: bn1+ReLU and bn3+residual+ReLU (SURVEY section 8f rank 1) run on the fused BatchNorm
         kernels (2 passes each way) instead of ATen's channels_last batch-norm kernels."""
         cl = torch.channels_last
-        x, residual = xs                           # two aliases of the previous block's output (or the same tensor twice)
+        residual = x
         y = fused.conv1x1_bn(x, self.conv1, self.bn1, relu=True)
         if self.avd is not None:
             y = fused.avg_pool3x3s2(y)              # nn.AvgPool2d(3, 2, padding=1) on the fused NHWC kernel
         y = self.conv2(y.contiguous(memory_format=cl))
         if self.downsample is not None:
             residual = fused.conv1x1_bn(residual, self.downsample[0], self.downsample[1], relu=False)
-        fork = self.fork_output and torch.is_grad_enabled() and self.training
         return fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=True,
-                                res=residual.contiguous(memory_format=cl), fork=fork, drop_scale=drop_scale)
+                                res=residual.contiguous(memory_format=cl), drop_scale=drop_scale)
 
 
 class StochasticDepth:
@@ -167,7 +157,6 @@ class CoTResNet(StochasticDepth, nn.Module):
                 blocks.append(Bottleneck(inplanes, planes, s, down, cardinality, base_width))
                 inplanes = planes * Bottleneck.expansion
             self.add_module("layer%d" % (i + 1), nn.Sequential(*blocks))
-        self.layer4[-1].fork_output = False          # the network's last block feeds the global pool only
         self.num_features = inplanes
         self.global_pool = nn.AdaptiveAvgPool2d(1)
         self.fc = nn.Linear(self.num_features, num_classes)

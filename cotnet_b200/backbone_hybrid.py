@@ -16,8 +16,6 @@ stage, avg-pool down-sampling, optional BlurPool anti-aliasing (152).
 """
 import math
 
-import os
-
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -124,12 +122,8 @@ class CoTBottleneck(nn.Module):
             return fused.avg_pool3x3s2(y)
         return self.avd(y)
 
-    fork_output = os.environ.get("COTB200_FORK", "0") != "0"             # see backbone.Bottleneck.fork_output
-
     def forward(self, x, drop_scale=None):
         cl = torch.channels_last
-        xs = x if isinstance(x, tuple) else (x, x)
-        x, xres = xs
         if fused.supported(x):      # channels_last CUDA tensors: fused BatchNorm(+ReLU,+residual) glue like backbone.Bottleneck
             y = fused.conv1x1_bn(x, self.conv1, self.bn1, relu=True)
             if self.avd is not None and self.avd_first:
@@ -137,13 +131,12 @@ class CoTBottleneck(nn.Module):
             y = self.conv2(y.contiguous(memory_format=cl))
             if self.avd is not None and not self.avd_first:
                 y = self._pool(y.contiguous(memory_format=cl))
-            residual = xres
+            residual = x
             if self.downsample is not None:
                 d = self.downsample
-                residual = fused.conv1x1_bn(d[0](xres).contiguous(memory_format=cl), d[1], d[2], relu=False)
-            fork = self.fork_output and torch.is_grad_enabled() and self.training
+                residual = fused.conv1x1_bn(d[0](x).contiguous(memory_format=cl), d[1], d[2], relu=False)
             return fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=True,
-                                    res=residual.contiguous(memory_format=cl), fork=fork, drop_scale=drop_scale)
+                                    res=residual.contiguous(memory_format=cl), drop_scale=drop_scale)
         residual = x
         y = self.act1(self.bn1(self.conv1(x)))
         if self.avd is not None and self.avd_first:
@@ -188,7 +181,6 @@ class CoTHybridNet(StochasticDepth, nn.Module):
                 blocks.append(CoTBottleneck(b, inplanes, planes, stride, down, aa_layer=aa_layer, **block_args))
                 inplanes = planes * 4
             setattr(self, "layer%d" % (i + 1), nn.Sequential(*blocks))
-        self.layer4[-1].fork_output = False          # the network's last block feeds the global pool only
         self.num_features = 2048
         self.global_pool = nn.AdaptiveAvgPool2d(1)
         self.fc = nn.Linear(self.num_features, num_classes)

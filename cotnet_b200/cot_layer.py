@@ -15,8 +15,6 @@ Forward maths is SURVEY.md Appendix A.  Differences from the reference's eager g
     ``.contiguous()`` gives; channels_last in -> channels_last out, no transposes), and the LocalConv runs on
     the H100 kernels (NHWC kernels for channels_last tensors).
 """
-import os
-
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -109,36 +107,32 @@ class CotLayer(nn.Module):
         # x has three consumers and k two: their gradients (two of them channel slices of the concat's) are summed by
         # one kernel each (fused.fan_out) instead of autograd's pairwise strided adds
         xk, xc, xv = fused.fan_out(x, 3)
-        be = self.train_conv_backend
-        if B * H * W < self.tc_min_pixels and be not in ("cudnn", "tc_e0"):
-            be = "tc_e0"           # small problems: only the concat-free embed.0 GEMM stays on wgmma (fixed per-launch costs dominate)
-        if (be.endswith("+k") and self.dim <= self.tc_key_max_dim and fused.tc_supported(x, self.dim)
-                and self.key_embed[0].weight.dtype == x.dtype):
+        # Which convolutions run on the wgmma kernels is a rule over geometry.  Below fused.TC_MIN_PIXELS pixels their fixed
+        # per-launch costs outweigh the byte savings, so only the concat-free embed.0 GEMM stays there; key_embed also needs
+        # dim <= fused.TC_KEY_MAX_DIM (stages 1-2).
+        tc_ok = fused.tc_supported(x, self.dim)
+        big = B * H * W >= fused.TC_MIN_PIXELS
+        if big and self.dim <= fused.TC_KEY_MAX_DIM and tc_ok and self.key_embed[0].weight.dtype == x.dtype:
             # key_embed on the haloed-tile wgmma convolution: forward with the BatchNorm statistics in the epilogue, data gradient by
             # the same kernel (flipped / transposed weights); the grouped weight gradient stays on cuDNN
             ke = self.key_embed
             k = fused.TcConv3x3Fn.apply(xk, ke[0].weight, ke[1].weight, ke[1].bias, ke[1], ke[0].groups, True)
-            be = be[:-2]
         else:
-            be = be[:-2] if be.endswith("+k") else be
             k = fused.bn_act(self.key_embed[0](xk).contiguous(memory_format=cl), self.key_embed[1], relu=True)
         kc, kt = fused.fan_out(k, 2)
-        hybrid = (be in ("tc_e0", "tc_1x1", "tc_e0e3", "tc_all1x1") and fused.tc_supported(x, self.dim)
-                  and k.dtype == x.dtype)
-        if hybrid:      # embed.0 as ONE wgmma GEMM over the operand pairs (x, W_x), (k, W_k): no concat, statistics in the epilogue
+        tc_ok = tc_ok and k.dtype == x.dtype
+        if tc_ok:       # embed.0 as ONE wgmma GEMM over the operand pairs (x, W_x), (k, W_k): no concat, statistics in the epilogue
             em = self.embed
             e = fused.TcConv1x1Fn.apply(xc, kc, em[0].weight, None, em[1].weight, em[1].bias, em[1], True, None)
         else:
             e = fused.bn_act(self.embed[0](torch.cat([xc, kc], dim=1)).contiguous(memory_format=cl), self.embed[1], relu=True)
         # embed.3 runs bias-free; its bias is added (and differentiated) inside the GroupNorm kernels
-        if hybrid and be in ("tc_e0e3", "tc_all1x1"):
+        if tc_ok and big:
             l = fused.TcConv1x1Fn.apply(e, None, self.embed[3].weight, None, None, None, None, False, None)
-        else:
-            l = F.conv2d(e, self.embed[3].weight, None)
-        if hybrid and be in ("tc_1x1", "tc_all1x1"):
             cv = self.conv1x1
             v = fused.TcConv1x1Fn.apply(xv, None, cv[0].weight, None, cv[1].weight, cv[1].bias, cv[1], False, None)
         else:
+            l = F.conv2d(e, self.embed[3].weight, None)
             v = fused.bn_act(self.conv1x1[0](xv).contiguous(memory_format=cl), self.conv1x1[1], relu=False)
         if l.dtype != v.dtype:
             l = l.to(v.dtype)
@@ -197,46 +191,14 @@ class CotLayer(nn.Module):
         u = fused.AggTapFn.apply(v.view(B, H, W, C).permute(0, 3, 1, 2), w, 1, gc)
         return fused.cot_tail(u, k, self.bn, self.se)
 
-    def _forward_tc_train(self, x):
-        """Autograd-capable path with every convolution of the block on the wgmma kernels (forward + data gradients;
-        BatchNorm batch statistics from the GEMM epilogues; no torch.cat, no separate statistics pass)."""
-        B, C, H, W = x.shape
-        ke, em, cv = self.key_embed, self.embed, self.conv1x1
-        k = fused.TcConv3x3Fn.apply(x, ke[0].weight, ke[1].weight, ke[1].bias, ke[1], 4, True)
-        e = fused.TcConv1x1Fn.apply(x, k, em[0].weight, None, em[1].weight, em[1].bias, em[1], True, None)
-        l = fused.TcConv1x1Fn.apply(e, None, em[3].weight, em[3].bias, None, None, None, False, None)
-        v = fused.TcConv1x1Fn.apply(x, None, cv[0].weight, None, cv[1].weight, cv[1].bias, cv[1], False, None)
-        gc = fused.tap_chunk(C // 8)
-        w = fused.group_norm9(l, em[4], gc)
-        u = fused.AggTapFn.apply(v, w, 1, gc)
-        return fused.cot_tail(u, k, self.bn, self.se)
-
-    #: Training-mode convolution backend of the block (COTB200_TRAIN_CONV):
-    #:   "cudnn"      cuDNN convolutions + the fused normalisation kernels
-    #:   "tc_e0"      embed.0 (the 2C -> C/2 conv on [x ; k]) as ONE concat-free two-operand-pair wgmma GEMM: forward with the
-    #:                BatchNorm statistics in the epilogue, data and weight gradients on the wgmma kernels
-    #:   "tc_1x1" / "tc_e0e3" / "tc_all1x1"   + conv1x1 / + embed.3 / + both (all three 1x1 convolutions of the block; with
-    #:                "tc_all1x1" the enclosing bottleneck's conv1 / conv3 / downsample of stages 1-2 as well, fused.conv1x1_bn)
-    #:   "...+k"      key_embed (grouped 3x3) on the haloed-tile wgmma convolution for dim <= tc_key_max_dim
-    #:   "tc"         the older all-wgmma autograd path (TcConv3x3Fn + TcConv1x1Fn for everything, per-tap conv at 7x7)
-    #: Inference (no_grad, eval) always takes the wgmma path when the shape allows.
-    #: "tc_all1x1+k" is the default (bf16 channels_last, dim % 64 == 0; anything else uses cuDNN for that convolution): it puts the
-    #: most of the step on this library.  tools/bench_conv.py and bench.py compare the backends (COTB200_TRAIN_CONV).
-    train_conv_backend = os.environ.get("COTB200_TRAIN_CONV", "tc_all1x1+k")
-    #: "+k" suffix of the backend: key_embed on the haloed-tile wgmma convolution for dim <= this (stages 1-2;
-    #: at 14x14 / 7x7 cuDNN's grouped kernels are used)
-    tc_key_max_dim = int(os.environ.get("COTB200_TC_KEY_MAX_DIM", "128"))
-    #: pixels (B*H*W) below which the backend degrades to "tc_e0": on the 14x14 / 7x7 stages the fixed per-launch costs of the
-    #: all-wgmma path outweigh its byte savings
-    tc_min_pixels = int(os.environ.get("COTB200_TC_MIN_PIXELS", "100000"))
+    #: the label bench.py reports for the training path; nothing branches on it
+    train_conv_backend = "tc_all1x1+k"
 
     def forward(self, x):
         B, C, H, W = x.shape
         if self.kernel_size == 3 and fused.supported(x):
             if self._tc_eval_ok(x):
                 return self._forward_tc_eval(x)
-            if self.train_conv_backend == "tc" and fused.tc_supported(x, self.dim):
-                return self._forward_tc_train(x)
             return self._forward_fused(x)
         k = self.key_embed(x)                                              # static context
         w = self.embed(torch.cat([x, k], dim=1))                           # logits, GroupNorm'ed, NOT softmaxed
@@ -298,33 +260,21 @@ class CoXtLayer(nn.Module):
         kc, kt = fused.fan_out(k, 2)
         wx, wk = _coxt_embed0_dense(self.embed[0].weight, G)
         w0 = torch.cat([wx, wk], 1).reshape(C // 2, 2 * C, 1, 1)
-        be = self.train_conv_backend.replace("+k", "")      # the grouped key conv of CoXt (groups 8, dense block-diagonal) stays on cuDNN
-        use_tc = be != "cudnn" and x.dtype == torch.bfloat16 and C % 16 == 0 and k.dtype == x.dtype and w0.dtype == x.dtype
         em, cv = self.embed, self.conv1x1
-        if use_tc:
+        # only embed.0 (the concat-free two-pair GEMM) runs on the wgmma kernels: the dense block-diagonal form of the other
+        # grouped convolutions doubles their FLOPs, and the grouped key conv (groups 8) stays on cuDNN as well
+        if x.dtype == torch.bfloat16 and C % 16 == 0 and k.dtype == x.dtype and w0.dtype == x.dtype:
             e = fused.TcConv1x1Fn.apply(xc, kc, w0, None, em[1].weight, em[1].bias, em[1], True, None)
         else:
             e = fused.bn_act(F.conv2d(torch.cat([xc, kc], dim=1), w0).contiguous(memory_format=cl), em[1], relu=True)
-        w3 = _dense_from_grouped(em[3].weight, G)
-        if use_tc and be in ("tc_e0e3", "tc_all1x1", "tc") and w3.shape[0] % 8 == 0:
-            l = fused.TcConv1x1Fn.apply(e, None, w3, None, None, None, None, False, None)
-        else:
-            l = F.conv2d(e, w3, None)
-        wv = _dense_from_grouped(cv[0].weight, G)
-        if use_tc and be in ("tc_1x1", "tc_all1x1", "tc"):
-            v = fused.TcConv1x1Fn.apply(xv, None, wv, None, cv[1].weight, cv[1].bias, cv[1], False, None)
-        else:
-            v = fused.bn_act(F.conv2d(xv, wv).contiguous(memory_format=cl), cv[1], relu=False)
+        l = F.conv2d(e, _dense_from_grouped(em[3].weight, G), None)
+        v = fused.bn_act(F.conv2d(xv, _dense_from_grouped(cv[0].weight, G)).contiguous(memory_format=cl), cv[1], relu=False)
         if l.dtype != v.dtype:
             l = l.to(v.dtype)
         gc = fused.tap_chunk(C // 8, self.dw_group)
         w = fused.group_norm9(l.contiguous(memory_format=torch.channels_last), self.embed[4], gc, self.embed[3].bias)
         u = fused.AggTapFn.apply(v.contiguous(memory_format=torch.channels_last), w, self.dw_group, gc)
         return fused.cot_tail(u, kt.contiguous(memory_format=torch.channels_last), self.bn, self.se)
-
-    #: CoXt: the dense block-diagonal form of its grouped 1x1 convolutions doubles their FLOPs, so only embed.0 (the concat-free
-    #: two-pair GEMM) runs on the wgmma kernels by default
-    train_conv_backend = os.environ.get("COTB200_TRAIN_CONV_COXT", "tc_e0")
 
     def forward(self, x):
         B, C, H, W = x.shape

@@ -10,17 +10,15 @@ They turn the reference block's long eager chains into a few HBM passes while ke
 
 All tensors are channels_last (NHWC memory); math is fp32; outputs keep the input dtype.
 """
-import os as _os
-
 import torch
 from torch.autograd import Function
 
 from . import _lib
 
-#: ReLU mask of the BatchNorm backward without reading y back (on by default; COTB200_BN_MASK=0 restores the y-reading path):
-#: with a residual the forward also writes a 1-bit mask (relu code 3), without one the wgmma functions recompute it from their
-#: own pre-activation and scale/shift (relu code 2).  Bit-identical either way; read at call time so tests can flip it.
-BN_MASK = _os.environ.get("COTB200_BN_MASK", "1") != "0"
+#: ReLU mask of the BatchNorm backward without reading y back: with a residual the forward also writes a 1-bit mask (relu
+#: code 3), without one the wgmma functions recompute it from their own pre-activation and scale/shift (relu code 2).
+#: False takes the y-reading path, which gives the same bits; it is read at call time so tests can compare the two.
+BN_MASK = True
 
 
 def _relu_mask_buf(x):
@@ -212,33 +210,32 @@ def _drop_scale(ds, x):
     return ds.float().contiguous()
 
 
-def _bn_bwd(lib, dt, B, HW, C, dy, dy2, x, y, scale, shift, mean, rstd, rcode, sums, batch, inv_n, dx, dres, ds, st):
-    """BatchNorm backward (sums + apply) of the plain / two-gradient form, or of the drop-path form when ds is given.
+def _bn_bwd(lib, dt, B, HW, C, dy, x, y, scale, shift, mean, rstd, rcode, sums, batch, inv_n, dx, dres, ds, st):
+    """BatchNorm backward (sums + apply) of the plain form, or of the drop-path form when ds is given.
     rcode 3: `y` is the 1-bit ReLU mask of _bn_apply_batch(mask=...)."""
     if rcode == 3:
         if sums is not None:
-            _lib.check(lib.cotb200_bn_bwd_sums_mask(dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), y.data_ptr(),
+            _lib.check(lib.cotb200_bn_bwd_sums_mask(dt, B, HW, C, dy.data_ptr(), None, x.data_ptr(), y.data_ptr(),
                                                     mean.data_ptr(), rstd.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(),
                                                     _lib.ptr(ds), st), "bn_bwd_sums_mask")
-        _lib.check(lib.cotb200_bn_bwd_apply_mask(dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), y.data_ptr(), scale.data_ptr(),
+        _lib.check(lib.cotb200_bn_bwd_apply_mask(dt, B, HW, C, dy.data_ptr(), None, x.data_ptr(), y.data_ptr(), scale.data_ptr(),
                                                  mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
                                                  _lib.ptr(sums[1]) if batch else None, inv_n, dx.data_ptr(), _lib.ptr(dres), _lib.ptr(ds),
                                                  st), "bn_bwd_apply_mask")
         return
     if sums is not None:
-        args = (dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), _lib.ptr(y), _lib.ptr(scale), _lib.ptr(shift),
-                mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(), sums[1].data_ptr())
+        rest = (x.data_ptr(), _lib.ptr(y), _lib.ptr(scale), _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), rcode,
+                sums[0].data_ptr(), sums[1].data_ptr())
         if ds is None:
-            _lib.check(lib.cotb200_bn_bwd_sums2(*args, st), "bn_bwd_sums")
+            _lib.check(lib.cotb200_bn_bwd_sums(dt, B, HW, C, dy.data_ptr(), *rest, st), "bn_bwd_sums")
         else:
-            _lib.check(lib.cotb200_bn_bwd_sums_ds(*args, ds.data_ptr(), st), "bn_bwd_sums_ds")
-    args = (dt, B, HW, C, dy.data_ptr(), _lib.ptr(dy2), x.data_ptr(), _lib.ptr(y), scale.data_ptr(), _lib.ptr(shift),
-            mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None, _lib.ptr(sums[1]) if batch else None,
-            inv_n, rcode, dx.data_ptr(), _lib.ptr(dres))
+            _lib.check(lib.cotb200_bn_bwd_sums_ds(dt, B, HW, C, dy.data_ptr(), None, *rest, ds.data_ptr(), st), "bn_bwd_sums_ds")
+    rest = (x.data_ptr(), _lib.ptr(y), scale.data_ptr(), _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(),
+            _lib.ptr(sums[0]) if batch else None, _lib.ptr(sums[1]) if batch else None, inv_n, rcode, dx.data_ptr(), _lib.ptr(dres))
     if ds is None:
-        _lib.check(lib.cotb200_bn_bwd_apply2(*args, st), "bn_bwd_apply")
+        _lib.check(lib.cotb200_bn_bwd_apply(dt, B, HW, C, dy.data_ptr(), *rest, st), "bn_bwd_apply")
     else:
-        _lib.check(lib.cotb200_bn_bwd_apply_ds(*args, ds.data_ptr(), st), "bn_bwd_apply_ds")
+        _lib.check(lib.cotb200_bn_bwd_apply_ds(dt, B, HW, C, dy.data_ptr(), None, *rest, ds.data_ptr(), st), "bn_bwd_apply_ds")
 
 
 class BNActFn(Function):
@@ -249,9 +246,8 @@ class BNActFn(Function):
     y = act(drop_scale[b]*BatchNorm2d(x) (+ res)) in the same kernels."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, res, bn, relu, fork=False, drop_scale=None):
+    def forward(ctx, x, weight, bias, res, bn, relu, drop_scale=None):
         assert _is_cl(x) and (res is None or (_is_cl(res) and res.dtype == x.dtype and res.shape == x.shape))
-        ctx.set_materialize_grads(False)
         B, C, H, W = x.shape
         lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.dtype_code(x)
         x = x.detach()
@@ -276,48 +272,31 @@ class BNActFn(Function):
         rcode = 0 if not relu else (2 if res is None else (3 if mask is not None else 1))
         ctx.save_for_backward(x, mask if rcode == 3 else (y if rcode == 1 else None), ss, ds)
         ctx.cfg = (rcode, batch, res is not None, weight.dtype, bias.dtype)
-        if fork:            # two aliases of ONE tensor: each consumer's gradient reaches backward() separately (see _two_grads)
-            return y, y.detach()
         return y
 
     @staticmethod
-    def backward(ctx, *grads):
+    def backward(ctx, dy):
         x, y, ss, ds = ctx.saved_tensors          # y: the forward output (rcode 1), its 1-bit ReLU mask (rcode 3) or None
         rcode, batch, has_res, wdt, bdt = ctx.cfg
         B, C, H, W = x.shape
         lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.dtype_code(x)
-        dy, dy2 = _two_grads(grads)
-        if dy is None:
-            return (None,) * 8
+        dy = dy.contiguous(memory_format=torch.channels_last)
         sums = None
         if batch or ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
             sums = torch.zeros(2, C, dtype=torch.float32, device=x.device)  # escapes as dgamma/dbeta
         dx = torch.empty_like(x, memory_format=torch.channels_last)
         dres = torch.empty_like(x, memory_format=torch.channels_last) if (has_res and ctx.needs_input_grad[3]) else None
-        _bn_bwd(lib, dt, B, H * W, C, dy, dy2, x, y, ss[0], ss[1], ss[2], ss[3], rcode, sums, batch, 1.0 / float(B * H * W), dx, dres,
-                ds, st)
+        _bn_bwd(lib, dt, B, H * W, C, dy, x, y, ss[0], ss[1], ss[2], ss[3], rcode, sums, batch, 1.0 / float(B * H * W), dx, dres, ds,
+                st)
         dgamma = sums[1].to(wdt) if ctx.needs_input_grad[1] else None
         dbeta = sums[0].to(bdt) if ctx.needs_input_grad[2] else None
-        return dx, dgamma, dbeta, dres, None, None, None, None
+        return dx, dgamma, dbeta, dres, None, None, None
 
 
-def _two_grads(grads):
-    """Incoming gradients of a (possibly forked) output: (dy, dy2) as channels_last tensors, dy2 None when there is one gradient.
-    A forked BatchNorm output feeds two consumers -- the next bottleneck's conv1 and its shortcut (models/cotnet.py:228-262) -- and
-    autograd would add their gradients with a separate kernel (read 2 + write 1 of the block-sized tensor);
-    handing both to the BatchNorm backward kernels, which sum them in fp32 while they stream dy anyway, costs one extra read each."""
-    g = [t.contiguous(memory_format=torch.channels_last) for t in grads if t is not None]
-    if not g:
-        return None, None
-    if len(g) == 1:
-        return g[0], None
-    return g[0], g[1]
-
-
-def bn_act(x, bn: torch.nn.BatchNorm2d, relu=False, res=None, fork=False, drop_scale=None):
+def bn_act(x, bn: torch.nn.BatchNorm2d, relu=False, res=None, drop_scale=None):
     """Fused BatchNorm2d (+ residual add) (+ ReLU) with the module's parameters / buffers / train-eval semantics.
-    fork=True returns two aliases of the output (see _two_grads); drop_scale: per-sample stochastic-depth scales [B] or None."""
-    return BNActFn.apply(x, bn.weight, bn.bias, res, bn, relu, fork, drop_scale)
+    drop_scale: per-sample stochastic-depth scales [B] or None."""
+    return BNActFn.apply(x, bn.weight, bn.bias, res, bn, relu, drop_scale)
 
 
 class GroupNorm9Fn(Function):
@@ -711,24 +690,16 @@ def _bn_eval_fold(bn, weight, bias):
 
 
 class TcConv1x1Fn(Function):
-    """y = act(BN(conv1x1([a1 ; a2]))) or conv1x1 + bias, on channels_last bf16 activations.
+    """y = act(BN(conv1x1([a1 ; a2]))) or a bias-free conv1x1 without BatchNorm or ReLU, on channels_last bf16 activations.
 
     a1 [B,K1,H,W], a2 [B,K2,H,W] or None (the concat-free embed.0 of models/cotnet.py:81,52), weight [N, K1+K2, 1, 1].
-    bn = nn.BatchNorm2d or None (then `cbias` is the conv bias or None)."""
+    bn = nn.BatchNorm2d or None.  cbias must be None: every convolution that runs here is bias-free (embed.3's bias is added
+    inside the GroupNorm kernels); the argument keeps the positional interface of the callers."""
 
     @staticmethod
     def forward(ctx, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res=None, drop_scale=None):
-        return TcConv1x1Fn._fwd(ctx, False, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res, drop_scale)
-
-    @staticmethod
-    def backward(ctx, *grads):
-        return TcConv1x1Fn._bwd(ctx, grads)
-
-    @staticmethod
-    def _fwd(ctx, fork, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res, drop_scale=None):
         assert _is_cl(a1) and a1.dtype == torch.bfloat16 and (a2 is None or (_is_cl(a2) and a2.dtype == a1.dtype))
-        if fork:
-            ctx.set_materialize_grads(False)
+        assert cbias is None and (bn is not None or not relu)
         assert res is None or (bn is not None and _is_cl(res) and res.dtype == a1.dtype)
         assert drop_scale is None or bn is not None
         B, K1, H, W = a1.shape
@@ -746,7 +717,7 @@ class TcConv1x1Fn(Function):
         batch = False
         rcode = 1 if relu else 0                 # ReLU mask of the backward: read from `out` unless the batch path below avoids it
         if bn is None:
-            _tc.gemm_bf16(a1, b1, a2, b2, shift=None if cbias is None else cbias.detach().float().contiguous(), relu=relu, out=out2d)
+            _tc.gemm_bf16(a1, b1, a2, b2, out=out2d)
         elif bn.training or bn.running_mean is None:
             batch = True
             sums = _zeros((2, N,), a1.device)
@@ -776,35 +747,27 @@ class TcConv1x1Fn(Function):
             _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(pre))
         ctx.save_for_backward(a1, a2, wb, pre, mask if rcode == 3 else (out if rcode == 1 else None), scale,
                               shift if rcode == 2 else None, mean, rstd, ds)
-        ctx.cfg = (relu, rcode, batch, bn is not None, cbias is not None, weight.dtype, weight.shape,
-                   None if bn_w is None else bn_w.dtype, None if cbias is None else cbias.dtype, K1, K2, res is not None)
-        if fork:
-            assert bn is not None, "fork needs the BatchNorm form (the sum of the two gradients happens in its backward kernels)"
-            return out, out.detach()
+        ctx.cfg = (rcode, batch, bn is not None, weight.dtype, weight.shape, None if bn_w is None else bn_w.dtype, K1, K2,
+                   res is not None)
         return out
 
     @staticmethod
-    def _bwd(ctx, grads):
+    def backward(ctx, dy):
         a1, a2, wb, pre, y, scale, shift, mean, rstd, ds = ctx.saved_tensors     # y: output (rcode 1), 1-bit mask (rcode 3) or None
-        relu, rcode, batch, has_bn, has_bias, wdt, wshape, bndt, cbdt, K1, K2, has_res = ctx.cfg
-        dy, dy2 = _two_grads(grads)
-        if dy is None:
-            return (None,) * 10
+        rcode, batch, has_bn, wdt, wshape, bndt, K1, K2, has_res = ctx.cfg
+        dy = dy.contiguous(memory_format=torch.channels_last)
         B, N, H, W = dy.shape
         M = B * H * W
         lib, st, dt = _lib.load(), _lib.stream_ptr(dy), _lib.BF16
-        dgamma = dbeta = dcb = dres = None
+        dgamma = dbeta = dres = None
+        dpre = dy
         if has_bn:
             sums = torch.zeros(2, N, dtype=torch.float32, device=dy.device)  # escapes as dgamma/dbeta
             if has_res and ctx.needs_input_grad[8]:
                 dres = torch.empty_like(dy, memory_format=torch.channels_last)
             dpre = torch.empty_like(dy, memory_format=torch.channels_last)
-            _bn_bwd(lib, dt, B, H * W, N, dy, dy2, pre, y, scale, shift, mean, rstd, rcode, sums, batch, 1.0 / M, dpre, dres, ds, st)
+            _bn_bwd(lib, dt, B, H * W, N, dy, pre, y, scale, shift, mean, rstd, rcode, sums, batch, 1.0 / M, dpre, dres, ds, st)
             dgamma, dbeta = sums[1].to(bndt), sums[0].to(bndt)
-        else:
-            dpre = dy if not relu else dy * (y > 0)
-            if has_bias:
-                dcb = _rows2d(dpre).float().sum(0).to(cbdt)
         d2 = _rows2d(dpre)
         da1 = da2 = None
         wt = wb.t().contiguous()                                  # [K1+K2, N]: B operand of the data-gradient GEMM
@@ -829,20 +792,7 @@ class TcConv1x1Fn(Function):
                 acc = _zeros((N, K1 + K2,), dy.device)
                 _tc.wgrad_bf16(dpre, a1, a2, out=acc)
                 dw = acc.reshape(wshape).to(wdt)
-        return da1, da2, dw, dcb, dgamma, dbeta, None, None, dres, None
-
-
-class TcConv1x1ForkFn(Function):
-    """TcConv1x1Fn whose output comes as TWO aliases (one per consumer); their gradients are summed inside the BatchNorm backward
-    kernels (_two_grads) instead of by an autograd add kernel."""
-
-    @staticmethod
-    def forward(ctx, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res=None, drop_scale=None):
-        return TcConv1x1Fn._fwd(ctx, True, a1, a2, weight, cbias, bn_w, bn_b, bn, relu, res, drop_scale)
-
-    @staticmethod
-    def backward(ctx, *grads):
-        return TcConv1x1Fn._bwd(ctx, grads)
+        return da1, da2, dw, None, dgamma, dbeta, None, None, dres, None
 
 
 class TcConv3x3Fn(Function):
@@ -886,15 +836,8 @@ class TcConv3x3Fn(Function):
         lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.BF16
         dy = dy.contiguous(memory_format=torch.channels_last)
         sums = torch.zeros(2, C, dtype=torch.float32, device=x.device)  # escapes as dgamma/dbeta
-        _lib.check(lib.cotb200_bn_bwd_sums(dt, B, H * W, C, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                           _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(),
-                                           sums[1].data_ptr(), st),
-                   "bn_bwd_sums")
         dpre = torch.empty_like(dy, memory_format=torch.channels_last)
-        _lib.check(lib.cotb200_bn_bwd_apply(dt, B, H * W, C, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                            _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
-                                            _lib.ptr(sums[1]) if batch else None, 1.0 / M, rcode,
-                                            dpre.data_ptr(), None, st), "bn_bwd_apply")
+        _bn_bwd(lib, dt, B, H * W, C, dy, pre, y, scale, shift, mean, rstd, rcode, sums, batch, 1.0 / M, dpre, None, None, st)
         dx = dw = None
         if ctx.needs_input_grad[0]:
             wpt, bnt = _tc.prepare_conv3x3_weight(weight, groups, transpose_for_dgrad=True)
@@ -951,14 +894,8 @@ class StemConvBNFn(Function):
         lib, st, dt = _lib.load(), _lib.stream_ptr(dy), _lib.BF16
         dy = dy.contiguous(memory_format=torch.channels_last)
         sums = torch.zeros(2, N, dtype=torch.float32, device=dy.device)  # escapes as dgamma/dbeta
-        _lib.check(lib.cotb200_bn_bwd_sums(dt, B, Ho * Wo, N, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                           _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), rcode, sums[0].data_ptr(),
-                                           sums[1].data_ptr(), st), "bn_bwd_sums")
         dpre = torch.empty_like(dy, memory_format=torch.channels_last)
-        _lib.check(lib.cotb200_bn_bwd_apply(dt, B, Ho * Wo, N, dy.data_ptr(), pre.data_ptr(), _lib.ptr(y), scale.data_ptr(),
-                                            _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
-                                            _lib.ptr(sums[1]) if batch else None, 1.0 / M, rcode,
-                                            dpre.data_ptr(), None, st), "bn_bwd_apply")
+        _bn_bwd(lib, dt, B, Ho * Wo, N, dy, pre, y, scale, shift, mean, rstd, rcode, sums, batch, 1.0 / M, dpre, None, None, st)
         dx = dw = None
         wq = weight.to(dpre.dtype)
         if ctx.needs_input_grad[0]:
@@ -986,34 +923,31 @@ def stem_conv_bn(x, conv, bn, relu=True):
     return bn_act(conv(x).contiguous(memory_format=torch.channels_last), bn, relu=relu)
 
 
-#: which 1x1 convolutions of the ENCLOSING bottleneck (conv1 / conv3 / stride-1 downsample) run on the wgmma kernels in
-#: training: "tc_all1x1" = all of them (forward with the BatchNorm statistics in the epilogue, data and weight gradients),
-#: anything else = cuDNN + the fused BatchNorm kernels.  Same environment variable as CotLayer.train_conv_backend.
-trunk_conv_backend = _os.environ.get("COTB200_TRAIN_CONV", "tc_all1x1+k").replace("+k", "")
+#: Training puts the CoT block's key_embed, embed.3 and conv1x1 and the enclosing bottleneck's 1x1 convolutions on the wgmma
+#: kernels only from this many pixels (B*H*W) up: on the 14x14 / 7x7 stages at bs256 the fixed per-launch costs of those
+#: kernels outweigh their byte savings.  The block's concat-free embed.0 GEMM runs there at every size.
+TC_MIN_PIXELS = 100000
 
+#: key_embed (grouped 3x3) runs on the haloed-tile wgmma convolution for dim <= this (stages 1-2)
+TC_KEY_MAX_DIM = 128
 
 #: the bottleneck convolutions of stages 3-4 (weights of 256K .. 1M elements, 12.5K-50K pixels) are compute-shaped
 #: (K = 1024 / 2048) and stay on cuDNN; the wgmma path takes the byte-heavy stages 1-2
-TC_TRUNK_MAX_WEIGHT = int(_os.environ.get("COTB200_TC_TRUNK_MAX_WEIGHT", str(128 * 1024)))
+TC_TRUNK_MAX_WEIGHT = 128 * 1024
 
 
-TC_MIN_PIXELS = int(_os.environ.get("COTB200_TC_MIN_PIXELS", "100000"))
-
-
-def conv1x1_bn(x, conv, bn, relu, res=None, fork=False, drop_scale=None):
+def conv1x1_bn(x, conv, bn, relu, res=None, drop_scale=None):
     """act(BN(conv1x1(x)) (+ res)) for the bottleneck's 1x1 convolutions (models/cotnet.py:229-235,249-262): on the wgmma
-    GEMMs when the backend says so and the geometry allows (bf16 channels_last, stride 1, dense, no bias), else cuDNN + the
-    fused BatchNorm kernels.  drop_scale: None or [B] stochastic-depth scales, act(drop_scale[b]*BN(conv1x1(x)) + res)
+    GEMMs when the geometry allows (bf16 channels_last, stride 1, dense, no bias, TC_TRUNK_MAX_WEIGHT, TC_MIN_PIXELS), else
+    cuDNN + the fused BatchNorm kernels.  drop_scale: None or [B] stochastic-depth scales, act(drop_scale[b]*BN(conv1x1(x)) + res)
     (models/cotnet.py:256-262)."""
     w = conv.weight
-    if (trunk_conv_backend == "tc_all1x1" and x.dtype == torch.bfloat16 and supported(x) and conv.kernel_size == (1, 1)
+    if (x.dtype == torch.bfloat16 and supported(x) and conv.kernel_size == (1, 1)
             and conv.stride == (1, 1) and conv.groups == 1 and conv.bias is None and w.shape[0] % 8 == 0 and w.shape[1] % 8 == 0
             and w.shape[0] * w.shape[1] <= TC_TRUNK_MAX_WEIGHT and x.shape[0] * x.shape[2] * x.shape[3] >= TC_MIN_PIXELS
             and (torch.is_grad_enabled() or not bn.training)):
-        if drop_scale is None:
-            return (TcConv1x1ForkFn if fork else TcConv1x1Fn).apply(x, None, w, None, bn.weight, bn.bias, bn, relu, res)
-        return (TcConv1x1ForkFn if fork else TcConv1x1Fn).apply(x, None, w, None, bn.weight, bn.bias, bn, relu, res, drop_scale)
-    return bn_act(conv(x).contiguous(memory_format=torch.channels_last), bn, relu=relu, res=res, fork=fork, drop_scale=drop_scale)
+        return TcConv1x1Fn.apply(x, None, w, None, bn.weight, bn.bias, bn, relu, res, drop_scale)
+    return bn_act(conv(x).contiguous(memory_format=torch.channels_last), bn, relu=relu, res=res, drop_scale=drop_scale)
 
 
 def tc_supported(x, dim):

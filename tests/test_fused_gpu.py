@@ -270,41 +270,3 @@ def test_cot_tail_eval_kernel_path(dtype, C, H, B):
     tol = 1e-4 if dtype == torch.float32 else 1.5e-2
     assert torch.allclose(got.float(), want, atol=tol, rtol=tol), (got.float() - want).abs().max().item()
     assert torch.allclose(got.float(), ref2.float(), atol=tol, rtol=tol)
-
-
-@pytest.mark.parametrize("dtype,tol", [(torch.float32, 1e-4), (torch.bfloat16, 2e-2)])
-@pytest.mark.parametrize("path", ["bn_act", "tc_conv1x1"])
-def test_forked_output_sums_the_two_gradients_in_the_bn_backward(dtype, tol, path, monkeypatch):
-    """fork=True: the output comes as two aliases; the gradients of their two consumers are summed inside the BatchNorm backward
-    kernels (cotb200_bn_bwd_{sums,apply}2) -- same parameter / input / residual gradients as the un-forked op behind an autograd add."""
-    import copy
-    from cotnet_b200 import fused
-    if path == "tc_conv1x1" and dtype != torch.bfloat16:
-        pytest.skip("the wgmma path is bf16 only")
-    g = torch.Generator(device="cuda").manual_seed(17)
-    B, K, N, H = 6, 64, 128, 14
-    x = torch.randn(B, K if path == "tc_conv1x1" else N, H, H, generator=g, device="cuda").to(dtype).contiguous(memory_format=torch.channels_last)
-    r = torch.randn(B, N, H, H, generator=g, device="cuda").to(dtype).contiguous(memory_format=torch.channels_last)
-    c1 = torch.randn(B, N, H, H, generator=g, device="cuda").to(dtype).contiguous(memory_format=torch.channels_last)
-    c2 = torch.randn(B, N, H, H, generator=g, device="cuda").to(dtype).contiguous(memory_format=torch.channels_last)
-    bn = torch.nn.BatchNorm2d(N).cuda().train()
-    conv = torch.nn.Conv2d(K, N, 1, bias=False).cuda().to(dtype)
-    if path == "tc_conv1x1":
-        monkeypatch.setattr(fused, "trunk_conv_backend", "tc_all1x1")
-        monkeypatch.setattr(fused, "TC_MIN_PIXELS", 0)
-    res = []
-    for fork in (False, True):
-        bn_, conv_ = copy.deepcopy(bn), copy.deepcopy(conv)
-        xx, rr = x.clone().requires_grad_(True), r.clone().requires_grad_(True)
-        if path == "bn_act":
-            out = fused.bn_act(xx, bn_, relu=True, res=rr, fork=fork)
-        else:
-            out = fused.conv1x1_bn(xx, conv_, bn_, relu=True, res=rr, fork=fork)
-        ya, yb = out if fork else (out, out)
-        assert (not fork) or (ya.data_ptr() == yb.data_ptr() and ya is not yb)
-        ((ya.float() * c1.float()).sum() + (yb.float() * c2.float()).sum()).backward()
-        res.append([xx.grad.float(), rr.grad.float(), bn_.weight.grad.float(), bn_.bias.grad.float()] +
-                   ([conv_.weight.grad.float()] if path != "bn_act" else []))
-    for a, b in zip(*res):
-        rel = ((a - b).norm() / b.norm().clamp_min(1e-6)).item()
-        assert rel <= tol, rel

@@ -340,9 +340,7 @@ def test_recipe_step_matches_reference_golden(monkeypatch):
     loss_plain.backward()
     errs_plain = _grad_errors({n: q.grad for n, q in mp_.named_parameters()}, g)
     del mp_
-    # (b) the bench path, every layer on the backend the bs256 bench takes (see test_bench_path_matches_reference_golden)
-    from cotnet_b200 import cot_layer as _cl
-    monkeypatch.setattr(_cl.CotLayer, "tc_min_pixels", 0)
+    # (b) the bench path, every layer on the path the bs256 bench takes in stages 1-2 (see test_bench_path_matches_reference_golden)
     monkeypatch.setattr(fused, "TC_MIN_PIXELS", 0)
     monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
     monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)

@@ -128,9 +128,6 @@ def main():
                 return run
             row["eager_train_fwdbwd_us"] = timeit(fb(lambda x: eager_forward(m, x)), xs, a.iters)
             row["fused_train_fwdbwd_us"] = timeit(fb(lambda x: m(x)), xs, a.iters)
-            m.train_conv_backend = "tc"
-            row["tc_train_fwdbwd_us"] = timeit(fb(lambda x: m(x)), xs, a.iters)
-            m.train_conv_backend = "cudnn"
         rows.append(row)
         print(json.dumps(row), flush=True)
         del xs, m

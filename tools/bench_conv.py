@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """conv1x1 -> BatchNorm(batch stats) -> ReLU, forward + backward, at every 1x1-conv shape of the CoTNet-50 bs256 step:
-cuDNN conv + fused BN kernels (the default training backend) against the wgmma GEMM with the statistics epilogue
-(TcConv1x1Fn).  Decides which convolutions the 'tc' training backend should take."""
+cuDNN conv + fused BN kernels against the wgmma GEMM with the statistics epilogue (TcConv1x1Fn).  In training, the
+geometry thresholds fused.TC_MIN_PIXELS and fused.TC_TRUNK_MAX_WEIGHT pick between the two per shape."""
 import argparse
 import json
 import os
