@@ -96,19 +96,10 @@ SYMBOLS = {
     "cotb200_tail_bwd_sums": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 7),
     "cotb200_tail_bwd_dz_sums": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_float] + [_VP] * 3),
     "cotb200_tail_bwd_apply": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 10 + [ctypes.c_float] * 2 + [_VP] * 3),
-    "cotb200_bn_apply": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 4 + [ctypes.c_int, _VP, _VP]),
-    "cotb200_bn_apply_batch": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_float] * 3 + [ctypes.c_int] * 2 + [_VP] * 6),
-    "cotb200_bn_bwd_sums": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 7 + [ctypes.c_int, _VP, _VP, _VP]),
-    "cotb200_bn_bwd_apply": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 9 + [ctypes.c_float, ctypes.c_int, _VP, _VP, _VP]),
-    "cotb200_bn_bwd_sums2": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_int, _VP, _VP, _VP]),
-    "cotb200_bn_bwd_apply2": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 10 + [ctypes.c_float, ctypes.c_int, _VP, _VP, _VP]),
-    "cotb200_bn_apply_ds": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 4 + [ctypes.c_int, _VP, _VP, _VP]),
-    "cotb200_bn_apply_batch_ds": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_float] * 3 + [ctypes.c_int] * 2 + [_VP] * 7),
-    "cotb200_bn_bwd_sums_ds": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_int, _VP, _VP, _VP, _VP]),
-    "cotb200_bn_bwd_apply_ds": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 10 + [ctypes.c_float, ctypes.c_int, _VP, _VP, _VP, _VP]),
-    "cotb200_bn_apply_batch_mask": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_float] * 3 + [ctypes.c_int] + [_VP] * 8),
-    "cotb200_bn_bwd_sums_mask": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 10),
-    "cotb200_bn_bwd_apply_mask": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 9 + [ctypes.c_float] + [_VP] * 4),
+    "cotb200_bn_apply": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 4 + [ctypes.c_int] + [_VP] * 3),
+    "cotb200_bn_apply_batch": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_float] * 3 + [ctypes.c_int] * 2 + [_VP] * 8),
+    "cotb200_bn_bwd_sums": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 8 + [ctypes.c_int] + [_VP] * 4),
+    "cotb200_bn_bwd_apply": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 10 + [ctypes.c_float, ctypes.c_int] + [_VP] * 4),
     "cotb200_bn_finalize": (ctypes.c_int, [ctypes.c_int] + [_VP] * 6 + [ctypes.c_float] * 3 + [ctypes.c_int] * 2 + [_VP] * 5),
     "cotb200_gn9_stats": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP] * 5),
     "cotb200_gn9_apply": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP] * 8),

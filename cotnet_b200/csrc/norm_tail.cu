@@ -380,7 +380,7 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
 // sum_dz[c] += dz ; sum_dzx[c] += dz * xhat.   DS: the BatchNorm output was scaled by ds[b], so its gradient is ds[b]*dz.
 template <typename T, int VEC, int ACT, bool DS = false>
 __global__ void __launch_bounds__(NT_THREADS)
-bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T* __restrict__ x, const T* __restrict__ y, const float* __restrict__ scale,
+bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ y, const float* __restrict__ scale,
                    const float* __restrict__ shift, const float* __restrict__ mu, const float* __restrict__ rstd,
                    float* __restrict__ sum_dz, float* __restrict__ sum_dzx, RowsGeo g, const float* __restrict__ ds, int ds_hw,
                    const unsigned char* __restrict__ mask, int mld) {
@@ -399,17 +399,15 @@ bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T*
     for (int r = r0 + ty; r < r1; r += g.ry) {
       const Pack<T, VEC> dv = ld_pack<T, VEC>(dy + base + (long long)r * g.ld);
       const Pack<T, VEC> xv = ld_pack<T, VEC>(x + base + (long long)r * g.ld);
-      Pack<T, VEC> yv, d2;
+      Pack<T, VEC> yv;
       unsigned mb = 0;
       if (ACT == 1) yv = ld_pack<T, VEC>(y + base + (long long)r * g.ld);
       if (ACT == 3) mb = load_mask_bits<VEC>(mask, (long long)r * mld, tx);
-      if (dy2) d2 = ld_pack<T, VEC>(dy2 + base + (long long)r * g.ld);    // two-consumer output: dy = dy + dy2, summed here in fp32
       float s = 1.f;
       if (DS) s = __ldg(ds + r / ds_hw);
 #pragma unroll
       for (int i = 0; i < VEC; ++i) {
         float dz = to_acc(dv.v[i]);
-        if (dy2) dz += to_acc(d2.v[i]);
         const float xf = to_acc(xv.v[i]);
         if (ACT == 1 && !(to_acc(yv.v[i]) > 0.f)) dz = 0.f;
         if (ACT == 3 && !((mb >> i) & 1u)) dz = 0.f;
@@ -428,7 +426,7 @@ bn_bwd_sums_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T*
 // DS: dx = scale * (ds[b]*dz - c1 - xhat*c2), dres = dz
 template <typename T, int VEC, int ACT, bool RES, bool DS = false>
 __global__ void __launch_bounds__(NT_THREADS)
-bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T* __restrict__ x, const T* __restrict__ y, const float* __restrict__ scale,
+bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ y, const float* __restrict__ scale,
                     const float* __restrict__ shift, const float* __restrict__ mu, const float* __restrict__ rstd,
                     const float* __restrict__ c1, const float* __restrict__ c2, float inv_n, T* __restrict__ dx,
                     T* __restrict__ dres, RowsGeo g, const float* __restrict__ ds, int ds_hw,
@@ -447,18 +445,16 @@ bn_bwd_apply_kernel(const T* __restrict__ dy, const T* __restrict__ dy2, const T
   for (int r = r0 + ty; r < r1; r += g.ry) {
     const Pack<T, VEC> dv = ld_pack<T, VEC>(dy + base + (long long)r * g.ld);
     const Pack<T, VEC> xv = ld_pack<T, VEC>(x + base + (long long)r * g.ld);
-    Pack<T, VEC> yv, d2;
+    Pack<T, VEC> yv;
     unsigned mb = 0;
     if (ACT == 1) yv = ld_pack<T, VEC>(y + base + (long long)r * g.ld);
     if (ACT == 3) mb = load_mask_bits<VEC>(mask, (long long)r * mld, tx);
-    if (dy2) d2 = ld_pack<T, VEC>(dy2 + base + (long long)r * g.ld);
     Pack<T, VEC> o, o2;
     float s = 1.f;
     if (DS) s = __ldg(ds + r / ds_hw);
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
       float dz = to_acc(dv.v[i]);
-      if (dy2) dz += to_acc(d2.v[i]);
       const float xf = to_acc(xv.v[i]);
       if (ACT == 1 && !(to_acc(yv.v[i]) > 0.f)) dz = 0.f;
       if (ACT == 3 && !((mb >> i) & 1u)) dz = 0.f;
@@ -1015,9 +1011,9 @@ static bool mask_geo_ok(int C, int vec) {
   const int cw = col_chunk(C, vec);
   return C % 8 == 0 && cw && cw % 8 == 0;
 }
-static int bn_apply_impl(const char* what, int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
-                         const float* shift, int relu, void* y, const BnFin* fin, const float* sscale, void* stream,
-                         unsigned char* mask = nullptr) {
+static int bn_apply_impl(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale, const float* shift,
+                         int relu, void* y, const BnFin* fin, const float* sscale, unsigned char* mask, void* stream) {
+  const char* what = fin ? "bn_apply_batch" : "bn_apply";
   if (dtype == COTB200_F64) { set_error("%s: fp64 not supported", what); return COTB200_EDTYPE; }
   const int ds_hw = HW;           // rows per sample: the sample of flattened row r is r / ds_hw
   const int mld = C / 8;          // mask row pitch (bytes)
@@ -1045,7 +1041,7 @@ static int bn_apply_impl(const char* what, int dtype, int B, int HW, int C, cons
           f.scale += c0; f.shift += c0; f.mean += c0; f.rstd += c0;
         }
         const float* scp = scale ? scale + c0 : nullptr; const float* shp = shift ? shift + c0 : nullptr;
-        COTB200_PROF_B(fin ? "bn_apply_batch" : "bn_apply", (double)B * HW * (cw * (2 + (res ? 1 : 0)) * sizeof(T) + (mask ? cw / 8 : 0)));
+        COTB200_PROF_B(what, (double)B * HW * (cw * (2 + (res ? 1 : 0)) * sizeof(T) + (mask ? cw / 8 : 0)));
         NT_DISPATCH_VEC(vec, {
           if (mask) {
             BN_APPLY_MASK_LAUNCH();
@@ -1066,59 +1062,34 @@ static int bn_apply_impl(const char* what, int dtype, int B, int HW, int C, cons
 }
 
 extern "C" int cotb200_bn_apply(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
-                                const float* shift, int relu, void* y, void* stream) {
+                                const float* shift, int relu, void* y, const float* sample_scale, void* stream) {
   if (!x || !scale || !shift || !y) { set_error("bn_apply: NULL pointer"); return COTB200_ENULL; }
-  return bn_apply_impl("bn_apply", dtype, B, HW, C, x, res, scale, shift, relu, y, nullptr, nullptr, stream);
-}
-
-extern "C" int cotb200_bn_apply_ds(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
-                                   const float* shift, int relu, void* y, const float* sample_scale, void* stream) {
-  if (!x || !scale || !shift || !y) { set_error("bn_apply_ds: NULL pointer"); return COTB200_ENULL; }
-  return bn_apply_impl("bn_apply_ds", dtype, B, HW, C, x, res, scale, shift, relu, y, nullptr, sample_scale, stream);
+  return bn_apply_impl(dtype, B, HW, C, x, res, scale, shift, relu, y, nullptr, sample_scale, nullptr, stream);
 }
 
 extern "C" int cotb200_bn_apply_batch(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum,
                                       const float* sq, const float* weight, const float* bias, float* running_mean,
                                       float* running_var, float n, float eps, float momentum, int update_running, int relu,
-                                      void* y, float* scale, float* shift, float* mean, float* rstd, void* stream) {
-  if (!x || !y || !sum || !sq || !scale || !shift || !mean || !rstd) { set_error("bn_apply_batch: NULL pointer"); return COTB200_ENULL; }
+                                      void* y, float* scale, float* shift, float* mean, float* rstd, const float* sample_scale,
+                                      unsigned char* mask, void* stream) {
+  if (!x || !y || !sum || !sq || !scale || !shift || !mean || !rstd || (mask && !res)) {
+    set_error("bn_apply_batch: NULL pointer"); return COTB200_ENULL; }
   if (update_running && (!running_mean || !running_var)) { set_error("bn_apply_batch: running buffers missing"); return COTB200_ENULL; }
+  if (mask && relu != 1) { set_error("bn_apply_batch: the 1-bit mask needs relu == 1"); return COTB200_EINVAL; }
   BnFin f{sum, sq, weight, bias, running_mean, running_var, n, eps, momentum, update_running, scale, shift, mean, rstd};
-  return bn_apply_impl("bn_apply_batch", dtype, B, HW, C, x, res, nullptr, nullptr, relu, y, &f, nullptr, stream);
-}
-
-extern "C" int cotb200_bn_apply_batch_ds(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum,
-                                         const float* sq, const float* weight, const float* bias, float* running_mean,
-                                         float* running_var, float n, float eps, float momentum, int update_running, int relu,
-                                         void* y, float* scale, float* shift, float* mean, float* rstd, const float* sample_scale,
-                                         void* stream) {
-  if (!x || !y || !sum || !sq || !scale || !shift || !mean || !rstd) { set_error("bn_apply_batch_ds: NULL pointer"); return COTB200_ENULL; }
-  if (update_running && (!running_mean || !running_var)) { set_error("bn_apply_batch_ds: running buffers missing"); return COTB200_ENULL; }
-  BnFin f{sum, sq, weight, bias, running_mean, running_var, n, eps, momentum, update_running, scale, shift, mean, rstd};
-  return bn_apply_impl("bn_apply_batch_ds", dtype, B, HW, C, x, res, nullptr, nullptr, relu, y, &f, sample_scale, stream);
-}
-
-extern "C" int cotb200_bn_apply_batch_mask(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum,
-                                           const float* sq, const float* weight, const float* bias, float* running_mean,
-                                           float* running_var, float n, float eps, float momentum, int update_running, void* y,
-                                           float* scale, float* shift, float* mean, float* rstd, const float* sample_scale,
-                                           unsigned char* mask, void* stream) {
-  if (!x || !res || !y || !mask || !sum || !sq || !scale || !shift || !mean || !rstd) {
-    set_error("bn_apply_batch_mask: NULL pointer"); return COTB200_ENULL; }
-  if (update_running && (!running_mean || !running_var)) { set_error("bn_apply_batch_mask: running buffers missing"); return COTB200_ENULL; }
-  BnFin f{sum, sq, weight, bias, running_mean, running_var, n, eps, momentum, update_running, scale, shift, mean, rstd};
-  return bn_apply_impl("bn_apply_batch_mask", dtype, B, HW, C, x, res, nullptr, nullptr, 1, y, &f, sample_scale, stream, mask);
+  return bn_apply_impl(dtype, B, HW, C, x, res, nullptr, nullptr, relu, y, &f, sample_scale, mask, stream);
 }
 
 #define BN_BWD_SUMS_LAUNCH(ACT, DS, YP)                                                                               \
   do { if ((rc = ensure_smem(bn_bwd_sums_kernel<T, V, ACT, DS>, smem))) return rc;                                    \
-       bn_bwd_sums_kernel<T, V, ACT, DS><<<NT_GRID, NT_THREADS, smem, st>>>(dp, d2p, xp, YP, scp, shp, mu + c0, rstd + c0,  \
-                                                                             sum_dz + c0, sum_dzx + c0, g, sscale, ds_hw, mp, mld); } while (0)
-// relu code 3 (the 1-bit mask of cotb200_bn_apply_batch_mask) is reached through the _mask entry points only
-static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                            const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
-                            float* sum_dz, float* sum_dzx, const float* sscale, void* stream, const unsigned char* mask = nullptr) {
-  if (relu < 0 || relu > (mask ? 3 : 2)) { set_error("bn_bwd_sums: relu must be 0, 1 or 2"); return COTB200_EINVAL; }
+       bn_bwd_sums_kernel<T, V, ACT, DS><<<NT_GRID, NT_THREADS, smem, st>>>(dp, xp, YP, scp, shp, mu + c0, rstd + c0,       \
+                                                                             sum_dz + c0, sum_dzx + c0, g, sample_scale, ds_hw, mp, mld); } while (0)
+extern "C" int cotb200_bn_bwd_sums(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y,
+                                   const unsigned char* mask, const float* scale, const float* shift, const float* mu,
+                                   const float* rstd, int relu, float* sum_dz, float* sum_dzx, const float* sample_scale,
+                                   void* stream) {
+  if (relu < 0 || relu > 3 || (mask && relu != 3)) {
+    set_error("bn_bwd_sums: relu must be 0, 1, 2 or 3, and 3 when a mask is given"); return COTB200_EINVAL; }
   if (!dy || !x || !mu || !rstd || !sum_dz || !sum_dzx || (relu == 1 && !y) || (relu == 2 && (!scale || !shift)) || (relu == 3 && !mask)) {
     set_error("bn_bwd_sums: NULL pointer"); return COTB200_ENULL; }
   const int mld = C / 8;          // mask row pitch (bytes)
@@ -1129,7 +1100,7 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
   cudaStream_t st = (cudaStream_t)stream;
   COTB200_DISPATCH_DTYPE(dtype, {
     if constexpr (!std::is_same<T, double>::value) {
-      const int vec = pick_vec<T>(C, dy, x, relu == 1 ? y : nullptr, dy2);
+      const int vec = pick_vec<T>(C, dy, x, relu == 1 ? y : nullptr);
       const int cw = col_chunk(C, vec);
       if (!cw) { set_error("bn_bwd_sums: cannot tile %d channels", C); return COTB200_EINVAL; }
       if (relu == 3 && !mask_geo_ok(C, vec)) { set_error("bn_bwd_sums: the 1-bit mask needs C %% 8 == 0 (C = %d)", C); return COTB200_EINVAL; }
@@ -1141,12 +1112,11 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
         if ((rc = det_geo(ds, g, 2, st))) return rc;
         g.ld = C;
         const T* dp = (const T*)dy + c0; const T* xp = (const T*)x + c0; const T* yp = y ? (const T*)y + c0 : nullptr;
-        const T* d2p = dy2 ? (const T*)dy2 + c0 : nullptr;
         const unsigned char* mp = relu == 3 ? mask + c0 / 8 : nullptr;
-        COTB200_PROF_B("bn_bwd_sums", (double)B * HW * (cw * (2 + (relu == 1 ? 1 : 0) + (dy2 ? 1 : 0)) * sizeof(T) + (relu == 3 ? cw / 8 : 0)));
+        COTB200_PROF_B("bn_bwd_sums", (double)B * HW * (cw * (2 + (relu == 1 ? 1 : 0)) * sizeof(T) + (relu == 3 ? cw / 8 : 0)));
         const float* scp = scale ? scale + c0 : nullptr; const float* shp = shift ? shift + c0 : nullptr;
         NT_DISPATCH_VEC(vec, {
-          if (sscale) {
+          if (sample_scale) {
             if (relu == 1) BN_BWD_SUMS_LAUNCH(1, true, yp); else if (relu == 2) BN_BWD_SUMS_LAUNCH(2, true, nullptr);
             else if (relu == 3) BN_BWD_SUMS_LAUNCH(3, true, nullptr); else BN_BWD_SUMS_LAUNCH(0, true, nullptr);
           } else {
@@ -1163,15 +1133,16 @@ static int bn_bwd_sums_impl(int dtype, int B, int HW, int C, const void* dy, con
 }
 
 #define BN_BWD_APPLY_LAUNCH(ACT, RES, YP, DRP)                                                                         \
-  do { if (sscale) bn_bwd_apply_kernel<T, V, ACT, RES, true><<<NT_GRID, NT_THREADS, 0, st>>>(dp, d2p, xp, YP, scale + c0, shp, mu + c0, \
-                                                               rstd + c0, k1, k2, inv_n, dxp, DRP, g, sscale, ds_hw, mp, mld); \
-       else bn_bwd_apply_kernel<T, V, ACT, RES><<<NT_GRID, NT_THREADS, 0, st>>>(dp, d2p, xp, YP, scale + c0, shp, mu + c0,  \
+  do { if (sample_scale) bn_bwd_apply_kernel<T, V, ACT, RES, true><<<NT_GRID, NT_THREADS, 0, st>>>(dp, xp, YP, scale + c0, shp, mu + c0, \
+                                                               rstd + c0, k1, k2, inv_n, dxp, DRP, g, sample_scale, ds_hw, mp, mld); \
+       else bn_bwd_apply_kernel<T, V, ACT, RES><<<NT_GRID, NT_THREADS, 0, st>>>(dp, xp, YP, scale + c0, shp, mu + c0,  \
                                                                rstd + c0, k1, k2, inv_n, dxp, DRP, g, nullptr, 1, mp, mld); } while (0)
-static int bn_bwd_apply_impl(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                             const float* scale, const float* shift, const float* mu, const float* rstd,
-                             const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres, const float* sscale,
-                             void* stream, const unsigned char* mask = nullptr) {
-  if (relu < 0 || relu > (mask ? 3 : 2)) { set_error("bn_bwd_apply: relu must be 0, 1 or 2"); return COTB200_EINVAL; }
+extern "C" int cotb200_bn_bwd_apply(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y,
+                                    const unsigned char* mask, const float* scale, const float* shift, const float* mu,
+                                    const float* rstd, const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres,
+                                    const float* sample_scale, void* stream) {
+  if (relu < 0 || relu > 3 || (mask && relu != 3)) {
+    set_error("bn_bwd_apply: relu must be 0, 1, 2 or 3, and 3 when a mask is given"); return COTB200_EINVAL; }
   if (!dy || !x || !scale || !mu || !rstd || !dx || (relu == 1 && !y) || (relu == 2 && !shift) || (relu == 3 && !mask)) {
     set_error("bn_bwd_apply: NULL pointer"); return COTB200_ENULL; }
   const int mld = C / 8;          // mask row pitch (bytes)
@@ -1184,7 +1155,6 @@ static int bn_bwd_apply_impl(int dtype, int B, int HW, int C, const void* dy, co
     if constexpr (!std::is_same<T, double>::value) {
       int vec = pick_vec<T>(C, dy, x, relu == 1 ? y : nullptr, dx);
       if (dres && ((uintptr_t)dres & (vec * sizeof(T) - 1))) vec = 1;
-      if (dy2 && ((uintptr_t)dy2 & (vec * sizeof(T) - 1))) vec = 1;
       const int cw = col_chunk(C, vec);
       if (!cw) { set_error("bn_bwd_apply: cannot tile %d channels", C); return COTB200_EINVAL; }
       if (relu == 3 && !mask_geo_ok(C, vec)) { set_error("bn_bwd_apply: the 1-bit mask needs C %% 8 == 0 (C = %d)", C); return COTB200_EINVAL; }
@@ -1195,10 +1165,9 @@ static int bn_bwd_apply_impl(int dtype, int B, int HW, int C, const void* dy, co
         g.ld = C;
         const T* dp = (const T*)dy + c0; const T* xp = (const T*)x + c0; const T* yp = y ? (const T*)y + c0 : nullptr;
         T* dxp = (T*)dx + c0; T* drp = dres ? (T*)dres + c0 : nullptr;
-        const T* d2p = dy2 ? (const T*)dy2 + c0 : nullptr;
         const float* k1 = c1 ? c1 + c0 : nullptr; const float* k2 = c2 ? c2 + c0 : nullptr;
         const unsigned char* mp = relu == 3 ? mask + c0 / 8 : nullptr;
-        COTB200_PROF_B("bn_bwd_apply", (double)B * HW * (cw * (3 + (relu == 1 ? 1 : 0) + (dres ? 1 : 0) + (dy2 ? 1 : 0)) * sizeof(T)
+        COTB200_PROF_B("bn_bwd_apply", (double)B * HW * (cw * (3 + (relu == 1 ? 1 : 0) + (dres ? 1 : 0)) * sizeof(T)
                                                          + (relu == 3 ? cw / 8 : 0)));
         const float* shp = shift ? shift + c0 : nullptr;
         NT_DISPATCH_VEC(vec, {
@@ -1227,54 +1196,4 @@ extern "C" int cotb200_bn_finalize(int C, const float* sum, const float* sq, con
   bn_finalize_kernel<<<(C + 127) / 128, 128, 0, st>>>(sum, sq, weight, bias, running_mean, running_var, n, eps, momentum, use_batch,
                                                      update_running, scale, shift, mean, rstd, C);
   return check_launch("bn_finalize");
-}
-
-
-// ---- public entry points of the BatchNorm backward: one incoming gradient, or two that are summed on the fly (fp32)
-extern "C" int cotb200_bn_bwd_sums(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y,
-                                   const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
-                                   float* sum_dz, float* sum_dzx, void* stream) {
-  return bn_bwd_sums_impl(dtype, B, HW, C, dy, nullptr, x, y, scale, shift, mu, rstd, relu, sum_dz, sum_dzx, nullptr, stream);
-}
-extern "C" int cotb200_bn_bwd_sums2(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                                    const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
-                                    float* sum_dz, float* sum_dzx, void* stream) {
-  return bn_bwd_sums_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, relu, sum_dz, sum_dzx, nullptr, stream);
-}
-extern "C" int cotb200_bn_bwd_sums_ds(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                                      const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
-                                      float* sum_dz, float* sum_dzx, const float* sample_scale, void* stream) {
-  return bn_bwd_sums_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, relu, sum_dz, sum_dzx, sample_scale, stream);
-}
-extern "C" int cotb200_bn_bwd_apply(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y,
-                                    const float* scale, const float* shift, const float* mu, const float* rstd,
-                                    const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres, void* stream) {
-  return bn_bwd_apply_impl(dtype, B, HW, C, dy, nullptr, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, nullptr, stream);
-}
-extern "C" int cotb200_bn_bwd_apply2(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                                     const float* scale, const float* shift, const float* mu, const float* rstd,
-                                     const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres, void* stream) {
-  return bn_bwd_apply_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, nullptr, stream);
-}
-extern "C" int cotb200_bn_bwd_apply_ds(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                                       const float* scale, const float* shift, const float* mu, const float* rstd,
-                                       const float* c1, const float* c2, float inv_n, int relu, void* dx, void* dres,
-                                       const float* sample_scale, void* stream) {
-  return bn_bwd_apply_impl(dtype, B, HW, C, dy, dy2, x, y, scale, shift, mu, rstd, c1, c2, inv_n, relu, dx, dres, sample_scale, stream);
-}
-// ---- 1-bit ReLU mask (relu code 3): the mask cotb200_bn_apply_batch_mask wrote replaces y
-extern "C" int cotb200_bn_bwd_sums_mask(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x,
-                                        const unsigned char* mask, const float* mu, const float* rstd, float* sum_dz, float* sum_dzx,
-                                        const float* sample_scale, void* stream) {
-  if (!mask) { set_error("bn_bwd_sums_mask: NULL pointer"); return COTB200_ENULL; }
-  return bn_bwd_sums_impl(dtype, B, HW, C, dy, dy2, x, nullptr, nullptr, nullptr, mu, rstd, 3, sum_dz, sum_dzx, sample_scale, stream,
-                          mask);
-}
-extern "C" int cotb200_bn_bwd_apply_mask(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x,
-                                         const unsigned char* mask, const float* scale, const float* mu, const float* rstd,
-                                         const float* c1, const float* c2, float inv_n, void* dx, void* dres, const float* sample_scale,
-                                         void* stream) {
-  if (!mask) { set_error("bn_bwd_apply_mask: NULL pointer"); return COTB200_ENULL; }
-  return bn_bwd_apply_impl(dtype, B, HW, C, dy, dy2, x, nullptr, scale, nullptr, mu, rstd, c1, c2, inv_n, 3, dx, dres, sample_scale,
-                           stream, mask);
 }

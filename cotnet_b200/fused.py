@@ -186,17 +186,11 @@ def _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds=Non
     update, mom, rm, rv = _bn_running(bn, True)
     w32 = None if weight is None else weight.detach().float().contiguous()
     b32 = None if bias is None else bias.detach().float().contiguous()
-    args = (dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), sums[0].data_ptr(), sums[1].data_ptr(), _lib.ptr(w32), _lib.ptr(b32),
-            _lib.ptr(rm), _lib.ptr(rv), float(B * H * W), float(bn.eps), float(mom), 1 if update else 0, 1 if relu else 0,
-            y.data_ptr(), ss[0].data_ptr(), ss[1].data_ptr(), ss[2].data_ptr(), ss[3].data_ptr())
-    if mask is not None:
-        assert relu and res is not None
-        margs = args[:16] + args[17:]          # the mask form has no relu argument: it is always ReLU
-        _lib.check(lib.cotb200_bn_apply_batch_mask(*margs, _lib.ptr(ds), mask.data_ptr(), st), "bn_apply_batch_mask")
-    elif ds is None:
-        _lib.check(lib.cotb200_bn_apply_batch(*args, st), "bn_apply_batch")
-    else:
-        _lib.check(lib.cotb200_bn_apply_batch_ds(*args, ds.data_ptr(), st), "bn_apply_batch_ds")
+    _lib.check(lib.cotb200_bn_apply_batch(dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), sums[0].data_ptr(), sums[1].data_ptr(),
+                                          _lib.ptr(w32), _lib.ptr(b32), _lib.ptr(rm), _lib.ptr(rv), float(B * H * W), float(bn.eps),
+                                          float(mom), 1 if update else 0, 1 if relu else 0, y.data_ptr(), ss[0].data_ptr(),
+                                          ss[1].data_ptr(), ss[2].data_ptr(), ss[3].data_ptr(), _lib.ptr(ds), _lib.ptr(mask), st),
+               "bn_apply_batch")
     _bn_running_writeback(bn, update, rm, rv)
     return ss
 
@@ -211,31 +205,14 @@ def _drop_scale(ds, x):
 
 
 def _bn_bwd(lib, dt, B, HW, C, dy, x, y, scale, shift, mean, rstd, rcode, sums, batch, inv_n, dx, dres, ds, st):
-    """BatchNorm backward (sums + apply) of the plain form, or of the drop-path form when ds is given.
-    rcode 3: `y` is the 1-bit ReLU mask of _bn_apply_batch(mask=...)."""
-    if rcode == 3:
-        if sums is not None:
-            _lib.check(lib.cotb200_bn_bwd_sums_mask(dt, B, HW, C, dy.data_ptr(), None, x.data_ptr(), y.data_ptr(),
-                                                    mean.data_ptr(), rstd.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(),
-                                                    _lib.ptr(ds), st), "bn_bwd_sums_mask")
-        _lib.check(lib.cotb200_bn_bwd_apply_mask(dt, B, HW, C, dy.data_ptr(), None, x.data_ptr(), y.data_ptr(), scale.data_ptr(),
-                                                 mean.data_ptr(), rstd.data_ptr(), _lib.ptr(sums[0]) if batch else None,
-                                                 _lib.ptr(sums[1]) if batch else None, inv_n, dx.data_ptr(), _lib.ptr(dres), _lib.ptr(ds),
-                                                 st), "bn_bwd_apply_mask")
-        return
+    """BatchNorm backward (sums + apply); ds: None or the drop-path scales of the forward.
+    `y` is the forward output for rcode 1 and its 1-bit ReLU mask (from _bn_apply_batch(mask=...)) for rcode 3."""
+    yp, mp = _lib.ptr(y) if rcode == 1 else None, _lib.ptr(y) if rcode == 3 else None
+    head = (dt, B, HW, C, dy.data_ptr(), x.data_ptr(), yp, mp, _lib.ptr(scale), _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr())
     if sums is not None:
-        rest = (x.data_ptr(), _lib.ptr(y), _lib.ptr(scale), _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(), rcode,
-                sums[0].data_ptr(), sums[1].data_ptr())
-        if ds is None:
-            _lib.check(lib.cotb200_bn_bwd_sums(dt, B, HW, C, dy.data_ptr(), *rest, st), "bn_bwd_sums")
-        else:
-            _lib.check(lib.cotb200_bn_bwd_sums_ds(dt, B, HW, C, dy.data_ptr(), None, *rest, ds.data_ptr(), st), "bn_bwd_sums_ds")
-    rest = (x.data_ptr(), _lib.ptr(y), scale.data_ptr(), _lib.ptr(shift), mean.data_ptr(), rstd.data_ptr(),
-            _lib.ptr(sums[0]) if batch else None, _lib.ptr(sums[1]) if batch else None, inv_n, rcode, dx.data_ptr(), _lib.ptr(dres))
-    if ds is None:
-        _lib.check(lib.cotb200_bn_bwd_apply(dt, B, HW, C, dy.data_ptr(), *rest, st), "bn_bwd_apply")
-    else:
-        _lib.check(lib.cotb200_bn_bwd_apply_ds(dt, B, HW, C, dy.data_ptr(), None, *rest, ds.data_ptr(), st), "bn_bwd_apply_ds")
+        _lib.check(lib.cotb200_bn_bwd_sums(*head, rcode, sums[0].data_ptr(), sums[1].data_ptr(), _lib.ptr(ds), st), "bn_bwd_sums")
+    _lib.check(lib.cotb200_bn_bwd_apply(*head, _lib.ptr(sums[0]) if batch else None, _lib.ptr(sums[1]) if batch else None, inv_n,
+                                        rcode, dx.data_ptr(), _lib.ptr(dres), _lib.ptr(ds), st), "bn_bwd_apply")
 
 
 class BNActFn(Function):
@@ -262,11 +239,8 @@ class BNActFn(Function):
             ss = _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds, mask)   # [4,C]: scale, shift, mean, rstd
         else:
             ss = _bn_prepare(bn, weight, bias, C, float(B * H * W), None, x.device, st)
-            args = (dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), ss[0].data_ptr(), ss[1].data_ptr(), 1 if relu else 0, y.data_ptr())
-            if ds is None:
-                _lib.check(lib.cotb200_bn_apply(*args, st), "bn_apply")
-            else:
-                _lib.check(lib.cotb200_bn_apply_ds(*args, ds.data_ptr(), st), "bn_apply_ds")
+            _lib.check(lib.cotb200_bn_apply(dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), ss[0].data_ptr(), ss[1].data_ptr(),
+                                            1 if relu else 0, y.data_ptr(), _lib.ptr(ds), st), "bn_apply")
         # ReLU mask in the backward: with a residual it comes from the 1-bit mask the forward wrote (relu code 3) or from y;
         # without one it is recomputed from x and the forward's own scale/shift (relu code 2) and y is neither saved nor read
         rcode = 0 if not relu else (2 if res is None else (3 if mask is not None else 1))
@@ -677,12 +651,6 @@ def _rows2d(t):
     return t.permute(0, 2, 3, 1).reshape(B * H * W, C)
 
 
-def _bn_from_sums(sums, n, bn, weight, bias):
-    """(scale, shift, mean, rstd) from epilogue column sums; updates the running buffers like nn.BatchNorm2d."""
-    ss = _bn_prepare(bn, weight, bias, sums.shape[1], n, sums, sums.device, torch.cuda.current_stream(sums.device).cuda_stream)
-    return ss[0], ss[1], ss[2], ss[3]
-
-
 def _bn_eval_fold(bn, weight, bias):
     ss = _bn_prepare(bn, weight, bias, weight.shape[0], 1.0, None, weight.device,
                      torch.cuda.current_stream(weight.device).cuda_stream)
@@ -735,12 +703,8 @@ class TcConv1x1Fn(Function):
             else:       # eval mode with a residual: raw GEMM, then the fused scale/shift + residual + ReLU kernel
                 pre = torch.empty_like(out, memory_format=torch.channels_last)
                 _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(pre))
-                args = (dt, B, H * W, N, pre.data_ptr(), _lib.ptr(res), scale.data_ptr(), shift.data_ptr(), 1 if relu else 0,
-                        out.data_ptr())
-                if ds is None:
-                    _lib.check(lib.cotb200_bn_apply(*args, st), "bn_apply")
-                else:
-                    _lib.check(lib.cotb200_bn_apply_ds(*args, ds.data_ptr(), st), "bn_apply_ds")
+                _lib.check(lib.cotb200_bn_apply(dt, B, H * W, N, pre.data_ptr(), _lib.ptr(res), scale.data_ptr(), shift.data_ptr(),
+                                                1 if relu else 0, out.data_ptr(), _lib.ptr(ds), st), "bn_apply")
         need_bwd = any(ctx.needs_input_grad)
         if need_bwd and bn is not None and pre is None:      # eval-mode module under grad: BN backward needs the raw conv output
             pre = torch.empty_like(out, memory_format=torch.channels_last)

@@ -166,72 +166,42 @@ int cotb200_se_eval(int B, int C, int A, const float* psum, float inv_hw, const 
                     void* stream);
 /* BatchNorm2d (+ReLU) (+residual add) on NHWC tensors: y = act(x*scale + shift (+ res)).  With cotb200_col_stats this
  * replaces nn.BatchNorm2d / nn.ReLU pairs of the block (models/cotnet.py:45-46,53-54,61-62) and of the enclosing
- * bottleneck (models/cotnet.py:231-235,:249-262) in 2 forward + 2 backward HBM passes.  relu: 0/1; res may be NULL. */
-int cotb200_bn_apply(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
-                     const float* shift, int relu, void* y, void* stream);
-/* Training-mode variant: the bookkeeping of cotb200_bn_finalize folded into the apply kernel's prologue (one launch less per
- * BatchNorm): scale/shift are derived from the batch sums of cotb200_col_stats (n rows), scale/shift/mean/rstd [C] are
- * written for the backward, the running statistics updated when update_running (momentum, unbiased variance). */
+ * bottleneck (models/cotnet.py:231-235,:249-262) in 2 forward + 2 backward HBM passes.  relu: 0/1; res may be NULL.
+ * sample_scale: NULL, or stochastic depth (DropPath after bn3, models/cotnet.py:256-257) in the same kernel: device fp32 [B]
+ * = s_b, 0 for a dropped sample and 1/keep for a kept one, and y = act(s_b*(x*scale + shift) (+ res)).  NULL runs the plain
+ * kernel, bit for bit the result of s_b = 1.  The kernels see flattened rows; the sample of row r is r / HW. */
+int cotb200_bn_apply(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale, const float* shift,
+                     int relu, void* y, const float* sample_scale, void* stream);
+/* Training-mode apply: the bookkeeping of cotb200_bn_finalize folded into the apply kernel's prologue (one launch less per
+ * BatchNorm): scale/shift are derived from the batch sums of cotb200_col_stats (n rows, every sample, dropped or not),
+ * scale/shift/mean/rstd [C] are written for the backward, the running statistics updated when update_running (momentum,
+ * unbiased variance).  relu, res and sample_scale as in cotb200_bn_apply.
+ * mask: NULL, or [B*HW, C/8] bytes that receive the 1-bit ReLU mask of y for relu code 3 of the backward: bit c%8 of byte c/8
+ * of a row = [y > 0] of the STORED y, so it equals relu code 1's mask bit for bit.  With a residual the mask cannot be
+ * recomputed from x (code 2), and reading y back costs two full passes of the widest tensors of the bottleneck.  A mask
+ * needs relu == 1 (else COTB200_EINVAL), res (else COTB200_ENULL) and C % 8 == 0. */
 int cotb200_bn_apply_batch(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum, const float* sq,
-                           const float* weight, const float* bias, float* running_mean, float* running_var, float n,
-                           float eps, float momentum, int update_running, int relu, void* y, float* scale, float* shift,
-                           float* mean, float* rstd, void* stream);
-/* dz = dy*mask ; sum_dz[c] += sum dz ; sum_dzx[c] += sum dz*xhat.
- * relu: 0 = no activation; 1 = ReLU, mask = [y > 0] read from the forward output y; 2 = ReLU, mask recomputed as
- * [x*scale + shift > 0] from the forward's own fp32 scale/shift (identical mask, y is NOT read: one HBM pass less; only for
- * BatchNorms without a residual input).  y may be NULL unless relu == 1; scale/shift may be NULL unless relu == 2. */
-int cotb200_bn_bwd_sums(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y, const float* scale,
-                        const float* shift, const float* mu, const float* rstd, int relu, float* sum_dz, float* sum_dzx,
-                        void* stream);
-/* Two-consumer form: the BatchNorm output fed TWO consumers (the next block's conv1 and its shortcut, models/cotnet.py:228-262) and
- * autograd would first add their gradients (one more kernel, three HBM passes); here dy := dy + dy2 is formed in fp32 inside the
- * backward kernels (dy2 may be NULL = the one-gradient form). */
-int cotb200_bn_bwd_sums2(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                         const float* scale, const float* shift, const float* mu, const float* rstd, int relu, float* sum_dz,
-                         float* sum_dzx, void* stream);
-int cotb200_bn_bwd_apply2(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                          const float* scale, const float* shift, const float* mu, const float* rstd, const float* c1,
-                          const float* c2, float inv_n, int relu, void* dx, void* dres, void* stream);
+                           const float* weight, const float* bias, float* running_mean, float* running_var, float n, float eps,
+                           float momentum, int update_running, int relu, void* y, float* scale, float* shift, float* mean,
+                           float* rstd, const float* sample_scale, unsigned char* mask, void* stream);
+/* g = dy*[y > 0] (g = dy for relu 0); the BatchNorm output gradient is dz = s_b*g (dz = g when sample_scale is NULL);
+ * sum_dz[c] += sum dz ; sum_dzx[c] += sum dz*xhat.  relu, the source of the ReLU mask:
+ *   0: no activation;
+ *   1: read from the forward output y;
+ *   2: recomputed as [s_b*(x*scale + shift) > 0] from the forward's own fp32 scale/shift (identical mask, y is NOT read: one
+ *      HBM pass less; only for BatchNorms without a residual input);
+ *   3: read from the 1-bit mask cotb200_bn_apply_batch wrote (C/8 bytes per row instead of C elements; C % 8 == 0).
+ * y may be NULL unless relu == 1, scale/shift unless relu == 2, and mask must be NULL unless relu == 3 (COTB200_EINVAL).
+ * sample_scale as in cotb200_bn_apply. */
+int cotb200_bn_bwd_sums(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y, const unsigned char* mask,
+                        const float* scale, const float* shift, const float* mu, const float* rstd, int relu,
+                        float* sum_dz, float* sum_dzx, const float* sample_scale, void* stream);
 /* dx = scale*(dz - c1*inv_n - xhat*c2*inv_n) (c1,c2 = the raw sums of cotb200_bn_bwd_sums, NULL in eval mode) ;
- * dres = dz when dres != NULL (gradient of the residual) */
-int cotb200_bn_bwd_apply(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y, const float* scale,
-                         const float* shift, const float* mu, const float* rstd, const float* c1, const float* c2,
-                         float inv_n, int relu, void* dx, void* dres, void* stream);
-/* Stochastic depth (DropPath after bn3, models/cotnet.py:256-257) inside the same kernels.  sample_scale: device fp32 [B] = s_b,
- * 0 for a dropped sample and 1/keep for a kept one (NULL = all 1: then each call is its plain form above, bit for bit).
- *   forward:  y = act(s_b*(x*scale + shift) (+ res))
- *   backward: g = dy*mask (dy := dy + dy2 when dy2 != NULL); dres = g; the BatchNorm output gradient is s_b*g, so
- *             sum_dz += sum s_b*g, sum_dzx += sum s_b*g*xhat and dx = scale*(s_b*g - c1*inv_n - xhat*c2*inv_n).
- * The batch statistics (cotb200_col_stats, the GEMM epilogue) still cover every sample, dropped or not. */
-int cotb200_bn_apply_ds(int dtype, int B, int HW, int C, const void* x, const void* res, const float* scale,
-                        const float* shift, int relu, void* y, const float* sample_scale, void* stream);
-int cotb200_bn_apply_batch_ds(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum, const float* sq,
-                              const float* weight, const float* bias, float* running_mean, float* running_var, float n,
-                              float eps, float momentum, int update_running, int relu, void* y, float* scale, float* shift,
-                              float* mean, float* rstd, const float* sample_scale, void* stream);
-int cotb200_bn_bwd_sums_ds(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                           const float* scale, const float* shift, const float* mu, const float* rstd, int relu, float* sum_dz,
-                           float* sum_dzx, const float* sample_scale, void* stream);
-int cotb200_bn_bwd_apply_ds(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x, const void* y,
-                            const float* scale, const float* shift, const float* mu, const float* rstd, const float* c1,
-                            const float* c2, float inv_n, int relu, void* dx, void* dres, const float* sample_scale,
-                            void* stream);
-/* 1-bit ReLU mask for BatchNorms with a residual input (relu code 3).  With a residual the mask cannot be recomputed from x
- * (code 2), and reading y back costs two full passes of the widest tensors of the bottleneck.  The training-mode apply writes,
- * next to y, mask [B*HW, C/8] bytes: bit c%8 of byte c/8 of a row = [y > 0] of the STORED y (so the mask equals relu code 1's
- * bit for bit); the backward kernels read the mask instead of y (C/8 bytes per row instead of C elements).  Needs C % 8 == 0.
- * Otherwise these are cotb200_bn_apply_batch_ds (relu = 1, res required), cotb200_bn_bwd_sums_ds and cotb200_bn_bwd_apply_ds:
- * dy2 and sample_scale may be NULL. */
-int cotb200_bn_apply_batch_mask(int dtype, int B, int HW, int C, const void* x, const void* res, const float* sum, const float* sq,
-                                const float* weight, const float* bias, float* running_mean, float* running_var, float n,
-                                float eps, float momentum, int update_running, void* y, float* scale, float* shift,
-                                float* mean, float* rstd, const float* sample_scale, unsigned char* mask, void* stream);
-int cotb200_bn_bwd_sums_mask(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x,
-                             const unsigned char* mask, const float* mu, const float* rstd, float* sum_dz, float* sum_dzx,
-                             const float* sample_scale, void* stream);
-int cotb200_bn_bwd_apply_mask(int dtype, int B, int HW, int C, const void* dy, const void* dy2, const void* x,
-                              const unsigned char* mask, const float* scale, const float* mu, const float* rstd, const float* c1,
-                              const float* c2, float inv_n, void* dx, void* dres, const float* sample_scale, void* stream);
+ * dres = g when dres != NULL (gradient of the residual).  g, dz, relu, y, mask and sample_scale as in cotb200_bn_bwd_sums;
+ * scale is always read, shift only for relu == 2. */
+int cotb200_bn_bwd_apply(int dtype, int B, int HW, int C, const void* dy, const void* x, const void* y, const unsigned char* mask,
+                         const float* scale, const float* shift, const float* mu, const float* rstd, const float* c1,
+                         const float* c2, float inv_n, int relu, void* dx, void* dres, const float* sample_scale, void* stream);
 /* One launch for the BatchNorm bookkeeping: from the column sums of cotb200_col_stats (or a GEMM epilogue) compute
  * scale = gamma*rstd, shift = beta - mean*scale, mean, rstd, and update running_mean / running_var like nn.BatchNorm2d
  * (momentum, unbiased variance).  use_batch = 0: eval mode, statistics read from the running buffers. */

@@ -21,7 +21,7 @@ def _p(t):
 
 # ------------------------------------------------------------------------------------------------ mask kernels (C ABI)
 def _inputs(dtype, B, HW, C, seed):
-    """x, res, dy, dy2 [B*HW, C] with exact zeros and values next to zero in x, res and the residual sum, so that the stored
+    """x, res, dy [B*HW, C] with exact zeros and values next to zero in x, res and the residual sum, so that the stored
     y has exact zeros, tiny positives and tiny negatives clamped to zero."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     n = B * HW
@@ -33,8 +33,7 @@ def _inputs(dtype, B, HW, C, seed):
     res[3::11, 1::4] = -1e-30
     res[4::13, 2::4] = 1e-38
     dy = torch.randn(n, C, generator=g, device="cuda")
-    dy2 = torch.randn(n, C, generator=g, device="cuda")
-    return [t.to(dtype).contiguous() for t in (x, res, dy, dy2)]
+    return [t.to(dtype).contiguous() for t in (x, res, dy)]
 
 
 def _forward(lib, dt, B, HW, C, x, res, ds, mask):
@@ -47,34 +46,24 @@ def _forward(lib, dt, B, HW, C, x, res, ds, mask):
     rm, rv = torch.zeros(C, device="cuda"), torch.ones(C, device="cuda")
     ss = torch.empty(4, C, device="cuda")
     y = torch.empty_like(x)
-    args = (dt, B, HW, C, _p(x), _p(res), _p(sums[0]), _p(sums[1]), _p(w), _p(b), _p(rm), _p(rv), float(B * HW), 1e-5, 0.1, 1)
-    outs = (_p(y), _p(ss[0]), _p(ss[1]), _p(ss[2]), _p(ss[3]))
-    if mask is not None:
-        _lib.check(lib.cotb200_bn_apply_batch_mask(*args, *outs, _p(ds), _p(mask), st), "bn_apply_batch_mask")
-    elif ds is not None:
-        _lib.check(lib.cotb200_bn_apply_batch_ds(*args, 1, *outs, _p(ds), st), "bn_apply_batch_ds")
-    else:
-        _lib.check(lib.cotb200_bn_apply_batch(*args, 1, *outs, st), "bn_apply_batch")
+    _lib.check(lib.cotb200_bn_apply_batch(dt, B, HW, C, _p(x), _p(res), _p(sums[0]), _p(sums[1]), _p(w), _p(b), _p(rm), _p(rv),
+                                          float(B * HW), 1e-5, 0.1, 1, 1, _p(y), _p(ss[0]), _p(ss[1]), _p(ss[2]), _p(ss[3]), _p(ds),
+                                          _p(mask), st), "bn_apply_batch")
     return y, ss, rm, rv
 
 
-def _backward(lib, dt, B, HW, C, dy, dy2, x, y_or_mask, ss, ds, rcode):
+def _backward(lib, dt, B, HW, C, dy, x, y_or_mask, ss, ds, rcode, dres_on):
+    """sums, dx and (dres_on) dres; without dres the kernels compile the residual-gradient store out."""
     st = torch.cuda.current_stream().cuda_stream
     sums = torch.zeros(2, C, device="cuda")
-    dx, dres = torch.empty_like(x), torch.empty_like(x)
+    dx, dres = torch.empty_like(x), (torch.empty_like(x) if dres_on else None)
     scale, mean, rstd = ss[0], ss[2], ss[3]
-    inv_n = 1.0 / (B * HW)
-    if rcode == 3:
-        _lib.check(lib.cotb200_bn_bwd_sums_mask(dt, B, HW, C, _p(dy), _p(dy2), _p(x), _p(y_or_mask), _p(mean), _p(rstd), _p(sums[0]),
-                                                _p(sums[1]), _p(ds), st), "bn_bwd_sums_mask")
-        _lib.check(lib.cotb200_bn_bwd_apply_mask(dt, B, HW, C, _p(dy), _p(dy2), _p(x), _p(y_or_mask), _p(scale), _p(mean), _p(rstd),
-                                                 _p(sums[0]), _p(sums[1]), inv_n, _p(dx), _p(dres), _p(ds), st), "bn_bwd_apply_mask")
-    else:
-        _lib.check(lib.cotb200_bn_bwd_sums_ds(dt, B, HW, C, _p(dy), _p(dy2), _p(x), _p(y_or_mask), _p(scale), None, _p(mean), _p(rstd),
-                                              1, _p(sums[0]), _p(sums[1]), _p(ds), st), "bn_bwd_sums_ds")
-        _lib.check(lib.cotb200_bn_bwd_apply_ds(dt, B, HW, C, _p(dy), _p(dy2), _p(x), _p(y_or_mask), _p(scale), None, _p(mean), _p(rstd),
-                                               _p(sums[0]), _p(sums[1]), inv_n, 1, _p(dx), _p(dres), _p(ds), st), "bn_bwd_apply_ds")
-    return sums, dx, dres
+    y, mask = (None, y_or_mask) if rcode == 3 else (y_or_mask, None)
+    head = (dt, B, HW, C, _p(dy), _p(x), _p(y), _p(mask), _p(scale), None, _p(mean), _p(rstd))
+    _lib.check(lib.cotb200_bn_bwd_sums(*head, rcode, _p(sums[0]), _p(sums[1]), _p(ds), st), "bn_bwd_sums")
+    _lib.check(lib.cotb200_bn_bwd_apply(*head, _p(sums[0]), _p(sums[1]), 1.0 / (B * HW), rcode, _p(dx), _p(dres), _p(ds), st),
+               "bn_bwd_apply")
+    return [sums, dx] + ([dres] if dres_on else [])
 
 
 def _unpack(mask, C):
@@ -83,19 +72,18 @@ def _unpack(mask, C):
 
 
 @pytest.mark.parametrize("ds_on", [False, True])
-@pytest.mark.parametrize("two", [False, True])
+@pytest.mark.parametrize("dres_on", [False, True])
 @pytest.mark.parametrize("C", [64, 2048, 200])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
-def test_mask_kernels_equal_y_path(dtype, C, two, ds_on):
-    """Forward: the mask form writes the same y, statistics and running buffers as the plain form, and its mask is [y > 0].
-    Backward: sums, dx and dres from the mask (code 3) equal those from y (code 1) bit for bit, with and without a second incoming
-    gradient and drop-path scales.  C = 2048 in fp32 runs in column chunks; C = 200 is not a multiple of 64 (fp32: two threads
-    share each mask byte)."""
+def test_mask_path_equals_y_path(dtype, C, dres_on, ds_on):
+    """Forward: with a mask, bn_apply_batch writes the same y, statistics and running buffers as without one, and the mask is
+    [y > 0].  Backward: sums, dx and dres from the mask (code 3) equal those from y (code 1) bit for bit, with and without drop-path
+    scales, and with and without a residual gradient.  C = 2048 in fp32 runs in column chunks; C = 200 is not a multiple of 64
+    (fp32: two threads share each mask byte)."""
     lib = _lib.load()
     dt = _lib.dtype_code(torch.empty(0, dtype=dtype))
     B, HW = 3, 37
-    x, res, dy, dy2 = _inputs(dtype, B, HW, C, seed=C + (1 if two else 0))
-    dy2 = dy2 if two else None
+    x, res, dy = _inputs(dtype, B, HW, C, seed=C)
     ds = torch.tensor([2.0, 0.0, 1.25], device="cuda") if ds_on else None
     y1, ss1, rm1, rv1 = _forward(lib, dt, B, HW, C, x, res, ds, None)
     mask = torch.full((B * HW, C // 8), 0xA5, dtype=torch.uint8, device="cuda")     # garbage: every byte must be written
@@ -104,21 +92,23 @@ def test_mask_kernels_equal_y_path(dtype, C, two, ds_on):
     m = _unpack(mask, C)
     assert torch.equal(m, y1.float() > 0)
     assert (y1 == 0).any() and m.any() and (~m).any()
-    got = _backward(lib, dt, B, HW, C, dy, dy2, x, mask, ss3, ds, 3)
-    want = _backward(lib, dt, B, HW, C, dy, dy2, x, y1, ss1, ds, 1)
+    got = _backward(lib, dt, B, HW, C, dy, x, mask, ss3, ds, 3, dres_on)
+    want = _backward(lib, dt, B, HW, C, dy, x, y1, ss1, ds, 1, dres_on)
+    assert len(got) == len(want) == (3 if dres_on else 2)
     for a, b, name in zip(got, want, ("sums", "dx", "dres")):
         assert torch.equal(a, b), name
 
 
-def test_mask_entry_points_reject_bad_channels():
+def test_mask_arguments_reject_bad_channels():
     lib = _lib.load()
     x = torch.zeros(4, 12, device="cuda", dtype=torch.bfloat16)
     m = torch.zeros(4, 2, dtype=torch.uint8, device="cuda")
     f = torch.zeros(12, device="cuda")
-    rc = lib.cotb200_bn_bwd_sums_mask(_lib.BF16, 1, 4, 12, _p(x), None, _p(x), _p(m), _p(f), _p(f), _p(f), _p(f), None, None)
+    rc = lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 12, _p(x), _p(x), None, _p(m), None, None, _p(f), _p(f), 3, _p(f), _p(f), None,
+                                 None)
     assert rc == -1                      # COTB200_EINVAL: C % 8 != 0
-    rc = lib.cotb200_bn_bwd_apply_mask(_lib.BF16, 1, 4, 8, _p(x), None, _p(x), None, _p(f), _p(f), _p(f), None, None, 0.25,
-                                       _p(x), None, None, None)
+    rc = lib.cotb200_bn_bwd_apply(_lib.BF16, 1, 4, 8, _p(x), _p(x), None, None, _p(f), None, _p(f), _p(f), None, None, 0.25, 3,
+                                  _p(x), None, None, None)
     assert rc == -5                      # COTB200_ENULL: no mask
 
 

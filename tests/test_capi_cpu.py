@@ -87,17 +87,36 @@ def test_row_kernel_argument_errors():
     assert lib.cotb200_sum_rows(_lib.BF16, 10, 8, P, 4, P, 8, None, 0, None, 0, P, 8, None) == EINVAL
     assert lib.cotb200_sum_rows(_lib.BF16, 10, 8, P, 8, P, 8, None, 0, None, 0, P, 4, None) == EINVAL
     assert lib.cotb200_sum_rows(_lib.F64, 10, 8, P, 8, P, 8, None, 0, None, 0, P, 8, None) == EDTYPE
-    # BatchNorm backward: relu code 1 needs y, code 2 needs scale AND shift, other codes are rejected
-    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 8, P, P, None, P, P, P, P, 1, P, P, None) == ENULL
-    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 8, P, P, None, P, None, P, P, 2, P, P, None) == ENULL
-    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 8, P, P, P, P, P, P, P, 3, P, P, None) == EINVAL
-    assert lib.cotb200_bn_bwd_apply(_lib.BF16, 1, 4, 8, P, P, None, P, None, P, P, None, None, 0.25, 2, P, None, None) == ENULL
-    assert lib.cotb200_bn_bwd_apply(_lib.F64, 1, 4, 8, P, P, P, P, P, P, P, None, None, 0.25, 1, P, None, None) == EDTYPE
-    # BatchNorm forward with in-kernel finalisation: running buffers required when they are to be updated
-    assert lib.cotb200_bn_apply_batch(_lib.BF16, 1, 4, 8, P, None, P, P, None, None, None, None, 4.0, 1e-5, 0.1, 1, 1, P, P, P, P, P,
-                                      None) == ENULL
     # GroupNorm(9 taps): chunk width must divide the weight channels; bwd_sums needs its workspace
     assert lib.cotb200_gn9_stats(_lib.BF16, 2, 9, 12, 8, P, None, P, P, None) == EINVAL
     assert lib.cotb200_gn9_apply(_lib.BF16, 2, 9, 12, 8, P, None, P, P, P, P, P, None) == EINVAL
     assert lib.cotb200_gn9_bwd_sums(_lib.BF16, 2, 9, 16, 8, P, P, None, P, P, P, None, P, P, P, P, None, None) == ENULL
+    assert lib.cotb200_last_error()
+
+
+def test_bn_argument_errors():
+    """Argument validation of the BatchNorm entry points (returns before any CUDA call)."""
+    lib = _lib.load()
+    P = 16          # any non-NULL "pointer": these calls must fail in validation, nothing is dereferenced
+    ENULL, EINVAL, EDTYPE = -5, -1, -2
+    # BatchNorm backward: relu code 1 needs y, code 2 needs scale AND shift, code 3 needs the mask, a mask needs code 3, other
+    # codes are rejected
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 8, P, P, None, None, P, P, P, P, 1, P, P, None, None) == ENULL
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 8, P, P, None, None, P, None, P, P, 2, P, P, None, None) == ENULL
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 8, P, P, P, None, P, P, P, P, 3, P, P, None, None) == ENULL
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 8, P, P, P, P, P, P, P, P, 1, P, P, None, None) == EINVAL
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 1, 4, 8, P, P, P, None, P, P, P, P, 4, P, P, None, None) == EINVAL
+    assert lib.cotb200_bn_bwd_apply(_lib.BF16, 1, 4, 8, P, P, None, None, P, None, P, P, None, None, 0.25, 2, P, None, None,
+                                    None) == ENULL
+    assert lib.cotb200_bn_bwd_apply(_lib.BF16, 1, 4, 8, P, P, None, P, P, P, P, P, None, None, 0.25, 2, P, None, None,
+                                    None) == EINVAL
+    assert lib.cotb200_bn_bwd_apply(_lib.BF16, 1, 4, 8, P, P, P, None, P, P, P, P, None, None, 0.25, 4, P, None, None,
+                                    None) == EINVAL
+    assert lib.cotb200_bn_bwd_apply(_lib.F64, 1, 4, 8, P, P, P, None, P, P, P, P, None, None, 0.25, 1, P, None, None, None) == EDTYPE
+    # BatchNorm forward with in-kernel finalisation: running buffers required when they are to be updated; the 1-bit mask
+    # needs the ReLU
+    assert lib.cotb200_bn_apply_batch(_lib.BF16, 1, 4, 8, P, None, P, P, None, None, None, None, 4.0, 1e-5, 0.1, 1, 1, P, P, P, P, P,
+                                      None, None, None) == ENULL
+    assert lib.cotb200_bn_apply_batch(_lib.BF16, 1, 4, 8, P, P, P, P, None, None, None, None, 4.0, 1e-5, 0.1, 0, 0, P, P, P, P, P,
+                                      None, P, None) == EINVAL
     assert lib.cotb200_last_error()

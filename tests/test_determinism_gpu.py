@@ -366,24 +366,23 @@ def test_col_stats(dtype, B, HW, C, reg):
     run_case(Case(nslots, [((C,), torch.float32, PREFILL, True)] * 2, call, reference), "col_stats %s" % reg)
 
 
-BN_BWD = [  # (two gradients, relu, dtype, B, HW, C, regime)
-    (False, 0, torch.bfloat16, 1, 16, 64, "R1"),
-    (False, 1, torch.bfloat16, 3, 100, 96, "R2"),
-    (False, 2, torch.bfloat16, 8, 3136, 64, "R3"),
-    (True, 1, torch.bfloat16, 8, 784, 128, "R3"),
-    (True, 2, torch.float32, 4, 196, 2048, "R3"),   # column chunks
-    (True, 0, torch.bfloat16, 2, 12, 256, "R1"),
+BN_BWD = [  # (relu, dtype, B, HW, C, regime)
+    (0, torch.bfloat16, 1, 16, 64, "R1"),
+    (1, torch.bfloat16, 3, 100, 96, "R2"),
+    (2, torch.bfloat16, 8, 3136, 64, "R3"),
+    (1, torch.bfloat16, 8, 784, 128, "R3"),
+    (2, torch.float32, 4, 196, 2048, "R3"),   # column chunks
+    (0, torch.bfloat16, 2, 12, 256, "R1"),
 ]
 
 
-@pytest.mark.parametrize("two,relu,dtype,B,HW,C,reg", BN_BWD)
-def test_bn_bwd_sums(two, relu, dtype, B, HW, C, reg):
+@pytest.mark.parametrize("relu,dtype,B,HW,C,reg", BN_BWD)
+def test_bn_bwd_sums(relu, dtype, B, HW, C, reg):
     code, es = _DT[dtype]
     nslots = rows_slots("flat", B, HW, C, es, _sms())
     assert regime(nslots) == reg, _geo_str(nslots)
     g = _gen(B * HW + C + relu)
     dy = _pos_mean((B, HW, C), g, dtype)
-    dy2 = _pos_mean((B, HW, C), g, dtype) if two else None
     x = _pos_mean((B, HW, C), g, dtype)
     y = _pos_mean((B, HW, C), g, dtype)               # relu 1: mask [y > 0] (about 84 % of the elements)
     scale = 0.5 + torch.rand(C, generator=g, device="cuda")
@@ -393,16 +392,12 @@ def test_bn_bwd_sums(two, relu, dtype, B, HW, C, reg):
     lib = _lib.load()
 
     def call(o, st):
-        args = (x.data_ptr(), y.data_ptr(), scale.data_ptr(), shift.data_ptr(), mu.data_ptr(), rstd.data_ptr(), relu,
-                o[0].data_ptr(), o[1].data_ptr(), st)
-        if two:
-            rc = lib.cotb200_bn_bwd_sums2(code, B, HW, C, dy.data_ptr(), dy2.data_ptr(), *args)
-        else:
-            rc = lib.cotb200_bn_bwd_sums(code, B, HW, C, dy.data_ptr(), *args)
-        _lib.check(rc, "bn_bwd_sums")
+        _lib.check(lib.cotb200_bn_bwd_sums(code, B, HW, C, dy.data_ptr(), x.data_ptr(), y.data_ptr(), None, scale.data_ptr(),
+                                           shift.data_ptr(), mu.data_ptr(), rstd.data_ptr(), relu, o[0].data_ptr(), o[1].data_ptr(),
+                                           None, st), "bn_bwd_sums")
 
     def reference(o):
-        dz = _d(dy) + (_d(dy2) if two else 0.0)
+        dz = _d(dy)
         xd = _d(x)
         if relu == 1:
             dz = dz * (_d(y) > 0)
@@ -414,7 +409,7 @@ def test_bn_bwd_sums(two, relu, dtype, B, HW, C, reg):
         return [(0, dz.sum(0), dz.abs().sum(0), True), (1, (dz * xh).sum(0), (dz.abs() * xa).sum(0), True)]
 
     run_case(Case(nslots, [((C,), torch.float32, PREFILL, True)] * 2, call, reference),
-             "bn_bwd_sums%s relu=%d %s" % ("2" if two else "", relu, reg))
+             "bn_bwd_sums relu=%d %s" % (relu, reg))
 
 
 # The tail kernels compute y = silu(u*scale + shift) with an approximate sigmoid.  The sums are checked on terms whose value is

@@ -103,18 +103,28 @@ def test_state_dict_unchanged_by_the_rates(fn):
     m.load_state_dict(a, strict=True)
 
 
+def test_drop_path_bn_argument_errors():
+    """The BatchNorm entry points with drop-path scales: rejected before any launch, like without them."""
+    lib = _lib.load()
+    P = 16
+    ENULL, EINVAL, EDTYPE = -5, -1, -2
+    assert lib.cotb200_bn_apply(_lib.BF16, 2, 4, 8, None, None, P, P, 1, P, P, None) == ENULL
+    assert lib.cotb200_bn_apply_batch(_lib.BF16, 2, 4, 8, P, None, P, P, None, None, None, None, 8.0, 1e-5, 0.1, 1, 1, P, P, P,
+                                      P, P, P, None, None) == ENULL
+    assert lib.cotb200_bn_apply_batch(_lib.BF16, 2, 4, 8, P, P, P, P, None, None, None, None, 8.0, 1e-5, 0.1, 0, 0, P, P, P,
+                                      P, P, P, P, None) == EINVAL
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 2, 4, 8, P, P, None, None, P, P, P, P, 1, P, P, P, None) == ENULL
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 2, 4, 8, P, P, P, None, P, P, P, P, 3, P, P, P, None) == ENULL
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 2, 4, 8, P, P, P, P, P, P, P, P, 2, P, P, P, None) == EINVAL
+    assert lib.cotb200_bn_bwd_sums(_lib.BF16, 2, 4, 8, P, P, P, None, P, P, P, P, 4, P, P, P, None) == EINVAL
+    assert lib.cotb200_bn_bwd_apply(_lib.F64, 2, 4, 8, P, P, P, None, P, P, P, P, None, None, 0.1, 1, P, None, P, None) == EDTYPE
+
+
 def test_new_entry_point_argument_errors():
     """NULL operands, an odd batch with mixing, bad dimensions / smoothing, fp64: rejected before any launch."""
     lib = _lib.load()
     P = 16
     ENULL, EINVAL, EDTYPE = -5, -1, -2
-    # BatchNorm with stochastic depth: same validation as the plain entry points
-    assert lib.cotb200_bn_apply_ds(_lib.BF16, 2, 4, 8, None, None, P, P, 1, P, P, None) == ENULL
-    assert lib.cotb200_bn_apply_batch_ds(_lib.BF16, 2, 4, 8, P, None, P, P, None, None, None, None, 8.0, 1e-5, 0.1, 1, 1, P, P, P,
-                                         P, P, P, None) == ENULL
-    assert lib.cotb200_bn_bwd_sums_ds(_lib.BF16, 2, 4, 8, P, None, P, None, P, P, P, P, 1, P, P, P, None) == ENULL
-    assert lib.cotb200_bn_bwd_sums_ds(_lib.BF16, 2, 4, 8, P, None, P, P, P, P, P, P, 3, P, P, P, None) == EINVAL
-    assert lib.cotb200_bn_bwd_apply_ds(_lib.F64, 2, 4, 8, P, None, P, P, P, P, P, P, None, None, 0.1, 1, P, None, P, None) == EDTYPE
     # the mixing input kernel
     f3 = (ctypes.c_float * 3)(1, 1, 1)
     assert lib.cotb200_u8_mix_to_nhwc(_lib.BF16, 4, 3, 8, 8, None, P, f3, f3, None, None, P, None) == ENULL

@@ -78,13 +78,13 @@ def main():
             rec[name + "_frac"] = round(gbs / pk, 3)
 
         run("col_stats", 1, lambda i: _lib.check(lib.cotb200_col_stats(dt, 1, rows, C, xs[i].data_ptr(), f[0].data_ptr(), f[1].data_ptr(), st), "cs"))
-        run("bn_apply", 2, lambda i: _lib.check(lib.cotb200_bn_apply(dt, 1, rows, C, xs[i].data_ptr(), None, f[3].data_ptr(), f[2].data_ptr(), 1, o1.data_ptr(), st), "ba"))
-        run("bn_apply_res", 3, lambda i: _lib.check(lib.cotb200_bn_apply(dt, 1, rows, C, xs[i].data_ptr(), ds[i].data_ptr(), f[3].data_ptr(), f[2].data_ptr(), 1, o1.data_ptr(), st), "bar"))
-        run("bn_bwd_sums", 3, lambda i: _lib.check(lib.cotb200_bn_bwd_sums(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), ys[i].data_ptr(), f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), 1, f[4].data_ptr(), f[5].data_ptr(), st), "bs"))
-        run("bn_bwd_sums_xmask", 2, lambda i: _lib.check(lib.cotb200_bn_bwd_sums(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), None, f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), 2, f[4].data_ptr(), f[5].data_ptr(), st), "bsx"))
-        run("bn_bwd_apply", 4, lambda i: _lib.check(lib.cotb200_bn_bwd_apply(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), ys[i].data_ptr(), f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), f[4].data_ptr(), f[5].data_ptr(), 1.0 / rows, 1, o1.data_ptr(), None, st), "bb"))
-        run("bn_bwd_apply_xmask", 3, lambda i: _lib.check(lib.cotb200_bn_bwd_apply(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), None, f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), f[4].data_ptr(), f[5].data_ptr(), 1.0 / rows, 2, o1.data_ptr(), None, st), "bbx"))
-        run("bn_bwd_apply_res", 5, lambda i: _lib.check(lib.cotb200_bn_bwd_apply(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), ys[i].data_ptr(), f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), f[4].data_ptr(), f[5].data_ptr(), 1.0 / rows, 1, o1.data_ptr(), o2.data_ptr(), st), "bbr"))
+        run("bn_apply", 2, lambda i: _lib.check(lib.cotb200_bn_apply(dt, 1, rows, C, xs[i].data_ptr(), None, f[3].data_ptr(), f[2].data_ptr(), 1, o1.data_ptr(), None, st), "ba"))
+        run("bn_apply_res", 3, lambda i: _lib.check(lib.cotb200_bn_apply(dt, 1, rows, C, xs[i].data_ptr(), ds[i].data_ptr(), f[3].data_ptr(), f[2].data_ptr(), 1, o1.data_ptr(), None, st), "bar"))
+        run("bn_bwd_sums", 3, lambda i: _lib.check(lib.cotb200_bn_bwd_sums(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), ys[i].data_ptr(), None, f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), 1, f[4].data_ptr(), f[5].data_ptr(), None, st), "bs"))
+        run("bn_bwd_sums_xmask", 2, lambda i: _lib.check(lib.cotb200_bn_bwd_sums(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), None, None, f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), 2, f[4].data_ptr(), f[5].data_ptr(), None, st), "bsx"))
+        run("bn_bwd_apply", 4, lambda i: _lib.check(lib.cotb200_bn_bwd_apply(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), ys[i].data_ptr(), None, f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), f[4].data_ptr(), f[5].data_ptr(), 1.0 / rows, 1, o1.data_ptr(), None, None, st), "bb"))
+        run("bn_bwd_apply_xmask", 3, lambda i: _lib.check(lib.cotb200_bn_bwd_apply(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), None, None, f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), f[4].data_ptr(), f[5].data_ptr(), 1.0 / rows, 2, o1.data_ptr(), None, None, st), "bbx"))
+        run("bn_bwd_apply_res", 5, lambda i: _lib.check(lib.cotb200_bn_bwd_apply(dt, 1, rows, C, ds[i].data_ptr(), xs[i].data_ptr(), ys[i].data_ptr(), None, f[3].data_ptr(), f[2].data_ptr(), f[2].data_ptr(), f[3].data_ptr(), f[4].data_ptr(), f[5].data_ptr(), 1.0 / rows, 1, o1.data_ptr(), o2.data_ptr(), None, st), "bbr"))
         run("sum_rows3", 4, lambda i: _lib.check(lib.cotb200_sum_rows(dt, rows, C, xs[i].data_ptr(), C, ys[i].data_ptr(), C, ds[i].data_ptr(), C, None, 0, o1.data_ptr(), C, st), "sr"))
         out.append(rec)
         print(json.dumps(rec), flush=True)
