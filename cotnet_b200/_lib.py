@@ -33,6 +33,12 @@ class Mix(ctypes.Structure):
                 ("y0", ctypes.c_int), ("y1", ctypes.c_int), ("x0", ctypes.c_int), ("x1", ctypes.c_int)]
 
 
+class MixRow(ctypes.Structure):
+    """struct cotb200_mix_row (include/cotb200.h): the per-sample Mixup / CutMix of one output row."""
+    _fields_ = [("mode", ctypes.c_int), ("partner", ctypes.c_int), ("lam", ctypes.c_float), ("one_minus_lam", ctypes.c_float),
+                ("target_lam", ctypes.c_float), ("y0", ctypes.c_int), ("y1", ctypes.c_int), ("x0", ctypes.c_int), ("x1", ctypes.c_int)]
+
+
 CLIP_NORM, CLIP_VALUE, CLIP_AGC = 1, 2, 3
 
 
@@ -143,6 +149,13 @@ SYMBOLS = {
     "cotb200_soft_ce": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP, _VP]),
     "cotb200_soft_ce_bwd": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP, _VP,
                                                                  ctypes.c_longlong, _VP]),
+    "cotb200_u8_mix_rows_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 6 + [_VP, _VP, ctypes.POINTER(ctypes.c_float),
+                                                                      ctypes.POINTER(ctypes.c_float), _VP, _VP, ctypes.POINTER(MixRow),
+                                                                      _VP, _VP]),
+    "cotb200_soft_ce_rows": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP, ctypes.c_float, _VP, _VP,
+                                                                  _VP]),
+    "cotb200_soft_ce_rows_bwd": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP, ctypes.c_float, _VP,
+                                                                      _VP, _VP, ctypes.c_longlong, _VP]),
     "cotb200_jsd_ce": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP, ctypes.c_longlong, _VP, ctypes.c_float, ctypes.c_float, _VP, _VP, _VP]),
     "cotb200_jsd_ce_bwd": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP, ctypes.c_longlong, _VP, ctypes.c_float, ctypes.c_float, _VP, _VP,
                                                                 _VP, ctypes.c_longlong, _VP]),

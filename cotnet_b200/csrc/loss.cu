@@ -5,7 +5,8 @@
 //   loss_b = lse(z_b) - sum_c t_bc z_bc,   sum_c t_bc z_bc = off*sum_c z_bc + (on - off)*(lam*z_b[y_b] + (1-lam)*z_b[y_{B-1-b}])
 // with off = smoothing/K, on = 1 - smoothing + off.  One CTA per row (two passes over the row, the second from L1/L2), then one
 // CTA adds the B row losses in a fixed order: the loss is bit-identical from run to run.  lam = mix->target_lam is read from
-// device memory so that a captured graph follows every step's Mixup / CutMix draw.
+// device memory so that a captured graph follows every step's Mixup / CutMix draw.  The per-sample modes read lam and the partner
+// row y_{partner(b)} from a device table (cotb200_mix_row) instead, through the same kernels.
 //
 // JsdCrossEntropy (loss/jsd.py) of the augmentation splits: label-smoothed cross entropy on the clean split plus alpha/S times
 // the KL divergence of every split's softmax from their clamped mixture.  One CTA per clean row handles its S rows; the row losses
@@ -35,7 +36,26 @@ __device__ __forceinline__ float ce_block_reduce(float v, float* sm, Op op) {
   return t;
 }
 
-__device__ __forceinline__ float ce_lam(const cotb200_mix* mix) { return mix ? mix->target_lam : 1.f; }
+// whose label takes the rest of row b's soft target, and row b's own weight: the batch draw (partner B-1-b, one lam; no mixing
+// without it) or the per-sample table (any partner, checked against the n_labels labels: -1 makes the row NaN)
+struct CeBatchMix {
+  const cotb200_mix* mix;
+  int B;
+  __device__ __forceinline__ bool on() const { return mix != nullptr; }
+  __device__ __forceinline__ float lam(int) const { return mix ? mix->target_lam : 1.f; }
+  __device__ __forceinline__ long long partner(int b) const { return B - 1 - b; }
+};
+
+struct CeRowMix {
+  const cotb200_mix_row* rows;
+  int n_labels;
+  __device__ __forceinline__ bool on() const { return true; }
+  __device__ __forceinline__ float lam(int b) const { return rows[b].target_lam; }
+  __device__ __forceinline__ long long partner(int b) const {
+    const int p = rows[b].partner;
+    return (p >= 0 && p < n_labels) ? p : -1;
+  }
+};
 
 // log-sum-exp and sum of one row, every thread of the CTA gets both
 template <typename T>
@@ -51,25 +71,25 @@ __device__ __forceinline__ float ce_row_lse(const T* __restrict__ zr, int K, flo
   return mx + logf(se);
 }
 
-template <typename T>
+template <typename T, class Mix>
 __global__ void __launch_bounds__(CE_THREADS)
-soft_ce_rows_kernel(const T* __restrict__ z, long long ld, const long long* __restrict__ labels, const cotb200_mix* __restrict__ mix,
-                    int B, int K, float off, float onoff, float* __restrict__ rows) {
+soft_ce_rows_kernel(const T* __restrict__ z, long long ld, const long long* __restrict__ labels, Mix mix, int B, int K, float off,
+                    float onoff, float* __restrict__ rows) {
   __shared__ float sm[CE_THREADS / 32];
   const int b = blockIdx.x;
   const T* zr = z + (long long)b * ld;
   float sz;
   const float lse = ce_row_lse(zr, K, sm, sz);
   if (threadIdx.x == 0) {
-    const float lam = ce_lam(mix);
+    const float lam = mix.lam(b);
     const long long y = labels[b];
     float own = __int_as_float(0x7fffffff), other = 0.f;
     if (y >= 0 && y < K) own = to_acc(zr[y]);
-    if (mix) {
-      const long long yp = labels[B - 1 - b];
+    if (mix.on()) {
+      const long long p = mix.partner(b), yp = p >= 0 ? labels[p] : -1;
       other = (yp >= 0 && yp < K) ? to_acc(zr[yp]) : __int_as_float(0x7fffffff);
     }
-    const float dot = off * sz + onoff * (mix ? lam * own + (1.f - lam) * other : own);
+    const float dot = off * sz + onoff * (mix.on() ? lam * own + (1.f - lam) * other : own);
     rows[b] = lse;
     rows[B + b] = lse - dot;
   }
@@ -84,18 +104,17 @@ soft_ce_mean_kernel(const float* __restrict__ row_loss, int B, float* __restrict
   if (threadIdx.x == 0) loss[0] = s / (float)B;
 }
 
-template <typename T>
+template <typename T, class Mix>
 __global__ void __launch_bounds__(CE_THREADS)
-soft_ce_bwd_kernel(const T* __restrict__ z, long long ld, const long long* __restrict__ labels, const cotb200_mix* __restrict__ mix,
-                   int B, int K, float off, float onoff, const float* __restrict__ rows, const float* __restrict__ dloss,
-                   float* __restrict__ dz, long long ldz) {
+soft_ce_bwd_kernel(const T* __restrict__ z, long long ld, const long long* __restrict__ labels, Mix mix, int B, int K, float off,
+                   float onoff, const float* __restrict__ rows, const float* __restrict__ dloss, float* __restrict__ dz, long long ldz) {
   const int b = blockIdx.x;
   const T* zr = z + (long long)b * ld;
   float* dr = dz + (long long)b * ldz;
-  const float lam = ce_lam(mix), g = __ldg(dloss) / (float)B, lse = rows[b];
-  const long long y = labels[b], yp = mix ? labels[B - 1 - b] : y;
+  const float lam = mix.lam(b), g = __ldg(dloss) / (float)B, lse = rows[b];
+  const long long y = labels[b], p = mix.on() ? mix.partner(b) : b, yp = p >= 0 ? labels[p] : -1;
   const bool ok = y >= 0 && y < K && yp >= 0 && yp < K;
-  const float w_own = onoff * (mix ? lam : 1.f), w_other = mix ? onoff * (1.f - lam) : 0.f;
+  const float w_own = onoff * (mix.on() ? lam : 1.f), w_other = mix.on() ? onoff * (1.f - lam) : 0.f;
   for (int c = threadIdx.x; c < K; c += CE_THREADS) {
     const float t = off + (c == y ? w_own : 0.f) + (c == yp ? w_other : 0.f);
     dr[c] = ok ? g * (expf(to_acc(zr[c]) - lse) - t) : __int_as_float(0x7fffffff);
@@ -299,7 +318,7 @@ extern "C" int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long
   COTB200_DISPATCH_DTYPE(dtype, {
     if constexpr (!std::is_same<T, double>::value) {
       COTB200_PROF_B("soft_ce", (double)B * K * sizeof(T));
-      soft_ce_rows_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, mix, B, K, off, onoff, rows);
+      soft_ce_rows_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeBatchMix{mix, B}, B, K, off, onoff, rows);
       if ((rc = check_launch("soft_ce"))) return rc;
       soft_ce_mean_kernel<<<1, CE_THREADS, 0, st>>>(rows + B, B, loss);
       return check_launch("soft_ce_mean");
@@ -320,8 +339,57 @@ extern "C" int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, 
   COTB200_DISPATCH_DTYPE(dtype, {
     if constexpr (!std::is_same<T, double>::value) {
       COTB200_PROF_B("soft_ce_bwd", (double)B * K * (sizeof(T) + 4));
-      soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, mix, B, K, off, onoff, rows, dloss, dz, ldz);
+      soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeBatchMix{mix, B}, B, K, off, onoff, rows, dloss,
+                                                       dz, ldz);
       return check_launch("soft_ce_bwd");
+    }
+  });
+  return 0;
+}
+
+static int soft_ce_rows_check(const char* what, int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
+                              int n_labels, const cotb200_mix_row* mix_rows, float smoothing) {
+  int rc = soft_ce_check(what, dtype, B, K, logits, ld, labels, nullptr, smoothing);
+  if (rc) return rc;
+  if (!mix_rows) { set_error("%s: NULL row table", what); return COTB200_ENULL; }
+  if (n_labels < B || (n_labels & 1)) { set_error("%s: %d labels for %d rows (an even count >= B)", what, n_labels, B); return COTB200_EINVAL; }
+  return 0;
+}
+
+extern "C" int cotb200_soft_ce_rows(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
+                                    const cotb200_mix_row* mix_rows, float smoothing, float* rows, float* loss, void* stream) {
+  int rc = soft_ce_rows_check("soft_ce_rows", dtype, B, K, logits, ld, labels, n_labels, mix_rows, smoothing);
+  if (rc) return rc;
+  if (!rows || !loss) { set_error("soft_ce_rows: NULL pointer"); return COTB200_ENULL; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const float off = smoothing / (float)K, onoff = 1.f - smoothing;
+  COTB200_DISPATCH_DTYPE(dtype, {
+    if constexpr (!std::is_same<T, double>::value) {
+      COTB200_PROF_B("soft_ce_rows", (double)B * K * sizeof(T));
+      soft_ce_rows_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeRowMix{mix_rows, n_labels}, B, K, off, onoff, rows);
+      if ((rc = check_launch("soft_ce_rows"))) return rc;
+      soft_ce_mean_kernel<<<1, CE_THREADS, 0, st>>>(rows + B, B, loss);
+      return check_launch("soft_ce_rows_mean");
+    }
+  });
+  return 0;
+}
+
+extern "C" int cotb200_soft_ce_rows_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
+                                        const cotb200_mix_row* mix_rows, float smoothing, const float* rows, const float* dloss, float* dz,
+                                        long long ldz, void* stream) {
+  int rc = soft_ce_rows_check("soft_ce_rows_bwd", dtype, B, K, logits, ld, labels, n_labels, mix_rows, smoothing);
+  if (rc) return rc;
+  if (!rows || !dloss || !dz) { set_error("soft_ce_rows_bwd: NULL pointer"); return COTB200_ENULL; }
+  if (ldz < K) { set_error("soft_ce_rows_bwd: ldz %lld < K %d", ldz, K); return COTB200_EINVAL; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const float off = smoothing / (float)K, onoff = 1.f - smoothing;
+  COTB200_DISPATCH_DTYPE(dtype, {
+    if constexpr (!std::is_same<T, double>::value) {
+      COTB200_PROF_B("soft_ce_rows_bwd", (double)B * K * (sizeof(T) + 4));
+      soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeRowMix{mix_rows, n_labels}, B, K, off, onoff, rows,
+                                                       dloss, dz, ldz);
+      return check_launch("soft_ce_rows_bwd");
     }
   });
   return 0;

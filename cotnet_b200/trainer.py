@@ -243,7 +243,7 @@ class TrainStep:
         if int(jsd_splits) != jsd_splits or jsd_splits < 0 or jsd_splits == 1:
             raise ValueError("TrainStep: jsd_splits must be 0 (off) or >= 2, got %r" % (jsd_splits,))
         self.jsd_splits = int(jsd_splits)
-        self._gmix = None
+        self._gmix = self._gmix_shape = None
         self.amp_dtype = amp_dtype
         self.nesterov = bool(nesterov)
         self.pg = process_group
@@ -482,10 +482,13 @@ class TrainStep:
             return JsdCrossEntropyFn.apply(out, lab, self.jsd_splits, self.label_smoothing, JSD_ALPHA)
         if mix_dev is None and self.label_smoothing == 0.:
             return self.loss_fn(out, lab)
-        return SoftTargetCrossEntropyFn.apply(out, lab, mix_dev, self.label_smoothing)
+        per_row = mix_dev is not None and mix_dev.numel() != ctypes.sizeof(_lib.Mix)
+        return SoftTargetCrossEntropyFn.apply(out, lab, mix_dev, self.label_smoothing, per_row)
 
     def forward_backward(self, x, lab, mix=None):
-        """mix: None, a MixParams (MixupCutmix.draw) or its 32-byte device struct -- the loss reads the mixed targets' lam from it."""
+        """mix: None, a MixParams / MixRows (MixupCutmix.draw), or its device copy (the 32-byte struct or a row table of 36 bytes
+        per row) -- the loss reads the mixed targets' lam and partners from it.  With a 'half' MixRows, x holds the B/2 mixed
+        images and lab the B labels of the input batch."""
         if self.jsd_splits:
             if mix is not None:
                 raise ValueError("TrainStep: the JSD loss takes augmentation splits, which the reference does not mix (train.py:157)")
@@ -576,7 +579,8 @@ class TrainStep:
     # ------------------------------------------------------------------ CUDA graph
     def capture(self, x, lab, warmup=3, capture_nccl=True, mix=None):
         """Warm up (cuDNN autotune, allocator) and capture the whole step.  Returns a dict describing the launch mode.
-        With `mix` (a MixParams) the graph's loss reads a static copy of the mixing parameters that step(mix=) refreshes."""
+        With `mix` (a MixParams or MixRows) the graph's loss reads a static copy of the mixing parameters that step(mix=)
+        refreshes; the graph then takes draws of that kind and size only."""
         side = torch.cuda.Stream(device=self.dev)
         side.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(side):
@@ -588,6 +592,7 @@ class TrainStep:
             t.done = None
         self._gx, self._glab = x.clone(), lab.clone()
         self._gmix = None if mix is None else mix.dev.clone()
+        self._gmix_shape = None if mix is None else mix.shape
         info = {"cuda_graph": True}
         lc0 = _lib.launch_count()
         try:
@@ -634,6 +639,9 @@ class TrainStep:
         if (mix is None) != (self._gmix is None):
             raise ValueError("TrainStep.step: this graph was captured %s mixing parameters; pass mix= %s"
                              % (("without", "to capture() first") if mix is not None else ("with", "(MixupCutmix.draw) at every step")))
+        if mix is not None and mix.shape != self._gmix_shape:
+            raise ValueError("TrainStep.step: this graph was captured with mixing parameters %s, not %s; capture() again for another "
+                             "mode or batch size" % (_mix_kind(self._gmix_shape), _mix_kind(mix.shape)))
         if mix is not None:
             self._gmix.copy_(mix.on_stream(self.dev), non_blocking=True)
         if self._graph[0] == "one":
@@ -769,14 +777,19 @@ class TrainStep:
         return out
 
 
+def _mix_kind(shape):
+    return "of one batch draw" if shape[0] == "batch" else "per row (%d rows from %d images)" % shape[1:]
+
+
 def normalize_u8(x_u8, mean, std, dtype=torch.bfloat16, mix=None):
     """uint8 NCHW batch [N,C,H,W] (CUDA) -> (x - mean)/std as a channels_last tensor of `dtype`: the PrefetchLoader's
     normalisation (datasets/loader.py:86-90) + the layout / precision the AMP forward wants, in ONE kernel.
-    mix: a MixParams of MixupCutmix.draw -- the batch is Mixup / CutMix-ed first, on the uint8 values, exactly like
-    FastCollateMixup (datasets/mixup.py:282-299), in the same kernel."""
+    mix: a MixParams or MixRows of MixupCutmix.draw -- the batch is Mixup / CutMix-ed first, on the uint8 values, exactly like
+    FastCollateMixup (datasets/mixup.py:223-299), in the same kernel.  A MixRows of mode 'half' gives N/2 rows from N."""
     assert x_u8.is_cuda and x_u8.dtype == torch.uint8 and x_u8.dim() == 4 and x_u8.is_contiguous()
     N, C, H, W = x_u8.shape
-    y = torch.empty((N, C, H, W), dtype=dtype, device=x_u8.device, memory_format=torch.channels_last)
+    n_out = mix.n_out if isinstance(mix, MixRows) else N
+    y = torch.empty((n_out, C, H, W), dtype=dtype, device=x_u8.device, memory_format=torch.channels_last)
     mean = [float(m) for m in mean]
     std = [float(s) for s in std]
     assert len(mean) == C and len(std) == C
@@ -791,6 +804,12 @@ def normalize_u8(x_u8, mean, std, dtype=torch.bfloat16, mix=None):
         _lib.check(rc, "u8_to_nhwc")
         return y
     mix.check(N, H, W)
+    if isinstance(mix, MixRows):
+        rc = _lib.load().cotb200_u8_mix_rows_to_nhwc(_lib.dtype_code(y), N, n_out, C, H, W, x_u8.data_ptr(), y.data_ptr(), mh, sh,
+                                                     _lib.ptr(md), _lib.ptr(sd), mix.host, mix.on_stream(x_u8.device).data_ptr(),
+                                                     _lib.stream_ptr(x_u8))
+        _lib.check(rc, "u8_mix_rows_to_nhwc")
+        return y
     rc = _lib.load().cotb200_u8_mix_to_nhwc(_lib.dtype_code(y), N, C, H, W, x_u8.data_ptr(), y.data_ptr(), mh, sh, _lib.ptr(md),
                                             _lib.ptr(sd), mix.on_stream(x_u8.device).data_ptr(), _lib.stream_ptr(x_u8))
     _lib.check(rc, "u8_mix_to_nhwc")
@@ -810,12 +829,17 @@ class MixParams:
     def __init__(self, host, device=None, target_lam=None):
         self.host = host
         self.target_lam = float(host.target_lam if target_lam is None else target_lam)
+        self._upload(device)
+
+    def _upload(self, device):
         self.dev = self._copied = None
         if device is not None:
-            self.dev = torch.frombuffer(bytearray(bytes(host)), dtype=torch.uint8).pin_memory().to(device, non_blocking=True)
+            self.dev = torch.frombuffer(bytearray(bytes(self.host)), dtype=torch.uint8).pin_memory().to(device, non_blocking=True)
             self._copied = torch.cuda.Event()
             self._copied.record(torch.cuda.current_stream(self.dev.device))
 
+    #: what a graph captured with this draw can take at later steps (TrainStep.step)
+    shape = ("batch",)
     mode = property(lambda self: self.host.mode)
     box = property(lambda self: (self.host.y0, self.host.y1, self.host.x0, self.host.x1))
 
@@ -838,14 +862,46 @@ class MixParams:
         return self.dev
 
 
+class MixRows(MixParams):
+    """One step's per-sample Mixup / CutMix ('elem', 'pair', 'half'): `host` a ctypes array of n_out _lib.MixRow (struct
+    cotb200_mix_row), one per output row, mixing input row n with input row host[n].partner out of n_in; `dev` its device copy,
+    made and consumed like MixParams's.  The kernels validate the rows themselves (cotb200_u8_mix_rows_to_nhwc)."""
+
+    def __init__(self, host, n_in, device=None):
+        self.host, self.n_in, self.n_out = host, int(n_in), len(host)
+        self.shape = ("rows", self.n_out, self.n_in)
+        self._upload(device)
+
+    target_lam = property(lambda self: np.array([r.target_lam for r in self.host], dtype=np.float32))
+
+    def check(self, N, H, W):
+        if N != self.n_in:
+            raise ValueError("mix: a batch of %d images for a row table drawn for %d" % (N, self.n_in))
+
+
+MIX_MODES = ("batch", "pair", "elem", "half")
+
+
 class MixupCutmix:
-    """Batch-mode Mixup / CutMix of the reference configs (FastCollateMixup, datasets/mixup.py; mode 'batch', correct_lam,
-    no cutmix_minmax), drawing its parameters from its own np.random.RandomState(seed) in the reference's call order:
-    rand < prob, rand < switch_prob, beta, randint (box centre row), randint (box centre column).
+    """Mixup / CutMix of the reference configs (FastCollateMixup, datasets/mixup.py, correct_lam), drawing its parameters from
+    its own np.random.RandomState(seed) in the reference's call order.  mode 'batch' (one draw per batch, a MixParams): rand < prob,
+    rand < switch_prob, beta, then the CutMix box.  'elem' / 'pair' / 'half' (a MixRows): _params_per_elem over B, B/2, B/2
+    elements -- rand(n) < switch_prob and both beta(n) arrays when both alphas are on, rand(n) < prob -- then one box per CutMix
+    element in index order; 'half' turns B images into B/2 mixed rows (and B/2 soft targets from the B labels).
+    The box: rand_bbox (randint centre row, randint centre column), or with cutmix_minmax = (lo, hi) rand_bbox_minmax (randint
+    height, width, top, left), which forces cutmix_alpha to 1 and always corrects lam by the box area (datasets/mixup.py:54-114).
     `enabled = False` turns mixing off (mixup_off_epoch); draws then give lam = 1 without consuming random numbers."""
 
     def __init__(self, mixup_alpha=0.8, cutmix_alpha=1.0, prob=1.0, switch_prob=0.5, label_smoothing=0.1, num_classes=1000,
-                 seed=0, correct_lam=True, device="cuda"):
+                 seed=0, correct_lam=True, device="cuda", mode="batch", cutmix_minmax=None):
+        if mode not in MIX_MODES:
+            raise ValueError("MixupCutmix: unknown mode %r (one of %s)" % (mode, ", ".join(MIX_MODES)))
+        self.mode = mode
+        self.cutmix_minmax = None if cutmix_minmax is None or len(cutmix_minmax) == 0 else tuple(float(v) for v in cutmix_minmax)
+        if self.cutmix_minmax is not None:
+            if len(self.cutmix_minmax) != 2:
+                raise ValueError("MixupCutmix: cutmix_minmax needs two ratios, got %r" % (cutmix_minmax,))
+            cutmix_alpha = 1.0
         if not (mixup_alpha > 0. or cutmix_alpha > 0.):
             raise ValueError("MixupCutmix: mixup_alpha or cutmix_alpha must be > 0")
         self.mixup_alpha, self.cutmix_alpha = float(mixup_alpha), float(cutmix_alpha)
@@ -871,45 +927,111 @@ class MixupCutmix:
             lam = float(lam_mix)
         return lam, bool(use_cutmix)
 
-    def draw(self, B, H, W):
-        """Parameters of the next batch of B images of H x W as a MixParams (host struct + device copy)."""
-        if B % 2:
-            raise ValueError("MixupCutmix: batch size %d must be even" % B)
-        lam, use_cutmix = self._params_per_batch()
-        m = _lib.Mix()
-        if use_cutmix:                                              # rand_bbox + cutmix_bbox_and_lam (:30-87), margin 0
+    def _params_per_elem(self, n):                                  # datasets/mixup.py:123-141
+        lam = np.ones(n, dtype=np.float32)
+        use_cutmix = np.zeros(n, dtype=bool)
+        if self.enabled:
+            if self.mixup_alpha > 0. and self.cutmix_alpha > 0.:
+                use_cutmix = self.rng.rand(n) < self.switch_prob
+                lam_mix = np.where(use_cutmix, self.rng.beta(self.cutmix_alpha, self.cutmix_alpha, size=n),
+                                   self.rng.beta(self.mixup_alpha, self.mixup_alpha, size=n))
+            elif self.mixup_alpha > 0.:
+                lam_mix = self.rng.beta(self.mixup_alpha, self.mixup_alpha, size=n)
+            else:
+                use_cutmix = np.ones(n, dtype=bool)
+                lam_mix = self.rng.beta(self.cutmix_alpha, self.cutmix_alpha, size=n)
+            lam = np.where(self.rng.rand(n) < self.prob, lam_mix.astype(np.float32), lam)
+        return lam, use_cutmix
+
+    def _cutmix_box(self, H, W, lam):
+        """cutmix_bbox_and_lam (datasets/mixup.py:30-87, margin 0): the box (y0, y1, x0, x1) and the corrected lam.  The
+        arithmetic follows lam's type: a float64 lam in batch mode, a numpy float32 one per element (sqrt and the box size in
+        fp32); the corrected lam is float64 either way."""
+        if self.cutmix_minmax is not None:                          # rand_bbox_minmax (:54-74)
+            lo, hi = self.cutmix_minmax
+            cut_h = self.rng.randint(int(H * lo), int(H * hi))
+            cut_w = self.rng.randint(int(W * lo), int(W * hi))
+            y0, x0 = self.rng.randint(0, H - cut_h), self.rng.randint(0, W - cut_w)
+            box = (int(y0), int(y0 + cut_h), int(x0), int(x0 + cut_w))
+        else:                                                       # rand_bbox (:30-51)
             ratio = np.sqrt(1 - lam)
             cut_h, cut_w = int(H * ratio), int(W * ratio)
             cy, cx = self.rng.randint(0, H), self.rng.randint(0, W)
-            m.y0, m.y1 = int(np.clip(cy - cut_h // 2, 0, H)), int(np.clip(cy + cut_h // 2, 0, H))
-            m.x0, m.x1 = int(np.clip(cx - cut_w // 2, 0, W)), int(np.clip(cx + cut_w // 2, 0, W))
-            if self.correct_lam:
-                lam = 1. - (m.y1 - m.y0) * (m.x1 - m.x0) / float(H * W)
+            box = (int(np.clip(cy - cut_h // 2, 0, H)), int(np.clip(cy + cut_h // 2, 0, H)),
+                   int(np.clip(cx - cut_w // 2, 0, W)), int(np.clip(cx + cut_w // 2, 0, W)))
+        if self.correct_lam or self.cutmix_minmax is not None:
+            lam = 1. - (box[1] - box[0]) * (box[3] - box[2]) / float(H * W)
+        return box, lam
+
+    def draw(self, B, H, W):
+        """Parameters of the next batch of B images of H x W: a MixParams (host struct + device copy) in mode 'batch', else a
+        MixRows (host row table + device copy)."""
+        if B % 2:
+            raise ValueError("MixupCutmix: batch size %d must be even" % B)
+        if self.mode != "batch":
+            return self._draw_rows(B, H, W)
+        lam, use_cutmix = self._params_per_batch()
+        m = _lib.Mix()
+        if use_cutmix:
+            (m.y0, m.y1, m.x0, m.x1), lam = self._cutmix_box(H, W, lam)
         m.mode = 0 if lam == 1. else (2 if use_cutmix else 1)
         # numpy 2 weak scalars: float32 pixels * python float multiplies by the float rounded to fp32 (:296)
         m.lam, m.one_minus_lam = float(np.float32(lam)), float(np.float32(1 - lam))
         m.target_lam = lam
         return MixParams(m, self.device, lam)
 
+    def _draw_rows(self, B, H, W):
+        """_mix_elem_collate / _mix_pair_collate (datasets/mixup.py:223-280) as a row table.  Each element's lam is fp32, its
+        blend weights fp32 lam and fp32(1 - lam), its corrected CutMix lam rounded back to fp32.  Partners are always the
+        unmixed input rows: row i mixes with row B-1-i; in 'pair' row B-1-i takes the same draw mixed the other way."""
+        pair = self.mode == "pair"
+        n = B if self.mode == "elem" else B // 2
+        lam, use_cutmix = self._params_per_elem(n)
+        rows = (_lib.MixRow * (B if pair else n))()
+        for i in range(n):
+            j = B - 1 - i
+            r = rows[i]
+            r.mode, r.partner, r.lam, r.one_minus_lam, r.target_lam = 0, j, 1., 0., 1.
+            if (lam[i] < 1.) if pair else (lam[i] != 1.):            # pair skips lam >= 1, elem / half lam == 1 (:238, :263)
+                if use_cutmix[i]:
+                    (r.y0, r.y1, r.x0, r.x1), corrected = self._cutmix_box(H, W, lam[i])
+                    lam[i] = corrected
+                    r.mode = 2
+                else:
+                    r.mode = 1
+                r.lam, r.one_minus_lam = float(lam[i]), float(np.float32(1) - lam[i])
+                r.target_lam = float(lam[i])
+            if pair:
+                rows[j] = r
+                rows[j].partner = i
+        return MixRows(rows, B, self.device)
+
 
 class SoftTargetCrossEntropyFn(torch.autograd.Function):
     """SoftTargetCrossEntropy()(logits, mixup_target(labels, K, lam, smoothing)) (loss/cross_entropy.py:29-36,
     datasets/mixup.py:17-27) on cotb200_soft_ce / cotb200_soft_ce_bwd; lam is read on the device from `mix_dev` (the struct of
     a MixParams; None = no mixing, i.e. LabelSmoothingCrossEntropy, and plain cross entropy with smoothing 0).  logits
-    [B, K] fp32 / bf16 / fp16 with unit column stride; labels int64 [B].  Returns the fp32 batch mean."""
+    [B, K] fp32 / bf16 / fp16 with unit column stride; labels int64 [B].  Returns the fp32 batch mean.
+    per_row: `mix_dev` is the row table of a MixRows (cotb200_soft_ce_rows / _bwd) and labels has n_labels >= B entries (2B in
+    'half'): row b mixes labels[b] with labels[partner of b]."""
 
     @staticmethod
-    def forward(ctx, logits, labels, mix_dev, smoothing):
+    def forward(ctx, logits, labels, mix_dev, smoothing, per_row):
         assert logits.is_cuda and logits.dim() == 2 and logits.stride(1) == 1 and labels.dtype == torch.int64
         B, K = logits.shape
         logits, labels = logits.detach(), labels.contiguous()
         rows = torch.empty(2, B, dtype=torch.float32, device=logits.device)
         loss = torch.empty((), dtype=torch.float32, device=logits.device)
         lib, st, dt = _lib.load(), _lib.stream_ptr(logits), _lib.dtype_code(logits)
-        _lib.check(lib.cotb200_soft_ce(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), _lib.ptr(mix_dev),
-                                       float(smoothing), rows.data_ptr(), loss.data_ptr(), st), "soft_ce")
+        if per_row:
+            _lib.check(lib.cotb200_soft_ce_rows(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), labels.numel(),
+                                                mix_dev.data_ptr(), float(smoothing), rows.data_ptr(), loss.data_ptr(), st),
+                       "soft_ce_rows")
+        else:
+            _lib.check(lib.cotb200_soft_ce(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), _lib.ptr(mix_dev),
+                                           float(smoothing), rows.data_ptr(), loss.data_ptr(), st), "soft_ce")
         ctx.save_for_backward(logits, labels, mix_dev, rows)
-        ctx.smoothing = float(smoothing)
+        ctx.smoothing, ctx.per_row = float(smoothing), bool(per_row)
         return loss
 
     @staticmethod
@@ -919,15 +1041,22 @@ class SoftTargetCrossEntropyFn(torch.autograd.Function):
         dloss = dloss.float().contiguous()
         dz = torch.empty(B, K, dtype=torch.float32, device=logits.device)
         lib, st, dt = _lib.load(), _lib.stream_ptr(logits), _lib.dtype_code(logits)
-        _lib.check(lib.cotb200_soft_ce_bwd(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), _lib.ptr(mix_dev),
-                                           ctx.smoothing, rows.data_ptr(), dloss.data_ptr(), dz.data_ptr(), K, st), "soft_ce_bwd")
-        return dz.to(logits.dtype), None, None, None
+        if ctx.per_row:
+            _lib.check(lib.cotb200_soft_ce_rows_bwd(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), labels.numel(),
+                                                    mix_dev.data_ptr(), ctx.smoothing, rows.data_ptr(), dloss.data_ptr(), dz.data_ptr(),
+                                                    K, st), "soft_ce_rows_bwd")
+        else:
+            _lib.check(lib.cotb200_soft_ce_bwd(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), _lib.ptr(mix_dev),
+                                               ctx.smoothing, rows.data_ptr(), dloss.data_ptr(), dz.data_ptr(), K, st), "soft_ce_bwd")
+        return dz.to(logits.dtype), None, None, None, None
 
 
 def soft_target_cross_entropy(logits, labels, mix=None, smoothing=0.):
     """The recipe's loss: mean over the batch of -sum_c t_c log softmax(logits)_c with t = mixup_target(labels, K, mix.target_lam,
-    smoothing).  mix: None or a MixParams (MixupCutmix.draw)."""
-    return SoftTargetCrossEntropyFn.apply(logits, labels, None if mix is None else mix.on_stream(logits.device), smoothing)
+    smoothing).  mix: None, a MixParams or a MixRows (MixupCutmix.draw); with a MixRows of mode 'half', labels are the B labels
+    of the B input images and logits the B/2 mixed rows."""
+    return SoftTargetCrossEntropyFn.apply(logits, labels, None if mix is None else mix.on_stream(logits.device), smoothing,
+                                          isinstance(mix, MixRows))
 
 
 #: JsdCrossEntropy's alpha as train.py:199-201 builds it (the module's default)

@@ -464,6 +464,35 @@ int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long long ld, c
 int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
                         const cotb200_mix* mix, float smoothing, const float* rows, const float* dloss, float* dz,
                         long long ldz, void* stream);
+/* Per-sample Mixup / CutMix of FastCollateMixup's 'elem', 'pair' and 'half' modes (datasets/mixup.py:123-141,223-280): one
+ * row per OUTPUT sample, an array in DEVICE memory read by the kernels like cotb200_mix.  Output row n reads input row n and
+ * input row `partner` (its pixels and its label).
+ *   mode 0: row n unchanged; 1: rint(x_n*lam + x_partner*one_minus_lam); 2: x_partner's pixels in rows [y0, y1) x columns [x0, x1).
+ *   lam, one_minus_lam: the fp32 blend weights (numpy's fp32 lam and fp32(1 - lam)).
+ *   target_lam: the weight of row n's own label in its soft target, (1 - target_lam) that of row partner's label. */
+typedef struct cotb200_mix_row {
+  int mode;
+  int partner;
+  float lam, one_minus_lam, target_lam;
+  int y0, y1, x0, x1;
+} cotb200_mix_row;
+/* cotb200_u8_mix_to_nhwc with one cotb200_mix_row per output row: N_in uint8 input rows (even), N_out <= N_in output rows
+ * (N_out = N_in / 2 in 'half'), the same per-pixel arithmetic.  rows_host / rows_dev: the same N_out rows on the host
+ * (validated) and on the device (read by the kernel).  Rejected with COTB200_EINVAL: odd N_in, N_out outside [1, N_in], a mode
+ * other than 0..2, a partner outside [0, N_in), a CutMix box outside the image.  A device row whose partner is outside
+ * [0, N_in) is never read out of bounds: its output is NaN. */
+int cotb200_u8_mix_rows_to_nhwc(int dtype, int N_in, int N_out, int C, int H, int W, const void* x_u8, void* y,
+                                const float* mean_host, const float* std_host, const float* mean_dev, const float* std_dev,
+                                const cotb200_mix_row* rows_host, const cotb200_mix_row* rows_dev, void* stream);
+/* cotb200_soft_ce / _bwd with the soft target of row b mixing labels[b] (weight mix_rows[b].target_lam) and
+ * labels[mix_rows[b].partner] (the rest): B rows of logits, n_labels >= B labels (even; 2B in 'half'), mix_rows: B rows in
+ * device memory.  Same row arithmetic and fixed-order mean as cotb200_soft_ce; a partner outside [0, n_labels) or a label
+ * outside [0, K) makes its row NaN. */
+int cotb200_soft_ce_rows(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
+                         const cotb200_mix_row* mix_rows, float smoothing, float* rows, float* loss, void* stream);
+int cotb200_soft_ce_rows_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
+                             const cotb200_mix_row* mix_rows, float smoothing, const float* rows, const float* dloss, float* dz,
+                             long long ldz, void* stream);
 /* JsdCrossEntropy(num_splits=S, alpha, smoothing) (loss/jsd.py) of the augmentation splits.  logits: fp32 / bf16 / fp16
  * [S*B, K] with row pitch ld, split-major (row b + s*B is view s of sample b, view 0 the clean one); labels int64, only the
  * first B read.  Per clean row b, with p_sc = softmax(z_{b+sB})_c and m_c = clamp((sum_{s=0..S-1} p_sc) / S, 1e-7, 1):
