@@ -16,7 +16,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import fused
+from . import dropblock, fused
 from .cot_layer import CotLayer, CoXtLayer
 
 
@@ -37,21 +37,39 @@ class Bottleneck(nn.Module):
         self.act3 = nn.ReLU(inplace=True)
         self.downsample = downsample
         self.stride = stride
+        self.drop_block = None          # the stage's dropblock.DropBlock (set by the trunk), applied after bn1 and bn3
+        self.drop_block_sites = ()
 
     def zero_init_last_bn(self):
         nn.init.zeros_(self.bn3.weight)
 
-    def forward(self, x, drop_scale=None):
+    def drop_block_site_names(self):
+        return ("bn1", "bn3")
+
+    def set_drop_block(self, spec, site):
+        """Give the block its stage's DropBlock (or None) and its site numbers from `site` on; returns the next free site."""
+        self.drop_block = spec
+        self.drop_block_sites = () if spec is None else (site, site + 1)
+        return site + len(self.drop_block_sites)
+
+    def forward(self, x, drop_scale=None, drop_block_key=None):
         """drop_scale: None or [B] per-sample stochastic-depth scales applied to bn3's output before the residual add
-        (models/cotnet.py:256-257); the trunk draws them (StochasticDepth)."""
+        (models/cotnet.py:256-257); drop_block_key: None or the trunk's [2] int64 DropBlock key of this forward (both drawn by
+        the trunk, StochasticDepth)."""
+        key = drop_block_key if self.drop_block is not None else None
         if fused.supported(x):
-            return self._forward_fused(x, drop_scale)
+            return self._forward_fused(x, drop_scale, key)
         residual = x
-        x = self.act1(self.bn1(self.conv1(x)))
+        x = self.bn1(self.conv1(x))
+        if key is not None:                                                     # models/cotnet.py:233-234
+            x = dropblock.drop_block(x, key, self.drop_block_sites[0], self.drop_block)
+        x = self.act1(x)
         if self.avd is not None:
             x = self.avd(x)
         x = self.conv2(x)
         x = self.bn3(self.conv3(x))
+        if key is not None:                                                     # :250-251
+            x = dropblock.drop_block(x, key, self.drop_block_sites[1], self.drop_block)
         if drop_scale is not None:
             x = x * drop_scale.to(x.dtype).view(-1, 1, 1, 1)
         if self.downsample is not None:
@@ -59,17 +77,25 @@ class Bottleneck(nn.Module):
         x += residual
         return self.act3(x)
 
-    def _forward_fused(self, x, drop_scale=None):
+    def _forward_fused(self, x, drop_scale=None, key=None):
         """channels_last path: bn1+ReLU and bn3+residual+ReLU (SURVEY section 8f rank 1) run on the fused BatchNorm
-        kernels (2 passes each way) instead of ATen's channels_last batch-norm kernels."""
+        kernels (2 passes each way) instead of ATen's channels_last batch-norm kernels.  With DropBlock the bn1 mask is applied
+        to the ReLU output (relu(a)*M*s == relu(a*M*s), s > 0) and bn3 runs without residual and ReLU, which the DropBlock
+        tail kernel adds."""
         cl = torch.channels_last
         residual = x
         y = fused.conv1x1_bn(x, self.conv1, self.bn1, relu=True)
+        if key is not None:
+            y = dropblock.drop_block(y, key, self.drop_block_sites[0], self.drop_block)
         if self.avd is not None:
             y = fused.avg_pool3x3s2(y)              # nn.AvgPool2d(3, 2, padding=1) on the fused NHWC kernel
         y = self.conv2(y.contiguous(memory_format=cl))
         if self.downsample is not None:
             residual = fused.conv1x1_bn(residual, self.downsample[0], self.downsample[1], relu=False)
+        if key is not None:
+            z = fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=False)
+            return dropblock.drop_block_res_relu(z, residual.contiguous(memory_format=cl), key, self.drop_block_sites[1],
+                                                 self.drop_block, drop_scale)
         return fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=True,
                                 res=residual.contiguous(memory_format=cl), drop_scale=drop_scale)
 
@@ -86,19 +112,41 @@ class StochasticDepth:
     While stochastic depth is active (training mode, drop_path_rate > 0) the trunk calls the bottlenecks one by one to hand each
     its scales, so the ``layer1`` .. ``layer4`` Sequential containers are not called: hooks registered on those four modules do
     not fire then (hooks on the blocks and everything inside them do).  In eval mode, or with drop_path_rate 0, the stages run
-    as before."""
+    as before.
+
+    DropBlock (``drop_block_rate``, models/resnet.py:397-401): stages 3 and 4 share one dropblock.DropBlock each; the trunk draws
+    ONE [2] int64 key per training forward (``torch.randint`` on the input's device, so a captured graph draws a new key at every
+    replay) and hands it to the blocks, whose sites are numbered in forward order (dropblock.py).  While it is active the trunk
+    calls its blocks one by one, as for stochastic depth."""
 
     #: test hook: a [n_blocks, B] tensor of per-sample scales used instead of the random draw (training mode only)
     fixed_drop_path_scales = None
+    #: test hook: a [2] int64 DropBlock key used instead of the random draw (training mode only)
+    fixed_drop_block_key = None
 
-    def _init_regularisers(self, drop_rate, drop_path_rate):
+    def _init_regularisers(self, drop_rate, drop_path_rate, drop_block_rate=0.):
         self.drop_rate = float(drop_rate)
         self.drop_path_rate = float(drop_path_rate)
+        self.drop_block_rate = float(drop_block_rate)
         blocks = self.blocks()
         n = len(blocks)
         for i, blk in enumerate(blocks):
             blk.drop_path_rate = self.drop_path_rate * i / (n - 1)
         self._dp_keep = {}
+        site = 0
+        for name, spec in zip(("layer1", "layer2", "layer3", "layer4"), dropblock.stage_drop_blocks(self.drop_block_rate)):
+            for blk in getattr(self, name):
+                site = blk.set_drop_block(spec, site)
+        self.n_drop_block_sites = site
+
+    def drop_block_table(self):
+        """[(block name, site name, site number, DropBlock)] of every DropBlock site, in forward order."""
+        out = []
+        for name in ("layer1", "layer2", "layer3", "layer4"):
+            for i, blk in enumerate(getattr(self, name)):
+                for where, s in zip(blk.drop_block_site_names(), blk.drop_block_sites):
+                    out.append(("%s.%d" % (name, i), where, s, blk.drop_block))
+        return out
 
     def blocks(self):
         return [b for name in ("layer1", "layer2", "layer3", "layer4") for b in getattr(self, name)]
@@ -120,12 +168,22 @@ class StochasticDepth:
             self._dp_keep[x.device] = keep
         return torch.floor(keep + torch.rand(keep.shape[0], B, dtype=torch.float32, device=x.device)) / keep
 
+    def _drop_block_key(self, x):
+        if not (self.training and self.drop_block_rate > 0.):
+            return None
+        if self.fixed_drop_block_key is not None:
+            k = self.fixed_drop_block_key.to(device=x.device, dtype=torch.int64)
+            assert k.shape == (2,), "fixed_drop_block_key must be [2] int64"
+            return k
+        return torch.randint(0, 2 ** 32, (2,), dtype=torch.int64, device=x.device)
+
     def _run_blocks(self, x):
         s = self._drop_path_scales(x)
-        if s is None:
+        key = self._drop_block_key(x)
+        if s is None and key is None:
             return self.layer4(self.layer3(self.layer2(self.layer1(x))))
         for i, blk in enumerate(self.blocks()):
-            x = blk(x, drop_scale=s[i] if blk.drop_path_rate > 0. else None)
+            x = blk(x, drop_scale=s[i] if (s is not None and blk.drop_path_rate > 0.) else None, drop_block_key=key)
         return x
 
     def _classifier(self, x):
@@ -136,7 +194,7 @@ class StochasticDepth:
 
 class CoTResNet(StochasticDepth, nn.Module):
     def __init__(self, layers, num_classes=1000, in_chans=3, cardinality=1, base_width=64, zero_init_last_bn=True,
-                 drop_rate=0., drop_path_rate=0.):
+                 drop_rate=0., drop_path_rate=0., drop_block_rate=0.):
         super().__init__()
         self.num_classes = num_classes
         inplanes = 64
@@ -160,7 +218,7 @@ class CoTResNet(StochasticDepth, nn.Module):
         self.num_features = inplanes
         self.global_pool = nn.AdaptiveAvgPool2d(1)
         self.fc = nn.Linear(self.num_features, num_classes)
-        self._init_regularisers(drop_rate, drop_path_rate)
+        self._init_regularisers(drop_rate, drop_path_rate, drop_block_rate)
         # models/resnet.py:575-584
         for m in self.modules():
             if isinstance(m, nn.Conv2d):

@@ -14,13 +14,14 @@ ReLU / residual glue of the bottleneck and the 3x3/s2 ``avd`` pooling reuse the 
 Only what ``se_cotnetd_{50,101,152}`` (:458-483) configure is implemented: deep stem, no stem max-pool, stride 2 in every
 stage, avg-pool down-sampling, optional BlurPool anti-aliasing (152).
 """
+import functools
 import math
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import fused
+from . import dropblock, fused
 from .backbone import StochasticDepth
 from .cot_layer import CoTLayer
 
@@ -57,12 +58,20 @@ class SplitAttnConv2d(nn.Module):
         self.act1 = nn.SiLU(inplace=True)
         self.fc2 = nn.Conv2d(attn_chs, mid_chs, 1, groups=groups)
 
-    def forward(self, x):
-        if self.radix == 1 and self.cardinality == 1 and fused.supported(x):
+    def forward(self, x, drop_block=None):
+        """drop_block: None or a function applied after bn0 (models/layers/split_attn.py:66-67).  With it, a channels_last CUDA
+        input runs bn0 on the fused BatchNorm kernels and the rest of the chain in plain PyTorch."""
+        if self.radix == 1 and self.cardinality == 1 and fused.supported(x) and drop_block is None:
             # channels_last CUDA tensors: everything after the convolution on the fused tail kernels (fused.split_attn_tail)
             u = self.conv(x).contiguous(memory_format=torch.channels_last)
             return fused.split_attn_tail(u, self.bn0, self.fc1, self.bn1, self.fc2)
-        x = self.act0(self.bn0(self.conv(x)))
+        if drop_block is not None and fused.supported(x):
+            x = fused.bn_act(self.conv(x).contiguous(memory_format=torch.channels_last), self.bn0)
+        else:
+            x = self.bn0(self.conv(x))
+        if drop_block is not None:
+            x = drop_block(x)
+        x = self.act0(x)
         B, RC, H, W = x.shape
         if self.radix > 1:
             xr = x.reshape(B, self.radix, RC // self.radix, H, W)
@@ -81,7 +90,8 @@ class SplitAttnConv2d(nn.Module):
 
 
 class CoTBottleneck(nn.Module):
-    """models/cotnet_hybrid.py:118-204 (cardinality 1, base_width 64, no drop block; drop path through forward's drop_scale)."""
+    """models/cotnet_hybrid.py:118-204 (cardinality 1, base_width 64; drop path through forward's drop_scale, DropBlock through its
+    drop_block_key)."""
     expansion = 4
 
     def __init__(self, block_idx, inplanes, planes, stride=1, downsample=None, aa_layer=None, radix=1, avd=False,
@@ -113,38 +123,74 @@ class CoTBottleneck(nn.Module):
         self.act3 = nn.ReLU(inplace=True)
         self.downsample = downsample
         self.stride = stride
+        self.drop_block = None          # the stage's dropblock.DropBlock (set by the trunk)
+        self.drop_block_sites = ()
 
     def zero_init_last_bn(self):
         nn.init.zeros_(self.bn3.weight)
+
+    def drop_block_site_names(self):
+        """bn1, bn0 of a split-attention conv2 (models/cotnet_hybrid.py:146), bn3."""
+        return ("bn1", "conv2.bn0", "bn3") if isinstance(self.conv2, SplitAttnConv2d) else ("bn1", "bn3")
+
+    def set_drop_block(self, spec, site):
+        """Give the block its stage's DropBlock (or None) and its site numbers from `site` on; returns the next free site."""
+        self.drop_block = spec
+        n = 0 if spec is None else len(self.drop_block_site_names())
+        self.drop_block_sites = tuple(range(site, site + n))
+        return site + n
+
+    def _site(self, key, i):
+        """drop_block(., key, site i) of this block, or None without DropBlock."""
+        if key is None:
+            return None
+        return functools.partial(dropblock.drop_block, key=key, site=self.drop_block_sites[i], spec=self.drop_block)
 
     def _pool(self, y):
         if isinstance(self.avd, nn.AvgPool2d) and self.avd.kernel_size == 3 and self.avd.stride == 2 and fused.supported(y):
             return fused.avg_pool3x3s2(y)
         return self.avd(y)
 
-    def forward(self, x, drop_scale=None):
+    def _conv2(self, y, key):
+        if key is not None and isinstance(self.conv2, SplitAttnConv2d):
+            return self.conv2(y, drop_block=self._site(key, 1))
+        return self.conv2(y)
+
+    def forward(self, x, drop_scale=None, drop_block_key=None):
         cl = torch.channels_last
+        key = drop_block_key if self.drop_block is not None else None
         if fused.supported(x):      # channels_last CUDA tensors: fused BatchNorm(+ReLU,+residual) glue like backbone.Bottleneck
             y = fused.conv1x1_bn(x, self.conv1, self.bn1, relu=True)
+            if key is not None:     # on the ReLU output: relu(a)*M*s == relu(a*M*s), s > 0
+                y = self._site(key, 0)(y)
             if self.avd is not None and self.avd_first:
                 y = self._pool(y)
-            y = self.conv2(y.contiguous(memory_format=cl))
+            y = self._conv2(y.contiguous(memory_format=cl), key)
             if self.avd is not None and not self.avd_first:
                 y = self._pool(y.contiguous(memory_format=cl))
             residual = x
             if self.downsample is not None:
                 d = self.downsample
                 residual = fused.conv1x1_bn(d[0](x).contiguous(memory_format=cl), d[1], d[2], relu=False)
+            if key is not None:
+                z = fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=False)
+                return dropblock.drop_block_res_relu(z, residual.contiguous(memory_format=cl), key, self.drop_block_sites[-1],
+                                                     self.drop_block, drop_scale)
             return fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=True,
                                     res=residual.contiguous(memory_format=cl), drop_scale=drop_scale)
         residual = x
-        y = self.act1(self.bn1(self.conv1(x)))
+        y = self.bn1(self.conv1(x))
+        if key is not None:                                                          # :177-178
+            y = self._site(key, 0)(y)
+        y = self.act1(y)
         if self.avd is not None and self.avd_first:
             y = self.avd(y)
-        y = self.conv2(y)
+        y = self._conv2(y, key)
         if self.avd is not None and not self.avd_first:
             y = self.avd(y)
         y = self.bn3(self.conv3(y))
+        if key is not None:                                                          # :191-192
+            y = self._site(key, -1)(y)
         if drop_scale is not None:                                                   # :194-195
             y = y * drop_scale.to(y.dtype).view(-1, 1, 1, 1)
         if self.downsample is not None:
@@ -163,7 +209,7 @@ class CoTHybridNet(StochasticDepth, nn.Module):
     """models/cotnet_hybrid.py:338-452 for stem_type='deep', avg_down=True, output_stride=32."""
 
     def __init__(self, layers, num_classes=1000, in_chans=3, stem_width=64, aa_layer=None, zero_init_last_bn=True,
-                 block_args=None, drop_rate=0., drop_path_rate=0.):
+                 block_args=None, drop_rate=0., drop_path_rate=0., drop_block_rate=0.):
         super().__init__()
         block_args = dict(block_args or {})
         inplanes = stem_width * 2
@@ -184,7 +230,7 @@ class CoTHybridNet(StochasticDepth, nn.Module):
         self.num_features = 2048
         self.global_pool = nn.AdaptiveAvgPool2d(1)
         self.fc = nn.Linear(self.num_features, num_classes)
-        self._init_regularisers(drop_rate, drop_path_rate)
+        self._init_regularisers(drop_rate, drop_path_rate, drop_block_rate)
         for m in self.modules():                                                     # :415-424
             if isinstance(m, nn.Conv2d):
                 nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")

@@ -610,6 +610,37 @@ typedef struct cotb200_erase_box {
 int cotb200_aug_erase(int dtype, int N, int C, int H, int W, void* y, const cotb200_erase* erase_host,
                       const cotb200_erase* erase_dev, void* stream);
 
+/* ---- DropBlock (models/layers/drop.py:drop_block_fast_2d, the fast / per-sample / noise-free form the models build) ----
+ * Random stream.  The library draws its own uniforms rather than torch.rand_like's: for an activation x [B, C, H, W] at site s
+ * (the trunk's DropBlock sites numbered from 0 in forward order) and key = two int64 words in DEVICE memory whose low 32 bits
+ * are k0, k1, element e = ((b*C + c)*H + h)*W + w (the logical NCHW index, whatever the memory layout) draws
+ *   r = lane (e & 3) of Philox4x32-10(counter (q mod 2^32, q >> 32, s, 0), key (k0, k1)),  q = e >> 2
+ *   u = (r >> 8) * 2^-24  (exact in fp32, in [0, 1)),  seed = u < gamma (fp32).
+ * The mask M is 1 - (the OR of the seeds over the cbs x cbs window centred on the element, clipped to the plane), and
+ *   s = fp32(numel) * (1 / (fp32(count) + 1e-7f)),  count = the exact number of kept elements rounded once to fp32,
+ * which is torch's  numel / (mask.float().sum() + 1e-7)  bit for bit while count < 2^24; above that torch's fp32 sum of the mask
+ * is itself rounded and may differ.  Applied, s is first rounded to the activation dtype.
+ *
+ * cotb200_dropblock_mask: mask [B*H*W, C/8] uint8 written, bit c%8 of byte (pixel row, c/8) = M (the layout of the BatchNorm
+ * entry points' 1-bit ReLU masks); count: one int32 in device memory that the call ADDS the kept count to (zero it first).
+ * C % 8 == 0, cbs odd and <= min(H, W), gamma not NaN (a negative gamma, which the reference's formula gives when the block is
+ * larger than the plane, draws no seeds); a plane too large for the kernel's shared memory (H*W above 24560)
+ * is COTB200_EUNSUPPORTED. */
+/* count must be 4-byte and key 8-byte aligned (COTB200_EALIGN), and count must not lie inside mask (COTB200_EINVAL). */
+int cotb200_dropblock_mask(int B, int C, int H, int W, int cbs, float gamma, int site, const long long* key, void* mask,
+                           int* count, void* stream);
+/* y = (x * M) * s on channels_last [B, HW, C] fp32 / bf16 / fp16 (16-byte aligned, C % 8 == 0); numel = B*HW*C.  The same call
+ * is the backward, dx = dy * M * s. */
+int cotb200_dropblock_apply(int dtype, int B, int HW, int C, const void* x, const void* mask, const int* count, void* y,
+                            void* stream);
+/* The site after the last BatchNorm of a bottleneck: y = relu(res + ds[b] * (z * M * s)) in fp32 with one rounding to the dtype,
+ * ds: NULL or [B] fp32 per-sample stochastic-depth scales.  relu_mask [B*HW, C/8] written with the bits [y > 0]. */
+int cotb200_dropblock_res_relu(int dtype, int B, int HW, int C, const void* z, const void* res, const void* mask,
+                               const int* count, const float* ds, void* y, void* relu_mask, void* stream);
+/* Its backward: dres = dy * [y > 0] (dres may be NULL), dz = dres * M * s * ds[b]. */
+int cotb200_dropblock_res_relu_bwd(int dtype, int B, int HW, int C, const void* dy, const void* relu_mask, const void* mask,
+                                   const int* count, const float* ds, void* dres, void* dz, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
