@@ -27,14 +27,8 @@ class AggDesc(ctypes.Structure):
             "x_sn", "x_sp", "w_sn", "w_sp", "y_sn", "y_sp")]
 
 
-class Mix(ctypes.Structure):
-    """struct cotb200_mix (include/cotb200.h): one step's batch Mixup / CutMix parameters."""
-    _fields_ = [("mode", ctypes.c_int), ("lam", ctypes.c_float), ("one_minus_lam", ctypes.c_float), ("target_lam", ctypes.c_float),
-                ("y0", ctypes.c_int), ("y1", ctypes.c_int), ("x0", ctypes.c_int), ("x1", ctypes.c_int)]
-
-
 class MixRow(ctypes.Structure):
-    """struct cotb200_mix_row (include/cotb200.h): the per-sample Mixup / CutMix of one output row."""
+    """struct cotb200_mix_row (include/cotb200.h): the Mixup / CutMix of one output row."""
     _fields_ = [("mode", ctypes.c_int), ("partner", ctypes.c_int), ("lam", ctypes.c_float), ("one_minus_lam", ctypes.c_float),
                 ("target_lam", ctypes.c_float), ("y0", ctypes.c_int), ("y1", ctypes.c_int), ("x0", ctypes.c_int), ("x1", ctypes.c_int)]
 
@@ -144,18 +138,12 @@ SYMBOLS = {
     "cotb200_lookahead_sync": (ctypes.c_int, [ctypes.c_longlong, _VP, _VP, ctypes.POINTER(Opt), _VP]),
     "cotb200_u8_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
                                           _VP, _VP, _VP]),
-    "cotb200_u8_mix_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP, _VP, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
-                                              _VP, _VP, _VP, _VP]),
-    "cotb200_soft_ce": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP, _VP]),
-    "cotb200_soft_ce_bwd": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP, _VP,
-                                                                 ctypes.c_longlong, _VP]),
     "cotb200_u8_mix_rows_to_nhwc": (ctypes.c_int, [ctypes.c_int] * 6 + [_VP, _VP, ctypes.POINTER(ctypes.c_float),
                                                                       ctypes.POINTER(ctypes.c_float), _VP, _VP, ctypes.POINTER(MixRow),
                                                                       _VP, _VP]),
-    "cotb200_soft_ce_rows": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP, ctypes.c_float, _VP, _VP,
-                                                                  _VP]),
-    "cotb200_soft_ce_rows_bwd": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP, ctypes.c_float, _VP,
-                                                                      _VP, _VP, ctypes.c_longlong, _VP]),
+    "cotb200_soft_ce": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP, ctypes.c_float, _VP, _VP, _VP]),
+    "cotb200_soft_ce_bwd": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP, ctypes.c_float, _VP, _VP,
+                                                                 _VP, ctypes.c_longlong, _VP]),
     "cotb200_jsd_ce": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP, ctypes.c_longlong, _VP, ctypes.c_float, ctypes.c_float, _VP, _VP, _VP]),
     "cotb200_jsd_ce_bwd": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP, ctypes.c_longlong, _VP, ctypes.c_float, ctypes.c_float, _VP, _VP,
                                                                 _VP, ctypes.c_longlong, _VP]),
@@ -226,6 +214,28 @@ def stream_ptr(t: torch.Tensor) -> int:
 
 def ptr(t):
     return None if t is None else t.data_ptr()
+
+
+class DeviceCopy:
+    """A device copy of a host table that kernels read (a Mixup / CutMix row table, an erase table).  The copy is made from a
+    freshly pinned buffer of torch's caching host allocator, which does not hand that buffer out again before the copy has
+    finished: the next table never races it.  The copy is issued on the stream current at creation; every consumer takes it
+    through on_stream(), which orders its own current stream after that copy (an event wait) and tells the allocator that stream
+    uses the memory, so creating and consuming on different streams is safe."""
+
+    def __init__(self, host, device):
+        self.dev = torch.frombuffer(bytearray(host), dtype=torch.uint8).pin_memory().to(device, non_blocking=True)
+        self._copied = torch.cuda.Event()
+        self._copied.record(torch.cuda.current_stream(self.dev.device))
+
+    def on_stream(self, device, what):
+        """The device copy, ready for use on `device`'s current stream."""
+        if self.dev.device != torch.device(device):
+            raise ValueError("%s: the device copy lives on %s, not %s" % (what, self.dev.device, device))
+        st = torch.cuda.current_stream(self.dev.device)
+        st.wait_event(self._copied)
+        self.dev.record_stream(st)
+        return self.dev
 
 
 def launch_count() -> int:

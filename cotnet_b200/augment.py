@@ -462,15 +462,12 @@ def run(batch, S, device=None, randaug=True, num_splits=0):
 
 # ---------------------------------------------------------------------------------------------------- random erasing
 class EraseParams:
-    """One batch's erase table (struct cotb200_erase + its boxes) on the host and on the device, ordered like MixParams: the
-    device copy is made from a freshly pinned buffer on the stream current at creation, and on_stream() orders the consumer's
-    current stream after that copy and tells the allocator that stream uses the memory."""
+    """One batch's erase table (struct cotb200_erase + its boxes): `host` the uint8 buffer and its device copy (_lib.DeviceCopy,
+    issued on the stream current at creation), which consumers take through on_stream()."""
 
     def __init__(self, host, device):
         self.host = host
-        self.dev = torch.from_numpy(host.copy()).pin_memory().to(device, non_blocking=True)
-        self._copied = torch.cuda.Event()
-        self._copied.record(torch.cuda.current_stream(self.dev.device))
+        self._copy = _lib.DeviceCopy(host, device)
 
     @property
     def header(self):
@@ -481,12 +478,7 @@ class EraseParams:
         return self.host[ERASE_DTYPE.itemsize:].view(ERASE_BOX_DTYPE)
 
     def on_stream(self, device):
-        st = torch.cuda.current_stream(self.dev.device)
-        if self.dev.device != torch.device(device):
-            raise ValueError("erase: the table lives on %s, not %s" % (self.dev.device, device))
-        st.wait_event(self._copied)
-        self.dev.record_stream(st)
-        return self.dev
+        return self._copy.on_stream(device, "erase")
 
 
 class RandomErasing:

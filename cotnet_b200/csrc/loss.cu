@@ -2,11 +2,10 @@
 // (loss/cross_entropy.py:29-36, datasets/mixup.py:17-27), which the reference selects whenever Mixup / CutMix is on (train.py:198-209).
 //
 // The [B, K] target is never formed.  Its rows sum to one, so per row b
-//   loss_b = lse(z_b) - sum_c t_bc z_bc,   sum_c t_bc z_bc = off*sum_c z_bc + (on - off)*(lam*z_b[y_b] + (1-lam)*z_b[y_{B-1-b}])
+//   loss_b = lse(z_b) - sum_c t_bc z_bc,   sum_c t_bc z_bc = off*sum_c z_bc + (on - off)*(lam*z_b[y_b] + (1-lam)*z_b[y_p])
 // with off = smoothing/K, on = 1 - smoothing + off.  One CTA per row (two passes over the row, the second from L1/L2), then one
-// CTA adds the B row losses in a fixed order: the loss is bit-identical from run to run.  lam = mix->target_lam is read from
-// device memory so that a captured graph follows every step's Mixup / CutMix draw.  The per-sample modes read lam and the partner
-// row y_{partner(b)} from a device table (cotb200_mix_row) instead, through the same kernels.
+// CTA adds the B row losses in a fixed order: the loss is bit-identical from run to run.  lam and the partner p of row b are
+// read from the device table of the Mixup / CutMix draw (cotb200_mix_row), so that a captured graph follows every step's draw.
 //
 // JsdCrossEntropy (loss/jsd.py) of the augmentation splits: label-smoothed cross entropy on the clean split plus alpha/S times
 // the KL divergence of every split's softmax from their clamped mixture.  One CTA per clean row handles its S rows; the row losses
@@ -36,14 +35,12 @@ __device__ __forceinline__ float ce_block_reduce(float v, float* sm, Op op) {
   return t;
 }
 
-// whose label takes the rest of row b's soft target, and row b's own weight: the batch draw (partner B-1-b, one lam; no mixing
-// without it) or the per-sample table (any partner, checked against the n_labels labels: -1 makes the row NaN)
-struct CeBatchMix {
-  const cotb200_mix* mix;
-  int B;
-  __device__ __forceinline__ bool on() const { return mix != nullptr; }
-  __device__ __forceinline__ float lam(int) const { return mix ? mix->target_lam : 1.f; }
-  __device__ __forceinline__ long long partner(int b) const { return B - 1 - b; }
+// whose label takes the rest of row b's soft target, and row b's own weight: no mixing (lam 1, the row's own label alone) or
+// the draw's table (any partner, checked against the n_labels labels: -1 makes the row NaN)
+struct CeNoMix {
+  __device__ __forceinline__ bool on() const { return false; }
+  __device__ __forceinline__ float lam(int) const { return 1.f; }
+  __device__ __forceinline__ long long partner(int b) const { return b; }
 };
 
 struct CeRowMix {
@@ -237,10 +234,12 @@ static int jsd_check(const char* what, int dtype, int S, int B, int K, const voi
 }
 
 static int soft_ce_check(const char* what, int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
-                         const cotb200_mix* mix, float smoothing) {
+                         int n_labels, const cotb200_mix_row* mix_rows, float smoothing) {
   if (!logits || !labels) { set_error("%s: NULL pointer", what); return COTB200_ENULL; }
   if (B <= 0 || K <= 0 || ld < K) { set_error("%s: bad dims B=%d K=%d ld=%lld", what, B, K, ld); return COTB200_EINVAL; }
-  if (mix && (B & 1)) { set_error("%s: batch size %d must be even when mixing", what, B); return COTB200_EINVAL; }
+  if (n_labels < B || (mix_rows && (n_labels & 1))) {
+    set_error("%s: %d labels for %d rows (>= B, and even when mixing)", what, n_labels, B); return COTB200_EINVAL;
+  }
   if (!(smoothing >= 0.f && smoothing < 1.f)) { set_error("%s: smoothing %g outside [0, 1)", what, (double)smoothing); return COTB200_EINVAL; }
   if (dtype == COTB200_F64) { set_error("%s: fp64 not supported", what); return COTB200_EDTYPE; }
   return 0;
@@ -308,9 +307,9 @@ topk_hits_kernel(const T* __restrict__ z, long long ld, const long long* __restr
 
 using namespace cotb200;
 
-extern "C" int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, const cotb200_mix* mix,
-                               float smoothing, float* rows, float* loss, void* stream) {
-  int rc = soft_ce_check("soft_ce", dtype, B, K, logits, ld, labels, mix, smoothing);
+extern "C" int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
+                               const cotb200_mix_row* mix_rows, float smoothing, float* rows, float* loss, void* stream) {
+  int rc = soft_ce_check("soft_ce", dtype, B, K, logits, ld, labels, n_labels, mix_rows, smoothing);
   if (rc) return rc;
   if (!rows || !loss) { set_error("soft_ce: NULL pointer"); return COTB200_ENULL; }
   cudaStream_t st = (cudaStream_t)stream;
@@ -318,7 +317,10 @@ extern "C" int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long
   COTB200_DISPATCH_DTYPE(dtype, {
     if constexpr (!std::is_same<T, double>::value) {
       COTB200_PROF_B("soft_ce", (double)B * K * sizeof(T));
-      soft_ce_rows_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeBatchMix{mix, B}, B, K, off, onoff, rows);
+      if (mix_rows)
+        soft_ce_rows_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeRowMix{mix_rows, n_labels}, B, K, off, onoff, rows);
+      else
+        soft_ce_rows_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeNoMix{}, B, K, off, onoff, rows);
       if ((rc = check_launch("soft_ce"))) return rc;
       soft_ce_mean_kernel<<<1, CE_THREADS, 0, st>>>(rows + B, B, loss);
       return check_launch("soft_ce_mean");
@@ -327,10 +329,10 @@ extern "C" int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long
   return 0;
 }
 
-extern "C" int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
-                                   const cotb200_mix* mix, float smoothing, const float* rows, const float* dloss, float* dz,
+extern "C" int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
+                                   const cotb200_mix_row* mix_rows, float smoothing, const float* rows, const float* dloss, float* dz,
                                    long long ldz, void* stream) {
-  int rc = soft_ce_check("soft_ce_bwd", dtype, B, K, logits, ld, labels, mix, smoothing);
+  int rc = soft_ce_check("soft_ce_bwd", dtype, B, K, logits, ld, labels, n_labels, mix_rows, smoothing);
   if (rc) return rc;
   if (!rows || !dloss || !dz) { set_error("soft_ce_bwd: NULL pointer"); return COTB200_ENULL; }
   if (ldz < K) { set_error("soft_ce_bwd: ldz %lld < K %d", ldz, K); return COTB200_EINVAL; }
@@ -339,57 +341,12 @@ extern "C" int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, 
   COTB200_DISPATCH_DTYPE(dtype, {
     if constexpr (!std::is_same<T, double>::value) {
       COTB200_PROF_B("soft_ce_bwd", (double)B * K * (sizeof(T) + 4));
-      soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeBatchMix{mix, B}, B, K, off, onoff, rows, dloss,
-                                                       dz, ldz);
+      if (mix_rows)
+        soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeRowMix{mix_rows, n_labels}, B, K, off, onoff, rows,
+                                                         dloss, dz, ldz);
+      else
+        soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeNoMix{}, B, K, off, onoff, rows, dloss, dz, ldz);
       return check_launch("soft_ce_bwd");
-    }
-  });
-  return 0;
-}
-
-static int soft_ce_rows_check(const char* what, int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
-                              int n_labels, const cotb200_mix_row* mix_rows, float smoothing) {
-  int rc = soft_ce_check(what, dtype, B, K, logits, ld, labels, nullptr, smoothing);
-  if (rc) return rc;
-  if (!mix_rows) { set_error("%s: NULL row table", what); return COTB200_ENULL; }
-  if (n_labels < B || (n_labels & 1)) { set_error("%s: %d labels for %d rows (an even count >= B)", what, n_labels, B); return COTB200_EINVAL; }
-  return 0;
-}
-
-extern "C" int cotb200_soft_ce_rows(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
-                                    const cotb200_mix_row* mix_rows, float smoothing, float* rows, float* loss, void* stream) {
-  int rc = soft_ce_rows_check("soft_ce_rows", dtype, B, K, logits, ld, labels, n_labels, mix_rows, smoothing);
-  if (rc) return rc;
-  if (!rows || !loss) { set_error("soft_ce_rows: NULL pointer"); return COTB200_ENULL; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const float off = smoothing / (float)K, onoff = 1.f - smoothing;
-  COTB200_DISPATCH_DTYPE(dtype, {
-    if constexpr (!std::is_same<T, double>::value) {
-      COTB200_PROF_B("soft_ce_rows", (double)B * K * sizeof(T));
-      soft_ce_rows_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeRowMix{mix_rows, n_labels}, B, K, off, onoff, rows);
-      if ((rc = check_launch("soft_ce_rows"))) return rc;
-      soft_ce_mean_kernel<<<1, CE_THREADS, 0, st>>>(rows + B, B, loss);
-      return check_launch("soft_ce_rows_mean");
-    }
-  });
-  return 0;
-}
-
-extern "C" int cotb200_soft_ce_rows_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
-                                        const cotb200_mix_row* mix_rows, float smoothing, const float* rows, const float* dloss, float* dz,
-                                        long long ldz, void* stream) {
-  int rc = soft_ce_rows_check("soft_ce_rows_bwd", dtype, B, K, logits, ld, labels, n_labels, mix_rows, smoothing);
-  if (rc) return rc;
-  if (!rows || !dloss || !dz) { set_error("soft_ce_rows_bwd: NULL pointer"); return COTB200_ENULL; }
-  if (ldz < K) { set_error("soft_ce_rows_bwd: ldz %lld < K %d", ldz, K); return COTB200_EINVAL; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const float off = smoothing / (float)K, onoff = 1.f - smoothing;
-  COTB200_DISPATCH_DTYPE(dtype, {
-    if constexpr (!std::is_same<T, double>::value) {
-      COTB200_PROF_B("soft_ce_rows_bwd", (double)B * K * (sizeof(T) + 4));
-      soft_ce_bwd_kernel<T><<<B, CE_THREADS, 0, st>>>((const T*)logits, ld, labels, CeRowMix{mix_rows, n_labels}, B, K, off, onoff, rows,
-                                                       dloss, dz, ldz);
-      return check_launch("soft_ce_rows_bwd");
     }
   });
   return 0;

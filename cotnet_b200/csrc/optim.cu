@@ -13,7 +13,7 @@
 //   cotb200_sgd_ema_step   SGD-momentum(-nesterov) + weight decay + EMA + bf16 shadow over a flat range
 //   cotb200_multi_lerp     EMA of the buffers (BatchNorm running statistics, integer counters) by pointer table
 //   cotb200_u8_to_nhwc     uint8 NCHW batch -> (x - mean)/std in bf16/fp16/fp32 channels_last
-//   cotb200_u8_mix_to_nhwc / cotb200_u8_mix_rows_to_nhwc   the same after Mixup / CutMix, per batch or per sample
+//   cotb200_u8_mix_rows_to_nhwc   the same after Mixup / CutMix, one table row per output sample
 //
 // All HBM-bound streaming kernels: 16-byte accesses, grid = a few waves of 132 SMs, no atomics.
 #include "common.cuh"
@@ -166,12 +166,10 @@ u8_to_nhwc_generic_kernel(const unsigned char* __restrict__ x, T* __restrict__ y
 }
 
 // ------------------------------------------------------------------------------------------------ u8 mix -> NHWC
-// FastCollateMixup._mix_batch_collate (datasets/mixup.py:282-299) on the uint8 batch, fused into the normalisation: the value
-// of sample n at (c, h, w) given its own byte a and the partner's (sample N-1-n) byte p.  Mixup is numpy's fp32 arithmetic
+// FastCollateMixup (datasets/mixup.py:223-299) on the uint8 batch, fused into the normalisation: the value of output row n at
+// (c, h, w) given its own byte a and the byte p of its partner row.  Mixup is numpy's fp32 arithmetic
 // (x.astype(float32)*lam + p.astype(float32)*(1-lam), then np.rint): two roundings of the products, one of the sum, no FMA.
-// M: cotb200_mix (one draw for the batch) or cotb200_mix_row (one per output row); both carry mode, weights and box.
-template <class M>
-__device__ __forceinline__ float mix_px(unsigned a, unsigned p, const M& m, int h, int w) {
+__device__ __forceinline__ float mix_px(unsigned a, unsigned p, const cotb200_mix_row& m, int h, int w) {
   if (m.mode == 0) return (float)a;
   if (m.mode == 1) return rintf(__fadd_rn(__fmul_rn((float)a, m.lam), __fmul_rn((float)p, m.one_minus_lam)));
   if (m.mode == 2) return (h >= m.y0 && h < m.y1 && w >= m.x0 && w < m.x1) ? (float)p : (float)a;
@@ -179,10 +177,10 @@ __device__ __forceinline__ float mix_px(unsigned a, unsigned p, const M& m, int 
 }
 
 // the 4 pixels hw..hw+3 of one image (HW % 4 == 0): own planes at xb, the partner's at xq -> 12 values stored contiguously at o
-template <typename T, class M>
+template <typename T>
 __device__ __forceinline__ void mix4_to_nhwc3(const unsigned char* __restrict__ xb, const unsigned char* __restrict__ xq, long long HW,
-                                              long long hw, int W, const M& m, const float (&mean)[3], const float (&sd)[3],
-                                              T* __restrict__ o) {
+                                              long long hw, int W, const cotb200_mix_row& m, const float (&mean)[3],
+                                              const float (&sd)[3], T* __restrict__ o) {
   float v[12];
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
@@ -200,19 +198,6 @@ __device__ __forceinline__ void mix4_to_nhwc3(const unsigned char* __restrict__ 
 #pragma unroll
     for (int e = 0; e < 4; ++e) q.v[e] = Elem<T>::from(v[k * 4 + e]);
     st_pack<T, 4>(o + k * 4, q);
-  }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256)
-u8_mix_to_nhwc3_kernel(const unsigned char* __restrict__ x, T* __restrict__ y, long long npix4, long long HW, int W, int N,
-                       const cotb200_mix* __restrict__ mix, float m0, float m1, float m2, float d0, float d1, float d2) {
-  const cotb200_mix m = mix ? *mix : cotb200_mix{0, 1.f, 0.f, 1.f, 0, 0, 0, 0};
-  const float mean[3] = {m0, m1, m2}, sd[3] = {d0, d1, d2};
-  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < npix4; i += (long long)gridDim.x * 256) {
-    const long long pix = i * 4;                 // HW % 4 == 0: the 4 pixels lie in one image
-    const long long n = pix / HW, hw = pix - n * HW;
-    mix4_to_nhwc3(x + n * 3 * HW + hw, x + (N - 1 - n) * 3 * HW + hw, HW, hw, W, m, mean, sd, y + pix * 3);
   }
 }
 
@@ -248,20 +233,6 @@ u8_mix_rows_to_nhwc_generic_kernel(const unsigned char* __restrict__ x, T* __res
     const int h = (int)(hw / W), w = (int)(hw - (long long)h * W);
     const cotb200_mix_row r = mix_row(rows, n, N_in);
     const float v = mix_px(x[(n * C + c) * HW + hw], x[((long long)r.partner * C + c) * HW + hw], r, h, w);
-    y[i] = Elem<T>::from((v - __ldg(mean + c)) / __ldg(stdv + c));
-  }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256)
-u8_mix_to_nhwc_generic_kernel(const unsigned char* __restrict__ x, T* __restrict__ y, long long total, int C, long long HW, int W,
-                              int N, const cotb200_mix* __restrict__ mix, const float* __restrict__ mean, const float* __restrict__ stdv) {
-  const cotb200_mix m = mix ? *mix : cotb200_mix{0, 1.f, 0.f, 1.f, 0, 0, 0, 0};
-  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
-    const int c = (int)(i % C);
-    const long long pix = i / C, n = pix / HW, hw = pix - n * HW;
-    const int h = (int)(hw / W), w = (int)(hw - (long long)h * W);
-    const float v = mix_px(x[(n * C + c) * HW + hw], x[((N - 1 - n) * C + c) * HW + hw], m, h, w);
     y[i] = Elem<T>::from((v - __ldg(mean + c)) / __ldg(stdv + c));
   }
 }
@@ -342,35 +313,6 @@ extern "C" int cotb200_u8_to_nhwc(int dtype, int N, int C, int H, int W, const v
         u8_to_nhwc_generic_kernel<T><<<stream_grid(total), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, total, C, HW, mean_dev, std_dev);
       }
       return check_launch("u8_to_nhwc");
-    }
-  });
-  return 0;
-}
-
-extern "C" int cotb200_u8_mix_to_nhwc(int dtype, int N, int C, int H, int W, const void* x_u8, void* y, const float* mean_host,
-                                      const float* std_host, const float* mean_dev, const float* std_dev, const cotb200_mix* mix,
-                                      void* stream) {
-  if (!x_u8 || !y) { set_error("u8_mix_to_nhwc: NULL pointer"); return COTB200_ENULL; }
-  if (N <= 0 || C <= 0 || H <= 0 || W <= 0) { set_error("u8_mix_to_nhwc: non-positive dims"); return COTB200_EINVAL; }
-  if (mix && (N & 1)) { set_error("u8_mix_to_nhwc: batch size %d must be even when mixing", N); return COTB200_EINVAL; }
-  if (dtype == COTB200_F64) { set_error("u8_mix_to_nhwc: fp64 not supported"); return COTB200_EDTYPE; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long HW = (long long)H * W;
-  const bool fast = C == 3 && (HW % 4) == 0 && mean_host && std_host && (reinterpret_cast<uintptr_t>(x_u8) & 3) == 0 && aligned16(y);
-  if (!fast && (!mean_dev || !std_dev)) { set_error("u8_mix_to_nhwc: generic path needs device mean / std arrays"); return COTB200_ENULL; }
-  COTB200_DISPATCH_DTYPE(dtype, {
-    if constexpr (!std::is_same<T, double>::value) {
-      COTB200_PROF_B("u8_mix_to_nhwc", (double)N * C * HW * (2.0 + sizeof(T)));
-      if (fast) {
-        const long long npix4 = (long long)N * HW / 4;
-        u8_mix_to_nhwc3_kernel<T><<<stream_grid(npix4), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, npix4, HW, W, N, mix, mean_host[0],
-                                                                       mean_host[1], mean_host[2], std_host[0], std_host[1], std_host[2]);
-      } else {
-        const long long total = (long long)N * C * HW;
-        u8_mix_to_nhwc_generic_kernel<T><<<stream_grid(total), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, total, C, HW, W, N, mix,
-                                                                              mean_dev, std_dev);
-      }
-      return check_launch("u8_mix_to_nhwc");
     }
   });
   return 0;

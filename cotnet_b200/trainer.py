@@ -482,19 +482,18 @@ class TrainStep:
             return JsdCrossEntropyFn.apply(out, lab, self.jsd_splits, self.label_smoothing, JSD_ALPHA)
         if mix_dev is None and self.label_smoothing == 0.:
             return self.loss_fn(out, lab)
-        per_row = mix_dev is not None and mix_dev.numel() != ctypes.sizeof(_lib.Mix)
-        return SoftTargetCrossEntropyFn.apply(out, lab, mix_dev, self.label_smoothing, per_row)
+        return SoftTargetCrossEntropyFn.apply(out, lab, mix_dev, self.label_smoothing)
 
     def forward_backward(self, x, lab, mix=None):
-        """mix: None, a MixParams / MixRows (MixupCutmix.draw), or its device copy (the 32-byte struct or a row table of 36 bytes
-        per row) -- the loss reads the mixed targets' lam and partners from it.  With a 'half' MixRows, x holds the B/2 mixed
-        images and lab the B labels of the input batch."""
+        """mix: None, a MixRows (MixupCutmix.draw), or its device copy (the row table, 36 bytes per row) -- the loss reads the
+        mixed targets' lam and partners from it.  With a 'half' MixRows, x holds the B/2 mixed images and lab the B labels of
+        the input batch."""
         if self.jsd_splits:
             if mix is not None:
                 raise ValueError("TrainStep: the JSD loss takes augmentation splits, which the reference does not mix (train.py:157)")
             if x.shape[0] % self.jsd_splits:
                 raise ValueError("TrainStep: batch of %d is not %d augmentation splits" % (x.shape[0], self.jsd_splits))
-        mix_dev = mix.on_stream(self.dev) if isinstance(mix, MixParams) else mix
+        mix_dev = mix if mix is None or torch.is_tensor(mix) else mix.on_stream(self.dev)
         if self._cuda:
             fused.step_begin(self.dev)
             # the ~100 `num_batches_tracked += 1` kernels become one multi-tensor add after the forward
@@ -579,8 +578,8 @@ class TrainStep:
     # ------------------------------------------------------------------ CUDA graph
     def capture(self, x, lab, warmup=3, capture_nccl=True, mix=None):
         """Warm up (cuDNN autotune, allocator) and capture the whole step.  Returns a dict describing the launch mode.
-        With `mix` (a MixParams or MixRows) the graph's loss reads a static copy of the mixing parameters that step(mix=)
-        refreshes; the graph then takes draws of that kind and size only."""
+        With `mix` (a MixRows) the graph's loss reads a static copy of the row table that step(mix=) refreshes; the graph then
+        takes tables of that size only (the same output rows from the same input rows)."""
         side = torch.cuda.Stream(device=self.dev)
         side.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(side):
@@ -592,7 +591,7 @@ class TrainStep:
             t.done = None
         self._gx, self._glab = x.clone(), lab.clone()
         self._gmix = None if mix is None else mix.dev.clone()
-        self._gmix_shape = None if mix is None else mix.shape
+        self._gmix_shape = None if mix is None else (mix.n_out, mix.n_in)
         info = {"cuda_graph": True}
         lc0 = _lib.launch_count()
         try:
@@ -639,9 +638,9 @@ class TrainStep:
         if (mix is None) != (self._gmix is None):
             raise ValueError("TrainStep.step: this graph was captured %s mixing parameters; pass mix= %s"
                              % (("without", "to capture() first") if mix is not None else ("with", "(MixupCutmix.draw) at every step")))
-        if mix is not None and mix.shape != self._gmix_shape:
-            raise ValueError("TrainStep.step: this graph was captured with mixing parameters %s, not %s; capture() again for another "
-                             "mode or batch size" % (_mix_kind(self._gmix_shape), _mix_kind(mix.shape)))
+        if mix is not None and (mix.n_out, mix.n_in) != self._gmix_shape:
+            raise ValueError("TrainStep.step: this graph was captured with a table of %d rows from %d images, not %d from %d; "
+                             "capture() again for another mode or batch size" % (self._gmix_shape + (mix.n_out, mix.n_in)))
         if mix is not None:
             self._gmix.copy_(mix.on_stream(self.dev), non_blocking=True)
         if self._graph[0] == "one":
@@ -777,18 +776,14 @@ class TrainStep:
         return out
 
 
-def _mix_kind(shape):
-    return "of one batch draw" if shape[0] == "batch" else "per row (%d rows from %d images)" % shape[1:]
-
-
 def normalize_u8(x_u8, mean, std, dtype=torch.bfloat16, mix=None):
     """uint8 NCHW batch [N,C,H,W] (CUDA) -> (x - mean)/std as a channels_last tensor of `dtype`: the PrefetchLoader's
     normalisation (datasets/loader.py:86-90) + the layout / precision the AMP forward wants, in ONE kernel.
-    mix: a MixParams or MixRows of MixupCutmix.draw -- the batch is Mixup / CutMix-ed first, on the uint8 values, exactly like
+    mix: a MixRows of MixupCutmix.draw -- the batch is Mixup / CutMix-ed first, on the uint8 values, exactly like
     FastCollateMixup (datasets/mixup.py:223-299), in the same kernel.  A MixRows of mode 'half' gives N/2 rows from N."""
     assert x_u8.is_cuda and x_u8.dtype == torch.uint8 and x_u8.dim() == 4 and x_u8.is_contiguous()
     N, C, H, W = x_u8.shape
-    n_out = mix.n_out if isinstance(mix, MixRows) else N
+    n_out = N if mix is None else mix.n_out
     y = torch.empty((n_out, C, H, W), dtype=dtype, device=x_u8.device, memory_format=torch.channels_last)
     mean = [float(m) for m in mean]
     std = [float(s) for s in std]
@@ -804,89 +799,46 @@ def normalize_u8(x_u8, mean, std, dtype=torch.bfloat16, mix=None):
         _lib.check(rc, "u8_to_nhwc")
         return y
     mix.check(N, H, W)
-    if isinstance(mix, MixRows):
-        rc = _lib.load().cotb200_u8_mix_rows_to_nhwc(_lib.dtype_code(y), N, n_out, C, H, W, x_u8.data_ptr(), y.data_ptr(), mh, sh,
-                                                     _lib.ptr(md), _lib.ptr(sd), mix.host, mix.on_stream(x_u8.device).data_ptr(),
-                                                     _lib.stream_ptr(x_u8))
-        _lib.check(rc, "u8_mix_rows_to_nhwc")
-        return y
-    rc = _lib.load().cotb200_u8_mix_to_nhwc(_lib.dtype_code(y), N, C, H, W, x_u8.data_ptr(), y.data_ptr(), mh, sh, _lib.ptr(md),
-                                            _lib.ptr(sd), mix.on_stream(x_u8.device).data_ptr(), _lib.stream_ptr(x_u8))
-    _lib.check(rc, "u8_mix_to_nhwc")
+    rc = _lib.load().cotb200_u8_mix_rows_to_nhwc(_lib.dtype_code(y), N, n_out, C, H, W, x_u8.data_ptr(), y.data_ptr(), mh, sh,
+                                                 _lib.ptr(md), _lib.ptr(sd), mix.host, mix.on_stream(x_u8.device).data_ptr(),
+                                                 _lib.stream_ptr(x_u8))
+    _lib.check(rc, "u8_mix_rows_to_nhwc")
     return y
 
 
 # ---------------------------------------------------------------------------------------------------- the training recipe
-class MixParams:
-    """One step's batch Mixup / CutMix parameters (struct cotb200_mix): `host` holds the values (a ctypes _lib.Mix), `dev` a
-    device copy that the kernels read, `target_lam` the float64 lam of the draw (the struct holds it rounded to fp32).
-    The device copy is made from a freshly pinned buffer of torch's caching host allocator, which does not hand that buffer out
-    again before the copy has finished: the next draw() never races it.  The copy is issued on the stream current at draw();
-    every consumer takes the struct through on_stream(), which orders its own current stream after that copy (an event wait)
-    and tells the allocator that stream uses the memory, so drawing and consuming on different streams is safe."""
-    MODES = (0, 1, 2)
+class MixRows:
+    """One step's Mixup / CutMix (MixupCutmix.draw): `host` a ctypes array of n_out _lib.MixRow (struct cotb200_mix_row), one per
+    output row, mixing input row n with input row host[n].partner out of n_in; `dev` its device copy (_lib.DeviceCopy; None
+    without a device), which the kernels read; `lam` the float64 lam of a batch draw (the rows hold it rounded to fp32), None
+    for per-element draws.  The kernels validate the rows themselves (cotb200_u8_mix_rows_to_nhwc)."""
 
-    def __init__(self, host, device=None, target_lam=None):
-        self.host = host
-        self.target_lam = float(host.target_lam if target_lam is None else target_lam)
-        self._upload(device)
+    def __init__(self, host, n_in, device=None, lam=None):
+        self.host, self.n_in, self.n_out, self.lam = host, int(n_in), len(host), lam
+        self._copy = None if device is None else _lib.DeviceCopy(host, device)
 
-    def _upload(self, device):
-        self.dev = self._copied = None
-        if device is not None:
-            self.dev = torch.frombuffer(bytearray(bytes(self.host)), dtype=torch.uint8).pin_memory().to(device, non_blocking=True)
-            self._copied = torch.cuda.Event()
-            self._copied.record(torch.cuda.current_stream(self.dev.device))
-
-    #: what a graph captured with this draw can take at later steps (TrainStep.step)
-    shape = ("batch",)
-    mode = property(lambda self: self.host.mode)
-    box = property(lambda self: (self.host.y0, self.host.y1, self.host.x0, self.host.x1))
-
-    def check(self, N, H, W):
-        h = self.host
-        if h.mode not in self.MODES:
-            raise ValueError("mix: unknown mode %d (0 none, 1 mixup, 2 cutmix)" % h.mode)
-        if N % 2:
-            raise ValueError("mix: batch size %d must be even (the partner of sample n is N-1-n)" % N)
-        if h.mode == 2 and not (0 <= h.y0 <= h.y1 <= H and 0 <= h.x0 <= h.x1 <= W):
-            raise ValueError("mix: CutMix box %s outside the %dx%d image" % (self.box, H, W))
-
-    def on_stream(self, device):
-        """The device struct, ready for use on `device`'s current stream."""
-        if self.dev is None or self.dev.device != torch.device(device):
-            raise ValueError("mix: no device copy on %s (MixupCutmix(device=...))" % device)
-        st = torch.cuda.current_stream(self.dev.device)
-        st.wait_event(self._copied)
-        self.dev.record_stream(st)
-        return self.dev
-
-
-class MixRows(MixParams):
-    """One step's per-sample Mixup / CutMix ('elem', 'pair', 'half'): `host` a ctypes array of n_out _lib.MixRow (struct
-    cotb200_mix_row), one per output row, mixing input row n with input row host[n].partner out of n_in; `dev` its device copy,
-    made and consumed like MixParams's.  The kernels validate the rows themselves (cotb200_u8_mix_rows_to_nhwc)."""
-
-    def __init__(self, host, n_in, device=None):
-        self.host, self.n_in, self.n_out = host, int(n_in), len(host)
-        self.shape = ("rows", self.n_out, self.n_in)
-        self._upload(device)
-
-    target_lam = property(lambda self: np.array([r.target_lam for r in self.host], dtype=np.float32))
+    dev = property(lambda self: None if self._copy is None else self._copy.dev)
 
     def check(self, N, H, W):
         if N != self.n_in:
             raise ValueError("mix: a batch of %d images for a row table drawn for %d" % (N, self.n_in))
 
+    def on_stream(self, device):
+        """The device table, ready for use on `device`'s current stream."""
+        if self._copy is None:
+            raise ValueError("mix: no device copy on %s (MixupCutmix(device=...))" % device)
+        return self._copy.on_stream(device, "mix")
+
 
 MIX_MODES = ("batch", "pair", "elem", "half")
+_MIX_ROW = np.dtype(_lib.MixRow)
 
 
 class MixupCutmix:
     """Mixup / CutMix of the reference configs (FastCollateMixup, datasets/mixup.py, correct_lam), drawing its parameters from
-    its own np.random.RandomState(seed) in the reference's call order.  mode 'batch' (one draw per batch, a MixParams): rand < prob,
-    rand < switch_prob, beta, then the CutMix box.  'elem' / 'pair' / 'half' (a MixRows): _params_per_elem over B, B/2, B/2
-    elements -- rand(n) < switch_prob and both beta(n) arrays when both alphas are on, rand(n) < prob -- then one box per CutMix
+    its own np.random.RandomState(seed) in the reference's call order, as a MixRows.  mode 'batch' (one draw per batch, the same
+    on every row): rand < prob, rand < switch_prob, beta, then the CutMix box.  'elem' / 'pair' / 'half': _params_per_elem over
+    B, B/2, B/2 elements -- rand(n) < switch_prob and both beta(n) arrays when both alphas are on, rand(n) < prob -- then one box per CutMix
     element in index order; 'half' turns B images into B/2 mixed rows (and B/2 soft targets from the B labels).
     The box: rand_bbox (randint centre row, randint centre column), or with cutmix_minmax = (lo, hi) rand_bbox_minmax (randint
     height, width, top, left), which forces cutmix_alpha to 1 and always corrects lam by the box area (datasets/mixup.py:54-114).
@@ -964,21 +916,23 @@ class MixupCutmix:
         return box, lam
 
     def draw(self, B, H, W):
-        """Parameters of the next batch of B images of H x W: a MixParams (host struct + device copy) in mode 'batch', else a
-        MixRows (host row table + device copy)."""
+        """The MixRows (host row table + device copy) of the next batch of B images of H x W."""
         if B % 2:
             raise ValueError("MixupCutmix: batch size %d must be even" % B)
         if self.mode != "batch":
             return self._draw_rows(B, H, W)
         lam, use_cutmix = self._params_per_batch()
-        m = _lib.Mix()
+        box = (0, 0, 0, 0)
         if use_cutmix:
-            (m.y0, m.y1, m.x0, m.x1), lam = self._cutmix_box(H, W, lam)
-        m.mode = 0 if lam == 1. else (2 if use_cutmix else 1)
+            box, lam = self._cutmix_box(H, W, lam)
+        rows = (_lib.MixRow * B)()
+        r = np.frombuffer(rows, dtype=_MIX_ROW)                     # the same draw on every row, filled without a row loop
+        r["mode"] = 0 if lam == 1. else (2 if use_cutmix else 1)
+        r["partner"] = np.arange(B - 1, -1, -1)
         # numpy 2 weak scalars: float32 pixels * python float multiplies by the float rounded to fp32 (:296)
-        m.lam, m.one_minus_lam = float(np.float32(lam)), float(np.float32(1 - lam))
-        m.target_lam = lam
-        return MixParams(m, self.device, lam)
+        r["lam"], r["one_minus_lam"], r["target_lam"] = np.float32(lam), np.float32(1 - lam), np.float32(lam)
+        r["y0"], r["y1"], r["x0"], r["x1"] = box
+        return MixRows(rows, B, self.device, lam)
 
     def _draw_rows(self, B, H, W):
         """_mix_elem_collate / _mix_pair_collate (datasets/mixup.py:223-280) as a row table.  Each element's lam is fp32, its
@@ -1009,29 +963,23 @@ class MixupCutmix:
 
 class SoftTargetCrossEntropyFn(torch.autograd.Function):
     """SoftTargetCrossEntropy()(logits, mixup_target(labels, K, lam, smoothing)) (loss/cross_entropy.py:29-36,
-    datasets/mixup.py:17-27) on cotb200_soft_ce / cotb200_soft_ce_bwd; lam is read on the device from `mix_dev` (the struct of
-    a MixParams; None = no mixing, i.e. LabelSmoothingCrossEntropy, and plain cross entropy with smoothing 0).  logits
-    [B, K] fp32 / bf16 / fp16 with unit column stride; labels int64 [B].  Returns the fp32 batch mean.
-    per_row: `mix_dev` is the row table of a MixRows (cotb200_soft_ce_rows / _bwd) and labels has n_labels >= B entries (2B in
-    'half'): row b mixes labels[b] with labels[partner of b]."""
+    datasets/mixup.py:17-27) on cotb200_soft_ce / cotb200_soft_ce_bwd; lam and the partners are read on the device from `mix_dev`
+    (the row table of a MixRows; None = no mixing, i.e. LabelSmoothingCrossEntropy, and plain cross entropy with smoothing 0):
+    row b mixes labels[b] with labels[partner of b].  logits [B, K] fp32 / bf16 / fp16 with unit column stride; labels int64
+    [n_labels >= B] (2B in 'half').  Returns the fp32 batch mean."""
 
     @staticmethod
-    def forward(ctx, logits, labels, mix_dev, smoothing, per_row):
+    def forward(ctx, logits, labels, mix_dev, smoothing):
         assert logits.is_cuda and logits.dim() == 2 and logits.stride(1) == 1 and labels.dtype == torch.int64
         B, K = logits.shape
         logits, labels = logits.detach(), labels.contiguous()
         rows = torch.empty(2, B, dtype=torch.float32, device=logits.device)
         loss = torch.empty((), dtype=torch.float32, device=logits.device)
         lib, st, dt = _lib.load(), _lib.stream_ptr(logits), _lib.dtype_code(logits)
-        if per_row:
-            _lib.check(lib.cotb200_soft_ce_rows(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), labels.numel(),
-                                                mix_dev.data_ptr(), float(smoothing), rows.data_ptr(), loss.data_ptr(), st),
-                       "soft_ce_rows")
-        else:
-            _lib.check(lib.cotb200_soft_ce(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), _lib.ptr(mix_dev),
-                                           float(smoothing), rows.data_ptr(), loss.data_ptr(), st), "soft_ce")
+        _lib.check(lib.cotb200_soft_ce(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), labels.numel(), _lib.ptr(mix_dev),
+                                       float(smoothing), rows.data_ptr(), loss.data_ptr(), st), "soft_ce")
         ctx.save_for_backward(logits, labels, mix_dev, rows)
-        ctx.smoothing, ctx.per_row = float(smoothing), bool(per_row)
+        ctx.smoothing = float(smoothing)
         return loss
 
     @staticmethod
@@ -1041,22 +989,17 @@ class SoftTargetCrossEntropyFn(torch.autograd.Function):
         dloss = dloss.float().contiguous()
         dz = torch.empty(B, K, dtype=torch.float32, device=logits.device)
         lib, st, dt = _lib.load(), _lib.stream_ptr(logits), _lib.dtype_code(logits)
-        if ctx.per_row:
-            _lib.check(lib.cotb200_soft_ce_rows_bwd(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), labels.numel(),
-                                                    mix_dev.data_ptr(), ctx.smoothing, rows.data_ptr(), dloss.data_ptr(), dz.data_ptr(),
-                                                    K, st), "soft_ce_rows_bwd")
-        else:
-            _lib.check(lib.cotb200_soft_ce_bwd(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), _lib.ptr(mix_dev),
-                                               ctx.smoothing, rows.data_ptr(), dloss.data_ptr(), dz.data_ptr(), K, st), "soft_ce_bwd")
-        return dz.to(logits.dtype), None, None, None, None
+        _lib.check(lib.cotb200_soft_ce_bwd(dt, B, K, logits.data_ptr(), logits.stride(0), labels.data_ptr(), labels.numel(),
+                                           _lib.ptr(mix_dev), ctx.smoothing, rows.data_ptr(), dloss.data_ptr(), dz.data_ptr(), K, st),
+                   "soft_ce_bwd")
+        return dz.to(logits.dtype), None, None, None
 
 
 def soft_target_cross_entropy(logits, labels, mix=None, smoothing=0.):
-    """The recipe's loss: mean over the batch of -sum_c t_c log softmax(logits)_c with t = mixup_target(labels, K, mix.target_lam,
-    smoothing).  mix: None, a MixParams or a MixRows (MixupCutmix.draw); with a MixRows of mode 'half', labels are the B labels
-    of the B input images and logits the B/2 mixed rows."""
-    return SoftTargetCrossEntropyFn.apply(logits, labels, None if mix is None else mix.on_stream(logits.device), smoothing,
-                                          isinstance(mix, MixRows))
+    """The recipe's loss: mean over the batch of -sum_c t_c log softmax(logits)_c with t = mixup_target(labels, K, lam,
+    smoothing), lam and the partner label per row from mix.  mix: None or a MixRows (MixupCutmix.draw); with a MixRows of mode
+    'half', labels are the B labels of the B input images and logits the B/2 mixed rows."""
+    return SoftTargetCrossEntropyFn.apply(logits, labels, None if mix is None else mix.on_stream(logits.device), smoothing)
 
 
 #: JsdCrossEntropy's alpha as train.py:199-201 builds it (the module's default)

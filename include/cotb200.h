@@ -434,65 +434,46 @@ int cotb200_lookahead_sync(long long n, float* P, void* Pb, const cotb200_opt* o
 int cotb200_u8_to_nhwc(int dtype, int N, int C, int H, int W, const void* x_u8, void* y, const float* mean_host,
                        const float* std_host, const float* mean_dev, const float* std_dev, void* stream);
 
-/* ---- the training recipe of the reference configs: batch Mixup / CutMix and the soft-target loss ----
- * Per-step parameters of FastCollateMixup in batch mode (datasets/mixup.py:143-159,282-299, correct_lam).  The struct lives
- * in DEVICE memory and is read by the kernels, never passed by value, so a captured CUDA graph follows every step's draw.
- *   mode 0: no mixing (lam = 1); 1: mixup; 2: CutMix with the box rows [y0, y1) x columns [x0, x1).
- *   lam, one_minus_lam: the blend weights, each rounded to fp32 from the float64 draw (numpy's weak-scalar rule).
- *   target_lam: the weight of the sample's own label in the soft target (the box-corrected lam for CutMix). */
-typedef struct cotb200_mix {
-  int mode;
-  float lam, one_minus_lam, target_lam;
-  int y0, y1, x0, x1;
-} cotb200_mix;
-/* cotb200_u8_to_nhwc of the mixed batch: sample n is mixed with its partner N-1-n before the normalisation.  mode 1:
- * rint(x_n*lam + x_p*(1-lam)) in fp32 without FMA contraction (ties to even, np.rint); mode 2: x_p's pixels inside the box;
- * mode 0: bit-equal to cotb200_u8_to_nhwc.  N must be even when mix != NULL; mix == NULL means mode 0. */
-int cotb200_u8_mix_to_nhwc(int dtype, int N, int C, int H, int W, const void* x_u8, void* y, const float* mean_host,
-                           const float* std_host, const float* mean_dev, const float* std_dev, const cotb200_mix* mix,
-                           void* stream);
-/* Soft-target cross entropy of SoftTargetCrossEntropy(mixup_target(labels, K, lam, smoothing)) (loss/cross_entropy.py:29-36,
- * datasets/mixup.py:17-27) without materialising the target: per row b, with off = smoothing/K, on = 1 - smoothing + off,
- *   loss_b = lse(z_b) - off*sum_c z_bc - (on - off)*(lam*z_b[y_b] + (1-lam)*z_b[y_{B-1-b}]),  lam = mix->target_lam.
- * mix == NULL: lam = 1 (LabelSmoothingCrossEntropy; with smoothing 0 plain cross entropy).  logits: fp32 / bf16 / fp16
- * [B, K] with row pitch ld; labels int64 [B].  rows: fp32 [2, B] written: rows[b] = lse(z_b) (the backward reads it),
- * rows[B + b] = loss_b.  loss: fp32 [1] written with the batch mean, the rows added in a fixed order.  A label outside
- * [0, K) makes its row (and the mean) NaN; it is never read out of bounds.  An odd B with mix != NULL is rejected. */
-int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, const cotb200_mix* mix,
-                    float smoothing, float* rows, float* loss, void* stream);
-/* dz[b, c] = dloss[0]/B * (softmax(z_b)_c - t_bc), fp32 [B, K] with row pitch ldz; dloss is read from device memory. */
-int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels,
-                        const cotb200_mix* mix, float smoothing, const float* rows, const float* dloss, float* dz,
-                        long long ldz, void* stream);
-/* Per-sample Mixup / CutMix of FastCollateMixup's 'elem', 'pair' and 'half' modes (datasets/mixup.py:123-141,223-280): one
- * row per OUTPUT sample, an array in DEVICE memory read by the kernels like cotb200_mix.  Output row n reads input row n and
- * input row `partner` (its pixels and its label).
+/* ---- the training recipe of the reference configs: Mixup / CutMix and the soft-target loss ----
+ * FastCollateMixup (datasets/mixup.py:123-159,223-299, correct_lam) as a table of one row per OUTPUT sample, an array in DEVICE
+ * memory read by the kernels, never passed by value, so a captured CUDA graph follows every step's draw.  Output row n reads
+ * input row n and input row `partner` (its pixels and its label).  A batch draw ('batch' mode) is the table in which every
+ * row has partner N-1-n and the same mode, weights and box; 'elem', 'pair' and 'half' draw each row on its own.
  *   mode 0: row n unchanged; 1: rint(x_n*lam + x_partner*one_minus_lam); 2: x_partner's pixels in rows [y0, y1) x columns [x0, x1).
  *   lam, one_minus_lam: the fp32 blend weights (numpy's fp32 lam and fp32(1 - lam)).
- *   target_lam: the weight of row n's own label in its soft target, (1 - target_lam) that of row partner's label. */
+ *   target_lam: the weight of row n's own label in its soft target, (1 - target_lam) that of row partner's label (the
+ *   box-corrected lam for CutMix). */
 typedef struct cotb200_mix_row {
   int mode;
   int partner;
   float lam, one_minus_lam, target_lam;
   int y0, y1, x0, x1;
 } cotb200_mix_row;
-/* cotb200_u8_mix_to_nhwc with one cotb200_mix_row per output row: N_in uint8 input rows (even), N_out <= N_in output rows
- * (N_out = N_in / 2 in 'half'), the same per-pixel arithmetic.  rows_host / rows_dev: the same N_out rows on the host
- * (validated) and on the device (read by the kernel).  Rejected with COTB200_EINVAL: odd N_in, N_out outside [1, N_in], a mode
- * other than 0..2, a partner outside [0, N_in), a CutMix box outside the image.  A device row whose partner is outside
- * [0, N_in) is never read out of bounds: its output is NaN. */
+/* cotb200_u8_to_nhwc of the mixed batch: N_in uint8 input rows (even), N_out <= N_in output rows (N_out = N_in / 2 in 'half'),
+ * each row mixed before the normalisation.  mode 1 is computed in fp32 without FMA contraction (two rounded products, a
+ * rounded sum, rint: ties to even, as np.rint); mode 0 is bit-equal to cotb200_u8_to_nhwc.  rows_host / rows_dev: the same
+ * N_out rows on the host (validated) and on the device (read by the kernel).  Rejected with COTB200_EINVAL: odd N_in, N_out
+ * outside [1, N_in], a mode other than 0..2, a partner outside [0, N_in), a CutMix box outside the image.  A device row whose
+ * partner is outside [0, N_in) is never read out of bounds: its output is NaN. */
 int cotb200_u8_mix_rows_to_nhwc(int dtype, int N_in, int N_out, int C, int H, int W, const void* x_u8, void* y,
                                 const float* mean_host, const float* std_host, const float* mean_dev, const float* std_dev,
                                 const cotb200_mix_row* rows_host, const cotb200_mix_row* rows_dev, void* stream);
-/* cotb200_soft_ce / _bwd with the soft target of row b mixing labels[b] (weight mix_rows[b].target_lam) and
- * labels[mix_rows[b].partner] (the rest): B rows of logits, n_labels >= B labels (even; 2B in 'half'), mix_rows: B rows in
- * device memory.  Same row arithmetic and fixed-order mean as cotb200_soft_ce; a partner outside [0, n_labels) or a label
- * outside [0, K) makes its row NaN. */
-int cotb200_soft_ce_rows(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
-                         const cotb200_mix_row* mix_rows, float smoothing, float* rows, float* loss, void* stream);
-int cotb200_soft_ce_rows_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
-                             const cotb200_mix_row* mix_rows, float smoothing, const float* rows, const float* dloss, float* dz,
-                             long long ldz, void* stream);
+/* Soft-target cross entropy of SoftTargetCrossEntropy(mixup_target(labels, K, lam, smoothing)) (loss/cross_entropy.py:29-36,
+ * datasets/mixup.py:17-27) without materialising the target: per row b, with off = smoothing/K, on = 1 - smoothing + off,
+ *   loss_b = lse(z_b) - off*sum_c z_bc - (on - off)*(lam*z_b[y_b] + (1-lam)*z_b[y_p]),
+ * lam = mix_rows[b].target_lam and p = mix_rows[b].partner.  mix_rows: B rows in device memory, or NULL for no mixing
+ * (lam = 1: LabelSmoothingCrossEntropy; with smoothing 0 plain cross entropy).  logits: fp32 / bf16 / fp16 [B, K] with row
+ * pitch ld; labels int64 [n_labels] (2B in 'half').  rows: fp32 [2, B] written: rows[b] = lse(z_b) (the backward reads it),
+ * rows[B + b] = loss_b.  loss: fp32 [1] written with the batch mean, the rows added in a fixed order.  A label outside [0, K)
+ * or a partner outside [0, n_labels) makes its row (and the mean) NaN; neither is read out of bounds.
+ * Argument rules: n_labels >= B always; n_labels even when mix_rows != NULL; 0 <= smoothing < 1; ld >= K (and ldz >= K in
+ * the backward).  NULL operands give COTB200_ENULL, bad dims or smoothing COTB200_EINVAL, fp64 COTB200_EDTYPE. */
+int cotb200_soft_ce(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
+                    const cotb200_mix_row* mix_rows, float smoothing, float* rows, float* loss, void* stream);
+/* dz[b, c] = dloss[0]/B * (softmax(z_b)_c - t_bc), fp32 [B, K] with row pitch ldz; dloss is read from device memory. */
+int cotb200_soft_ce_bwd(int dtype, int B, int K, const void* logits, long long ld, const long long* labels, int n_labels,
+                        const cotb200_mix_row* mix_rows, float smoothing, const float* rows, const float* dloss, float* dz,
+                        long long ldz, void* stream);
 /* JsdCrossEntropy(num_splits=S, alpha, smoothing) (loss/jsd.py) of the augmentation splits.  logits: fp32 / bf16 / fp16
  * [S*B, K] with row pitch ld, split-major (row b + s*B is view s of sample b, view 0 the clean one); labels int64, only the
  * first B read.  Per clean row b, with p_sc = softmax(z_{b+sB})_c and m_c = clamp((sum_{s=0..S-1} p_sc) / S, 1e-7, 1):
@@ -603,7 +584,7 @@ typedef struct cotb200_erase_box {
   int top, left, h, w;
 } cotb200_erase_box;
 /* Erases the boxes in place in y, a channels_last [N, C, H, W] tensor of dtype fp32 / bf16 / fp16 (the output of
- * cotb200_u8_to_nhwc / cotb200_u8_mix_to_nhwc); written values are rounded to the dtype (round to nearest even).  erase_host /
+ * cotb200_u8_to_nhwc / cotb200_u8_mix_rows_to_nhwc); written values are rounded to the dtype (round to nearest even).  erase_host /
  * erase_dev: the same buffer on the host (validated) and on the device (read by the kernel).  Only the erased pixels are
  * touched; n_boxes = 0 launches nothing.  Rejected with COTB200_EINVAL: a bad mode, a box outside its image or the batch, boxes
  * out of order, a sample with more than COTB200_ERASE_MAX_COUNT boxes; COTB200_EDTYPE: another dtype. */

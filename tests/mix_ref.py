@@ -1,6 +1,6 @@
-"""numpy restatement of what a per-sample Mixup / CutMix row table (struct cotb200_mix_row, trainer.MixRows) means: the mixed
-uint8 batch of FastCollateMixup's _mix_elem_collate / _mix_pair_collate (datasets/mixup.py:223-280) and the soft targets of
-mixup_target (:17-27), what cotb200_u8_mix_rows_to_nhwc and cotb200_soft_ce_rows compute.
+"""numpy restatement of what a Mixup / CutMix row table (struct cotb200_mix_row, trainer.MixRows) means: the mixed uint8 batch
+of FastCollateMixup's _mix_batch_collate / _mix_elem_collate / _mix_pair_collate (datasets/mixup.py:223-299) and the soft
+targets of mixup_target (:17-27), what cotb200_u8_mix_rows_to_nhwc and cotb200_soft_ce compute.
 
 rows: a sequence of objects with mode, partner, lam, one_minus_lam, target_lam, y0, y1, x0, x1 (a ctypes array of _lib.MixRow).
 """
@@ -31,3 +31,13 @@ def soft_targets(labels, rows, num_classes, smoothing):
     on = 1.0 - smoothing + off
     eye = np.eye(num_classes) * (on - off) + off
     return np.stack([r.target_lam * eye[labels[n]] + (1.0 - r.target_lam) * eye[labels[r.partner]] for n, r in enumerate(rows)])
+
+
+def batch_row(t, B):
+    """The row of a batch draw: asserts that the table has B rows from B images, that row n's partner is B-1-n and that every
+    row carries row 0's mode, weights and box; returns row 0."""
+    assert (t.n_out, t.n_in) == (B, B) and t.lam is not None
+    r0 = t.host[0]
+    for n, r in enumerate(t.host):
+        assert r.partner == B - 1 - n and bytes(r)[:4] == bytes(r0)[:4] and bytes(r)[8:] == bytes(r0)[8:], n
+    return r0

@@ -216,7 +216,8 @@ def _step_errors(name, monkeypatch):
 @pytest.mark.parametrize("name", ["cotnet50", "se_cotnetd_50"])
 def test_step_matches_reference_golden(name, monkeypatch):
     """The bench path (bf16 weights, autocast, channels_last, one captured graph) with drop_block_rate 0.1 and the fixture's key
-    against the reference's fp64 step with the same uniforms; gates of test_recipe_gpu.test_recipe_step_matches_reference_golden."""
+    against the reference's fp64 step with the same uniforms; gates of
+    test_recipe_gpu.test_recipe_step_with_batch_table_matches_reference_golden."""
     monkeypatch.setattr(torch.backends.cudnn, "allow_tf32", False)
     monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
     loss, lref, lplain, errs, errs_plain = _step_errors(name, monkeypatch)

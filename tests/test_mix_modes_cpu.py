@@ -62,17 +62,18 @@ def test_row_draws_equal_reference(mode, aset, prob):
 
 
 @pytest.mark.parametrize("prob", [1.0, 0.5])
-def test_batch_minmax_draws_equal_reference(prob):
+def test_batch_minmax_tables_equal_reference(prob):
     """Batch mode with cutmix_minmax: the reference's lam (always box-corrected), switch and min-max box, exactly."""
     want = GOLDEN["batch_minmax_%s" % ("p10" if prob == 1.0 else "p05")]
     modes = set()
     for seed, (lam, use_cutmix, yl, yh, xl, xh) in enumerate(want):
         p = trainer.MixupCutmix(0.8, 1.0, prob=prob, seed=seed, device=None, cutmix_minmax=[0.2, 0.8]).draw(8, 128, 128)
-        assert isinstance(p, trainer.MixParams) and p.target_lam == lam, (seed, p.target_lam, lam)
-        assert p.mode == (0 if lam == 1. else (2 if use_cutmix else 1)), seed
-        if p.mode == 2:
-            assert p.box == (yl, yh, xl, xh), seed
-        modes.add(p.mode)
+        r = mix_ref.batch_row(p, 8)
+        assert p.lam == lam and r.target_lam == float(np.float32(lam)), (seed, p.lam, lam)
+        assert r.mode == (0 if lam == 1. else (2 if use_cutmix else 1)), seed
+        if r.mode == 2:
+            assert (r.y0, r.y1, r.x0, r.x1) == (yl, yh, xl, xh), seed
+        modes.add(r.mode)
     assert modes == ({1, 2} if prob == 1.0 else {0, 1, 2})
 
 
@@ -87,16 +88,15 @@ def test_minmax_forces_cutmix_alpha_and_empty_list_is_off():
 
 
 @pytest.mark.parametrize("mode", ("batch",) + MODES)
-def test_disabled_draws_consume_no_random_numbers(mode):
+def test_disabled_draws_are_unmixed_tables_and_consume_no_random_numbers(mode):
     mc = trainer.MixupCutmix(seed=3, device=None, mode=mode, cutmix_minmax=[0.2, 0.8])
     mc.enabled = False
     state = mc.rng.get_state()[1].copy(), mc.rng.get_state()[2]
     t = mc.draw(8, 16, 16)
     assert np.array_equal(mc.rng.get_state()[1], state[0]) and mc.rng.get_state()[2] == state[1]
     if mode == "batch":
-        assert t.mode == 0 and t.target_lam == 1.0
-    else:
-        assert all(r.mode == 0 and r.target_lam == 1.0 for r in t.host)
+        assert mix_ref.batch_row(t, 8).mode == 0 and t.lam == 1.0
+    assert all(r.mode == 0 and r.target_lam == 1.0 for r in t.host)
 
 
 @pytest.mark.parametrize("case", ["%s_%s" % (m, a) for m in MODES for a in ALPHAS] + ["%s_both_generic" % m for m in MODES])
@@ -116,7 +116,7 @@ def test_mix_row_struct():
     assert ctypes.sizeof(_lib.MixRow) == 36
 
 
-def test_row_entry_point_argument_errors():
+def test_row_table_entry_point_argument_errors():
     """NULL operands, odd N, N_out > N_in, a partner or box out of range, a bad mode, n_labels < B: rejected before any launch."""
     lib = _lib.load()
     P = 16
@@ -149,24 +149,26 @@ def test_row_entry_point_argument_errors():
     assert u8(4, 4, table(4), dtype=_lib.F64) == EDTYPE
     assert u8(4, 2, table(2), dtype=_lib.F64) == EDTYPE                    # 'half': the rows pass, only the dtype is refused
     # the loss
-    assert lib.cotb200_soft_ce_rows(_lib.BF16, 4, 10, None, 10, P, 4, P, 0.1, P, P, None) == ENULL
-    assert lib.cotb200_soft_ce_rows(_lib.BF16, 4, 10, P, 10, P, 4, None, 0.1, P, P, None) == ENULL
-    assert lib.cotb200_soft_ce_rows(_lib.BF16, 4, 10, P, 10, P, 4, P, 0.1, None, P, None) == ENULL
-    assert lib.cotb200_soft_ce_rows(_lib.BF16, 4, 10, P, 10, P, 3, P, 0.1, P, P, None) == EINVAL        # n_labels < B
-    assert lib.cotb200_soft_ce_rows(_lib.BF16, 3, 10, P, 10, P, 5, P, 0.1, P, P, None) == EINVAL        # odd n_labels
-    assert lib.cotb200_soft_ce_rows(_lib.BF16, 4, 10, P, 8, P, 4, P, 0.1, P, P, None) == EINVAL         # ld < K
-    assert lib.cotb200_soft_ce_rows(_lib.BF16, 4, 10, P, 10, P, 4, P, 1.0, P, P, None) == EINVAL        # smoothing
-    assert lib.cotb200_soft_ce_rows(_lib.F64, 4, 10, P, 10, P, 8, P, 0.1, P, P, None) == EDTYPE
-    assert lib.cotb200_soft_ce_rows_bwd(_lib.F32, 4, 10, P, 10, P, 4, None, 0.1, P, P, P, 10, None) == ENULL
-    assert lib.cotb200_soft_ce_rows_bwd(_lib.F32, 4, 10, P, 10, P, 4, P, 0.1, P, None, P, 10, None) == ENULL
-    assert lib.cotb200_soft_ce_rows_bwd(_lib.F32, 4, 10, P, 10, P, 4, P, 0.1, P, P, P, 5, None) == EINVAL
-    assert lib.cotb200_soft_ce_rows_bwd(_lib.F32, 4, 10, P, 10, P, 2, P, 0.1, P, P, P, 10, None) == EINVAL
+    assert lib.cotb200_soft_ce(_lib.BF16, 4, 10, None, 10, P, 4, P, 0.1, P, P, None) == ENULL
+    assert lib.cotb200_soft_ce(_lib.BF16, 4, 10, P, 10, None, 4, P, 0.1, P, P, None) == ENULL
+    assert lib.cotb200_soft_ce(_lib.BF16, 4, 10, P, 10, P, 4, P, 0.1, None, P, None) == ENULL
+    assert lib.cotb200_soft_ce(_lib.BF16, 4, 10, P, 10, P, 3, P, 0.1, P, P, None) == EINVAL        # n_labels < B
+    assert lib.cotb200_soft_ce(_lib.BF16, 4, 10, P, 10, P, 3, None, 0.1, P, P, None) == EINVAL     # n_labels < B, no table
+    assert lib.cotb200_soft_ce(_lib.BF16, 3, 10, P, 10, P, 5, P, 0.1, P, P, None) == EINVAL        # odd n_labels
+    assert lib.cotb200_soft_ce(_lib.BF16, 4, 10, P, 8, P, 4, P, 0.1, P, P, None) == EINVAL         # ld < K
+    assert lib.cotb200_soft_ce(_lib.BF16, 4, 10, P, 10, P, 4, P, 1.0, P, P, None) == EINVAL        # smoothing
+    assert lib.cotb200_soft_ce(_lib.F64, 4, 10, P, 10, P, 8, P, 0.1, P, P, None) == EDTYPE
+    assert lib.cotb200_soft_ce_bwd(_lib.F32, 4, 10, P, 10, None, 4, P, 0.1, P, P, P, 10, None) == ENULL
+    assert lib.cotb200_soft_ce_bwd(_lib.F32, 4, 10, P, 10, P, 4, P, 0.1, P, None, P, 10, None) == ENULL
+    assert lib.cotb200_soft_ce_bwd(_lib.F32, 4, 10, P, 10, P, 4, P, 0.1, P, P, P, 5, None) == EINVAL
+    assert lib.cotb200_soft_ce_bwd(_lib.F32, 4, 10, P, 10, P, 2, P, 0.1, P, P, P, 10, None) == EINVAL
+    assert lib.cotb200_soft_ce_bwd(_lib.F32, 3, 10, P, 10, P, 5, P, 0.1, P, P, P, 10, None) == EINVAL  # odd n_labels
     assert lib.cotb200_last_error()
 
 
-def test_row_table_batch_size_and_step_kinds():
+def test_row_table_sizes():
     t = trainer.MixupCutmix(seed=0, device=None, mode="half").draw(8, 16, 16)
-    assert t.shape == ("rows", 4, 8)
+    assert (t.n_out, t.n_in) == (4, 8) and t.lam is None
     with pytest.raises(ValueError, match="drawn for 8"):
         t.check(6, 16, 16)
-    assert trainer.MixupCutmix(seed=0, device=None).draw(8, 16, 16).shape == ("batch",)
+    mix_ref.batch_row(trainer.MixupCutmix(seed=0, device=None).draw(8, 16, 16), 8)

@@ -1,6 +1,6 @@
 """Per-sample Mixup / CutMix on the GPU: cotb200_u8_mix_rows_to_nhwc against the reference's own mixed batches
-(tests/golden/mix_modes.npz) on the fast and the generic path, tied bit for bit to the batch kernel and loss when a table restates
-a batch draw, cotb200_soft_ce_rows against fp64 SoftTargetCrossEntropy, and row tables in a captured training step."""
+(tests/golden/mix_modes.npz) on the fast and the generic path and against the numpy restatement, cotb200_soft_ce with a row table
+against fp64 SoftTargetCrossEntropy, and row tables in a captured training step."""
 import ctypes
 import os
 
@@ -27,23 +27,6 @@ def _rows(n_in, spec):
     return trainer.MixRows(rows, n_in, "cuda")
 
 
-def _batch_mix(mode, lam, box):
-    m = _lib.Mix()
-    m.mode, m.lam, m.one_minus_lam, m.target_lam = mode, float(np.float32(lam)), float(np.float32(1 - lam)), lam
-    m.y0, m.y1, m.x0, m.x1 = box
-    return trainer.MixParams(m, "cuda", lam)
-
-
-def _restated(p, N):
-    """The batch draw p as a row table: partner N-1-n, the same weights and box on every row."""
-    h = p.host
-    rows = (_lib.MixRow * N)()
-    for n, r in enumerate(rows):
-        r.mode, r.partner, r.lam, r.one_minus_lam, r.target_lam = h.mode, N - 1 - n, h.lam, h.one_minus_lam, h.target_lam
-        r.y0, r.y1, r.x0, r.x1 = h.y0, h.y1, h.x0, h.x1
-    return trainer.MixRows(rows, N, "cuda")
-
-
 # ------------------------------------------------------------------------------------------------ input kernel
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("case", ["%s_%s" % (m, a) for m in MODES for a in ALPHAS] + ["%s_both_generic" % m for m in MODES])
@@ -60,9 +43,9 @@ def test_rows_kernel_equals_reference_mixed_batch(case, dtype):
 
 
 @pytest.mark.parametrize("shape", [(8, 3, 16, 20), (4, 3, 15, 19), (4, 5, 8, 8)])
-def test_rows_kernel_mode0_and_batch_restatement(shape):
-    """A table of mode-0 rows equals plain normalize_u8; a table restating a batch draw equals the batch kernel; every row kind
-    together equals the numpy restatement -- fp32 and bf16, bit for bit."""
+def test_rows_kernel_mode0_batch_and_any_partner_tables(shape):
+    """A table of mode-0 rows equals plain normalize_u8; a batch-shaped table (partner N-1-n, one draw on every row) and a table
+    of every row kind with any partners equal the numpy restatement -- fp32 and bf16, bit for bit."""
     N, C, H, W = shape
     x = torch.from_numpy(np.random.RandomState(N * H).randint(0, 256, size=shape).astype(np.uint8)).cuda()
     mean, std = (MEAN + [100.0, 50.0])[:C], (STD + [60.0, 70.0])[:C]
@@ -72,14 +55,11 @@ def test_rows_kernel_mode0_and_batch_restatement(shape):
         plain = trainer.normalize_u8(x, mean, std, dtype)
         zero = _rows(N, [(0, N - 1 - n, 1.0, 1.0, (0, 0, 0, 0)) for n in range(N)])
         assert torch.equal(trainer.normalize_u8(x, mean, std, dtype, mix=zero), plain)
-        for mode, lam in ((1, 0.37), (2, 0.8)):
-            p = _batch_mix(mode, lam, box)
-            assert torch.equal(trainer.normalize_u8(x, mean, std, dtype, mix=_restated(p, N)),
-                               trainer.normalize_u8(x, mean, std, dtype, mix=p))
-        t = _rows(N, spec)
-        want = mix_ref.mixed_batch(x.cpu().numpy(), t.host)
-        assert torch.equal(trainer.normalize_u8(x, mean, std, dtype, mix=t),
-                           trainer.normalize_u8(torch.from_numpy(want).cuda(), mean, std, dtype))
+        batch = [_rows(N, [(mode, N - 1 - n, lam, lam, box) for n in range(N)]) for mode, lam in ((1, 0.37), (2, 0.8))]
+        for t in batch + [_rows(N, spec)]:
+            want = mix_ref.mixed_batch(x.cpu().numpy(), t.host)
+            assert torch.equal(trainer.normalize_u8(x, mean, std, dtype, mix=t),
+                               trainer.normalize_u8(torch.from_numpy(want).cuda(), mean, std, dtype))
 
 
 def test_rows_kernel_device_partner_out_of_range_is_nan():
@@ -122,21 +102,6 @@ def test_soft_ce_rows_matches_fp64(mode, K, B, dtype):
     err = (gz.double() - gd).abs().max().item()
     assert err <= (1e-6 if dtype == torch.float32 else 0.5 ** 8 * gd.abs().max().item() + 1e-6), err
     assert torch.equal(loss, trainer.soft_target_cross_entropy(z, labels, t, 0.1))
-
-
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-def test_soft_ce_rows_restating_a_batch_draw_is_bit_identical(dtype):
-    """A table with partner B-1-b and the batch draw's target lam on every row: the same loss and gradient bits as cotb200_soft_ce."""
-    B, K = 256, 1000
-    g = torch.Generator(device="cuda").manual_seed(11)
-    z = (torch.randn(B, K, generator=g, device="cuda") * 3).to(dtype).requires_grad_(True)
-    labels = torch.randint(0, K, (B,), generator=g, device="cuda")
-    for p in (_batch_mix(1, 0.37, (0, 0, 0, 0)), _batch_mix(2, 0.61, (1, 5, 2, 9))):
-        a = trainer.soft_target_cross_entropy(z, labels, p, 0.1)
-        (ga,) = torch.autograd.grad(a, [z])
-        b = trainer.soft_target_cross_entropy(z, labels, _restated(p, B), 0.1)
-        (gb,) = torch.autograd.grad(b, [z])
-        assert torch.equal(a, b) and torch.equal(ga, gb)
 
 
 def test_soft_ce_rows_partner_out_of_range_is_nan():
@@ -203,8 +168,9 @@ def test_identically_seeded_elem_runs_are_bit_identical(monkeypatch):
     assert all(torch.equal(runs[0][1][k], runs[1][1][k]) for k in runs[0][1])
 
 
-def test_half_step_and_refused_kinds():
-    """'half': B/2 mixed images and the B labels, eager and replayed; a graph refuses a draw of another kind or size."""
+def test_half_step_and_graph_table_sizes(monkeypatch):
+    """'half': B/2 mixed images and the B labels, eager and replayed; a graph refuses a table of another size (output rows,
+    input rows), and a graph captured with a batch draw follows an 'elem' table of its size bit for bit."""
     xu, lab = _batch(6)
     mc = trainer.MixupCutmix(seed=1, mode="half")
     t = mc.draw(8, 96, 96)
@@ -215,14 +181,20 @@ def test_half_step_and_refused_kinds():
     ts.capture(x, lab, warmup=1, mix=t)
     t2 = mc.draw(8, 96, 96)
     assert torch.isfinite(ts.step(trainer.normalize_u8(xu, MEAN, STD, mix=t2), lab, mix=t2))
-    with pytest.raises(ValueError, match="captured with mixing parameters per row"):
+    with pytest.raises(ValueError, match="captured with a table of 4 rows from 8 images, not 8 from 8"):
         ts.step(x, lab, mix=trainer.MixupCutmix(seed=1).draw(8, 96, 96))
-    with pytest.raises(ValueError, match="captured with mixing parameters per row"):
+    with pytest.raises(ValueError, match="captured with a table of 4 rows from 8 images, not 8 from 8"):
         ts.step(x, lab, mix=trainer.MixupCutmix(seed=1, mode="elem").draw(8, 96, 96))
-    tb = trainer.TrainStep(_model(), lr=0.01, label_smoothing=0.1)
+    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
+    tsg, tse = [trainer.TrainStep(_model(), lr=0.0, momentum=0.0, weight_decay=0.0, label_smoothing=0.1) for _ in range(2)]
     p = trainer.MixupCutmix(seed=2).draw(8, 96, 96)
     xb = trainer.normalize_u8(xu, MEAN, STD, mix=p)
-    tb.capture(xb, lab, warmup=1, mix=p)
-    with pytest.raises(ValueError, match="of one batch draw"):
-        tb.step(xb, lab, mix=trainer.MixupCutmix(seed=2, mode="elem").draw(8, 96, 96))
+    tsg.capture(xb, lab, warmup=1, mix=p)
+    tse.step_eager(xb, lab, p)
+    with pytest.raises(ValueError, match="captured with a table of 8 rows from 8 images, not 4 from 8"):
+        tsg.step(xb, lab, mix=t2)
+    e = trainer.MixupCutmix(seed=2, mode="elem").draw(8, 96, 96)
+    xe = trainer.normalize_u8(xu, MEAN, STD, mix=e)
+    lg, le = tsg.step(xe, lab, mix=e).item(), tse.step_eager(xe, lab, e).item()
+    assert lg == le and lg != tse.step_eager(xb, lab, p).item(), (lg, le)
     assert ctypes.sizeof(_lib.MixRow) * 4 == t.dev.numel()

@@ -28,37 +28,39 @@ def _mix_batch(seed):
     return x, rng.randint(0, 1000, size=4).astype(np.int64)
 
 
-def _mix(mode, lam=1.0, box=(0, 0, 0, 0)):
-    m = _lib.Mix()
-    m.mode, m.lam, m.one_minus_lam, m.target_lam = mode, float(np.float32(lam)), float(np.float32(1 - lam)), lam
-    m.y0, m.y1, m.x0, m.x1 = box
-    return trainer.MixParams(m, "cuda", lam)
+def _mix(B, mode, lam=1.0, box=(0, 0, 0, 0)):
+    """A batch draw as MixupCutmix makes it: B rows, partner B-1-n, the same mode, fp32 weights and box on every row."""
+    rows = (_lib.MixRow * B)()
+    for n, r in enumerate(rows):
+        r.mode, r.partner, r.lam, r.one_minus_lam, r.target_lam = mode, B - 1 - n, float(np.float32(lam)), float(np.float32(1 - lam)), lam
+        r.y0, r.y1, r.x0, r.x1 = box
+    return trainer.MixRows(rows, B, "cuda", lam)
 
 
 # ------------------------------------------------------------------------------------------------ Mixup / CutMix input kernel
 @pytest.mark.parametrize("kind", ["mixup", "cutmix"])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-def test_mix_kernel_equals_reference_mixed_batch(kind, dtype):
+def test_batch_table_equals_reference_mixed_batch(kind, dtype):
     """C = 3 fast path: normalize_u8(x, mix=draw) == normalize_u8(the reference's mixed uint8 batch), bit for bit."""
     seed = int(GOLDEN[kind + "_seed"])
     x, _ = _mix_batch(seed)
     p = trainer.MixupCutmix(seed=seed).draw(4, 16, 20)
-    assert p.mode == (1 if kind == "mixup" else 2)
+    assert p.host[0].mode == (1 if kind == "mixup" else 2)
     xd = torch.from_numpy(x).cuda()
     got = trainer.normalize_u8(xd, MEAN, STD, dtype, mix=p)
     want = trainer.normalize_u8(torch.from_numpy(GOLDEN[kind + "_out"]).cuda(), MEAN, STD, dtype)
     assert torch.equal(got, want)
-    assert torch.equal(trainer.normalize_u8(xd, MEAN, STD, dtype, mix=_mix(0)), trainer.normalize_u8(xd, MEAN, STD, dtype))
+    assert torch.equal(trainer.normalize_u8(xd, MEAN, STD, dtype, mix=_mix(4, 0)), trainer.normalize_u8(xd, MEAN, STD, dtype))
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
 @pytest.mark.parametrize("shape", [(4, 3, 15, 19), (2, 5, 8, 8)])
-def test_mix_kernel_generic_path(mode, shape):
+def test_batch_table_generic_path(mode, shape):
     """Generic path (C != 3 or H*W % 4 != 0) against the reference's numpy arithmetic (datasets/mixup.py:291-298)."""
     N, C, H, W = shape
     x = np.random.RandomState(7).randint(0, 256, size=shape).astype(np.uint8)
     lam, box = 0.37 if mode == 1 else 0.8, (3, H - 2, 2, W - 5)
-    p = _mix(mode, lam, box)
+    p = _mix(N, mode, lam, box)
     if mode == 1:
         want = np.rint(x.astype(np.float32) * np.float32(lam) + x[::-1].astype(np.float32) * np.float32(1 - lam)).astype(np.uint8)
     elif mode == 2:
@@ -161,11 +163,11 @@ def _soft_ce_ref(z, labels, lam, smoothing):
 @pytest.mark.parametrize("B", [2, 256])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("lam", [1.0, 0.37])
-def test_soft_ce_matches_fp64(K, B, dtype, lam):
+def test_soft_ce_batch_table_matches_fp64(K, B, dtype, lam):
     g = torch.Generator(device="cuda").manual_seed(K + B)
     z = (torch.randn(B, K, generator=g, device="cuda") * 3).to(dtype).requires_grad_(True)
     labels = torch.randint(0, K, (B,), generator=g, device="cuda")
-    for smoothing, mix in ((0.1, _mix(1, lam)), (0.1, None), (0.0, None)):
+    for smoothing, mix in ((0.1, _mix(B, 1, lam)), (0.1, None), (0.0, None)):
         lam_eff = lam if mix is not None else 1.0
         loss = trainer.soft_target_cross_entropy(z, labels, mix, smoothing)
         (gz,) = torch.autograd.grad(loss * 1.7, [z])
@@ -183,33 +185,33 @@ def test_soft_ce_matches_fp64(K, B, dtype, lam):
         assert torch.equal(loss, again)
 
 
-def test_soft_ce_fp32_gradients_before_the_cast():
+def test_soft_ce_table_fp32_gradients_before_the_cast():
     """The kernel's own fp32 gradient (what the bf16 logits receive before the storage cast) against fp64: <= 1e-6 abs."""
     B, K = 256, 1000
     g = torch.Generator(device="cuda").manual_seed(3)
     z = (torch.randn(B, K, generator=g, device="cuda") * 3).to(torch.bfloat16)
     labels = torch.randint(0, K, (B,), generator=g, device="cuda")
-    mix = _mix(1, 0.37)
+    mix = _mix(B, 1, 0.37)
     lib, st = _lib.load(), torch.cuda.current_stream().cuda_stream
     rows = torch.empty(2, B, device="cuda")
     loss = torch.empty((), device="cuda")
-    _lib.check(lib.cotb200_soft_ce(_lib.BF16, B, K, z.data_ptr(), K, labels.data_ptr(), mix.dev.data_ptr(), 0.1, rows.data_ptr(),
-                                   loss.data_ptr(), st), "soft_ce")
+    _lib.check(lib.cotb200_soft_ce(_lib.BF16, B, K, z.data_ptr(), K, labels.data_ptr(), B, mix.dev.data_ptr(), 0.1,
+                                   rows.data_ptr(), loss.data_ptr(), st), "soft_ce")
     one = torch.ones((), device="cuda")
     dz = torch.empty(B, K, device="cuda")
-    _lib.check(lib.cotb200_soft_ce_bwd(_lib.BF16, B, K, z.data_ptr(), K, labels.data_ptr(), mix.dev.data_ptr(), 0.1, rows.data_ptr(),
-                                       one.data_ptr(), dz.data_ptr(), K, st), "soft_ce_bwd")
+    _lib.check(lib.cotb200_soft_ce_bwd(_lib.BF16, B, K, z.data_ptr(), K, labels.data_ptr(), B, mix.dev.data_ptr(), 0.1,
+                                       rows.data_ptr(), one.data_ptr(), dz.data_ptr(), K, st), "soft_ce_bwd")
     zd = z.double().requires_grad_(True)
     (gd,) = torch.autograd.grad(_soft_ce_ref(zd, labels, 0.37, 0.1), [zd])
     assert (dz.double() - gd).abs().max().item() <= 1e-6
 
 
-def test_soft_ce_invalid_label_is_nan():
+def test_soft_ce_invalid_label_with_or_without_table_is_nan():
     z = torch.randn(4, 10, device="cuda")
     labels = torch.tensor([1, 2, 10, 3], device="cuda")
     assert torch.isnan(trainer.soft_target_cross_entropy(z, labels, None, 0.1))
     labels[2] = -1
-    assert torch.isnan(trainer.soft_target_cross_entropy(z, labels, _mix(1, 0.5), 0.1))
+    assert torch.isnan(trainer.soft_target_cross_entropy(z, labels, _mix(4, 1, 0.5), 0.1))
 
 
 # ------------------------------------------------------------------------------------------------ the recipe in a training step
@@ -224,7 +226,7 @@ def _batch(seed, B=8, res=96):
     return x, torch.randint(0, 100, (B,), generator=g0).cuda()
 
 
-def test_graph_replays_follow_each_steps_mix_and_draw_new_masks(monkeypatch):
+def test_graph_replays_follow_each_steps_batch_table_and_draw_new_masks(monkeypatch):
     """Over 4 replays of one captured step the drop-path scales change; and with fixed masks and lr 0 the replayed loss equals,
     bit for bit, the eager step's loss for each step's target_lam, so the graph reads every step's mixing parameters."""
     monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
@@ -240,22 +242,22 @@ def test_graph_replays_follow_each_steps_mix_and_draw_new_masks(monkeypatch):
     ts = trainer.TrainStep(m, lr=0.0, momentum=0.0, weight_decay=0.0, label_smoothing=0.1)
     xu, lab = _batch(1)
     x = trainer.normalize_u8(xu, MEAN, STD)
-    ts.capture(x, lab, warmup=1, mix=_mix(1, 0.5))
+    ts.capture(x, lab, warmup=1, mix=_mix(8, 1, 0.5))
     graph_scales = seen[-1]
     masks = []
     for lam in (0.2, 0.4, 0.6, 0.8):
-        ts.step(x, lab, mix=_mix(1, lam))
+        ts.step(x, lab, mix=_mix(8, 1, lam))
         masks.append(graph_scales.clone())
     assert len({tuple(t.flatten().tolist()) for t in masks}) == 4
     tsg, tse = [trainer.TrainStep(_model(drop_path_rate=0.5), lr=0.0, momentum=0.0, weight_decay=0.0, label_smoothing=0.1)
                 for _ in range(2)]
     for t in (tsg, tse):
         t.model.fixed_drop_path_scales = torch.tensor([1.0, 0.0, 1.5, 2.0], device="cuda").repeat_interleave(2).view(1, 8).repeat(4, 1)
-    tsg.capture(x, lab, warmup=1, mix=_mix(1, 0.5))
-    tse.step_eager(x, lab, _mix(1, 0.5))
+    tsg.capture(x, lab, warmup=1, mix=_mix(8, 1, 0.5))
+    tse.step_eager(x, lab, _mix(8, 1, 0.5))
     lams = (0.1, 0.3, 0.9, 0.3)
-    lg = [tsg.step(x, lab, mix=_mix(1, lam)).item() for lam in lams]
-    le = [tse.step_eager(x, lab, _mix(1, lam)).item() for lam in lams]
+    lg = [tsg.step(x, lab, mix=_mix(8, 1, lam)).item() for lam in lams]
+    le = [tse.step_eager(x, lab, _mix(8, 1, lam)).item() for lam in lams]
     assert lg == le and len(set(lg)) == 3, (lg, le)
 
 
@@ -300,7 +302,7 @@ def _step_batch(g):
     return u8, y
 
 
-def test_recipe_step_matches_reference_golden(monkeypatch):
+def test_recipe_step_with_batch_table_matches_reference_golden(monkeypatch):
     """The bench.py path (bf16 weights, autocast, channels_last, the whole step replayed from one CUDA graph, gradients from the
     flat bucket) with the recipe -- drop_path_rate 0.1 with the reference's own DropPath masks injected, the batch mixed by
     normalize_u8(mix=) from MixupCutmix's draw, the soft-target loss with smoothing 0.1 -- against one step of the reference's
@@ -316,9 +318,9 @@ def test_recipe_step_matches_reference_golden(monkeypatch):
     y = y.cuda()
     # the draw of the reference's collate, and its mixed batch
     p = trainer.MixupCutmix(seed=int(GOLDEN["step_mix_seed"])).draw(B, R, R)
-    assert p.mode == 1 and p.target_lam == float(GOLDEN["step_lam"])
+    assert p.host[0].mode == 1 and p.lam == float(GOLDEN["step_lam"])
     un = u8.numpy()
-    mixed = np.rint(un.astype(np.float32) * np.float32(p.host.lam) + un[::-1].astype(np.float32) * np.float32(p.host.one_minus_lam))
+    mixed = np.rint(un.astype(np.float32) * np.float32(p.host[0].lam) + un[::-1].astype(np.float32) * np.float32(p.host[0].one_minus_lam))
     assert int(mixed.astype(np.int64).sum()) == int(GOLDEN["step_mixed_sum"])
     xc = trainer.normalize_u8(u8.cuda(), MEAN, STD, torch.bfloat16, mix=p)
     assert torch.equal(xc, trainer.normalize_u8(torch.from_numpy(mixed.astype(np.uint8)).cuda(), MEAN, STD, torch.bfloat16))
@@ -336,7 +338,7 @@ def test_recipe_step_matches_reference_golden(monkeypatch):
     mp_ = copy.deepcopy(m).cuda().train()
     mp_.fixed_drop_path_scales = scales
     with torch.autocast("cuda", dtype=torch.bfloat16):
-        loss_plain = _soft_ce_ref(mp_(xc.float().contiguous()).float(), y, p.target_lam, 0.1)
+        loss_plain = _soft_ce_ref(mp_(xc.float().contiguous()).float(), y, p.lam, 0.1)
     loss_plain.backward()
     errs_plain = _grad_errors({n: q.grad for n, q in mp_.named_parameters()}, g)
     del mp_

@@ -2,9 +2,9 @@
 
     python tools/bench_mix_modes.py [--model cotnet50] [--batch 256] [--res 224] [--launches 200] [--steps 20] [--rounds 3]
 
-* kernel: normalize_u8 of a uint8 3 x res^2 batch to bf16 with a batch draw (cotb200_u8_mix_to_nhwc) and with an 'elem' row table
-  (cotb200_u8_mix_rows_to_nhwc), CUDA events over --launches launches, the two alternating in 5 rounds; bytes/s from the bytes
-  the kernel must move (two uint8 reads and one bf16 write per element; the row reads are not counted).
+* kernel: normalize_u8 of a uint8 3 x res^2 batch to bf16 (cotb200_u8_mix_rows_to_nhwc) with a batch draw's table and with an
+  'elem' table, CUDA events over --launches launches, the two alternating in 5 rounds; bytes/s from the bytes the kernel must
+  move (two uint8 reads and one bf16 write per element; the row reads are not counted).
 * graph: the TrainStep graph step time (bench.py's workload: bf16 weights, autocast, channels_last, cuDNN deterministic, label
   smoothing 0.1) with a new batch draw and with a new 'elem' table every step, in alternating rounds; each round captures its
   own step and frees it before the next.
