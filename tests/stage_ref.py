@@ -1,0 +1,676 @@
+"""Stage-by-stage references of the bf16 training step: a recorder of the autograd functions in cotnet_b200/fused.py and
+cotnet_b200/dropblock.py, fp64 restatements of each stage from the inputs that stage actually received, error bounds derived
+from the fp32 accumulation chains, and a Python mirror of the dispatch predicates that pick the wgmma functions.
+
+Comparing each stage with fp64 of its own recorded inputs keeps bf16 rounding from cascading through batch-statistics BatchNorms,
+so the bounds are as tight as the kernel tests': 1/2 bf16 ulp of the stored value plus the fp32 error of the stage.
+
+Rounding model.  u = 2^-24.  A sequential fp32 sum of n terms (chain length n) is within gamma(n) * sum|terms| of the exact sum,
+gamma(n) = n*u / (1 - n*u), when every add rounds to nearest.  Tensor-core accumulation aligns a k-group's products and truncates,
+so the wgmma and cuDNN convolution chains use gamma_tc(n), the same bound with 2u per add.  Every order of summation of n terms has a chain of at most n, so n = number of terms is a valid
+bound wherever a kernel's order is not pinned here; the wgmma weight gradients pin theirs (wgrad_chain) because a bound over all
+M pixels would let a bf16-rounded weight gradient (relative error 2^-9) pass.
+"""
+import os
+
+import torch
+
+U32 = 2.0 ** -24
+#: abs error of the 16-bit tensors' sigmoid, 0.5 + 0.5*tanh.approx(z/2) (csrc/norm_tail.cu sigmoid_t): tanh.approx.f32 is within
+#: 2^-10.99 absolute, halved by the 0.5 factor, plus the fma; 2^-11 bounds it
+SIGMOID_ERR_16 = 2.0 ** -11
+#: fp32 tensors: __fdividef(1, 1 + __expf(-z)): a few ulp of 1
+SIGMOID_ERR_32 = 2.0 ** -20
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+# ------------------------------------------------------------------------------------------------ rounding and bounds
+def round_mant(x, bits):
+    """Round-to-nearest-even of fp64 values to `bits` significand bits (8 = bfloat16, 24 = float32); normal range only."""
+    x = x.double()
+    m, e = torch.frexp(x)                                 # x = m * 2^e, 0.5 <= |m| < 1
+    r = torch.round(torch.ldexp(m, torch.full_like(e, bits)))      # torch.round: half to even; exact in fp64 for bits <= 52
+    return torch.ldexp(r, e - bits)
+
+
+def bf16(x):
+    return round_mant(x, 8)
+
+
+def f32(x):
+    return round_mant(x, 24)
+
+
+def ulp(x, bits):
+    """unit in the last place at |x| for a `bits`-bit significand (fp64 tensor; zero maps to the smallest normal's ulp)"""
+    e = torch.frexp(x.double().abs().clamp_min(2.0 ** -126))[1]
+    return torch.ldexp(torch.ones_like(x, dtype=torch.float64), e - bits)
+
+
+def gamma(n):
+    """Higham's gamma_n for fp32: the relative bound of an n-term sequential sum, in units of sum|terms|"""
+    nu = n * U32
+    assert nu < 1.0
+    return nu / (1.0 - nu)
+
+
+def gamma_tc(n):
+    """gamma_n with 2u per add: the tensor-core accumulations (wgmma GEMMs, convolutions, weight gradients) align the products of a
+    k-group to the largest exponent and truncate, so one add may cost up to one fp32 ulp instead of half of one"""
+    nu = 2 * n * U32
+    assert nu < 1.0
+    return nu / (1.0 - nu)
+
+
+def store_bound(exact, err, dtype):
+    """|stored - exact| bound of a value computed in fp32 within `err` of `exact` and stored as `dtype` (round to nearest)"""
+    if dtype == torch.float32:
+        return err + 0.5 * ulp(exact.abs() + err, 24)
+    if dtype == torch.bfloat16:
+        return err + 0.5 * ulp(exact.abs() + err, 8)
+    raise ValueError(dtype)
+
+
+def within(got, exact, bound, what):
+    """assert |got - exact| <= bound elementwise; returns the fraction of elements that differ from the correctly rounded exact
+    value (for a bf16 `got`: the one-ulp differences)"""
+    g = got.detach().double()
+    exact = exact.double().to(g.device)
+    bound = torch.as_tensor(bound, dtype=torch.float64, device=g.device).expand_as(exact)
+    err = (g - exact).abs()
+    bad = ~(err <= bound)
+    if bool(bad.any()):
+        i = int(bad.flatten().nonzero()[0])
+        raise AssertionError("%s: %d of %d beyond the bound, e.g. got %r want %r bound %r (max err/bound %.3g)" % (
+            what, int(bad.sum()), g.numel(), g.flatten()[i].item(), exact.flatten()[i].item(), bound.flatten()[i].item(),
+            (err / bound.clamp_min(1e-300)).max().item()))
+    if got.dtype == torch.bfloat16:
+        return float((g != bf16(exact)).double().mean()) if g.numel() else 0.0
+    return 0.0
+
+
+def equal(got, want, what):
+    if not torch.equal(got, want):
+        d = (got.double() - want.double()).abs()
+        raise AssertionError("%s: %d of %d elements differ (max %g), dtypes %s/%s" % (
+            what, int((d != 0).sum()), got.numel(), d.max().item(), got.dtype, want.dtype))
+
+
+# ------------------------------------------------------------------------------------------------ dispatch mirror
+#: The source lines the predicates below restate (tests/test_stage_grads_cpu.py pins them: editing one fails a CPU test).
+SOURCE_ANCHORS = {
+    "cotnet_b200/fused.py": [
+        "if N * (K1 + K2) >= 1024 * 1024 or (N * (K1 + K2) >= 256 * 1024 and M >= 40000):",
+        "and conv.stride == (1, 1) and conv.groups == 1 and conv.bias is None and w.shape[0] % 8 == 0 and w.shape[1] % 8 == 0",
+        "and w.shape[0] * w.shape[1] <= TC_TRUNK_MAX_WEIGHT and x.shape[0] * x.shape[2] * x.shape[3] >= TC_MIN_PIXELS",
+        "return (x.is_cuda and x.dtype == torch.bfloat16 and _is_cl(x) and not x.is_contiguous() and dim % 64 == 0",
+        "and _tc.conv_tile(dim, 4) is not None and x.shape[3] <= 128)",
+        "and x.shape[2] % 2 == 0 and x.shape[3] % 2 == 0 and w.shape[0] % 8 == 0 and w.shape[0] <= 256",
+        "TC_MIN_PIXELS = 100000",
+        "TC_KEY_MAX_DIM = 128",
+        "TC_TRUNK_MAX_WEIGHT = 128 * 1024",
+        "rcode = 0 if not relu else (2 if res is None else (3 if mask is not None else 1))",
+        "rcode = 3 if mask is not None else (2 if res is None else 1)",
+        "rcode = 0 if not relu else (2 if (batch and BN_MASK) else 1)",
+    ],
+    "cotnet_b200/cot_layer.py": [
+        "big = B * H * W >= fused.TC_MIN_PIXELS",
+        "if big and self.dim <= fused.TC_KEY_MAX_DIM and tc_ok and self.key_embed[0].weight.dtype == x.dtype:",
+        "if tc_ok and big:",
+        "if x.dtype == torch.bfloat16 and C % 16 == 0 and k.dtype == x.dtype and w0.dtype == x.dtype:",
+    ],
+    "cotnet_b200/tc.py": [
+        "for bn in (64, 128, 192, 256):",
+        "if C % bn == 0 and (bn % cg == 0):",
+        "if a2 is not None and K1 % 64:",
+    ],
+    "cotnet_b200/csrc/tc_wgrad.cu": [
+        "p.tiles_c = (cc64 + 255) / 256;",
+        "p.tiles_r = (R + WG_BR - 1) / WG_BR;",
+        "int splits = (num_sms() + tiles - 1) / tiles;",
+        "const int max_splits = (p.kb_total + 3) / 4;",
+        "const int per = (p.kb_total + splits - 1) / splits;",
+        "splits = (p.kb_total + per - 1) / per;",
+        "int splits = num_sms();",
+        "if (splits > p.kb_total) splits = p.kb_total;",
+        "for (int s = 0; s < splits; ++s) t += __ldg(part + (size_t)s * n + i);",
+        "if ((H & 1) || (W & 1) || (Wh & 15) || Wh > 128 || (N & 7) || N > 128 || (reinterpret_cast<uintptr_t>(dWm) & 15)) {",
+    ],
+}
+
+TC_MIN_PIXELS = 100000
+TC_KEY_MAX_DIM = 128
+TC_TRUNK_MAX_WEIGHT = 128 * 1024
+
+
+def mm_wgrad(N, K, M):
+    """TcConv1x1Fn takes its weight gradient from torch.mm (bf16 result) instead of the wgmma kernel (fp32)"""
+    return N * K >= 1024 * 1024 or (N * K >= 256 * 1024 and M >= 40000)
+
+
+def conv_tile(C, groups):
+    cg = C // groups
+    for bn in (64, 128, 192, 256):
+        if C % bn == 0 and bn % cg == 0:
+            return bn
+    return None
+
+
+def tc_supported(dim, W):
+    """fused.tc_supported for a bf16 channels_last input of width W"""
+    return dim % 64 == 0 and conv_tile(dim, 4) is not None and W <= 128
+
+
+def conv1x1_tc(cin, cout, M, stride=1, min_pixels=TC_MIN_PIXELS):
+    """fused.conv1x1_bn on a bf16 channels_last input with a bias-free dense 1x1 convolution, under grad"""
+    return stride == 1 and cout % 8 == 0 and cin % 8 == 0 and cin * cout <= TC_TRUNK_MAX_WEIGHT and M >= min_pixels
+
+
+def cot_dispatch(B, dim, H, W, min_pixels=TC_MIN_PIXELS):
+    """CotLayer._forward_fused on bf16: (key conv on wgmma, embed.0 on wgmma, embed.3 and conv1x1 on wgmma)"""
+    tc_ok = tc_supported(dim, W)
+    big = B * H * W >= min_pixels
+    return big and dim <= TC_KEY_MAX_DIM and tc_ok, tc_ok, tc_ok and big
+
+
+def stem_tc(H, W, N):
+    return H % 2 == 0 and W % 2 == 0 and N % 8 == 0 and N <= 256
+
+
+def stem_wgrad_tc(H, W, N):
+    """the stem's weight gradient runs on the wgmma kernel (else cuDNN, bf16 result)"""
+    Wh = W // 2
+    return H % 2 == 0 and W % 2 == 0 and Wh % 16 == 0 and Wh <= 128 and N % 8 == 0 and N <= 128
+
+
+def _wgrad_launch_chain(M, R, Cc, sms):
+    cc64 = (Cc + 63) // 64 * 64
+    tiles_c = (cc64 + 255) // 256
+    tiles_r = (R + 127) // 128
+    kb = (M + 63) // 64
+    tiles = tiles_r * tiles_c
+    splits = max(1, min((sms + tiles - 1) // tiles, (kb + 3) // 4))
+    per = (kb + splits - 1) // splits
+    splits = (kb + per - 1) // per
+    return per * 64 + splits + 1          # pixels of one split in the accumulator, the split-order reduction, the add to OUT
+
+
+def wgrad_chain(M, N, K1, K2, sms):
+    """Longest fp32 chain of one dW element of tc.wgrad_bf16 (csrc/tc_wgrad.cu): a split's pixels, then the partials in split order.
+    Both orientations and the two-launch form are bounded (the larger chain is taken)."""
+    cands = [_wgrad_launch_chain(M, N, K1 + K2, sms), _wgrad_launch_chain(M, K1 + K2, N, sms)]
+    if K2:
+        cands += [_wgrad_launch_chain(M, N, K1, sms), _wgrad_launch_chain(M, K1, N, sms),
+                  _wgrad_launch_chain(M, N, K2, sms), _wgrad_launch_chain(M, K2, N, sms)]
+    return max(cands)
+
+
+def stem_wgrad_chain(B, Ho, Wo, sms):
+    """tc_stem_wgrad: one pipeline stage = one output row (Wo pixels); splits = min(SMs, rows)"""
+    kb = B * Ho
+    splits = min(sms, kb)
+    per = (kb + splits - 1) // splits
+    splits = (kb + per - 1) // per
+    return per * Wo + splits + 1
+
+
+# ------------------------------------------------------------------------------------------------ the recorder
+FUSED_FNS = ("BNActFn", "GroupNorm9Fn", "FanOutFn", "CotTailFn", "AggTapFn", "Pool3x3S2Fn", "TcConv1x1Fn", "TcConv3x3Fn",
+             "StemConvBNFn")
+DROPBLOCK_FNS = ("DropBlockFn", "DropBlockResReluFn")
+
+
+def _snap(v):
+    if isinstance(v, torch.Tensor):
+        return v.detach().clone()
+    if isinstance(v, (tuple, list)):
+        return type(v)(_snap(t) for t in v)
+    return v
+
+
+class Call:
+    """One autograd function application: args (the objects passed), inp (tensor snapshots), out, saved (ctx tensors at the end of
+    the forward), gin (incoming gradients), gout (returned gradients), apply / bwd (captured _bn_apply_batch / _bn_bwd), extra."""
+
+    def __init__(self, name, args):
+        self.name = name
+        self.args = args
+        self.inp = tuple(_snap(a) for a in args)
+        self.out = self.saved = self.gin = self.gout = None
+        self.apply = self.bwd = None
+        self.extra = {}
+
+    def __repr__(self):
+        return "Call(%s)" % self.name
+
+
+class Recorder:
+    """Swaps every fused autograd function for a subclass that calls the parent and records it; wraps _bn_apply_batch and _bn_bwd
+    to capture `pre` / `dpre` and the BatchNorm statistics of the wgmma functions.  Changes no bit and no launch."""
+
+    def __init__(self, monkeypatch):
+        from cotnet_b200 import dropblock, fused
+        self.calls = []
+        self._stack = []
+        for mod, names in ((fused, FUSED_FNS), (dropblock, DROPBLOCK_FNS)):
+            for n in names:
+                monkeypatch.setattr(mod, n, self._subclass(getattr(mod, n)))
+        apply0, bwd0 = fused._bn_apply_batch, fused._bn_bwd
+        rec = self
+
+        def bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds=None, mask=None):
+            cap = dict(x=_snap(x), res=_snap(res), sums=_snap(sums), weight=_snap(weight), bias=_snap(bias), relu=relu, ds=_snap(ds),
+                       eps=bn.eps, rm0=_snap(bn.running_mean), rv0=_snap(bn.running_var), n=x.shape[0] * x.shape[2] * x.shape[3])
+            ss = apply0(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds, mask)
+            cap.update(y=_snap(y), ss=_snap(ss), mask=_snap(mask), rm1=_snap(bn.running_mean), rv1=_snap(bn.running_var),
+                       momentum=bn.momentum, nbt=None if bn.num_batches_tracked is None else int(bn.num_batches_tracked))
+            rec._stack[-1].apply = cap
+            return ss
+
+        def bn_bwd(lib, dt, B, HW, C, dy, x, y, scale, shift, mean, rstd, rcode, sums, batch, inv_n, dx, dres, ds, st):
+            cap = dict(dy=_snap(dy), x=_snap(x), y=_snap(y), scale=_snap(scale), shift=_snap(shift), mean=_snap(mean), rstd=_snap(rstd),
+                       rcode=rcode, batch=batch, inv_n=inv_n, ds=_snap(ds), B=B, HW=HW, C=C)
+            bwd0(lib, dt, B, HW, C, dy, x, y, scale, shift, mean, rstd, rcode, sums, batch, inv_n, dx, dres, ds, st)
+            cap.update(sums=_snap(sums), dx=_snap(dx), dres=_snap(dres))
+            rec._stack[-1].bwd = cap
+        monkeypatch.setattr(fused, "_bn_apply_batch", bn_apply_batch)
+        monkeypatch.setattr(fused, "_bn_bwd", bn_bwd)
+
+    def _subclass(self, cls):
+        rec = self
+
+        class Rec(cls):
+            @staticmethod
+            def forward(ctx, *args):
+                call = Call(cls.__name__, args)
+                rec.calls.append(call)
+                rec._stack.append(call)
+                try:
+                    out = cls.forward(ctx, *args)
+                finally:
+                    rec._stack.pop()
+                call.out = _snap(out)
+                call.out_ptr = tuple(o.data_ptr() for o in (out if isinstance(out, tuple) else (out,)))
+                call.saved = _snap(tuple(getattr(ctx, "to_save", ()) or ()))
+                if cls.__name__ == "CotTailFn":
+                    call.extra["p"] = _snap(ctx.graph[0])
+                    call.extra["training"] = ctx.training
+                ctx._stage_call = call
+                return out
+
+            @staticmethod
+            def backward(ctx, *grads):
+                call = ctx._stage_call
+                call.gin = _snap(grads)
+                rec._stack.append(call)
+                grad0 = torch.autograd.grad
+                if cls.__name__ == "CotTailFn":         # the MLP's backward inside: its incoming S and its fp32 results
+
+                    def grad(outputs, inputs, grad_outputs=None, **kw):
+                        res = grad0(outputs, inputs, grad_outputs=grad_outputs, **kw)
+                        call.extra["S"], call.extra["mlp_grads"] = _snap(grad_outputs), _snap(res)
+                        return res
+                    torch.autograd.grad = grad
+                try:
+                    gout = cls.backward(ctx, *grads)
+                finally:
+                    torch.autograd.grad = grad0
+                    rec._stack.pop()
+                call.gout = _snap(gout)
+                return gout
+
+        Rec.__name__ = Rec.__qualname__ = cls.__name__
+        return Rec
+
+    def named(self, name):
+        return [c for c in self.calls if c.name == name]
+
+
+# ------------------------------------------------------------------------------------------------ fp64 restatements
+def bn_stats_ref(x, n):
+    """fp64 column sums (sum x, sum x^2) of a channels_last [B,C,H,W] tensor and their sum|terms| for the bound"""
+    x = x.double()
+    s0 = x.sum((0, 2, 3))
+    s1 = (x * x).sum((0, 2, 3))
+    return s0, s1, x.abs().sum((0, 2, 3))
+
+
+def bn_apply_ref(x, scale, shift, relu, res=None, ds=None):
+    """y = act(ds[b] * (x*scale + shift) (+ res)) in fp64 from the captured fp32 scale / shift; returns (y, fp32 error bound)"""
+    x = x.double()
+    sc, sh = scale.double().view(1, -1, 1, 1), shift.double().view(1, -1, 1, 1)
+    z = x * sc + sh
+    mag = (x * sc).abs() + sh.abs()
+    if ds is not None:
+        d = ds.double().view(-1, 1, 1, 1)
+        z, mag = z * d, mag * d.abs()
+    if res is not None:
+        z = z + res.double()
+        mag = mag + res.double().abs()
+    return (torch.relu(z) if relu else z), 4 * U32 * mag
+
+
+def bn_bwd_ref(dy, x, gate, scale, mean, rstd, sums_got, batch, ds=None):
+    """BatchNorm backward of y = act(ds*(x*scale+shift) + res) in fp64, with the ReLU decision `gate` (bool, from the library's y)
+    and the captured fp32 statistics.  Returns dict(dres, s0, s1, s_abs, dx, dx_err): dres = dy*gate (exact), s0 / s1 the dbeta /
+    dgamma column sums with their sum|terms| bound inputs, dx from the captured fp32 sums `sums_got` (the stage's own inputs)."""
+    dy = dy.double()
+    g = dy * gate.double() if gate is not None else dy
+    dz = g * (ds.double().view(-1, 1, 1, 1) if ds is not None else 1.0)
+    m, r, sc = mean.double().view(1, -1, 1, 1), rstd.double().view(1, -1, 1, 1), scale.double().view(1, -1, 1, 1)
+    x = x.double()
+    xh = (x - m) * r
+    xh_err = 4 * U32 * (x.abs() + m.abs()) * r                 # the kernels may form xhat as x*rstd - mean*rstd
+    out = dict(dres=g, s0=dz.sum((0, 2, 3)), s1=(dz * xh).sum((0, 2, 3)), s0_abs=dz.abs().sum((0, 2, 3)),
+               s1_abs=(dz.abs() * (xh.abs() + xh_err)).sum((0, 2, 3)) + (dz.abs() * xh_err).sum((0, 2, 3)))
+    if batch:
+        n = x.shape[0] * x.shape[2] * x.shape[3]
+        c0, c1 = sums_got[0].double().view(1, -1, 1, 1) / n, sums_got[1].double().view(1, -1, 1, 1) / n
+        out["dx"] = sc * (dz - c0 - xh * c1)
+        out["dx_err"] = 8 * U32 * sc.abs() * (dz.abs() + c0.abs() + (xh.abs() + 1) * c1.abs()) + sc.abs() * c1.abs() * xh_err
+    else:
+        out["dx"] = sc * dz
+        out["dx_err"] = 2 * U32 * (sc * dz).abs()
+    return out
+
+
+def gemm_ref(a_list, w_list):
+    """sum_i a_i @ w_i^T over NHWC rows, fp64, and sum|terms| ; a_i [B,K,H,W] channels_last, w_i [N,K]"""
+    acc = mag = None
+    for a, w in zip(a_list, w_list):
+        a2 = a.double().permute(0, 2, 3, 1).reshape(-1, a.shape[1])
+        w2 = w.double()
+        t, tm = a2 @ w2.t(), a2.abs() @ w2.abs().t()
+        acc, mag = (t, tm) if acc is None else (acc + t, mag + tm)
+    B, _, H, W = a_list[0].shape
+    N = w_list[0].shape[0]
+    shp = lambda t: t.view(B, H, W, N).permute(0, 3, 1, 2)        # noqa: E731
+    return shp(acc), shp(mag)
+
+
+def rows(t):
+    return t.double().permute(0, 2, 3, 1).reshape(-1, t.shape[1])
+
+
+def gn9_ref(l, lb, gam, beta, mean, rstd, gc, eps):
+    """GroupNorm9Fn forward in fp64 from the recorded logits and the captured fp32 statistics: (out in storage order, bound,
+    xhat in reference order, fp64 mean / rstd of the logits and their bounds)"""
+    B, J, H, W = l.shape
+    wc = J // 9
+    x = (l.double() + (0 if lb is None else lb.double().view(1, -1, 1, 1))).contiguous()
+    xg = x.view(B, wc, 9 * H * W)
+    n = 9 * H * W
+    m64 = xg.mean(2)
+    v64 = ((xg - m64.unsqueeze(2)) ** 2).mean(2)
+    m, r = mean.double().view(B, wc, 1), rstd.double().view(B, wc, 1)
+    xh = ((xg - m) * r).view(B, J, H, W)
+    gm, bt = gam.double().view(1, -1, 1, 1), beta.double().view(1, -1, 1, 1)
+    out = xh * gm + bt
+    err = 8 * U32 * ((x.abs().view(B, wc, -1) + m.abs()) * r).view(B, J, H, W) * gm.abs() + 4 * U32 * bt.abs()
+    # statistics: sums of n terms (gamma(n)); var = E[x^2] - mean^2 in fp32
+    ax = x.abs().view(B, wc, -1)
+    m_err = gamma(n + 1) * ax.mean(2) + 2 * U32 * (lb.double().abs().max() if lb is not None else 0) + U32 * m64.abs()
+    e2 = (xg * xg).mean(2)
+    v_err = gamma(n + 1) * e2 * 2 + 2 * m64.abs() * m_err + 4 * U32 * (e2 + m64 * m64)
+    r64 = 1.0 / torch.sqrt(v64 + eps)
+    r_err = 0.5 * r64 * v_err / (v64 + eps) * 1.01 + 4 * ulp(r64, 24)
+    return to_storage(out, gc), to_storage(err, gc), xh, (m64, m_err, r64, r_err)
+
+
+def to_storage(t, gc):
+    """reference channel order (g*9+t) -> tap-major chunks of gc (COTB200_NHWC_TAP), [B, J, H, W]"""
+    if gc == 0:
+        return t
+    B, J, H, W = t.shape
+    wc = J // 9
+    return t.reshape(B, wc // gc, gc, 9, H, W).permute(0, 1, 3, 2, 4, 5).reshape(B, J, H, W)
+
+
+def from_storage(t, gc):
+    if gc == 0:
+        return t
+    B, J, H, W = t.shape
+    wc = J // 9
+    return t.reshape(B, wc // gc, 9, gc, H, W).permute(0, 1, 3, 2, 4, 5).reshape(B, J, H, W)
+
+
+def gn9_bwd_ref(dg_ref_order, xh, gam, rstd, n_group):
+    """GroupNorm backward in fp64 (reference order): dl, its fp32 error, dgamma, dbeta, dlbias and their sum|terms|"""
+    B, J, H, W = dg_ref_order.shape
+    wc = J // 9
+    dg = dg_ref_order.double().contiguous()
+    gd = dg * gam.double().view(1, -1, 1, 1)
+    g3, x3 = gd.reshape(B, wc, -1), xh.reshape(B, wc, -1)
+    m1 = g3.mean(2, keepdim=True)
+    m2 = (g3 * x3).mean(2, keepdim=True)
+    r = rstd.double().view(B, wc, 1)
+    dl = (r * (g3 - m1 - x3 * m2)).view(B, J, H, W)
+    e_m1 = gamma(n_group + 1) * g3.abs().mean(2, keepdim=True)
+    e_m2 = gamma(n_group + 1) * (g3 * x3).abs().mean(2, keepdim=True) * 2
+    dl_err = (r * (8 * U32 * (g3.abs() + m1.abs() + (x3.abs() + 1) * m2.abs()) + e_m1 + x3.abs() * e_m2)).view(B, J, H, W)
+    return dict(dl=dl, dl_err=dl_err, dgamma=(dg * xh).sum((0, 2, 3)), dbeta=dg.sum((0, 2, 3)), dlbias=dl.sum((0, 2, 3)),
+                dgamma_abs=(dg.abs() * (xh.abs() + 1e-30)).sum((0, 2, 3)), dbeta_abs=dg.abs().sum((0, 2, 3)),
+                dlbias_abs=dl.abs().sum((0, 2, 3)), dlbias_err=dl_err.sum((0, 2, 3)))
+
+
+def _mlp_fwd(p, mods, kind, training):
+    """fp64 forward of the tail MLP with a first-order bound of each fp32 intermediate (dict of values and errors)"""
+    c0, b1, c3 = mods
+    F = torch.nn.functional
+    B, C = p.shape
+    w0, bb0 = c0.weight.detach().double().flatten(1), (c0.bias.detach().double() if c0.bias is not None else 0.0)
+    w3, bb3 = c3.weight.detach().double().flatten(1), (c3.bias.detach().double() if c3.bias is not None else 0.0)
+    p = p.detach().double()
+    z1 = p @ w0.t() + bb0
+    e1 = gamma(w0.shape[1] + 1) * (p.abs() @ w0.abs().t() + (bb0.abs() if torch.is_tensor(bb0) else 0.0))
+    g1, be1 = b1.weight.detach().double(), b1.bias.detach().double()
+    if training:
+        mu = z1.mean(0, keepdim=True)
+        sd = torch.sqrt(z1.var(0, unbiased=False, keepdim=True) + b1.eps)
+        zh = (z1 - mu) / sd
+        e_sd = 2 * e1.max(0, keepdim=True)[0] + 4 * U32 * sd       # any perturbation of the B values moves sd by at most its max
+        e_h = (2 * e1.max(0, keepdim=True)[0] / sd) * (1 + zh.abs()) + 16 * U32 * (zh.abs() + 1)
+    else:
+        sd = torch.sqrt(b1.running_var.double() + b1.eps)
+        zh = (z1 - b1.running_mean.double()) / sd
+        e_sd = 4 * U32 * sd
+        e_h = e1 / sd + 16 * U32 * (zh.abs() + 1)
+    z2 = zh * g1 + be1
+    e2 = e_h * g1.abs() + 4 * U32 * (z2.abs() + be1.abs())
+    if kind == "cot":
+        h, eh = torch.relu(z2), e2
+    else:
+        h, eh = F.silu(z2), 1.1 * e2 + 4 * U32 * z2.abs()
+    z3 = h @ w3.t() + bb3
+    e3 = eh @ w3.abs().t() + gamma(w3.shape[1] + 1) * (h.abs() @ w3.abs().t() + (bb3.abs() if torch.is_tensor(bb3) else 0.0))
+    if kind == "cot":
+        z3, e3 = z3.view(B, C, 2), e3.view(B, C, 2)
+        a = torch.softmax(z3, 2)
+        ea = (0.25 * (e3[..., :1] + e3[..., 1:]) + 8 * U32).expand_as(a)
+    else:
+        g = torch.sigmoid(z3)
+        a = torch.stack([g, torch.zeros_like(g)], 2)
+        ea = torch.stack([0.25 * e3 + 8 * U32, torch.zeros_like(e3)], 2)
+    return dict(p=p, w0=w0, w3=w3, z1=z1, e1=e1, g1=g1, sd=sd, e_sd=e_sd, zh=zh, e_h=e_h, z2=z2, e2=e2, h=h, eh=eh, a=a, ea=ea)
+
+
+def mlp_ref(p, mods, kind, training):
+    """the CoT `se` MLP (+ radix-2 softmax) or the split-attention gate MLP (+ sigmoid) in fp64 on the pooled mean p [B, C], and a
+    first-order bound of the fp32 result.  mods: (conv0, bn, conv3)."""
+    f = _mlp_fwd(p, mods, kind, training)
+    return f["a"], f["ea"]
+
+
+def mlp_bwd_ref(p, S, mods, kind, training):
+    """The tail MLP's backward in fp64 for the incoming gradient S [B, C, 2] (d/da) at the pooled mean p: (dp, [dW0, db0, dgamma1,
+    dbeta1, dW3, db3]) and a first-order bound of each, from the fp32 forward intermediates' bounds (_mlp_fwd) and the rounding of
+    every backward op (gamma(n) for an n-term sum).  A ReLU whose input lies within its bound of zero may take either branch."""
+    f = _mlp_fwd(p, mods, kind, training)
+    U = U32
+    B, C = f["p"].shape
+    a, ea, S = f["a"], f["ea"], S.double()
+    if kind == "cot":                       # softmax backward: a * (S - sum(a*S))
+        aS = (a * S).sum(2, keepdim=True)
+        dz3 = a * (S - aS)
+        aSa = (a * S).abs().sum(2, keepdim=True)
+        e_dz3 = ea * (S.abs() + aSa) + a.abs() * (ea * S.abs()).sum(2, keepdim=True) + 4 * U * a.abs() * (S.abs() + aSa)
+        dz3, e_dz3 = dz3.reshape(B, 2 * C), e_dz3.reshape(B, 2 * C)
+    else:                                   # sigmoid backward on the gate; the stacked zeros take no gradient
+        g, eg, S0 = a[..., 0], ea[..., 0], S[..., 0]
+        dz3 = S0 * g * (1 - g)
+        e_dz3 = S0.abs() * eg * (1 + eg) + 4 * U * dz3.abs()
+    h, eh, w3 = f["h"], f["eh"], f["w3"]
+    dW3 = dz3.t() @ h
+    e_dW3 = e_dz3.t() @ h.abs() + dz3.abs().t() @ eh + gamma(B + 1) * (dz3.abs().t() @ h.abs())
+    db3, e_db3 = dz3.sum(0), e_dz3.sum(0) + gamma(B + 1) * dz3.abs().sum(0)
+    dh = dz3 @ w3
+    e_dh = e_dz3 @ w3.abs() + gamma(w3.shape[0] + 1) * (dz3.abs() @ w3.abs())
+    z2, e2 = f["z2"], f["e2"]
+    if kind == "cot":
+        dz2 = dh * (z2 > 0)
+        e_dz2 = e_dh * (z2 > 0) + dh.abs() * (z2.abs() <= e2)
+    else:
+        sg = torch.sigmoid(z2)
+        dz2 = dh * sg * (1 + z2 * (1 - sg))
+        e_dz2 = 1.1 * e_dh + 0.5 * dh.abs() * e2 + 4 * U * dz2.abs()
+    zh, e_h, g1, sd, e_sd = f["zh"], f["e_h"], f["g1"], f["sd"], f["e_sd"]
+    dg1 = (dz2 * zh).sum(0)
+    e_dg1 = (e_dz2 * zh.abs() + dz2.abs() * e_h).sum(0) + gamma(B + 1) * (dz2 * zh).abs().sum(0)
+    db1, e_db1 = dz2.sum(0), e_dz2.sum(0) + gamma(B + 1) * dz2.abs().sum(0)
+    dzh = dz2 * g1
+    e_dzh = e_dz2 * g1.abs() + U * dzh.abs()
+    if training:
+        m1, m2 = dzh.mean(0, keepdim=True), (dzh * zh).mean(0, keepdim=True)
+        dz1 = (dzh - m1 - zh * m2) / sd
+        e_dz1 = ((e_dzh + e_dzh.mean(0, keepdim=True) + zh.abs() * (e_dzh * zh.abs() + dzh.abs() * e_h).mean(0, keepdim=True)
+                  + e_h * m2.abs() + gamma(B + 1) * (dzh.abs().mean(0, keepdim=True) + zh.abs() * (dzh * zh).abs().mean(0, keepdim=True)))
+                 / sd + dz1.abs() * e_sd / sd + 8 * U * (dzh.abs() + m1.abs() + (zh * m2).abs()) / sd)
+    else:
+        dz1 = dzh / sd
+        e_dz1 = e_dzh / sd + dz1.abs() * e_sd / sd + 4 * U * dz1.abs()
+    pp, w0 = f["p"], f["w0"]
+    dW0 = dz1.t() @ pp
+    e_dW0 = e_dz1.t() @ pp.abs() + gamma(B + 1) * (dz1.abs().t() @ pp.abs())
+    db0, e_db0 = dz1.sum(0), e_dz1.sum(0) + gamma(B + 1) * dz1.abs().sum(0)
+    dp = dz1 @ w0
+    e_dp = e_dz1 @ w0.abs() + gamma(w0.shape[0] + 1) * (dz1.abs() @ w0.abs())
+    return (dp, e_dp), [(dW0, e_dW0), (db0, e_db0), (dg1, e_dg1), (db1, e_db1), (dW3, e_dW3), (db3, e_db3)]
+
+
+def tail_bwd_ref(u, k, scale, shift, mean, rstd, a_c, dout, dpn, training, sig_err):
+    """CotTailFn's backward in fp64 from the recorded u, k, fp32 scale / shift / mean / rstd, attention weights a_c, incoming dout
+    and the MLP's fp32 d/dp (dpn).  Returns dict of S (the per-sample sums the MLP backward takes), dbeta / dgamma, du, dk, each
+    with its bound.  Pooling p = mean(y + k) sends dpn / HW to every pixel of both y and k."""
+    U = U32
+    B, C, H, W = u.shape
+    HW, M = H * W, B * H * W
+    sc, sh = scale.double().view(1, -1, 1, 1), shift.double().view(1, -1, 1, 1)
+    uu, do = u.double(), dout.double()
+    z = uu * sc + sh
+    ze = 4 * U * ((uu * sc).abs() + sh.abs())
+    sg = torch.sigmoid(z)
+    y = z * sg
+    ye = z.abs() * sig_err + 1.1 * ze + 4 * U * y.abs()
+    out = {}
+    out["S0"] = (do * y).sum((2, 3))
+    out["S0_err"] = (do.abs() * ye).sum((2, 3)) + gamma(HW + 1) * (do * y).abs().sum((2, 3))
+    if k is not None:
+        kk = k.double()
+        out["S1"] = (do * kk).sum((2, 3))
+        out["S1_err"] = gamma(HW + 1) * (do * kk).abs().sum((2, 3))
+    a0, a1 = a_c[..., 0].double().view(B, C, 1, 1), a_c[..., 1].double().view(B, C, 1, 1)
+    dpp = dpn.double().view(B, C, 1, 1) / HW
+    dyt = do * a0 + dpp
+    ds = sg * (1 + z * (1 - sg))                                    # silu'
+    dz = dyt * ds
+    e_dz = dyt.abs() * (sig_err * (1 + z.abs()) + 0.5 * ze + 8 * U * ds.abs()) + 4 * U * (do * a0).abs() + 4 * U * dpp.abs()
+    m, r = mean.double().view(1, -1, 1, 1), rstd.double().view(1, -1, 1, 1)
+    xh = (uu - m) * r
+    xh_err = 4 * U * (uu.abs() + m.abs()) * r
+    out["dbeta"] = dz.sum((0, 2, 3))
+    out["dbeta_err"] = e_dz.sum((0, 2, 3)) + gamma(M + 1) * dz.abs().sum((0, 2, 3))
+    out["dgamma"] = (dz * xh).sum((0, 2, 3))
+    out["dgamma_err"] = (e_dz * (xh.abs() + xh_err) + dz.abs() * xh_err).sum((0, 2, 3)) + gamma(M + 1) * (dz * xh).abs().sum((0, 2, 3))
+    if training:
+        c0, c1 = out["dbeta"].view(1, -1, 1, 1) / M, out["dgamma"].view(1, -1, 1, 1) / M
+        e0, e1 = out["dbeta_err"].view(1, -1, 1, 1) / M, out["dgamma_err"].view(1, -1, 1, 1) / M
+        out["du"] = sc * (dz - c0 - xh * c1)
+        out["du_err"] = sc.abs() * (e_dz + e0 + (xh.abs() + xh_err) * e1 + xh_err * c1.abs()
+                                    + 8 * U * (dz.abs() + c0.abs() + (xh.abs() + 1) * c1.abs()))
+    else:
+        out["du"] = sc * dz
+        out["du_err"] = sc.abs() * e_dz + 2 * U * (sc * dz).abs()
+    if k is not None:
+        out["dk"] = do * a1 + dpp
+        out["dk_err"] = 4 * U * ((do * a1).abs() + dpp.abs())
+    return out
+
+
+def agg_ref(v, w, fold, gc):
+    """AggTapFn forward in fp64: out[b,c,p] = sum_t v[b,c,p+off_t] * w[b, wch(c), t, p] with zero padding; and sum|terms|"""
+    B, C, H, W = v.shape
+    J = w.shape[1]
+    wc = J // 9
+    wr = from_storage(w.double(), gc).view(B, wc, 9, H, W)
+    cf = C // fold
+    wcf = wc // fold
+    c = torch.arange(C, device=v.device)
+    wch = (c // cf) * wcf + (c % cf) % wcf
+    vu = torch.nn.functional.unfold(v.double(), 3, padding=1).view(B, C, 9, H, W)
+    wt = wr[:, wch]
+    return (vu * wt).sum(2), (vu.abs() * wt.abs()).sum(2)
+
+
+# ------------------------------------------------------------------------------------------------ expected call lists
+_STAGE1_CUDNN = ["BNActFn(relu)", "FanOutFn(3)", "BNActFn(relu)", "FanOutFn(2)", "TcConv1x1Fn(two,relu)", "BNActFn(plain)",
+                 "GroupNorm9Fn(gc8+lbias)", "AggTapFn(fold1,gc8)", "CotTailFn(k)", "BNActFn(plain)", "BNActFn(relu+res)"]
+_STAGE1_TC = ["TcConv1x1Fn(one,relu)", "FanOutFn(3)", "TcConv3x3Fn", "FanOutFn(2)", "TcConv1x1Fn(two,relu)", "TcConv1x1Fn(one,nobn)",
+              "TcConv1x1Fn(one,bn)", "GroupNorm9Fn(gc8+lbias)", "AggTapFn(fold1,gc8)", "CotTailFn(k)", "TcConv1x1Fn(one,bn)",
+              "TcConv1x1Fn(one,relu+res)"]
+_STAGE4 = [c for c in _STAGE1_CUDNN[:9]] + ["BNActFn(relu+res)"]
+#: Dataflow between recorded calls, "consumer.argument<-producer.output" (x: the block input).  Inputs that come out of a torch
+#: convolution in the glue (cuDNN conv1 / key conv / embed.3 / conv1x1 / downsample / conv3) have no recorded producer.
+_FLOW_STAGE1_CUDNN = ["1.0<-0.0", "3.0<-2.0", "4.0<-1.1", "4.1<-3.0", "7.0<-5.0", "7.1<-6.0", "8.0<-7.0", "8.1<-3.1", "10.3<-9.0"]
+_FLOW_STAGE1_TC = ["0.0<-x", "1.0<-0.0", "2.0<-1.0", "3.0<-2.0", "4.0<-1.1", "4.1<-3.0", "5.0<-4.0", "6.0<-1.2", "7.0<-5.0", "8.0<-6.0",
+                   "8.1<-7.0", "9.0<-8.0", "9.1<-3.1", "10.0<-x", "11.0<-9.0", "11.8<-10.0"]
+#: CoT bottlenecks of cotnet50 (bf16 weights and activations, channels_last, training): geometry, the recorded forward calls and
+#: their dataflow
+BLOCK_CASES = {
+    # the real bench dispatch at the default threshold: B*H*W = 100352 pixels, every 1x1 conv and the key conv on wgmma
+    "stage1_b32": dict(model="cotnet50", block="layer1.0", B=32, cin=64, cout=256, H=56, stride=1, min_pixels=None, calls=_STAGE1_TC,
+                       flow=_FLOW_STAGE1_TC),
+    # 6272 pixels: only embed.0 on wgmma
+    "stage1_b2": dict(model="cotnet50", block="layer1.0", B=2, cin=64, cout=256, H=56, stride=1, min_pixels=None, calls=_STAGE1_CUDNN,
+                      flow=_FLOW_STAGE1_CUDNN),
+    # the golden tests' threshold 0 at the same size
+    "stage1_b2_all_wgmma": dict(model="cotnet50", block="layer1.0", B=2, cin=64, cout=256, H=56, stride=1, min_pixels=0,
+                                calls=_STAGE1_TC, flow=_FLOW_STAGE1_TC),
+    # the stride-2 first block of stage 2: avd average pool, stride-2 downsample on cuDNN
+    "stage2_first_b2": dict(model="cotnet50", block="layer2.0", B=2, cin=256, cout=512, H=28, stride=2, min_pixels=None,
+                            calls=["BNActFn(relu)", "Pool3x3S2Fn(avg)"] + _STAGE1_CUDNN[1:],
+                            flow=["1.0<-0.0", "2.0<-1.0", "4.0<-3.0", "5.0<-2.1", "5.1<-4.0", "8.0<-6.0", "8.1<-7.0", "9.0<-8.0", "9.1<-4.1",
+                                  "11.3<-10.0"]),
+    # a stage-4 block: key conv (dim 512) and every trunk convolution on cuDNN, the residual is the block input
+    "stage4_b2": dict(model="cotnet50", block="layer4.1", B=2, cin=2048, cout=2048, H=7, stride=1, min_pixels=None, calls=_STAGE4,
+                      flow=_FLOW_STAGE1_CUDNN[:-1] + ["9.3<-x"]),
+}
+
+
+def bottleneck_calls(B, cin, width, cout, H, stride, min_pixels=TC_MIN_PIXELS):
+    """the forward calls of backbone.Bottleneck._forward_fused with a CotLayer, from the dispatch predicates above"""
+    M = B * H * H
+    Ho = H // stride
+    out = ["TcConv1x1Fn(one,relu)" if conv1x1_tc(cin, width, M, 1, min_pixels) else "BNActFn(relu)"]
+    if stride > 1:
+        out.append("Pool3x3S2Fn(avg)")
+    key_tc, e0_tc, rest_tc = cot_dispatch(B, width, Ho, Ho, min_pixels)
+    out += ["FanOutFn(3)", "TcConv3x3Fn" if key_tc else "BNActFn(relu)", "FanOutFn(2)",
+            "TcConv1x1Fn(two,relu)" if e0_tc else "BNActFn(relu)"]
+    out += ["TcConv1x1Fn(one,nobn)", "TcConv1x1Fn(one,bn)"] if rest_tc else ["BNActFn(plain)"]
+    gc = 8 if (width // 8) % 8 == 0 else 0
+    out += ["GroupNorm9Fn(gc%d+lbias)" % gc, "AggTapFn(fold1,gc%d)" % gc, "CotTailFn(k)"]
+    if stride > 1 or cin != cout:
+        out.append("TcConv1x1Fn(one,bn)" if conv1x1_tc(cin, cout, B * Ho * Ho, stride, min_pixels) else "BNActFn(plain)")
+    out.append("TcConv1x1Fn(one,relu+res)" if conv1x1_tc(width, cout, B * Ho * Ho, 1, min_pixels) else "BNActFn(relu+res)")
+    return out
