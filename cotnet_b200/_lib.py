@@ -47,7 +47,7 @@ class ClipSeg(ctypes.Structure):
 
 
 class Clip(ctypes.Structure):
-    """struct cotb200_clip (include/cotb200.h): the clip of one cotb200_sgd_ema_step_clip call."""
+    """struct cotb200_clip (include/cotb200.h): the clip of one cotb200_opt_step call."""
     _fields_ = [("mode", ctypes.c_int), ("value", ctypes.c_float), ("factor", ctypes.c_void_p), ("segs", ctypes.c_void_p),
                 ("n_segs", ctypes.c_int), ("pad_", ctypes.c_int)]
 
@@ -124,14 +124,11 @@ SYMBOLS = {
     "cotb200_se_eval": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_float] + [_VP] * 9),
     "cotb200_gather_chunk": (ctypes.c_int, []),
     "cotb200_multi_gather": (ctypes.c_int, [_VP, _VP, ctypes.c_int, ctypes.c_int, _VP, ctypes.c_float, _VP]),
-    "cotb200_sgd_ema_step": (ctypes.c_int, [ctypes.c_longlong, _VP, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP]),
     "cotb200_multi_lerp": (ctypes.c_int, [_VP, ctypes.c_int, _VP, _VP]),
     "cotb200_clip_seg_max": (ctypes.c_int, []),
     "cotb200_grad_norm": (ctypes.c_int, [ctypes.c_longlong, ctypes.c_int, _VP, _VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP]),
     "cotb200_unit_norms": (ctypes.c_int, [ctypes.c_int, _VP, ctypes.c_longlong, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, ctypes.c_float,
                                           _VP, _VP, _VP]),
-    "cotb200_sgd_ema_step_clip": (ctypes.c_int, [ctypes.c_longlong, _VP, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int,
-                                                 ctypes.POINTER(Clip), _VP]),
     "cotb200_opt_prepare": (ctypes.c_int, [ctypes.POINTER(Opt), _VP, ctypes.c_int, _VP]),
     "cotb200_opt_step": (ctypes.c_int, [ctypes.c_longlong, _VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.POINTER(Opt), ctypes.POINTER(Clip),
                                         _VP]),

@@ -7,8 +7,8 @@
 //   cotb200_grad_norm          NORM: N = ||g'|| over both buckets, one launch, deterministic (det_finish); f = min(1, c/(N+1e-6))
 //   cotb200_unit_norms         AGC: ||P_u||, ||g'_u|| and the factor of every unit, one warp per unit
 //
-// The update passes that apply the factors -- cotb200_sgd_ema_step_clip and cotb200_opt_step -- are in opt.cu.  With a factor of 1
-// or a clamp that does not bind, g' goes into the update unchanged: the same arithmetic, bit for bit, as cotb200_sgd_ema_step.
+// The update pass that applies the factors, cotb200_opt_step, is in opt.cu.  With a factor of 1 or a clamp that does not bind, g'
+// goes into the update unchanged: the same arithmetic, bit for bit, as the pass without a clip.
 #include "common.cuh"
 
 namespace cotb200 {

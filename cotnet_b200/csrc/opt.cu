@@ -3,12 +3,12 @@
 // One streaming pass per flat range for every update rule the library runs: read G*grad_scale, clip it (clip.cu makes the
 // factors), apply the rule, the Lookahead synchronisation when this step has one, the EMA of the final weights
 // (train.py:276-277) and the bf16 shadow.  The walkers -- a grid-stride float4 loop for no clip / norm / value, one warp per
-// segment for AGC -- are templated on the rule; the SGD instantiations are the arithmetic of cotb200_sgd_ema_step.
+// segment for AGC -- are templated on the rule.
 //
-//   cotb200_opt_prepare        one thread: advance the step counter t and compute what depends only on t and lr (fp64)
+//   cotb200_opt_prepare        one thread: advance the step counter t and compute what depends only on t and lr (fp64); plain
+//                              SGD / momentum without Lookahead needs none of it and runs on the state as initialised
 //   cotb200_opt_step           the pass, any rule, any clip mode (cotb200_clip, nullable)
 //   cotb200_lookahead_sync     Lookahead.sync_lookahead (train.py:295-296): S += alpha (P - S); P = S; the bf16 shadow
-//   cotb200_sgd_ema_step_clip  the SGD pass with a clip (clip.cu's entry point; no counter, no Lookahead)
 //
 // Everything depending on the step lives in device memory (hyper, cotb200_opt_state): a captured CUDA graph follows the LR
 // schedule and the bias corrections, and a replay computes exactly what an eager step computes.
@@ -28,7 +28,7 @@ __device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return
 
 template <bool NESTEROV>
 __device__ __forceinline__ void sgd_elem(float& p, float& m, float gc, float lr, float mu, float wd) {
-  const float g = fmaf(wd, p, gc);                // gc replaces grad*gscale of sgd_ema_kernel (optim.cu)
+  const float g = fmaf(wd, p, gc);                // gc: the clipped grad*gscale
   m = fmaf(mu, m, g);
   const float st = NESTEROV ? fmaf(mu, m, g) : m;
   p = fmaf(-lr, st, p);
@@ -50,7 +50,7 @@ struct OptArgs {
   const TG* G;
   __nv_bfloat16* Pb;
   const float* hyper;                                      // {lr, momentum, weight_decay, ema_decay, grad_scale}
-  const cotb200_opt_state* state;                          // NULL: plain SGD pass (no coefficients, no Lookahead)
+  const cotb200_opt_state* state;
   float eps, la;
 };
 
@@ -351,7 +351,7 @@ static OptArgs<TG> make_args(float* P, float* M, float* V, float* S, float* E, c
   return OptArgs<TG>{P, M, V, S, E, (const TG*)G, (__nv_bfloat16*)Pb, hyper, state, eps, la};
 }
 
-// Shared argument checks of the two pass entry points (after their own).
+// Argument checks of the pass over a flat range (after those of the descriptor).
 static int check_pass(const char* who, long long n, const float* P, const float* M, const float* V, const float* S, int g_dtype,
                       const void* G, const float* E, const void* Pb) {
   if (n <= 0 || (n & 3)) { set_error("%s: n=%lld must be a positive multiple of 4 (pad the flat range)", who, n); return COTB200_EINVAL; }
@@ -371,22 +371,6 @@ static double pass_bytes(long long n, bool m, bool v, int sync_bytes, int g_dtyp
 }  // namespace cotb200
 
 using namespace cotb200;
-
-extern "C" int cotb200_sgd_ema_step_clip(long long n, float* P, float* M, int g_dtype, const void* G, float* E, void* Pb,
-                                         const float* hyper_dev, int nesterov, const cotb200_clip* clip, void* stream) {
-  if (!P || !M || !G || !hyper_dev || !clip) { set_error("sgd_ema_step_clip: NULL pointer"); return COTB200_ENULL; }
-  if (n <= 0 || (n & 3)) { set_error("sgd_ema_step_clip: n=%lld must be a positive multiple of 4 (pad the flat range)", n); return COTB200_EINVAL; }
-  if (int rc = check_clip("sgd_ema_step_clip", clip)) return rc;
-  if (int rc = check_pass("sgd_ema_step_clip", n, P, M, nullptr, nullptr, g_dtype, G, E, Pb)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  double bytes = pass_bytes(n, true, false, 0, g_dtype, E, Pb);
-  bytes += clip->mode == COTB200_CLIP_AGC ? (double)clip->n_segs * (16.0 + 4.0) : (clip->mode == COTB200_CLIP_NORM ? 4.0 : 0.0);
-  COTB200_PROF_B("sgd_ema_step_clip", bytes);
-  const int rule = nesterov ? COTB200_OPT_SGD : COTB200_OPT_MOMENTUM;
-  if (g_dtype == COTB200_F32) launch_rule<float>(rule, make_args<float>(P, M, nullptr, nullptr, E, G, Pb, hyper_dev, nullptr, 0.f, 0.f), n / 4, clip, st);
-  else launch_rule<__nv_bfloat16>(rule, make_args<__nv_bfloat16>(P, M, nullptr, nullptr, E, G, Pb, hyper_dev, nullptr, 0.f, 0.f), n / 4, clip, st);
-  return check_launch("sgd_ema_step_clip");
-}
 
 extern "C" int cotb200_opt_prepare(const cotb200_opt* opt, const float* hyper_dev, int advance, void* stream) {
   if (!opt || !opt->state || !hyper_dev) { set_error("opt_prepare: NULL pointer"); return COTB200_ENULL; }

@@ -7,10 +7,9 @@
 //   P  fp32 master weights, M momentum, E EMA   -- flat buffers, one element order
 //   G  the step's gradients, gathered into ONE flat bucket (the unit of the NCCL all-reduce)
 //   Pb the bf16 copy of the >=2-D weights the convolutions actually read
-// and the whole parameter update is ONE pass:  read G, P, M, E  ->  write P, M, E, Pb   (4+4+4+4+2 .. bytes/element).
+// and the whole parameter update is ONE pass (cotb200_opt_step, opt.cu):  read G, P, M, E  ->  write P, M, E, Pb.
 //
 //   cotb200_multi_gather   gradients (any mix of fp32 / bf16 tensors) -> flat bucket (fp32 or bf16), optional scale
-//   cotb200_sgd_ema_step   SGD-momentum(-nesterov) + weight decay + EMA + bf16 shadow over a flat range
 //   cotb200_multi_lerp     EMA of the buffers (BatchNorm running statistics, integer counters) by pointer table
 //   cotb200_u8_to_nhwc     uint8 NCHW batch -> (x - mean)/std in bf16/fp16/fp32 channels_last
 //   cotb200_u8_mix_rows_to_nhwc   the same after Mixup / CutMix, one table row per output sample
@@ -58,45 +57,6 @@ multi_gather_kernel(const cotb200_seg* __restrict__ segs, const int2* __restrict
   if (s.dtype == COTB200_F32) gather_chunk<float, TD>((const float*)s.ptr + off, d, n, scale);
   else if (s.dtype == COTB200_BF16) gather_chunk<__nv_bfloat16, TD>((const __nv_bfloat16*)s.ptr + off, d, n, scale);
   else gather_chunk<__half, TD>((const __half*)s.ptr + off, d, n, scale);
-}
-
-// ------------------------------------------------------------------------------------------------ sgd_ema_step
-// torch.optim.SGD semantics (the reference's optimizer, optim/optim_factory.py:54-56):
-//   g = grad*gscale + wd*p ;  m = mu*m + g ;  step = nesterov ? g + mu*m : m ;  p -= lr*step
-// then ModelEmaV2.update (utils/model_ema.py:52-53):  e = decay*e + (1-decay)*p_new ; and the bf16 copy the convs read.
-// hyper (device, fp32[5]) = lr, mu, wd, ema_decay, gscale: device-resident so a captured graph follows the LR schedule.
-template <typename TG, bool NESTEROV>
-__global__ void __launch_bounds__(256)
-sgd_ema_kernel(float* __restrict__ P, float* __restrict__ M, const TG* __restrict__ G, float* __restrict__ E,
-               __nv_bfloat16* __restrict__ Pb, const float* __restrict__ hyper, long long n4) {
-  const float lr = __ldg(hyper), mu = __ldg(hyper + 1), wd = __ldg(hyper + 2), dec = __ldg(hyper + 3), gs = __ldg(hyper + 4);
-  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
-    float4 p = reinterpret_cast<float4*>(P)[i];
-    float4 m = reinterpret_cast<float4*>(M)[i];
-    const Pack<TG, 4> gp = ld_pack<TG, 4>(G + i * 4);
-    float pv[4] = {p.x, p.y, p.z, p.w}, mv[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float g = fmaf(wd, pv[k], (float)to_acc(gp.v[k]) * gs);
-      mv[k] = fmaf(mu, mv[k], g);
-      const float st = NESTEROV ? fmaf(mu, mv[k], g) : mv[k];
-      pv[k] = fmaf(-lr, st, pv[k]);
-    }
-    reinterpret_cast<float4*>(P)[i] = make_float4(pv[0], pv[1], pv[2], pv[3]);
-    reinterpret_cast<float4*>(M)[i] = make_float4(mv[0], mv[1], mv[2], mv[3]);
-    if (E) {
-      float4 e = reinterpret_cast<float4*>(E)[i];
-      e.x = fmaf(dec, e.x, (1.f - dec) * pv[0]); e.y = fmaf(dec, e.y, (1.f - dec) * pv[1]);
-      e.z = fmaf(dec, e.z, (1.f - dec) * pv[2]); e.w = fmaf(dec, e.w, (1.f - dec) * pv[3]);
-      reinterpret_cast<float4*>(E)[i] = e;
-    }
-    if (Pb) {
-      Pack<__nv_bfloat16, 4> o;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) o.v[k] = __float2bfloat16_rn(pv[k]);
-      st_pack<__nv_bfloat16, 4>(Pb + i * 4, o);
-    }
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ multi_lerp
@@ -262,26 +222,6 @@ extern "C" int cotb200_multi_gather(const cotb200_seg* segs_dev, const int* bloc
 }
 
 extern "C" int cotb200_gather_chunk(void) { return GATHER_CHUNK; }
-
-extern "C" int cotb200_sgd_ema_step(long long n, float* P, float* M, int g_dtype, const void* G, float* E, void* Pb,
-                                    const float* hyper_dev, int nesterov, void* stream) {
-  if (!P || !M || !G || !hyper_dev) { set_error("sgd_ema_step: NULL pointer"); return COTB200_ENULL; }
-  if (n <= 0 || (n & 3)) { set_error("sgd_ema_step: n=%lld must be a positive multiple of 4 (pad the flat range)", n); return COTB200_EINVAL; }
-  if (!aligned16(P) || !aligned16(M) || (E && !aligned16(E)) || (reinterpret_cast<uintptr_t>(G) & (g_dtype == COTB200_F32 ? 15 : 7)) || (Pb && (reinterpret_cast<uintptr_t>(Pb) & 7))) {
-    set_error("sgd_ema_step: flat buffers must be 16-byte aligned"); return COTB200_EALIGN;
-  }
-  if (g_dtype != COTB200_F32 && g_dtype != COTB200_BF16) { set_error("sgd_ema_step: gradient dtype must be fp32 or bf16"); return COTB200_EDTYPE; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long n4 = n / 4;
-  const unsigned grid = stream_grid(n4);
-  const double bytes = (double)n * (8.0 + 8.0 + (g_dtype == COTB200_F32 ? 4.0 : 2.0) + (E ? 8.0 : 0.0) + (Pb ? 2.0 : 0.0));
-  COTB200_PROF_B("sgd_ema_step", bytes);
-#define GO(TG, NES) sgd_ema_kernel<TG, NES><<<grid, 256, 0, st>>>(P, M, (const TG*)G, E, (__nv_bfloat16*)Pb, hyper_dev, n4)
-  if (g_dtype == COTB200_F32) { if (nesterov) GO(float, true); else GO(float, false); }
-  else { if (nesterov) GO(__nv_bfloat16, true); else GO(__nv_bfloat16, false); }
-#undef GO
-  return check_launch("sgd_ema_step");
-}
 
 extern "C" int cotb200_multi_lerp(const cotb200_seg2* segs_dev, int n_segs, const float* hyper_dev, void* stream) {
   if (!segs_dev || !hyper_dev) { set_error("multi_lerp: NULL pointer"); return COTB200_ENULL; }

@@ -15,10 +15,10 @@ Mirrors the body of the reference's training loop -- forward under autocast, los
   backward of the earlier layers is still running.  Everything -- forward, backward, gathers, NCCL, optimizer -- is
   captured in ONE CUDA graph (fork/join through events); if NCCL cannot be captured the collectives run eagerly between
   a fwd+bwd graph and an optimizer graph.
-* **One optimizer pass.**  ``cotb200_sgd_ema_step``: SGD-nesterov + weight decay + EMA + bf16 copy, hyper-parameters read
-  from device memory (LR schedules work under graph replay); ``cotb200_multi_lerp`` for the EMA of the buffers.  The other
-  update rules of the reference's create_optimizer (``opt=``) are ``cotb200_opt_prepare`` (the per-step scalars, on the device)
-  and one ``cotb200_opt_step`` pass per bucket.
+* **One optimizer pass.**  ``cotb200_opt_step`` per bucket: the update rule of the reference's create_optimizer (``opt=``,
+  SGD-nesterov by default) + weight decay + EMA + bf16 copy, hyper-parameters read from device memory (LR schedules work
+  under graph replay); before it ``cotb200_opt_prepare`` (the per-step scalars, on the device) for the rules that have any and
+  for Lookahead; ``cotb200_multi_lerp`` for the EMA of the buffers.
 
 There is no CPU fallback of the kernels; the planning logic (``plan_flat``) is pure Python and unit-tested on CPU.
 """
@@ -231,9 +231,7 @@ class TrainStep:
         weight_decay are the factory's, everything else its defaults."""
         if clip_mode not in CLIP_MODES:
             raise ValueError("TrainStep: unknown clip_mode %r (one of %s)" % (clip_mode, ", ".join(CLIP_MODES)))
-        self.opt_name, rule, self.lookahead = parse_opt(opt, nesterov)
-        if rule in (_lib.OPT_SGD, _lib.OPT_MOMENTUM):
-            nesterov = rule == _lib.OPT_SGD
+        self.opt_name, self.rule, self.lookahead = parse_opt(opt, nesterov)
         self.clip_grad = float(clip_grad) if clip_grad is not None and clip_grad > 0 else None
         self.clip_mode = clip_mode
         self.grad_norm = None
@@ -245,7 +243,6 @@ class TrainStep:
         self.jsd_splits = int(jsd_splits)
         self._gmix = self._gmix_shape = None
         self.amp_dtype = amp_dtype
-        self.nesterov = bool(nesterov)
         self.pg = process_group
         self.world = dist.get_world_size(process_group) if (dist.is_available() and dist.is_initialized()) else 1
         dev = next(model.parameters()).device
@@ -334,17 +331,15 @@ class TrainStep:
         self._clips = None
         if self.clip_grad is not None and self._cuda:
             self._init_clip()
-        self._opts = None                           # plain SGD without Lookahead: cotb200_sgd_ema_step(_clip), no step counter
-        self.V_big = self.V_small = self.S_big = self.S_small = self.opt_state = None
-        if (rule not in (_lib.OPT_SGD, _lib.OPT_MOMENTUM) or self.lookahead) and self._cuda:
-            self._init_opt(rule, float(opt_eps), momentum)
+        self._init_opt(float(opt_eps), momentum)
 
     # ------------------------------------------------------------------ update rules
-    def _init_opt(self, rule, eps, momentum):
-        """State buffers and the two cotb200_opt descriptors (big, small) of a rule other than plain SGD."""
+    def _init_opt(self, eps, momentum):
+        """State buffers, the device cotb200_opt_state and the two cotb200_opt descriptors (big, small) of the update rule."""
         f32 = dict(dtype=torch.float32, device=self.dev)
         nb, ns = self.plan["n_big"], self.plan["n_small"]
-        self.rule = rule
+        rule = self.rule
+        self.V_big = self.V_small = self.S_big = self.S_small = None
         if rule not in (_lib.OPT_SGD, _lib.OPT_MOMENTUM):
             fill = 1.0 if rule == _lib.OPT_RMSPROPTF else 0.0       # rmsprop_tf.py:94: square_avg starts at 1
             self.V_big, self.V_small = torch.full((nb,), fill, **f32), torch.full((ns,), fill, **f32)
@@ -353,6 +348,8 @@ class TrainStep:
         st = _lib.OptState(m_schedule=1.0)
         self.opt_state = torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(self.dev)
         self._opt_uses_m = not (rule in (_lib.OPT_RMSPROP, _lib.OPT_RMSPROPTF) and not momentum > 0)
+        # plain SGD / momentum without Lookahead has no per-step scalar: its pass runs on the state as initialised
+        self._prepare = rule not in (_lib.OPT_SGD, _lib.OPT_MOMENTUM) or self.lookahead
         self._opts = []
         for M, V, S in ((self.M_big, self.V_big, self.S_big), (self.M_small, self.V_small, self.S_small)):
             self._opts.append(_lib.Opt(rule=rule, eps=eps, lookahead_k=LOOKAHEAD_K if self.lookahead else 0,
@@ -516,33 +513,12 @@ class TrainStep:
         return loss
 
     def optimizer_step(self):
+        """optimizer.step(): the per-step scalars (when the rule or Lookahead has any), the clip factors, one cotb200_opt_step per
+        bucket, the EMA of the buffers."""
         st = torch.cuda.current_stream(self.dev).cuda_stream
         lib = self.lib
-        if self._opts is not None:
-            self._rule_step(st)
-            return
-        if self._clips is not None:
-            self._launch_clip_factors(st)
-            sgd = lambda *a, clip: lib.cotb200_sgd_ema_step_clip(*a, ctypes.byref(clip), st)   # noqa: E731
-        else:
-            sgd = lambda *a, clip: lib.cotb200_sgd_ema_step(*a, st)                            # noqa: E731
-        clips = self._clips or (None, None)
-        if self.plan["n_big"]:
-            _lib.check(sgd(self.plan["n_big"], self.P_big.data_ptr(), self.M_big.data_ptr(), _lib.dtype_code(self.G_big),
-                           self.G_big.data_ptr(), _lib.ptr(self.E_big), _lib.ptr(self.Pb), self.hyper.data_ptr(),
-                           1 if self.nesterov else 0, clip=clips[0]), "sgd_ema_step")
-        if self.plan["n_small"]:
-            _lib.check(sgd(self.plan["n_small"], self.P_small.data_ptr(), self.M_small.data_ptr(), _lib.F32,
-                           self.G_small.data_ptr(), _lib.ptr(self.E_small), None, self.hyper_small.data_ptr(),
-                           1 if self.nesterov else 0, clip=clips[1]), "sgd_ema_step")
-        if self.ema and self._lerp_n:
-            _lib.check(lib.cotb200_multi_lerp(self._lerp_tab.data_ptr(), self._lerp_n, self.hyper.data_ptr(), st), "multi_lerp")
-
-    def _rule_step(self, st):
-        """optimizer.step() of a rule other than plain SGD: the per-step scalars, one cotb200_opt_step per bucket, the EMA of the
-        buffers."""
-        lib = self.lib
-        _lib.check(lib.cotb200_opt_prepare(ctypes.byref(self._opts[0]), self.hyper.data_ptr(), 1, st), "opt_prepare")
+        if self._prepare:
+            _lib.check(lib.cotb200_opt_prepare(ctypes.byref(self._opts[0]), self.hyper.data_ptr(), 1, st), "opt_prepare")
         if self._clips is not None:
             self._launch_clip_factors(st)
         clips = [ctypes.byref(c) for c in self._clips] if self._clips is not None else [None, None]
@@ -560,7 +536,7 @@ class TrainStep:
         for every parameter (the first synchronisation only creates the slow weights), and the bf16 copy of the weights.  Runs
         eagerly on the current stream; the step counter and the EMA do not move.  Nothing happens without Lookahead, as the
         reference only calls it on a Lookahead optimizer."""
-        if not self.lookahead or self._opts is None:
+        if not self.lookahead:
             return
         st = torch.cuda.current_stream(self.dev).cuda_stream
         lib = self.lib
@@ -697,13 +673,12 @@ class TrainStep:
         """name -> {state key of the reference's optimizer: view}: fp32 views into the flat state buffers (exp_avg, exp_avg_sq,
         square_avg, acc_delta, momentum_buffer, slow_buffer) and 0-dim fp64 views of the device scalars `step` (updates done)
         and, for nadam, `m_schedule`.  slow_buffer holds the slow weights once the first Lookahead synchronisation has run."""
-        rule = self.rule if self._opts is not None else (_lib.OPT_SGD if self.nesterov else _lib.OPT_MOMENTUM)
-        uses_m = self._opt_uses_m if self._opts is not None else True
+        rule = self.rule
         keys = {_lib.OPT_ADADELTA: ("acc_delta", "square_avg"), _lib.OPT_RMSPROP: ("momentum_buffer", "square_avg"),
                 _lib.OPT_RMSPROPTF: ("momentum_buffer", "square_avg"), _lib.OPT_SGD: ("momentum_buffer", None),
                 _lib.OPT_MOMENTUM: ("momentum_buffer", None)}.get(rule, ("exp_avg", "exp_avg_sq"))
         scal = {}
-        if self.opt_state is not None and rule not in (_lib.OPT_SGD, _lib.OPT_MOMENTUM):
+        if rule not in (_lib.OPT_SGD, _lib.OPT_MOMENTUM):
             d = self.opt_state[:16].view(torch.float64)
             scal["step"] = d[0]
             if rule == _lib.OPT_NADAM:
@@ -712,7 +687,7 @@ class TrainStep:
         for key, M, V, S in (("big", self.M_big, self.V_big, self.S_big), ("small", self.M_small, self.V_small, self.S_small)):
             for n, p, off in self.plan[key]:
                 d = dict(scal)
-                if uses_m:
+                if self._opt_uses_m:
                     d[keys[0]] = _strided_view(M, p, off)
                 if V is not None:
                     d[keys[1]] = _strided_view(V, p, off)

@@ -328,14 +328,9 @@ int cotb200_gather_chunk(void);
  * tensors) into ONE flat fp32 or bf16 bucket = the unit of the NCCL all-reduce (replaces DDP's bucket copies, train.py:113-115). */
 int cotb200_multi_gather(const cotb200_seg* segs_dev, const int* blocks_dev, int n_blocks, int dst_dtype, void* dst,
                          float scale, void* stream);
-/* Over a flat range of n (multiple of 4) elements: torch.optim.SGD update with momentum (nesterov flag), weight decay,
- * then EMA  E = decay*E + (1-decay)*P  (E NULL: none) and the bf16 copy Pb of the new weights (NULL: none).
- * G is fp32 or bf16 (g_dtype).  hyper_dev = device fp32[5] {lr, momentum, weight_decay, ema_decay, grad_scale}: device
- * resident so that a captured CUDA graph follows the learning-rate schedule. */
-int cotb200_sgd_ema_step(long long n, float* P, float* M, int g_dtype, const void* G, float* E, void* Pb,
-                         const float* hyper_dev, int nesterov, void* stream);
 /* dst = decay*dst + (1-decay)*src per segment (fp32; int64 with the reference's float round trip): ModelEmaV2 over the
- * BUFFERS of the state_dict (BatchNorm running statistics / counters), one launch. decay = hyper_dev[3]. */
+ * BUFFERS of the state_dict (BatchNorm running statistics / counters), one launch.  decay = hyper_dev[3], the hyper_dev of
+ * cotb200_opt_step. */
 int cotb200_multi_lerp(const cotb200_seg2* segs_dev, int n_segs, const float* hyper_dev, void* stream);
 
 /* ---- gradient clipping on the flat buckets (train.py:270-273 -> utils/clip_grad.py:dispatch_clip_grad) ----
@@ -357,7 +352,7 @@ typedef struct cotb200_clip_seg {     /* AGC: one piece of the optimizer's flat 
   int numel;                          /* 1 .. cotb200_clip_seg_max() */
   int unit;                           /* index into the factors; -1: factor 1 (slot padding, parameters left out) */
 } cotb200_clip_seg;
-typedef struct cotb200_clip {         /* the clip of one cotb200_sgd_ema_step_clip call */
+typedef struct cotb200_clip {         /* the clip of one cotb200_opt_step call */
   int mode;                           /* COTB200_CLIP_* */
   float value;                        /* VALUE: c (> 0) */
   const float* factor;                /* NORM: device pointer to f (out[1] of cotb200_grad_norm); AGC: device per-unit factors */
@@ -379,15 +374,11 @@ int cotb200_grad_norm(long long n0, int g0_dtype, const void* G0, const float* g
 int cotb200_unit_norms(int n_units, const cotb200_clip_unit* units_dev, long long unit_elems, const float* P0, int g0_dtype,
                        const void* G0, const float* gs0, const float* P1, const float* G1, const float* gs1, float clip_factor,
                        float* factor, float* norms, void* stream);
-/* cotb200_sgd_ema_step with the clip applied to g' = G*grad_scale on the way in: the update reads the clipped g' in place of
- * G*grad_scale.  A factor of 1 or a clamp that does not bind gives bit-for-bit the result of cotb200_sgd_ema_step. */
-int cotb200_sgd_ema_step_clip(long long n, float* P, float* M, int g_dtype, const void* G, float* E, void* Pb,
-                              const float* hyper_dev, int nesterov, const cotb200_clip* clip, void* stream);
 
 /* ---- the update rules of create_optimizer (optim/optim_factory.py) on the flat buckets ----
  * One pass per flat range: g' = G*grad_scale, the clip (cotb200_clip, NULL: none), the rule, the Lookahead synchronisation when
- * this step has one, E = decay*E + (1-decay)*P of the final weights, and the bf16 copy Pb.  hyper_dev is the fp32[5] of
- * cotb200_sgd_ema_step ({lr, momentum, weight_decay, ema_decay, grad_scale}); betas, rho and alpha are the factory's defaults:
+ * this step has one, E = decay*E + (1-decay)*P of the final weights, and the bf16 copy Pb.  Betas, rho and alpha are the
+ * factory's defaults:
  *   SGD / MOMENTUM  torch.optim.SGD, nesterov / not                     M = momentum_buffer
  *   ADAM            torch.optim.Adam (L2 decay), betas (0.9, 0.999)     M = exp_avg, V = exp_avg_sq
  *   ADAMW           optim/adamw.py: P *= 1 - lr*wd, then Adam           M, V as ADAM
@@ -423,7 +414,10 @@ typedef struct cotb200_opt {          /* the optimizer of one flat range */
  * (bias corrections, Nadam's momentum caches and m_schedule, RAdam's N_sma and step size, the Lookahead flag).  advance = 0:
  * only the flag, set to synchronise now (TrainStep.sync_lookahead).  One thread. */
 int cotb200_opt_prepare(const cotb200_opt* opt, const float* hyper_dev, int advance, void* stream);
-/* The pass over a flat range of n (multiple of 4) elements.  G fp32 or bf16 (g_dtype); E, Pb NULL: none; clip NULL: none. */
+/* The pass over a flat range of n (multiple of 4) elements.  G fp32 or bf16 (g_dtype); E, Pb NULL: none; clip NULL: none.
+ * hyper_dev = device fp32[5] {lr, momentum, weight_decay, ema_decay, grad_scale}: device resident so that a captured CUDA graph
+ * follows the learning-rate schedule.  opt->state is required; plain SGD / MOMENTUM without Lookahead uses none of its
+ * coefficients and runs on the state as initialised, without cotb200_opt_prepare. */
 int cotb200_opt_step(long long n, float* P, int g_dtype, const void* G, float* E, void* Pb, const float* hyper_dev,
                      const cotb200_opt* opt, const cotb200_clip* clip, void* stream);
 /* The Lookahead synchronisation prepared by cotb200_opt_prepare(advance = 0), and the bf16 copy Pb (NULL: none). */

@@ -143,7 +143,7 @@ def test_trainstep_rejects_unknown_clip_mode():
 
 
 # ------------------------------------------------------------------------------------------------ C entry points
-def test_clip_entry_points_reject_bad_arguments():
+def test_clip_and_clipped_opt_step_reject_bad_arguments():
     """Validation happens before any CUDA call: the pointers below are never dereferenced."""
     from cotnet_b200 import _lib
     lib = _lib.load()
@@ -162,11 +162,10 @@ def test_clip_entry_points_reject_bad_arguments():
     assert lib.cotb200_unit_norms(4, P, 16, P, _lib.BF16, P, P, P, None, P, 0.01, P, None, None) == ENULL
     assert lib.cotb200_unit_norms(0, P, 16, P, _lib.BF16, P, P, None, None, None, 0.01, P, None, None) == EINVAL
     assert lib.cotb200_unit_norms(4, P, 16, P, _lib.F64, P, P, None, None, None, 0.01, P, None, None) == EDTYPE
-    # sgd_ema_step_clip
+    # the clipped SGD pass: opt_step with rule SGD
     def step(n=8, gdt=_lib.F32, G=P, clip=None):
-        return lib.cotb200_sgd_ema_step_clip(n, P, P, gdt, G, None, None, P, 1, clip, None)
+        return lib.cotb200_opt_step(n, P, gdt, G, None, None, P, _lib.Opt(rule=_lib.OPT_SGD, M=P, state=P), clip, None)
     norm = _lib.Clip(mode=_lib.CLIP_NORM, factor=P)
-    assert step(clip=None) == ENULL
     assert step(n=6, clip=norm) == EINVAL
     assert step(clip=_lib.Clip(mode=7, factor=P)) == EINVAL
     assert step(clip=_lib.Clip(mode=_lib.CLIP_NORM)) == ENULL

@@ -2,6 +2,7 @@
 restatement of utils/clip_grad.py (tests/clip_ref.py) followed by the SGD / EMA formulas in fp64, bit-identity with the plain
 optimizer pass when the clip does not bind, NaN propagation, and TrainStep end to end (eager, captured, launch counts)."""
 import copy
+import ctypes
 
 import numpy as np
 import pytest
@@ -110,19 +111,16 @@ class _Flat:
             v.copy_(g)
         return out
 
-    # the library's sequence for one step (what TrainStep.optimizer_step launches)
+    # the library's sequence for one step (what TrainStep.optimizer_step launches for opt="sgd"); plain: without the clip
     def step(self, mode, c, plain=False):
         from cotnet_b200 import _lib, trainer
         lib = _lib.load()
         B = self.bufs
+        state = torch.zeros(ctypes.sizeof(_lib.OptState), dtype=torch.uint8, device="cuda")    # SGD runs without opt_prepare
+        self.keep = [state]
         if plain:
-            for b in B:
-                _lib.check(lib.cotb200_sgd_ema_step(b["n"], b["P"].data_ptr(), b["M"].data_ptr(), _lib.dtype_code(b["G"]), b["G"].data_ptr(),
-                                                    b["E"].data_ptr(), _lib.ptr(b["Pb"]), b["hyper"].data_ptr(), 1, _st()), "sgd")
-            return None
-        code = trainer.CLIP_MODES[mode]
-        descs = [_lib.Clip(mode=code, value=c), _lib.Clip(mode=code, value=c)]
-        self.keep = []
+            mode = None
+        descs = [None, None] if mode is None else [_lib.Clip(mode=trainer.CLIP_MODES[mode], value=c) for _ in range(2)]
         out = None
         if mode == "norm":
             out = torch.zeros(2, device="cuda")
@@ -148,8 +146,9 @@ class _Flat:
             self.keep += [utab, fac]
             self.factors = fac
         for b, d in zip(B, descs):
-            _lib.check(lib.cotb200_sgd_ema_step_clip(b["n"], b["P"].data_ptr(), b["M"].data_ptr(), _lib.dtype_code(b["G"]), b["G"].data_ptr(),
-                                                     b["E"].data_ptr(), _lib.ptr(b["Pb"]), b["hyper"].data_ptr(), 1, d, _st()), "sgd_clip")
+            opt = _lib.Opt(rule=_lib.OPT_SGD, M=b["M"].data_ptr(), state=state.data_ptr())
+            _lib.check(lib.cotb200_opt_step(b["n"], b["P"].data_ptr(), _lib.dtype_code(b["G"]), b["G"].data_ptr(), b["E"].data_ptr(),
+                                            _lib.ptr(b["Pb"]), b["hyper"].data_ptr(), opt, d, _st()), "opt_step")
         torch.cuda.synchronize()
         return out
 
@@ -188,7 +187,7 @@ def _oracle(f, mode, c):
 # ------------------------------------------------------------------------------------------------ 2. clipped update vs the oracle
 @pytest.mark.parametrize("mode", clip_ref.MODES)
 @pytest.mark.parametrize("gdt", [torch.bfloat16, torch.float32])
-def test_clipped_update_matches_oracle(mode, gdt):
+def test_clipped_opt_step_matches_oracle(mode, gdt):
     from cotnet_b200 import trainer
     f = _Flat(gdt, seed=1)
     c, margin = _binding_value(f, mode)
@@ -221,7 +220,7 @@ def test_clipped_update_matches_oracle(mode, gdt):
 # ------------------------------------------------------------------------------------------------ 3. a clip that does not bind
 @pytest.mark.parametrize("mode", clip_ref.MODES)
 @pytest.mark.parametrize("gdt", [torch.bfloat16, torch.float32])
-def test_non_binding_clip_is_bit_identical(mode, gdt):
+def test_non_binding_clip_equals_unclipped_opt_step(mode, gdt):
     a = _Flat(gdt, seed=2)
     b = a.clone()
     a.step(mode, 1e30)
@@ -235,7 +234,7 @@ def test_non_binding_clip_is_bit_identical(mode, gdt):
 
 # ------------------------------------------------------------------------------------------------ 4. NaN propagation
 @pytest.mark.parametrize("mode", clip_ref.MODES)
-def test_nan_propagation(mode):
+def test_clipped_opt_step_propagates_nan(mode):
     f = _Flat(torch.bfloat16, seed=3)
     name, p, off = f.plan["big"][1]                        # conv2.weight [16, 8, 1, 1]
     assert name == "conv2.weight"

@@ -181,6 +181,18 @@ def test_opt_entry_points_reject_bad_arguments():
     assert lib.cotb200_last_error()
 
 
+def test_sgd_pass_rejects_bad_arguments():
+    """The plain SGD pass as TrainStep launches it (rule SGD, no clip); no pointer below is dereferenced."""
+    from cotnet_b200 import _lib
+    lib = _lib.load()
+    P = 16
+    ENULL, EINVAL, EDTYPE = -5, -1, -2
+    o = _lib.Opt(rule=_lib.OPT_SGD, M=P, state=P)
+    assert lib.cotb200_opt_step(6, P, _lib.F32, P, None, None, P, o, None, None) == EINVAL
+    assert lib.cotb200_opt_step(8, None, _lib.F32, P, None, None, P, o, None, None) == ENULL
+    assert lib.cotb200_opt_step(8, P, _lib.F64, P, None, None, P, o, None, None) == EDTYPE
+
+
 def test_struct_layouts():
     import ctypes
     from cotnet_b200 import _lib

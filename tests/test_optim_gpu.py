@@ -329,6 +329,21 @@ def test_sync_lookahead():
     plain.sync_lookahead()                                    # no Lookahead: nothing to do
 
 
+def test_plain_sgd_leaves_the_state_as_initialised():
+    """opt='sgd' without Lookahead launches no cotb200_opt_prepare: after steps the device state still has t = 0, no coefficient,
+    no synchronisation (m_schedule its initial 1), and optimizer_state() reports no `step`, as torch.optim.SGD keeps none."""
+    from cotnet_b200 import _lib, trainer
+    x, y = _batch(4, torch.bfloat16)
+    ts = trainer.TrainStep(_small_model(), lr=1e-3, ema_decay=0.99, amp_dtype=torch.bfloat16, weights="bf16", opt="sgd")
+    P0 = ts.P_big.clone()
+    for _ in range(2):
+        ts.step_eager(x, y)
+    torch.cuda.synchronize()
+    assert not torch.equal(ts.P_big, P0)
+    assert bytes(ts.opt_state.cpu().numpy()) == bytes(_lib.OptState(m_schedule=1.0))
+    assert all(set(d) == {"momentum_buffer"} for d in ts.optimizer_state().values())
+
+
 # ------------------------------------------------------------------------------------------------ 6. launches per replay
 def test_launch_count_is_sgd_plus_prepare():
     from cotnet_b200 import trainer

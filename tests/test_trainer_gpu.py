@@ -43,7 +43,8 @@ def _record(name, payload):
 # ------------------------------------------------------------------------------------------------ kernels
 @pytest.mark.parametrize("gdt", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("nesterov", [True, False])
-def test_sgd_ema_kernel_matches_torch(gdt, nesterov):
+def test_sgd_pass_matches_torch(gdt, nesterov):
+    """cotb200_opt_step as TrainStep runs plain SGD: rule SGD (nesterov) or MOMENTUM on a zeroed state, no cotb200_opt_prepare."""
     from cotnet_b200 import _lib
     lib = _lib.load()
     n = 4 * 12345
@@ -54,14 +55,16 @@ def test_sgd_ema_kernel_matches_torch(gdt, nesterov):
     Pb = torch.empty(n, device="cuda", dtype=torch.bfloat16)
     lr, mu, wd, dec = 0.1, 0.9, 1e-2, 0.99
     hyper = torch.tensor([lr, mu, wd, dec, 1.0], device="cuda")
+    state = torch.zeros(ctypes.sizeof(_lib.OptState), dtype=torch.uint8, device="cuda")
+    od = _lib.Opt(rule=_lib.OPT_SGD if nesterov else _lib.OPT_MOMENTUM, M=M.data_ptr(), state=state.data_ptr())
     p_ref = torch.nn.Parameter(P.clone())
     opt = torch.optim.SGD([p_ref], lr=lr, momentum=mu, weight_decay=wd, nesterov=nesterov)
     e_ref = P.clone()
     for step in range(3):
         G = torch.randn(n, device="cuda", generator=g0).to(gdt)
-        rc = lib.cotb200_sgd_ema_step(n, P.data_ptr(), M.data_ptr(), _lib.dtype_code(G), G.data_ptr(), E.data_ptr(), Pb.data_ptr(),
-                                      hyper.data_ptr(), 1 if nesterov else 0, torch.cuda.current_stream().cuda_stream)
-        _lib.check(rc, "sgd_ema_step")
+        rc = lib.cotb200_opt_step(n, P.data_ptr(), _lib.dtype_code(G), G.data_ptr(), E.data_ptr(), Pb.data_ptr(), hyper.data_ptr(),
+                                  ctypes.byref(od), None, torch.cuda.current_stream().cuda_stream)
+        _lib.check(rc, "opt_step")
         p_ref.grad = G.float()
         opt.step()
         e_ref = dec * e_ref + (1.0 - dec) * p_ref.detach()               # utils/model_ema.py:52-53
@@ -69,16 +72,6 @@ def test_sgd_ema_kernel_matches_torch(gdt, nesterov):
     assert torch.allclose(E, e_ref, rtol=1e-5, atol=1e-6)
     assert torch.equal(Pb, P.to(torch.bfloat16))
     assert torch.allclose(M, opt.state[p_ref]["momentum_buffer"], rtol=1e-5, atol=1e-6)
-
-
-def test_sgd_ema_kernel_argument_errors():
-    from cotnet_b200 import _lib
-    lib = _lib.load()
-    t = torch.zeros(64, device="cuda")
-    h = torch.zeros(5, device="cuda")
-    assert lib.cotb200_sgd_ema_step(6, t.data_ptr(), t.data_ptr(), _lib.F32, t.data_ptr(), None, None, h.data_ptr(), 1, None) == -1
-    assert lib.cotb200_sgd_ema_step(8, None, t.data_ptr(), _lib.F32, t.data_ptr(), None, None, h.data_ptr(), 1, None) == -5
-    assert lib.cotb200_sgd_ema_step(8, t.data_ptr(), t.data_ptr(), _lib.F64, t.data_ptr(), None, None, h.data_ptr(), 1, None) == -2
 
 
 @pytest.mark.parametrize("bucket", [torch.float32, torch.bfloat16])

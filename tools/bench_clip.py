@@ -24,7 +24,7 @@ from bench_recipe import gpu_info, timed  # noqa: E402
 from cotnet_b200 import _lib, backbone, trainer  # noqa: E402
 
 MODES = (None, "norm", "value", "agc")
-KERNELS = ("sgd_ema_step", "sgd_ema_step_clip", "grad_norm", "unit_norms", "multi_lerp")
+KERNELS = ("opt_step", "grad_norm", "unit_norms", "multi_lerp")
 
 
 def one_round(a, mode, x, lab, profile):

@@ -4,8 +4,9 @@
 
 * passes: each rule's optimizer pass over the big bucket at the model's real flat size (plan_flat), bf16 gradients, EMA and the
   bf16 shadow, timed with CUDA events over --iters back-to-back launches (the per-step prepare launch included for the rules that
-  have one); GB/s from the byte model per element: P r/w 8, G 2, E r/w 8, Pb 2, plus 8 per fp32 state buffer (M, V), plus 8
-  for a Lookahead synchronisation step (S r/w).  SGD = 28 B, the Adam family / RMSprop with momentum / Adadelta = 36 B.
+  have one and for Lookahead, as TrainStep launches them); GB/s from the byte model per element: P r/w 8, G 2, E r/w 8, Pb 2,
+  plus 8 per fp32 state buffer (M, V), plus 8 for a Lookahead synchronisation step (S r/w).  SGD = 28 B, the Adam family /
+  RMSprop with momentum / Adadelta = 36 B.
 * graph: the TrainStep graph step time (bench.py's workload: bf16 weights, autocast, channels_last, cuDNN deterministic) for
   sgd, adamw, rmsproptf and lookahead_sgd, alternating within each of --rounds rounds in one process.
 * the GPU name and power limit next to the numbers.
@@ -45,16 +46,15 @@ def bench_passes(a, n):
         ms = timed(fn, a.iters)
         out[name] = {"ms": ms, "bytes_per_elem": per_elem, "GB_per_s": n * per_elem / 1e9 / (ms / 1e3)}
 
-    record("sgd (cotb200_sgd_ema_step)", lambda: lib.cotb200_sgd_ema_step(n, P.data_ptr(), M.data_ptr(), _lib.BF16, G.data_ptr(),
-                                                                          E.data_ptr(), Pb.data_ptr(), hyper.data_ptr(), 1, st), 28)
     for name in PASS_RULES + ("lookahead_adamw sync step",):
         base, rule, la = trainer.parse_opt(name.split(" ")[0])
         state = torch.frombuffer(bytearray(bytes(_lib.OptState(m_schedule=1.0, slow_init=1))), dtype=torch.uint8).to(dev)
         o = _lib.Opt(rule=rule, eps=1e-8, lookahead_k=1 if la else 0, lookahead_alpha=0.5, M=M.data_ptr(),
                      V=V.data_ptr() if base not in ("sgd",) else None, S=S.data_ptr(), state=state.data_ptr())
 
-        def run(o=o):
-            lib.cotb200_opt_prepare(ctypes.byref(o), hyper.data_ptr(), 1, st)
+        def run(o=o, prepare=base not in ("sgd", "momentum") or la):
+            if prepare:                                   # as TrainStep: plain SGD has no per-step scalar
+                lib.cotb200_opt_prepare(ctypes.byref(o), hyper.data_ptr(), 1, st)
             lib.cotb200_opt_step(n, P.data_ptr(), _lib.BF16, G.data_ptr(), E.data_ptr(), Pb.data_ptr(), hyper.data_ptr(), ctypes.byref(o),
                                  None, st)
         per = 28 + (8 if base != "sgd" else 0) + (8 if la else 0)
