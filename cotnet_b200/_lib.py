@@ -149,6 +149,8 @@ SYMBOLS = {
     "cotb200_aug_resize_crop": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP, ctypes.c_longlong, _VP, _VP, _VP, ctypes.c_longlong, _VP, _VP]),
     "cotb200_aug_randaug": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP] * 4),
     "cotb200_aug_color_jitter": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP] * 4),
+    "cotb200_aug_randaug_cluster": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP] * 4),
+    "cotb200_aug_color_jitter_cluster": (ctypes.c_int, [ctypes.c_int] * 2 + [_VP] * 4),
     "cotb200_aug_erase": (ctypes.c_int, [ctypes.c_int] * 5 + [_VP] * 4),
     "cotb200_dropblock_mask": (ctypes.c_int, [ctypes.c_int] * 5 + [ctypes.c_float, ctypes.c_int] + [_VP] * 4),
     "cotb200_dropblock_apply": (ctypes.c_int, [ctypes.c_int] * 4 + [_VP] * 5),

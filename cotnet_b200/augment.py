@@ -8,6 +8,8 @@ DataLoader workers still decode (JPEG -> RGB uint8 HWC, the reference dataset's 
   equals what the reference's transforms draw from the global generators; ``collate`` does that inside DataLoader workers
   and packs the batch into one ragged buffer; ``__call__`` runs the kernels (cotb200_aug_resize_crop, cotb200_aug_randaug)
   and returns the uint8 NCHW batch that fast_collate builds, ready for ``normalize_u8(mix=MixupCutmix.draw(...))``.
+  Above 256 x 256 (the 288 and 320 data configs) RandAugment and ColorJitter run on their thread-block-cluster kernels
+  (cotb200_aug_randaug_cluster, cotb200_aug_color_jitter_cluster), up to 512 x 512.
   With ``vflip`` a RandomVerticalFlip follows the horizontal one; without ``auto_augment``, ``color_jitter`` gives torchvision's
   ColorJitter (:100-109), both in one more kernel (cotb200_aug_color_jitter) between resize-crop and RandAugment.
   With ``num_splits`` S >= 2 it is the reference's AugMixDataset over the separated transform (datasets/dataset.py:181-215,
@@ -38,6 +40,8 @@ OPS = ("AutoContrast", "Equalize", "Invert", "Rotate", "Posterize", "Solarize", 
 AFFINE_OPS = (3, 11, 12, 13, 14)
 MAX_LEVEL = 10.          # rand_augment.py _MAX_LEVEL (level -> argument scale)
 MAG_CLIP = 15            # AugmentOp.MAX_LEVEL (magnitude clip)
+ONE_CTA_MAX_S = 256      # the largest output size of cotb200_aug_randaug / cotb200_aug_color_jitter (one CTA per image)
+CLUSTER_MAX_S = 512      # COTB200_AUG_CLUSTER_MAX_S, the *_cluster entry points' (one thread-block cluster per image)
 
 _OP_DTYPE = np.dtype([("op", "<i4"), ("filter", "<i4"), ("v", "<i4", (4,)), ("factor", "<f4"), ("pad_", "<i4"),
                       ("m", "<f8", (6,))], align=True)
@@ -409,12 +413,21 @@ class EvalTransform:
         return out, batch.labels.to(out.device, non_blocking=True)
 
 
-def run(batch, S, device=None, randaug=True, num_splits=0):
+def uses_cluster_kernels(S):
+    """Whether run() takes the thread-block-cluster kernels at output size S: above ONE_CTA_MAX_S, where one CTA's shared
+    memory cannot hold the image."""
+    return S > ONE_CTA_MAX_S
+
+
+def run(batch, S, device=None, randaug=True, num_splits=0, cluster=None):
     """The kernels on an AugBatch: H2D copies of the ragged buffer and the structs, resize-crop (+ flip), vertical flip and
     ColorJitter when the batch carries them, then RandAugment in place.  Returns uint8 [N, 3, S, S] on `device` (default: the
     current CUDA device).  With num_splits >= 2 (TrainAugment(num_splits=...)'s batch of B images) the clean views are
     resized, cropped and flipped into out[:B] and copied into each of the num_splits - 1 blocks after it, where the views'
-    ColorJitter or RandAugment run in place: N = num_splits * B."""
+    ColorJitter or RandAugment run in place: N = num_splits * B.
+    ColorJitter and RandAugment run one CTA per image up to S = ONE_CTA_MAX_S and one thread-block cluster per image above
+    it, up to CLUSTER_MAX_S, with the same bytes; `cluster` True / False forces one kind (None: by size)."""
+    cluster = uses_cluster_kernels(S) if cluster is None else bool(cluster)
     device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     rec = batch.params.numpy().view(SAMPLE_DTYPE)
     N = len(rec)
@@ -442,15 +455,15 @@ def run(batch, S, device=None, randaug=True, num_splits=0):
 
     def jitter(lo, hi):
         if jdev is not None and (jrec["vflip"][lo:hi].any() or (jrec["order"][lo:hi] >= 0).any()):
-            _lib.check(lib.cotb200_aug_color_jitter(hi - lo, S, jrec[lo:].ctypes.data_as(ctypes.c_void_p),
-                                                    jdev.data_ptr() + lo * JITTER_DTYPE.itemsize, out[lo].data_ptr(), st),
-                       "aug_color_jitter")
+            fn = lib.cotb200_aug_color_jitter_cluster if cluster else lib.cotb200_aug_color_jitter
+            _lib.check(fn(hi - lo, S, jrec[lo:].ctypes.data_as(ctypes.c_void_p), jdev.data_ptr() + lo * JITTER_DTYPE.itemsize,
+                          out[lo].data_ptr(), st), "aug_color_jitter")
 
     def randaug_(lo, hi):
         if randaug and (rec["ops"]["op"][lo:hi] >= 0).any():
-            _lib.check(lib.cotb200_aug_randaug(hi - lo, S, rec[lo:].ctypes.data_as(ctypes.c_void_p),
-                                               params.data_ptr() + lo * SAMPLE_DTYPE.itemsize, out[lo].data_ptr(), st),
-                       "aug_randaug")
+            fn = lib.cotb200_aug_randaug_cluster if cluster else lib.cotb200_aug_randaug
+            _lib.check(fn(hi - lo, S, rec[lo:].ctypes.data_as(ctypes.c_void_p), params.data_ptr() + lo * SAMPLE_DTYPE.itemsize,
+                          out[lo].data_ptr(), st), "aug_randaug")
     jitter(0, B)
     if splits > 1:                                  # the augmented views start from the clean view, vertical flip included
         for k in range(1, splits):

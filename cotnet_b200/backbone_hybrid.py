@@ -276,4 +276,10 @@ def se_cotnetd_152(**kw):                                                       
     return CoTHybridNet([3, 8, 36, 3], stem_width=64, aa_layer=BlurPool2d, block_args=_args(36, avd=True, avd_first=False), **kw)
 
 
+def se_cotnetd_152_L(**kw):                                                          # :476-482
+    """The SE-CoTNetD-152 trunk under the name the reference registers for its 320 x 320 data config (cot_l, crop_pct 0.909).
+    MODELS lists each distinct trunk once, so this second name of se_cotnetd_152 is not in it."""
+    return se_cotnetd_152(**kw)
+
+
 MODELS = {"se_cotnetd_50": se_cotnetd_50, "se_cotnetd_101": se_cotnetd_101, "se_cotnetd_152": se_cotnetd_152}

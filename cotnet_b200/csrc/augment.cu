@@ -16,6 +16,11 @@
 //
 // ColorJitter (+ RandomVerticalFlip), the reference's colour transform when RandAugment is off, runs the same way: one CTA per
 // image in shared memory, between resize-crop and RandAugment, sharing RandAugment's enhance blends.
+//
+// Both have a second kernel for images up to 512 x 512 that do not fit one CTA's shared memory: one thread-block cluster of up
+// to 4 CTAs per image, each holding a band of rows, with the same per-pixel arithmetic (the *_cluster entry points).
+#include <cooperative_groups.h>
+
 #include "common.cuh"
 
 namespace cotb200 {
@@ -247,31 +252,90 @@ __device__ __forceinline__ int smooth_px(const unsigned char* pl, int S, int x, 
   return ss <= 0.f ? 0 : ss >= 255.f ? 255 : (int)__fadd_rn(ss, 0.5f);
 }
 
-// ImageEnhance.Color / Contrast / Brightness (op OP_COLOR, OP_CONTRAST, OP_BRIGHTNESS) of the planar image img [3][n_pix] in
-// shared memory, in place: Image.blend(degenerate, img, factor) with the degenerate L (Color), int(mean(L) + 0.5) (Contrast) or
-// 0 (Brightness).  Every thread of the CTA calls it; lsum is a shared scratch word.  Ends with the CTA synchronised.
+// The enhance blends work on n pixels of a planar image img [3][plane] in shared memory (the whole image, or one CTA's band of
+// rows in the cluster kernels).  Every thread of the CTA calls these.
+// Sum of L over the n pixels into the shared word *lsum; ends with the CTA synchronised.
+__device__ void l_sum(const unsigned char* img, int plane, int n, unsigned long long* lsum) {
+  if (threadIdx.x == 0) *lsum = 0;
+  __syncthreads();
+  unsigned long long part = 0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) part += l_of(img[i], img[plane + i], img[2 * plane + i]);
+  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+  if ((threadIdx.x & 31) == 0) atomicAdd(lsum, part);
+  __syncthreads();
+}
+
+// int(mean(L) + 0.5) of an image of n_pix pixels whose L values sum to `sum` (ImageEnhance.Contrast's degenerate)
+__device__ __forceinline__ int contrast_mean(unsigned long long sum, int n_pix) {
+  return (int)__dadd_rn(__ddiv_rn((double)sum, (double)n_pix), 0.5);
+}
+
+// ImageEnhance.Color / Contrast / Brightness (op OP_COLOR, OP_CONTRAST, OP_BRIGHTNESS) in place: Image.blend(degenerate, img,
+// factor) with the degenerate L (Color), `mean` (Contrast) or 0 (Brightness).  Ends with the CTA synchronised.
+__device__ void enhance_apply(unsigned char* img, int plane, int n, int op, float factor, int mean) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int r = img[i], gg = img[plane + i], b = img[2 * plane + i];
+    const int d = op == OP_COLOR ? l_of(r, gg, b) : op == OP_CONTRAST ? mean : 0;
+    img[i] = blend_px(d, r, factor);
+    img[plane + i] = blend_px(d, gg, factor);
+    img[2 * plane + i] = blend_px(d, b, factor);
+  }
+  __syncthreads();
+}
+
+// The enhance blend of the whole image img [3][n_pix] held by one CTA; lsum is a shared scratch word.
 __device__ void enhance_blend(unsigned char* img, int n_pix, int op, float factor, unsigned long long* lsum) {
   int mean = 0;
-  if (op == OP_CONTRAST) {                            // int(mean(L) + 0.5), ImageEnhance.Contrast
-    if (threadIdx.x == 0) *lsum = 0;
-    __syncthreads();
-    unsigned long long part = 0;
-    for (int i = threadIdx.x; i < n_pix; i += blockDim.x) part += l_of(img[i], img[n_pix + i], img[2 * n_pix + i]);
-    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(lsum, part);
-    __syncthreads();
-    mean = (int)__dadd_rn(__ddiv_rn((double)*lsum, (double)n_pix), 0.5);
+  if (op == OP_CONTRAST) {
+    l_sum(img, n_pix, n_pix, lsum);
+    mean = contrast_mean(*lsum, n_pix);
   } else {
     __syncthreads();
   }
-  for (int i = threadIdx.x; i < n_pix; i += blockDim.x) {
-    const int r = img[i], gg = img[n_pix + i], b = img[2 * n_pix + i];
-    const int d = op == OP_COLOR ? l_of(r, gg, b) : op == OP_CONTRAST ? mean : 0;
-    img[i] = blend_px(d, r, factor);
-    img[n_pix + i] = blend_px(d, gg, factor);
-    img[2 * n_pix + i] = blend_px(d, b, factor);
+  enhance_apply(img, n_pix, n_pix, op, factor, mean);
+}
+
+// ImageOps.autocontrast / equalize of one channel: the LUT from its histogram h (one thread per channel)
+__device__ void hist_lut(int op, const int* h, unsigned char* lut) {
+  if (op == OP_AUTOCONTRAST) {
+    int lo = 0, hi = 255;
+    while (lo < 255 && !h[lo]) ++lo;
+    while (hi > 0 && !h[hi]) --hi;
+    if (hi <= lo) {
+      for (int i = 0; i < 256; ++i) lut[i] = (unsigned char)i;
+    } else {
+      const double scale = __ddiv_rn(255.0, (double)(hi - lo));
+      const double offset = __dmul_rn((double)(-lo), scale);
+      for (int i = 0; i < 256; ++i) {
+        const int v = (int)__dadd_rn(__dmul_rn((double)i, scale), offset);
+        lut[i] = (unsigned char)(v < 0 ? 0 : v > 255 ? 255 : v);
+      }
+    }
+  } else {
+    long long tot = 0, last = 0;
+    int nz = 0;
+    for (int i = 0; i < 256; ++i) if (h[i]) { tot += h[i]; last = h[i]; ++nz; }
+    const long long step = nz <= 1 ? 0 : (tot - last) / 255;
+    if (!step) {
+      for (int i = 0; i < 256; ++i) lut[i] = (unsigned char)i;
+    } else {
+      long long nn = step / 2;
+      for (int i = 0; i < 256; ++i) {
+        const long long v = nn / step;
+        lut[i] = (unsigned char)(v > 255 ? 255 : v);
+        nn += h[i];
+      }
+    }
   }
-  __syncthreads();
+}
+
+// Invert / Posterize / Solarize / SolarizeAdd of the value v (every other op: v unchanged)
+__device__ __forceinline__ int point_lut(const cotb200_aug_op& op, int v) {
+  if (op.op == OP_INVERT) return 255 - v;
+  if (op.op == OP_POSTERIZE) return op.v[0] >= 8 ? v : v & (~((1 << (8 - op.v[0])) - 1) & 255);
+  if (op.op == OP_SOLARIZE) return v < op.v[0] ? v : 255 - v;
+  if (op.op == OP_SOLARIZEADD) return v < 128 ? min(255, v + op.v[0]) : v;
+  return v;
 }
 
 __global__ void __launch_bounds__(RA_THREADS)
@@ -337,50 +401,9 @@ aug_randaug_kernel(const cotb200_aug_sample* __restrict__ params, int S, unsigne
       __syncthreads();
       for (int i = threadIdx.x; i < n_all; i += blockDim.x) atomicAdd(&hist[i / n_pix][sm_img[i]], 1);
       __syncthreads();
-      if (threadIdx.x < 3) {                          // ImageOps.autocontrast / equalize, per channel
-        const int c = threadIdx.x;
-        const int* h = hist[c];
-        if (op.op == OP_AUTOCONTRAST) {
-          int lo = 0, hi = 255;
-          while (lo < 255 && !h[lo]) ++lo;
-          while (hi > 0 && !h[hi]) --hi;
-          if (hi <= lo) {
-            for (int i = 0; i < 256; ++i) lut[c][i] = (unsigned char)i;
-          } else {
-            const double scale = __ddiv_rn(255.0, (double)(hi - lo));
-            const double offset = __dmul_rn((double)(-lo), scale);
-            for (int i = 0; i < 256; ++i) {
-              const int v = (int)__dadd_rn(__dmul_rn((double)i, scale), offset);
-              lut[c][i] = (unsigned char)(v < 0 ? 0 : v > 255 ? 255 : v);
-            }
-          }
-        } else {
-          long long tot = 0, last = 0;
-          int nz = 0;
-          for (int i = 0; i < 256; ++i) if (h[i]) { tot += h[i]; last = h[i]; ++nz; }
-          const long long step = nz <= 1 ? 0 : (tot - last) / 255;
-          if (!step) {
-            for (int i = 0; i < 256; ++i) lut[c][i] = (unsigned char)i;
-          } else {
-            long long nn = step / 2;
-            for (int i = 0; i < 256; ++i) {
-              const long long v = nn / step;
-              lut[c][i] = (unsigned char)(v > 255 ? 255 : v);
-              nn += h[i];
-            }
-          }
-        }
-      }
+      if (threadIdx.x < 3) hist_lut(op.op, hist[threadIdx.x], lut[threadIdx.x]);   // per channel
     } else {
-      for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) {
-        const int v = i & 255;
-        int r = v;
-        if (op.op == OP_INVERT) r = 255 - v;
-        else if (op.op == OP_POSTERIZE) r = op.v[0] >= 8 ? v : v & (~((1 << (8 - op.v[0])) - 1) & 255);
-        else if (op.op == OP_SOLARIZE) r = v < op.v[0] ? v : 255 - v;
-        else if (op.op == OP_SOLARIZEADD) r = v < 128 ? min(255, v + op.v[0]) : v;
-        lut[i >> 8][v] = (unsigned char)r;
-      }
+      for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i >> 8][i & 255] = (unsigned char)point_lut(op, i & 255);
     }
     __syncthreads();
     for (int i = threadIdx.x; i < n_all; i += blockDim.x) sm_img[i] = lut[i / n_pix][sm_img[i]];
@@ -436,14 +459,35 @@ __device__ __forceinline__ void hsv_to_rgb_px(int h, int s, int v, int& r, int& 
   }
 }
 
+// np.int32(hue_factor * 255).astype(np.uint8)
+__device__ __forceinline__ int hue_shift(double hue) { return (int)(unsigned char)(int)__dmul_rn(hue, 255.0); }
+
+// adjust_hue of pixel i of the planar image img [3][plane], in place
+__device__ __forceinline__ void hue_px(unsigned char* img, int plane, int i, int shift) {
+  int h, s, v, r, gg, b;
+  rgb_to_hsv_px(img[i], img[plane + i], img[2 * plane + i], h, s, v);
+  hsv_to_rgb_px((h + shift) & 255, s, v, r, gg, b);
+  img[i] = (unsigned char)r;
+  img[plane + i] = (unsigned char)gg;
+  img[2 * plane + i] = (unsigned char)b;
+}
+
+__device__ __forceinline__ bool jitter_any(const cotb200_aug_jitter& p) {
+  bool any = p.vflip != 0;
+  for (int k = 0; k < JIT_COUNT; ++k) any = any || p.order[k] >= 0;
+  return any;
+}
+
+__device__ __forceinline__ int jitter_enhance_op(int op) {
+  return op == JIT_BRIGHTNESS ? OP_BRIGHTNESS : op == JIT_CONTRAST ? OP_CONTRAST : OP_COLOR;
+}
+
 __global__ void __launch_bounds__(RA_THREADS)
 aug_jitter_kernel(const cotb200_aug_jitter* __restrict__ params, int S, unsigned char* out) {
   extern __shared__ unsigned char sm_img[];          // [3][S][S]
   __shared__ unsigned long long lsum;
   const cotb200_aug_jitter p = params[blockIdx.x];
-  bool any = p.vflip != 0;
-  for (int k = 0; k < JIT_COUNT; ++k) any = any || p.order[k] >= 0;
-  if (!any) return;                                  // the image stays as resize-crop wrote it
+  if (!jitter_any(p)) return;                        // the image stays as resize-crop wrote it
   const int n_pix = S * S, n_all = 3 * n_pix;
   unsigned char* g = out + (long long)blockIdx.x * n_all;
   for (int i = threadIdx.x; i < n_all; i += blockDim.x) {
@@ -455,27 +499,290 @@ aug_jitter_kernel(const cotb200_aug_jitter* __restrict__ params, int S, unsigned
     const int op = p.order[k];
     if (op < 0) continue;
     if (op == JIT_HUE) {
-      const int shift = (int)(unsigned char)(int)__dmul_rn(p.hue, 255.0);   // np.int32(hue_factor * 255).astype(np.uint8)
-      for (int i = threadIdx.x; i < n_pix; i += blockDim.x) {
-        int h, s, v, r, gg, b;
-        rgb_to_hsv_px(sm_img[i], sm_img[n_pix + i], sm_img[2 * n_pix + i], h, s, v);
-        hsv_to_rgb_px((h + shift) & 255, s, v, r, gg, b);
-        sm_img[i] = (unsigned char)r;
-        sm_img[n_pix + i] = (unsigned char)gg;
-        sm_img[2 * n_pix + i] = (unsigned char)b;
-      }
+      const int shift = hue_shift(p.hue);
+      for (int i = threadIdx.x; i < n_pix; i += blockDim.x) hue_px(sm_img, n_pix, i, shift);
       __syncthreads();
     } else {
-      enhance_blend(sm_img, n_pix, op == JIT_BRIGHTNESS ? OP_BRIGHTNESS : op == JIT_CONTRAST ? OP_CONTRAST : OP_COLOR, p.factor[op], &lsum);
+      enhance_blend(sm_img, n_pix, jitter_enhance_op(op), p.factor[op], &lsum);
     }
   }
   for (int i = threadIdx.x; i < n_all; i += blockDim.x) g[i] = sm_img[i];
 }
 
+// ---------------------------------------------------------------- the same two transforms on thread-block clusters (S <= 512)
+// An S x S x 3 image above 261 rows does not fit the 200 KB budget of one CTA, so one cluster of cs CTAs holds it: CTA r keeps
+// rows [r R, min(S, (r + 1) R)) of all three planes (R = ceil(S / cs)) in its shared memory.  The whole-image quantities
+// (AutoContrast's and Equalize's histograms, Contrast's L sum) are integer sums: each CTA builds its band's partial, and after a
+// cluster barrier every CTA adds the cs partials in rank order through distributed shared memory, so every CTA holds the exact
+// total the one-CTA kernel computes and builds the same LUT or mean.  A cluster barrier follows every such read, before the
+// partial is rebuilt and before any CTA exits, since a CTA's shared memory must outlive its neighbours' reads of it.
+// Ops that read neighbouring rows (Sharpness, the affine ops) read the previous state of the whole image from `out` in global
+// memory, as the one-CTA kernel does; every CTA writes its band there first, and a cluster barrier orders those writes before
+// the other CTAs' reads.
+namespace cg = cooperative_groups;
+
+// barrier.cluster.arrive.release + barrier.cluster.wait.acquire (PTX ISA, "Parallel Synchronization and Communication
+// Instructions: barrier.cluster", and the memory consistency model's release and acquire patterns): every memory access a
+// thread of the cluster made before its arrive, to shared, distributed shared or global memory, happens before every access a
+// thread of the cluster makes after its wait.  It also synchronises the threads of each CTA, as __syncthreads does.
+__device__ __forceinline__ void cluster_barrier() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+struct Band {
+  int img, rank, cs, y0, plane;      // the image of this cluster, this CTA's rank, its first row and its rows * S
+};
+
+__device__ __forceinline__ Band band_of(int S, int R) {
+  cg::cluster_group cl = cg::this_cluster();
+  Band b;
+  b.cs = (int)cl.num_blocks();
+  b.rank = (int)cl.block_rank();
+  b.img = blockIdx.x / b.cs;
+  b.y0 = min(S, b.rank * R);
+  b.plane = (min(S, b.y0 + R) - b.y0) * S;
+  return b;
+}
+
+// The whole image's sum of the cs CTAs' partials *part, in rank order (a cluster barrier must precede it).
+__device__ __forceinline__ unsigned long long cluster_sum(unsigned long long* part, int cs) {
+  cg::cluster_group cl = cg::this_cluster();
+  unsigned long long t = 0;
+  for (int r = 0; r < cs; ++r) t += *cl.map_shared_rank(part, r);
+  return t;
+}
+
+// enhance_blend on a band: Contrast's mean comes from the cluster's L sum
+__device__ void enhance_blend_band(unsigned char* img, const Band& b, int n_pix, int op, float factor, unsigned long long* lsum) {
+  int mean = 0;
+  if (op == OP_CONTRAST) {
+    l_sum(img, b.plane, b.plane, lsum);
+    cluster_barrier();
+    const unsigned long long tot = cluster_sum(lsum, b.cs);
+    cluster_barrier();
+    mean = contrast_mean(tot, n_pix);
+  } else {
+    __syncthreads();
+  }
+  enhance_apply(img, b.plane, b.plane, op, factor, mean);
+}
+
+__global__ void __launch_bounds__(RA_THREADS)
+aug_randaug_cluster_kernel(const cotb200_aug_sample* __restrict__ params, int S, int R, unsigned char* out) {
+  extern __shared__ unsigned char sm_img[];          // [3][rows of the band][S]
+  __shared__ int hist[3][256];                       // this band's histograms
+  __shared__ int htot[3][256];                       // the image's
+  __shared__ unsigned char lut[3][256];
+  __shared__ unsigned long long lsum;
+  const Band b = band_of(S, R);
+  const cotb200_aug_sample& p = params[b.img];
+  const int n_pix = S * S, n_band = 3 * b.plane;
+  unsigned char* g = out + (long long)b.img * 3 * n_pix;
+  auto gi = [&](int i) { return (i / b.plane) * n_pix + b.y0 * S + i % b.plane; };   // band index -> image index
+  bool loaded = false, g_current = true;
+  const int fill[3] = {124, 116, 104};
+  for (int s = 0; s < COTB200_AUG_MAX_OPS; ++s) {
+    const cotb200_aug_op op = p.ops[s];
+    if (op.op < 0) continue;
+    if (op.op == OP_SHARPNESS || is_affine(op.op)) {
+      if (!g_current) {
+        for (int i = threadIdx.x; i < n_band; i += blockDim.x) g[gi(i)] = sm_img[i];
+        cluster_barrier();                           // every band is in `out` before any CTA reads its neighbours' rows
+      }
+      for (int i = threadIdx.x; i < n_band; i += blockDim.x) {
+        const int c = i / b.plane, y = b.y0 + (i % b.plane) / S, x = i % S;
+        if (op.op == OP_SHARPNESS) {
+          const unsigned char* pl = g + (long long)c * n_pix;
+          const int v = pl[y * S + x];
+          const int d = (x == 0 || y == 0 || x == S - 1 || y == S - 1) ? v : smooth_px(pl, S, x, y);
+          sm_img[i] = blend_px(d, v, op.factor);
+        } else {
+          sm_img[i] = affine_px(g, S, c, op, x, y, fill[c]);
+        }
+      }
+      cluster_barrier();                             // every CTA has read `out` before any CTA writes its band there again
+      loaded = true;
+      g_current = false;
+      continue;
+    }
+    if (!loaded) {
+      for (int i = threadIdx.x; i < n_band; i += blockDim.x) sm_img[i] = g[gi(i)];
+      loaded = true;
+    }
+    if (op.op == OP_CUTOUT) {                        // the box clipped to the band
+      __syncthreads();
+      const int x0 = max(op.v[0], 0), y0 = max(op.v[1], b.y0), x1 = min(op.v[2], S - 1);
+      const int y1 = min(op.v[3], b.y0 + b.plane / S - 1);
+      const int bw = x1 - x0 + 1, bh = y1 - y0 + 1;
+      if (bw > 0 && bh > 0)
+        for (int i = threadIdx.x; i < 3 * bw * bh; i += blockDim.x) {
+          const int c = i / (bw * bh), y = y0 + (i % (bw * bh)) / bw, x = x0 + i % bw;
+          sm_img[c * b.plane + (y - b.y0) * S + x] = (unsigned char)fill[c];
+        }
+      __syncthreads();
+      g_current = false;
+      continue;
+    }
+    if (op.op >= OP_COLOR && op.op <= OP_BRIGHTNESS) {
+      enhance_blend_band(sm_img, b, n_pix, op.op, op.factor, &lsum);
+      g_current = false;
+      continue;
+    }
+    if (op.op == OP_AUTOCONTRAST || op.op == OP_EQUALIZE) {
+      for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) (&hist[0][0])[i] = 0;
+      __syncthreads();
+      for (int i = threadIdx.x; i < n_band; i += blockDim.x) atomicAdd(&hist[i / b.plane][sm_img[i]], 1);
+      cluster_barrier();
+      cg::cluster_group cl = cg::this_cluster();
+      for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) {
+        int t = 0;
+        for (int r = 0; r < b.cs; ++r) t += cl.map_shared_rank(&hist[0][0], r)[i];
+        (&htot[0][0])[i] = t;
+      }
+      cluster_barrier();
+      if (threadIdx.x < 3) hist_lut(op.op, htot[threadIdx.x], lut[threadIdx.x]);
+    } else {
+      for (int i = threadIdx.x; i < 3 * 256; i += blockDim.x) lut[i >> 8][i & 255] = (unsigned char)point_lut(op, i & 255);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < n_band; i += blockDim.x) sm_img[i] = lut[i / b.plane][sm_img[i]];
+    __syncthreads();
+    g_current = false;
+  }
+  if (!g_current)
+    for (int i = threadIdx.x; i < n_band; i += blockDim.x) g[gi(i)] = sm_img[i];
+}
+
+__global__ void __launch_bounds__(RA_THREADS)
+aug_jitter_cluster_kernel(const cotb200_aug_jitter* __restrict__ params, int S, int R, unsigned char* out) {
+  extern __shared__ unsigned char sm_img[];          // [3][rows of the band][S]
+  __shared__ unsigned long long lsum;
+  const Band b = band_of(S, R);
+  const cotb200_aug_jitter p = params[b.img];
+  if (!jitter_any(p)) return;                        // the whole cluster returns: the image stays as resize-crop wrote it
+  const int n_pix = S * S, n_band = 3 * b.plane;
+  unsigned char* g = out + (long long)b.img * 3 * n_pix;
+  for (int i = threadIdx.x; i < n_band; i += blockDim.x) {
+    const int c = i / b.plane, y = b.y0 + (i % b.plane) / S, x = i % S;
+    sm_img[i] = g[c * n_pix + (p.vflip ? S - 1 - y : y) * S + x];   // the vertical flip reads the mirrored rows
+  }
+  if (p.vflip) cluster_barrier();                    // every CTA has read its mirrored rows before any CTA writes its band
+  __syncthreads();
+  for (int k = 0; k < JIT_COUNT; ++k) {
+    const int op = p.order[k];
+    if (op < 0) continue;
+    if (op == JIT_HUE) {
+      const int shift = hue_shift(p.hue);
+      for (int i = threadIdx.x; i < b.plane; i += blockDim.x) hue_px(sm_img, b.plane, i, shift);
+      __syncthreads();
+    } else {
+      enhance_blend_band(sm_img, b, n_pix, jitter_enhance_op(op), p.factor[op], &lsum);
+    }
+  }
+  for (int i = threadIdx.x; i < n_band; i += blockDim.x) g[(i / b.plane) * n_pix + b.y0 * S + i % b.plane] = sm_img[i];
+}
+
+// ---------------------------------------------------------------- host: argument checks shared by both kernel families
 static int check_samples(const char* what, int N, int S, const cotb200_aug_sample* h) {
   if (!h) { set_error("%s: params_host is NULL", what); return COTB200_ENULL; }
   if (N <= 0 || S <= 0) { set_error("%s: bad dims N=%d S=%d", what, N, S); return COTB200_EINVAL; }
   return 0;
+}
+
+// cotb200_aug_randaug's arguments, for images of at most max_s rows held in the shared memory of `where`
+static int check_randaug(const char* what, int N, int S, int max_s, const char* where, const cotb200_aug_sample* params_host,
+                         const cotb200_aug_sample* params_dev, const unsigned char* out) {
+  int rc = check_samples(what, N, S, params_host);
+  if (rc) return rc;
+  if (!params_dev || !out) { set_error("%s: NULL pointer", what); return COTB200_ENULL; }
+  if (S > max_s) { set_error("%s: S=%d above %d (the image is held in %s)", what, S, max_s, where); return COTB200_EUNSUPPORTED; }
+  for (int n = 0; n < N; ++n)
+    for (int s = 0; s < COTB200_AUG_MAX_OPS; ++s) {
+      const cotb200_aug_op& op = params_host[n].ops[s];
+      bool ok = op.op >= -1 && op.op < OP_COUNT;
+      if (ok && is_affine(op.op)) {
+        ok = op.filter == 0 || op.filter == 1;
+        for (int i = 0; i < 6; ++i) ok = ok && isfinite(op.m[i]);
+      }
+      if (ok && op.op == OP_POSTERIZE) ok = op.v[0] >= 0;
+      if (ok && op.op >= OP_COLOR && op.op <= OP_SHARPNESS) ok = isfinite(op.factor);
+      if (!ok) { set_error("%s: sample %d op %d: unknown op id %d or bad argument", what, n, s, op.op); return COTB200_EINVAL; }
+    }
+  return 0;
+}
+
+// cotb200_aug_color_jitter's arguments, likewise
+static int check_jitter(const char* what, int N, int S, int max_s, const char* where, const cotb200_aug_jitter* params_host,
+                        const cotb200_aug_jitter* params_dev, const unsigned char* out) {
+  if (!params_host) { set_error("%s: params_host is NULL", what); return COTB200_ENULL; }
+  if (N <= 0 || S <= 0) { set_error("%s: bad dims N=%d S=%d", what, N, S); return COTB200_EINVAL; }
+  if (!params_dev || !out) { set_error("%s: NULL pointer", what); return COTB200_ENULL; }
+  if (S > max_s) { set_error("%s: S=%d above %d (the image is held in %s)", what, S, max_s, where); return COTB200_EUNSUPPORTED; }
+  for (int n = 0; n < N; ++n) {
+    const cotb200_aug_jitter& p = params_host[n];
+    if (p.vflip != 0 && p.vflip != 1) { set_error("%s: sample %d: vflip %d not 0 or 1", what, n, p.vflip); return COTB200_EINVAL; }
+    bool seen[JIT_COUNT] = {};
+    for (int k = 0; k < JIT_COUNT; ++k) {
+      const int op = p.order[k];
+      if (op == -1) continue;
+      if (op < -1 || op >= JIT_COUNT || seen[op]) {
+        set_error("%s: sample %d: order[%d] = %d is unknown or repeated", what, n, k, op); return COTB200_EINVAL;
+      }
+      seen[op] = true;
+      if (op == JIT_HUE ? !(p.hue >= -0.5 && p.hue <= 0.5) : !(isfinite(p.factor[op]) && p.factor[op] >= 0.f)) {
+        set_error("%s: sample %d: factor of op %d out of range", what, n, op); return COTB200_EINVAL;
+      }
+    }
+  }
+  return 0;
+}
+
+static const char* const ONE_CTA = "shared memory";
+static const char* const CLUSTER = "the shared memory of a cluster of at most 4 CTAs";
+
+// The cluster size of an S x S image: the smallest cs in 1..4 whose band of ceil(S / cs) rows fits AUG_MAX_SMEM (0: none does)
+static int cluster_size(int S) {
+  for (int cs = 1; cs <= 4; ++cs)
+    if (3LL * ((S + cs - 1) / cs) * S <= AUG_MAX_SMEM) return cs;
+  return 0;
+}
+
+// One cluster of cluster_size(S) CTAs per image.  The occupancy query is memoised per kernel, device and cluster size.
+template <typename P>
+static int launch_cluster(const char* what, void (*kernel)(const P*, int, int, unsigned char*), int N, int S, const P* params_dev,
+                          unsigned char* out, cudaStream_t st) {
+  static int fits[64][5] = {};                       // 0 unknown, 1 fits, -1 does not
+  const int cs = cluster_size(S), R = (S + cs - 1) / cs;
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cs;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.gridDim = dim3(N * cs);
+  cfg.blockDim = dim3(RA_THREADS);
+  cfg.dynamicSmemBytes = (size_t)3 * R * S;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int& f = fits[cur_dev_slot()][cs];
+  if (!f) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AUG_MAX_SMEM);
+    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
+    int clusters = 0;
+    e = cudaOccupancyMaxActiveClusters(&clusters, kernel, &cfg);
+    if (e != cudaSuccess) { set_error("%s: cudaOccupancyMaxActiveClusters: %s", what, cudaGetErrorString(e)); return (int)e; }
+    f = clusters > 0 ? 1 : -1;
+  }
+  if (f < 0) {
+    set_error("%s: the device cannot run a cluster of %d CTAs with %d B of shared memory each (S=%d)", what, cs,
+              (int)cfg.dynamicSmemBytes, S);
+    return COTB200_EUNSUPPORTED;
+  }
+  COTB200_PROF_B(what, 6.0 * N * S * S);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, params_dev, S, R, out);
+  if (e != cudaSuccess) { set_error("%s: %s", what, cudaGetErrorString(e)); return (int)e; }
+  return check_launch(what);
 }
 
 }  // namespace cotb200
@@ -534,22 +841,8 @@ extern "C" int cotb200_aug_resize_crop(int N, int S, const unsigned char* src, l
 
 extern "C" int cotb200_aug_randaug(int N, int S, const cotb200_aug_sample* params_host, const cotb200_aug_sample* params_dev,
                                    unsigned char* out, void* stream) {
-  int rc = check_samples("aug_randaug", N, S, params_host);
+  int rc = check_randaug("aug_randaug", N, S, RA_MAX_S, ONE_CTA, params_host, params_dev, out);
   if (rc) return rc;
-  if (!params_dev || !out) { set_error("aug_randaug: NULL pointer"); return COTB200_ENULL; }
-  if (S > RA_MAX_S) { set_error("aug_randaug: S=%d above %d (the image is held in shared memory)", S, RA_MAX_S); return COTB200_EUNSUPPORTED; }
-  for (int n = 0; n < N; ++n)
-    for (int s = 0; s < COTB200_AUG_MAX_OPS; ++s) {
-      const cotb200_aug_op& op = params_host[n].ops[s];
-      bool ok = op.op >= -1 && op.op < OP_COUNT;
-      if (ok && is_affine(op.op)) {
-        ok = op.filter == 0 || op.filter == 1;
-        for (int i = 0; i < 6; ++i) ok = ok && isfinite(op.m[i]);
-      }
-      if (ok && op.op == OP_POSTERIZE) ok = op.v[0] >= 0;
-      if (ok && op.op >= OP_COLOR && op.op <= OP_SHARPNESS) ok = isfinite(op.factor);
-      if (!ok) { set_error("aug_randaug: sample %d op %d: unknown op id %d or bad argument", n, s, op.op); return COTB200_EINVAL; }
-    }
   cudaStream_t st = (cudaStream_t)stream;
   const int smem = 3 * S * S;
   cudaError_t e = cudaFuncSetAttribute(aug_randaug_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * RA_MAX_S * RA_MAX_S);
@@ -561,30 +854,26 @@ extern "C" int cotb200_aug_randaug(int N, int S, const cotb200_aug_sample* param
 
 extern "C" int cotb200_aug_color_jitter(int N, int S, const cotb200_aug_jitter* params_host, const cotb200_aug_jitter* params_dev,
                                   unsigned char* out, void* stream) {
-  if (!params_host) { set_error("aug_color_jitter: params_host is NULL"); return COTB200_ENULL; }
-  if (N <= 0 || S <= 0) { set_error("aug_color_jitter: bad dims N=%d S=%d", N, S); return COTB200_EINVAL; }
-  if (!params_dev || !out) { set_error("aug_color_jitter: NULL pointer"); return COTB200_ENULL; }
-  if (S > RA_MAX_S) { set_error("aug_color_jitter: S=%d above %d (the image is held in shared memory)", S, RA_MAX_S); return COTB200_EUNSUPPORTED; }
-  for (int n = 0; n < N; ++n) {
-    const cotb200_aug_jitter& p = params_host[n];
-    if (p.vflip != 0 && p.vflip != 1) { set_error("aug_color_jitter: sample %d: vflip %d not 0 or 1", n, p.vflip); return COTB200_EINVAL; }
-    bool seen[JIT_COUNT] = {};
-    for (int k = 0; k < JIT_COUNT; ++k) {
-      const int op = p.order[k];
-      if (op == -1) continue;
-      if (op < -1 || op >= JIT_COUNT || seen[op]) {
-        set_error("aug_color_jitter: sample %d: order[%d] = %d is unknown or repeated", n, k, op); return COTB200_EINVAL;
-      }
-      seen[op] = true;
-      if (op == JIT_HUE ? !(p.hue >= -0.5 && p.hue <= 0.5) : !(isfinite(p.factor[op]) && p.factor[op] >= 0.f)) {
-        set_error("aug_color_jitter: sample %d: factor of op %d out of range", n, op); return COTB200_EINVAL;
-      }
-    }
-  }
+  const int rc = check_jitter("aug_color_jitter", N, S, RA_MAX_S, ONE_CTA, params_host, params_dev, out);
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaFuncSetAttribute(aug_jitter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * RA_MAX_S * RA_MAX_S);
   if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
   COTB200_PROF_B("aug_jitter", 6.0 * N * S * S);
   aug_jitter_kernel<<<N, RA_THREADS, 3 * S * S, st>>>(params_dev, S, out);
   return check_launch("aug_jitter");
+}
+
+extern "C" int cotb200_aug_randaug_cluster(int N, int S, const cotb200_aug_sample* params_host, const cotb200_aug_sample* params_dev,
+                                           unsigned char* out, void* stream) {
+  const int rc = check_randaug("aug_randaug_cluster", N, S, COTB200_AUG_CLUSTER_MAX_S, CLUSTER, params_host, params_dev, out);
+  if (rc) return rc;
+  return launch_cluster("aug_randaug_cluster", aug_randaug_cluster_kernel, N, S, params_dev, out, (cudaStream_t)stream);
+}
+
+extern "C" int cotb200_aug_color_jitter_cluster(int N, int S, const cotb200_aug_jitter* params_host, const cotb200_aug_jitter* params_dev,
+                                                unsigned char* out, void* stream) {
+  const int rc = check_jitter("aug_color_jitter_cluster", N, S, COTB200_AUG_CLUSTER_MAX_S, CLUSTER, params_host, params_dev, out);
+  if (rc) return rc;
+  return launch_cluster("aug_jitter_cluster", aug_jitter_cluster_kernel, N, S, params_dev, out, (cudaStream_t)stream);
 }

@@ -560,6 +560,16 @@ typedef struct cotb200_aug_jitter {
  * [-0.5, 0.5]; S above 256 with COTB200_EUNSUPPORTED. */
 int cotb200_aug_color_jitter(int N, int S, const cotb200_aug_jitter* params_host, const cotb200_aug_jitter* params_dev,
                        unsigned char* out, void* stream);
+/* cotb200_aug_randaug and cotb200_aug_color_jitter for 1 <= S <= COTB200_AUG_CLUSTER_MAX_S: the same arguments, validation and
+ * bytes, with the image held by one thread-block cluster instead of one CTA.  The cluster has the fewest CTAs (1..4) for which
+ * a band of ceil(S / cs) rows of the three planes fits 200 KB of shared memory (cs = 1 up to S = 261, 2 at 288 and 320, 3 at
+ * 384 and 448, 4 at 512); CTA r holds rows [r R, min(S, (r + 1) R)), R = ceil(S / cs).  S above the maximum, or a device that
+ * cannot run such a cluster, gives COTB200_EUNSUPPORTED. */
+#define COTB200_AUG_CLUSTER_MAX_S 512
+int cotb200_aug_randaug_cluster(int N, int S, const cotb200_aug_sample* params_host, const cotb200_aug_sample* params_dev,
+                                unsigned char* out, void* stream);
+int cotb200_aug_color_jitter_cluster(int N, int S, const cotb200_aug_jitter* params_host, const cotb200_aug_jitter* params_dev,
+                                     unsigned char* out, void* stream);
 /* Random erasing of the normalised batch (datasets/random_erasing.py, applied by PrefetchLoader after the normalisation,
  * datasets/loader.py:90-91).  The host draws the boxes; one buffer holds a cotb200_erase header followed directly by its n_boxes
  * cotb200_erase_box entries, grouped by sample n in increasing order, each sample's boxes in draw order with k = 0, 1, ...
