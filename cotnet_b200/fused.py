@@ -597,6 +597,11 @@ def _se_eval_params(se):
 def _cot_tail_eval(u, k, bn, se):
     """Inference form of models/cotnet.py:89-104 in three launches: pool (bn + SiLU + (y + k) summed over the pixels), the
     whole SE MLP + radix-2 softmax (cotb200_se_eval), recombination."""
+    return _cot_tail_eval_stages(u, k, bn, se)[-1]
+
+
+def _cot_tail_eval_stages(u, k, bn, se):
+    """_cot_tail_eval with its intermediates: (ss [4, C] = the BatchNorm fold, psum [B, C], a [B, C, 2], out)."""
     B, C, H, W = u.shape
     lib, st, dt = _lib.load(), _lib.stream_ptr(u), _lib.dtype_code(u)
     ss = _bn_prepare(bn, bn.weight, bn.bias, C, float(B * H * W), None, u.device, st)
@@ -611,7 +616,7 @@ def _cot_tail_eval(u, k, bn, se):
     out = torch.empty_like(u, memory_format=torch.channels_last)
     _lib.check(lib.cotb200_tail_combine(dt, B, H * W, C, u.data_ptr(), k.data_ptr(), ss[0].data_ptr(), ss[1].data_ptr(), a.data_ptr(),
                                         out.data_ptr(), st), "tail_combine")
-    return out
+    return ss, psum, a, out
 
 
 def cot_tail(u, k, bn: torch.nn.BatchNorm2d, se: torch.nn.Module):

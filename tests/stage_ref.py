@@ -21,6 +21,11 @@ U32 = 2.0 ** -24
 SIGMOID_ERR_16 = 2.0 ** -11
 #: fp32 tensors: __fdividef(1, 1 + __expf(-z)): a few ulp of 1
 SIGMOID_ERR_32 = 2.0 ** -20
+#: __expf(x) is within (2 + floor(|1.173 * x|)) ulp of e^x: CUDA C++ Programming Guide (12.x), appendix "Mathematical Functions",
+#: table "Single-Precision Floating-Point Intrinsic Functions".  Results below the normal range are flushed to zero (ex2.approx.ftz).
+EXPF_ULP_BASE, EXPF_ULP_SLOPE = 2.0, 1.173
+#: rsqrtf (torch.rsqrt of an fp32 CUDA tensor) is within 2 ulp: the same guide, table "Single-Precision Mathematical Functions"
+RSQRTF_ULP = 2.0
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -70,6 +75,60 @@ def store_bound(exact, err, dtype):
     if dtype == torch.bfloat16:
         return err + 0.5 * ulp(exact.abs() + err, 8)
     raise ValueError(dtype)
+
+
+def epilogue_ref(acc, scale, shift, relu):
+    """The wgmma epilogue on an exact fp64 accumulator: fmaf(acc, scale, shift) (one fp32 rounding; scale None = 1, shift None =
+    0), ReLU, then the bf16 store.  Exact whenever acc * scale + shift is exact in fp64 (small-integer acc, fp32 scale / shift)."""
+    z = acc.double()
+    if scale is not None:
+        z = z * scale.double()
+    if shift is not None:
+        z = z + shift.double()
+    z = f32(z)
+    return bf16(z.clamp_min(0.0) if relu else z)
+
+
+def expf_rel_err(x):
+    """relative error bound of __expf at fp64 arguments x (EXPF_ULP_*; an ulp of a normal fp32 result is at most 2^-23 of it)"""
+    return (EXPF_ULP_BASE + torch.floor(EXPF_ULP_SLOPE * x.abs())) * 2.0 ** -23
+
+
+def softmax2_fast_ref(z, e):
+    """cotb200_se_eval's radix-2 softmax on logits z [..., 2] (fp64, each within e of the fp32 logits the kernel holds):
+    m = max(u, v), eu = __expf(u - m), ev = __expf(v - m), a = e_r * (1 / (eu + ev)).  Returns (softmax(z), bound).
+
+    Relative errors d0, d1 of eu, ev move a_r by a_r * a_(1-r) * (d0 + d1) to first order.  Each d_r is __expf's own error plus
+    that of its argument: u - m rounds once (not exact when u and m differ in sign or scale), an absolute u|u - m| that moves the
+    exponential by the same relative amount.  The sum, the IEEE division and the product round three times (3u of a_r); a flushed
+    __expf result (an argument below -87) leaves a_r < 2^-125.  A logit error moves a_r by at most (e_u + e_v) / 4 (the softmax's
+    derivative, a0 * a1 <= 1/4), which also bounds the shift of the arguments."""
+    a = torch.softmax(z.double(), -1)
+    es = e.double().sum(-1, keepdim=True)
+    d = z.double() - z.double().max(-1, keepdim=True)[0]
+    arg = d.abs() + es
+    dexp = (expf_rel_err(arg) + U32 * arg).sum(-1, keepdim=True)
+    ap = a + 0.25 * es
+    return a, 0.25 * es + ap * (ap.flip(-1) * dexp + 3 * U32) * 1.01 + 2.0 ** -125
+
+
+def fold_bound(bn):
+    """fp64 eval-mode BatchNorm fold of the module's running statistics and a bound of each fp32 result, for the three forms the
+    library uses (CotLayer._tc_params and fused._se_eval_params: torch ops; _bn_eval_fold: bn_finalize):
+      rstd  = rsqrt(fl(var + eps)): RSQRTF_ULP ulp (an ulp is at most 2u of the result), plus u/2 from the add and u/2 from eps as fp32
+      scale = fl(gamma * rstd): one more u
+      shift = fl(beta - fl(mean * scale)) (or one fma): |mean * scale| * (rel(scale) + u) + u |shift|
+    First order, with a 1% margin for the products of the small relative errors.  Returns dict of values and absolute bounds."""
+    rv, rm = bn.running_var.detach().double(), bn.running_mean.detach().double()
+    g = bn.weight.detach().double() if bn.weight is not None else torch.ones_like(rv)
+    b = bn.bias.detach().double() if bn.bias is not None else torch.zeros_like(rv)
+    rstd = 1.0 / torch.sqrt(rv + bn.eps)
+    rel_r = 2 * RSQRTF_ULP * U32 + U32
+    rel_s = rel_r + U32
+    scale = g * rstd
+    shift = b - rm * scale
+    return dict(rstd=rstd, rstd_err=1.01 * rel_r * rstd, scale=scale, scale_err=1.01 * rel_s * scale.abs(), shift=shift,
+                shift_err=1.01 * ((rel_s + U32) * (rm * scale).abs() + U32 * shift.abs()))
 
 
 def within(got, exact, bound, what):
@@ -454,8 +513,9 @@ def gn9_bwd_ref(dg_ref_order, xh, gam, rstd, n_group):
                 dlbias_abs=dl.abs().sum((0, 2, 3)), dlbias_err=dl_err.sum((0, 2, 3)))
 
 
-def _mlp_fwd(p, mods, kind, training):
-    """fp64 forward of the tail MLP with a first-order bound of each fp32 intermediate (dict of values and errors)"""
+def _mlp_fwd(p, mods, kind, training, se_eval=False):
+    """fp64 forward of the tail MLP with a first-order bound of each fp32 intermediate (dict of values and errors).
+    se_eval: the inference kernel cotb200_se_eval instead of the fp32 PyTorch MLP (see mlp_ref)."""
     c0, b1, c3 = mods
     F = torch.nn.functional
     B, C = p.shape
@@ -463,8 +523,22 @@ def _mlp_fwd(p, mods, kind, training):
     w3, bb3 = c3.weight.detach().double().flatten(1), (c3.bias.detach().double() if c3.bias is not None else 0.0)
     p = p.detach().double()
     z1 = p @ w0.t() + bb0
-    e1 = gamma(w0.shape[1] + 1) * (p.abs() @ w0.abs().t() + (bb0.abs() if torch.is_tensor(bb0) else 0.0))
+    # the kernel forms its operand psum * inv_hw in fp32: one more rounding in the chain
+    e1 = gamma(w0.shape[1] + (2 if se_eval else 1)) * (p.abs() @ w0.abs().t() + (bb0.abs() if torch.is_tensor(bb0) else 0.0))
     g1, be1 = b1.weight.detach().double(), b1.bias.detach().double()
+    if se_eval:
+        # fmaf(fl(acc + b0), s1, t1) with the fold of fused._se_eval_params (fold_bound): the chain's error, u of the add, the
+        # fold's errors of s1 (times |z1|) and t1, then u of the fma
+        assert not training and kind == "cot"
+        fb = fold_bound(b1)
+        s1 = fb["scale"]
+        z2 = z1 * s1 + fb["shift"]
+        e2 = s1.abs() * (e1 + U32 * z1.abs()) + fb["scale_err"] * z1.abs() + fb["shift_err"] + U32 * z2.abs()
+        h, eh = torch.relu(z2), e2
+        z3 = h @ w3.t() + bb3
+        e3 = eh @ w3.abs().t() + gamma(w3.shape[1] + 1) * (h.abs() @ w3.abs().t() + (bb3.abs() if torch.is_tensor(bb3) else 0.0))
+        a, ea = softmax2_fast_ref(z3.view(B, C, 2), e3.view(B, C, 2))
+        return dict(p=p, z1=z1, e1=e1, z2=z2, e2=e2, h=h, eh=eh, a=a, ea=ea)
     if training:
         mu = z1.mean(0, keepdim=True)
         sd = torch.sqrt(z1.var(0, unbiased=False, keepdim=True) + b1.eps)
@@ -495,10 +569,12 @@ def _mlp_fwd(p, mods, kind, training):
     return dict(p=p, w0=w0, w3=w3, z1=z1, e1=e1, g1=g1, sd=sd, e_sd=e_sd, zh=zh, e_h=e_h, z2=z2, e2=e2, h=h, eh=eh, a=a, ea=ea)
 
 
-def mlp_ref(p, mods, kind, training):
+def mlp_ref(p, mods, kind, training, se_eval=False):
     """the CoT `se` MLP (+ radix-2 softmax) or the split-attention gate MLP (+ sigmoid) in fp64 on the pooled mean p [B, C], and a
-    first-order bound of the fp32 result.  mods: (conv0, bn, conv3)."""
-    f = _mlp_fwd(p, mods, kind, training)
+    first-order bound of the fp32 result.  mods: (conv0, bn, conv3).  The default bounds the fp32 PyTorch MLP (a correctly rounded
+    exp); se_eval=True bounds cotb200_se_eval instead: the BatchNorm folded into the fc1 epilogue and the __expf softmax
+    (softmax2_fast_ref), with p = psum * inv_hw as the kernel's fp32 operands give it."""
+    f = _mlp_fwd(p, mods, kind, training, se_eval)
     return f["a"], f["ea"]
 
 
@@ -605,6 +681,27 @@ def tail_bwd_ref(u, k, scale, shift, mean, rstd, a_c, dout, dpn, training, sig_e
         out["dk"] = do * a1 + dpp
         out["dk_err"] = 4 * U * ((do * a1).abs() + dpp.abs())
     return out
+
+
+def tail_pool_ref(u, k, scale, shift, sig_err):
+    """cotb200_tail_pool in fp64 from the recorded u, k and fp32 scale / shift: psum[b, c] = sum over the pixels of silu(u*scale +
+    shift) + k, with its bound (the fma, the sigmoid's sig_err, any order of the HW-term sum); also y and its bound for the combine"""
+    sc, sh = scale.double().view(1, -1, 1, 1), shift.double().view(1, -1, 1, 1)
+    z = u.double() * sc + sh
+    ze = 4 * U32 * ((u.double() * sc).abs() + sh.abs())
+    y = torch.nn.functional.silu(z)
+    ye = z.abs() * sig_err + 1.1 * ze + 4 * U32 * y.abs()
+    t = y + k.double()
+    HW = u.shape[2] * u.shape[3]
+    return t.sum((2, 3)), ye.sum((2, 3)) + gamma(HW + 1) * t.abs().sum((2, 3)), y, ye
+
+
+def tail_combine_ref(y, ye, k, a):
+    """cotb200_tail_combine in fp64: out = a0 * y + a1 * k from the recorded a, and the fp32 bound (before the storage rounding)"""
+    B, C = a.shape[0], a.shape[1]
+    a0, a1 = a[..., 0].double().view(B, C, 1, 1), a[..., 1].double().view(B, C, 1, 1)
+    o = a0 * y + a1 * k.double()
+    return o, a0.abs() * ye + 4 * U32 * (o.abs() + (a1 * k.double()).abs())
 
 
 def agg_ref(v, w, fold, gc):

@@ -2,7 +2,9 @@
 (tests/stage_ref.py): BNActFn, GroupNorm9Fn, FanOutFn, CotTailFn (forward and backward, with its MLP), AggTapFn, Pool3x3S2Fn,
 TcConv1x1Fn, TcConv3x3Fn and StemConvBNFn in the configurations the CoT blocks reach, and cotnet50 CoT bottlenecks of stages 1, 2 and
 4 parameter by parameter.  Not covered here: DropBlockFn / DropBlockResReluFn, the CoXt, DropBlock, stochastic-depth, stem and hybrid
-blocks, and whole-model steps.
+blocks, and whole-model steps.  Eval-mode flags are checked only under grad, where CotLayer takes _forward_fused and cot_tail takes
+CotTailFn; the inference path (_forward_tc_eval, _cot_tail_eval, cotb200_se_eval) is tested in test_eval_kernels_gpu.py and
+test_eval_stages_gpu.py.
 
 Bounds are per element: 1/2 ulp of the stored dtype plus the fp32 error of the stage, with fp32 sums bounded by gamma(n) * sum|terms|
 (gamma_tc(n), 2u per add, on the tensor cores) for the chain length n of the kernel.  Where operands are small integers the GEMM /
