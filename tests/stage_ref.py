@@ -68,6 +68,13 @@ def gamma_tc(n):
     return nu / (1.0 - nu)
 
 
+def gamma_bf16(n):
+    """gamma_n for bf16 adds (u = 2^-8): autograd sums the gradients of a tensor with several consumers in its dtype"""
+    nu = n * 2.0 ** -8
+    assert nu < 1.0
+    return nu / (1.0 - nu)
+
+
 def store_bound(exact, err, dtype):
     """|stored - exact| bound of a value computed in fp32 within `err` of `exact` and stored as `dtype` (round to nearest)"""
     if dtype == torch.float32:
@@ -172,12 +179,32 @@ SOURCE_ANCHORS = {
         "rcode = 0 if not relu else (2 if res is None else (3 if mask is not None else 1))",
         "rcode = 3 if mask is not None else (2 if res is None else 1)",
         "rcode = 0 if not relu else (2 if (batch and BN_MASK) else 1)",
+        "return 8 if (wc // fold) % 8 == 0 else 0",
     ],
     "cotnet_b200/cot_layer.py": [
         "big = B * H * W >= fused.TC_MIN_PIXELS",
         "if big and self.dim <= fused.TC_KEY_MAX_DIM and tc_ok and self.key_embed[0].weight.dtype == x.dtype:",
         "if tc_ok and big:",
         "if x.dtype == torch.bfloat16 and C % 16 == 0 and k.dtype == x.dtype and w0.dtype == x.dtype:",
+        "k = fused.bn_act(F.conv2d(xk, wkey, None, 1, self.kernel_size // 2).contiguous(memory_format=cl), self.key_embed[1], relu=True)",
+        "v = fused.bn_act(F.conv2d(xv, _dense_from_grouped(cv[0].weight, G)).contiguous(memory_format=cl), cv[1], relu=False)",
+        "gc = fused.tap_chunk(C // 8, self.dw_group)",
+    ],
+    "cotnet_b200/backbone.py": [
+        "y = dropblock.drop_block(y, key, self.drop_block_sites[0], self.drop_block)",
+        "if key is not None:\n            z = fused.conv1x1_bn(y.contiguous(memory_format=cl), self.conv3, self.bn3, relu=False)",
+        "x = fused.max_pool3x3s2(fused.stem_conv_bn(x, self.conv1, self.bn1, relu=True))",
+    ],
+    "cotnet_b200/backbone_hybrid.py": [
+        "if self.radix == 1 and self.cardinality == 1 and fused.supported(x) and drop_block is None:",
+        "if drop_block is not None and fused.supported(x):",
+        "if (width in conv_dim) or (width == c4_dim and block_idx not in c4_idx):",
+        "if stride > 1 and avd:",
+        "if self.avd is not None and self.avd_first:",
+        "if self.avd is not None and not self.avd_first:",
+        "return dict(radix=1, conv_dim={64, 128}, c4_dim=256, c4_idx=set(range(0, n_l3, 2)), **kw)",
+        "stride = 2 if b == 0 else 1",
+        "x = fused.bn_act(c[6](x).contiguous(memory_format=cl), self.bn1, relu=True)",
     ],
     "cotnet_b200/tc.py": [
         "for bn in (64, 128, 192, 256):",
@@ -278,6 +305,7 @@ def stem_wgrad_chain(B, Ho, Wo, sms):
 FUSED_FNS = ("BNActFn", "GroupNorm9Fn", "FanOutFn", "CotTailFn", "AggTapFn", "Pool3x3S2Fn", "TcConv1x1Fn", "TcConv3x3Fn",
              "StemConvBNFn")
 DROPBLOCK_FNS = ("DropBlockFn", "DropBlockResReluFn")
+TRAINER_FNS = ("SoftTargetCrossEntropyFn",)
 
 
 def _snap(v):
@@ -309,10 +337,10 @@ class Recorder:
     to capture `pre` / `dpre` and the BatchNorm statistics of the wgmma functions.  Changes no bit and no launch."""
 
     def __init__(self, monkeypatch):
-        from cotnet_b200 import dropblock, fused
+        from cotnet_b200 import dropblock, fused, trainer
         self.calls = []
         self._stack = []
-        for mod, names in ((fused, FUSED_FNS), (dropblock, DROPBLOCK_FNS)):
+        for mod, names in ((fused, FUSED_FNS), (dropblock, DROPBLOCK_FNS), (trainer, TRAINER_FNS)):
             for n in names:
                 monkeypatch.setattr(mod, n, self._subclass(getattr(mod, n)))
         apply0, bwd0 = fused._bn_apply_batch, fused._bn_bwd
@@ -335,6 +363,15 @@ class Recorder:
             rec._stack[-1].bwd = cap
         monkeypatch.setattr(fused, "_bn_apply_batch", bn_apply_batch)
         monkeypatch.setattr(fused, "_bn_bwd", bn_bwd)
+        # where each DropBlock mask came from: the key, site and DropBlock the caller passed (the DropBlock calls carry them)
+        self._masks = {}
+        device_mask0 = dropblock.device_mask
+
+        def device_mask(x, key, site, spec):
+            mask, count = device_mask0(x, key, site, spec)
+            rec._masks[mask.data_ptr()] = dict(key=_snap(key), site=site, spec=spec)
+            return mask, count
+        monkeypatch.setattr(dropblock, "device_mask", device_mask)
 
     def _subclass(self, cls):
         rec = self
@@ -355,6 +392,8 @@ class Recorder:
                 if cls.__name__ == "CotTailFn":
                     call.extra["p"] = _snap(ctx.graph[0])
                     call.extra["training"] = ctx.training
+                if cls.__name__ in DROPBLOCK_FNS:
+                    call.extra.update(rec._masks[args[1 if cls.__name__ == "DropBlockFn" else 2].data_ptr()])
                 ctx._stage_call = call
                 return out
 
@@ -466,7 +505,10 @@ def gn9_ref(l, lb, gam, beta, mean, rstd, gc, eps):
     xh = ((xg - m) * r).view(B, J, H, W)
     gm, bt = gam.double().view(1, -1, 1, 1), beta.double().view(1, -1, 1, 1)
     out = xh * gm + bt
-    err = 8 * U32 * ((x.abs().view(B, wc, -1) + m.abs()) * r).view(B, J, H, W) * gm.abs() + 4 * U32 * bt.abs()
+    # the kernels (csrc/gn72.cu) apply fmaf(l, a, beta - (mean - lbias) * a) with a = rstd * gamma: the roundings scale with |l|,
+    # |lbias| and |mean| separately, not with |l + lbias| (which cancels when lbias ~ -l)
+    xa = l.double().abs() + (0 if lb is None else lb.double().abs().view(1, -1, 1, 1))
+    err = 8 * U32 * ((xa.contiguous().view(B, wc, -1) + m.abs()) * r).view(B, J, H, W) * gm.abs() + 4 * U32 * bt.abs()
     # statistics: sums of n terms (gamma(n)); var = E[x^2] - mean^2 in fp32
     ax = x.abs().view(B, wc, -1)
     m_err = gamma(n + 1) * ax.mean(2) + 2 * U32 * (lb.double().abs().max() if lb is not None else 0) + U32 * m64.abs()
@@ -683,6 +725,51 @@ def tail_bwd_ref(u, k, scale, shift, mean, rstd, a_c, dout, dpn, training, sig_e
     return out
 
 
+def dense_from_grouped_adjoint(g, groups):
+    """adjoint of cot_layer._dense_from_grouped: the gradient [N, K, ...] of the block-diagonal dense weight -> the gradient of
+    the grouped weight [N, K/groups, ...], the diagonal blocks gathered (a gather: exact in any dtype)"""
+    if groups == 1:
+        return g
+    N, K = g.shape[0], g.shape[1]
+    ng, kg, rest = N // groups, K // groups, tuple(g.shape[2:])
+    idx = torch.arange(groups, device=g.device)
+    return g.reshape((groups, ng, groups, kg) + rest)[idx, :, idx].reshape((N, kg) + rest)
+
+
+def coxt_embed0_adjoint(gx, gk, groups):
+    """adjoint of cot_layer._coxt_embed0_dense: the gradients of the dense operand-pair weights (Wx, Wk) [N, C] -> the gradient
+    of the grouped embed.0 weight [N, 2C/groups, 1, 1], whose input channels interleave x and k (x0, k0, x1, k1, ...)"""
+    N, C = gx.shape[0], gx.shape[1]
+    ng, ch = N // groups, C // groups
+    idx = torch.arange(groups, device=gx.device)
+    bx = gx.reshape(groups, ng, groups, ch)[idx, :, idx]
+    bk = gk.reshape(groups, ng, groups, ch)[idx, :, idx]
+    return torch.stack([bx, bk], 3).reshape(N, 2 * ch, 1, 1)
+
+
+class DerivedRecorder:
+    """Wraps cot_layer._dense_from_grouped / _coxt_embed0_dense, recording only: which parameter each dense weight came from.
+    of[id(parameter)] = [dict(kind="grouped", groups, dense) | dict(kind="embed0", groups, wx, wk)]"""
+
+    def __init__(self, monkeypatch):
+        from cotnet_b200 import cot_layer
+        self.of = {}
+        dfg0, e00 = cot_layer._dense_from_grouped, cot_layer._coxt_embed0_dense
+
+        def dense_from_grouped(w, groups):
+            out = dfg0(w, groups)
+            if groups != 1:
+                self.of.setdefault(id(w), []).append(dict(kind="grouped", groups=groups, dense=out))
+            return out
+
+        def coxt_embed0_dense(w, groups):
+            wx, wk = e00(w, groups)
+            self.of.setdefault(id(w), []).append(dict(kind="embed0", groups=groups, wx=wx, wk=wk))
+            return wx, wk
+        monkeypatch.setattr(cot_layer, "_dense_from_grouped", dense_from_grouped)
+        monkeypatch.setattr(cot_layer, "_coxt_embed0_dense", coxt_embed0_dense)
+
+
 def tail_pool_ref(u, k, scale, shift, sig_err):
     """cotb200_tail_pool in fp64 from the recorded u, k and fp32 scale / shift: psum[b, c] = sum over the pixels of silu(u*scale +
     shift) + k, with its bound (the fma, the sigmoid's sig_err, any order of the HW-term sum); also y and its bound for the combine"""
@@ -754,20 +841,208 @@ BLOCK_CASES = {
 }
 
 
-def bottleneck_calls(B, cin, width, cout, H, stride, min_pixels=TC_MIN_PIXELS):
-    """the forward calls of backbone.Bottleneck._forward_fused with a CotLayer, from the dispatch predicates above"""
+def tap_chunk(wc, fold=1):
+    return 8 if (wc // fold) % 8 == 0 else 0
+
+
+def cot_calls(B, dim, H, min_pixels=TC_MIN_PIXELS):
+    """the forward calls of CotLayer._forward_fused on a bf16 channels_last input (bf16 weights)"""
+    key_tc, e0_tc, rest_tc = cot_dispatch(B, dim, H, H, min_pixels)
+    out = ["FanOutFn(3)", "TcConv3x3Fn" if key_tc else "BNActFn(relu)", "FanOutFn(2)",
+           "TcConv1x1Fn(two,relu)" if e0_tc else "BNActFn(relu)"]
+    out += ["TcConv1x1Fn(one,nobn)", "TcConv1x1Fn(one,bn)"] if rest_tc else ["BNActFn(plain)"]
+    gc = tap_chunk(dim // 8)
+    return out + ["GroupNorm9Fn(gc%d+lbias)" % gc, "AggTapFn(fold1,gc%d)" % gc, "CotTailFn(k)"]
+
+
+def coxt_calls(dim):
+    """the forward calls of CoXtLayer._forward_fused on bf16: the dense key conv on cuDNN, embed.0 on the wgmma GEMM when
+    C % 16 == 0, embed.3 and conv1x1 on cuDNN, the fold-2 GroupNorm and LocalConv"""
+    gc = tap_chunk(dim // 8, 2)
+    return ["FanOutFn(3)", "BNActFn(relu)", "FanOutFn(2)", "TcConv1x1Fn(two,relu)" if dim % 16 == 0 else "BNActFn(relu)",
+            "BNActFn(plain)", "GroupNorm9Fn(gc%d+lbias)" % gc, "AggTapFn(fold2,gc%d)" % gc, "CotTailFn(k)"]
+
+
+def _tail_calls(B, width, cout, Ho, min_pixels, drop_block, ds):
+    """conv3 + bn3 (+ DropBlock) (+ drop path) + residual + ReLU"""
+    tc = conv1x1_tc(width, cout, B * Ho * Ho, 1, min_pixels)
+    if drop_block:
+        return ["TcConv1x1Fn(one,bn)" if tc else "BNActFn(plain)", "DropBlockResReluFn"]
+    return ["TcConv1x1Fn(one,relu+res%s)" % ("+ds" if ds else "") if tc else "BNActFn(relu+res%s)" % ("+ds" if ds else "")]
+
+
+def bottleneck_calls(B, cin, width, cout, H, stride, min_pixels=TC_MIN_PIXELS, coxt=False, drop_block=False, ds=False):
+    """the forward calls of backbone.Bottleneck._forward_fused with a CotLayer (or a CoXtLayer), from the dispatch predicates
+    above; drop_block: a DropBlock key reaches the block (sites bn1 and bn3); ds: a drop_scale reaches it"""
     M = B * H * H
     Ho = H // stride
     out = ["TcConv1x1Fn(one,relu)" if conv1x1_tc(cin, width, M, 1, min_pixels) else "BNActFn(relu)"]
+    if drop_block:
+        out.append("DropBlockFn")
     if stride > 1:
         out.append("Pool3x3S2Fn(avg)")
-    key_tc, e0_tc, rest_tc = cot_dispatch(B, width, Ho, Ho, min_pixels)
-    out += ["FanOutFn(3)", "TcConv3x3Fn" if key_tc else "BNActFn(relu)", "FanOutFn(2)",
-            "TcConv1x1Fn(two,relu)" if e0_tc else "BNActFn(relu)"]
-    out += ["TcConv1x1Fn(one,nobn)", "TcConv1x1Fn(one,bn)"] if rest_tc else ["BNActFn(plain)"]
-    gc = 8 if (width // 8) % 8 == 0 else 0
-    out += ["GroupNorm9Fn(gc%d+lbias)" % gc, "AggTapFn(fold1,gc%d)" % gc, "CotTailFn(k)"]
+    out += coxt_calls(width) if coxt else cot_calls(B, width, Ho, min_pixels)
     if stride > 1 or cin != cout:
         out.append("TcConv1x1Fn(one,bn)" if conv1x1_tc(cin, cout, B * Ho * Ho, stride, min_pixels) else "BNActFn(plain)")
-    out.append("TcConv1x1Fn(one,relu+res)" if conv1x1_tc(width, cout, B * Ho * Ho, 1, min_pixels) else "BNActFn(relu+res)")
+    return out + _tail_calls(B, width, cout, Ho, min_pixels, drop_block, ds)
+
+
+def hybrid_split(width, block_idx, conv_dim=(64, 128), c4_dim=256, c4_idx=(0, 2, 4)):
+    """backbone_hybrid.CoTBottleneck: conv2 is a SplitAttnConv2d (else the CoT layer); se_cotnetd_50's block arguments"""
+    return width in conv_dim or (width == c4_dim and block_idx not in c4_idx)
+
+
+def hybrid_block_calls(B, block_idx, cin, width, H, stride, min_pixels=TC_MIN_PIXELS, drop_block=False, ds=False, avd=False,
+                       avd_first=True):
+    """the forward calls of backbone_hybrid.CoTBottleneck.forward on a bf16 channels_last input: a split-attention conv2 runs
+    the cuDNN 3x3 convolution (stride 2 itself unless avd) and the fused gate tail, or with DropBlock bn0 on BNActFn, the
+    DropBlock and the rest of the gate in torch; a CoT conv2 pools first (avd) at stride 2; the avg_down downsample pools in
+    torch before its 1x1 convolution"""
+    cout = 4 * width
+    Ho = H // stride
+    split = hybrid_split(width, block_idx)
+    pool = stride > 1 and (avd if split else True)
+    out = ["TcConv1x1Fn(one,relu)" if conv1x1_tc(cin, width, B * H * H, 1, min_pixels) else "BNActFn(relu)"]
+    if drop_block:
+        out.append("DropBlockFn")
+    if pool and avd_first:
+        out.append("Pool3x3S2Fn(avg)")
+    if split:
+        out += ["BNActFn(plain)", "DropBlockFn"] if drop_block else ["CotTailFn(gate)"]
+    else:
+        out += cot_calls(B, width, Ho if avd_first else H, min_pixels)
+    if pool and not avd_first:
+        out.append("Pool3x3S2Fn(avg)")
+    if block_idx == 0:
+        out.append("TcConv1x1Fn(one,bn)" if conv1x1_tc(cin, cout, B * Ho * Ho, 1, min_pixels) else "BNActFn(plain)")
+    return out + _tail_calls(B, width, cout, Ho, min_pixels, drop_block, ds)
+
+
+def stem_calls(model, H, W):
+    """the stems: cotnet50's 7x7/s2 StemConvBNFn (wgmma for even sizes) + the max pool; the deep stem's three cuDNN 3x3
+    convolutions, each followed by a BatchNorm + ReLU"""
+    if model == "se_cotnetd_50":
+        return ["BNActFn(relu)"] * 3
+    return ["StemConvBNFn" if stem_tc(H, W, 64) else "BNActFn(relu)", "Pool3x3S2Fn(max)"]
+
+
+def case_calls(c):
+    """the call list of a STEP_BLOCK_CASES entry, from the generators"""
+    mp = TC_MIN_PIXELS if c.get("min_pixels") is None else c["min_pixels"]
+    if c["kind"] == "stem":
+        return stem_calls(c["model"], c["H"], c["W"])
+    db, ds = bool(c.get("sites")), c.get("ds") is not None
+    if c["model"] == "se_cotnetd_50":
+        return hybrid_block_calls(c["B"], int(c["block"].split(".")[1]), c["cin"], c["width"], c["H"], c["stride"], mp, db, ds)
+    return bottleneck_calls(c["B"], c["cin"], c["width"], c["cout"], c["H"], c["stride"], mp, c["model"] != "cotnet50", db, ds)
+
+
+#: Blocks beyond the cotnet50 CoT bottlenecks: CoXt, SE-CoTNetD (split attention, avg_down, c4_idx), stochastic depth, DropBlock
+#: and the two stems.  ds: the drop_scale handed to the block (1.25 = 1/keep at keep 0.8, exact in bf16); sites: the DropBlock
+#: site numbers the block must use in its model (stages 1-2 have none; cotnet50's layer3.0 takes 0 and 1, se_cotnetd_50's
+#: layer3.0 (CoT) 0 and 1, its layer3.1 (split attention: bn1, conv2.bn0, bn3) 2, 3 and 4).  flow: as BLOCK_CASES, plus "c<j>":
+#: the input of the j-th torch convolution of the block (cuDNN glue: conv1 / downsample / conv3 off the wgmma path, the key conv,
+#: embed.3, conv1x1, the split-attention 3x3 and its gate's fc1 / fc2) where it is a recorded call's output or x.
+_DS = (0.0, 1.25)
+_COXT = ["FanOutFn(3)", "BNActFn(relu)", "FanOutFn(2)", "TcConv1x1Fn(two,relu)", "BNActFn(plain)"]
+_COT_E0 = ["FanOutFn(3)", "BNActFn(relu)", "FanOutFn(2)", "TcConv1x1Fn(two,relu)", "BNActFn(plain)", "GroupNorm9Fn(gc8+lbias)",
+           "AggTapFn(fold1,gc8)", "CotTailFn(k)"]
+STEP_BLOCK_CASES = {
+    "coxt_stage1_b2": dict(model="cotnext50_2x48d", kind="block", block="layer1.0", B=2, cin=64, width=96, cout=256, H=56, stride=1,
+        calls=["BNActFn(relu)"] + _COXT + ["GroupNorm9Fn(gc0+lbias)", "AggTapFn(fold2,gc0)", "CotTailFn(k)", "BNActFn(plain)", "BNActFn(relu+res)"],
+        flow=['1.0<-0.0', '10.3<-9.0', '3.0<-2.0', '4.0<-1.2', '4.1<-3.1', '7.0<-5.0', '7.1<-6.0', '8.0<-7.0', '8.1<-3.1', 'c0<-x', 'c1<-1.2', 'c2<-4.0', 'c3<-1.2', 'c4<-x', 'c5<-8.0']),
+    "coxt_stage1_b2_all_wgmma": dict(model="cotnext50_2x48d", kind="block", block="layer1.0", B=2, cin=64, width=96, cout=256, H=56,
+                                     stride=1, min_pixels=0,
+        calls=["TcConv1x1Fn(one,relu)"] + _COXT + ["GroupNorm9Fn(gc0+lbias)", "AggTapFn(fold2,gc0)", "CotTailFn(k)", "TcConv1x1Fn(one,bn)", "TcConv1x1Fn(one,relu+res)"],
+        flow=['0.0<-x', '1.0<-0.0', '10.0<-8.0', '10.8<-9.0', '3.0<-2.0', '4.0<-1.2', '4.1<-3.1', '7.0<-5.0', '7.1<-6.0', '8.0<-7.0', '8.1<-3.1', '9.0<-x', 'c0<-1.2', 'c1<-4.0', 'c2<-1.2']),
+    "coxt_stage2_first_b2": dict(model="cotnext50_2x48d", kind="block", block="layer2.0", B=2, cin=256, width=192, cout=512, H=28,
+                                 stride=2,
+        calls=["BNActFn(relu)", "Pool3x3S2Fn(avg)"] + _COXT + ["GroupNorm9Fn(gc0+lbias)", "AggTapFn(fold2,gc0)", "CotTailFn(k)", "BNActFn(plain)", "BNActFn(relu+res)"],
+        flow=['1.0<-0.0', '11.3<-10.0', '2.0<-1.0', '4.0<-3.0', '5.0<-2.2', '5.1<-4.1', '8.0<-6.0', '8.1<-7.0', '9.0<-8.0', '9.1<-4.1', 'c0<-x', 'c1<-2.2', 'c2<-5.0', 'c3<-2.2', 'c4<-x', 'c5<-9.0']),
+    "coxt_stage4_b2": dict(model="cotnext50_2x48d", kind="block", block="layer4.1", B=2, cin=2048, width=768, cout=2048, H=7, stride=1,
+        calls=["BNActFn(relu)"] + _COXT + ["GroupNorm9Fn(gc8+lbias)", "AggTapFn(fold2,gc8)", "CotTailFn(k)", "BNActFn(relu+res)"],
+        flow=['1.0<-0.0', '3.0<-2.0', '4.0<-1.2', '4.1<-3.1', '7.0<-5.0', '7.1<-6.0', '8.0<-7.0', '8.1<-3.1', '9.3<-x', 'c0<-x', 'c1<-1.2', 'c2<-4.0', 'c3<-1.2', 'c4<-8.0']),
+    "hybrid_stage1_first_b2": dict(model="se_cotnetd_50", kind="block", block="layer1.0", B=2, cin=64, width=64, cout=256, H=56,
+                                   stride=2,
+        calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(plain)", "BNActFn(relu+res)"],
+        flow=['3.3<-2.0', 'c0<-x', 'c1<-0.0', 'c3<-1.0']),
+    "hybrid_stage3_cot_first_b2": dict(model="se_cotnetd_50", kind="block", block="layer3.0", B=2, cin=512, width=256, cout=1024, H=28,
+                                       stride=2,
+        calls=["BNActFn(relu)", "Pool3x3S2Fn(avg)"] + _COT_E0 + ["BNActFn(plain)", "BNActFn(relu+res)"],
+        flow=['1.0<-0.0', '11.3<-10.0', '2.0<-1.0', '4.0<-3.0', '5.0<-2.2', '5.1<-4.1', '8.0<-6.0', '8.1<-7.0', '9.0<-8.0', '9.1<-4.1', 'c0<-x', 'c1<-2.2', 'c2<-5.0', 'c3<-2.2', 'c5<-9.0']),
+    "hybrid_stage3_split_b2": dict(model="se_cotnetd_50", kind="block", block="layer3.1", B=2, cin=1024, width=256, cout=1024, H=14,
+                                   stride=1,
+        calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(relu+res)"],
+        flow=['2.3<-x', 'c0<-x', 'c1<-0.0', 'c2<-1.0']),
+    "hybrid_stage4_first_b2": dict(model="se_cotnetd_50", kind="block", block="layer4.0", B=2, cin=1024, width=512, cout=2048, H=14,
+                                   stride=2,
+        calls=["BNActFn(relu)", "Pool3x3S2Fn(avg)"] + _COT_E0 + ["BNActFn(plain)", "BNActFn(relu+res)"],
+        flow=['1.0<-0.0', '11.3<-10.0', '2.0<-1.0', '4.0<-3.0', '5.0<-2.2', '5.1<-4.1', '8.0<-6.0', '8.1<-7.0', '9.0<-8.0', '9.1<-4.1', 'c0<-x', 'c1<-2.2', 'c2<-5.0', 'c3<-2.2', 'c5<-9.0']),
+    "cotnet_stage2_drop_path_b2": dict(model="cotnet50", kind="block", block="layer2.1", B=2, cin=512, width=128, cout=512, H=28,
+                                       stride=1, ds=_DS,
+        calls=["BNActFn(relu)"] + _COT_E0 + ["BNActFn(relu+res+ds)"],
+        flow=['1.0<-0.0', '3.0<-2.0', '4.0<-1.2', '4.1<-3.1', '7.0<-5.0', '7.1<-6.0', '8.0<-7.0', '8.1<-3.1', '9.3<-x', 'c0<-x', 'c1<-1.2', 'c2<-4.0', 'c3<-1.2', 'c4<-8.0']),
+    "hybrid_stage2_drop_path_b2": dict(model="se_cotnetd_50", kind="block", block="layer2.1", B=2, cin=512, width=128, cout=512, H=28,
+                                       stride=1, ds=_DS,
+        calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(relu+res+ds)"],
+        flow=['2.3<-x', 'c0<-x', 'c1<-0.0', 'c2<-1.0']),
+    "cotnet_stage3_dropblock_b2": dict(model="cotnet50", kind="block", block="layer3.0", B=2, cin=512, width=256, cout=1024, H=28,
+                                       stride=2, sites=(0, 1),
+        calls=["BNActFn(relu)", "DropBlockFn", "Pool3x3S2Fn(avg)"] + _COT_E0 + ["BNActFn(plain)", "BNActFn(plain)", "DropBlockResReluFn"],
+        flow=['1.0<-0.0', '10.0<-9.0', '10.1<-5.1', '13.0<-12.0', '13.1<-11.0', '2.0<-1.0', '3.0<-2.0', '5.0<-4.0', '6.0<-3.2', '6.1<-5.1', '9.0<-7.0', '9.1<-8.0', 'c0<-x', 'c1<-3.2', 'c2<-6.0', 'c3<-3.2', 'c4<-x', 'c5<-10.0']),
+    "hybrid_stage3_split_dropblock_b4": dict(model="se_cotnetd_50", kind="block", block="layer3.1", B=4, cin=1024, width=256, cout=1024,
+                                             H=14, stride=1, sites=(2, 3, 4), ds=(0.0, 1.25, 1.25, 1.25),
+        calls=["BNActFn(relu)", "DropBlockFn", "BNActFn(plain)", "DropBlockFn", "BNActFn(plain)", "DropBlockResReluFn"],
+        flow=['1.0<-0.0', '3.0<-2.0', '5.0<-4.0', '5.1<-x', 'c0<-x', 'c1<-1.0']),
+    "cotnet_stem_wgmma_wgrad": dict(model="cotnet50", kind="stem", B=2, H=96, W=96,
+        calls=["StemConvBNFn", "Pool3x3S2Fn(max)"],
+        flow=['1.0<-0.0']),
+    "cotnet_stem_cudnn_wgrad": dict(model="cotnet50", kind="stem", B=2, H=64, W=72,
+        calls=["StemConvBNFn", "Pool3x3S2Fn(max)"],
+        flow=['1.0<-0.0']),
+    "hybrid_deep_stem": dict(model="se_cotnetd_50", kind="stem", B=2, H=64, W=64,
+        calls=["BNActFn(relu)"] * 3,
+        flow=['c1<-0.0', 'c2<-1.0']),
+}
+
+
+def model_blocks(model, H0):
+    """[(name, block index in its stage, cin, width, cout, H in, stride)] of every bottleneck of cotnet50 / cotnext50_2x48d /
+    se_cotnetd_50 for an H0 x H0 image: cotnet's 7x7/s2 stem and max pool (H0/4), stride 2 from stage 2 on; the deep stem's
+    stride 2 (H0/2), stride 2 in every stage (backbone.CoTResNet, backbone_hybrid.CoTHybridNet)"""
+    hybrid = model == "se_cotnetd_50"
+    H, cin = (H0 // 2, 64) if hybrid else (H0 // 4, 64)
+    out = []
+    for si, (planes, n) in enumerate(zip((64, 128, 256, 512), (3, 4, 6, 3))):
+        width = planes * 48 // 64 * 2 if model == "cotnext50_2x48d" else planes
+        for b in range(n):
+            stride = 2 if b == 0 and (hybrid or si > 0) else 1
+            out.append(("layer%d.%d" % (si + 1, b), b, cin, width, planes * 4, H, stride))
+            cin, H = planes * 4, H // stride
+    return out
+
+
+def model_calls(model, B, H0, min_pixels=TC_MIN_PIXELS):
+    """the recorded calls of one TrainStep forward with drop path (every block but the first) and DropBlock (stages 3-4) on, as
+    [stem calls, [calls of each block], loss calls]"""
+    blocks = []
+    for i, (name, b, cin, width, cout, H, stride) in enumerate(model_blocks(model, H0)):
+        db = name.startswith(("layer3", "layer4"))
+        if model == "se_cotnetd_50":
+            blocks.append(hybrid_block_calls(B, b, cin, width, H, stride, min_pixels, db, i > 0))
+        else:
+            blocks.append(bottleneck_calls(B, cin, width, cout, H, stride, min_pixels, model != "cotnet50", db, i > 0))
+    return stem_calls(model, H0, H0), blocks, ["SoftTargetCrossEntropyFn"]
+
+
+def model_sites(model):
+    """the DropBlock site numbers of every block, counted here in forward order: stages 3-4 only; bn1 and bn3, and conv2.bn0
+    between them in a split-attention block"""
+    out, site = {}, 0
+    for name, b, cin, width, cout, H, stride in model_blocks(model, 224):
+        if not name.startswith(("layer3", "layer4")):
+            continue
+        n = 3 if model == "se_cotnetd_50" and hybrid_split(width, b) else 2
+        out[name] = tuple(range(site, site + n))
+        site += n
     return out

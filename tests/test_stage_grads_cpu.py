@@ -297,3 +297,84 @@ def test_tail_backward_restatement_matches_autograd(kind, train):
     assert torch.allclose(r["dbeta"], bn.bias.grad, rtol=0, atol=1e-12)
     if k is not None:
         assert torch.allclose(r["dk"], k.grad, rtol=0, atol=1e-12)
+
+
+@pytest.mark.parametrize("geo", sorted(S.STEP_BLOCK_CASES))
+def test_step_block_call_lists_follow_the_mirror(geo):
+    """CoXt, SE-CoTNetD, drop-path, DropBlock and stem cases: the pinned list is what the generators derive"""
+    c = S.STEP_BLOCK_CASES[geo]
+    assert S.case_calls(c) == c["calls"]
+
+
+def test_step_block_cases_match_the_models():
+    """each case's geometry is its block's in the model: input / width / output channels, stride, conv2 kind, DropBlock sites"""
+    from cotnet_b200 import backbone, backbone_hybrid
+    from cotnet_b200.backbone_hybrid import SplitAttnConv2d
+    from cotnet_b200.cot_layer import CoXtLayer
+    models = {"cotnet50": backbone.cotnet50(drop_block_rate=0.1), "cotnext50_2x48d": backbone.cotnext50_2x48d(drop_block_rate=0.1),
+              "se_cotnetd_50": backbone_hybrid.se_cotnetd_50(drop_block_rate=0.1)}
+    for geo, c in S.STEP_BLOCK_CASES.items():
+        if c["kind"] != "block":
+            continue
+        m = models[c["model"]]
+        stage, i = c["block"].split(".")
+        blk = getattr(m, stage)[int(i)]
+        assert (blk.conv1.in_channels, blk.conv1.out_channels, blk.conv3.out_channels) == (c["cin"], c["width"], c["cout"]), geo
+        if c["model"] == "se_cotnetd_50":
+            assert isinstance(blk.conv2, SplitAttnConv2d) == S.hybrid_split(c["width"], int(i)), geo
+            assert (2 if int(i) == 0 else 1) == c["stride"]
+        else:
+            assert isinstance(blk.conv2, CoXtLayer) == (c["model"] != "cotnet50") and blk.stride == c["stride"], geo
+        if "sites" in c:
+            assert blk.drop_block_sites == c["sites"], geo
+    # every se_cotnetd_50 block's conv2 kind follows the mirror
+    m = models["se_cotnetd_50"]
+    for stage in ("layer1", "layer2", "layer3", "layer4"):
+        for i, blk in enumerate(getattr(m, stage)):
+            assert isinstance(blk.conv2, SplitAttnConv2d) == S.hybrid_split(blk.conv1.out_channels, i), (stage, i)
+
+
+@pytest.mark.parametrize("groups,shape", [(2, (48, 96, 1, 1)), (8, (96, 12, 3, 3)), (2, (96, 48, 1, 1))])
+def test_dense_from_grouped_adjoint_matches_autograd(groups, shape):
+    """the gather of the diagonal blocks is the gradient autograd gives the grouped weight through _dense_from_grouped, bit for
+    bit (in bf16 too); the dense weight's convolution equals the grouped convolution"""
+    from cotnet_b200.cot_layer import _dense_from_grouped
+    g = torch.Generator().manual_seed(groups + shape[1])
+    for dtype in (torch.float64, torch.bfloat16):
+        w = torch.randn(shape, generator=g).to(dtype).requires_grad_(True)
+        dense = _dense_from_grouped(w, groups)
+        gd = torch.randn(dense.shape, generator=g).to(dtype)
+        dense.backward(gd)
+        got = S.dense_from_grouped_adjoint(gd, groups)
+        assert got.dtype == dtype and torch.equal(got, w.grad)
+    x = torch.randn(2, shape[1] * groups, 5, 5, generator=g, dtype=torch.float64)
+    w = torch.randn(shape, generator=g, dtype=torch.float64)
+    p = shape[2] // 2
+    assert torch.allclose(F.conv2d(x, _dense_from_grouped(w, groups), padding=p), F.conv2d(x, w, padding=p, groups=groups),
+                          rtol=0, atol=1e-12)
+
+
+@pytest.mark.parametrize("C", [96, 192, 768])
+def test_coxt_embed0_adjoint_matches_autograd(C):
+    """the de-interleave of (dWx, dWk) is the gradient autograd gives embed.0's grouped weight through _coxt_embed0_dense and
+    the cat of the concat-free GEMM, bit for bit; and x @ Wx^T + k @ Wk^T is the grouped convolution of the interleave of x, k"""
+    from cotnet_b200.cot_layer import _coxt_embed0_dense
+    G = 2
+    g = torch.Generator().manual_seed(C)
+    for dtype in (torch.float64, torch.bfloat16):
+        w = torch.randn(C // 2, 2 * C // G, 1, 1, generator=g).to(dtype).requires_grad_(True)
+        wx, wk = _coxt_embed0_dense(w, G)
+        w0 = torch.cat([wx, wk], 1).reshape(C // 2, 2 * C, 1, 1)          # as CoXtLayer._forward_fused hands it to the GEMM
+        gd = torch.randn(w0.shape, generator=g).to(dtype)
+        w0.backward(gd)
+        g2 = gd.reshape(C // 2, 2 * C)
+        got = S.coxt_embed0_adjoint(g2[:, :C], g2[:, C:], G)
+        assert got.dtype == dtype and torch.equal(got, w.grad)
+    x = torch.randn(2, C, 3, 3, generator=g, dtype=torch.float64)
+    k = torch.randn(2, C, 3, 3, generator=g, dtype=torch.float64)
+    w = torch.randn(C // 2, 2 * C // G, 1, 1, generator=g, dtype=torch.float64)
+    wx, wk = _coxt_embed0_dense(w, G)
+    qk = torch.stack([x, k], 2).reshape(2, 2 * C, 3, 3)                    # models/cotnet.py:153-154
+    want = F.conv2d(qk, w, groups=G)
+    got = torch.einsum("bchw,nc->bnhw", x, wx) + torch.einsum("bchw,nc->bnhw", k, wk)
+    assert torch.allclose(got, want, rtol=0, atol=1e-12)

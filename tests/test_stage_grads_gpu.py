@@ -1,8 +1,8 @@
 """The bf16 training step's fused autograd functions stage by stage, each stage against fp64 of the inputs it actually received
 (tests/stage_ref.py): BNActFn, GroupNorm9Fn, FanOutFn, CotTailFn (forward and backward, with its MLP), AggTapFn, Pool3x3S2Fn,
 TcConv1x1Fn, TcConv3x3Fn and StemConvBNFn in the configurations the CoT blocks reach, and cotnet50 CoT bottlenecks of stages 1, 2 and
-4 parameter by parameter.  Not covered here: DropBlockFn / DropBlockResReluFn, the CoXt, DropBlock, stochastic-depth, stem and hybrid
-blocks, and whole-model steps.  Eval-mode flags are checked only under grad, where CotLayer takes _forward_fused and cot_tail takes
+4 parameter by parameter.  The DropBlock functions' checks, the CoXt, SE-CoTNetD, DropBlock, stochastic-depth and stem cases and
+the derived-weight accounting are used by test_step_stages_gpu.py.  Not covered: whole-model steps.  Eval-mode flags are checked only under grad, where CotLayer takes _forward_fused and cot_tail takes
 CotTailFn; the inference path (_forward_tc_eval, _cot_tail_eval, cotb200_se_eval) is tested in test_eval_kernels_gpu.py and
 test_eval_stages_gpu.py.
 
@@ -439,6 +439,49 @@ def check_pool(call, what="Pool3x3S2Fn"):
         S.equal(call.gout[0], dxp[:, :, 1:H + 1, 1:W + 1].to(x.dtype), what + " max dx routed by the saved index")
 
 
+def _dropblock_mask(call, x, mask, count, what):
+    """the call's mask and count against dropblock.host_mask for the (key, site, DropBlock) its caller passed; returns the keep
+    mask [B, C, H, W] (fp64, 0 / 1) and the scale as the kernels apply it: fp32 s rounded to the activation dtype"""
+    from cotnet_b200 import dropblock
+    e = call.extra
+    keep, cnt, s = dropblock.host_mask(tuple(x.shape), e["site"], e["key"], e["spec"])
+    m = torch.from_numpy(keep).to(DEV)
+    S.equal(_unpack(mask, x.shape[1]), _rows_of(m), what + " mask == host_mask(key, site %d)" % e["site"])
+    assert int(count.item()) == cnt, "%s: count %d, host count %d" % (what, int(count.item()), cnt)
+    s64 = torch.tensor(float(s), dtype=torch.float64)
+    sb = S.bf16(s64) if x.dtype == BF else (s64 if x.dtype == torch.float32 else s64.to(x.dtype).double())
+    return m.double(), float(sb)
+
+
+def check_dropblock(call, what="DropBlockFn"):
+    """y = x * M * s: x * s of two bf16 values is exact in fp32 and fp64, so the one rounding to bf16 is the whole error and y is
+    compared bit for bit; the backward is the same map on dy"""
+    x, mask, count = call.inp
+    m, s = _dropblock_mask(call, x, mask, count, what)
+    rnd = S.bf16 if x.dtype == BF else S.f32
+    S.equal(call.out.double(), rnd(x.double() * m * s), what + " y = bf16(x * M * s)")
+    if call.gout is not None:
+        S.equal(call.gout[0].double(), rnd(call.gin[0].double() * m * s), what + " dx = bf16(dy * M * s)")
+
+
+def check_dropblock_res_relu(call, what="DropBlockResReluFn"):
+    """y = relu(res + ds[b] * (z * M * s)): z * s is exact in fp32, then one fma (or add): 1/2 ulp of fp32 of |res + ds*a|, then
+    the bf16 store.  dres = dy * [y > 0] exactly; dz = dres * ds[b] * M * s: fl(fl(g * s) * d), the first product exact."""
+    z, res, mask, count, ds = call.inp
+    m, s = _dropblock_mask(call, z, mask, count, what)
+    d = ds.double().view(-1, 1, 1, 1) if ds is not None else 1.0
+    v = res.double() + d * (z.double() * m * s)
+    _w(call.out, torch.relu(v), S.U32 * v.abs(), what + " y", "dropblock_res_relu")
+    if call.gout is None:
+        return
+    dy = call.gin[0].double()
+    dres = dy * (call.out > 0).double()
+    if call.gout[1] is not None:
+        S.equal(call.gout[1].double(), dres, what + " dres = dy * [y > 0]")
+    dz = dres * d * m * s
+    _w(call.gout[0], dz, S.U32 * dz.abs(), what + " dz", "dropblock_res_relu_bwd")
+
+
 def check_call(call, mods=None):
     n = call.name
     if n == "BNActFn":
@@ -460,6 +503,10 @@ def check_call(call, mods=None):
         check_agg(call)
     elif n == "Pool3x3S2Fn":
         check_pool(call)
+    elif n == "DropBlockFn":
+        check_dropblock(call)
+    elif n == "DropBlockResReluFn":
+        check_dropblock_res_relu(call)
     else:
         raise AssertionError("no stage check for " + n)
 
@@ -681,7 +728,8 @@ def test_pool(mode, monkeypatch):
 
 # ------------------------------------------------------------------------------------------------ blocks, parameter by parameter
 class ConvRecorder:
-    """F.conv2d calls (cuDNN glue: key conv, embed.3, trunk convolutions off the wgmma path) with input, weight and incoming gradient"""
+    """F.conv2d calls (cuDNN glue: key conv, embed.3, trunk convolutions off the wgmma path) with input (and its storage), weight,
+    incoming gradient and, for a weight that is not a leaf (the dense weights CoXtLayer derives), the weight's gradient"""
 
     def __init__(self, monkeypatch):
         self.calls = []
@@ -689,16 +737,118 @@ class ConvRecorder:
 
         def conv2d(input, weight, bias=None, stride=1, padding=0, dilation=1, groups=1):
             out = conv0(input, weight, bias, stride, padding, dilation, groups)
-            rec = dict(x=input.detach().clone(), w=weight, stride=stride, padding=padding, dilation=dilation, groups=groups, g=None)
+            rec = dict(x=input.detach().clone(), ptr=input.data_ptr(), w=weight, b=bias, stride=stride, padding=padding,
+                       dilation=dilation, groups=groups, g=None, gw=None, out_ptr=out.data_ptr(), y=out.detach().clone())
             if out.requires_grad:
                 out.register_hook(lambda gr: rec.__setitem__("g", gr.detach().clone()))
+            if weight.requires_grad and weight.grad_fn is not None:
+                weight.register_hook(lambda gr: rec.__setitem__("gw", gr.detach().clone()))
             self.calls.append(rec)
             return out
         monkeypatch.setattr(torch.nn.functional, "conv2d", conv2d)
 
 
-def account_params(model, calls, convs, what):
-    """every trainable parameter's .grad is a recorded returned gradient (bitwise) or the fp64 weight gradient of its torch conv"""
+class TorchBNRecorder:
+    """F.batch_norm calls in training mode (BatchNorms the glue runs in plain PyTorch: the split-attention gate's bn1 when DropBlock
+    sits after bn0) with input, weight, bias and the gradient of the output"""
+
+    def __init__(self, monkeypatch):
+        self.calls = []
+        bn0 = F.batch_norm
+
+        def batch_norm(input, running_mean, running_var, weight=None, bias=None, training=False, momentum=0.1, eps=1e-5):
+            out = bn0(input, running_mean, running_var, weight, bias, training, momentum, eps)
+            rec = dict(x=input.detach().clone(), w=weight, b=bias, training=training, eps=eps, g=None, y=out.detach().clone())
+            if out.requires_grad:
+                out.register_hook(lambda gr: rec.__setitem__("g", gr.detach().clone()))
+            self.calls.append(rec)
+            return out
+        monkeypatch.setattr(torch.nn.functional, "batch_norm", batch_norm)
+
+
+def torch_bn_bwd_ref(r):
+    """fp64 backward of a recorded training-mode torch BatchNorm from its recorded input and output gradient: dx, dgamma, dbeta and
+    bounds.  torch forms the batch statistics in fp32 (Welford): mean within gamma(n+1) mean|x|, var within gamma(2n+2) E[x^2],
+    so rstd within e_r = gamma(2n+2) E[x^2] / (2 var) + 2u relative -- E[x^2] / var is the conditioning |x| / std squared -- and
+    xhat = (x - mean) rstd within |xhat| e_r + e_m rstd.  The sums of n terms add gamma(n+1); results are stored in the
+    parameter / activation dtype (store_bound at the call site)."""
+    x, g = r["x"].double(), r["g"].double()
+    dims = (0,) + tuple(range(2, x.dim()))
+    n = x.numel() // x.shape[1]
+    shp = (1, -1) + (1,) * (x.dim() - 2)
+    m = x.mean(dims, keepdim=True)
+    var = ((x - m) ** 2).mean(dims, keepdim=True)
+    rs = 1.0 / torch.sqrt(var + r["eps"])
+    e2 = (x * x).mean(dims, keepdim=True)
+    e_m = S.gamma(n + 1) * x.abs().mean(dims, keepdim=True)
+    e_r = S.gamma(2 * n + 2) * e2 / (2 * (var + r["eps"])) + 2 * S.U32
+    xh = (x - m) * rs
+    xh_err = xh.abs() * e_r + e_m * rs + 2 * S.U32 * xh.abs()
+    gam = r["w"].detach().double().view(shp) if r["w"] is not None else torch.ones_like(rs)
+    out = dict(dbeta=g.sum(dims), dbeta_err=S.gamma(n + 1) * g.abs().sum(dims),
+               dgamma=(g * xh).sum(dims), dgamma_err=(g.abs() * xh_err).sum(dims) + S.gamma(n + 1) * (g * xh).abs().sum(dims))
+    gd = g * gam
+    c0, c1 = gd.mean(dims, keepdim=True), (gd * xh).mean(dims, keepdim=True)
+    e_c1 = (gd.abs() * xh_err).mean(dims, keepdim=True) + S.gamma(n + 1) * (gd * xh).abs().mean(dims, keepdim=True)
+    out["dx"] = rs * (gd - c0 - xh * c1)
+    out["dx_err"] = (out["dx"].abs() * e_r + rs * (xh_err * c1.abs() + xh.abs() * e_c1 + S.gamma(n + 1) * gd.abs().mean(dims, keepdim=True)
+                                                   + 8 * S.U32 * (gd.abs() + c0.abs() + (xh * c1).abs())))
+    return out
+
+
+def _conv_wgrad_check(r, shape, got, what):
+    """a torch convolution's weight gradient `got` (of weight shape `shape`) against fp64 of its recorded input and gradient"""
+    kw = dict(stride=r["stride"], padding=r["padding"], dilation=r["dilation"], groups=r["groups"])
+    gd = r["g"].double()
+    ref = torch.nn.grad.conv2d_weight(r["x"].double(), shape, gd, **kw)
+    mag = torch.nn.grad.conv2d_weight(r["x"].double().abs(), shape, gd.abs(), **kw)
+    terms = gd.shape[0] * gd.shape[2] * gd.shape[3]
+    # cuDNN's bf16 weight gradients may store split-K partial sums in bf16 before adding them: each partial rounds once, within
+    # 2^-9 of its magnitude, and the partials' magnitudes sum to at most sum|terms|
+    S.within(got, ref, _dw_bound(ref, mag, terms + 1, True, got.dtype) + (2.0 ** -9 * mag if got.dtype == BF else 0.0), what)
+
+
+def _derived_grad(p, entries, calls, convs, what):
+    """the gradient of the dense weight a parameter was derived into, from its one consumer: a TcConv1x1Fn (returned dW, checked
+    by check_tc1x1) or a torch convolution (hooked, checked here against fp64); then its restated adjoint"""
+    (e,) = entries
+    if e["kind"] == "grouped":
+        dense = e["dense"]
+        srcs = [r for r in convs if r["w"] is dense]
+        tcs = [c for c in calls if c.name == "TcConv1x1Fn" and c.args[2] is dense]
+    else:
+        dense = torch.cat([e["wx"], e["wk"]], 1).detach()
+        srcs = [r for r in convs if r["w"].shape[:2] == dense.shape and torch.equal(r["w"].detach().reshape(dense.shape), dense)]
+        tcs = [c for c in calls if c.name == "TcConv1x1Fn" and c.args[2].shape[:2] == dense.shape
+               and torch.equal(c.inp[2].reshape(dense.shape), dense)]
+    assert len(srcs) + len(tcs) == 1, "%s: %d consumers of the dense weight" % (what, len(srcs) + len(tcs))
+    if tcs:
+        gd = tcs[0].gout[2]
+    else:
+        r = srcs[0]
+        gd = r["gw"]
+        assert gd is not None, what + ": the dense weight's gradient was not recorded"
+        _conv_wgrad_check(r, tuple(r["w"].shape), gd, what + " dense weight gradient")
+    if e["kind"] == "grouped":
+        return S.dense_from_grouped_adjoint(gd, e["groups"])
+    C = dense.shape[1] // 2
+    g2 = gd.reshape(dense.shape)
+    return S.coxt_embed0_adjoint(g2[:, :C], g2[:, C:], e["groups"])
+
+
+def _leaf_of(t):
+    """the parameter behind an autocast copy (ToCopyBackward -> AccumulateGrad), or t itself"""
+    fn = t.grad_fn
+    if fn is not None and type(fn).__name__.startswith("ToCopyBackward"):
+        v = getattr(fn.next_functions[0][0], "variable", None)
+        return v if v is not None else t
+    return t
+
+
+def account_params(model, calls, convs, what, derived=None, skip=(), bns=()):
+    """every trainable parameter's .grad is a recorded returned gradient (bitwise), the fp64 weight (or bias) gradient of its torch
+    conv, the fp64 gradient of its torch BatchNorm (bns: TorchBNRecorder.calls), or (derived: DerivedRecorder.of) bit for bit the
+    restated adjoint of the gradient of the dense weight it was derived into.  `skip`: names checked elsewhere."""
     owner = {}
     for c in calls:
         for i, a in enumerate(c.args):
@@ -707,7 +857,17 @@ def account_params(model, calls, convs, what):
     conv_of = {}
     for r in convs:
         conv_of.setdefault(id(r["w"]), []).append(r)
+    derived = derived or {}
+    bias_of = {id(_leaf_of(r["b"])): r for r in convs if r["b"] is not None}
+    bn_of = {}
+    for r in bns:
+        if r["training"] and r["g"] is not None:
+            for k in ("w", "b"):
+                if r[k] is not None:
+                    bn_of.setdefault(id(r[k]), []).append((k, r))
     for name, p in model.named_parameters():
+        if name in skip:
+            continue
         assert p.grad is not None and bool((p.grad != 0).any()), "%s %s: no or zero gradient" % (what, name)
         src = owner.get(id(p), [])
         if len(src) == 1:
@@ -715,14 +875,31 @@ def account_params(model, calls, convs, what):
             S.equal(p.grad, c.gout[i], "%s %s: .grad == %s's returned gradient %d" % (what, name, c.name, i))
             continue
         assert not src, "%s %s: %d recorded contributors" % (what, name, len(src))
+        if id(p) in derived:
+            assert id(p) not in conv_of, "%s %s: used directly and through a derived weight" % (what, name)
+            ref = _derived_grad(p, derived[id(p)], calls, convs, "%s %s" % (what, name))
+            S.equal(p.grad, ref.to(p.grad.dtype), "%s %s: .grad == the adjoint of its dense weight's gradient" % (what, name))
+            continue
+        if id(p) in bias_of:
+            r = bias_of[id(p)]
+            gd = r["g"].double()
+            ref = gd.sum((0, 2, 3))
+            err = S.gamma(gd.numel() // gd.shape[1] + 1) * gd.abs().sum((0, 2, 3))
+            dt = r["y"].dtype                     # under autocast an fp32 bias is used (and differentiated) as a bf16 copy
+            S.within(p.grad, ref, S.store_bound(ref, err, dt) if dt != torch.float32 else err + S.ulp(ref, 24),
+                     "%s %s: torch conv bias gradient" % (what, name))
+            continue
+        if id(p) in bn_of:
+            ((k, r),) = bn_of[id(p)]
+            br = torch_bn_bwd_ref(r)
+            key = "dgamma" if k == "w" else "dbeta"
+            ref, err = br[key], br[key + "_err"]
+            S.within(p.grad, ref, S.store_bound(ref, err, p.grad.dtype) if p.grad.dtype != torch.float32 else err + S.ulp(ref, 24),
+                     "%s %s: torch BatchNorm %s" % (what, name, key))
+            continue
         (r,) = conv_of.get(id(p), [None])
         assert r is not None, "%s %s: gradient from no recorded call" % (what, name)
-        kw = dict(stride=r["stride"], padding=r["padding"], dilation=r["dilation"], groups=r["groups"])
-        gd = r["g"].double()
-        ref = torch.nn.grad.conv2d_weight(r["x"].double(), p.shape, gd, **kw)
-        mag = torch.nn.grad.conv2d_weight(r["x"].double().abs(), p.shape, gd.abs(), **kw)
-        terms = gd.shape[0] * gd.shape[2] * gd.shape[3]
-        S.within(p.grad, ref, _dw_bound(ref, mag, terms + 1, True, p.grad.dtype), "%s %s: torch conv weight gradient" % (what, name))
+        _conv_wgrad_check(r, p.shape, p.grad, "%s %s: torch conv weight gradient" % (what, name))
 
 
 def _cfg(call):
