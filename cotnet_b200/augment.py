@@ -3,7 +3,9 @@
 DataLoader workers still decode (JPEG -> RGB uint8 HWC, the reference dataset's ``.convert('RGB')``).  From there:
 
 * ``TrainAugment``: RandomResizedCrop(scale, ratio, interpolation) + RandomHorizontalFlip(0.5) + RandAugment
-  (``rand-m15-mstd0.5-n2`` and its hyper-parameters, datasets/transforms_factory.py:44-129).  ``draw`` consumes a
+  (``rand-m15-mstd0.5-n2`` and every config rand_augment_transform parses: any magnitude, std and number of layers, and the
+  weighted op choice ``w0``; datasets/transforms_factory.py:44-129).  Two ops per sample go in one RandAugment launch, so
+  ``n`` layers take ceil(n / 2) launches in sequence on the same images.  ``draw`` consumes a
   ``random.Random``, an ``np.random.RandomState`` and a torch CPU ``Generator`` in the reference's call order, so a seeded draw
   equals what the reference's transforms draw from the global generators; ``collate`` does that inside DataLoader workers
   and packs the batch into one ragged buffer; ``__call__`` runs the kernels (cotb200_aug_resize_crop, cotb200_aug_randaug)
@@ -15,7 +17,8 @@ DataLoader workers still decode (JPEG -> RGB uint8 HWC, the reference dataset's 
   With ``num_splits`` S >= 2 it is the reference's AugMixDataset over the separated transform (datasets/dataset.py:181-215,
   transforms_factory.py:44-129): a clean view (crop, flips) and S - 1 views that each add their own RandAugment or ColorJitter
   draw to the same crop, in fast_collate's split-major order, for the JSD loss (trainer.jsd_cross_entropy).
-* ``EvalTransform``: Resize(floor(size / crop_pct)) + CenterCrop(size) (:132-166) on the same resize kernel.
+* ``EvalTransform``: Resize(floor(size / crop_pct)) + CenterCrop(size) (:132-166) on the same resize kernel; with
+  crop_pct=1.0 also the train transform of augmentation.no_aug (transforms_noaug_train, :17-41).
 * ``RandomErasing``: the reference's random erasing of the normalised batch (datasets/random_erasing.py, applied by
   PrefetchLoader, datasets/loader.py:72-91), boxes drawn on the host in its order and erased by one kernel (cotb200_aug_erase).
 
@@ -67,12 +70,25 @@ assert JITTER_DTYPE.itemsize == 40 and ERASE_DTYPE.itemsize == 16 and ERASE_BOX_
 AugBatch = namedtuple("AugBatch", "data params labels jitter", defaults=(None,))
 
 
+#: rand_augment.py _RAND_CHOICE_WEIGHTS_0, in OPS order: the op-choice weights of the 'w0' section
+_CHOICE_WEIGHTS_0 = (0.025, .005, 0, 0.2, 0, .005, .005, .025, .005, .005, 0.025, 0.2, 0.2, 0.1, 0.1, 0.1)
+
+
+def choice_weights(weight_idx):
+    """_select_rand_weights(weight_idx) (rand_augment.py:312-318): the weights over OPS divided by their np.sum, float64, bit for
+    bit (numpy's choice compares their cumulative sum against its uniforms, so any other rounding can pick another op)."""
+    if weight_idx != 0:
+        raise ValueError("RandAugment weight index must be 0 (the reference's only weight set), got %d" % weight_idx)
+    probs = list(_CHOICE_WEIGHTS_0)
+    return np.asarray(probs, np.float64) / np.sum(probs)
+
+
 def _parse_rand(config_str):
-    """rand_augment_transform's config string -> (magnitude, num_layers, magnitude_std)."""
+    """rand_augment_transform's config string -> (magnitude, num_layers, magnitude_std, choice weights or None)."""
     parts = config_str.split("-")
     if parts[0] != "rand":
         raise ValueError("only RandAugment ('rand-...') is supported, got %r" % config_str)
-    mag, n, mstd = 10, 2, 0.
+    mag, n, mstd, weights = 10, 2, 0., None
     for c in parts[1:]:
         cs = re.split(r"(\d.*)", c)
         if len(cs) < 2:
@@ -84,13 +100,19 @@ def _parse_rand(config_str):
             mag = int(val)
         elif key == "n":
             n = int(val)
+        elif key == "w":
+            weights = choice_weights(int(val))
         elif key == "inc":
             pass
         else:
             raise ValueError("RandAugment section %r is not supported" % c)
-    if n > 2:
-        raise ValueError("at most 2 RandAugment layers are supported, got %d" % n)
-    return mag, n, mstd
+    if n < 0:
+        raise ValueError("RandAugment layer count must be >= 0, got %d" % n)
+    # without replacement, numpy's choice needs n ops of non-zero weight; the reference finds out on its first image
+    if weights is not None and n > np.count_nonzero(weights):
+        raise ValueError("RandAugment with weights picks %d distinct ops, but only %d have a non-zero weight"
+                         % (n, np.count_nonzero(weights)))
+    return mag, n, mstd, weights
 
 
 def _check_input(value, name, center=1., bound=(0., float("inf")), clip_first_on_zero=True):
@@ -180,7 +202,10 @@ class TrainAugment:
     def __init__(self, size=224, scale=(0.08, 1.0), ratio=(3. / 4., 4. / 3.), interpolation="bicubic", hflip=0.5,
                  auto_augment="rand-m15-mstd0.5-n2", translate_const=100, cutout_const=40, vflip=0., color_jitter=None,
                  num_splits=0):
-        """num_splits: augmentation.aug_splits of the reference (0 and 1: one view per image)."""
+        """num_splits: augmentation.aug_splits of the reference (0 and 1: one view per image).
+        auto_augment: a rand_augment_transform config string ('rand-m9-n3-mstd0.5', 'rand-mstd1-w0', ...) or None.  One
+        difference: 'w0' with n above the 14 ops of non-zero weight raises ValueError here, where the reference's numpy
+        choice raises on the first image."""
         if int(num_splits) != num_splits or num_splits < 0:
             raise ValueError("num_splits must be 0 or a positive integer, got %r" % (num_splits,))
         self.num_splits = int(num_splits) if num_splits >= 2 else 0
@@ -191,7 +216,8 @@ class TrainAugment:
         self.interpolation = interpolation
         self.hflip = hflip
         self.vflip = float(vflip)
-        self.magnitude, self.num_layers, self.mstd = _parse_rand(auto_augment) if auto_augment else (0, 0, 0.)
+        parsed = _parse_rand(auto_augment) if auto_augment else (0, 0, 0., None)
+        self.magnitude, self.num_layers, self.mstd, self.choice_weights = parsed
         self.translate_const, self.cutout_const = translate_const, cutout_const
         # ColorJitter is the reference's colour transform only when RandAugment is off (transforms_factory.py:79-109)
         self.jitter = None if auto_augment or color_jitter is None else jitter_ranges(color_jitter)
@@ -244,8 +270,9 @@ class TrainAugment:
     def _secondary(self, rnd, nrnd, tgen):
         """The colour part's draws: RandAugment's ops, or ColorJitter's."""
         p = dict(ops=[])
-        if self.num_layers:
-            for k in nrnd.choice(len(OPS), self.num_layers, replace=True):
+        if self.num_layers:                             # RandAugment.__call__: without replacement when weighted
+            w = self.choice_weights
+            for k in nrnd.choice(len(OPS), self.num_layers, replace=w is None, p=w):
                 p["ops"].append(self._op(int(k), rnd, nrnd))
         elif self.jitter is not None:                   # ColorJitter.get_params + forward (torchvision)
             perm = torch.randperm(4, generator=tgen).tolist()
@@ -272,10 +299,12 @@ class TrainAugment:
 
     def draw(self, sizes, py_random, np_random, torch_gen):
         """Per-sample parameters of images of `sizes` [(H, W), ...], drawn image by image in the reference's order:
-        crop, filter (interpolation 'random' only), flip, vertical flip (vflip > 0 only), the op choice, then per op apply /
-        magnitude / sign (/ filter) and Cutout's two positions; or, with ColorJitter, randperm(4) and one uniform per enabled
-        factor in brightness, contrast, saturation, hue order.  Returns the list of dicts; ``pack`` and ``pack_jitter`` turn it
-        into the device structs; ``pack_views`` the augmented views' ones when num_splits >= 2."""
+        crop, filter (interpolation 'random' only), flip, vertical flip (vflip > 0 only), the op choice (num_layers ops, with
+        replacement, or without it by the choice weights of a 'w0' config), then per op apply / magnitude / sign (/ filter) and
+        Cutout's two positions; or, with ColorJitter, randperm(4) and one uniform per enabled factor in brightness, contrast,
+        saturation, hue order.  Returns the list of dicts; ``pack`` and ``pack_jitter`` turn it into the device structs;
+        ``pack_views`` the augmented views' ones when num_splits >= 2, ``pack_pass`` those of ops 2k and 2k + 1 when
+        num_layers > 2."""
         return [self.draw_one(int(H), int(W), py_random, np_random, torch_gen) for H, W in sizes]
 
     def pack(self, sizes, draws):
@@ -299,11 +328,19 @@ class TrainAugment:
         """numpy SAMPLE_DTYPE [(S-1) * N] of the augmented views' RandAugment ops, split-major (view v of sample n at
         v * N + n); the other fields stay 0, as cotb200_aug_randaug reads only the ops."""
         views = [p["views"][v] for v in range(self.num_splits - 1) for p in draws]
-        rec = np.zeros(len(views), SAMPLE_DTYPE)
-        for r, p in zip(rec, views):
-            for s in range(2):
-                pack_op(r["ops"][s], p["ops"][s] if s < len(p["ops"]) else None)
-        return rec
+        return _pack_ops(views, 0)
+
+    @property
+    def passes(self):
+        """RandAugment launches per batch: ceil(num_layers / 2), as a launch applies COTB200_AUG_MAX_OPS = 2 ops per sample
+        (at least 1: pass 0 also carries the resize-crop structs)."""
+        return max(1, -(-self.num_layers // 2))
+
+    def pack_pass(self, draws, k):
+        """numpy SAMPLE_DTYPE of pass k >= 1: ops 2k and 2k + 1 of every row of pass 0 (the N samples, then with num_splits S
+        the (S-1) * N views split-major); only the ops are set, as cotb200_aug_randaug reads nothing else."""
+        rows = list(draws) + [p["views"][v] for v in range(self.num_splits - 1) for p in draws]
+        return _pack_ops(rows, k)
 
     @property
     def has_jitter_kernel(self):
@@ -344,13 +381,16 @@ class TrainAugment:
     def collate_draws(self, imgs, labels, draws):
         """AugBatch of HWC uint8 `imgs` with their labels and draws.  With num_splits S >= 2 each image is shipped once; the
         structs are the B clean samples then the (S-1) * B views (pack_views), the jitter structs and the labels cover all S * B
-        rows in fast_collate's order (labels repeated per split)."""
+        rows in fast_collate's order (labels repeated per split).  With more than two RandAugment layers the structs hold
+        `passes` such blocks, pass k carrying ops 2k and 2k + 1 (pack_pass)."""
         sizes = [a.shape[:2] for a in imgs]
         rec = self.pack(sizes, draws)
         jit = [draws]
         if self.num_splits:
             rec = np.concatenate([rec, self.pack_views(draws)])
             jit += [[p["views"][k] for p in draws] for k in range(self.num_splits - 1)]
+        if self.passes > 1:                             # pass-major: then the ops 2k, 2k + 1 of the same rows
+            rec = np.concatenate([rec] + [self.pack_pass(draws, k) for k in range(1, self.passes)])
         data = torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs]))
         jitter = None
         if self.has_jitter_kernel:
@@ -360,8 +400,18 @@ class TrainAugment:
 
     def __call__(self, batch, device=None):
         """AugBatch -> (uint8 [N, 3, S, S] on `device`, labels on `device`), on the current stream."""
-        out = run(batch, self.size, device, randaug=self.num_layers > 0, num_splits=self.num_splits)
+        out = run(batch, self.size, device, randaug=self.num_layers > 0, num_splits=self.num_splits, passes=self.passes)
         return out, batch.labels.to(out.device, non_blocking=True)
+
+
+def _pack_ops(rows, k):
+    """SAMPLE_DTYPE [len(rows)] with only the ops set: ops 2k and 2k + 1 of each row's draws (op -1 past its list)."""
+    rec = np.zeros(len(rows), SAMPLE_DTYPE)
+    for r, p in zip(rec, rows):
+        ops = p.get("ops", [])[2 * k:2 * k + 2]
+        for s in range(2):
+            pack_op(r["ops"][s], ops[s] if s < len(ops) else None)
+    return rec
 
 
 def pack_op(dst, op):
@@ -382,10 +432,13 @@ def pack_op(dst, op):
 
 
 class EvalTransform:
-    """transforms_imagenet_eval (use_prefetcher=True): Resize(floor(size / crop_pct), interpolation) + CenterCrop(size)."""
+    """transforms_imagenet_eval (use_prefetcher=True): Resize(floor(size / crop_pct), interpolation) + CenterCrop(size).
+    Interpolation 'random' is bilinear here, as the reference's _pil_interp makes it.  With crop_pct=1.0 this is also the
+    reference's train transform under augmentation.no_aug (transforms_noaug_train: Resize(size) + CenterCrop(size))."""
 
     def __init__(self, size=224, crop_pct=0.875, interpolation="bicubic"):
-        self.size, self.crop_pct, self.filter = int(size), crop_pct, _INTERP[interpolation]
+        self.size, self.crop_pct = int(size), crop_pct
+        self.filter = BILINEAR if interpolation == "random" else _INTERP[interpolation]
 
     def pack(self, sizes):
         S = self.size
@@ -419,18 +472,22 @@ def uses_cluster_kernels(S):
     return S > ONE_CTA_MAX_S
 
 
-def run(batch, S, device=None, randaug=True, num_splits=0, cluster=None):
+def run(batch, S, device=None, randaug=True, num_splits=0, cluster=None, passes=1):
     """The kernels on an AugBatch: H2D copies of the ragged buffer and the structs, resize-crop (+ flip), vertical flip and
     ColorJitter when the batch carries them, then RandAugment in place.  Returns uint8 [N, 3, S, S] on `device` (default: the
     current CUDA device).  With num_splits >= 2 (TrainAugment(num_splits=...)'s batch of B images) the clean views are
     resized, cropped and flipped into out[:B] and copied into each of the num_splits - 1 blocks after it, where the views'
     ColorJitter or RandAugment run in place: N = num_splits * B.
+    The structs are `passes` blocks of N (TrainAugment.passes, pass-major): pass 0 drives every kernel, and each pass k
+    launches RandAugment once more on the same rows, applying its ops after those of pass k - 1.
     ColorJitter and RandAugment run one CTA per image up to S = ONE_CTA_MAX_S and one thread-block cluster per image above
     it, up to CLUSTER_MAX_S, with the same bytes; `cluster` True / False forces one kind (None: by size)."""
     cluster = uses_cluster_kernels(S) if cluster is None else bool(cluster)
     device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     rec = batch.params.numpy().view(SAMPLE_DTYPE)
-    N = len(rec)
+    if int(passes) != passes or passes < 1 or len(rec) % passes:
+        raise ValueError("AugBatch: %d sample structs are not %r passes" % (len(rec), passes))
+    N = len(rec) // passes
     splits = num_splits if num_splits >= 2 else 1
     if N % splits:
         raise ValueError("AugBatch: %d sample structs are not %d splits" % (N, splits))
@@ -459,17 +516,18 @@ def run(batch, S, device=None, randaug=True, num_splits=0, cluster=None):
             _lib.check(fn(hi - lo, S, jrec[lo:].ctypes.data_as(ctypes.c_void_p), jdev.data_ptr() + lo * JITTER_DTYPE.itemsize,
                           out[lo].data_ptr(), st), "aug_color_jitter")
 
-    def randaug_(lo, hi):
-        if randaug and (rec["ops"]["op"][lo:hi] >= 0).any():
+    def randaug_(lo, hi, base):                     # rows lo..hi of out, their structs at base + lo
+        if randaug and (rec["ops"]["op"][base + lo:base + hi] >= 0).any():
             fn = lib.cotb200_aug_randaug_cluster if cluster else lib.cotb200_aug_randaug
-            _lib.check(fn(hi - lo, S, rec[lo:].ctypes.data_as(ctypes.c_void_p), params.data_ptr() + lo * SAMPLE_DTYPE.itemsize,
-                          out[lo].data_ptr(), st), "aug_randaug")
+            _lib.check(fn(hi - lo, S, rec[base + lo:].ctypes.data_as(ctypes.c_void_p),
+                          params.data_ptr() + (base + lo) * SAMPLE_DTYPE.itemsize, out[lo].data_ptr(), st), "aug_randaug")
     jitter(0, B)
     if splits > 1:                                  # the augmented views start from the clean view, vertical flip included
         for k in range(1, splits):
             out[k * B:(k + 1) * B].copy_(out[:B])
         jitter(B, N)
-    randaug_(B if splits > 1 else 0, N)
+    for k in range(passes):                         # in order on one stream: pass k works on pass k - 1's output
+        randaug_(B if splits > 1 else 0, N, k * N)
     return out
 
 
