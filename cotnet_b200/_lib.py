@@ -124,6 +124,7 @@ SYMBOLS = {
     "cotb200_se_eval": (ctypes.c_int, [ctypes.c_int] * 3 + [_VP, ctypes.c_float] + [_VP] * 9),
     "cotb200_gather_chunk": (ctypes.c_int, []),
     "cotb200_multi_gather": (ctypes.c_int, [_VP, _VP, ctypes.c_int, ctypes.c_int, _VP, ctypes.c_float, _VP]),
+    "cotb200_multi_gather_acc": (ctypes.c_int, [_VP, _VP, ctypes.c_int, _VP, ctypes.c_int, _VP, ctypes.c_float, _VP]),
     "cotb200_multi_lerp": (ctypes.c_int, [_VP, ctypes.c_int, _VP, _VP]),
     "cotb200_clip_seg_max": (ctypes.c_int, []),
     "cotb200_grad_norm": (ctypes.c_int, [ctypes.c_longlong, ctypes.c_int, _VP, _VP, ctypes.c_longlong, _VP, _VP, ctypes.c_float, _VP, _VP]),

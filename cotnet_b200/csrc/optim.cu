@@ -10,6 +10,8 @@
 // and the whole parameter update is ONE pass (cotb200_opt_step, opt.cu):  read G, P, M, E  ->  write P, M, E, Pb.
 //
 //   cotb200_multi_gather   gradients (any mix of fp32 / bf16 tensors) -> flat bucket (fp32 or bf16), optional scale
+//   cotb200_multi_gather_acc   the same added to an fp32 accumulator, optionally emitted into the bucket: the gradient sum over
+//                          the micro-batches of a step with virtual ranks
 //   cotb200_multi_lerp     EMA of the buffers (BatchNorm running statistics, integer counters) by pointer table
 //   cotb200_u8_to_nhwc     uint8 NCHW batch -> (x - mean)/std in bf16/fp16/fp32 channels_last
 //   cotb200_u8_mix_rows_to_nhwc   the same after Mixup / CutMix, one table row per output sample
@@ -24,39 +26,72 @@ namespace cotb200 {
 // second table built by the host (rows are cut into chunks of GATHER_CHUNK elements) so no thread searches.
 static constexpr int GATHER_CHUNK = 8192;       // elements per block: 32 KB of fp32
 
-template <typename TS, typename TD>
-__device__ __forceinline__ void gather_chunk(const TS* __restrict__ src, TD* __restrict__ dst, long long n, float scale) {
-  // n <= GATHER_CHUNK elements; src/dst each aligned to at least their element size.  Vector path when both are 16-byte aligned.
-  constexpr int VS = 16 / (int)sizeof(TS), VD = 16 / (int)sizeof(TD);
-  constexpr int V = VS < VD ? VS : VD;           // elements per thread step (4 for any fp32 side, 8 for bf16 -> bf16)
-  const bool vec = ((reinterpret_cast<uintptr_t>(src) % (V * sizeof(TS))) == 0) && ((reinterpret_cast<uintptr_t>(dst) % (V * sizeof(TD))) == 0);
+// Modes of the gather (cotb200_multi_gather / cotb200_multi_gather_acc).  The two accumulating modes add in fp32 with
+// __fmul_rn / __fadd_rn (no FMA contraction), so a sum over micro-batches is bit-exact against torch fp32 adds in the same order.
+enum GatherMode {
+  GATHER_STORE = 0,   // dst[i] = TD(g * scale)
+  GATHER_ACC = 1,     // acc[i] = acc[i] + g * scale          (dst is acc, TD = float)
+  GATHER_EMIT = 2,    // dst[i] = TD(acc[i] + g * scale)      (dst may be acc itself when TD = float)
+};
+
+template <int MODE, typename TD>
+__device__ __forceinline__ TD gather_elem(float g, float a, float scale) {
+  if constexpr (MODE == GATHER_STORE) return Elem<TD>::from(g * scale);
+  else return Elem<TD>::from(__fadd_rn(a, __fmul_rn(g, scale)));
+}
+
+template <int MODE, typename TS, typename TD>
+__device__ __forceinline__ void gather_chunk(const TS* __restrict__ src, const float* acc, TD* dst, long long n, float scale) {
+  // n <= GATHER_CHUNK elements; src/dst/acc each aligned to at least their element size.  Vector path when all are aligned to
+  // the packet.  acc and dst may alias (GATHER_ACC, and GATHER_EMIT into an fp32 bucket): each element is read and then written
+  // by the same thread, so they carry no __restrict__.
+  constexpr int VS = 16 / (int)sizeof(TS), VD = 16 / (int)sizeof(TD), VA = MODE == GATHER_STORE ? 16 : 4;
+  constexpr int V0 = VS < VD ? VS : VD;
+  constexpr int V = V0 < VA ? V0 : VA;           // elements per thread step (4 for any fp32 side, 8 for a bf16 -> bf16 store)
+  const bool vec = ((reinterpret_cast<uintptr_t>(src) % (V * sizeof(TS))) == 0) && ((reinterpret_cast<uintptr_t>(dst) % (V * sizeof(TD))) == 0) &&
+                   (MODE == GATHER_STORE || (reinterpret_cast<uintptr_t>(acc) % (V * sizeof(float))) == 0);
+  long long i0 = 0;
   if (vec) {
     const long long nv = n / V;
     for (long long i = threadIdx.x; i < nv; i += blockDim.x) {
       const Pack<TS, V> s = ld_pack<TS, V>(src + i * V);
+      Pack<float, V> a;
+      if constexpr (MODE != GATHER_STORE) a = *reinterpret_cast<const Pack<float, V>*>(acc + i * V);
       Pack<TD, V> d;
 #pragma unroll
-      for (int k = 0; k < V; ++k) d.v[k] = Elem<TD>::from((float)to_acc(s.v[k]) * scale);
+      for (int k = 0; k < V; ++k) d.v[k] = gather_elem<MODE, TD>((float)to_acc(s.v[k]), MODE == GATHER_STORE ? 0.f : a.v[k], scale);
       st_pack<TD, V>(dst + i * V, d);
     }
-    for (long long i = nv * V + threadIdx.x; i < n; i += blockDim.x) dst[i] = Elem<TD>::from((float)to_acc(src[i]) * scale);
-  } else {
-    for (long long i = threadIdx.x; i < n; i += blockDim.x) dst[i] = Elem<TD>::from((float)to_acc(src[i]) * scale);
+    i0 = nv * V;
   }
+  for (long long i = i0 + threadIdx.x; i < n; i += blockDim.x)
+    dst[i] = gather_elem<MODE, TD>((float)to_acc(src[i]), MODE == GATHER_STORE ? 0.f : acc[i], scale);
 }
 
+// A segment without a source (a parameter that got no gradient in this micro-batch) contributes zero: nothing to add, and the
+// emit pass converts the accumulator alone.
 template <typename TD>
+__device__ __forceinline__ void emit_only(const float* acc, TD* dst, long long n) {
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) dst[i] = Elem<TD>::from(acc[i]);
+}
+
+template <int MODE, typename TD>
 __global__ void __launch_bounds__(256)
-multi_gather_kernel(const cotb200_seg* __restrict__ segs, const int2* __restrict__ blocks, TD* __restrict__ dst, float scale) {
+multi_gather_kernel(const cotb200_seg* __restrict__ segs, const int2* __restrict__ blocks, const float* acc, TD* dst, float scale) {
   const int2 b = blocks[blockIdx.x];              // (row, chunk index inside the row)
   const cotb200_seg s = segs[b.x];
   const long long off = (long long)b.y * GATHER_CHUNK;
   long long n = s.numel - off;
   if (n > GATHER_CHUNK) n = GATHER_CHUNK;
   TD* d = dst + s.offset + off;
-  if (s.dtype == COTB200_F32) gather_chunk<float, TD>((const float*)s.ptr + off, d, n, scale);
-  else if (s.dtype == COTB200_BF16) gather_chunk<__nv_bfloat16, TD>((const __nv_bfloat16*)s.ptr + off, d, n, scale);
-  else gather_chunk<__half, TD>((const __half*)s.ptr + off, d, n, scale);
+  const float* a = MODE == GATHER_STORE ? nullptr : acc + s.offset + off;
+  if (MODE != GATHER_STORE && s.ptr == nullptr) {
+    if (MODE == GATHER_EMIT) emit_only<TD>(a, d, n);
+    return;
+  }
+  if (s.dtype == COTB200_F32) gather_chunk<MODE, float, TD>((const float*)s.ptr + off, a, d, n, scale);
+  else if (s.dtype == COTB200_BF16) gather_chunk<MODE, __nv_bfloat16, TD>((const __nv_bfloat16*)s.ptr + off, a, d, n, scale);
+  else gather_chunk<MODE, __half, TD>((const __half*)s.ptr + off, a, d, n, scale);
 }
 
 // ------------------------------------------------------------------------------------------------ multi_lerp
@@ -216,12 +251,37 @@ extern "C" int cotb200_multi_gather(const cotb200_seg* segs_dev, const int* bloc
   if (dst_dtype != COTB200_F32 && dst_dtype != COTB200_BF16) { set_error("multi_gather: bucket dtype must be fp32 or bf16"); return COTB200_EDTYPE; }
   cudaStream_t st = (cudaStream_t)stream;
   COTB200_PROF("multi_gather");
-  if (dst_dtype == COTB200_F32) multi_gather_kernel<float><<<n_blocks, 256, 0, st>>>(segs_dev, (const int2*)blocks_dev, (float*)dst, scale);
-  else multi_gather_kernel<__nv_bfloat16><<<n_blocks, 256, 0, st>>>(segs_dev, (const int2*)blocks_dev, (__nv_bfloat16*)dst, scale);
+  if (dst_dtype == COTB200_F32)
+    multi_gather_kernel<GATHER_STORE, float><<<n_blocks, 256, 0, st>>>(segs_dev, (const int2*)blocks_dev, nullptr, (float*)dst, scale);
+  else
+    multi_gather_kernel<GATHER_STORE, __nv_bfloat16><<<n_blocks, 256, 0, st>>>(segs_dev, (const int2*)blocks_dev, nullptr,
+                                                                               (__nv_bfloat16*)dst, scale);
   return check_launch("multi_gather");
 }
 
 extern "C" int cotb200_gather_chunk(void) { return GATHER_CHUNK; }
+
+extern "C" int cotb200_multi_gather_acc(const cotb200_seg* segs_dev, const int* blocks_dev, int n_blocks, float* acc, int dst_dtype,
+                                        void* dst, float scale, void* stream) {
+  if (!segs_dev || !blocks_dev || !acc) { set_error("multi_gather_acc: NULL pointer"); return COTB200_ENULL; }
+  if (n_blocks <= 0) { set_error("multi_gather_acc: no blocks"); return COTB200_EINVAL; }
+  if (!aligned16(acc)) { set_error("multi_gather_acc: accumulator not 16-byte aligned"); return COTB200_EALIGN; }
+  if (dst && dst_dtype != COTB200_F32 && dst_dtype != COTB200_BF16) {
+    set_error("multi_gather_acc: bucket dtype must be fp32 or bf16"); return COTB200_EDTYPE;
+  }
+  if (dst == (void*)acc && dst_dtype != COTB200_F32) { set_error("multi_gather_acc: only an fp32 bucket can be its own accumulator"); return COTB200_EINVAL; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int2* blocks = (const int2*)blocks_dev;
+  if (!dst) {
+    COTB200_PROF("multi_gather_acc");
+    multi_gather_kernel<GATHER_ACC, float><<<n_blocks, 256, 0, st>>>(segs_dev, blocks, acc, acc, scale);
+    return check_launch("multi_gather_acc");
+  }
+  COTB200_PROF("multi_gather_emit");
+  if (dst_dtype == COTB200_F32) multi_gather_kernel<GATHER_EMIT, float><<<n_blocks, 256, 0, st>>>(segs_dev, blocks, acc, (float*)dst, scale);
+  else multi_gather_kernel<GATHER_EMIT, __nv_bfloat16><<<n_blocks, 256, 0, st>>>(segs_dev, blocks, acc, (__nv_bfloat16*)dst, scale);
+  return check_launch("multi_gather_emit");
+}
 
 extern "C" int cotb200_multi_lerp(const cotb200_seg2* segs_dev, int n_segs, const float* hyper_dev, void* stream) {
   if (!segs_dev || !hyper_dev) { set_error("multi_lerp: NULL pointer"); return COTB200_ENULL; }

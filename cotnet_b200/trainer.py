@@ -15,6 +15,10 @@ Mirrors the body of the reference's training loop -- forward under autocast, los
   backward of the earlier layers is still running.  Everything -- forward, backward, gathers, NCCL, optimizer -- is
   captured in ONE CUDA graph (fork/join through events); if NCCL cannot be captured the collectives run eagerly between
   a fwd+bwd graph and an optimizer graph.
+* **Virtual ranks.**  ``virtual_ranks=K`` makes one process K of the reference's ranks: the step takes the K ranks' batches
+  concatenated and runs one forward and backward per rank inside the same graph; ``cotb200_multi_gather_acc`` sums their
+  gradients in fp32 (the last micro-batch emits the sum into the bucket), and every BatchNorm buffer (and its EMA copy) is kept
+  per rank.  Clipping, the update and the EMA run once per step on the gradient averaged over K x world ranks.
 * **One optimizer pass.**  ``cotb200_opt_step`` per bucket: the update rule of the reference's create_optimizer (``opt=``,
   SGD-nesterov by default) + weight decay + EMA + bf16 copy, hyper-parameters read from device memory (LR schedules work
   under graph replay); before it ``cotb200_opt_prepare`` (the per-step scalars, on the device) for the rules that have any and
@@ -217,7 +221,8 @@ class TrainStep:
 
     def __init__(self, model, lr=0.05, momentum=0.9, weight_decay=1e-4, nesterov=True, ema_decay=None,
                  loss_fn=None, amp_dtype=torch.bfloat16, weights="bf16", bucket_dtype=None, comm_chunks=3, overlap=True,
-                 process_group=None, label_smoothing=0., clip_grad=None, clip_mode="norm", opt="sgd", opt_eps=1e-8, jsd_splits=0):
+                 process_group=None, label_smoothing=0., clip_grad=None, clip_mode="norm", opt="sgd", opt_eps=1e-8, jsd_splits=0,
+                 virtual_ranks=1):
         """label_smoothing > 0, or a `mix` given to the step, selects the soft-target loss (soft_target_cross_entropy) that the
         reference recipe trains with (train.py:198-209); otherwise the loss is `loss_fn` (default F.cross_entropy).
         jsd_splits = S >= 2 selects JsdCrossEntropy(num_splits=S, alpha=12, smoothing=label_smoothing) (jsd_cross_entropy), the
@@ -228,7 +233,17 @@ class TrainStep:
         (clip_grad_value_) or 'agc' (adaptive_clip_grad without the classifier head).  None or <= 0: no clipping.
         opt / opt_eps are solver.opt / solver.opt_eps of create_optimizer (parse_opt): sgd (nesterov per `nesterov`), nesterov,
         momentum, adam, adamw, nadam, radam, adadelta, rmsprop, rmsproptf, each optionally as lookahead_<name>; lr, momentum and
-        weight_decay are the factory's, everything else its defaults."""
+        weight_decay are the factory's, everything else its defaults.
+        virtual_ranks = K >= 1: this process acts as K ranks of the reference's DistributedDataParallel run, so a step is its step
+        at K x world ranks.  The step takes the K ranks' batches concatenated (rows [k B, (k+1) B) are rank k's; with a 'half'
+        MixRows x holds K B/2 rows and lab K B), and `mix` is None or a list of K MixRows, one MixupCutmix.draw(B, H, W) per rank.
+        Each rank's batch runs its own forward and backward, in rank order, with its own BatchNorm buffers (rank_buffers); their
+        gradients are summed in fp32 and the update reads the sum / (K x world).  The returned loss is the mean of the K losses.
+        Outside a step the model's buffers hold rank 0's values; distribute_bn averages over all K x world ranks."""
+        if isinstance(virtual_ranks, bool) or int(virtual_ranks) != virtual_ranks or virtual_ranks < 1:
+            raise ValueError("TrainStep: virtual_ranks must be an integer >= 1, got %r" % (virtual_ranks,))
+        self.virtual_ranks = K = int(virtual_ranks)
+        self._micro = 0                                             # the micro-batch (virtual rank) being run
         if clip_mode not in CLIP_MODES:
             raise ValueError("TrainStep: unknown clip_mode %r (one of %s)" % (clip_mode, ", ".join(CLIP_MODES)))
         self.opt_name, self.rule, self.lookahead = parse_opt(opt, nesterov)
@@ -267,6 +282,9 @@ class TrainStep:
             self.Pb = torch.zeros(nb, dtype=torch.bfloat16, device=dev) if self.weights_bf16 else None
             self.G_big = torch.zeros(nb, dtype=bucket_dtype, device=dev)
             self.G_small = torch.zeros(ns, **f32)
+            # micro-batch 0 of a step stores its gradients here, later ones add to it (fp32) and the last emits the sum into G_big:
+            # an fp32 bucket is its own accumulator; with one virtual rank this is the bucket, and the gather its only pass
+            self.G_acc = torch.zeros(nb, **f32) if (K > 1 and bucket_dtype != torch.float32) else self.G_big
             for _, p, off in plan["big"]:
                 _strided_view(self.P_big, p, off).copy_(p.detach())
                 if self.weights_bf16:
@@ -282,21 +300,27 @@ class TrainStep:
             self.ema = ema_decay is not None
             self.E_big = self.P_big.clone() if self.ema else None
             self.E_small = self.P_small.clone() if self.ema else None
+            # per-rank buffers: set 0 is the model's own storage (it never moves), sets 1..K-1 are copies; during micro-batch k each
+            # buffer's .data is set k's tensor
+            self._bufs = [b for _, b in model.named_buffers()]
+            self._buf_sets = [[b.detach() for b in self._bufs]] + [[b.detach().clone() for b in self._bufs] for _ in range(K - 1)]
             self.ema_buffers = None
+            self._ema_sets = None
             if self.ema:
-                bufs = [b for _, b in model.named_buffers()]
-                self.ema_buffers = [b.detach().clone() for b in bufs]
-                segs = (_Seg2 * max(1, len(bufs)))()
+                self.ema_buffers = [b.detach().clone() for b in self._bufs]
+                self._ema_sets = [self.ema_buffers] + [[e.clone() for e in self.ema_buffers] for _ in range(K - 1)]
+                segs = (_Seg2 * max(1, K * len(self._bufs)))()
                 keep = 0
-                for b, e in zip(bufs, self.ema_buffers):
-                    if b.dtype == torch.float32:
-                        code = _lib.F32
-                    elif b.dtype == torch.int64:
-                        code = 100
-                    else:
-                        continue
-                    segs[keep].dst, segs[keep].src, segs[keep].numel, segs[keep].dtype = e.data_ptr(), b.data_ptr(), b.numel(), code
-                    keep += 1
+                for bset, eset in zip(self._buf_sets, self._ema_sets):      # rank k's EMA buffers follow rank k's buffers
+                    for b, e in zip(bset, eset):
+                        if b.dtype == torch.float32:
+                            code = _lib.F32
+                        elif b.dtype == torch.int64:
+                            code = 100
+                        else:
+                            continue
+                        segs[keep].dst, segs[keep].src, segs[keep].numel, segs[keep].dtype = e.data_ptr(), b.data_ptr(), b.numel(), code
+                        keep += 1
                 self._lerp_tab = None
                 if keep:
                     raw = torch.frombuffer(bytearray(bytes(segs)), dtype=torch.uint8)[:keep * ctypes.sizeof(_Seg2)]
@@ -305,16 +329,21 @@ class TrainStep:
         self.hyper = torch.tensor([lr, momentum, weight_decay, ema_decay if self.ema else 0.0, 1.0], **f32)
         self.hyper_small = self.hyper.clone()
         self.hyper_small[2] = 0.0                                   # no weight decay on 1-D parameters / biases
-        if self.world > 1 and dist.get_backend(process_group) != "nccl":
-            self.hyper[4] = self.hyper_small[4] = 1.0 / self.world  # SUM all-reduce: the optimizer kernel applies 1/world
-        # gather tables: one per comm chunk of the big bucket + one for the small bucket
+        # the optimizer kernel applies 1/K to the gradient sum over the virtual ranks, and 1/world after a SUM all-reduce
+        denom = K * (self.world if (self.world > 1 and dist.get_backend(process_group) != "nccl") else 1)
+        if denom > 1:
+            self.hyper[4] = self.hyper_small[4] = 1.0 / denom
+        # gather tables: one per comm chunk of the big bucket + one for the small bucket, per micro-batch (a captured graph
+        # re-reads each pinned table at every replay, so the micro-batches cannot share one)
         def blocks_of(items):
             return sum((p.numel() + self.chunk_elems - 1) // self.chunk_elems for _, p, _ in items)
-        if self._cuda:
-            self._tabs = [_GatherTable(len(idx), blocks_of([plan["big"][i] for i in idx]), dev) for _, _, idx in plan["chunks"]]
-            self._tab_small = _GatherTable(max(1, len(plan["small"])), max(1, blocks_of(plan["small"])), dev)
-        else:
-            self._tabs, self._tab_small = [None] * len(plan["chunks"]), None
+        self._tab_sets = []
+        for _ in range(K):
+            if self._cuda:
+                self._tab_sets.append(([_GatherTable(len(idx), blocks_of([plan["big"][i] for i in idx]), dev) for _, _, idx in plan["chunks"]],
+                                       _GatherTable(max(1, len(plan["small"])), max(1, blocks_of(plan["small"])), dev)))
+            else:
+                self._tab_sets.append(([None] * len(plan["chunks"]), None))
         self._chunk_of = {}
         for c, (_, _, idx) in enumerate(plan["chunks"]):
             for i in idx:
@@ -410,12 +439,16 @@ class TrainStep:
         if self._pending[c] == 0:
             self._flush_chunk(c)
 
-    def _entries(self, items):
+    def _entries(self, items, null_missing=False):
+        """Gather table rows of the parameters in `items` that have a gradient; with `null_missing` the others get a row without a
+        source (they contribute zero to cotb200_multi_gather_acc)."""
         ent, missing = [], False
         for _, p, off in items:
             g = p.grad
             if g is None:
                 missing = True
+                if null_missing:
+                    ent.append((0, off, p.numel(), _lib.F32))
                 continue
             if any(a_ != b_ for a_, b_, n_ in zip(g.stride(), p.stride(), p.shape) if n_ != 1):   # same memory order? (size-1 dims are free)
                 t = torch.empty_strided(p.size(), p.stride(), dtype=g.dtype, device=g.device)
@@ -424,13 +457,20 @@ class TrainStep:
             ent.append((g.data_ptr(), off, g.numel(), _lib.dtype_code(g)))
         return ent, missing
 
-    def _gather(self, tab, items, bucket, lo, hi):
-        ent, missing = self._entries(items)
-        if missing:
-            bucket[lo:hi].zero_()
-        if not ent:
-            return
-        self._launch_gather(tab, ent, bucket, [p.grad for _, p, _ in items if p.grad is not None])
+    def _gather(self, tab, items, bucket, acc, lo, hi):
+        """The gradients of `items` (bucket range [lo, hi)) for the current micro-batch: micro-batch 0 stores them into `acc` (the
+        bucket itself with one virtual rank), later ones add them to it, the last one emits acc + its gradients into the bucket."""
+        K, k = self.virtual_ranks, self._micro
+        emit = K > 1 and k == K - 1
+        ent, missing = self._entries(items, null_missing=emit)
+        grads = [p.grad for _, p, _ in items if p.grad is not None]
+        if k == 0:
+            if missing:
+                acc[lo:hi].zero_()
+            if ent:
+                self._launch_gather(tab, ent, acc, grads)
+        elif ent:
+            self._launch_gather_acc(tab, ent, acc, bucket if emit else None, grads)
 
     def _launch_gather(self, tab, ent, bucket, grads):
         nb = tab.fill(ent, self.chunk_elems)
@@ -438,6 +478,14 @@ class TrainStep:
         st = torch.cuda.current_stream(self.dev).cuda_stream
         _lib.check(self.lib.cotb200_multi_gather(tab.seg_d.data_ptr(), tab.blk_d.data_ptr(), nb, _lib.dtype_code(bucket),
                                                  bucket.data_ptr(), 1.0, st), "multi_gather")
+
+    def _launch_gather_acc(self, tab, ent, acc, dst, grads):
+        nb = tab.fill(ent, self.chunk_elems)
+        tab.upload(self._capturing)
+        st = torch.cuda.current_stream(self.dev).cuda_stream
+        _lib.check(self.lib.cotb200_multi_gather_acc(tab.seg_d.data_ptr(), tab.blk_d.data_ptr(), nb, acc.data_ptr(),
+                                                     _lib.F32 if dst is None else _lib.dtype_code(dst), _lib.ptr(dst), 1.0, st),
+                   "multi_gather_acc")
 
     def _all_reduce(self, t):
         if dist.get_backend(self.pg) == "nccl":
@@ -458,19 +506,20 @@ class TrainStep:
         """Gather chunk c of the big bucket on the current (backward) stream and all-reduce it on the side stream."""
         lo, hi, idx = self.plan["chunks"][c]
         self._flushed[c] = True
-        self._gather(self._tabs[c], [self.plan["big"][i] for i in idx], self.G_big, lo, hi)
-        if self.world > 1:
+        self._gather(self._tab_sets[self._micro][0][c], [self.plan["big"][i] for i in idx], self.G_big, self.G_acc, lo, hi)
+        if self.world > 1 and self._micro == self.virtual_ranks - 1:       # collectives once per step, on the last micro-batch
             self._all_reduce_side(self.G_big[lo:hi])
 
     def _finish_grads(self):
+        last = self._micro == self.virtual_ranks - 1
         for c in range(len(self.plan["chunks"])):
             if not self._flushed[c]:
                 self._flush_chunk(c)
         if self.plan["small"]:
-            self._gather(self._tab_small, self.plan["small"], self.G_small, 0, self.plan["n_small"])
-            if self.world > 1:
+            self._gather(self._tab_sets[self._micro][1], self.plan["small"], self.G_small, self.G_small, 0, self.plan["n_small"])
+            if self.world > 1 and last:
                 self._all_reduce_side(self.G_small)
-        if self.world > 1 and self.comm_stream is not None:
+        if self.world > 1 and self.comm_stream is not None and last:
             torch.cuda.current_stream(self.dev).wait_stream(self.comm_stream)
 
     # ------------------------------------------------------------------ the step
@@ -481,15 +530,79 @@ class TrainStep:
             return self.loss_fn(out, lab)
         return SoftTargetCrossEntropyFn.apply(out, lab, mix_dev, self.label_smoothing)
 
+    def _mix_list(self, mix):
+        """mix as one entry per virtual rank: None, or a list of K (a single MixRows / row table is rank 0's at K = 1)."""
+        K = self.virtual_ranks
+        if mix is None:
+            return None
+        if not isinstance(mix, (list, tuple)):
+            if K == 1:
+                return [mix]
+            raise ValueError("TrainStep: virtual_ranks=%d takes mix=None or a list of %d MixRows (one MixupCutmix.draw per rank), "
+                             "not a %s" % (K, K, type(mix).__name__))
+        if len(mix) != K or any(m is None for m in mix):
+            raise ValueError("TrainStep: virtual_ranks=%d takes a list of %d MixRows (one MixupCutmix.draw per rank), got %d entries%s"
+                             % (K, K, len(mix), " with a None" if any(m is None for m in mix) else ""))
+        return list(mix)
+
+    def _split(self, x, lab, mix):
+        """(x, lab, mix) of a step -> one (x, lab, mix) per virtual rank, validated."""
+        K = self.virtual_ranks
+        mixes = self._mix_list(mix)
+        if x.shape[0] % K or lab.shape[0] % K:
+            raise ValueError("TrainStep: %d images / %d labels do not split into %d virtual ranks" % (x.shape[0], lab.shape[0], K))
+        bx, bl = x.shape[0] // K, lab.shape[0] // K
+        if self.jsd_splits:
+            if mixes is not None:
+                raise ValueError("TrainStep: the JSD loss takes augmentation splits, which the reference does not mix (train.py:157)")
+            if bx % self.jsd_splits:
+                raise ValueError("TrainStep: batch of %d is not %d augmentation splits" % (bx, self.jsd_splits))
+        if mixes is None:
+            mixes = [None] * K
+        if K == 1:
+            return [(x, lab, mixes[0])]
+        return [(x[k * bx:(k + 1) * bx], lab[k * bl:(k + 1) * bl], mixes[k]) for k in range(K)]
+
+    def _bind_rank(self, k):
+        """Point every buffer of the model at virtual rank k's set."""
+        for b, t in zip(self._bufs, self._buf_sets[k]):
+            b.data = t
+
+    def rank_buffers(self, k, ema=False):
+        """name -> virtual rank k's buffer (with `ema`, its EMA copy).  Rank 0's are the model's own buffers (ema_buffers)."""
+        if not 0 <= k < self.virtual_ranks:
+            raise ValueError("TrainStep.rank_buffers: rank %r outside [0, %d)" % (k, self.virtual_ranks))
+        if ema and not self.ema:
+            raise ValueError("TrainStep.rank_buffers: no EMA (ema_decay=None)")
+        sets = self._ema_sets if ema else self._buf_sets
+        return {n: t for (n, _), t in zip(self.model.named_buffers(), sets[k])}
+
     def forward_backward(self, x, lab, mix=None):
         """mix: None, a MixRows (MixupCutmix.draw), or its device copy (the row table, 36 bytes per row) -- the loss reads the
         mixed targets' lam and partners from it.  With a 'half' MixRows, x holds the B/2 mixed images and lab the B labels of
-        the input batch."""
-        if self.jsd_splits:
-            if mix is not None:
-                raise ValueError("TrainStep: the JSD loss takes augmentation splits, which the reference does not mix (train.py:157)")
-            if x.shape[0] % self.jsd_splits:
-                raise ValueError("TrainStep: batch of %d is not %d augmentation splits" % (x.shape[0], self.jsd_splits))
+        the input batch.  With virtual ranks, x / lab are the K ranks' batches concatenated and mix a list of K (see __init__);
+        the micro-batches run in rank order and the loss returned is the mean of their losses."""
+        parts = self._split(x, lab, mix)
+        K = self.virtual_ranks
+        if K == 1:
+            self._micro = 0
+            return self._micro_batch(*parts[0])
+        losses = []
+        try:
+            for k, (xk, lk, mk) in enumerate(parts):
+                self._micro = k
+                self._bind_rank(k)
+                losses.append(self._micro_batch(xk, lk, mk).detach())
+        finally:
+            self._bind_rank(0)
+            self._micro = 0
+        loss = losses[0]
+        for lk in losses[1:]:
+            loss = loss + lk
+        return loss / K
+
+    def _micro_batch(self, x, lab, mix):
+        """Forward, backward and gather of one rank's batch."""
         mix_dev = mix if mix is None or torch.is_tensor(mix) else mix.on_stream(self.dev)
         if self._cuda:
             fused.step_begin(self.dev)
@@ -563,11 +676,15 @@ class TrainStep:
                 self.step_eager(x, lab, mix)
         torch.cuda.current_stream(self.dev).wait_stream(side)
         torch.cuda.synchronize(self.dev)
-        for t in self._tabs + [self._tab_small]:
-            t.done = None
+        for tabs, tab_small in self._tab_sets:
+            for t in tabs + [tab_small]:
+                t.done = None
+        mixes = self._mix_list(mix)
+        if mixes is not None and len({(m.n_out, m.n_in) for m in mixes}) > 1:
+            raise ValueError("TrainStep.capture: the ranks' mix tables differ in size")
         self._gx, self._glab = x.clone(), lab.clone()
-        self._gmix = None if mix is None else mix.dev.clone()
-        self._gmix_shape = None if mix is None else (mix.n_out, mix.n_in)
+        self._gmix = None if mixes is None else [m.dev.clone() for m in mixes]           # one static table per virtual rank
+        self._gmix_shape = None if mixes is None else (mixes[0].n_out, mixes[0].n_in)
         info = {"cuda_graph": True}
         lc0 = _lib.launch_count()
         try:
@@ -611,14 +728,16 @@ class TrainStep:
         if x is not None and x is not self._gx:
             self._gx.copy_(x, non_blocking=True)
             self._glab.copy_(lab, non_blocking=True)
-        if (mix is None) != (self._gmix is None):
+        mixes = self._mix_list(mix)
+        if (mixes is None) != (self._gmix is None):
             raise ValueError("TrainStep.step: this graph was captured %s mixing parameters; pass mix= %s"
                              % (("without", "to capture() first") if mix is not None else ("with", "(MixupCutmix.draw) at every step")))
-        if mix is not None and (mix.n_out, mix.n_in) != self._gmix_shape:
-            raise ValueError("TrainStep.step: this graph was captured with a table of %d rows from %d images, not %d from %d; "
-                             "capture() again for another mode or batch size" % (self._gmix_shape + (mix.n_out, mix.n_in)))
-        if mix is not None:
-            self._gmix.copy_(mix.on_stream(self.dev), non_blocking=True)
+        for m in mixes or ():
+            if (m.n_out, m.n_in) != self._gmix_shape:
+                raise ValueError("TrainStep.step: this graph was captured with a table of %d rows from %d images, not %d from %d; "
+                                 "capture() again for another mode or batch size" % (self._gmix_shape + (m.n_out, m.n_in)))
+        for g, m in zip(self._gmix or (), mixes or ()):
+            g.copy_(m.on_stream(self.dev), non_blocking=True)
         if self._graph[0] == "one":
             self._graph[1].replay()
         else:
@@ -712,34 +831,39 @@ class TrainStep:
     def distribute_bn(self, reduce=True, ema=True):
         """The reference's end-of-epoch distribute_bn (utils/distributed.py:57-67; train.py:346-352), for the model and, with
         `ema`, again for the EMA copies of its buffers: every buffer whose name contains running_mean / running_var is averaged
-        over the ranks (`reduce`: SUM, then / float(world), the reference's arithmetic) or broadcast from rank 0.  All of them
-        travel in ONE flat fp32 collective and are copied back into the original tensors, whose storage does not move (the EMA
-        lerp table and captured graphs hold their pointers).  num_batches_tracked is untouched.  Nothing happens at world 1."""
-        if self.world <= 1:
+        over the K x world ranks (`reduce`: the K virtual ranks' sets added in rank order, SUM over the processes, then
+        / float(K x world), the reference's arithmetic with the local sum first) or copied from global rank 0's set 0.  All of
+        them travel in ONE flat fp32 collective and are copied back into every set, whose storage does not move (the EMA lerp
+        table and captured graphs hold their pointers).  num_batches_tracked is untouched.  Nothing happens at one rank."""
+        K = self.virtual_ranks
+        if self.world <= 1 and K == 1:
             return
         names = [n for n, _ in self.model.named_buffers()]
         pick = [i for i, n in enumerate(names) if "running_mean" in n or "running_var" in n]
-        bufs = list(self.model.buffers())
-        sel = [bufs[i] for i in pick]
+        sets = [[bs[i] for i in pick] for bs in self._buf_sets]
         if ema and self.ema:
-            sel += [self.ema_buffers[i] for i in pick]
-        if not sel:
+            sets = [s + [es[i] for i in pick] for s, es in zip(sets, self._ema_sets)]
+        if not sets[0]:
             return
-        bad = [names[i] for i in pick if bufs[i].dtype != torch.float32]
+        bad = [names[i] for i in pick if self._buf_sets[0][i].dtype != torch.float32]
         if bad:
             raise TypeError("distribute_bn: running statistics must be fp32 (%s)" % ", ".join(bad[:3]))
         with torch.no_grad():
-            flat = torch.cat([b.reshape(-1) for b in sel])
+            flat = torch.cat([b.reshape(-1) for b in sets[0]])
             if reduce:
-                dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=self.pg)
-                flat /= float(self.world)
-            else:
+                for s in sets[1:]:
+                    flat += torch.cat([b.reshape(-1) for b in s])
+                if self.world > 1:
+                    dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=self.pg)
+                flat /= float(K * self.world)
+            elif self.world > 1:
                 dist.broadcast(flat, src=0 if self.pg is None else dist.get_global_rank(self.pg, 0), group=self.pg)
-            off = 0
-            for b in sel:
-                n = b.numel()
-                b.copy_(flat[off:off + n].view_as(b))
-                off += n
+            for s in sets:
+                off = 0
+                for b in s:
+                    n = b.numel()
+                    b.copy_(flat[off:off + n].view_as(b))
+                    off += n
 
     def grads(self):
         """name -> gradient view into the flat buckets (after forward_backward / a step)."""

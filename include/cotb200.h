@@ -328,6 +328,15 @@ int cotb200_gather_chunk(void);
  * tensors) into ONE flat fp32 or bf16 bucket = the unit of the NCCL all-reduce (replaces DDP's bucket copies, train.py:113-115). */
 int cotb200_multi_gather(const cotb200_seg* segs_dev, const int* blocks_dev, int n_blocks, int dst_dtype, void* dst,
                          float scale, void* stream);
+/* The gradient sum over the micro-batches of one step (TrainStep(virtual_ranks=K)), on the segment / block tables of
+ * cotb200_multi_gather.  acc is an fp32 array laid out like the bucket (16-byte aligned); g = src_seg[i], added in fp32 with no
+ * FMA contraction (bit-exact against torch fp32 adds in the same order):
+ *   dst == NULL:  acc[seg.offset + i] = acc[seg.offset + i] + g * scale                  (dst_dtype ignored)
+ *   otherwise:    dst[seg.offset + i] = (dst type)(acc[seg.offset + i] + g * scale)     (fp32 or bf16; dst may be acc for fp32)
+ * A segment whose ptr is NULL contributes zero (a parameter without a gradient in this micro-batch): nothing is added, and
+ * with a dst the accumulator is converted alone. */
+int cotb200_multi_gather_acc(const cotb200_seg* segs_dev, const int* blocks_dev, int n_blocks, float* acc, int dst_dtype, void* dst,
+                             float scale, void* stream);
 /* dst = decay*dst + (1-decay)*src per segment (fp32; int64 with the reference's float round trip): ModelEmaV2 over the
  * BUFFERS of the state_dict (BatchNorm running statistics / counters), one launch.  decay = hyper_dev[3], the hyper_dev of
  * cotb200_opt_step. */
