@@ -9,6 +9,7 @@
 //   * bf16/fp16 are widened to fp32 for the FMA (exact products, fp32 accumulation).
 // Requires W % PXV == 0 (56, 28 -> 4; 14 -> 2); other widths use the first-generation scalar kernels.
 #include "common.cuh"
+#include "agg.cuh"
 
 namespace cotb200 {
 

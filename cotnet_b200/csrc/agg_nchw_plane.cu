@@ -12,6 +12,7 @@
 // One pass over every tensor: (3C + 9wc) + (C + 9wc) elements per pixel (dy, x, w in; dx, dw out).
 // The forward stays on the tiled kernels, which are faster there.
 #include "common.cuh"
+#include "agg.cuh"
 
 namespace cotb200 {
 

@@ -19,6 +19,7 @@
 // fp32 W in {56, 28, ..}, 16-bit W = 56; everything else stays on agg_nchw2.cu / the generic kernels.
 #include <cuda.h>
 #include "common.cuh"
+#include "agg.cuh"
 #include "tma.cuh"
 
 namespace cotb200 {
@@ -198,35 +199,14 @@ agg3_nchw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
 }
 
 // ------------------------------------------------------------------------------------------------ host
-typedef CUresult (*NtEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static NtEncodeFn nt_encode_fn() {
-  static NtEncodeFn fn = nullptr;
-  if (!fn) {
-    void* q = nullptr;
-    cudaDriverEntryPointQueryResult r;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &r) == cudaSuccess && r == cudaDriverEntryPointSuccess)
-      fn = (NtEncodeFn)q;
-  }
-  return fn;
-}
-template <typename T> static CUtensorMapDataType nt_dtype();
-template <> CUtensorMapDataType nt_dtype<float>() { return CU_TENSOR_MAP_DATA_TYPE_FLOAT32; }
-template <> CUtensorMapDataType nt_dtype<__nv_bfloat16>() { return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
-template <> CUtensorMapDataType nt_dtype<__half>() { return CU_TENSOR_MAP_DATA_TYPE_FLOAT16; }
-
 // generic 5-D map over a dense tensor: dims d[0..4] (d[0] innermost, unit stride), strides st[0..3] in ELEMENTS for d[1..4]
 template <typename T>
 static bool nt_make_map(CUtensorMap* m, const void* base, const long long (&d)[5], const long long (&st)[4], const int (&box)[5]) {
-  NtEncodeFn enc = nt_encode_fn();
-  if (!enc) return false;
   cuuint64_t dims[5], strides[4];
-  cuuint32_t b[5], es[5] = {1, 1, 1, 1, 1};
+  cuuint32_t b[5];
   for (int i = 0; i < 5; ++i) { dims[i] = (cuuint64_t)d[i]; b[i] = (cuuint32_t)box[i]; }
   for (int i = 0; i < 4; ++i) strides[i] = (cuuint64_t)st[i] * sizeof(T);
-  return enc(m, nt_dtype<T>(), 5, const_cast<void*>(base), dims, strides, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  return tma_encode(m, tma_dtype<T>(), 5, base, dims, strides, b, CU_TENSOR_MAP_SWIZZLE_NONE) == CUDA_SUCCESS;
 }
 
 static inline int nt_round_up(int a, int b) { return (a + b - 1) / b * b; }

@@ -12,6 +12,7 @@
 // Weight layouts: COTB200_NHWC (g*9+t, the torch channels_last view) for forward; COTB200_NHWC_TAP (tap-major chunks
 // of gc = 8 weight channels, the block-internal layout) for forward, dX and dW.
 #include "common.cuh"
+#include "agg.cuh"
 
 namespace cotb200 {
 
@@ -207,11 +208,6 @@ agg3_dw_nhwc2_kernel(const T* __restrict__ dy, const T* __restrict__ x, T* __res
 }
 
 // ------------------------------------------------------------------------------------------------ host dispatch
-struct Nhwc2Args {
-  int N, C, H, W, wc, fold, layout, gc, dtype;
-  long long x_sn, x_sp, w_sn, w_sp, y_sn, y_sp;
-};
-
 template <typename T>
 static bool nhwc2_ok(const Nhwc2Args& a, const void* p0, const void* p1, const void* p2, bool need_tap, G2& g) {
   constexpr int VEC = 16 / (int)sizeof(T);

@@ -14,6 +14,7 @@
 // Weight layout: COTB200_NHWC_TAP (tap-major chunks of gc weight channels) -- the block-internal layout.
 #include <cuda.h>
 #include "common.cuh"
+#include "agg.cuh"
 #include "tma.cuh"
 
 namespace cotb200 {
@@ -251,59 +252,27 @@ agg3_dw_tma_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_consta
 
 
 // ------------------------------------------------------------------------------------------------ host
-typedef CUresult (*AtEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static AtEncodeFn at_encode_fn() {
-  static AtEncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (AtEncodeFn)p;
-  }
-  return fn;
-}
-
-template <typename T> static CUtensorMapDataType at_dtype();
-template <> CUtensorMapDataType at_dtype<float>() { return CU_TENSOR_MAP_DATA_TYPE_FLOAT32; }
-template <> CUtensorMapDataType at_dtype<__nv_bfloat16>() { return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
-template <> CUtensorMapDataType at_dtype<__half>() { return CU_TENSOR_MAP_DATA_TYPE_FLOAT16; }
-
 // NHWC tensor [N,H,W,Cdim] with pixel pitch sp / batch pitch sn (elements); box {b0, b1, b2, 1}
 template <typename T>
 static bool at_make_map(CUtensorMap* m, const void* base, int N, int H, int W, int Cdim, long long sp, long long sn, int b0, int b1,
                         int b2, bool swizzle) {
-  AtEncodeFn enc = at_encode_fn();
-  if (!enc) return false;
   cuuint64_t dims[4] = {(cuuint64_t)Cdim, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
   cuuint64_t strides[3] = {(cuuint64_t)sp * sizeof(T), (cuuint64_t)sp * sizeof(T) * W, (cuuint64_t)sn * sizeof(T)};
   cuuint32_t box[4] = {(cuuint32_t)b0, (cuuint32_t)b1, (cuuint32_t)b2, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  return enc(m, at_dtype<T>(), 4, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  return tma_encode(m, tma_dtype<T>(), 4, base, dims, strides, box,
+                    swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE) == CUDA_SUCCESS;
 }
 
 // weights [N,H,W,J] as 5-D {jbox, jboxes, W, H, N}; box {jbox, jboxes, bw, bh, 1} -> smem [bh][bw][J]
 template <typename T>
 static bool at_make_map_w(CUtensorMap* m, const void* base, int N, int H, int W, int jbox, int jboxes, long long sp, long long sn,
                           int bw, int bh) {
-  AtEncodeFn enc = at_encode_fn();
-  if (!enc) return false;
   cuuint64_t dims[5] = {(cuuint64_t)jbox, (cuuint64_t)jboxes, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
   cuuint64_t strides[4] = {(cuuint64_t)jbox * sizeof(T), (cuuint64_t)sp * sizeof(T), (cuuint64_t)sp * sizeof(T) * W,
                            (cuuint64_t)sn * sizeof(T)};
   cuuint32_t box[5] = {(cuuint32_t)jbox, (cuuint32_t)jboxes, (cuuint32_t)bw, (cuuint32_t)bh, 1};
-  cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  return enc(m, at_dtype<T>(), 5, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  return tma_encode(m, tma_dtype<T>(), 5, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE) == CUDA_SUCCESS;
 }
-
-struct Nhwc2Args {
-  int N, C, H, W, wc, fold, layout, gc, dtype;
-  long long x_sn, x_sp, w_sn, w_sp, y_sn, y_sp;
-};
 
 // mode 0: a = x, b = w, out = y      mode 1: a = dy, b = w, out = dx      mode 2: a = x, b = dy, out = dw
 // returns 1 if handled (rc in *rc), 0 if the caller should use the register-resident kernels

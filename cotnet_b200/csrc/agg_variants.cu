@@ -290,13 +290,6 @@ dilate_fwd_fast(const T* __restrict__ x, const T* __restrict__ w, const T* __res
   }
 }
 
-static int vgrid(long long total) {
-  long long need = (total + 255) / 256;
-  const long long cap = (long long)num_sms() * 16;
-  if (need < 1) need = 1;
-  return (int)(need < cap ? need : cap);
-}
-
 static int vresolve(const cotb200_agg_desc* d, VGeo& g, const char* what, bool dilate) {
   if (!d) { set_error("%s: desc is NULL", what); return COTB200_ENULL; }
   if (d->layout != COTB200_NCHW) { set_error("%s supports the NCHW layout only (the reference contract)", what); return COTB200_ELAYOUT; }
@@ -337,11 +330,11 @@ extern "C" int cotb200_agg_refpad_fwd(const cotb200_agg_desc* d, const void* x, 
     const long long items = total / g.rep;
     const bool small = total < (1LL << 31) && (long long)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO < (1LL << 31) && g.H * g.W < (1 << 24);
     if (small && g.KH == g.KW && (g.KH == 3 || g.KH == 5 || g.KH == 7)) {
-      if (g.KH == 3) refpad_fwd_fast<T, 3><<<vgrid(items), 256, 0, st>>>((const T*)x, (const T*)w, (T*)y, g, (int)items);
-      else if (g.KH == 5) refpad_fwd_fast<T, 5><<<vgrid(items), 256, 0, st>>>((const T*)x, (const T*)w, (T*)y, g, (int)items);
-      else refpad_fwd_fast<T, 7><<<vgrid(items), 256, 0, st>>>((const T*)x, (const T*)w, (T*)y, g, (int)items);
+      if (g.KH == 3) refpad_fwd_fast<T, 3><<<grid_stride_blocks(items, 256, 16), 256, 0, st>>>((const T*)x, (const T*)w, (T*)y, g, (int)items);
+      else if (g.KH == 5) refpad_fwd_fast<T, 5><<<grid_stride_blocks(items, 256, 16), 256, 0, st>>>((const T*)x, (const T*)w, (T*)y, g, (int)items);
+      else refpad_fwd_fast<T, 7><<<grid_stride_blocks(items, 256, 16), 256, 0, st>>>((const T*)x, (const T*)w, (T*)y, g, (int)items);
     } else {
-      refpad_fwd_kernel<T><<<vgrid(total), 256, 0, st>>>((const T*)x, (const T*)w, (T*)y, g, total);
+      refpad_fwd_kernel<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)x, (const T*)w, (T*)y, g, total);
     }
     return check_launch("agg_refpad_fwd");
   });
@@ -359,14 +352,14 @@ extern "C" int cotb200_agg_refpad_bwd(const cotb200_agg_desc* d, const void* dy,
     if (dx) {
       const long long total = (long long)g.N * g.C * g.H * g.W;
       COTB200_PROF("agg_refpad_dx");
-      refpad_dx_kernel<T><<<vgrid(total), 256, 0, st>>>((const T*)dy, (const T*)w, (T*)dx, g, total);
+      refpad_dx_kernel<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)w, (T*)dx, g, total);
       rc = check_launch("agg_refpad_dx");
       if (rc) return rc;
     }
     if (dw) {
       const long long total = (long long)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO;
       COTB200_PROF("agg_refpad_dw");
-      refpad_dw_kernel<T><<<vgrid(total), 256, 0, st>>>((const T*)dy, (const T*)x, (T*)dw, g, total);
+      refpad_dw_kernel<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)x, (T*)dw, g, total);
       rc = check_launch("agg_refpad_dw");
     }
     return rc;
@@ -385,9 +378,9 @@ extern "C" int cotb200_agg_zeropad_dilate_fwd(const cotb200_agg_desc* d, const v
   COTB200_DISPATCH_DTYPE(d->dtype, {
     COTB200_PROF_B("agg_dilate_fwd", ((double)g.N * g.H * g.W) * ((double)g.C + g.heads * (g.wc * 9.0 + g.C)) * sizeof(T));
     if (total < (1LL << 31) && (long long)g.N * g.heads * g.wc * 9 * g.H * g.W < (1LL << 31))
-      dilate_fwd_fast<T><<<vgrid(total / g.rep), 256, 0, st>>>((const T*)x, (const T*)w, (const T*)dilation, (T*)y, g, (int)(total / g.rep));
+      dilate_fwd_fast<T><<<grid_stride_blocks(total / g.rep, 256, 16), 256, 0, st>>>((const T*)x, (const T*)w, (const T*)dilation, (T*)y, g, (int)(total / g.rep));
     else
-      dilate_fwd_kernel<T><<<vgrid(total), 256, 0, st>>>((const T*)x, (const T*)w, (const T*)dilation, (T*)y, g, total);
+      dilate_fwd_kernel<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)x, (const T*)w, (const T*)dilation, (T*)y, g, total);
     return check_launch("agg_zeropad_dilate_fwd");
   });
   return 0;
@@ -404,14 +397,14 @@ extern "C" int cotb200_agg_zeropad_dilate_bwd(const cotb200_agg_desc* d, const v
     if (dx) {
       const long long total = (long long)g.N * g.C * g.H * g.W;
       COTB200_PROF("agg_dilate_dx");
-      dilate_dx_kernel<T><<<vgrid(total), 256, 0, st>>>((const T*)dy, (const T*)w, (const T*)dilation, (T*)dx, g, total);
+      dilate_dx_kernel<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)w, (const T*)dilation, (T*)dx, g, total);
       rc = check_launch("agg_dilate_dx");
       if (rc) return rc;
     }
     if (dw) {
       const long long total = (long long)g.N * g.heads * g.wc * 9 * g.H * g.W;
       COTB200_PROF("agg_dilate_dw");
-      dilate_dw_kernel<T><<<vgrid(total), 256, 0, st>>>((const T*)dy, (const T*)x, (const T*)dilation, (T*)dw, g, total);
+      dilate_dw_kernel<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)x, (const T*)dilation, (T*)dw, g, total);
       rc = check_launch("agg_dilate_dw");
     }
     return rc;

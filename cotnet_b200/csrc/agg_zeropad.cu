@@ -16,6 +16,7 @@
 //   * generic path: any kernel size / stride / dilation / heads / dtype (incl. fp64), 64-bit indexing.
 // Accumulation is fp32 (fp64 for double).  Zero padding == skipped taps, exactly like the reference.
 #include "common.cuh"
+#include "agg.cuh"
 
 namespace cotb200 {
 
@@ -472,35 +473,7 @@ agg3_dw_nhwc_fast(const T* __restrict__ dy, const T* __restrict__ x, T* __restri
   }
 }
 
-// second-generation NHWC kernels (agg_nhwc2.cu)
-struct Nhwc2Args {
-  int N, C, H, W, wc, fold, layout, gc, dtype;
-  long long x_sn, x_sp, w_sn, w_sp, y_sn, y_sp;
-};
-template <typename T> int nhwc2_fwd(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
-template <typename T> int agg_tma_fwd(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);   // agg_tma.cu
-template <typename T> int agg_tma_dx(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
-template <typename T> int agg_tma_dw(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
-template <typename T> int nhwc2_dx(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
-template <typename T> int nhwc2_dw(const Nhwc2Args&, const T*, const T*, T*, cudaStream_t, int*);
-// TMA-pipelined NCHW kernels (agg_nchw_tma.cu): mode 0 fwd / 1 dX / 2 dW
-template <typename T> int nchw_tma_launch(int, int, int, int, int, int, long long, long long, long long, const T*, const T*, T*,
-                                          cudaStream_t, int*);
-// small-plane NCHW backward kernels (agg_nchw_plane.cu): mode 1 dX / 2 dW / 3 dX + dW
-template <typename T> int nchw_plane_launch(int, int, int, int, int, int, long long, long long, long long, const T*, const T*, const T*, T*, T*,
-                                            cudaStream_t, int*);
-// second-generation NCHW kernels (agg_nchw2.cu)
-template <typename T> int nchw2_fwd(int, int, int, int, int, long long, const T*, const T*, T*, cudaStream_t, int*);
-template <typename T> int nchw2_bwd(int, int, int, int, int, long long, const T*, const T*, const T*, T*, T*, cudaStream_t, int*);
-
 // ------------------------------------------------------------------------------------------------ host
-static int grid_for(long long total, int block, int per_sm = 8) {
-  long long need = (total + block - 1) / block;
-  long long cap = (long long)num_sms() * per_sm;     // grid-stride loop covers the rest
-  if (need < 1) need = 1;
-  return (int)(need < cap ? need : cap);
-}
-
 static int resolve(const cotb200_agg_desc* d, Geo& g) {
   if (!d) { set_error("desc is NULL"); return COTB200_ENULL; }
   if (d->n <= 0 || d->c <= 0 || d->h <= 0 || d->w <= 0 || d->heads <= 0 || d->wc <= 0 || d->kh <= 0 || d->kw <= 0 ||
@@ -591,7 +564,7 @@ static int fwd_impl(const Geo& g, const T* x, const T* w, T* y, cudaStream_t st)
   if (g.layout == COTB200_NCHW && nofold(g) && fits32(g) && (is_same3(g, 3) || is_same3(g, 5))) {
     if constexpr (!std::is_same<T, double>::value) {
       const int total = g.N * g.wc * g.H * g.W;
-      const int grid = grid_for(total, 256);
+      const int grid = grid_stride_blocks(total, 256, 8);
       COTB200_PROF_B(g.KH == 3 ? "agg_fwd_nchw_k3" : "agg_fwd_nchw_k5", ((double)g.N * g.C * g.H * g.W + (double)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO + (double)g.N * g.heads * g.C * g.HO * g.WO) * sizeof(T));
       if (g.KH == 3) agg_fwd_nchw_fast<T, 3><<<grid, 256, 0, st>>>(x, w, y, g.N, g.C, g.H, g.W, g.wc, g.rep, g.y_sn, g.w_sn, total);
       else agg_fwd_nchw_fast<T, 5><<<grid, 256, 0, st>>>(x, w, y, g.N, g.C, g.H, g.W, g.wc, g.rep, g.y_sn, g.w_sn, total);
@@ -603,7 +576,7 @@ static int fwd_impl(const Geo& g, const T* x, const T* w, T* y, cudaStream_t st)
       const int vec = nhwc_vec<T>(g, x, w, y);
       if (vec) {
         const int total = g.N * g.H * g.W * (g.C / vec);
-        const int grid = grid_for(total, 256);
+        const int grid = grid_stride_blocks(total, 256, 8);
         const bool tap = g.layout == COTB200_NHWC_TAP;
         COTB200_PROF_B("agg3_fwd_nhwc", ((double)g.N * g.C * g.H * g.W + (double)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO + (double)g.N * g.heads * g.C * g.HO * g.WO) * sizeof(T));
 #define COTB200_LAUNCH_FWD(V)                                                                                     \
@@ -622,7 +595,7 @@ static int fwd_impl(const Geo& g, const T* x, const T* w, T* y, cudaStream_t st)
   }
   const long long total = (long long)g.N * g.heads * g.C * g.HO * g.WO;
   COTB200_PROF_B("agg_fwd_generic", ((double)g.N * g.C * g.H * g.W + (double)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO + (double)g.N * g.heads * g.C * g.HO * g.WO) * sizeof(T));
-  agg_fwd_generic<T><<<grid_for(total, 256, 16), 256, 0, st>>>(x, w, y, g, total);
+  agg_fwd_generic<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>(x, w, y, g, total);
   return check_launch("agg_fwd_generic");
 }
 
@@ -647,7 +620,7 @@ static int bwd_impl(const Geo& g, const T* dy, const T* x, const T* w, T* dx, T*
   if (g.layout == COTB200_NCHW && nofold(g) && fits32(g) && (is_same3(g, 3) || is_same3(g, 5))) {
     if constexpr (!std::is_same<T, double>::value) {
       const int total = g.N * g.wc * g.H * g.W;
-      const int grid = grid_for(total, 256);
+      const int grid = grid_stride_blocks(total, 256, 8);
       COTB200_PROF_B(dx && dw ? "agg_bwd_nchw_dxdw" : (dx ? "agg_bwd_nchw_dx" : "agg_bwd_nchw_dw"), (dx && dw ? 1.0 : 0.0) * ((double)g.N * g.C * g.H * g.W + (double)g.N * g.wc * g.K2 * g.HO * g.WO) * sizeof(T) + ((double)g.N * g.C * g.H * g.W + (double)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO + (double)g.N * g.heads * g.C * g.HO * g.WO) * sizeof(T));
 #define COTB200_LAUNCH_BWD(K, DX, DW, ACC)                                                                          \
   agg_bwd_nchw_fast<T, K, DX, DW, ACC><<<grid, 256, 0, st>>>(dy, x, w, dx, dw, g.N, g.C, g.H, g.W, g.wc, g.rep,      \
@@ -685,7 +658,7 @@ static int bwd_impl(const Geo& g, const T* dy, const T* x, const T* w, T* dx, T*
   if (vec == V) {                                                                                                    \
     if (dx) {                                                                                                        \
       const int total = g.N * g.H * g.W * (g.C / V);                                                                 \
-      const int grid = grid_for(total, 256);                                                                         \
+      const int grid = grid_stride_blocks(total, 256, 8);                                                            \
       COTB200_PROF_B("agg3_dx_nhwc", ((double)g.N * g.C * g.H * g.W + (double)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO + (double)g.N * g.heads * g.C * g.HO * g.WO) * sizeof(T));                                                                                 \
       if (tap) agg3_dx_nhwc_fast<T, V, true><<<grid, 256, 0, st>>>(dy, w, dx, g.N, g.C, g.H, g.W, g.Cf, g.wcf, g.x_sn, \
                                                                     g.x_sw, g.w_sn, g.w_sw, g.y_sn, g.y_sw, total);  \
@@ -696,7 +669,7 @@ static int bwd_impl(const Geo& g, const T* dy, const T* x, const T* w, T* dx, T*
     }                                                                                                                \
     if (dw) {                                                                                                        \
       const int total = g.N * g.H * g.W * (g.wc / V);                                                                \
-      const int grid = grid_for(total, 256);                                                                         \
+      const int grid = grid_stride_blocks(total, 256, 8);                                                            \
       COTB200_PROF_B("agg3_dw_nhwc", ((double)g.N * g.C * g.H * g.W + (double)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO + (double)g.N * g.heads * g.C * g.HO * g.WO) * sizeof(T));                                                                                 \
       if (tap) agg3_dw_nhwc_fast<T, V, true><<<grid, 256, 0, st>>>(dy, x, dw, g.N, g.C, g.H, g.W, g.wc, g.Cf, g.wcf, g.rep, \
                                                                     g.x_sn, g.x_sw, g.w_sn, g.w_sw, g.y_sn, g.y_sw,  \
@@ -717,15 +690,15 @@ static int bwd_impl(const Geo& g, const T* dy, const T* x, const T* w, T* dx, T*
   if (dx) {
     const long long total = (long long)g.N * g.C * g.H * g.W;
     COTB200_PROF_B("agg_dx_generic", ((double)g.N * g.C * g.H * g.W + (double)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO + (double)g.N * g.heads * g.C * g.HO * g.WO) * sizeof(T));
-    if (acc_dx) agg_dx_generic<T, true><<<grid_for(total, 256, 16), 256, 0, st>>>(dy, w, dx, g, total);
-    else agg_dx_generic<T, false><<<grid_for(total, 256, 16), 256, 0, st>>>(dy, w, dx, g, total);
+    if (acc_dx) agg_dx_generic<T, true><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>(dy, w, dx, g, total);
+    else agg_dx_generic<T, false><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>(dy, w, dx, g, total);
     rc = check_launch("agg_dx_generic");
     if (rc) return rc;
   }
   if (dw) {
     const long long total = (long long)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO;
     COTB200_PROF_B("agg_dw_generic", ((double)g.N * g.C * g.H * g.W + (double)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO + (double)g.N * g.heads * g.C * g.HO * g.WO) * sizeof(T));
-    agg_dw_generic<T><<<grid_for(total, 256, 16), 256, 0, st>>>(dy, x, dw, g, total);
+    agg_dw_generic<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>(dy, x, dw, g, total);
     rc = check_launch("agg_dw_generic");
   }
   return rc;
@@ -784,8 +757,8 @@ extern "C" int cotb200_agg_zeropad_mix_fwd(const cotb200_agg_desc* d, int k2h, i
       if (is_same3(g1, 3) && is_same3(g2, 5) && fits32(g2) && 2 * half * g1.N < (1LL << 31)) {
         const int total = g1.N * g1.wc * g1.H * g1.W;
         COTB200_PROF("agg_mix_fwd_nchw");
-        agg_mix_fwd_nchw_fast<T><<<grid_for(total, 256), 256, 0, st>>>((const T*)x, (const T*)w1, (const T*)w2, (T*)y, g1.N,
-                                                                      g1.C, g1.H, g1.W, g1.wc, g1.rep, total);
+        agg_mix_fwd_nchw_fast<T><<<grid_stride_blocks(total, 256, 8), 256, 0, st>>>((const T*)x, (const T*)w1, (const T*)w2, (T*)y, g1.N,
+                                                                                   g1.C, g1.H, g1.W, g1.wc, g1.rep, total);
         return check_launch("agg_mix_fwd_nchw_fast");
       }
     }
@@ -816,8 +789,8 @@ extern "C" int cotb200_agg_zeropad_mix_bwd(const cotb200_agg_desc* d, int k2h, i
     if (dx) {   // both halves of dX in one fp32-accumulating pass
       const long long total = (long long)g1.N * g1.C * g1.H * g1.W;
       COTB200_PROF("agg_mix_dx");
-      agg_dx_generic2<T><<<grid_for(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)w1, g1, (const T*)dy + half,
-                                                                  (const T*)w2, g2, (T*)dx, total);
+      agg_dx_generic2<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)w1, g1, (const T*)dy + half,
+                                                                            (const T*)w2, g2, (T*)dx, total);
       rc = check_launch("agg_mix_dx");
       if (rc) return rc;
     }
@@ -878,19 +851,19 @@ extern "C" int cotb200_agg_zeropad_mix_merge_bwd(const cotb200_agg_desc* d, int 
     if (dx) {
       const long long total = (long long)g1.N * g1.C * g1.H * g1.W;
       COTB200_PROF("agg_mix_merge_dx");
-      agg_dx_generic2<T><<<grid_for(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)w, g1, (const T*)dy + half,
-                                                                  (const T*)w + off2, g2, (T*)dx, total);
+      agg_dx_generic2<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)w, g1, (const T*)dy + half,
+                                                                            (const T*)w + off2, g2, (T*)dx, total);
       rc = check_launch("agg_mix_merge_dx");
       if (rc) return rc;
     }
     if (dw) {
       COTB200_PROF("agg_mix_merge_dw");
       const long long t1 = (long long)g1.N * g1.heads * g1.wc * g1.K2 * g1.HO * g1.WO;
-      agg_dw_generic<T><<<grid_for(t1, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)x, (T*)dw, g1, t1);
+      agg_dw_generic<T><<<grid_stride_blocks(t1, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)x, (T*)dw, g1, t1);
       rc = check_launch("agg_mix_merge_dw");
       if (rc) return rc;
       const long long t2 = (long long)g2.N * g2.heads * g2.wc * g2.K2 * g2.HO * g2.WO;
-      agg_dw_generic<T><<<grid_for(t2, 256, 16), 256, 0, st>>>((const T*)dy + half, (const T*)x, (T*)dw + off2, g2, t2);
+      agg_dw_generic<T><<<grid_stride_blocks(t2, 256, 16), 256, 0, st>>>((const T*)dy + half, (const T*)x, (T*)dw + off2, g2, t2);
       rc = check_launch("agg_mix_merge_dw");
     }
     return rc;

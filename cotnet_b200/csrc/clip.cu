@@ -105,14 +105,6 @@ unit_norms_kernel(const cotb200_clip_unit* __restrict__ units, int n_units, cons
   if (norms) { norms[2 * u] = pn; norms[2 * u + 1] = gn; }
 }
 
-static unsigned clip_stream_grid(long long items, int per_sm) {
-  long long blocks = (items + 255) / 256;
-  const long long cap = (long long)num_sms() * per_sm;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (unsigned)blocks;
-}
-
 }  // namespace cotb200
 
 using namespace cotb200;
@@ -131,7 +123,7 @@ extern "C" int cotb200_grad_norm(long long n0, int g0_dtype, const void* G0, con
   }
   cudaStream_t st = (cudaStream_t)stream;
   const long long n04 = n0 / 4, n14 = n1 / 4;
-  const int b0 = (int)clip_stream_grid(n04, 4), b1 = n14 ? (int)clip_stream_grid(n14, 1) : 0;
+  const int b0 = grid_stride_blocks(n04, 256, 4), b1 = n14 ? grid_stride_blocks(n14, 256, 1) : 0;
   DetScratch ds;
   if (int rc = ds.alloc(det_floats(b0 + b1, 1), 1, st)) return rc;
   COTB200_PROF_B("grad_norm", (double)n0 * (g0_dtype == COTB200_F32 ? 4.0 : 2.0) + (double)n1 * 4.0 + 8.0);

@@ -60,6 +60,23 @@ inline int num_sms() {
   }
   return s;
 }
+// CTAs of a grid-stride launch of `threads`-thread CTAs over `items` work items: enough to cover them, at least one, at most
+// per_sm per SM (the loop inside the kernel covers the rest).
+inline int grid_stride_blocks(long long items, int threads, int per_sm) {
+  const long long need = (items + threads - 1) / threads;
+  const long long cap = (long long)num_sms() * per_sm;
+  return (int)(need < 1 ? 1 : need < cap ? need : cap);
+}
+
+// Opts a kernel into `smem` bytes of dynamic shared memory when that is more than the default 48 KB.
+template <typename KFn>
+inline int ensure_smem(KFn fn, size_t smem) {
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
+  }
+  return 0;
+}
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 

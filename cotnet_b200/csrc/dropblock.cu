@@ -192,11 +192,6 @@ dropblock_res_relu_bwd_kernel(const T* __restrict__ dy, const unsigned char* __r
   }
 }
 
-static int db_grid(long long npk) {
-  const long long want = (npk + DB_THREADS - 1) / DB_THREADS, cap = (long long)num_sms() * 16;
-  return (int)(want < cap ? (want > 0 ? want : 1) : cap);
-}
-
 // shared checks of the elementwise entry points: B*HW*C elements of a 16-bit or fp32 NHWC tensor, C % 8 == 0
 static int db_rows_check(const char* what, int dtype, int B, int HW, int C) {
   if (B <= 0 || HW <= 0 || C <= 0 || C % 8) { set_error("%s: bad geometry B=%d HW=%d C=%d (C %% 8 == 0)", what, B, HW, C); return COTB200_EINVAL; }
@@ -253,7 +248,7 @@ extern "C" int cotb200_dropblock_apply(int dtype, int B, int HW, int C, const vo
     {
       const long long npk = n / 8;
       COTB200_PROF_B("dropblock_apply", (double)n * (2 * sizeof(T)) + n / 8.0);
-      dropblock_apply_kernel<T><<<db_grid(npk), DB_THREADS, 0, st>>>((const T*)x, (const unsigned char*)mask, count, n, (T*)y, npk);
+      dropblock_apply_kernel<T><<<grid_stride_blocks(npk, DB_THREADS, 16), DB_THREADS, 0, st>>>((const T*)x, (const unsigned char*)mask, count, n, (T*)y, npk);
       return check_launch("dropblock_apply");
     }
   });
@@ -271,9 +266,9 @@ extern "C" int cotb200_dropblock_res_relu(int dtype, int B, int HW, int C, const
     {
       const long long npk = n / 8;
       COTB200_PROF_B("dropblock_res_relu", (double)n * (3 * sizeof(T)) + n / 4.0);
-      if (ds) dropblock_res_relu_kernel<T, true><<<db_grid(npk), DB_THREADS, 0, st>>>(
+      if (ds) dropblock_res_relu_kernel<T, true><<<grid_stride_blocks(npk, DB_THREADS, 16), DB_THREADS, 0, st>>>(
           (const T*)z, (const T*)res, (const unsigned char*)mask, count, n, ds, per, (T*)y, (unsigned char*)relu_mask, npk);
-      else dropblock_res_relu_kernel<T, false><<<db_grid(npk), DB_THREADS, 0, st>>>(
+      else dropblock_res_relu_kernel<T, false><<<grid_stride_blocks(npk, DB_THREADS, 16), DB_THREADS, 0, st>>>(
           (const T*)z, (const T*)res, (const unsigned char*)mask, count, n, ds, per, (T*)y, (unsigned char*)relu_mask, npk);
       return check_launch("dropblock_res_relu");
     }
@@ -293,9 +288,9 @@ extern "C" int cotb200_dropblock_res_relu_bwd(int dtype, int B, int HW, int C, c
     {
       const long long npk = n / 8;
       COTB200_PROF_B("dropblock_res_relu_bwd", (double)n * ((dres ? 3 : 2) * sizeof(T)) + n / 4.0);
-      if (ds) dropblock_res_relu_bwd_kernel<T, true><<<db_grid(npk), DB_THREADS, 0, st>>>(
+      if (ds) dropblock_res_relu_bwd_kernel<T, true><<<grid_stride_blocks(npk, DB_THREADS, 16), DB_THREADS, 0, st>>>(
           (const T*)dy, (const unsigned char*)relu_mask, (const unsigned char*)mask, count, n, ds, per, (T*)dres, (T*)dz, npk);
-      else dropblock_res_relu_bwd_kernel<T, false><<<db_grid(npk), DB_THREADS, 0, st>>>(
+      else dropblock_res_relu_bwd_kernel<T, false><<<grid_stride_blocks(npk, DB_THREADS, 16), DB_THREADS, 0, st>>>(
           (const T*)dy, (const unsigned char*)relu_mask, (const unsigned char*)mask, count, n, ds, per, (T*)dres, (T*)dz, npk);
       return check_launch("dropblock_res_relu_bwd");
     }

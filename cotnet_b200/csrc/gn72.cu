@@ -18,6 +18,7 @@
 //     dbeta AND the bias gradient of the embed.3 convolution analytically (no extra pass over dl).
 // Algorithmic bytes: stats J, apply 2J, bwd_sums 2J, bwd_apply 3J (x px x s) -- unchanged; the point is reaching them.
 #include "common.cuh"
+#include "gn72.cuh"
 #include "tma.cuh"
 
 namespace cotb200 {
@@ -394,21 +395,12 @@ static GN72 make_gn72(int B, int HW, int wc, int tb) {
   return g;
 }
 
-template <typename KFn>
-static int g7_smem_attr(KFn fn, size_t smem) {
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
-  }
-  return 0;
-}
-
 template <typename T>
 int gn72_stats_launch(int B, int HW, int wc, const void* l, const float* lbias, float* gsum, float* gsq, cudaStream_t st) {
   constexpr int TB = G7<T>::TB;
   GN72 g = make_gn72(B, HW, wc, TB);
   const size_t smem = (size_t)2 * TB * 72 * sizeof(T);
-  int rc = g7_smem_attr(gn72_stats_kernel<T>, smem);
+  int rc = ensure_smem(gn72_stats_kernel<T>, smem);
   if (rc) return rc;
   // walkers per sample: enough CTAs for ~4 per SM, never more than the sample has tiles
   const int ntiles = (g.bps + TB - 1) / TB;
@@ -428,7 +420,7 @@ int gn72_apply_launch(int B, int HW, int wc, const void* l, const float* lbias, 
   constexpr int TB = G7<T>::TB;
   const GN72 g = make_gn72(B, HW, wc, TB);
   const size_t smem = (size_t)TB * 72 * sizeof(T);
-  int rc = g7_smem_attr(gn72_apply_kernel<T>, smem);
+  int rc = ensure_smem(gn72_apply_kernel<T>, smem);
   if (rc) return rc;
   gn72_apply_kernel<T><<<dim3((g.bps + TB - 1) / TB, B), TB, smem, st>>>((const T*)l, lbias, mean, rstd, gamma, beta, (T*)out, g);
   return check_launch("gn9_apply(gn72)");
@@ -439,7 +431,7 @@ int gn72_bwd_sums_launch(int B, int HW, int wc, const void* dg, const void* l, f
   constexpr int TB = G7<T>::TB;
   GN72 g = make_gn72(B, HW, wc, TB);
   const size_t smem = (size_t)2 * TB * 72 * sizeof(T);
-  int rc = g7_smem_attr(gn72_bwd_sums_kernel<T>, smem);
+  int rc = ensure_smem(gn72_bwd_sums_kernel<T>, smem);
   if (rc) return rc;
   const int PR = TB / g.nchunk;
   DetScratch ds;
@@ -461,7 +453,7 @@ int gn72_bwd_apply_launch(int B, int HW, int wc, const void* dg, const void* l, 
   constexpr int TB = G7<T>::TB;
   const GN72 g = make_gn72(B, HW, wc, TB);
   const size_t smem = (size_t)2 * TB * 72 * sizeof(T);
-  int rc = g7_smem_attr(gn72_bwd_apply_kernel<T>, smem);
+  int rc = ensure_smem(gn72_bwd_apply_kernel<T>, smem);
   if (rc) return rc;
   gn72_bwd_apply_kernel<T><<<dim3((g.bps + TB - 1) / TB, B), TB, smem, st>>>((const T*)dg, (const T*)l, lbias, mean, rstd, gamma, s1, s2, (T*)dl, g);
   return check_launch("gn9_bwd_apply(gn72)");

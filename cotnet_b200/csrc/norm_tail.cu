@@ -11,6 +11,7 @@
 // warp always touches whole 128-byte lines; per-column partial sums live in registers, are reduced across ty through
 // shared memory and leave the CTA through one deterministic reduction per column (det_cols).
 #include "common.cuh"
+#include "gn72.cuh"
 
 namespace cotb200 {
 
@@ -726,27 +727,6 @@ static int col_chunk(int C, int vec) {
     case 2: { constexpr int V = 2; __VA_ARGS__; } break;           \
     default: { constexpr int V = 1; __VA_ARGS__; } break;          \
   }
-
-template <typename KFn>
-static int ensure_smem(KFn fn, size_t smem) {
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
-  }
-  return 0;
-}
-
-// block-of-72 kernels (gn72.cu)
-bool gn72_ok(int dtype, int wc, int gc, bool permuting, const void* p0, const void* p1, const void* p2);
-template <typename T> int gn72_stats_launch(int B, int HW, int wc, const void* l, const float* lbias, float* gsum, float* gsq, cudaStream_t st);
-template <typename T> int gn72_apply_launch(int B, int HW, int wc, const void* l, const float* lbias, const float* mean, const float* rstd,
-                                            const float* gamma, const float* beta, void* out, cudaStream_t st);
-template <typename T> int gn72_bwd_sums_launch(int B, int HW, int wc, const void* dg, const void* l, float* P, cudaStream_t st);
-template <typename T> int gn72_bwd_apply_launch(int B, int HW, int wc, const void* dg, const void* l, const float* lbias, const float* mean,
-                                                const float* rstd, const float* gamma, const float* s1, const float* s2, void* dl,
-                                                cudaStream_t st);
-int gn_bwd_finish_launch(int B, int HW, int wc, const float* P, int raw, const float* lbias, const float* mean, const float* rstd,
-                         const float* gamma, float* s1, float* s2, float* dgamma, float* dbeta, float* dlbias, cudaStream_t st);
 
 }  // namespace cotb200
 

@@ -293,14 +293,6 @@ lookahead_sync_kernel(float* __restrict__ P, float* __restrict__ S, __nv_bfloat1
   }
 }
 
-static unsigned opt_stream_grid(long long items, int per_sm) {
-  long long blocks = (items + 255) / 256;
-  const long long cap = (long long)num_sms() * per_sm;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (unsigned)blocks;
-}
-
 static bool rule_known(int r) { return r >= COTB200_OPT_SGD && r <= COTB200_OPT_RMSPROPTF; }
 
 // Validation of a clip descriptor (NULL: no clip); 0 or an error code with the message set.
@@ -324,7 +316,7 @@ static void launch_pass(const OptArgs<TG>& a, long long n4, const cotb200_clip* 
     opt_agc_kernel<TG, RULE><<<(unsigned)((clip->n_segs + 7) / 8), 256, 0, st>>>(a, clip->segs, clip->n_segs, clip->factor);
     return;
   }
-  const unsigned grid = opt_stream_grid(n4, 16);
+  const int grid = grid_stride_blocks(n4, 256, 16);
   if (mode == COTB200_CLIP_NORM) opt_uniform_kernel<TG, RULE, COTB200_CLIP_NORM><<<grid, 256, 0, st>>>(a, n4, clip->factor, 0.f);
   else if (mode == COTB200_CLIP_VALUE) opt_uniform_kernel<TG, RULE, COTB200_CLIP_VALUE><<<grid, 256, 0, st>>>(a, n4, nullptr, clip->value);
   else opt_uniform_kernel<TG, RULE, 0><<<grid, 256, 0, st>>>(a, n4, nullptr, 0.f);
@@ -420,6 +412,6 @@ extern "C" int cotb200_lookahead_sync(long long n, float* P, void* Pb, const cot
   }
   cudaStream_t st = (cudaStream_t)stream;
   COTB200_PROF_B("lookahead_sync", (double)n * (16.0 + (Pb ? 2.0 : 0.0)));
-  lookahead_sync_kernel<<<opt_stream_grid(n / 4, 16), 256, 0, st>>>(P, opt->S, (__nv_bfloat16*)Pb, opt->state, opt->lookahead_alpha, n / 4);
+  lookahead_sync_kernel<<<grid_stride_blocks(n / 4, 256, 16), 256, 0, st>>>(P, opt->S, (__nv_bfloat16*)Pb, opt->state, opt->lookahead_alpha, n / 4);
   return check_launch("lookahead_sync");
 }

@@ -232,14 +232,6 @@ u8_mix_rows_to_nhwc_generic_kernel(const unsigned char* __restrict__ x, T* __res
   }
 }
 
-static unsigned stream_grid(long long items) {
-  long long blocks = (items + 255) / 256;
-  const long long cap = (long long)num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return (unsigned)blocks;
-}
-
 }  // namespace cotb200
 
 using namespace cotb200;
@@ -306,11 +298,11 @@ extern "C" int cotb200_u8_to_nhwc(int dtype, int N, int C, int H, int W, const v
       COTB200_PROF_B("u8_to_nhwc", (double)N * C * HW * (1.0 + sizeof(T)));
       if (fast) {
         const long long npix4 = (long long)N * HW / 4;
-        u8_to_nhwc3_kernel<T><<<stream_grid(npix4), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, npix4, HW, mean_host[0], mean_host[1],
+        u8_to_nhwc3_kernel<T><<<grid_stride_blocks(npix4, 256, 16), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, npix4, HW, mean_host[0], mean_host[1],
                                                                    mean_host[2], std_host[0], std_host[1], std_host[2]);
       } else {
         const long long total = (long long)N * C * HW;
-        u8_to_nhwc_generic_kernel<T><<<stream_grid(total), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, total, C, HW, mean_dev, std_dev);
+        u8_to_nhwc_generic_kernel<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, total, C, HW, mean_dev, std_dev);
       }
       return check_launch("u8_to_nhwc");
     }
@@ -344,12 +336,12 @@ extern "C" int cotb200_u8_mix_rows_to_nhwc(int dtype, int N_in, int N_out, int C
       COTB200_PROF_B("u8_mix_rows_to_nhwc", (double)N_out * C * HW * (2.0 + sizeof(T)));
       if (fast) {
         const long long npix4 = (long long)N_out * HW / 4;
-        u8_mix_rows_to_nhwc3_kernel<T><<<stream_grid(npix4), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, npix4, HW, W, N_in, rows_dev,
+        u8_mix_rows_to_nhwc3_kernel<T><<<grid_stride_blocks(npix4, 256, 16), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, npix4, HW, W, N_in, rows_dev,
                                                                             mean_host[0], mean_host[1], mean_host[2], std_host[0],
                                                                             std_host[1], std_host[2]);
       } else {
         const long long total = (long long)N_out * C * HW;
-        u8_mix_rows_to_nhwc_generic_kernel<T><<<stream_grid(total), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, total, C, HW, W, N_in,
+        u8_mix_rows_to_nhwc_generic_kernel<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const unsigned char*)x_u8, (T*)y, total, C, HW, W, N_in,
                                                                                    rows_dev, mean_dev, std_dev);
       }
       return check_launch("u8_mix_rows_to_nhwc");

@@ -72,15 +72,13 @@ extern "C" int cotb200_sum_rows(int dtype, long long rows, int C, const void* sr
       while (vec > 1 && !fits(vec)) vec >>= 1;
       const int CQ = C / vec;
       const long long total = rows * CQ;
-      long long blocks = (total + 255) / 256;
-      const long long cap = (long long)num_sms() * 16;        // grid-stride: 2 waves of 8 CTAs per SM
-      if (blocks > cap) blocks = cap;
+      const int blocks = grid_stride_blocks(total, 256, 16);   // 2 waves of 8 CTAs per SM
       COTB200_PROF_B("sum_rows", (double)rows * C * (nsrc + 1) * sizeof(T));
       switch (vec) {
-        case 8: if constexpr (sizeof(T) == 2) sum_rows_launch<T, 8>(nsrc, s, (T*)out, ldo, rows, CQ, (unsigned)blocks, st); break;
-        case 4: sum_rows_launch<T, 4>(nsrc, s, (T*)out, ldo, rows, CQ, (unsigned)blocks, st); break;
-        case 2: sum_rows_launch<T, 2>(nsrc, s, (T*)out, ldo, rows, CQ, (unsigned)blocks, st); break;
-        default: sum_rows_launch<T, 1>(nsrc, s, (T*)out, ldo, rows, CQ, (unsigned)blocks, st); break;
+        case 8: if constexpr (sizeof(T) == 2) sum_rows_launch<T, 8>(nsrc, s, (T*)out, ldo, rows, CQ, blocks, st); break;
+        case 4: sum_rows_launch<T, 4>(nsrc, s, (T*)out, ldo, rows, CQ, blocks, st); break;
+        case 2: sum_rows_launch<T, 2>(nsrc, s, (T*)out, ldo, rows, CQ, blocks, st); break;
+        default: sum_rows_launch<T, 1>(nsrc, s, (T*)out, ldo, rows, CQ, blocks, st); break;
       }
       return check_launch("sum_rows");
     }

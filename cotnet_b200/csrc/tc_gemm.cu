@@ -306,50 +306,24 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant_
 }
 
 // ---------------------------------------------------------------------------------------------- host
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
 // 2-D bf16 row-major [rows, cols] with pitch ld (elements); box {64, box_rows}, 128B swizzle, zero OOB fill
 static int make_map_2d(CUtensorMap* m, const void* base, long long rows, long long cols, long long ld, int box_rows) {
-  EncodeTiledFn enc = encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return COTB200_EINVAL; }
   if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ld * 2) & 15)) { set_error("TMA operand not 16-byte aligned (ld=%lld)", ld); return COTB200_EALIGN; }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
   cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)box_rows};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = tma_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(2d) failed: %d", (int)r); return COTB200_EINVAL; }
   return 0;
 }
 
 // 4-D NHWC bf16 activation [B,H,W,C] (pixel pitch ldc); box {64, W, hbox, bbox}
 static int make_map_nhwc(CUtensorMap* m, const void* base, int B, int H, int W, int C, long long ldc, int hbox, int bbox) {
-  EncodeTiledFn enc = encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return COTB200_EINVAL; }
   if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ldc * 2) & 15)) { set_error("TMA operand not 16-byte aligned"); return COTB200_EALIGN; }
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
   cuuint64_t strides[3] = {(cuuint64_t)ldc * 2, (cuuint64_t)ldc * 2 * W, (cuuint64_t)ldc * 2 * W * H};
   cuuint32_t box[4] = {(cuuint32_t)TC_BK, (cuuint32_t)W, (cuuint32_t)hbox, (cuuint32_t)bbox};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = tma_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(4d) failed: %d", (int)r); return COTB200_EINVAL; }
   return 0;
 }
@@ -625,16 +599,12 @@ static int conv3x3_halo_launch(int B, int H, int W, int C, const void* X, long l
   p.relu = relu;
   p.scale = scale; p.shift = shift; p.col_sum = col_sum; p.col_sqsum = col_sqsum;
   CUtensorMap mx, mw, md;
-  EncodeTiledFn enc = encode_fn();
-  if (!enc) return 0;
   {
     if ((reinterpret_cast<uintptr_t>(X) & 15) || (reinterpret_cast<uintptr_t>(D) & 15)) return 0;
     cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2 * W, (cuuint64_t)C * 2 * W * H};
     cuuint32_t box[4] = {64, (cuuint32_t)Wpad, (cuuint32_t)(R + 2), 1};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    if (enc(&mx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(X), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) return 0;
+    if (tma_encode(&mx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, X, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B) != CUDA_SUCCESS) return 0;
   }
   if (make_map_2d(&mw, Wp, C, 9LL * 64, 9LL * 64, 64)) return 0;
   if (make_map_2d(&md, D, (long long)B * H * W, C, ldd, R * W)) return 0;
@@ -759,16 +729,11 @@ stem_s2d_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__
 // s2d image [B, Hh, Wh+4, 16] seen as the matrix of overlapping 4-cell windows: {64 elements (window), Wh+1 window starts (32 B
 // apart), Hh rows, B}; box {64, tw, 1, 1}.  Rows outside [0, Hh) are zero-filled by the TMA = the vertical padding.
 static int make_map_stem(CUtensorMap* m, const void* base, int B, int Hh, int Wh, int tw) {
-  EncodeTiledFn enc = encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return COTB200_EINVAL; }
   const long long Wp = Wh + 4;
   cuuint64_t dims[4] = {64, (cuuint64_t)(Wh + 1), (cuuint64_t)Hh, (cuuint64_t)B};
   cuuint64_t strides[3] = {32, (cuuint64_t)Wp * 32, (cuuint64_t)Wp * 32 * Hh};
   cuuint32_t box[4] = {64, (cuuint32_t)tw, 1, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = tma_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(stem windows) failed: %d", (int)r); return COTB200_EUNSUPPORTED; }
   return 0;
 }
@@ -805,8 +770,7 @@ extern "C" int cotb200_stem7x7s2_bf16(int B, int H, int W, const void* X, const 
   if ((rc = make_map_2d(&b1, Wm, N, 256, 256, p.bn))) return rc;
   {
     const long long cells = (long long)B * Hh * (Wh + 4);
-    long long g = (cells + 255) / 256;
-    const int grid = (int)(g < (long long)num_sms() * 16 ? g : (long long)num_sms() * 16);
+    const int grid = grid_stride_blocks(cells, 256, 16);
     COTB200_PROF_B("stem_s2d", (double)B * H * W * 3 * 2 + (double)cells * 32);
     stem_s2d_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)X, (__nv_bfloat16*)scratch, B, H, W);
     if ((rc = check_launch("stem_s2d"))) return rc;

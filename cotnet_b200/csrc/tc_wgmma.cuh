@@ -1,5 +1,4 @@
-// wgmma (Hopper warpgroup MMA) PTX wrappers and the tensor-map helper shared by the tensor-core kernels (tc_gemm.cu, tc_wgrad.cu),
-// sm_90a.
+// wgmma (Hopper warpgroup MMA) PTX wrappers shared by the tensor-core kernels (tc_gemm.cu, tc_wgrad.cu), sm_90a.
 //
 // Every tensor-core kernel uses one instruction shape, m64n64k16 bf16 x bf16 -> fp32, with both operands read from shared memory
 // through matrix descriptors.  A warpgroup owns a 64-row slice of the tile and keeps its accumulators in registers: 32 floats per
@@ -54,21 +53,6 @@ __device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, 
         "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB)
       : "memory");
-}
-
-typedef CUresult (*TcEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-inline TcEncodeTiledFn tc_encode_fn() {
-  static TcEncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = (TcEncodeTiledFn)p;
-  }
-  return fn;
 }
 
 }  // namespace cotb200

@@ -189,7 +189,7 @@ static int wgrad_launch(const CUtensorMap& ma, const CUtensorMap& mb1, const CUt
     if ((rc = check_launch(what))) return rc;
   }
   const long long n = (long long)p.R * p.Cc;
-  const int rgrid = (int)((n + 255) / 256 < 4LL * num_sms() ? (n + 255) / 256 : 4LL * num_sms());
+  const int rgrid = grid_stride_blocks(n, 256, 4);
   COTB200_PROF_B("wgrad_reduce", 4.0 * (double)n * (p.splits + 2));
   wgrad_reduce_kernel<<<rgrid, 256, 0, st>>>(p.part, p.splits, p.R, p.Cc, p.out, p.ldo, p.transpose);
   return check_launch("wgrad_reduce");
@@ -197,15 +197,11 @@ static int wgrad_launch(const CUtensorMap& ma, const CUtensorMap& mb1, const CUt
 
 // bf16 pixel matrix [rows = pixels, cols = channels] with pitch ld: box {64 channels, 64 pixels}, 128B swizzle, zero OOB fill
 static int wg_make_map(CUtensorMap* m, const void* base, long long pixels, long long channels, long long ld) {
-  TcEncodeTiledFn enc = tc_encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return COTB200_EINVAL; }
   if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ld * 2) & 15)) { set_error("wgrad: TMA operand not 16-byte aligned (ld=%lld)", ld); return COTB200_EALIGN; }
   cuuint64_t dims[2] = {(cuuint64_t)channels, (cuuint64_t)pixels};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
   cuuint32_t box[2] = {64, (cuuint32_t)WG_PX};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = tma_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(wgrad) failed: %d", (int)r); return COTB200_EINVAL; }
   return 0;
 }
@@ -283,16 +279,12 @@ extern "C" int cotb200_stem7x7s2_wgrad_bf16(int B, int H, int W, const void* dY,
   if (p.stages > WG_STAGES) p.stages = WG_STAGES;
   if (p.stages < 2) { set_error("stem7x7s2_wgrad: row of %d pixels does not fit two pipeline stages", Wh); return COTB200_EUNSUPPORTED; }
   CUtensorMap ma, mb;
-  TcEncodeTiledFn enc = tc_encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return COTB200_EINVAL; }
   {
     if ((reinterpret_cast<uintptr_t>(dY) & 15) || ((ldy * 2) & 15)) { set_error("stem7x7s2_wgrad: dY not 16-byte aligned"); return COTB200_EALIGN; }
     cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)p.M};
     cuuint64_t strides[1] = {(cuuint64_t)ldy * 2};
     cuuint32_t box[2] = {64, (cuuint32_t)p.px};
-    cuuint32_t es[2] = {1, 1};
-    if (enc(&ma, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(dY), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
+    if (tma_encode(&ma, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dY, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B) != CUDA_SUCCESS) {
       set_error("cuTensorMapEncodeTiled(stem wgrad dY) failed"); return COTB200_EINVAL;
     }
   }
@@ -301,9 +293,7 @@ extern "C" int cotb200_stem7x7s2_wgrad_bf16(int B, int H, int W, const void* dY,
     cuuint64_t dims[4] = {64, (cuuint64_t)(Wh + 1), (cuuint64_t)Hh, (cuuint64_t)B};
     cuuint64_t strides[3] = {32, (cuuint64_t)Wp * 32, (cuuint64_t)Wp * 32 * Hh};
     cuuint32_t box[4] = {64, (cuuint32_t)p.px, 1, 1};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    if (enc(&mb, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(scratch), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
+    if (tma_encode(&mb, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, scratch, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B) != CUDA_SUCCESS) {
       set_error("cuTensorMapEncodeTiled(stem wgrad windows) failed"); return COTB200_EUNSUPPORTED;
     }
   }

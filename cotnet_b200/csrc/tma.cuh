@@ -1,10 +1,45 @@
-// PTX wrappers shared by the TMA / mbarrier pipelines (agg_tma.cu, agg_nchw_tma.cu, gn72.cu, tc_gemm.cu), sm_90a.
+// PTX wrappers shared by the TMA / mbarrier pipelines (agg_tma.cu, agg_nchw_tma.cu, gn72.cu, tc_gemm.cu, tc_wgrad.cu), sm_90a,
+// and the host-side tensor-map encoder of those that use tensor maps.
 // Every wait is a BOUNDED try_wait spin that __trap()s: a broken pipeline aborts the launch instead of hanging the GPU.
 #pragma once
 #include <cuda.h>
+#include <cuda_runtime.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cstdint>
 
 namespace cotb200 {
+
+// ---------------------------------------------------------------- host: tensor maps
+template <typename T> CUtensorMapDataType tma_dtype();
+template <> inline CUtensorMapDataType tma_dtype<float>() { return CU_TENSOR_MAP_DATA_TYPE_FLOAT32; }
+template <> inline CUtensorMapDataType tma_dtype<__nv_bfloat16>() { return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16; }
+template <> inline CUtensorMapDataType tma_dtype<__half>() { return CU_TENSOR_MAP_DATA_TYPE_FLOAT16; }
+
+// cuTensorMapEncodeTiled with what every map of the library shares: unit element strides, no interleave, 128-byte L2
+// promotion, zero fill out of bounds.  dims[rank] (dims[0] innermost, unit stride), strides[rank - 1] in BYTES of dims[1..],
+// box[rank].  The driver entry point is looked up through the runtime (the library links no libcuda) once per process;
+// CUDA_ERROR_NOT_FOUND when the driver does not have it.
+inline CUresult tma_encode(CUtensorMap* m, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,
+                           const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
+  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static const EncodeFn enc = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+                    q == cudaDriverEntryPointSuccess;
+    return ok ? (EncodeFn)p : nullptr;
+  }();
+  if (!enc) return CUDA_ERROR_NOT_FOUND;
+  if (rank < 1 || rank > 5) return CUDA_ERROR_INVALID_VALUE;
+  const cuuint32_t es[5] = {1, 1, 1, 1, 1};
+  return enc(m, dtype, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+// ---------------------------------------------------------------- device: mbarriers and bulk copies
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

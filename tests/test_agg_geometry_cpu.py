@@ -118,7 +118,7 @@ class Pred:
 
     def add(self, name, *tags, loop=None):
         t = set(tags)
-        if loop is not None:                     # grid-stride kernel: (total threads, CTAs per SM of grid_for's cap)
+        if loop is not None:                     # grid-stride kernel: (total threads, CTAs per SM of grid_stride_blocks' cap)
             total, per_sm = loop
             for sms in SMS_H100:
                 grid = min(max(1, _cdiv(total, 256)), sms * per_sm)
@@ -596,7 +596,7 @@ CASES = [
                                                         "agg_bwd_nchw_dw/K5"}),
     case("nchw-k5-bf16", "bf16", D(2, 16, 12, 12, 8, k=5), {"agg_fwd_nchw_k5", "agg_bwd_nchw_dxdw/K5"}),
     case("limit-nchw2", "bf16", D(4097, 16, 4, 4, 16), {"nchw2-declined/N*wc", "agg_fwd_nchw_k3", "agg_bwd_nchw_dxdw/K3"}),
-    # ---- grid-stride loops past grid_for's cap on both SM counts
+    # ---- grid-stride loops past grid_stride_blocks' cap on both SM counts
     case("loop-nchw-k5", "fp32", D(4, 32, 72, 72, 16, k=5),
          {"agg_fwd_nchw_k5/loop2@132", "agg_fwd_nchw_k5/loop2@114", "agg_bwd_nchw_dxdw/loop2@132"}),
     case("loop-nhwc-v4", "bf16", D(8, 48, 56, 56, 12, layout=NHWC),
@@ -737,8 +737,6 @@ ANCHORS = {
         "if (bytes < 4 && vec != 1) continue;",
         "if (g.wcf % vec) continue;",
         "if (!oks(g.x_sw) || !oks(g.x_sn) || !oks(g.w_sw) || !oks(g.w_sn) || !oks(g.y_sw) || !oks(g.y_sn)) continue;",
-        "long long need = (total + block - 1) / block;",
-        "long long cap = (long long)num_sms() * per_sm;",
         "if (agg_tma_fwd<T>(nhwc2_args(g), x, w, y, st, &rc2)) return rc2;",
         "if (nhwc2_fwd<T>(nhwc2_args(g), x, w, y, st, &rc2)) return rc2;",
         "if (g.layout == COTB200_NCHW && nofold(g) && fits32(g) && is_same3(g, 3) && g.w_sn == (long long)g.wc * 9 * g.H * g.W) {",
@@ -747,7 +745,6 @@ ANCHORS = {
         "if (g.layout == COTB200_NCHW && nofold(g) && fits32(g) && (is_same3(g, 3) || is_same3(g, 5))) {",
         "const int vec = nhwc_vec<T>(g, x, w, y);",
         "const int total = g.N * g.H * g.W * (g.C / vec);",
-        "agg_fwd_generic<T><<<grid_for(total, 256, 16), 256, 0, st>>>(x, w, y, g, total);",
         "if (g.layout == COTB200_NCHW && nofold(g) && fits32(g) && is_same3(g, 3) && !acc_dx && g.w_sn == (long long)g.wc * 9 * g.H * g.W) {",
         "if (g.H * g.W <= 256 && nchw_plane_launch<T>(dx && dw ? 3 : (dx ? 1 : 2), g.N, g.C, g.H, g.W, g.wc, g.x_sn, g.y_sn, g.w_sn, dy, x, w,",
         "if (dx && nchw_tma_launch<T>(1, g.N, g.C, g.H, g.W, g.wc, g.y_sn, 0, g.x_sn, dy, w, dx, st, &rc2)) { if (rc2) return rc2; done_dx = 1; }",
@@ -763,12 +760,10 @@ ANCHORS = {
         "if (vec && okp(dx) && okp(dw)) {",
         "const int total = g.N * g.H * g.W * (g.wc / V);",
         "const long long total = (long long)g.N * g.heads * g.wc * g.K2 * g.HO * g.WO;",
-        "agg_dw_generic<T><<<grid_for(total, 256, 16), 256, 0, st>>>(dy, x, dw, g, total);",
         "g1.y_sn *= 2; g2.y_sn *= 2;",
         "if (is_same3(g1, 3) && is_same3(g2, 5) && fits32(g2) && 2 * half * g1.N < (1LL << 31)) {",
         "if (sizeof(T) >= 4 && is_same3(g1, 3) && is_same3(g2, 5) && fits32(g2)) {",
         "return bwd_impl<T>(g2, (const T*)dy + half, (const T*)x, (const T*)w2, (T*)dx, (T*)dw2, dx != nullptr, st);",
-        "agg_dx_generic2<T><<<grid_for(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)w1, g1, (const T*)dy + half,",
         "rc = bwd_impl<T>(g1, (const T*)dy, (const T*)x, (const T*)w1, (T*)nullptr, (T*)dw1, false, st);",
     ],
     "agg_nhwc2.cu": [
@@ -824,13 +819,42 @@ ANCHORS = {
 }
 
 
+# Pred.add's loop=(total, per_sm): grid_stride_blocks (common.cuh) and the (threads, per_sm) each grid-stride launch passes it
+GRID_ANCHORS = {
+    "common.cuh": [
+        "inline int grid_stride_blocks(long long items, int threads, int per_sm) {",
+        "const long long need = (items + threads - 1) / threads;",
+        "const long long cap = (long long)num_sms() * per_sm;",
+        "return (int)(need < 1 ? 1 : need < cap ? need : cap);",
+    ],
+    "agg_zeropad.cu": [
+        "const int grid = grid_stride_blocks(total, 256, 8);",
+        "agg_fwd_generic<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>(x, w, y, g, total);",
+        "agg_dw_generic<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>(dy, x, dw, g, total);",
+        "agg_dx_generic2<T><<<grid_stride_blocks(total, 256, 16), 256, 0, st>>>((const T*)dy, (const T*)w1, g1, (const T*)dy + half,",
+        "agg_mix_fwd_nchw_fast<T><<<grid_stride_blocks(total, 256, 8), 256, 0, st>>>(",
+    ],
+}
+
+
+def _missing_anchors(fname, anchors):
+    squash = lambda s: re.sub(r"\s+", " ", s)
+    src = squash(_src(fname))
+    return [a for a in anchors if squash(a) not in src]
+
+
 @pytest.mark.parametrize("fname", sorted(ANCHORS))
 def test_dispatch_anchors(fname):
     """the conditions the mirror copies are still the ones in the sources (whitespace-insensitive)"""
-    squash = lambda s: re.sub(r"\s+", " ", s)
-    src = squash(_src(fname))
-    missing = [a for a in ANCHORS[fname] if squash(a) not in src]
+    missing = _missing_anchors(fname, ANCHORS[fname])
     assert not missing, "%s no longer contains (update the mirror in this file): %s" % (fname, missing)
+
+
+def test_grid_stride_anchors():
+    """the grid-stride sizing the mirror copies (whitespace-insensitive)"""
+    for fname, anchors in sorted(GRID_ANCHORS.items()):
+        missing = _missing_anchors(fname, anchors)
+        assert not missing, "%s no longer contains (update the mirror in this file): %s" % (fname, missing)
 
 
 def test_every_launch_name_is_profiled():

@@ -331,10 +331,17 @@ def test_mirror_matches_the_sources():
         assert snippet in g, snippet
     r = _src("sum_rows.cu")
     for snippet in ("int vec = 16 / (int)sizeof(T);", "if (((uintptr_t)s.p[k] & m) || (s.ld[k] % v)) return false;",
-                    "return !((uintptr_t)out & m) && !(ldo % v);", "long long blocks = (total + 255) / 256;",
-                    "const long long cap = (long long)num_sms() * 16;",
-                    "item < total; item += (long long)gridDim.x * 256"):
+                    "return !((uintptr_t)out & m) && !(ldo % v);", "item < total; item += (long long)gridDim.x * 256"):
         assert snippet in r, snippet
+
+
+def test_sum_rows_grid_matches_the_sources():
+    """sum_rows_grid's capped grid: the (threads, per_sm) of the sum_rows launch and grid_stride_blocks in common.cuh."""
+    assert "const int blocks = grid_stride_blocks(total, 256, 16);" in _src("sum_rows.cu")
+    c = _src("common.cuh")
+    for snippet in ("const long long need = (items + threads - 1) / threads;", "const long long cap = (long long)num_sms() * per_sm;",
+                    "return (int)(need < 1 ? 1 : need < cap ? need : cap);"):
+        assert snippet in c, snippet
 
 
 def test_mirror_known_geometry():
