@@ -180,6 +180,13 @@ SOURCE_ANCHORS = {
         "rcode = 3 if mask is not None else (2 if res is None else 1)",
         "rcode = 0 if not relu else (2 if (batch and BN_MASK) else 1)",
         "return 8 if (wc // fold) % 8 == 0 else 0",
+        # the eval dispatch (eval_* generators below)
+        "if (not torch.is_grad_enabled() and not bn.training and not se[1].training and k is not None and se[1].running_mean is not None",
+        "and bn.running_mean is not None and isinstance(se[2], torch.nn.ReLU)):",
+        "if not (torch.is_grad_enabled() and x.requires_grad):\n        return (x,) * n",
+        "if res is None and ds is None:",
+        "and (torch.is_grad_enabled() or not bn.training)):",
+        "if _tc.stem7x7s2_bf16(xd, wm, scale=scale, shift=shift, relu=relu, out=out) is None:",
     ],
     "cotnet_b200/cot_layer.py": [
         "big = B * H * W >= fused.TC_MIN_PIXELS",
@@ -189,6 +196,11 @@ SOURCE_ANCHORS = {
         "k = fused.bn_act(F.conv2d(xk, wkey, None, 1, self.kernel_size // 2).contiguous(memory_format=cl), self.key_embed[1], relu=True)",
         "v = fused.bn_act(F.conv2d(xv, _dense_from_grouped(cv[0].weight, G)).contiguous(memory_format=cl), cv[1], relu=False)",
         "gc = fused.tap_chunk(C // 8, self.dw_group)",
+        "return (not self.training and not torch.is_grad_enabled() and x.dtype == torch.bfloat16 and self.kernel_size == 3",
+        "and self.dim % 64 == 0 and tc.conv_tile(self.dim, 4) is not None and x.shape[3] <= 128)",
+        "if self._tc_eval_ok(x):\n                return self._forward_tc_eval(x)\n            return self._forward_fused(x)",
+        "if ks == 3 and fused.supported(x):\n            return self._forward_fused(x)",
+        "w = fused.group_norm9(l.view(B, H, W, J).permute(0, 3, 1, 2), self.embed[4], gc)",
     ],
     "cotnet_b200/backbone.py": [
         "y = dropblock.drop_block(y, key, self.drop_block_sites[0], self.drop_block)",
@@ -336,10 +348,13 @@ class Recorder:
     """Swaps every fused autograd function for a subclass that calls the parent and records it; wraps _bn_apply_batch and _bn_bwd
     to capture `pre` / `dpre` and the BatchNorm statistics of the wgmma functions.  Changes no bit and no launch."""
 
-    def __init__(self, monkeypatch):
+    def __init__(self, monkeypatch, keep_outputs=False):
         from cotnet_b200 import dropblock, fused, trainer
         self.calls = []
         self._stack = []
+        # keep_outputs: hold every recorded output, so that no later tensor reuses its storage (under no_grad nothing else holds
+        # them, and the dataflow checks match producers by storage)
+        self.kept = [] if keep_outputs else None
         for mod, names in ((fused, FUSED_FNS), (dropblock, DROPBLOCK_FNS), (trainer, TRAINER_FNS)):
             for n in names:
                 monkeypatch.setattr(mod, n, self._subclass(getattr(mod, n)))
@@ -388,6 +403,8 @@ class Recorder:
                     rec._stack.pop()
                 call.out = _snap(out)
                 call.out_ptr = tuple(o.data_ptr() for o in (out if isinstance(out, tuple) else (out,)))
+                if rec.kept is not None:
+                    rec.kept.append(out)
                 call.saved = _snap(tuple(getattr(ctx, "to_save", ()) or ()))
                 if cls.__name__ == "CotTailFn":
                     call.extra["p"] = _snap(ctx.graph[0])
@@ -1006,19 +1023,29 @@ STEP_BLOCK_CASES = {
 }
 
 
-def model_blocks(model, H0):
-    """[(name, block index in its stage, cin, width, cout, H in, stride)] of every bottleneck of cotnet50 / cotnext50_2x48d /
-    se_cotnetd_50 for an H0 x H0 image: cotnet's 7x7/s2 stem and max pool (H0/4), stride 2 from stage 2 on; the deep stem's
-    stride 2 (H0/2), stride 2 in every stage (backbone.CoTResNet, backbone_hybrid.CoTHybridNet)"""
+def conv_out(H, stride):
+    """output size of every stride-2 stage of the trunks (7x7/s2 pad 3, 3x3/s2 pad 1 convolutions and pools, the avg_down 2x2/s2
+    ceil-mode pool): (H - 1) // 2 + 1, which is H // 2 only for even H"""
+    return H if stride == 1 else (H - 1) // 2 + 1
+
+
+def model_blocks(model, H0, W0=None):
+    """[(name, block index in its stage, cin, width, cout, H in, W in, stride)] of every bottleneck of cotnet50 / cotnext50_2x48d /
+    se_cotnetd_50 for an H0 x W0 image: cotnet's 7x7/s2 stem and max pool, stride 2 from stage 2 on; the deep stem's stride 2,
+    stride 2 in every stage (backbone.CoTResNet, backbone_hybrid.CoTHybridNet)"""
+    W0 = H0 if W0 is None else W0
     hybrid = model == "se_cotnetd_50"
-    H, cin = (H0 // 2, 64) if hybrid else (H0 // 4, 64)
+    H, W = conv_out(H0, 2), conv_out(W0, 2)
+    if not hybrid:
+        H, W = conv_out(H, 2), conv_out(W, 2)
+    cin = 64
     out = []
     for si, (planes, n) in enumerate(zip((64, 128, 256, 512), (3, 4, 6, 3))):
         width = planes * 48 // 64 * 2 if model == "cotnext50_2x48d" else planes
         for b in range(n):
             stride = 2 if b == 0 and (hybrid or si > 0) else 1
-            out.append(("layer%d.%d" % (si + 1, b), b, cin, width, planes * 4, H, stride))
-            cin, H = planes * 4, H // stride
+            out.append(("layer%d.%d" % (si + 1, b), b, cin, width, planes * 4, H, W, stride))
+            cin, H, W = planes * 4, conv_out(H, stride), conv_out(W, stride)
     return out
 
 
@@ -1026,7 +1053,7 @@ def model_calls(model, B, H0, min_pixels=TC_MIN_PIXELS):
     """the recorded calls of one TrainStep forward with drop path (every block but the first) and DropBlock (stages 3-4) on, as
     [stem calls, [calls of each block], loss calls]"""
     blocks = []
-    for i, (name, b, cin, width, cout, H, stride) in enumerate(model_blocks(model, H0)):
+    for i, (name, b, cin, width, cout, H, W, stride) in enumerate(model_blocks(model, H0)):
         db = name.startswith(("layer3", "layer4"))
         if model == "se_cotnetd_50":
             blocks.append(hybrid_block_calls(B, b, cin, width, H, stride, min_pixels, db, i > 0))
@@ -1039,10 +1066,198 @@ def model_sites(model):
     """the DropBlock site numbers of every block, counted here in forward order: stages 3-4 only; bn1 and bn3, and conv2.bn0
     between them in a split-attention block"""
     out, site = {}, 0
-    for name, b, cin, width, cout, H, stride in model_blocks(model, 224):
+    for name, b, cin, width, cout, H, W, stride in model_blocks(model, 224):
         if not name.startswith(("layer3", "layer4")):
             continue
         n = 3 if model == "se_cotnetd_50" and hybrid_split(width, b) else 2
         out[name] = tuple(range(site, site + n))
         site += n
     return out
+
+
+# ------------------------------------------------------------------------------------------------ the eval dispatch
+#: An eval forward runs as EvalStep._body runs it: model.eval(), no_grad, bf16 autocast (cache_enabled=False), step arena off, on a
+#: bf16 channels_last image.  Besides the autograd functions above, the eval recorder of tests/test_eval_stages_gpu.py lists the
+#: top-level wgmma calls of CotLayer._forward_tc_eval (conv3x3_bf16, gemm_bf16) and its tail (cot_tail_eval); the GEMMs that
+#: TcConv1x1Fn makes inside itself are part of that call.  What differs from training:
+#:   * a CotLayer takes _forward_tc_eval whenever _tc_eval_ok (dim, and W <= 128), whatever the pixel count; above W = 128 it
+#:     takes _forward_fused under no_grad: no FanOutFn (fan_out falls through), cuDNN convolutions, and the eval tail;
+#:   * cot_tail takes _cot_tail_eval (running statistics, cotb200_se_eval); the split-attention gate stays CotTailFn;
+#:   * conv1x1_bn takes TcConv1x1Fn in eval at the same geometry rule as in training (weights of any dtype are cast to bf16);
+#:   * CoXt's embed.0 is on the wgmma GEMM only with bf16 weights: fp32 weights under autocast go to cuDNN + BNActFn.
+EVAL_LAYER_TC = ["conv3x3_bf16", "gemm_bf16", "gemm_bf16", "gemm_bf16"]
+
+
+def eval_cot_calls(B, dim, H, W, bf16_weights, min_pixels=TC_MIN_PIXELS):
+    """the recorded calls of a CotLayer's eval forward on a bf16 channels_last [B, dim, H, W] input; only W and dim decide between
+    _forward_tc_eval and _forward_fused, the rest matter inside _forward_fused"""
+    gc = tap_chunk(dim // 8)
+    if tc_supported(dim, W):                         # CotLayer._tc_eval_ok: the same dim conditions and W <= 128
+        return EVAL_LAYER_TC + ["GroupNorm9Fn(gc%d)" % gc, "AggTapFn(fold1,gc%d)" % gc, "cot_tail_eval"]
+    key_tc, e0_tc, rest_tc = cot_dispatch(B, dim, H, W, min_pixels)
+    out = ["TcConv3x3Fn" if key_tc and bf16_weights else "BNActFn(relu)", "TcConv1x1Fn(two,relu)" if e0_tc else "BNActFn(relu)"]
+    out += ["TcConv1x1Fn(one,nobn)", "TcConv1x1Fn(one,bn)"] if rest_tc else ["BNActFn(plain)"]
+    return out + ["GroupNorm9Fn(gc%d+lbias)" % gc, "AggTapFn(fold1,gc%d)" % gc, "cot_tail_eval"]
+
+
+def eval_coxt_calls(dim, bf16_weights):
+    """CoXtLayer's eval forward: _forward_fused under no_grad; embed.0 on the wgmma GEMM only when its dense weight is bf16"""
+    gc = tap_chunk(dim // 8, 2)
+    e0 = "TcConv1x1Fn(two,relu)" if bf16_weights and dim % 16 == 0 else "BNActFn(relu)"
+    return ["BNActFn(relu)", e0, "BNActFn(plain)", "GroupNorm9Fn(gc%d+lbias)" % gc, "AggTapFn(fold2,gc%d)" % gc, "cot_tail_eval"]
+
+
+def _eval_1x1(cin, cout, M, stride, min_pixels, label):
+    return "TcConv1x1Fn(one,%s)" % label if conv1x1_tc(cin, cout, M, stride, min_pixels) else "BNActFn(%s)" % label.replace("bn", "plain")
+
+
+def eval_bottleneck_calls(B, cin, width, cout, H, W, stride, bf16_weights, min_pixels=TC_MIN_PIXELS, coxt=False):
+    """backbone.Bottleneck._forward_fused in eval: conv1 + bn1 + ReLU, the avd pool at stride 2, conv2, the downsample, conv3 + bn3 +
+    residual + ReLU"""
+    Ho, Wo = conv_out(H, stride), conv_out(W, stride)
+    out = [_eval_1x1(cin, width, B * H * W, 1, min_pixels, "relu")]
+    if stride > 1:
+        out.append("Pool3x3S2Fn(avg)")
+    out += eval_coxt_calls(width, bf16_weights) if coxt else eval_cot_calls(B, width, Ho, Wo, bf16_weights, min_pixels)
+    if stride > 1 or cin != cout:
+        out.append(_eval_1x1(cin, cout, B * Ho * Wo, stride, min_pixels, "bn"))
+    return out + [_eval_1x1(width, cout, B * Ho * Wo, 1, min_pixels, "relu+res")]
+
+
+def eval_hybrid_block_calls(B, block_idx, cin, width, H, W, stride, bf16_weights, min_pixels=TC_MIN_PIXELS, avd=False,
+                            avd_first=True):
+    """backbone_hybrid.CoTBottleneck.forward in eval: a split-attention conv2 is the cuDNN 3x3 (stride 2 itself unless avd) and the
+    gate on CotTailFn with running statistics; a CoT conv2 pools first at stride 2; the avg_down downsample pools in torch"""
+    cout = 4 * width
+    Ho, Wo = conv_out(H, stride), conv_out(W, stride)
+    split = hybrid_split(width, block_idx)
+    pool = stride > 1 and (avd if split else True)
+    out = [_eval_1x1(cin, width, B * H * W, 1, min_pixels, "relu")]
+    if pool and avd_first:
+        out.append("Pool3x3S2Fn(avg)")
+    if split:
+        out.append("CotTailFn(gate)")
+    else:
+        out += eval_cot_calls(B, width, Ho if avd_first else H, Wo if avd_first else W, bf16_weights, min_pixels)
+    if pool and not avd_first:
+        out.append("Pool3x3S2Fn(avg)")
+    if block_idx == 0:
+        out.append(_eval_1x1(cin, cout, B * Ho * Wo, 1, min_pixels, "bn"))
+    return out + [_eval_1x1(width, cout, B * Ho * Wo, 1, min_pixels, "relu+res")]
+
+
+def eval_stem_calls(model, H, W):
+    """the stems in eval: as in training (the wgmma stem folds the running statistics into its epilogue)"""
+    return stem_calls(model, H, W)
+
+
+def eval_model_calls(model, B, H0, W0, bf16_weights, min_pixels=TC_MIN_PIXELS):
+    """the recorded calls of one eval forward of the whole network: (stem calls, [calls of each block]); the global pool and fc
+    are torch ops"""
+    blocks = []
+    for name, b, cin, width, cout, H, W, stride in model_blocks(model, H0, W0):
+        if model == "se_cotnetd_50":
+            blocks.append(eval_hybrid_block_calls(B, b, cin, width, H, W, stride, bf16_weights, min_pixels))
+        else:
+            blocks.append(eval_bottleneck_calls(B, cin, width, cout, H, W, stride, bf16_weights, min_pixels,
+                                                model != "cotnet50"))
+    return eval_stem_calls(model, H0, W0), blocks
+
+
+def eval_case_calls(c):
+    """the call list of an EVAL_BLOCK_CASES entry, from the generators"""
+    mp = TC_MIN_PIXELS if c.get("min_pixels") is None else c["min_pixels"]
+    if c["kind"] == "stem":
+        return eval_stem_calls(c["model"], c["H"], c["W"])
+    if c["model"] == "se_cotnetd_50":
+        return eval_hybrid_block_calls(c["B"], int(c["block"].split(".")[1]), c["cin"], c["width"], c["H"], c["W"], c["stride"],
+                                       c["bf16"], mp)
+    return eval_bottleneck_calls(c["B"], c["cin"], c["width"], c["cout"], c["H"], c["W"], c["stride"], c["bf16"], mp,
+                                 c["model"] != "cotnet50")
+
+
+#: Eval blocks and stems.  calls: as the eval recorder labels them (BNActFn / TcConv1x1Fn / ... as in the training lists; the wgmma
+#: CoT layer as EVAL_LAYER_TC + GroupNorm9Fn + AggTapFn + cot_tail_eval, whose output 3 is the layer output).  flow: as
+#: STEP_BLOCK_CASES ("consumer.argument<-producer.output", "c<j>" the input of the j-th torch convolution), producers matched by
+#: storage and by value in NHWC row order (a gemm_bf16 output [B*H*W, N] is the next stage's [B, N, H, W] input).
+_EVAL_TC = EVAL_LAYER_TC + ["GroupNorm9Fn(gc8)", "AggTapFn(fold1,gc8)", "cot_tail_eval"]
+
+
+def _tc_layer_flow(i, x):
+    """the dataflow inside a wgmma CoT layer whose first call is number i and whose input is `x`"""
+    return ["%d.0<-%s" % (i, x), "%d.0<-%s" % (i + 1, x), "%d.2<-%d.0" % (i + 1, i), "%d.0<-%d.0" % (i + 2, i + 1),
+            "%d.0<-%s" % (i + 3, x), "%d.0<-%d.0" % (i + 4, i + 2), "%d.0<-%d.0" % (i + 5, i + 3), "%d.1<-%d.0" % (i + 5, i + 4),
+            "%d.0<-%d.0" % (i + 6, i + 5), "%d.1<-%d.0" % (i + 6, i)]
+
+
+EVAL_BLOCK_CASES = {
+    # the bench's stage-1 dispatch: B*H*W = 100352, conv1, downsample and conv3 on wgmma (conv3: raw GEMM + bn_apply with the residual)
+    "cot_stage1_b32": dict(model="cotnet50", kind="block", block="layer1.0", B=32, cin=64, width=64, cout=256, H=56, W=56, stride=1,
+                           bf16=True, calls=["TcConv1x1Fn(one,relu)"] + _EVAL_TC + ["TcConv1x1Fn(one,bn)", "TcConv1x1Fn(one,relu+res)"],
+                           flow=["0.0<-x"] + _tc_layer_flow(1, "0.0") + ["8.0<-x", "9.0<-7.3", "9.8<-8.0"]),
+    # 6272 pixels: the trunk 1x1 convolutions on cuDNN, the CoT layer on wgmma all the same
+    "cot_stage1_b2": dict(model="cotnet50", kind="block", block="layer1.0", B=2, cin=64, width=64, cout=256, H=56, W=56, stride=1,
+                          bf16=True, calls=["BNActFn(relu)"] + _EVAL_TC + ["BNActFn(plain)", "BNActFn(relu+res)"],
+                          flow=_tc_layer_flow(1, "0.0") + ["9.3<-8.0", "c0<-x", "c1<-x", "c2<-7.3"]),
+    # stride 2: the avd average pool in front of the CoT layer, the stride-2 downsample on cuDNN
+    "cot_stage2_first_b2": dict(model="cotnet50", kind="block", block="layer2.0", B=2, cin=256, width=128, cout=512, H=28, W=28,
+                                stride=2, bf16=True,
+                                calls=["BNActFn(relu)", "Pool3x3S2Fn(avg)"] + _EVAL_TC + ["BNActFn(plain)", "BNActFn(relu+res)"],
+                                flow=["1.0<-0.0"] + _tc_layer_flow(2, "1.0") + ["10.3<-9.0", "c0<-x", "c1<-x", "c2<-8.3"]),
+    # 7x7, dim 512: the conv-mode key convolution; the residual is the block input
+    "cot_stage4_b2": dict(model="cotnet50", kind="block", block="layer4.1", B=2, cin=2048, width=512, cout=2048, H=7, W=7, stride=1,
+                          bf16=True, calls=["BNActFn(relu)"] + _EVAL_TC + ["BNActFn(relu+res)"],
+                          flow=_tc_layer_flow(1, "0.0") + ["8.3<-x", "c0<-x", "c1<-7.3"]),
+    # W = 130 > 128: CotLayer._forward_fused under no_grad (no FanOutFn, cuDNN convolutions) and the eval tail
+    "cot_stage1_wide_b1": dict(model="cotnet50", kind="block", block="layer1.0", B=1, cin=64, width=64, cout=256, H=130, W=130,
+                               stride=1, bf16=True,
+                               calls=["BNActFn(relu)", "BNActFn(relu)", "BNActFn(relu)", "BNActFn(plain)", "GroupNorm9Fn(gc8+lbias)",
+                                      "AggTapFn(fold1,gc8)", "cot_tail_eval", "BNActFn(plain)", "BNActFn(relu+res)"],
+                               flow=["5.0<-3.0", "5.1<-4.0", "6.0<-5.0", "6.1<-1.0", "8.3<-7.0", "c0<-x", "c1<-0.0", "c3<-2.0",
+                                     "c4<-0.0", "c5<-x", "c6<-6.3"]),
+    # CoXt, embed.0 on the wgmma GEMM (bf16 weights) or on cuDNN (fp32 weights under autocast)
+    "coxt_stage1_b2_bf16w": dict(model="cotnext50_2x48d", kind="block", block="layer1.0", B=2, cin=64, width=96, cout=256, H=56, W=56,
+                                 stride=1, bf16=True,
+                                 calls=["BNActFn(relu)", "BNActFn(relu)", "TcConv1x1Fn(two,relu)", "BNActFn(plain)",
+                                        "GroupNorm9Fn(gc0+lbias)", "AggTapFn(fold2,gc0)", "cot_tail_eval", "BNActFn(plain)",
+                                        "BNActFn(relu+res)"],
+                                 flow=["2.0<-0.0", "2.1<-1.0", "5.0<-3.0", "5.1<-4.0", "6.0<-5.0", "6.1<-1.0", "8.3<-7.0", "c0<-x",
+                                       "c1<-0.0", "c2<-2.0", "c3<-0.0", "c4<-x", "c5<-6.3"]),
+    "coxt_stage1_b2_fp32w": dict(model="cotnext50_2x48d", kind="block", block="layer1.0", B=2, cin=64, width=96, cout=256, H=56, W=56,
+                                 stride=1, bf16=False,
+                                 calls=["BNActFn(relu)", "BNActFn(relu)", "BNActFn(relu)", "BNActFn(plain)", "GroupNorm9Fn(gc0+lbias)",
+                                        "AggTapFn(fold2,gc0)", "cot_tail_eval", "BNActFn(plain)", "BNActFn(relu+res)"],
+                                 flow=["5.0<-3.0", "5.1<-4.0", "6.0<-5.0", "6.1<-1.0", "8.3<-7.0", "c0<-x", "c1<-0.0", "c3<-2.0",
+                                       "c4<-0.0", "c5<-x", "c6<-6.3"]),
+    "coxt_stage4_b2": dict(model="cotnext50_2x48d", kind="block", block="layer4.1", B=2, cin=2048, width=768, cout=2048, H=7, W=7,
+                           stride=1, bf16=True,
+                           calls=["BNActFn(relu)", "BNActFn(relu)", "TcConv1x1Fn(two,relu)", "BNActFn(plain)", "GroupNorm9Fn(gc8+lbias)",
+                                  "AggTapFn(fold2,gc8)", "cot_tail_eval", "BNActFn(relu+res)"],
+                           flow=["2.0<-0.0", "2.1<-1.0", "5.0<-3.0", "5.1<-4.0", "6.0<-5.0", "6.1<-1.0", "7.3<-x", "c0<-x", "c1<-0.0",
+                                 "c2<-2.0", "c3<-0.0", "c4<-6.3"]),
+    # SE-CoTNetD: split attention with the stride-2 cuDNN 3x3 and avg_down; the CoT layer of layer3.0 (c4_idx); split attention at
+    # 14x14 and at a non-square 29x25 (the gate's H*W normaliser)
+    "hybrid_stage1_first_b2": dict(model="se_cotnetd_50", kind="block", block="layer1.0", B=2, cin=64, width=64, cout=256, H=56, W=56,
+                                   stride=2, bf16=True,
+                                   calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(plain)", "BNActFn(relu+res)"],
+                                   flow=["3.3<-2.0", "c0<-x", "c1<-0.0", "c3<-1.0"]),
+    "hybrid_stage3_cot_first_b2": dict(model="se_cotnetd_50", kind="block", block="layer3.0", B=2, cin=512, width=256, cout=1024, H=28,
+                                       W=28, stride=2, bf16=True,
+                                       calls=["BNActFn(relu)", "Pool3x3S2Fn(avg)"] + _EVAL_TC + ["BNActFn(plain)", "BNActFn(relu+res)"],
+                                       flow=["1.0<-0.0"] + _tc_layer_flow(2, "1.0") + ["10.3<-9.0", "c0<-x", "c2<-8.3"]),
+    "hybrid_stage3_split_b2": dict(model="se_cotnetd_50", kind="block", block="layer3.1", B=2, cin=1024, width=256, cout=1024, H=14,
+                                   W=14, stride=1, bf16=True, calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(relu+res)"],
+                                   flow=["2.3<-x", "c0<-x", "c1<-0.0", "c2<-1.0"]),
+    "hybrid_stage2_29x25_b2": dict(model="se_cotnetd_50", kind="block", block="layer2.1", B=2, cin=512, width=128, cout=512, H=29,
+                                   W=25, stride=1, bf16=True, calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(relu+res)"],
+                                   flow=["2.3<-x", "c0<-x", "c1<-0.0", "c2<-1.0"]),
+    # stems: the wgmma 7x7/s2 stem at even sizes, cuDNN at odd ones, the deep stem on cuDNN
+    "cotnet_stem_224": dict(model="cotnet50", kind="stem", B=2, H=224, W=224, bf16=True, calls=["StemConvBNFn", "Pool3x3S2Fn(max)"],
+                            flow=["0.0<-x", "1.0<-0.0"]),
+    "cotnet_stem_225": dict(model="cotnet50", kind="stem", B=2, H=225, W=225, bf16=True, calls=["BNActFn(relu)", "Pool3x3S2Fn(max)"],
+                            flow=["1.0<-0.0", "c0<-x"]),
+    "cotnet_stem_232x200": dict(model="cotnet50", kind="stem", B=2, H=232, W=200, bf16=False, calls=["StemConvBNFn", "Pool3x3S2Fn(max)"],
+                                flow=["0.0<-x", "1.0<-0.0"]),
+    "hybrid_deep_stem": dict(model="se_cotnetd_50", kind="stem", B=2, H=224, W=224, bf16=True, calls=["BNActFn(relu)"] * 3,
+                             flow=["c0<-x", "c1<-0.0", "c2<-1.0"]),
+}

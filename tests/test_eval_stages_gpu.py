@@ -104,14 +104,24 @@ def _rows2(t):
 
 class _EvalRecorder:
     """S.Recorder (GroupNorm9Fn, AggTapFn, ...) plus the wgmma calls of _forward_tc_eval (tc.gemm_bf16, tc.conv3x3_bf16) and the eval
-    tail's stages (fused._cot_tail_eval_stages), all into one ordered call list.  Snapshots only: no bit and no launch changes."""
+    tail's stages (fused._cot_tail_eval_stages), all into one ordered call list.  Only top-level wgmma calls are listed: the GEMM a
+    recorded function (TcConv1x1Fn) makes inside itself is part of that call.  The eval BatchNorm fold of the wgmma functions
+    (fused._bn_eval_fold) is captured into their call's extra["fold"].  Snapshots only: no bit and no launch changes."""
 
-    def __init__(self, monkeypatch):
-        self.rec = S.Recorder(monkeypatch)
-        calls = self.rec.calls
-        gemm0, conv0, tail0 = tc.gemm_bf16, tc.conv3x3_bf16, fused._cot_tail_eval_stages
+    def __init__(self, monkeypatch, keep_outputs=False):
+        self.rec = S.Recorder(monkeypatch, keep_outputs)
+        calls, stack, kept = self.rec.calls, self.rec._stack, self.rec.kept
+        gemm0, conv0, tail0, fold0 = tc.gemm_bf16, tc.conv3x3_bf16, fused._cot_tail_eval_stages, fused._bn_eval_fold
+
+        def done(c, o):
+            c.out = S._snap(o)
+            c.out_ptr = tuple(t.data_ptr() for t in (o if isinstance(o, tuple) else (o,)))
+            if kept is not None:
+                kept.append(o)
 
         def gemm_w(*a, **kw):
+            if stack:
+                return gemm0(*a, **kw)
             c = S.Call("gemm_bf16", (None,))
             calls.append(c)
             o = gemm0(*a, **kw)
@@ -120,26 +130,36 @@ class _EvalRecorder:
             assert args.get("stats") is None
             c.args = tuple(args.get(n) for n in names[:7])
             c.inp = tuple(S._snap(v) for v in c.args)
-            c.out = S._snap(o)
+            done(c, o)
             return o
 
         def conv_w(x, wp, bn, scale=None, shift=None, relu=False, stats=None, out=None):
+            if stack:
+                return conv0(x, wp, bn, scale=scale, shift=shift, relu=relu, stats=stats, out=out)
             assert stats is None
             c = S.Call("conv3x3_bf16", (x, wp, bn, scale, shift, relu))
             calls.append(c)
             o = conv0(x, wp, bn, scale=scale, shift=shift, relu=relu, out=out)
-            c.out = S._snap(o)
+            done(c, o)
             return o
 
         def tail_w(u, k, bn, se):
             c = S.Call("cot_tail_eval", (u, k))
+            c.extra.update(bn=bn, se=se)
             calls.append(c)
             r = tail0(u, k, bn, se)
-            c.out = S._snap(r)
+            done(c, r)
+            return r
+
+        def fold_w(bn, weight, bias):
+            r = fold0(bn, weight, bias)
+            if stack:
+                stack[-1].extra["fold"] = (bn,) + tuple(S._snap(t) for t in r)
             return r
         monkeypatch.setattr(tc, "gemm_bf16", gemm_w)
         monkeypatch.setattr(tc, "conv3x3_bf16", conv_w)
         monkeypatch.setattr(fused, "_cot_tail_eval_stages", tail_w)
+        monkeypatch.setattr(fused, "_bn_eval_fold", fold_w)
         self.calls = calls
 
 
@@ -207,12 +227,18 @@ def test_cot_layer_eval_stage_by_stage(dim, H, B, layout, monkeypatch):
     out = _fwd(m, x)
     assert _lib.launch_count() - lc == n_launch, "the recorder changed the launches"
     S.equal(out, plain, "recorded forward == plain forward")
-    calls = rec.calls
+    check_eval_layer(rec.calls, m, x, out, "CotLayer(%d) eval %dx%d B=%d %s" % (dim, H, H, B, layout))
+
+
+def check_eval_layer(calls, m, x, out, what):
+    """CotLayer m's recorded _forward_tc_eval calls on input x with output out: (a) the call list, (b) every producer -> consumer
+    edge bit for bit, (c) every stage within 1/2 bf16 ulp plus its fp32 chain bound of fp64 of its own inputs, (d) every BatchNorm
+    fold within its fold_bound of fp64 of the module's running statistics"""
     assert [c.name for c in calls] == EVAL_LAYER_CALLS, [c.name for c in calls]
+    B, dim, H, W = x.shape
     conv, e0, e3, v1, gn, agg, tail = calls
-    what = "CotLayer(%d) eval %dx%d B=%d %s" % (dim, H, H, B, layout)
     J = 9 * dim // 8
-    nhwc = lambda t, n: t.view(B, H, H, n).permute(0, 3, 1, 2)        # noqa: E731
+    nhwc = lambda t, n: t.view(B, H, W, n).permute(0, 3, 1, 2)        # noqa: E731
     # (b) dataflow
     for c, i in ((conv, 0), (e0, 0), (v1, 0)):
         S.equal(c.inp[i], x, what + " %s input = x" % c.name)
@@ -239,10 +265,6 @@ def test_cot_layer_eval_stage_by_stage(dim, H, B, layout, monkeypatch):
     _check_fold(conv.inp[3], conv.inp[4], m.key_embed[1], what + " key_embed.1")
     _check_fold(e0.inp[4], e0.inp[5], m.embed[1], what + " embed.1")
     _check_fold(v1.inp[4], v1.inp[5], m.conv1x1[1], what + " conv1x1.1")
-    ss, psum, a, tout = tail.out
-    _check_fold(ss[0], ss[1], m.bn, what + " bn (tail)")
-    fb = S.fold_bound(m.bn)
-    S.within(ss[3], fb["rstd"], fb["rstd_err"], what + " bn (tail) rstd")
     # (c) every stage against fp64 of its own inputs
     _check_conv(conv, m.key_embed[0].weight.detach(), what + " key conv")
     _check_gemm(e0, what + " embed.0", "eval_gemm")
@@ -250,11 +272,22 @@ def test_cot_layer_eval_stage_by_stage(dim, H, B, layout, monkeypatch):
     _check_gemm(v1, what + " conv1x1", "eval_gemm")
     check_gn9(gn, what + " GroupNorm9Fn")
     check_agg(agg, what + " AggTapFn")
+    check_tail_eval(tail, m.bn, m.se, what)
+
+
+def check_tail_eval(tail, bn, se, what):
+    """fused._cot_tail_eval_stages, recorded: the BatchNorm fold (bn_finalize of the running statistics), the pooled sums, the
+    attention weights of cotb200_se_eval at p = psum * fl(1 / (H * W)) and the recombination, each against fp64 of its own inputs"""
     u, k = tail.inp
+    H, W = u.shape[2], u.shape[3]
+    ss, psum, a, tout = tail.out
+    _check_fold(ss[0], ss[1], bn, what + " bn (tail)")
+    fb = S.fold_bound(bn)
+    S.within(ss[3], fb["rstd"], fb["rstd_err"], what + " bn (tail) rstd")
     ps, pe, y, ye = S.tail_pool_ref(u, k, ss[0], ss[1], S.SIGMOID_ERR_16)
     S.within(psum, ps, pe, what + " tail_pool psum")
-    p = psum.double() * torch.tensor(1.0 / (H * H), dtype=torch.float32).double()
-    ar, ea = S.mlp_ref(p, (m.se[0], m.se[1], m.se[3]), "cot", False, se_eval=True)
+    p = psum.double() * torch.tensor(1.0 / (H * W), dtype=torch.float32).double()
+    ar, ea = S.mlp_ref(p, (se[0], se[1], se[3]), "cot", False, se_eval=True)
     S.within(a, ar, ea, what + " se_eval attention weights")
     o, oe = S.tail_combine_ref(y, ye, k, a)
     _w(tout, o, oe, what + " tail_combine", "eval_tail")

@@ -3,8 +3,8 @@
 TcConv1x1Fn, TcConv3x3Fn and StemConvBNFn in the configurations the CoT blocks reach, and cotnet50 CoT bottlenecks of stages 1, 2 and
 4 parameter by parameter.  The DropBlock functions' checks, the CoXt, SE-CoTNetD, DropBlock, stochastic-depth and stem cases and
 the derived-weight accounting are used by test_step_stages_gpu.py.  Not covered: whole-model steps.  Eval-mode flags are checked only under grad, where CotLayer takes _forward_fused and cot_tail takes
-CotTailFn; the inference path (_forward_tc_eval, _cot_tail_eval, cotb200_se_eval) is tested in test_eval_kernels_gpu.py and
-test_eval_stages_gpu.py.
+CotTailFn; the inference path (_forward_tc_eval, _cot_tail_eval, cotb200_se_eval) is tested in test_eval_kernels_gpu.py,
+test_eval_stages_gpu.py and, in whole blocks and networks, test_eval_blocks_gpu.py.
 
 Bounds are per element: 1/2 ulp of the stored dtype plus the fp32 error of the stage, with fp32 sums bounded by gamma(n) * sum|terms|
 (gamma_tc(n), 2u per add, on the tensor cores) for the chain length n of the kernel.  Where operands are small integers the GEMM /
