@@ -26,6 +26,27 @@ from .backbone import StochasticDepth
 from .cot_layer import CoTLayer
 
 
+class _ReflectPad1(torch.autograd.Function):
+    """F.pad(x, (1, 1, 1, 1), mode="reflect") with a backward that adds the border gradients in a fixed order.  The CUDA backward of
+    the reflect padding accumulates them with atomic adds, so in bf16 the rounding, and with it the whole training step, changes
+    from run to run."""
+
+    @staticmethod
+    def forward(ctx, x):
+        return F.pad(x, (1, 1, 1, 1), mode="reflect")
+
+    @staticmethod
+    def backward(ctx, g):
+        gx = g[:, :, 1:-1, 1:-1].clone()
+        gx[:, :, 1] += g[:, :, 0, 1:-1]                 # padded row 0 is row 1, padded row H + 1 is row H - 2; columns alike
+        gx[:, :, -2] += g[:, :, -1, 1:-1]
+        gx[:, :, :, 1] += g[:, :, 1:-1, 0]
+        gx[:, :, :, -2] += g[:, :, 1:-1, -1]
+        for r, c in ((0, 0), (0, -1), (-1, 0), (-1, -1)):   # the corners: row and column reflected
+            gx[:, :, 1 if r == 0 else -2, 1 if c == 0 else -2] += g[:, :, r, c]
+        return gx
+
+
 class BlurPool2d(nn.Module):
     """models/layers/blur_pool.py:19-58 with filt_size 3: reflect-pad 1, depthwise [1,2,1]x[1,2,1]/16, stride 2."""
 
@@ -37,7 +58,7 @@ class BlurPool2d(nn.Module):
         self.register_buffer("_filt", (c[:, None] * c[None, :])[None, None].repeat(channels, 1, 1, 1), persistent=False)
 
     def forward(self, x):
-        return F.conv2d(F.pad(x, (1, 1, 1, 1), mode="reflect"), self._filt.to(x.dtype), stride=self.stride, groups=x.shape[1])
+        return F.conv2d(_ReflectPad1.apply(x), self._filt.to(x.dtype), stride=self.stride, groups=x.shape[1])
 
 
 class SplitAttnConv2d(nn.Module):

@@ -217,6 +217,17 @@ SOURCE_ANCHORS = {
         "return dict(radix=1, conv_dim={64, 128}, c4_dim=256, c4_idx=set(range(0, n_l3, 2)), **kw)",
         "stride = 2 if b == 0 else 1",
         "x = fused.bn_act(c[6](x).contiguous(memory_format=cl), self.bn1, relu=True)",
+        # the stride-2 pool of conv2 (HYBRID: which trunk pools how, and where)
+        "return nn.AvgPool2d(3, s, padding=1) if aa_layer is None else aa_layer(channels=width, stride=s)",
+        "self.avd = pool(stride)\n                stride = 1",
+        "if stride > 1:\n                self.avd = pool(stride)",
+        "if isinstance(self.avd, nn.AvgPool2d) and self.avd.kernel_size == 3 and self.avd.stride == 2 and fused.supported(y):",
+        "return F.pad(x, (1, 1, 1, 1), mode=\"reflect\")",
+        "return F.conv2d(_ReflectPad1.apply(x), self._filt.to(x.dtype), stride=self.stride, groups=x.shape[1])",
+        "c = torch.tensor([0.25, 0.5, 0.25])",
+        "return CoTHybridNet([3, 4, 6, 3], stem_width=32, block_args=_args(6, avd=False, avd_first=True), **kw)",
+        "return CoTHybridNet([3, 8, 36, 3], stem_width=64, aa_layer=BlurPool2d, block_args=_args(36, avd=True, avd_first=False), **kw)",
+        "return se_cotnetd_152(**kw)",
     ],
     "cotnet_b200/tc.py": [
         "for bn in (64, 128, 192, 256):",
@@ -904,32 +915,48 @@ def bottleneck_calls(B, cin, width, cout, H, stride, min_pixels=TC_MIN_PIXELS, c
     return out + _tail_calls(B, width, cout, Ho, min_pixels, drop_block, ds)
 
 
-def hybrid_split(width, block_idx, conv_dim=(64, 128), c4_dim=256, c4_idx=(0, 2, 4)):
-    """backbone_hybrid.CoTBottleneck: conv2 is a SplitAttnConv2d (else the CoT layer); se_cotnetd_50's block arguments"""
+#: The SE-CoTNetD trunks (backbone_hybrid.se_cotnetd_*): blocks per stage, deep-stem width, the pool of a stride-2 conv2 (the
+#: 3x3/s2 average pool on Pool3x3S2Fn, or BlurPool2d: F.pad reflect + a depthwise [1,2,1]x[1,2,1]/16 torch convolution, so no
+#: recorded call), avd (a split-attention conv2 runs at stride 1 and pools), avd_first (the pool before conv2, else after it),
+#: c4_idx (the stage-3 blocks whose conv2 is a CoT layer: the even ones)
+HYBRID = {
+    "se_cotnetd_50": dict(layers=(3, 4, 6, 3), stem_width=32, blur=False, avd=False, avd_first=True, c4_idx=tuple(range(0, 6, 2))),
+    "se_cotnetd_152": dict(layers=(3, 8, 36, 3), stem_width=64, blur=True, avd=True, avd_first=False,
+                           c4_idx=tuple(range(0, 36, 2))),
+}
+#: the model name each trunk's block configuration is registered under (se_cotnetd_152_L is se_cotnetd_152 at 320)
+HYBRID["se_cotnetd_152_L"] = HYBRID["se_cotnetd_152"]
+
+
+def hybrid_split(width, block_idx, conv_dim=(64, 128), c4_dim=256, c4_idx=HYBRID["se_cotnetd_50"]["c4_idx"]):
+    """backbone_hybrid.CoTBottleneck: conv2 is a SplitAttnConv2d (else the CoT layer); se_cotnetd_50's block arguments unless
+    c4_idx says otherwise"""
     return width in conv_dim or (width == c4_dim and block_idx not in c4_idx)
 
 
-def hybrid_block_calls(B, block_idx, cin, width, H, stride, min_pixels=TC_MIN_PIXELS, drop_block=False, ds=False, avd=False,
-                       avd_first=True):
+def hybrid_block_calls(B, block_idx, cin, width, H, stride, min_pixels=TC_MIN_PIXELS, drop_block=False, ds=False,
+                       model="se_cotnetd_50"):
     """the forward calls of backbone_hybrid.CoTBottleneck.forward on a bf16 channels_last input: a split-attention conv2 runs
     the cuDNN 3x3 convolution (stride 2 itself unless avd) and the fused gate tail, or with DropBlock bn0 on BNActFn, the
-    DropBlock and the rest of the gate in torch; a CoT conv2 pools first (avd) at stride 2; the avg_down downsample pools in
-    torch before its 1x1 convolution"""
+    DropBlock and the rest of the gate in torch; a CoT conv2 pools at stride 2, before it (avd_first) at the output size or
+    after it at the input size; a BlurPool is torch glue; the avg_down downsample pools in torch before its 1x1 convolution"""
+    cfg = HYBRID[model]
     cout = 4 * width
-    Ho = H // stride
-    split = hybrid_split(width, block_idx)
-    pool = stride > 1 and (avd if split else True)
+    Ho = conv_out(H, stride)
+    split = hybrid_split(width, block_idx, c4_idx=cfg["c4_idx"])
+    pool = stride > 1 and (cfg["avd"] if split else True)
+    avd_first, pool_call = cfg["avd_first"], [] if cfg["blur"] else ["Pool3x3S2Fn(avg)"]
     out = ["TcConv1x1Fn(one,relu)" if conv1x1_tc(cin, width, B * H * H, 1, min_pixels) else "BNActFn(relu)"]
     if drop_block:
         out.append("DropBlockFn")
     if pool and avd_first:
-        out.append("Pool3x3S2Fn(avg)")
+        out += pool_call
     if split:
         out += ["BNActFn(plain)", "DropBlockFn"] if drop_block else ["CotTailFn(gate)"]
     else:
-        out += cot_calls(B, width, Ho if avd_first else H, min_pixels)
+        out += cot_calls(B, width, Ho if pool and avd_first else H, min_pixels)
     if pool and not avd_first:
-        out.append("Pool3x3S2Fn(avg)")
+        out += pool_call
     if block_idx == 0:
         out.append("TcConv1x1Fn(one,bn)" if conv1x1_tc(cin, cout, B * Ho * Ho, 1, min_pixels) else "BNActFn(plain)")
     return out + _tail_calls(B, width, cout, Ho, min_pixels, drop_block, ds)
@@ -938,7 +965,7 @@ def hybrid_block_calls(B, block_idx, cin, width, H, stride, min_pixels=TC_MIN_PI
 def stem_calls(model, H, W):
     """the stems: cotnet50's 7x7/s2 StemConvBNFn (wgmma for even sizes) + the max pool; the deep stem's three cuDNN 3x3
     convolutions, each followed by a BatchNorm + ReLU"""
-    if model == "se_cotnetd_50":
+    if model in HYBRID:
         return ["BNActFn(relu)"] * 3
     return ["StemConvBNFn" if stem_tc(H, W, 64) else "BNActFn(relu)", "Pool3x3S2Fn(max)"]
 
@@ -949,8 +976,9 @@ def case_calls(c):
     if c["kind"] == "stem":
         return stem_calls(c["model"], c["H"], c["W"])
     db, ds = bool(c.get("sites")), c.get("ds") is not None
-    if c["model"] == "se_cotnetd_50":
-        return hybrid_block_calls(c["B"], int(c["block"].split(".")[1]), c["cin"], c["width"], c["H"], c["stride"], mp, db, ds)
+    if c["model"] in HYBRID:
+        return hybrid_block_calls(c["B"], int(c["block"].split(".")[1]), c["cin"], c["width"], c["H"], c["stride"], mp, db, ds,
+                                  c["model"])
     return bottleneck_calls(c["B"], c["cin"], c["width"], c["cout"], c["H"], c["stride"], mp, c["model"] != "cotnet50", db, ds)
 
 
@@ -1021,6 +1049,60 @@ STEP_BLOCK_CASES = {
         calls=["BNActFn(relu)"] * 3,
         flow=['c1<-0.0', 'c2<-1.0']),
 }
+#: SE-CoTNetD-152 at its 320 (cot_l) and 256 (cot_s) configs: BlurPool after conv2 of every stride-2 block (avd, avd_first=False),
+#: so a split-attention conv2 of a first block runs at stride 1 on the block's input size and a CoT layer of layer3.0 / layer4.0
+#: before the pool.  min_pixels=0 where the bench's bs64 step is above TC_MIN_PIXELS (stages 1-2 and layer3.0 at 320: 102400
+#: pixels), the default below it; layer3.0 at B=64 takes the real threshold.  ds: drop path at the config's rate 0.15.  In the
+#: flows, "c<j><-pad(k.o)": torch convolution j (the BlurPool) reads the reflect padding of k.o; "<-c<j>": the BlurPool's output.
+_DS152 = (0.0, 1.0 / 0.85)
+_HYB152 = dict(model="se_cotnetd_152", kind="block")
+_COT152_FIRST = ["BNActFn(relu)"] + _COT_E0 + ["BNActFn(plain)", "BNActFn(relu+res)"]
+_FLOW152_FIRST = ['1.0<-0.0', '3.0<-2.0', '4.0<-1.2', '4.1<-3.1', '7.0<-5.0', '7.1<-6.0', '8.0<-7.0', '8.1<-3.1', '10.3<-9.0', 'c0<-x',
+                  'c1<-1.2', 'c2<-4.0', 'c3<-1.2', 'c4<-pad(8.0)', 'c6<-c4']
+_COT152 = ["BNActFn(relu)"] + _COT_E0
+_FLOW152 = ['1.0<-0.0', '3.0<-2.0', '4.0<-1.2', '4.1<-3.1', '7.0<-5.0', '7.1<-6.0', '8.0<-7.0', '8.1<-3.1', '9.3<-x', 'c0<-x', 'c1<-1.2',
+            'c2<-4.0', 'c3<-1.2', 'c4<-8.0']
+#: layer3.0 with its CoT layer's embed.3 and conv1x1 on wgmma (embed.3: N = 288, three 128-wide tiles), conv1 too; the key conv
+#: (dim 256 > TC_KEY_MAX_DIM), the downsample and conv3 (weights above TC_TRUNK_MAX_WEIGHT) on cuDNN
+_L30_TC = ["TcConv1x1Fn(one,relu)", "FanOutFn(3)", "BNActFn(relu)", "FanOutFn(2)", "TcConv1x1Fn(two,relu)", "TcConv1x1Fn(one,nobn)",
+           "TcConv1x1Fn(one,bn)", "GroupNorm9Fn(gc8+lbias)", "AggTapFn(fold1,gc8)", "CotTailFn(k)", "BNActFn(plain)", "BNActFn(relu+res)"]
+_L30_TC_FLOW = ['0.0<-x', '1.0<-0.0', '3.0<-2.0', '4.0<-1.2', '4.1<-3.1', '5.0<-4.0', '6.0<-1.2', '7.0<-5.0', '8.0<-6.0', '8.1<-7.0',
+                '9.0<-8.0', '9.1<-3.1', '11.3<-10.0', 'c0<-1.2', 'c1<-pad(9.0)', 'c3<-c1']
+STEP_BLOCK_CASES.update({
+    "hybrid152_320_layer1_first_b2": dict(_HYB152, block="layer1.0", B=2, cin=128, width=64, cout=256, H=160, stride=2, min_pixels=0,
+        calls=["TcConv1x1Fn(one,relu)", "CotTailFn(gate)", "TcConv1x1Fn(one,bn)", "TcConv1x1Fn(one,relu+res)"],
+        flow=['0.0<-x', '3.0<-c1', '3.8<-2.0', 'c0<-0.0', 'c1<-pad(1.0)']),
+    "hybrid152_320_layer2_split_drop_path_b2": dict(_HYB152, block="layer2.3", B=2, cin=512, width=128, cout=512, H=40, stride=1,
+                                                     min_pixels=0, ds=_DS152,
+        calls=["TcConv1x1Fn(one,relu)", "CotTailFn(gate)", "TcConv1x1Fn(one,relu+res+ds)"],
+        flow=['0.0<-x', '2.0<-1.0', '2.8<-x', 'c0<-0.0']),
+    "hybrid152_320_layer3_cot_first_b2": dict(_HYB152, block="layer3.0", B=2, cin=512, width=256, cout=1024, H=40, stride=2,
+                                               min_pixels=0, calls=_L30_TC, flow=_L30_TC_FLOW),
+    "hybrid152_320_layer3_cot_first_b64": dict(_HYB152, block="layer3.0", B=64, cin=512, width=256, cout=1024, H=40, stride=2,
+                                                calls=_L30_TC, flow=_L30_TC_FLOW),
+    "hybrid152_320_layer3_split_b2": dict(_HYB152, block="layer3.17", B=2, cin=1024, width=256, cout=1024, H=20, stride=1,
+        calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(relu+res)"],
+        flow=['2.3<-x', 'c0<-x', 'c1<-0.0', 'c2<-1.0']),
+    "hybrid152_320_layer3_cot_drop_path_b2": dict(_HYB152, block="layer3.2", B=2, cin=1024, width=256, cout=1024, H=20, stride=1,
+                                                   ds=_DS152, calls=_COT152 + ["BNActFn(relu+res+ds)"], flow=_FLOW152),
+    "hybrid152_320_layer4_first_b2": dict(_HYB152, block="layer4.0", B=2, cin=1024, width=512, cout=2048, H=20, stride=2,
+                                           calls=_COT152_FIRST, flow=_FLOW152_FIRST),
+    "hybrid152_320_layer4_b2": dict(_HYB152, block="layer4.1", B=2, cin=2048, width=512, cout=2048, H=10, stride=1,
+                                     calls=_COT152 + ["BNActFn(relu+res)"], flow=_FLOW152),
+    # 256: at bs64 layer3.0 sees 65536 pixels, below the threshold
+    "hybrid152_256_layer3_cot_first_b2": dict(_HYB152, block="layer3.0", B=2, cin=512, width=256, cout=1024, H=32, stride=2,
+                                               calls=_COT152_FIRST, flow=_FLOW152_FIRST),
+    "hybrid152_256_layer3_cot_b2": dict(_HYB152, block="layer3.34", B=2, cin=1024, width=256, cout=1024, H=16, stride=1,
+                                         calls=_COT152 + ["BNActFn(relu+res)"], flow=_FLOW152),
+    "hybrid152_256_layer4_first_b2": dict(_HYB152, block="layer4.0", B=2, cin=1024, width=512, cout=2048, H=16, stride=2,
+                                           calls=_COT152_FIRST, flow=_FLOW152_FIRST),
+    "hybrid152_256_layer4_drop_path_b2": dict(_HYB152, block="layer4.2", B=2, cin=2048, width=512, cout=2048, H=8, stride=1,
+                                               ds=_DS152, calls=_COT152 + ["BNActFn(relu+res+ds)"], flow=_FLOW152),
+    "hybrid152_deep_stem_320": dict(model="se_cotnetd_152", kind="stem", B=2, H=320, W=320, calls=["BNActFn(relu)"] * 3,
+                                    flow=['c1<-0.0', 'c2<-1.0']),
+    "hybrid152_deep_stem_256": dict(model="se_cotnetd_152", kind="stem", B=2, H=256, W=256, calls=["BNActFn(relu)"] * 3,
+                                    flow=['c1<-0.0', 'c2<-1.0']),
+})
 
 
 def conv_out(H, stride):
@@ -1031,16 +1113,18 @@ def conv_out(H, stride):
 
 def model_blocks(model, H0, W0=None):
     """[(name, block index in its stage, cin, width, cout, H in, W in, stride)] of every bottleneck of cotnet50 / cotnext50_2x48d /
-    se_cotnetd_50 for an H0 x W0 image: cotnet's 7x7/s2 stem and max pool, stride 2 from stage 2 on; the deep stem's stride 2,
-    stride 2 in every stage (backbone.CoTResNet, backbone_hybrid.CoTHybridNet)"""
+    the SE-CoTNetD trunks for an H0 x W0 image: cotnet's 7x7/s2 stem and max pool, stride 2 from stage 2 on; the deep stem's
+    stride 2 (2 * stem_width channels out), stride 2 in every stage (backbone.CoTResNet, backbone_hybrid.CoTHybridNet).  A stride-2
+    BlurPool (reflect pad 1, 3x3, stride 2) gives the same size as the 3x3/s2 average pool."""
     W0 = H0 if W0 is None else W0
-    hybrid = model == "se_cotnetd_50"
+    hybrid = model in HYBRID
     H, W = conv_out(H0, 2), conv_out(W0, 2)
     if not hybrid:
         H, W = conv_out(H, 2), conv_out(W, 2)
-    cin = 64
+    cin = 2 * HYBRID[model]["stem_width"] if hybrid else 64
+    layers = HYBRID[model]["layers"] if hybrid else (3, 4, 6, 3)
     out = []
-    for si, (planes, n) in enumerate(zip((64, 128, 256, 512), (3, 4, 6, 3))):
+    for si, (planes, n) in enumerate(zip((64, 128, 256, 512), layers)):
         width = planes * 48 // 64 * 2 if model == "cotnext50_2x48d" else planes
         for b in range(n):
             stride = 2 if b == 0 and (hybrid or si > 0) else 1
@@ -1049,14 +1133,14 @@ def model_blocks(model, H0, W0=None):
     return out
 
 
-def model_calls(model, B, H0, min_pixels=TC_MIN_PIXELS):
-    """the recorded calls of one TrainStep forward with drop path (every block but the first) and DropBlock (stages 3-4) on, as
-    [stem calls, [calls of each block], loss calls]"""
+def model_calls(model, B, H0, min_pixels=TC_MIN_PIXELS, drop_block=True):
+    """the recorded calls of one TrainStep forward with drop path (every block but the first) and DropBlock (stages 3-4, unless
+    drop_block is False) on, as [stem calls, [calls of each block], loss calls]"""
     blocks = []
     for i, (name, b, cin, width, cout, H, W, stride) in enumerate(model_blocks(model, H0)):
-        db = name.startswith(("layer3", "layer4"))
-        if model == "se_cotnetd_50":
-            blocks.append(hybrid_block_calls(B, b, cin, width, H, stride, min_pixels, db, i > 0))
+        db = drop_block and name.startswith(("layer3", "layer4"))
+        if model in HYBRID:
+            blocks.append(hybrid_block_calls(B, b, cin, width, H, stride, min_pixels, db, i > 0, model))
         else:
             blocks.append(bottleneck_calls(B, cin, width, cout, H, stride, min_pixels, model != "cotnet50", db, i > 0))
     return stem_calls(model, H0, H0), blocks, ["SoftTargetCrossEntropyFn"]
@@ -1069,7 +1153,7 @@ def model_sites(model):
     for name, b, cin, width, cout, H, W, stride in model_blocks(model, 224):
         if not name.startswith(("layer3", "layer4")):
             continue
-        n = 3 if model == "se_cotnetd_50" and hybrid_split(width, b) else 2
+        n = 3 if model in HYBRID and hybrid_split(width, b, c4_idx=HYBRID[model]["c4_idx"]) else 2
         out[name] = tuple(range(site, site + n))
         site += n
     return out
@@ -1124,23 +1208,26 @@ def eval_bottleneck_calls(B, cin, width, cout, H, W, stride, bf16_weights, min_p
     return out + [_eval_1x1(width, cout, B * Ho * Wo, 1, min_pixels, "relu+res")]
 
 
-def eval_hybrid_block_calls(B, block_idx, cin, width, H, W, stride, bf16_weights, min_pixels=TC_MIN_PIXELS, avd=False,
-                            avd_first=True):
+def eval_hybrid_block_calls(B, block_idx, cin, width, H, W, stride, bf16_weights, min_pixels=TC_MIN_PIXELS, model="se_cotnetd_50"):
     """backbone_hybrid.CoTBottleneck.forward in eval: a split-attention conv2 is the cuDNN 3x3 (stride 2 itself unless avd) and the
-    gate on CotTailFn with running statistics; a CoT conv2 pools first at stride 2; the avg_down downsample pools in torch"""
+    gate on CotTailFn with running statistics; a CoT conv2 pools at stride 2, before or after it as avd_first says (a BlurPool
+    is torch glue); the avg_down downsample pools in torch"""
+    cfg = HYBRID[model]
     cout = 4 * width
     Ho, Wo = conv_out(H, stride), conv_out(W, stride)
-    split = hybrid_split(width, block_idx)
-    pool = stride > 1 and (avd if split else True)
+    split = hybrid_split(width, block_idx, c4_idx=cfg["c4_idx"])
+    pool = stride > 1 and (cfg["avd"] if split else True)
+    avd_first, pool_call = cfg["avd_first"], [] if cfg["blur"] else ["Pool3x3S2Fn(avg)"]
     out = [_eval_1x1(cin, width, B * H * W, 1, min_pixels, "relu")]
     if pool and avd_first:
-        out.append("Pool3x3S2Fn(avg)")
+        out += pool_call
     if split:
         out.append("CotTailFn(gate)")
     else:
-        out += eval_cot_calls(B, width, Ho if avd_first else H, Wo if avd_first else W, bf16_weights, min_pixels)
+        first = pool and avd_first
+        out += eval_cot_calls(B, width, Ho if first else H, Wo if first else W, bf16_weights, min_pixels)
     if pool and not avd_first:
-        out.append("Pool3x3S2Fn(avg)")
+        out += pool_call
     if block_idx == 0:
         out.append(_eval_1x1(cin, cout, B * Ho * Wo, 1, min_pixels, "bn"))
     return out + [_eval_1x1(width, cout, B * Ho * Wo, 1, min_pixels, "relu+res")]
@@ -1156,8 +1243,8 @@ def eval_model_calls(model, B, H0, W0, bf16_weights, min_pixels=TC_MIN_PIXELS):
     are torch ops"""
     blocks = []
     for name, b, cin, width, cout, H, W, stride in model_blocks(model, H0, W0):
-        if model == "se_cotnetd_50":
-            blocks.append(eval_hybrid_block_calls(B, b, cin, width, H, W, stride, bf16_weights, min_pixels))
+        if model in HYBRID:
+            blocks.append(eval_hybrid_block_calls(B, b, cin, width, H, W, stride, bf16_weights, min_pixels, model))
         else:
             blocks.append(eval_bottleneck_calls(B, cin, width, cout, H, W, stride, bf16_weights, min_pixels,
                                                 model != "cotnet50"))
@@ -1169,9 +1256,9 @@ def eval_case_calls(c):
     mp = TC_MIN_PIXELS if c.get("min_pixels") is None else c["min_pixels"]
     if c["kind"] == "stem":
         return eval_stem_calls(c["model"], c["H"], c["W"])
-    if c["model"] == "se_cotnetd_50":
+    if c["model"] in HYBRID:
         return eval_hybrid_block_calls(c["B"], int(c["block"].split(".")[1]), c["cin"], c["width"], c["H"], c["W"], c["stride"],
-                                       c["bf16"], mp)
+                                       c["bf16"], mp, c["model"])
     return eval_bottleneck_calls(c["B"], c["cin"], c["width"], c["cout"], c["H"], c["W"], c["stride"], c["bf16"], mp,
                                  c["model"] != "cotnet50")
 
@@ -1261,3 +1348,41 @@ EVAL_BLOCK_CASES = {
     "hybrid_deep_stem": dict(model="se_cotnetd_50", kind="stem", B=2, H=224, W=224, bf16=True, calls=["BNActFn(relu)"] * 3,
                              flow=["c0<-x", "c1<-0.0", "c2<-1.0"]),
 }
+#: SE-CoTNetD-152 at 320 and 256 (see STEP_BLOCK_CASES): the BlurPool after conv2, and the wgmma key convolution of every CoT layer
+#: geometry the trunk has: dim 256 on the haloed kernel at 40x40 (R = 5), 20x20 (R = 10), 32x32 (R = 4) and 16x16 (R = 8), dim
+#: 512 in conv mode at 20x20 (100-row bands), 10x10 (100-row tiles), 16x16 (128-row bands) and 8x8 (two samples per tile)
+_EVAL152_FIRST = ["BNActFn(relu)"] + _EVAL_TC + ["BNActFn(plain)", "BNActFn(relu+res)"]
+_EVAL152_FIRST_FLOW = _tc_layer_flow(1, "0.0") + ["9.3<-8.0", "c0<-x", "c1<-pad(7.3)", "c3<-c1"]
+_EVAL152 = ["BNActFn(relu)"] + _EVAL_TC + ["BNActFn(relu+res)"]
+_EVAL152_FLOW = _tc_layer_flow(1, "0.0") + ["8.3<-x", "c0<-x", "c1<-7.3"]
+_EVAL152_SPLIT = dict(calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(relu+res)"], flow=["2.3<-x", "c0<-x", "c1<-0.0", "c2<-1.0"])
+EVAL_BLOCK_CASES.update({
+    "hybrid152_320_layer1_first_b2": dict(_HYB152, block="layer1.0", B=2, cin=128, width=64, cout=256, H=160, W=160, stride=2,
+                                          bf16=True, calls=["BNActFn(relu)", "CotTailFn(gate)", "BNActFn(plain)", "BNActFn(relu+res)"],
+                                          flow=["3.3<-2.0", "c0<-x", "c1<-0.0", "c2<-pad(1.0)", "c4<-c2"]),
+    "hybrid152_320_layer2_split_b2": dict(_HYB152, block="layer2.5", B=2, cin=512, width=128, cout=512, H=40, W=40, stride=1, bf16=True,
+                                          **_EVAL152_SPLIT),
+    "hybrid152_320_layer3_cot_first_b2": dict(_HYB152, block="layer3.0", B=2, cin=512, width=256, cout=1024, H=40, W=40, stride=2,
+                                              bf16=True, calls=_EVAL152_FIRST, flow=_EVAL152_FIRST_FLOW),
+    "hybrid152_320_layer3_split_b2": dict(_HYB152, block="layer3.1", B=2, cin=1024, width=256, cout=1024, H=20, W=20, stride=1,
+                                          bf16=True, **_EVAL152_SPLIT),
+    "hybrid152_320_layer3_cot_b2": dict(_HYB152, block="layer3.2", B=2, cin=1024, width=256, cout=1024, H=20, W=20, stride=1,
+                                        bf16=True, calls=_EVAL152, flow=_EVAL152_FLOW),
+    "hybrid152_320_layer4_first_b2": dict(_HYB152, block="layer4.0", B=2, cin=1024, width=512, cout=2048, H=20, W=20, stride=2,
+                                          bf16=True, calls=_EVAL152_FIRST, flow=_EVAL152_FIRST_FLOW),
+    "hybrid152_320_layer4_b3": dict(_HYB152, block="layer4.1", B=3, cin=2048, width=512, cout=2048, H=10, W=10, stride=1, bf16=True,
+                                    calls=_EVAL152, flow=_EVAL152_FLOW),
+    "hybrid152_256_layer3_cot_first_b2": dict(_HYB152, block="layer3.0", B=2, cin=512, width=256, cout=1024, H=32, W=32, stride=2,
+                                              bf16=True, calls=_EVAL152_FIRST, flow=_EVAL152_FIRST_FLOW),
+    "hybrid152_256_layer3_cot_b2": dict(_HYB152, block="layer3.20", B=2, cin=1024, width=256, cout=1024, H=16, W=16, stride=1,
+                                        bf16=True, calls=_EVAL152, flow=_EVAL152_FLOW),
+    "hybrid152_256_layer4_first_b2": dict(_HYB152, block="layer4.0", B=2, cin=1024, width=512, cout=2048, H=16, W=16, stride=2,
+                                          bf16=True, calls=_EVAL152_FIRST, flow=_EVAL152_FIRST_FLOW),
+    # odd B: a half-empty last tile of the two-sample conv mode
+    "hybrid152_256_layer4_b3": dict(_HYB152, block="layer4.2", B=3, cin=2048, width=512, cout=2048, H=8, W=8, stride=1, bf16=True,
+                                    calls=_EVAL152, flow=_EVAL152_FLOW),
+    "hybrid152_deep_stem_320": dict(model="se_cotnetd_152", kind="stem", B=2, H=320, W=320, bf16=True, calls=["BNActFn(relu)"] * 3,
+                                    flow=["c0<-x", "c1<-0.0", "c2<-1.0"]),
+    "hybrid152_deep_stem_256": dict(model="se_cotnetd_152", kind="stem", B=2, H=256, W=256, bf16=True, calls=["BNActFn(relu)"] * 3,
+                                    flow=["c0<-x", "c1<-0.0", "c2<-1.0"]),
+})

@@ -23,7 +23,7 @@ from cotnet_b200 import _lib, evaler, fused
 from cotnet_b200.cot_layer import CotLayer
 from test_eval_gpu import rank_rule_counts
 from test_eval_stages_gpu import _EvalRecorder, _check_fold, check_eval_layer, check_tail_eval
-from test_stage_grads_gpu import ONE_ULP, ConvRecorder, _cfg, _w, check_call, tail_mods
+from test_stage_grads_gpu import ONE_ULP, ConvRecorder, PadRecorder, _cfg, _w, blur_convs, check_blur, check_call, tail_mods
 from test_step_stages_gpu import _Order
 
 pytestmark = pytest.mark.gpu
@@ -67,7 +67,8 @@ def _cl(t):
 
 def _ctor(name):
     from cotnet_b200 import backbone, backbone_hybrid
-    return {"cotnet50": backbone.cotnet50, "cotnext50_2x48d": backbone.cotnext50_2x48d, "se_cotnetd_50": backbone_hybrid.se_cotnetd_50}[name]
+    return {"cotnet50": backbone.cotnet50, "cotnext50_2x48d": backbone.cotnext50_2x48d, "se_cotnetd_50": backbone_hybrid.se_cotnetd_50,
+            "se_cotnetd_152": backbone_hybrid.se_cotnetd_152, "se_cotnetd_152_L": backbone_hybrid.se_cotnetd_152_L}[name]
 
 
 def _randomise(mod, seed):
@@ -147,34 +148,40 @@ def _rows_view(t):
     return t.permute(0, 2, 3, 1).reshape(-1, t.shape[1]) if t.dim() == 4 else t
 
 
-def eval_flow(calls, convs, order, x):
+def eval_flow(calls, convs, order, x, blurs=None):
     """every recorded call argument and torch convolution input that is an earlier recorded output (or x), matched by storage and
     compared by value in NHWC row order: sorted "consumer<-producer" edges.  The recorder holds every output, so no storage is
-    reused during the forward."""
+    reused during the forward.  blurs ({conv index: pad record}): a BlurPool's output is a producer ("c<j>") and its convolution
+    reads "pad(k.o)", the reflect padding of a recorded output."""
     prod = {}
+    # times: call i at (i, 1, 0); torch convolution j, made after order[j] recorded calls, at (order[j], 0, j)
     for i, c in enumerate(calls):
         for o, (pt, snap) in enumerate(zip(c.out_ptr, c.out if isinstance(c.out, tuple) else (c.out,))):
-            prod.setdefault(pt, []).append(("%d.%d" % (i, o), i, snap))
-    prod.setdefault(x.data_ptr(), []).append(("x", -1, x.detach()))
+            prod.setdefault(pt, []).append(("%d.%d" % (i, o), (i, 1, 0), snap))
+    prod.setdefault(x.data_ptr(), []).append(("x", (-1, 1, 0), x.detach()))
+    for j in sorted(blurs or ()):
+        prod.setdefault(convs[j]["out_ptr"], []).append(("c%d" % j, (order[j], 0, j), convs[j]["y"]))
 
-    def find(ptr, snap, upto, what):
-        cands = [(n, s) for n, i, s in prod.get(ptr, []) if i < upto and _rows_view(s).shape == _rows_view(snap).shape]
+    def find(ptr, snap, t, what):
+        cands = sorted([(tp, n, s) for n, tp, s in prod.get(ptr, []) if tp < t and _rows_view(s).shape == _rows_view(snap).shape],
+                       key=lambda e: e[0])
         if not cands:
             return None
-        n, s = cands[-1]
+        _, n, s = cands[-1]
         S.equal(_rows_view(snap), _rows_view(s), "%s == %s" % (what, n))
         return n
     edges = {}
     for i, c in enumerate(calls):
         for a, arg in enumerate(c.args):
             if isinstance(arg, torch.Tensor):
-                n = find(arg.data_ptr(), c.inp[a], i, "%d.%d" % (i, a))
+                n = find(arg.data_ptr(), c.inp[a], (i, 1, 0), "%d.%d" % (i, a))
                 if n is not None:
                     edges["%d.%d" % (i, a)] = n
     for j, r in enumerate(convs):
-        n = find(r["ptr"], r["x"], order[j], "c%d" % j)
+        src = (blurs or {}).get(j)
+        n = find(src["ptr"] if src else r["ptr"], src["x"] if src else r["x"], (order[j], 0, j), "c%d" % j)
         if n is not None:
-            edges["c%d" % j] = n
+            edges["c%d" % j] = "pad(%s)" % n if src else n
     return sorted("%s<-%s" % kv for kv in edges.items())
 
 
@@ -207,12 +214,15 @@ def test_eval_block_stage_by_stage(geo, monkeypatch):
         n_plain = _lib.launch_count() - n0
     rec = _EvalRecorder(monkeypatch, keep_outputs=True)
     conv_rec = ConvRecorder(monkeypatch)
+    pad_rec = PadRecorder(monkeypatch, conv_rec.calls)
     order_rec = _Order(monkeypatch, rec)
     with _eval_body():
         n0 = _lib.launch_count()
         out = run(x)
         n_rec = _lib.launch_count() - n0
     calls, convs, order = rec.calls, list(conv_rec.calls), list(order_rec.order)
+    blurs = blur_convs(convs, pad_rec.calls)
+    assert len(blurs) == (1 if case["model"] == "se_cotnetd_152" and case.get("stride") == 2 else 0), geo
     # (e)
     assert n_rec == n_plain, "the recorders changed the launches"
     S.equal(out, plain, geo + " output with / without the recorders")
@@ -223,8 +233,10 @@ def test_eval_block_stage_by_stage(geo, monkeypatch):
     # (c)
     for j, r in enumerate(convs):
         check_torch_conv(r, "%s c%d" % (geo, j))
+    for j, p in blurs.items():
+        check_blur(convs[j], p, "%s c%d" % (geo, j))
     # (d)
-    got = eval_flow(calls, convs, order, x)
+    got = eval_flow(calls, convs, order, x, blurs)
     assert got == sorted(case["flow"]), "%s dataflow: %s" % (geo, got)
     S.equal(out, calls[-1].out if not isinstance(calls[-1].out, tuple) else calls[-1].out[-1], geo + " output = the last call's")
 
@@ -251,10 +263,22 @@ def test_eval_network_stage_by_stage(name, monkeypatch):
     (3) stem -> block -> block dataflow and each block's input shape, (4) the global average pool and fc, (5) a captured EvalStep
     on the same batch gives the same logits bit for bit and the rank rule's counts of them"""
     mname, (H0, W0), bf16, mp = NET_CASES[name]
+    eval_network_stage_by_stage(name, mname, H0, W0, bf16, mp, monkeypatch)
+
+
+def eval_network_stage_by_stage(name, mname, H0, W0, bf16, mp, monkeypatch, B=2, bn3_gain=1.0):
+    """the body of test_eval_network_stage_by_stage for any model, image size and batch; every BlurPool (se_cotnetd_152) against
+    fp64 of its filter on the reflect-padded input.  bn3_gain scales each block's last BatchNorm weight: random running statistics
+    do not normalise, so each residual branch multiplies the activations by a factor of order its bn3 gain, and over a deep trunk
+    (50 blocks) they would leave fp32's range."""
     if mp is not None:
         monkeypatch.setattr(fused, "TC_MIN_PIXELS", mp)
-    K, B, ks = 100, 2, (1, 5)
+    K, ks = 100, (1, 5)
     model = _net(mname, bf16, K)
+    if bn3_gain != 1.0:
+        with torch.no_grad():
+            for blk in model.blocks():
+                blk.bn3.weight.mul_(bn3_gain)
     g = torch.Generator(device=DEV).manual_seed(3)
     x = _cl(torch.randn(B, 3, H0, W0, generator=g, device=DEV).to(BF))
     lab = torch.randint(0, K, (B,), generator=g, device=DEV)
@@ -268,6 +292,7 @@ def test_eval_network_stage_by_stage(name, monkeypatch):
     assert [getattr(model, n.split(".")[0])[int(n.split(".")[1])] for n, *_ in mb] == blocks
     rec = _EvalRecorder(monkeypatch, keep_outputs=True)
     conv_rec = ConvRecorder(monkeypatch)
+    pad_rec = PadRecorder(monkeypatch, conv_rec.calls)
     info = [dict() for _ in blocks]
     hooks = []
     for i, blk in enumerate(blocks):
@@ -297,6 +322,10 @@ def test_eval_network_stage_by_stage(name, monkeypatch):
     check_eval_calls(calls, model, name)
     for j, r in enumerate(convs):
         check_torch_conv(r, "%s c%d" % (name, j))
+    blurs = blur_convs(convs, pad_rec.calls)
+    assert len(blurs) == (4 if mname.startswith("se_cotnetd_152") else 0), name
+    for j, p in blurs.items():
+        check_blur(convs[j], p, "%s c%d" % (name, j))
     # (3) the stem's output is block 0's input; block i's output (its last call's) is block i+1's input; input shapes
     n_stem = len(stem)
     assert info[0]["x_ptr"] == calls[n_stem - 1].out_ptr[0]

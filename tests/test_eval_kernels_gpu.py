@@ -74,8 +74,13 @@ def _conv_plan(C, H, B, bn):
 
 @pytest.mark.parametrize("case", CONV_CASES, ids=lambda c: "C%d-%dx%d-B%d-bn%d" % (c[0], c[1], c[1], c[2], c[3]))
 def test_key_conv_eval_epilogue_exact(case):
+    key_conv_exact(case, _conv_plan(*case))
+
+
+def key_conv_exact(case, plan):
+    """cotb200_conv3x3_bf16 on {-1, 0, 1} operands at (C, H, B, bn), with and without ReLU: torch.equal to the epilogue of the exact
+    accumulator, and the planned kernel ran"""
     C, H, B, bn = case
-    plan = _conv_plan(C, H, B, bn)
     print("key conv %s: %s" % (case, plan))
     g = _cpu_gen(C + H + B)
     cg = C // 4
@@ -112,8 +117,14 @@ GEMM_FORMS = {
 @pytest.mark.parametrize("stage", STAGES, ids=lambda s: "C%d-%dx%d" % (s[0], s[1], s[1]))
 def test_gemm_eval_epilogue_exact(stage, form):
     C, H = stage
+    gemm_exact(C, 3 * H * H, form)
+
+
+def gemm_exact(C, M, form, pad_cols=0):
+    """cotb200_gemm_bf16 in the epilogue form `form` of a dim-C CoT layer on M rows of {-1, 0, 1} operands: torch.equal to the
+    epilogue of the exact accumulator.  pad_cols > 0: D is the left part of a [M, N + pad_cols] buffer (ldd = N + pad_cols) whose
+    columns past N hold a pattern the kernel must leave as it is."""
     K1, K2, N, has_scale, has_shift, relu = GEMM_FORMS[form](C)
-    M = 3 * H * H
     g = _cpu_gen(C + K1 + N)
     a1, b1 = _ints((M, K1), -1, 1, g, BF), _ints((N, K1), -1, 1, g, BF)
     a2 = _ints((M, K2), -1, 1, g, BF) if K2 else None
@@ -121,17 +132,23 @@ def test_gemm_eval_epilogue_exact(stage, form):
     scale, shift = _scale_shift(N, g)
     scale = scale if has_scale else None
     shift = shift if has_shift else None
-    D = torch.full((M, N), float("nan"), dtype=BF, device=DEV)
+    ldd = N + pad_cols
+    buf = torch.full((M, ldd), float("nan"), dtype=BF, device=DEV)
+    if pad_cols:
+        buf[:, N:] = _ints((M, pad_cols), -100, 100, g, BF)
+    outside = buf[:, N:].clone()
     lib = _lib.load()
     with kernels_ran("tc_gemm_1x1"):
         _lib.check(lib.cotb200_gemm_bf16(M, N, K1, a1.data_ptr(), K1, b1.data_ptr(), K1, K2, _lib.ptr(a2), K2, _lib.ptr(b2), K2,
-                                         D.data_ptr(), N, _lib.ptr(scale), _lib.ptr(shift), 1 if relu else 0, None, None, _st()),
+                                         buf.data_ptr(), ldd, _lib.ptr(scale), _lib.ptr(shift), 1 if relu else 0, None, None, _st()),
                    "gemm_bf16")
     torch.cuda.synchronize()
     acc = a1.double() @ b1.double().t()
     if K2:
         acc = acc + a2.double() @ b2.double().t()
-    S.equal(D, S.epilogue_ref(acc, scale, shift, relu).to(BF), "gemm %s at C=%d (M=%d N=%d K=%d+%d)" % (form, C, M, N, K1, K2))
+    what = "gemm %s at C=%d (M=%d N=%d K=%d+%d ldd=%d)" % (form, C, M, N, K1, K2, ldd)
+    S.equal(buf[:, :N], S.epilogue_ref(acc, scale, shift, relu).to(BF), what)
+    S.equal(buf[:, N:], outside, what + ": columns past N")
 
 
 # ================================================================================================ cotb200_se_eval

@@ -16,7 +16,8 @@ def test_eval_call_lists_follow_the_mirror(geo):
 
 def _models():
     from cotnet_b200 import backbone, backbone_hybrid
-    return {"cotnet50": backbone.cotnet50(), "cotnext50_2x48d": backbone.cotnext50_2x48d(), "se_cotnetd_50": backbone_hybrid.se_cotnetd_50()}
+    return {"cotnet50": backbone.cotnet50(), "cotnext50_2x48d": backbone.cotnext50_2x48d(), "se_cotnetd_50": backbone_hybrid.se_cotnetd_50(),
+            "se_cotnetd_152": backbone_hybrid.se_cotnetd_152()}
 
 
 def test_eval_block_cases_match_the_models():
@@ -27,13 +28,13 @@ def test_eval_block_cases_match_the_models():
     for geo, c in S.EVAL_BLOCK_CASES.items():
         m = models[c["model"]]
         if c["kind"] == "stem":
-            assert isinstance(m.conv1, nn.Sequential) == (c["model"] == "se_cotnetd_50"), geo
+            assert isinstance(m.conv1, nn.Sequential) == (c["model"] in S.HYBRID), geo
             continue
         stage, i = c["block"].split(".")
         blk = getattr(m, stage)[int(i)]
         assert (blk.conv1.in_channels, blk.conv1.out_channels, blk.conv3.out_channels) == (c["cin"], c["width"], c["cout"]), geo
-        if c["model"] == "se_cotnetd_50":
-            assert isinstance(blk.conv2, SplitAttnConv2d) == S.hybrid_split(c["width"], int(i)), geo
+        if c["model"] in S.HYBRID:
+            assert isinstance(blk.conv2, SplitAttnConv2d) == S.hybrid_split(c["width"], int(i), c4_idx=S.HYBRID[c["model"]]["c4_idx"]), geo
             assert (2 if int(i) == 0 else 1) == c["stride"], geo
         else:
             assert isinstance(blk.conv2, CoXtLayer) == (c["model"] != "cotnet50") and blk.stride == c["stride"], geo
@@ -43,8 +44,8 @@ def test_eval_block_cases_match_the_models():
         assert c["H"] in sizes and c["W"] in sizes, geo
 
 
-@pytest.mark.parametrize("H0,W0", [(224, 224), (232, 200), (225, 225), (96, 72)])
-@pytest.mark.parametrize("model", ["cotnet50", "se_cotnetd_50"])
+@pytest.mark.parametrize("H0,W0", [(224, 224), (232, 200), (225, 225), (96, 72), (320, 320), (256, 256)])
+@pytest.mark.parametrize("model", ["cotnet50", "se_cotnetd_50", "se_cotnetd_152"])
 def test_model_blocks_follow_the_modules(model, H0, W0):
     """every block's input size in model_blocks is the one the trunk's own torch modules give, odd sizes included: a CPU forward of
     the trunk with its CoT layers (stride 1, shape-preserving, GPU-only kernels) replaced by identities"""
@@ -89,3 +90,21 @@ def test_eval_model_calls(model):
         assert blocks0[0][0] == "TcConv1x1Fn(one,relu)" and blocks0[0][-1] == "TcConv1x1Fn(one,relu+res)"
         assert stem0 == stem
     assert S.eval_model_calls("cotnet50", 2, 225, 225, True)[0] == ["BNActFn(relu)", "Pool3x3S2Fn(max)"]
+
+
+def test_eval_model_calls_se_cotnetd_152():
+    """se_cotnetd_152 at 320 and 256, B = 2: every CoT layer (the 18 even stage-3 blocks and stage 4) on the wgmma eval path, the
+    BlurPools are torch glue (no recorded pool), the CoT layers of layer3.0 / layer4.0 at the stage's input size"""
+    for res in (320, 256):
+        stem, blocks = S.eval_model_calls("se_cotnetd_152", 2, res, res, True)
+        assert len(blocks) == 50 and stem == ["BNActFn(relu)"] * 3
+        flat = sum(blocks, [])
+        assert flat.count("conv3x3_bf16") == 21 and flat.count("CotTailFn(gate)") == 29
+        assert not any(c.startswith("Pool3x3S2Fn") for c in flat)
+        assert blocks[11] == ["BNActFn(relu)"] + S.EVAL_LAYER_TC + ["GroupNorm9Fn(gc8)", "AggTapFn(fold1,gc8)", "cot_tail_eval",
+                                                                   "BNActFn(plain)", "BNActFn(relu+res)"]
+    # the stage-by-stage eval cases cover every key-conv geometry of the trunk at both sizes
+    geos = {(bl[3], bl[5]) for res in (320, 256) for bl in S.model_blocks("se_cotnetd_152", res)
+            if not S.hybrid_split(bl[3], bl[1], c4_idx=S.HYBRID["se_cotnetd_152"]["c4_idx"])}
+    cases = {(c["width"], c["H"]) for c in S.EVAL_BLOCK_CASES.values() if c["model"] == "se_cotnetd_152" and c["kind"] == "block"}
+    assert geos == {(256, 40), (256, 20), (512, 20), (512, 10), (256, 32), (256, 16), (512, 16), (512, 8)} and geos <= cases

@@ -312,7 +312,7 @@ def test_step_block_cases_match_the_models():
     from cotnet_b200.backbone_hybrid import SplitAttnConv2d
     from cotnet_b200.cot_layer import CoXtLayer
     models = {"cotnet50": backbone.cotnet50(drop_block_rate=0.1), "cotnext50_2x48d": backbone.cotnext50_2x48d(drop_block_rate=0.1),
-              "se_cotnetd_50": backbone_hybrid.se_cotnetd_50(drop_block_rate=0.1)}
+              "se_cotnetd_50": backbone_hybrid.se_cotnetd_50(drop_block_rate=0.1), "se_cotnetd_152": backbone_hybrid.se_cotnetd_152()}
     for geo, c in S.STEP_BLOCK_CASES.items():
         if c["kind"] != "block":
             continue
@@ -320,18 +320,62 @@ def test_step_block_cases_match_the_models():
         stage, i = c["block"].split(".")
         blk = getattr(m, stage)[int(i)]
         assert (blk.conv1.in_channels, blk.conv1.out_channels, blk.conv3.out_channels) == (c["cin"], c["width"], c["cout"]), geo
-        if c["model"] == "se_cotnetd_50":
-            assert isinstance(blk.conv2, SplitAttnConv2d) == S.hybrid_split(c["width"], int(i)), geo
+        if c["model"] in S.HYBRID:
+            assert isinstance(blk.conv2, SplitAttnConv2d) == S.hybrid_split(c["width"], int(i), c4_idx=S.HYBRID[c["model"]]["c4_idx"]), geo
             assert (2 if int(i) == 0 else 1) == c["stride"]
         else:
             assert isinstance(blk.conv2, CoXtLayer) == (c["model"] != "cotnet50") and blk.stride == c["stride"], geo
         if "sites" in c:
             assert blk.drop_block_sites == c["sites"], geo
-    # every se_cotnetd_50 block's conv2 kind follows the mirror
-    m = models["se_cotnetd_50"]
+        if c["model"] == "se_cotnetd_152":          # the input size the block sees in the named config
+            res = 320 if "_320_" in geo else 256
+            (H,) = [h for n, _, _, _, _, h, _, _ in S.model_blocks(c["model"], res) if n == c["block"]]
+            assert H == c["H"], geo
+    # every hybrid block's conv2 kind and pool follow the mirror
+    for name in ("se_cotnetd_50", "se_cotnetd_152"):
+        _check_hybrid_blocks(name, models[name])
+
+
+def _check_hybrid_blocks(name, m):
+    """conv2 kind (c4_idx), the pool of a stride-2 conv2 (BlurPool2d or the 3x3/s2 average pool; present on a split-attention
+    conv2 only with avd), avd_first and the deep stem's width: what stage_ref.HYBRID says of the trunk"""
+    from cotnet_b200.backbone_hybrid import BlurPool2d, SplitAttnConv2d
+    cfg = S.HYBRID[name]
+    assert m.conv1[0].out_channels == cfg["stem_width"] and m.bn1.num_features == 2 * cfg["stem_width"], name
+    assert tuple(len(getattr(m, "layer%d" % (s + 1))) for s in range(4)) == cfg["layers"], name
     for stage in ("layer1", "layer2", "layer3", "layer4"):
         for i, blk in enumerate(getattr(m, stage)):
-            assert isinstance(blk.conv2, SplitAttnConv2d) == S.hybrid_split(blk.conv1.out_channels, i), (stage, i)
+            split = S.hybrid_split(blk.conv1.out_channels, i, c4_idx=cfg["c4_idx"])
+            assert isinstance(blk.conv2, SplitAttnConv2d) == split, (name, stage, i)
+            pooled = i == 0 and (cfg["avd"] if split else True)
+            assert (blk.avd is not None) == pooled and blk.avd_first == cfg["avd_first"], (name, stage, i)
+            if pooled:
+                assert isinstance(blk.avd, BlurPool2d) == cfg["blur"], (name, stage, i)
+                assert isinstance(blk.avd, BlurPool2d) or (blk.avd.kernel_size, blk.avd.stride, blk.avd.padding) == (3, 2, 1)
+            if split:
+                assert blk.conv2.conv.stride == ((1, 1) if pooled or i else (2, 2)), (name, stage, i)
+
+
+def test_hybrid152_call_lists():
+    """se_cotnetd_152 at 320 and 256 through the training mirror: no recorded pool anywhere (every stride-2 conv2 is followed by a
+    BlurPool); the bench's bs64 step at 320 puts layer3.0's embed.3 and conv1x1 on wgmma (102400 pixels), at 256 it does not
+    (65536); one more pixel of threshold moves layer3.0 back; the CoT layers are the even stage-3 blocks and stage 4"""
+    for res, tc in ((320, True), (256, False)):
+        stem, blocks, _ = S.model_calls("se_cotnetd_152", 64, res, drop_block=False)
+        assert len(blocks) == 50 and stem == ["BNActFn(relu)"] * 3
+        flat = sum(blocks, [])
+        assert not any(c.startswith("Pool3x3S2Fn") for c in flat), res
+        assert flat.count("CotTailFn(k)") == 18 + 3 and flat.count("CotTailFn(gate)") == 3 + 8 + 18, res
+        l30 = blocks[3 + 8]
+        assert ("TcConv1x1Fn(one,nobn)" in l30 and "TcConv1x1Fn(one,bn)" in l30) == tc, (res, l30)
+        assert all("TcConv1x1Fn(one,nobn)" not in b for b in blocks[3 + 8 + 1:]), res
+    l30 = S.model_calls("se_cotnetd_152", 64, 320, 102401, drop_block=False)[1][11]
+    assert "TcConv1x1Fn(one,nobn)" not in l30 and l30[0] == "BNActFn(relu)"
+    l30 = S.model_calls("se_cotnetd_152", 64, 320, 102400, drop_block=False)[1][11]
+    assert "TcConv1x1Fn(one,nobn)" in l30 and l30[0] == "TcConv1x1Fn(one,relu)"
+    # the CoT layers of layer3.0 / layer4.0 run before the pool: at the stage's input size
+    mb = {n: (H, s) for n, _, _, _, _, H, _, s in S.model_blocks("se_cotnetd_152", 320)}
+    assert mb["layer1.0"] == (160, 2) and mb["layer3.0"] == (40, 2) and mb["layer4.0"] == (20, 2) and mb["layer4.1"] == (10, 1)
 
 
 @pytest.mark.parametrize("groups,shape", [(2, (48, 96, 1, 1)), (8, (96, 12, 3, 3)), (2, (96, 48, 1, 1))])
@@ -378,3 +422,18 @@ def test_coxt_embed0_adjoint_matches_autograd(C):
     want = F.conv2d(qk, w, groups=G)
     got = torch.einsum("bchw,nc->bnhw", x, wx) + torch.einsum("bchw,nc->bnhw", k, wk)
     assert torch.allclose(got, want, rtol=0, atol=1e-12)
+
+
+@pytest.mark.parametrize("H,W", [(2, 2), (3, 5), (8, 7), (40, 40)])
+def test_blurpool_reflect_padding_matches_torch(H, W):
+    """BlurPool2d's padding: the values of F.pad(mode="reflect") and, bit for bit in fp64, the gradient autograd gives through it"""
+    from cotnet_b200.backbone_hybrid import _ReflectPad1
+    g = torch.Generator().manual_seed(H * 100 + W)
+    x = torch.randn(2, 3, H, W, generator=g, dtype=torch.float64, requires_grad=True)
+    dy = torch.randn(2, 3, H + 2, W + 2, generator=g, dtype=torch.float64)
+    want = F.pad(x, (1, 1, 1, 1), mode="reflect")
+    got = _ReflectPad1.apply(x)
+    assert torch.equal(got, want)
+    (gw,) = torch.autograd.grad(want, x, dy)
+    (gg,) = torch.autograd.grad(got, x, dy)
+    assert torch.allclose(gg, gw, rtol=0, atol=1e-12)

@@ -748,6 +748,73 @@ class ConvRecorder:
         monkeypatch.setattr(torch.nn.functional, "conv2d", conv2d)
 
 
+class PadRecorder:
+    """F.pad calls that are not zero padding (the BlurPool's reflect padding; the library zero-pads elsewhere) with input (and its
+    storage), output storage and `conv`: the index in `convs` (a ConvRecorder's list) of the next torch convolution, the one that
+    reads the padded tensor"""
+
+    def __init__(self, monkeypatch, convs):
+        self.calls = []
+        pad0 = F.pad
+
+        def pad(input, pad, mode="constant", value=None):
+            out = pad0(input, pad, mode, value)
+            if mode != "constant":
+                self.calls.append(dict(x=input.detach().clone(), ptr=input.data_ptr(), pad=tuple(pad), mode=mode,
+                                       out_ptr=out.data_ptr(), conv=len(convs)))
+            return out
+        monkeypatch.setattr(torch.nn.functional, "pad", pad)
+
+
+#: backbone_hybrid.BlurPool2d's filter, [1,2,1] x [1,2,1] / 16 (models/layers/blur_pool.py with filt_size 3)
+BLUR_TAPS = torch.tensor([1.0, 2.0, 1.0], dtype=torch.float64) / 4
+
+
+def blur_convs(convs, pads):
+    """{j: pad record} for every torch convolution j that reads a recorded F.pad output: the BlurPools"""
+    out = {}
+    for p in pads:
+        j = p["conv"]
+        assert j < len(convs) and convs[j]["ptr"] == p["out_ptr"], "an F.pad whose output no torch convolution read next"
+        out[j] = p
+    return out
+
+
+def check_blur(r, p, what, producer=None):
+    """a BlurPool: the reflect padding by 1 and the stride-2 depthwise [1,2,1] x [1,2,1] / 16 convolution, its output against fp64 of
+    that filter on the reflect-padded recorded input (the weight the module passes must be the filter, exactly); with `producer`
+    (the recorded call whose output the pad read), the gradient autograd delivered to that output against fp64 of the convolution's
+    data gradient (fp32 chain of at most 9 terms, bf16 store) pulled back through the padding (up to 4 bf16 adds per element)"""
+    x = p["x"]
+    C = x.shape[1]
+    assert p["mode"] == "reflect" and p["pad"] == (1, 1, 1, 1), what + ": %s padding %s" % (p["mode"], p["pad"])
+    assert (r["stride"], r["padding"], r["groups"]) in (((2, 2), (0, 0), C), (2, 0, C)), what + ": %s" % ((r["stride"], r["padding"],
+                                                                                                            r["groups"]),)
+    filt = (BLUR_TAPS[:, None] * BLUR_TAPS[None, :]).to(DEV)
+    S.equal(r["w"].detach().double(), filt.expand(C, 1, 3, 3), what + ": the BlurPool filter")
+    xp = F.pad(x.double(), (1, 1, 1, 1), mode="reflect")
+    S.equal(r["x"].double(), xp, what + ": the convolution's input is the reflect padding of the pad's input")
+    w = filt.expand(C, 1, 3, 3)
+    ref = F.conv2d(xp, w, stride=2, groups=C)
+    mag = F.conv2d(xp.abs(), w, stride=2, groups=C)
+    _w(r["y"], ref, S.gamma_tc(10) * mag, what + " BlurPool output", "blur_pool")
+    if producer is None:
+        return
+    g = r["g"]
+    assert g is not None, what + ": the BlurPool's output received no gradient"
+    shp = tuple(xp.shape)
+    gp = torch.nn.grad.conv2d_input(shp, w, g.double(), stride=2, groups=C)
+    e_gp = S.store_bound(gp, S.gamma_tc(10) * torch.nn.grad.conv2d_input(shp, w, g.double().abs(), stride=2, groups=C), BF)
+
+    def unpad(t):                                   # the adjoint of the reflect padding: a sum with non-negative weights
+        x64 = torch.zeros(x.shape, dtype=torch.float64, device=DEV, requires_grad=True)
+        (d,) = torch.autograd.grad(F.pad(x64, (1, 1, 1, 1), mode="reflect"), x64, t)
+        return d
+    ref = unpad(gp)
+    err = unpad(e_gp) + S.gamma_bf16(3) * unpad(gp.abs() + e_gp)
+    S.within(producer.gin[0], ref, err, what + " gradient at the BlurPool's input (through the reflect padding)")
+
+
 class TorchBNRecorder:
     """F.batch_norm calls in training mode (BatchNorms the glue runs in plain PyTorch: the split-attention gate's bn1 when DropBlock
     sits after bn0) with input, weight, bias and the gradient of the output"""

@@ -20,8 +20,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 import stage_ref as S
-from test_stage_grads_gpu import ONE_ULP, ConvRecorder, TorchBNRecorder, _cfg, account_params, check_call, check_dropblock, \
-    check_dropblock_res_relu, tail_mods, torch_bn_bwd_ref
+from test_stage_grads_gpu import ONE_ULP, ConvRecorder, PadRecorder, TorchBNRecorder, _cfg, account_params, blur_convs, check_blur, \
+    check_call, check_dropblock, check_dropblock_res_relu, tail_mods, torch_bn_bwd_ref
 from cotnet_b200 import _lib, dropblock, fused
 
 pytestmark = pytest.mark.gpu
@@ -90,7 +90,7 @@ def _model(case):
     from cotnet_b200 import backbone, backbone_hybrid
     torch.manual_seed(5)
     ctor = {"cotnet50": backbone.cotnet50, "cotnext50_2x48d": backbone.cotnext50_2x48d,
-            "se_cotnetd_50": backbone_hybrid.se_cotnetd_50}[case["model"]]
+            "se_cotnetd_50": backbone_hybrid.se_cotnetd_50, "se_cotnetd_152": backbone_hybrid.se_cotnetd_152}[case["model"]]
     return ctor(drop_block_rate=0.1 if case.get("sites") else 0.0)
 
 
@@ -189,43 +189,63 @@ def check_split_gate(blk, db_call, hk, convs, bns, what):
              what + " gate: gradient reaching the DropBlock output")
 
 
-def observed_flow(calls, convs, x_ptr, x):
+def observed_flow(calls, convs, x_ptr, x, blurs=None, order=None):
     """every recorded call argument and torch convolution input that is (by storage, shape and value) an earlier recorded call's
-    output or the block input x: {"i.a" or "c<j>": "k.o" or "x"}"""
+    output or the block input x: {"i.a" or "c<j>": "k.o" or "x"}.  blurs ({conv index: pad record}, with `order`): a BlurPool's output
+    is a producer too ("c<j>"), and its convolution reads "pad(k.o)", the reflect padding of a recorded output."""
     ptrs = {}
+    # times: call i at (i, 1, 0); torch convolution j, made after order[j] recorded calls, at (order[j], 0, j)
     for i, c in enumerate(calls):
         for o, (pt, snap) in enumerate(zip(c.out_ptr, c.out if isinstance(c.out, tuple) else (c.out,))):
-            ptrs.setdefault(pt, []).append(("%d.%d" % (i, o), i, snap))
+            ptrs.setdefault(pt, []).append(("%d.%d" % (i, o), (i, 1, 0), snap))
     if x is not None:
-        ptrs.setdefault(x_ptr, []).append(("x", -1, x.detach()))
+        ptrs.setdefault(x_ptr, []).append(("x", (-1, 1, 0), x.detach()))
+    for j in sorted(blurs or ()):
+        r = convs[j]
+        ptrs.setdefault(r["out_ptr"], []).append(("c%d" % j, (order[j], 0, j), r["y"]))
     edges = {}
 
-    def find(ptr, shape, val, upto):
-        cands = [(n, sn) for n, i, sn in ptrs.get(ptr, []) if i < upto and tuple(sn.shape) == shape]
+    def find(ptr, shape, val, t):
+        cands = sorted([(tp, n, sn) for n, tp, sn in ptrs.get(ptr, []) if tp < t and tuple(sn.shape) == shape], key=lambda e: e[0])
         if not cands:
             return None
-        n, sn = cands[-1]                                    # the latest producer at that storage
+        _, n, sn = cands[-1]                                 # the latest producer at that storage
         S.equal(val, sn, "%s == %s" % ("consumer", n))
         return n
     for i, c in enumerate(calls):
         for a, arg in enumerate(c.args):
             if isinstance(arg, torch.Tensor):
-                n = find(arg.data_ptr(), tuple(arg.shape), c.inp[a], i)
+                n = find(arg.data_ptr(), tuple(arg.shape), c.inp[a], (i, 1, 0))
                 if n is not None:
                     edges["%d.%d" % (i, a)] = n
     return edges, ptrs
 
 
-def _conv_edges(convs, ptrs, order):
-    """torch convolution inputs produced by recorded calls: order[j] is the number of recorded calls made before conv j"""
+def _conv_edges(convs, ptrs, order, blurs=None):
+    """torch convolution inputs produced by recorded calls (or by a BlurPool): order[j] is the number of recorded calls made before
+    conv j; a BlurPool's convolution reads the padding of its producer's output ("pad(k.o)")"""
     edges = {}
     for j, r in enumerate(convs):
-        cands = [(n, sn) for n, i, sn in ptrs.get(r["ptr"], []) if i < order[j] and tuple(sn.shape) == tuple(r["x"].shape)]
+        src = (blurs or {}).get(j)
+        ptr, val = (src["ptr"], src["x"]) if src is not None else (r["ptr"], r["x"])
+        cands = sorted([(tp, n, sn) for n, tp, sn in ptrs.get(ptr, []) if tp < (order[j], 0, j) and tuple(sn.shape) == tuple(val.shape)],
+                       key=lambda e: e[0])
         if cands:
-            n, sn = cands[-1]
-            S.equal(r["x"], sn, "c%d == %s" % (j, n))
-            edges["c%d" % j] = n
+            _, n, sn = cands[-1]
+            S.equal(val, sn, "c%d == %s" % (j, n))
+            edges["c%d" % j] = "pad(%s)" % n if src is not None else n
     return edges
+
+
+def blur_producers(calls, convs, blurs, order):
+    """{conv index: the recorded call whose output the BlurPool's pad read} (the latest at that storage before the pad)"""
+    out = {}
+    for j, p in blurs.items():
+        cands = [c for i, c in enumerate(calls) if i < order[j] and c.out_ptr[0] == p["ptr"] and tuple(c.out.shape if not
+                 isinstance(c.out, tuple) else c.out[0].shape) == tuple(p["x"].shape)]
+        assert cands, "c%d: the BlurPool's input is no recorded call's output" % j
+        out[j] = cands[-1]
+    return out
 
 
 class _Order:
@@ -291,6 +311,7 @@ def test_block_stage_by_stage(geo, monkeypatch):
         _gate_hooks(part, hooks)
     rec = S.Recorder(monkeypatch)
     convs = ConvRecorder(monkeypatch).calls
+    pads = PadRecorder(monkeypatch, convs).calls
     bns = TorchBNRecorder(monkeypatch).calls
     order = _Order(monkeypatch, rec).order
     derived = S.DerivedRecorder(monkeypatch).of
@@ -323,14 +344,19 @@ def test_block_stage_by_stage(geo, monkeypatch):
         _check_input_grad(x, x.grad, rec.calls, convs, hooks.get("pool"), geo)
     if gate:
         check_split_gate(part, dbc[1], hooks, convs, bns, geo)
+    # the BlurPools (se_cotnetd_152): output against fp64 of the filter on the reflect-padded input, the gradient reaching their input
+    blurs = blur_convs(convs, pads)
+    for j, prod in blur_producers(rec.calls, convs, blurs, order).items():
+        check_blur(convs[j], blurs[j], "%s c%d" % (geo, j), prod)
+    assert len(blurs) == (1 if case["model"] == "se_cotnetd_152" and case.get("stride") == 2 else 0), geo
     # (e)
     account_params(part, rec.calls, convs, geo, derived, bns=bns)
     if case["model"] == "cotnext50_2x48d":
         assert len(derived) == 4, "CoXt: key conv, embed.0, embed.3 and conv1x1 weights derive dense weights"
     # (f) the stated dataflow: every recorded input (call argument or torch convolution input) that is an earlier call's output or
     # the block input, and nothing else
-    edges, ptrs = observed_flow(rec.calls, convs, x.data_ptr(), x if case["kind"] == "block" else None)
-    edges.update(_conv_edges(convs, ptrs, order))
+    edges, ptrs = observed_flow(rec.calls, convs, x.data_ptr(), x if case["kind"] == "block" else None, blurs, order)
+    edges.update(_conv_edges(convs, ptrs, order, blurs))
     got = sorted("%s<-%s" % kv for kv in edges.items())
     assert got == sorted(case.get("flow", ())), "%s dataflow: %s" % (geo, got)
 
@@ -420,14 +446,21 @@ def test_train_step_stage_by_stage(name, monkeypatch):
     and DropBlock 0.1 (fixed key): (1) the call list, (2) every block's drop-path row and DropBlock sites, (3) every stage check,
     (4) block-to-block dataflow, (5) the gradient at every block input and at the last block's output as the sum of its
     consumers', (6) the head, (7) the flat buckets against .grad and every parameter accounted for"""
-    from cotnet_b200 import backbone, backbone_hybrid, trainer
     mname, mp = TRAIN_CASES[name]
+    train_step_stage_by_stage(name, mname, mp, monkeypatch)
+
+
+def train_step_stage_by_stage(name, mname, mp, monkeypatch, B=4, H0=96, drop_path=0.1, drop_block=0.1):
+    """the body of test_train_step_stage_by_stage for any model, batch, image size and rates (drop_block 0: no DropBlock); the
+    BlurPools of se_cotnetd_152 are checked as in test_block_stage_by_stage"""
+    from cotnet_b200 import backbone, backbone_hybrid, trainer
     if mp is not None:
         monkeypatch.setattr(fused, "TC_MIN_PIXELS", mp)
     torch.manual_seed(5)
-    K, B, H0 = 100, 4, 96
-    ctor = {"cotnet50": backbone.cotnet50, "cotnext50_2x48d": backbone.cotnext50_2x48d, "se_cotnetd_50": backbone_hybrid.se_cotnetd_50}
-    model = ctor[mname](num_classes=K, drop_path_rate=0.1, drop_block_rate=0.1)
+    K = 100
+    ctor = {"cotnet50": backbone.cotnet50, "cotnext50_2x48d": backbone.cotnext50_2x48d, "se_cotnetd_50": backbone_hybrid.se_cotnetd_50,
+            "se_cotnetd_152": backbone_hybrid.se_cotnetd_152}
+    model = ctor[mname](num_classes=K, drop_path_rate=drop_path, drop_block_rate=drop_block)
     _randomise_bn(model)
     model = model.to(DEV).to(memory_format=CL).train()
     scales = _fixed_scales(model, B)
@@ -439,7 +472,9 @@ def test_train_step_stage_by_stage(name, monkeypatch):
     assert [getattr(model, n.split(".")[0])[int(n.split(".")[1])] for n in names] == blocks
     rec = S.Recorder(monkeypatch)
     convs = ConvRecorder(monkeypatch).calls
+    pads = PadRecorder(monkeypatch, convs).calls
     bns = TorchBNRecorder(monkeypatch).calls
+    order = _Order(monkeypatch, rec).order
     derived = S.DerivedRecorder(monkeypatch).of
     info = [dict() for _ in blocks]
     for i, blk in enumerate(blocks):
@@ -466,13 +501,13 @@ def test_train_step_stage_by_stage(name, monkeypatch):
     lab = torch.randint(0, K, (B,), generator=g, device=DEV)
     ts.forward_backward(x, lab)
     # (1)
-    stem, bl, loss_calls = S.model_calls(mname, B, H0, S.TC_MIN_PIXELS if mp is None else mp)
+    stem, bl, loss_calls = S.model_calls(mname, B, H0, S.TC_MIN_PIXELS if mp is None else mp, drop_block > 0)
     cfgs = [_cfg(c) for c in rec.calls]
     assert cfgs == stem + sum(bl, []) + loss_calls, cfgs
     for i in range(len(blocks)):
         assert cfgs[info[i]["c0"]:info[i]["c1"]] == bl[i], (names[i], cfgs[info[i]["c0"]:info[i]["c1"]])
     # (2) drop path and DropBlock per block
-    sites = S.model_sites(mname)
+    sites = S.model_sites(mname) if drop_block > 0 else {}
     table = {}
     for bname, _, site, _ in model.drop_block_table():
         table.setdefault(bname, []).append(site)
@@ -507,6 +542,11 @@ def test_train_step_stage_by_stage(name, monkeypatch):
         prod = rec.calls[n_stem - 1] if i == 0 else rec.calls[info[i - 1]["c1"] - 1]
         _check_input_grad(info[i]["x"], prod.gin[0], rec.calls[info[i]["c0"]:info[i]["c1"]], convs[info[i]["v0"]:info[i]["v1"]],
                           info[i].get("pool"), "%s %s" % (name, names[i]))
+    # every BlurPool: its output, and the gradient reaching its input, against fp64 (the pooled blocks of se_cotnetd_152)
+    blurs = blur_convs(convs, pads)
+    for j, prod in blur_producers(rec.calls, convs, blurs, order).items():
+        check_blur(convs[j], blurs[j], "%s c%d" % (name, j), prod)
+    assert len(blurs) == (4 if mname == "se_cotnetd_152" else 0), name
     # (6) head: global average pool -> fc -> loss
     (ce,) = rec.named("SoftTargetCrossEntropyFn")
     dz = ce.gout[0].double()
