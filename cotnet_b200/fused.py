@@ -16,8 +16,8 @@ from torch.autograd import Function
 from . import _lib
 
 #: ReLU mask of the BatchNorm backward without reading y back: with a residual the forward also writes a 1-bit mask (relu
-#: code 3), without one the wgmma functions recompute it from their own pre-activation and scale/shift (relu code 2).
-#: False takes the y-reading path, which gives the same bits; it is read at call time so tests can compare the two.
+#: code 3), without one it is recomputed from the pre-activation and the row kernel's own scale/shift (relu code 2; see
+#: _bn_epilogue).  False takes the y-reading path, which gives the same bits; it is read at call time so tests can compare the two.
 BN_MASK = True
 
 
@@ -147,20 +147,23 @@ def _bn_running_writeback(bn, update, rm, rv):
             bn.running_var.copy_(rv)
 
 
-def _bn_prepare(bn, weight, bias, C, n, sums, device, st):
-    """[4, C] fp32 = (scale, shift, mean, rstd) in ONE launch (cotb200_bn_finalize).  `sums` = [2, C] column sums of the
-    batch (training mode) or None (eval: running statistics).  Training updates the module's running buffers exactly like
-    nn.BatchNorm2d (momentum, unbiased variance, num_batches_tracked)."""
-    lib = _lib.load()
-    out = torch.empty(4, C, dtype=torch.float32, device=device)
+def _bn_eval_fold(bn, weight, bias, sums=None, n=1.0):
+    """[4, C] fp32 = (scale, shift, mean, rstd) of the module's running statistics (eval mode) in ONE launch
+    (cotb200_bn_finalize), which does not read n.  With `sums` = [2, C] column sums of the n rows of a batch (CotTailFn in
+    training) the batch statistics instead, and the running buffers updated exactly like nn.BatchNorm2d (momentum, unbiased
+    variance, num_batches_tracked)."""
     use_batch = sums is not None
+    src = sums if use_batch else bn.running_mean
+    C = src.shape[-1]
+    out = torch.empty(4, C, dtype=torch.float32, device=src.device)
     update, mom, rm, rv = _bn_running(bn, use_batch)
-    w32 = None if weight is None else weight.detach().float().contiguous()
-    b32 = None if bias is None else bias.detach().float().contiguous()
-    _lib.check(lib.cotb200_bn_finalize(C, _lib.ptr(sums[0]) if use_batch else None, _lib.ptr(sums[1]) if use_batch else None,
-                                       _lib.ptr(w32), _lib.ptr(b32), _lib.ptr(rm), _lib.ptr(rv), float(n), float(bn.eps),
-                                       float(mom), 1 if use_batch else 0, 1 if update else 0, out[0].data_ptr(),
-                                       out[1].data_ptr(), out[2].data_ptr(), out[3].data_ptr(), st), "bn_finalize")
+    w32 = None if weight is None else _f32(weight)
+    b32 = None if bias is None else _f32(bias)
+    _lib.check(_lib.load().cotb200_bn_finalize(C, _lib.ptr(sums[0]) if use_batch else None, _lib.ptr(sums[1]) if use_batch else None,
+                                               _lib.ptr(w32), _lib.ptr(b32), _lib.ptr(rm), _lib.ptr(rv), float(n), float(bn.eps),
+                                               float(mom), 1 if use_batch else 0, 1 if update else 0, out[0].data_ptr(),
+                                               out[1].data_ptr(), out[2].data_ptr(), out[3].data_ptr(), _lib.stream_ptr(src)),
+               "bn_finalize")
     _bn_running_writeback(bn, update, rm, rv)
     return out
 
@@ -171,8 +174,8 @@ def _bn_batch_stats(x, bn, weight, bias, lib, st, dt):
     if bn.training or bn.running_mean is None:
         sums = _zeros((2, C,), x.device)
         _lib.check(lib.cotb200_col_stats(dt, B, H * W, C, x.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(), st), "col_stats")
-        return _bn_prepare(bn, weight, bias, C, float(B * H * W), sums, x.device, st), True
-    return _bn_prepare(bn, weight, bias, C, float(B * H * W), None, x.device, st), False
+        return _bn_eval_fold(bn, weight, bias, sums, float(B * H * W)), True
+    return _bn_eval_fold(bn, weight, bias), False
 
 
 def _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds=None, mask=None):
@@ -215,55 +218,88 @@ def _bn_bwd(lib, dt, B, HW, C, dy, x, y, scale, shift, mean, rstd, rcode, sums, 
                                         rcode, dx.data_ptr(), _lib.ptr(dres), _lib.ptr(ds), st), "bn_bwd_apply")
 
 
+def _bn_epilogue(ctx, out, produce, bn, weight, bias, relu, res=None, drop_scale=None):
+    """out = act(BatchNorm2d(pre) (+ res)), the BatchNorm that ends BNActFn and the wgmma functions, with bn's train / eval
+    semantics; drop_scale: None or the [B] per-sample drop-path scales applied to the BatchNorm output before the residual add.
+    `produce` makes pre: a tensor that already holds it (BNActFn's x: the column sums come from cotb200_col_stats), or a
+    callable produce(dst, stats=None, scale=None, shift=None, relu=False) that writes its output into dst with the column sums
+    added into stats = (sum, sq), or with act(pre*scale + shift) applied in its epilogue.
+      training: column sums, then ONE kernel that finalises the statistics in its prologue and applies them (_bn_apply_batch),
+                with the 1-bit ReLU mask when a residual is added;
+      eval:     the running statistics folded into the producer's epilogue, or -- with a residual, drop-path scales or no
+                epilogue -- cotb200_bn_apply on the raw pre; a raw pre the backward needs is computed as well.
+    Returns the tensors _bn_epilogue_bwd takes, (pre, y | mask | None, ss, ds), for ctx.save_for_backward; the rest of the
+    configuration goes to ctx.bn_cfg."""
+    B, C, H, W = out.shape
+    lib, st, dt = _lib.load(), _lib.stream_ptr(out), _lib.dtype_code(out)
+    res = None if res is None else res.detach()
+    ds = _drop_scale(drop_scale, out)
+    epilogue = callable(produce)
+    pre = None if epilogue else produce
+    batch = bool(bn.training or bn.running_mean is None)
+    mask = None
+    row = True                                # the row kernel writes out, not the producer's epilogue
+    if batch:
+        sums = _zeros((2, C,), out.device)
+        if epilogue:
+            pre = torch.empty_like(out, memory_format=torch.channels_last)
+            produce(pre, stats=(sums[0], sums[1]))
+        else:
+            _lib.check(lib.cotb200_col_stats(dt, B, H * W, C, pre.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(), st), "col_stats")
+        mask = _relu_mask_buf(pre) if (relu and res is not None) else None
+        ss = _bn_apply_batch(pre, res, sums, bn, weight, bias, relu, out, lib, st, dt, ds, mask)   # [4,C]: scale, shift, mean, rstd
+    else:
+        ss = _bn_eval_fold(bn, weight, bias)
+        row = not epilogue or res is not None or ds is not None
+        if not row:
+            produce(out, scale=ss[0], shift=ss[1], relu=relu)
+        if pre is None and (row or any(ctx.needs_input_grad)):
+            pre = torch.empty_like(out, memory_format=torch.channels_last)
+            produce(pre)
+        if row:
+            _lib.check(lib.cotb200_bn_apply(dt, B, H * W, C, pre.data_ptr(), _lib.ptr(res), ss[0].data_ptr(), ss[1].data_ptr(),
+                                            1 if relu else 0, out.data_ptr(), _lib.ptr(ds), st), "bn_apply")
+    # ReLU mask of the backward: the 1-bit mask the forward wrote (relu code 3); without a residual, recomputed from pre and the
+    # row kernel's own scale/shift (relu code 2: a convolution epilogue applies them to its fp32 accumulator, not to the stored
+    # pre); else read back from y (relu code 1)
+    rcode = 0 if not relu else (3 if mask is not None else (2 if (BN_MASK and res is None and row) else 1))
+    ctx.bn_cfg = (rcode, batch, res is not None, None if weight is None else weight.dtype, None if bias is None else bias.dtype)
+    return pre, (mask if rcode == 3 else (out if rcode == 1 else None)), ss, ds
+
+
+def _bn_epilogue_bwd(ctx, dy, pre, y, ss, ds, i_weight, i_res=None):
+    """Backward of _bn_epilogue from the tensors it returned: (dpre, dweight, dbias, dres).  i_weight: the position of the
+    BatchNorm weight among the autograd function's inputs (its bias follows), i_res: that of the residual.  The parameter
+    gradients are the column sums of the backward, which run when the batch statistics or a parameter gradient need them."""
+    rcode, batch, has_res, wdt, bdt = ctx.bn_cfg
+    need_w, need_b = ctx.needs_input_grad[i_weight], ctx.needs_input_grad[i_weight + 1]
+    B, C, H, W = pre.shape
+    lib, st, dt = _lib.load(), _lib.stream_ptr(pre), _lib.dtype_code(pre)
+    sums = torch.zeros(2, C, dtype=torch.float32, device=pre.device) if (batch or need_w or need_b) else None  # escapes as dgamma/dbeta
+    dpre = torch.empty_like(pre, memory_format=torch.channels_last)
+    dres = torch.empty_like(pre, memory_format=torch.channels_last) if (has_res and ctx.needs_input_grad[i_res]) else None
+    _bn_bwd(lib, dt, B, H * W, C, dy, pre, y, ss[0], ss[1], ss[2], ss[3], rcode, sums, batch, 1.0 / (B * H * W), dpre, dres, ds, st)
+    return dpre, (sums[1].to(wdt) if need_w else None), (sums[0].to(bdt) if need_b else None), dres
+
+
 class BNActFn(Function):
-    """y = act(BatchNorm2d(x) (+ res)) on channels_last tensors: col_stats + bn_finalize + bn_apply forward,
-    bn_bwd_sums + bn_bwd_apply backward.  Replaces the nn.BatchNorm2d / nn.ReLU (/ residual add) modules of
-    models/cotnet.py:45-46,53-54,61-62 and :231-235,:249-262 -- ATen's channels_last batch-norm kernels are the largest
-    single cost of the eager step.  drop_scale: None or [B] per-sample stochastic-depth scales (models/cotnet.py:256-257),
-    y = act(drop_scale[b]*BatchNorm2d(x) (+ res)) in the same kernels."""
+    """y = act(BatchNorm2d(x) (+ res)) on channels_last tensors: col_stats + bn_apply_batch (training) or bn_finalize +
+    bn_apply (eval) forward, bn_bwd_sums + bn_bwd_apply backward (_bn_epilogue).  Replaces the nn.BatchNorm2d / nn.ReLU
+    (/ residual add) modules of models/cotnet.py:45-46,53-54,61-62 and :231-235,:249-262 -- ATen's channels_last batch-norm
+    kernels are the largest single cost of the eager step.  drop_scale: None or [B] per-sample stochastic-depth scales
+    (models/cotnet.py:256-257), y = act(drop_scale[b]*BatchNorm2d(x) (+ res)) in the same kernels."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, res, bn, relu, drop_scale=None):
         assert _is_cl(x) and (res is None or (_is_cl(res) and res.dtype == x.dtype and res.shape == x.shape))
-        B, C, H, W = x.shape
-        lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.dtype_code(x)
         x = x.detach()
-        ds = _drop_scale(drop_scale, x)
         y = torch.empty_like(x, memory_format=torch.channels_last)
-        batch = bool(bn.training or bn.running_mean is None)
-        mask = None
-        if batch:       # training: column sums, then ONE kernel that finalises the statistics in its prologue and applies them
-            sums = _zeros((2, C,), x.device)
-            _lib.check(lib.cotb200_col_stats(dt, B, H * W, C, x.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(), st), "col_stats")
-            mask = _relu_mask_buf(x) if (relu and res is not None) else None
-            ss = _bn_apply_batch(x, res, sums, bn, weight, bias, relu, y, lib, st, dt, ds, mask)   # [4,C]: scale, shift, mean, rstd
-        else:
-            ss = _bn_prepare(bn, weight, bias, C, float(B * H * W), None, x.device, st)
-            _lib.check(lib.cotb200_bn_apply(dt, B, H * W, C, x.data_ptr(), _lib.ptr(res), ss[0].data_ptr(), ss[1].data_ptr(),
-                                            1 if relu else 0, y.data_ptr(), _lib.ptr(ds), st), "bn_apply")
-        # ReLU mask in the backward: with a residual it comes from the 1-bit mask the forward wrote (relu code 3) or from y;
-        # without one it is recomputed from x and the forward's own scale/shift (relu code 2) and y is neither saved nor read
-        rcode = 0 if not relu else (2 if res is None else (3 if mask is not None else 1))
-        ctx.save_for_backward(x, mask if rcode == 3 else (y if rcode == 1 else None), ss, ds)
-        ctx.cfg = (rcode, batch, res is not None, weight.dtype, bias.dtype)
+        ctx.save_for_backward(*_bn_epilogue(ctx, y, x, bn, weight, bias, relu, res, drop_scale))
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, y, ss, ds = ctx.saved_tensors          # y: the forward output (rcode 1), its 1-bit ReLU mask (rcode 3) or None
-        rcode, batch, has_res, wdt, bdt = ctx.cfg
-        B, C, H, W = x.shape
-        lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.dtype_code(x)
-        dy = dy.contiguous(memory_format=torch.channels_last)
-        sums = None
-        if batch or ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            sums = torch.zeros(2, C, dtype=torch.float32, device=x.device)  # escapes as dgamma/dbeta
-        dx = torch.empty_like(x, memory_format=torch.channels_last)
-        dres = torch.empty_like(x, memory_format=torch.channels_last) if (has_res and ctx.needs_input_grad[3]) else None
-        _bn_bwd(lib, dt, B, H * W, C, dy, x, y, ss[0], ss[1], ss[2], ss[3], rcode, sums, batch, 1.0 / float(B * H * W), dx, dres, ds,
-                st)
-        dgamma = sums[1].to(wdt) if ctx.needs_input_grad[1] else None
-        dbeta = sums[0].to(bdt) if ctx.needs_input_grad[2] else None
+        dx, dgamma, dbeta, dres = _bn_epilogue_bwd(ctx, dy.contiguous(memory_format=torch.channels_last), *ctx.saved_tensors, 1, 3)
         return dx, dgamma, dbeta, dres, None, None, None
 
 
@@ -604,7 +640,7 @@ def _cot_tail_eval_stages(u, k, bn, se):
     """_cot_tail_eval with its intermediates: (ss [4, C] = the BatchNorm fold, psum [B, C], a [B, C, 2], out)."""
     B, C, H, W = u.shape
     lib, st, dt = _lib.load(), _lib.stream_ptr(u), _lib.dtype_code(u)
-    ss = _bn_prepare(bn, bn.weight, bn.bias, C, float(B * H * W), None, u.device, st)
+    ss = _bn_eval_fold(bn, bn.weight, bn.bias)
     psum = torch.zeros(B, C, dtype=torch.float32, device=u.device)
     _lib.check(lib.cotb200_tail_pool(dt, B, H * W, C, u.data_ptr(), k.data_ptr(), ss[0].data_ptr(), ss[1].data_ptr(), psum.data_ptr(), st),
                "tail_pool")
@@ -656,12 +692,6 @@ def _rows2d(t):
     return t.permute(0, 2, 3, 1).reshape(B * H * W, C)
 
 
-def _bn_eval_fold(bn, weight, bias):
-    ss = _bn_prepare(bn, weight, bias, weight.shape[0], 1.0, None, weight.device,
-                     torch.cuda.current_stream(weight.device).cuda_stream)
-    return ss[0], ss[1], ss[2], ss[3]
-
-
 class TcConv1x1Fn(Function):
     """y = act(BN(conv1x1([a1 ; a2]))) or a bias-free conv1x1 without BatchNorm or ReLU, on channels_last bf16 activations.
 
@@ -678,65 +708,32 @@ class TcConv1x1Fn(Function):
         B, K1, H, W = a1.shape
         K2 = 0 if a2 is None else a2.shape[1]
         N = weight.shape[0]
-        M = B * H * W
-        lib, st, dt = _lib.load(), _lib.stream_ptr(a1), _lib.dtype_code(a1)
         a1, a2 = a1.detach(), (None if a2 is None else a2.detach())
-        ds = _drop_scale(drop_scale, a1)
         wb = weight.detach().reshape(N, K1 + K2).to(torch.bfloat16).contiguous()
         b1, b2 = wb[:, :K1], (wb[:, K1:] if K2 else None)
         out = torch.empty((B, N, H, W), dtype=torch.bfloat16, device=a1.device, memory_format=torch.channels_last)
-        out2d = _rows2d(out)
-        pre = scale = shift = mean = rstd = mask = None
-        batch = False
-        rcode = 1 if relu else 0                 # ReLU mask of the backward: read from `out` unless the batch path below avoids it
+        pre = y = ds = None
+        ss = (None,) * 4
         if bn is None:
-            _tc.gemm_bf16(a1, b1, a2, b2, out=out2d)
-        elif bn.training or bn.running_mean is None:
-            batch = True
-            sums = _zeros((2, N,), a1.device)
-            pre = torch.empty_like(out, memory_format=torch.channels_last)
-            _tc.gemm_bf16(a1, b1, a2, b2, stats=(sums[0], sums[1]), out=_rows2d(pre))
-            if relu and BN_MASK:                 # 1-bit mask with a residual, recomputed from pre (code 2) without one
-                mask = _relu_mask_buf(pre) if res is not None else None
-                rcode = 3 if mask is not None else (2 if res is None else 1)
-            ss = _bn_apply_batch(pre, None if res is None else res.detach(), sums, bn, bn_w, bn_b, relu, out, lib, st, dt, ds, mask)
-            scale, shift, mean, rstd = ss[0], ss[1], ss[2], ss[3]
+            _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(out))
         else:
-            scale, shift, mean, rstd = _bn_eval_fold(bn, bn_w, bn_b)
-            if res is None and ds is None:
-                _tc.gemm_bf16(a1, b1, a2, b2, scale=scale, shift=shift, relu=relu, out=out2d)
-            else:       # eval mode with a residual: raw GEMM, then the fused scale/shift + residual + ReLU kernel
-                pre = torch.empty_like(out, memory_format=torch.channels_last)
-                _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(pre))
-                _lib.check(lib.cotb200_bn_apply(dt, B, H * W, N, pre.data_ptr(), _lib.ptr(res), scale.data_ptr(), shift.data_ptr(),
-                                                1 if relu else 0, out.data_ptr(), _lib.ptr(ds), st), "bn_apply")
-        need_bwd = any(ctx.needs_input_grad)
-        if need_bwd and bn is not None and pre is None:      # eval-mode module under grad: BN backward needs the raw conv output
-            pre = torch.empty_like(out, memory_format=torch.channels_last)
-            _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(pre))
-        ctx.save_for_backward(a1, a2, wb, pre, mask if rcode == 3 else (out if rcode == 1 else None), scale,
-                              shift if rcode == 2 else None, mean, rstd, ds)
-        ctx.cfg = (rcode, batch, bn is not None, weight.dtype, weight.shape, None if bn_w is None else bn_w.dtype, K1, K2,
-                   res is not None)
+            pre, y, ss, ds = _bn_epilogue(ctx, out, lambda dst, **epi: _tc.gemm_bf16(a1, b1, a2, b2, out=_rows2d(dst), **epi),
+                                          bn, bn_w, bn_b, relu, res, drop_scale)
+        ctx.save_for_backward(a1, a2, wb, pre, y, *ss, ds)
+        ctx.cfg = (bn is not None, weight.dtype, weight.shape, K1, K2)
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        a1, a2, wb, pre, y, scale, shift, mean, rstd, ds = ctx.saved_tensors     # y: output (rcode 1), 1-bit mask (rcode 3) or None
-        rcode, batch, has_bn, wdt, wshape, bndt, K1, K2, has_res = ctx.cfg
+        a1, a2, wb, pre, y, *ss, ds = ctx.saved_tensors
+        has_bn, wdt, wshape, K1, K2 = ctx.cfg
         dy = dy.contiguous(memory_format=torch.channels_last)
         B, N, H, W = dy.shape
         M = B * H * W
-        lib, st, dt = _lib.load(), _lib.stream_ptr(dy), _lib.BF16
         dgamma = dbeta = dres = None
         dpre = dy
         if has_bn:
-            sums = torch.zeros(2, N, dtype=torch.float32, device=dy.device)  # escapes as dgamma/dbeta
-            if has_res and ctx.needs_input_grad[8]:
-                dres = torch.empty_like(dy, memory_format=torch.channels_last)
-            dpre = torch.empty_like(dy, memory_format=torch.channels_last)
-            _bn_bwd(lib, dt, B, H * W, N, dy, pre, y, scale, shift, mean, rstd, rcode, sums, batch, 1.0 / M, dpre, dres, ds, st)
-            dgamma, dbeta = sums[1].to(bndt), sums[0].to(bndt)
+            dpre, dgamma, dbeta, dres = _bn_epilogue_bwd(ctx, dy, pre, y, ss, ds, 4, 8)
         d2 = _rows2d(dpre)
         da1 = da2 = None
         wt = wb.t().contiguous()                                  # [K1+K2, N]: B operand of the data-gradient GEMM
@@ -770,43 +767,19 @@ class TcConv3x3Fn(Function):
     @staticmethod
     def forward(ctx, x, weight, bn_w, bn_b, bn, groups, relu):
         assert _is_cl(x) and x.dtype == torch.bfloat16
-        B, C, H, W = x.shape
-        M = B * H * W
-        lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.BF16
         x = x.detach()
         wp, bnt = _tc.prepare_conv3x3_weight(weight, groups)
         out = torch.empty_like(x, memory_format=torch.channels_last)
-        pre = None
-        batch = bn.training or bn.running_mean is None
-        if batch:
-            sums = _zeros((2, C,), x.device)
-            pre = torch.empty_like(x, memory_format=torch.channels_last)
-            _tc.conv3x3_bf16(x, wp, bnt, stats=(sums[0], sums[1]), out=pre)
-            ss = _bn_apply_batch(pre, None, sums, bn, bn_w, bn_b, relu, out, lib, st, dt)
-            scale, shift, mean, rstd = ss[0], ss[1], ss[2], ss[3]
-        else:
-            scale, shift, mean, rstd = _bn_eval_fold(bn, bn_w, bn_b)
-            _tc.conv3x3_bf16(x, wp, bnt, scale=scale, shift=shift, relu=relu, out=out)
-            if any(ctx.needs_input_grad):
-                pre = _tc.conv3x3_bf16(x, wp, bnt)
-        # ReLU mask of the backward: recomputed from pre and the apply kernel's own scale/shift (code 2) in training; the eval
-        # output comes out of the convolution's epilogue (fp32 accumulator, not the stored pre), so there it is read from `out`
-        rcode = 0 if not relu else (2 if (batch and BN_MASK) else 1)
-        ctx.save_for_backward(x, weight.detach(), pre, out if rcode == 1 else None, scale, shift if rcode == 2 else None, mean, rstd)
-        ctx.cfg = (rcode, batch, groups, bn_w.dtype)
+        pre, y, ss, _ = _bn_epilogue(ctx, out, lambda dst, **epi: _tc.conv3x3_bf16(x, wp, bnt, out=dst, **epi), bn, bn_w, bn_b, relu)
+        ctx.save_for_backward(x, weight.detach(), pre, y, *ss)
+        ctx.groups = groups
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, pre, y, scale, shift, mean, rstd = ctx.saved_tensors
-        rcode, batch, groups, bndt = ctx.cfg
-        B, C, H, W = x.shape
-        M = B * H * W
-        lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.BF16
-        dy = dy.contiguous(memory_format=torch.channels_last)
-        sums = torch.zeros(2, C, dtype=torch.float32, device=x.device)  # escapes as dgamma/dbeta
-        dpre = torch.empty_like(dy, memory_format=torch.channels_last)
-        _bn_bwd(lib, dt, B, H * W, C, dy, pre, y, scale, shift, mean, rstd, rcode, sums, batch, 1.0 / M, dpre, None, None, st)
+        x, weight, pre, y, *ss = ctx.saved_tensors
+        groups = ctx.groups
+        dpre, dgamma, dbeta, _ = _bn_epilogue_bwd(ctx, dy.contiguous(memory_format=torch.channels_last), pre, y, ss, None, 2)
         dx = dw = None
         if ctx.needs_input_grad[0]:
             wpt, bnt = _tc.prepare_conv3x3_weight(weight, groups, transpose_for_dgrad=True)
@@ -814,7 +787,7 @@ class TcConv3x3Fn(Function):
         if ctx.needs_input_grad[1]:
             # weight gradient: cuDNN grouped wgrad through torch (DESIGN.md section 6)
             dw = torch.nn.grad.conv2d_weight(x, weight.shape, dpre, stride=1, padding=1, dilation=1, groups=groups).to(weight.dtype)
-        return dx, dw, sums[1].to(bndt), sums[0].to(bndt), None, None, None
+        return dx, dw, dgamma, dbeta, None, None, None
 
 
 class StemConvBNFn(Function):
@@ -827,44 +800,26 @@ class StemConvBNFn(Function):
     def forward(ctx, x, weight, bn_w, bn_b, bn, relu):
         B, _, H, W = x.shape
         N = weight.shape[0]
-        lib, st, dt = _lib.load(), _lib.stream_ptr(x), _lib.BF16
         xd = x.detach()
         wm = _tc.prepare_stem_weight(weight)
         out = torch.empty((B, N, H // 2, W // 2), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
-        pre = scale = mean = rstd = scratch = None
-        batch = bn.training or bn.running_mean is None
-        if batch:
-            sums = _zeros((2, N,), x.device)
-            pre = torch.empty_like(out, memory_format=torch.channels_last)
-            r = _tc.stem7x7s2_bf16(xd, wm, stats=(sums[0], sums[1]), out=pre, return_scratch=True)
+        scratch = [None]            # the space-to-depth image of the statistics pass, for the wgmma weight gradient
+
+        def produce(dst, stats=None, **epi):
+            r = _tc.stem7x7s2_bf16(xd, wm, stats=stats, out=dst, return_scratch=True, **epi)
             if r is None:
                 raise RuntimeError("cotb200 stem7x7s2: geometry not supported")
-            scratch = r[1]
-            ss = _bn_apply_batch(pre, None, sums, bn, bn_w, bn_b, relu, out, lib, st, dt)
-            scale, shift, mean, rstd = ss[0], ss[1], ss[2], ss[3]
-        else:
-            scale, shift, mean, rstd = _bn_eval_fold(bn, bn_w, bn_b)
-            if _tc.stem7x7s2_bf16(xd, wm, scale=scale, shift=shift, relu=relu, out=out) is None:
-                raise RuntimeError("cotb200 stem7x7s2: geometry not supported")
-            if any(ctx.needs_input_grad):
-                pre = _tc.stem7x7s2_bf16(xd, wm)
-        rcode = 0 if not relu else (2 if (batch and BN_MASK) else 1)    # as in TcConv3x3Fn
-        ctx.save_for_backward(xd, weight.detach(), pre, out if rcode == 1 else None, scale, shift if rcode == 2 else None, mean, rstd,
-                              scratch)
-        ctx.cfg = (rcode, batch, bn_w.dtype)
+            if stats is not None:
+                scratch[0] = r[1]
+        pre, y, ss, _ = _bn_epilogue(ctx, out, produce, bn, bn_w, bn_b, relu)
+        ctx.save_for_backward(xd, weight.detach(), pre, y, *ss, scratch[0])
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, pre, y, scale, shift, mean, rstd, scratch = ctx.saved_tensors
-        rcode, batch, bndt = ctx.cfg
-        B, N, Ho, Wo = dy.shape
-        M = B * Ho * Wo
-        lib, st, dt = _lib.load(), _lib.stream_ptr(dy), _lib.BF16
-        dy = dy.contiguous(memory_format=torch.channels_last)
-        sums = torch.zeros(2, N, dtype=torch.float32, device=dy.device)  # escapes as dgamma/dbeta
-        dpre = torch.empty_like(dy, memory_format=torch.channels_last)
-        _bn_bwd(lib, dt, B, Ho * Wo, N, dy, pre, y, scale, shift, mean, rstd, rcode, sums, batch, 1.0 / M, dpre, None, None, st)
+        x, weight, pre, y, *ss, scratch = ctx.saved_tensors
+        N = dy.shape[1]
+        dpre, dgamma, dbeta, _ = _bn_epilogue_bwd(ctx, dy.contiguous(memory_format=torch.channels_last), pre, y, ss, None, 2)
         dx = dw = None
         wq = weight.to(dpre.dtype)
         if ctx.needs_input_grad[0]:
@@ -877,7 +832,7 @@ class StemConvBNFn(Function):
             if dw is None:
                 dw = torch.nn.grad.conv2d_weight(x, weight.shape, dpre, stride=2, padding=3)
             dw = dw.to(weight.dtype)
-        return dx, dw, sums[1].to(bndt), sums[0].to(bndt), None, None
+        return dx, dw, dgamma, dbeta, None, None
 
 
 def stem_conv_bn(x, conv, bn, relu=True):

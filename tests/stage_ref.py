@@ -176,17 +176,16 @@ SOURCE_ANCHORS = {
         "TC_MIN_PIXELS = 100000",
         "TC_KEY_MAX_DIM = 128",
         "TC_TRUNK_MAX_WEIGHT = 128 * 1024",
-        "rcode = 0 if not relu else (2 if res is None else (3 if mask is not None else 1))",
-        "rcode = 3 if mask is not None else (2 if res is None else 1)",
-        "rcode = 0 if not relu else (2 if (batch and BN_MASK) else 1)",
+        "rcode = 0 if not relu else (3 if mask is not None else (2 if (BN_MASK and res is None and row) else 1))",
         "return 8 if (wc // fold) % 8 == 0 else 0",
         # the eval dispatch (eval_* generators below)
         "if (not torch.is_grad_enabled() and not bn.training and not se[1].training and k is not None and se[1].running_mean is not None",
         "and bn.running_mean is not None and isinstance(se[2], torch.nn.ReLU)):",
         "if not (torch.is_grad_enabled() and x.requires_grad):\n        return (x,) * n",
-        "if res is None and ds is None:",
+        "row = not epilogue or res is not None or ds is not None",
+        "produce(out, scale=ss[0], shift=ss[1], relu=relu)",
         "and (torch.is_grad_enabled() or not bn.training)):",
-        "if _tc.stem7x7s2_bf16(xd, wm, scale=scale, shift=shift, relu=relu, out=out) is None:",
+        "r = _tc.stem7x7s2_bf16(xd, wm, stats=stats, out=dst, return_scratch=True, **epi)",
     ],
     "cotnet_b200/cot_layer.py": [
         "big = B * H * W >= fused.TC_MIN_PIXELS",

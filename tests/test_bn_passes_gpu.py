@@ -1,5 +1,5 @@
 """The BatchNorm backward without reading the forward output back: the 1-bit ReLU mask of residual BatchNorms (relu code 3) and
-the mask recomputed from the pre-activation on the wgmma convolutions (relu code 2).  Both must reproduce the y-reading path
+the mask recomputed from the pre-activation (relu code 2).  Both must reproduce the y-reading path
 (relu code 1) bit for bit: kernels, autograd functions, and three graph-replayed training steps of cotnet50."""
 import copy
 
@@ -150,6 +150,29 @@ def test_tc_conv1x1_mask_paths(monkeypatch, res):
         y = fused.TcConv1x1Fn.apply(x, None, conv.weight, None, bn.weight, bn.bias, bn, True, r)
         ins = [x, conv.weight, bn.weight, bn.bias] + ([r] if res else [])
         return [y] + list(torch.autograd.grad(y, ins, cot)) + [bn.running_mean, bn.running_var]
+    _run_both(monkeypatch, run)
+
+
+@pytest.mark.parametrize("ds_on", [False, True])
+@pytest.mark.parametrize("train", [True, False])
+def test_bnact_code2(monkeypatch, train, ds_on):
+    """BNActFn with ReLU and no residual: code 2 (recomputed from x and the forward's scale/shift) against code 1, in training
+    and eval, with and without drop-path scales."""
+    g = torch.Generator(device="cuda").manual_seed(14)
+    B, C, H = 4, 96, 14
+    bn0 = _bn(C, g).train(train)
+    with torch.no_grad():
+        bn0.running_mean.normal_(0, 0.3, generator=g)
+        bn0.running_var.uniform_(0.5, 1.5, generator=g)
+    x0 = _cl(torch.randn(B, C, H, H, generator=g, device="cuda").bfloat16())
+    cot = _cl(torch.randn(B, C, H, H, generator=g, device="cuda").bfloat16())
+    ds = torch.tensor([2.0, 0.0, 1.25, 1.25], device="cuda") if ds_on else None
+
+    def run():
+        bn = copy.deepcopy(bn0)
+        x = x0.clone().requires_grad_(True)
+        y = fused.BNActFn.apply(x, bn.weight, bn.bias, None, bn, True, ds)
+        return [y] + list(torch.autograd.grad(y, [x, bn.weight, bn.bias], cot)) + [bn.running_mean, bn.running_var]
     _run_both(monkeypatch, run)
 
 

@@ -247,6 +247,22 @@ def test_bn_exact(case):
                     if use_dres:
                         _eq(dres, gd, what + " dres")
 
+    # codes 1 and 2 agree bit for bit, with and without drop-path scales: code 1 reads the y bn_apply stored, code 2 recomputes
+    # its sign from x and the same scale / shift
+    for use_ds in (False, True):
+        dsp = _p(ds) if use_ds else None
+        y = _at((n, C), T, off)
+        _lib.check(lib.cotb200_bn_apply(dt, B, HW, C, _p(x), None, _p(sc), _p(sh), 1, _p(y), dsp, st), "bn_apply")
+        got = []
+        for relu, yp, shp in ((1, _p(y), None), (2, None, _p(sh))):
+            head = (dt, B, HW, C, _p(dy), _p(x), yp, None, _p(sc), shp, _p(mu), _p(rstd))
+            s, dx = torch.zeros(2, C, device=DEV), _at((n, C), T, off)
+            _lib.check(lib.cotb200_bn_bwd_sums(*head, relu, _p(s[0]), _p(s[1]), dsp, st), "bn_bwd_sums")
+            _lib.check(lib.cotb200_bn_bwd_apply(*head, _p(s[0]), _p(s[1]), inv_n, relu, _p(dx), None, dsp, st), "bn_bwd_apply")
+            got.append((s, dx))
+        _eq(got[1][0], got[0][0], "bn_bwd code 2 == code 1 ds=%d sums" % use_ds)
+        _eq(got[1][1], got[0][1], "bn_bwd code 2 == code 1 ds=%d dx" % use_ds)
+
 
 @pytest.mark.parametrize("n,use_batch,update", [(1.0, 1, 1), (2.0, 1, 1), (2.0, 1, 0), (6.0, 0, 0)])
 def test_bn_finalize_exact(n, use_batch, update):
