@@ -307,8 +307,11 @@ static int vresolve(const cotb200_agg_desc* d, VGeo& g, const char* what, bool d
   }
   if (d->sh <= 0 || d->sw <= 0 || d->dh <= 0 || d->dw <= 0 || d->ph < 0 || d->pw < 0) { set_error("%s: bad stride / dilation / padding", what); return COTB200_EINVAL; }
   if (d->ph >= d->h || d->pw >= d->w) { set_error("%s: reflect padding must be smaller than the input (pad %d,%d vs %dx%d)", what, d->ph, d->pw, d->h, d->w); return COTB200_EINVAL; }
-  const int ho = (d->h + 2 * d->ph - (d->dh * (d->kh - 1) + 1)) / d->sh + 1;
-  const int wo = (d->w + 2 * d->pw - (d->dw * (d->kw - 1) + 1)) / d->sw + 1;
+  const int span_h = d->h + 2 * d->ph - (d->dh * (d->kh - 1) + 1), span_w = d->w + 2 * d->pw - (d->dw * (d->kw - 1) + 1);
+  // a window larger than the padded input has no output position; the division below truncates towards zero, so it would
+  // yield a size of 1, or two negative sizes whose product matches the weight plane, and the taps would reflect off the planes
+  if (span_h < 0 || span_w < 0) { set_error("%s: kernel window larger than the padded input %dx%d", what, d->h + 2 * d->ph, d->w + 2 * d->pw); return COTB200_EINVAL; }
+  const int ho = span_h / d->sh + 1, wo = span_w / d->sw + 1;
   if (ho * wo != d->ho * d->wo) { set_error("%s: output size %dx%d does not match weight spatial size %dx%d", what, ho, wo, d->ho, d->wo); return COTB200_EINVAL; }
   g.SH = d->sh; g.SW = d->sw; g.PH = d->ph; g.PW = d->pw; g.DH = d->dh; g.DW = d->dw; g.HO = ho; g.WO = wo;
   return 0;

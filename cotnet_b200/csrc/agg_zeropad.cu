@@ -482,8 +482,11 @@ static int resolve(const cotb200_agg_desc* d, Geo& g) {
   }
   if (d->c % d->wc) { set_error("input channels %d not divisible by weight channels %d", d->c, d->wc); return COTB200_EINVAL; }
   // aggregation_zeropad.py:119-122
-  const int ho = (d->h + 2 * d->ph - (d->dh * (d->kh - 1) + 1)) / d->sh + 1;
-  const int wo = (d->w + 2 * d->pw - (d->dw * (d->kw - 1) + 1)) / d->sw + 1;
+  const int span_h = d->h + 2 * d->ph - (d->dh * (d->kh - 1) + 1), span_w = d->w + 2 * d->pw - (d->dw * (d->kw - 1) + 1);
+  // a window larger than the padded input has no output position (the division below truncates towards zero: it would
+  // yield a size of 1, or two negative sizes whose product matches the weight plane)
+  if (span_h < 0 || span_w < 0) { set_error("kernel window larger than the padded input %dx%d", d->h + 2 * d->ph, d->w + 2 * d->pw); return COTB200_EINVAL; }
+  const int ho = span_h / d->sh + 1, wo = span_w / d->sw + 1;
   if (ho * wo != d->ho * d->wo) {
     set_error("output size %dx%d does not match weight spatial size %dx%d", ho, wo, d->ho, d->wo); return COTB200_EINVAL;
   }

@@ -160,11 +160,13 @@ def agg_refpad_fwd_loops(x, w, k=3, s=1, p=0, d=1):
 
 
 def agg_refpad_unfold(x, w, k=3, s=1, p=0, d=1):
-    """aggregation_refpad.py:236-239 (the self-test's right-hand side): Unfold of the ReflectionPad2d'ed input."""
+    """aggregation_refpad.py:236-239 (the self-test's right-hand side): Unfold of the ReflectionPad2d'ed input.
+    k, s, p, d are ints or (height, width) pairs."""
     N, C, H, W = x.shape
     _, heads, wc, K2, Ho, Wo = w.shape
-    unfold = torch.nn.Unfold(kernel_size=k, dilation=d, padding=0, stride=s)
-    x2 = unfold(torch.nn.ReflectionPad2d(p)(x)).view(N, C // wc, wc, K2, Ho, Wo)
+    ph, pw = _pair(p)
+    unfold = torch.nn.Unfold(kernel_size=_pair(k), dilation=_pair(d), padding=0, stride=_pair(s))
+    x2 = unfold(torch.nn.ReflectionPad2d((pw, pw, ph, ph))(x)).view(N, C // wc, wc, K2, Ho, Wo)
     return (w.unsqueeze(2) * x2.unsqueeze(1)).sum(-3).view(N, heads * C, Ho, Wo)
 
 
@@ -201,7 +203,7 @@ def agg_dilate_unfold(x, w, dil):
         unfold = torch.nn.Unfold(kernel_size=3, dilation=dd, padding=dd, stride=1)
         x2 = unfold(xg).view(N, C // wc, 9, H, W)
         yg = (w[:, :, g].unsqueeze(2) * x2.unsqueeze(1)).sum(-3)          # [N, heads, C/wc, H, W]
-        idx = torch.arange(g, C, wc)
+        idx = torch.arange(g, C, wc, device=x.device)
         out = out.index_add(2, idx, yg)
     return out.view(N, heads * C, H, W)
 
